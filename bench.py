@@ -2,9 +2,10 @@
 """bench.py -- the measurement contract.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload all|q6|sum|q1|bruteforce|ivf|dropin]
+                    [--dump-outputs DIR]
 
 The default run covers ALL FIVE BASELINE.json configs in one JSON line.  The headline (top-level keys) is config 2, TPC-H Q6
-(3-predicate filter + SUM, fp64) over SF100 synthetic lineitem columns (600 037 902 rows, 28 B/row = 16.8 GB) on one B200; the other
+(3-predicate filter + SUM, fp64) over SF100 synthetic lineitem columns (600 037 902 rows, 28 B/row = 16.8 GB) on one H100; the other
 configs are under "workloads": sum (config 1), q1 (config 3), bruteforce (config 4), ivf (config 5), plus "dropin" (what one
 8192-row block costs through the C-ABI from host pointers).  Every workload carries
 
@@ -20,7 +21,11 @@ configs are under "workloads": sum (config 1), q1 (config 3), bruteforce (config
 
 Multi-GPU (one process per GPU, torchrun): q6 and sum are WEAK scaling (every rank owns an SF100-sized / 10 M-row disjoint block range),
 q1 is STRONG scaling of ONE SF100 table (shard.block_range, BASELINE config 3), bruteforce shards the 1 M rows, ivf shards the
-10 M-row index (config 5) over the ranks.  The exchange (MergeGroup / MergeTop) stays on the device.
+5 M-row index (config 5) over the ranks.  The exchange (MergeGroup / MergeTop) stays on the device.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step handed back to its caller as DIR/<workload>_<name>.npy
+(float64; 64-bit integers as exact (high, low) 32-bit halves).  Inputs are generated from fixed seeds, so two builds run with the
+same arguments can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -44,7 +49,8 @@ WORKLOADS = {
     "q1": dict(name="tpch_q1_sf100_fp64_packed_keys", metric="scan+filter+group-agg rows/sec (TPC-H Q1, fp64)", bytes_per_row=38.0, rows=SF100_ROWS, unit="rows/s", dtype="f64", scaling="strong"),
     "sum": dict(name="int64_sum_10m_rows", metric="int64 SUM rows/sec", bytes_per_row=8.0, rows=10_000_000, unit="rows/s", dtype="int64", scaling="weak"),
     "bruteforce": dict(name="bruteforce_l2_top10_1Mx768_10k_queries", metric="ANN top-k qps (768-d, brute-force L2 top-10)", bytes_per_row=None, rows=1_000_000, unit="queries/s", dtype="f32", scaling="strong"),
-    "ivf": dict(name="ivfflat_l2_top10_10Mx768_nlist1024_nprobe32_10k_queries", metric="ANN top-k qps (768-d, IVF-flat nlist=1024 nprobe=32 top-10)", bytes_per_row=None, rows=10_000_000, unit="queries/s", dtype="f32", scaling="strong"),
+    # 5 M rows: the entries (15.4 GB) and their split tensor-core operand (23 GB) fit one 80 GB H100 with room for the build
+    "ivf": dict(name="ivfflat_l2_top10_5Mx768_nlist1024_nprobe32_10k_queries", metric="ANN top-k qps (768-d, IVF-flat nlist=1024 nprobe=32 top-10)", bytes_per_row=None, rows=5_000_000, unit="queries/s", dtype="f32", scaling="strong"),
     "dropin": dict(name="xcall_go_arith_int64_block8192_host_pointers", metric="rows/sec of one 8192-row block through XCall from host pointers", bytes_per_row=24.0, rows=8192, unit="rows/s", dtype="int64", scaling="weak"),
 }
 ALL = ["q6", "sum", "q1", "bruteforce", "ivf", "dropin"]
@@ -69,7 +75,7 @@ def mem_available():
 
 
 class ClockSampler:
-    """nvidia-smi clocks during the timed region (B200_PROFILING.md recipe); one process per bench run, sliced per workload"""
+    """nvidia-smi clocks during the timed region; one process per bench run, sliced per workload"""
     Q = "timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, gpu_index):
@@ -124,7 +130,7 @@ class ClockSampler:
 
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    out = {"hbm": (6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"), "bf16": (1590.0, "fallback (B200_PROFILING.md 1.59 PFLOP/s)")}
+    out = {"hbm": (3350.0, "H100 SXM data sheet 3.35 TB/s (not measured)"), "bf16": (989.0, "H100 SXM data sheet 989 TFLOP/s dense (not measured)")}
     if os.path.exists(p):
         try:
             d = json.load(open(p))
@@ -332,6 +338,12 @@ class Env:
             self.sampler.start()
         self.W = max(3, args.warmup)
         self.K = max(1, args.steps)
+        self.dumps = {}
+
+    def dump(self, name, arr):
+        """keep an output of the last timed step for --dump-outputs (rank 0)"""
+        if self.args.dump_outputs and self.rank == 0:
+            self.dumps[name] = np.array(arr, dtype=np.float64, copy=True)
 
     def check(self, rc):
         return self.capi.check(rc, self.lib)
@@ -364,8 +376,9 @@ class Env:
         self.check(self.lib.MoB200_Memset(b.ptr, 0, max(nbytes, 8)))
         return b.ptr, b
 
-    def timed(self, step, K=None, W=None):
-        """W warm-up steps, then EXACTLY K steps between CUDA events on the library stream, barrier + synchronise on both sides"""
+    def timed(self, step, K=None, W=None, after=None):
+        """W warm-up steps, then EXACTLY K steps between CUDA events on the library stream, barrier + synchronise on both sides;
+        after() runs right behind the K-th step, so it sees what the last timed step produced (not the untimed clock-sampling steps)"""
         K = K or self.K
         W = self.W if W is None else W
         for _ in range(W):
@@ -384,6 +397,8 @@ class Env:
         self.check(self.lib.MoB200_TimerStop(C.byref(ms)))
         self.barrier_sync()
         wall_ms = (time.perf_counter() - t_wall0) * 1e3
+        if after is not None:
+            after()
         t_region1 = time.time()
         launches = self.lib.MoB200_KernelLaunchCount() - launches0
         total_ms = self.max_over_ranks(max(ms.value, 0.0))
@@ -414,6 +429,24 @@ class Env:
             out.append(kms.value)
         self.sync()
         return statistics.mean(out)
+
+
+def split_int64(a):
+    """int64 values as exact float64 (high signed 32 bits, low unsigned 32 bits) pairs, shape (n, 2)"""
+    a = np.asarray(a, dtype=np.int64).reshape(-1)
+    return np.stack([(a >> 32).astype(np.float64), (a & 0xFFFFFFFF).astype(np.float64)], axis=1)
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def write_dumps(d, dumps):
+    total = sum(a.nbytes for a in dumps.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise RuntimeError("outputs to dump take %d bytes, more than %d" % (total, DUMP_LIMIT_BYTES))
+    os.makedirs(d, exist_ok=True)
+    for name, a in dumps.items():
+        np.save(os.path.join(d, name + ".npy"), a)
 
 
 def rel_err(a, b):
@@ -452,8 +485,15 @@ def run_q6(env, n=None):
         else:
             env.check(lib.MoB200_DownloadAsync(host.ptr, part_ptr, 16))
 
-    t = env.timed(step)
-    final = (float(host.array[0]), int(host.array.view(np.int64)[1]))
+    last = {}
+
+    def grab():
+        last["r"] = (float(host.array[0]), int(host.array.view(np.int64)[1]))
+        env.dump("q6_sum", np.asarray([last["r"][0]]))
+        env.dump("q6_rows", split_int64(np.asarray([last["r"][1]], dtype=np.int64)))
+
+    t = env.timed(step, after=grab)
+    final = last["r"]
     # cross-check of the device seam against the synchronous API + the host-side merge (shard.py; covered by the gloo CPU test)
     sres = ops.q6_filter_sum(bufs["shipdate"], bufs["discount"], bufs["quantity"], bufs["extendedprice"], n, *P)
     seam_ok = None
@@ -555,7 +595,7 @@ def run_sum(env):
     wl = WORKLOADS["sum"]
     n = env.args.rows or wl["rows"]
     world, rank = env.world, env.rank
-    R = 4    # rotate over 4 distinct columns (320 MB > the 126 MB L2): every timed launch reads HBM, not L2
+    R = 4    # rotate over 4 distinct columns (320 MB > the 50 MB L2): every timed launch reads HBM, not L2
     cols = []
     for r in range(R):
         b = DeviceBuffer(8 * n, lib)
@@ -586,7 +626,9 @@ def run_sum(env):
         else:
             env.check(lib.MoB200_DownloadAsync(host.ptr, part_ptr, 24))
 
-    t = env.timed(step, K=max(env.K, 200))      # a 12-25 us launch: more steps for a stable figure (reported in the line)
+    # the 24-byte SUM state of the last timed step (value: 128-bit, two words; count); the steps rotate over the columns, so it is the
+    # state of column (warm-up + steps - 1) % R
+    t = env.timed(step, after=lambda: env.dump("sum_state", split_int64(host.array.view(np.int64))))
     it[0] = 0
     kern_ms = env.kernel_ms(step, reps=8)
     value = n * world * t["steps"] / (t["total_ms"] * 1e-3)
@@ -605,7 +647,7 @@ def run_sum(env):
                "timer": "wall clock around the C-ABI calls, max over ranks"}
         pa.free()
     out = {"value": value, "units_per_step": n * world, "timing": t, "kernel_ms": kern_ms, "alg_bytes": 8.0 * n, "kernel": "agg_kernel<int64, SUM>", "e2e": e2e, "rows_per_gpu": n,
-           "l2": "4 distinct 80 MB columns used in rotation (320 MB > the 126 MB L2)",
+           "l2": "4 distinct 80 MB columns used in rotation (320 MB > the 50 MB L2)",
            "parallelism": ("row-range shards x%d (weak), NCCL all_gather of 24-byte states + merge kernel" % world) if world > 1 else "1 GPU"}
     if rank == 0 and not env.args.no_cpu:
         threads = os.cpu_count() or 1
@@ -652,8 +694,15 @@ def run_q1(env):
         else:
             env.check(lib.MoB200_DownloadAsync(host.ptr, part_ptr, RB))
 
-    t = env.timed(step)
-    final = ops.q1_result_from_bytes(host.array.tobytes())
+    last = {}
+
+    def grab():
+        last["r"] = ops.q1_result_from_bytes(host.array.tobytes())
+        for f in ("returnflag", "linestatus", "count_order", "sum_qty", "sum_base_price", "sum_disc_price", "sum_charge", "avg_qty", "avg_price", "avg_disc"):
+            env.dump("q1_" + f, np.asarray([g[f] for g in last["r"]], dtype=np.float64))
+
+    t = env.timed(step, after=grab)
+    final = last["r"]
     # cross-check: synchronous API + host-side merge (shard.merge_q1) must give the same groups
     sres = ops.q1_group_agg(bufs["shipdate"], bufs["quantity"], bufs["extendedprice"], bufs["discount"], bufs["tax"], bufs["returnflag"], bufs["linestatus"], n, cut)
     if env.dist is not None:
@@ -741,7 +790,7 @@ def run_search(env, which):
         centers = env.datagen.vectors_f32(30, 0, nlist, dim) * np.float32(4.0)
         dcent = DeviceBuffer.from_numpy(centers, lib)
         t_b0 = time.perf_counter()
-        # LISTS are sharded (config 5: "lists sharded 8 x B200"): rank r keeps the whole lists l with l % world == r of the ONE 10 M-row table
+        # LISTS are sharded (config 5): rank r keeps the whole lists l with l % world == r of the ONE 10 M-row table
         ivf = ops.IvfflatSearchIndex.build_list_shard(lambda r0, m, ptr: env.check(lib.MoB200_GenVectorsF32(31, r0, m, dim, ptr, dcent.ptr, nlist, 1.0)),
                                                       total, centers, rank, world, capi.METRIC_L2, lib)
         build_s = time.perf_counter() - t_b0
@@ -781,8 +830,11 @@ def run_search(env, which):
             env.check(lib.MoB200_DownloadAsync(hk.ptr, kd.ptr, nq * k * 8))
             env.check(lib.MoB200_DownloadAsync(hd.ptr, dd.ptr, nq * k * 8))
 
-    t = env.timed(step)
-    final_k, final_d = hk.array.copy(), hd.array.copy()
+    def grab():
+        env.dump(which + "_keys", hk.array.astype(np.float64))      # row keys < 2^53: exact
+        env.dump(which + "_dists", hd.array)
+
+    t = env.timed(step, after=grab)
     kms = C.c_float()
     env.check(lib.MoB200_LastKernelMs(C.byref(kms)))    # the candidate pass of the last timed step
     kern_ms = kms.value
@@ -792,10 +844,10 @@ def run_search(env, which):
     if which == "ivf":
         pairs = float(nq) * nprobe * (total / float(nlist)) / world    # (query, probed row) pairs this rank scans: its share of the lists
         flop = 2.0 * pairs * kused
-        kernel = "tc_candidates_kernel (tcgen05 bf16, K = %d per pair) over (list, query-tile) units" % kused
+        kernel = "tc_candidates_kernel (wgmma bf16, K = %d per pair) over (list, query-tile) units" % kused
     else:
         flop = 2.0 * nq * n_local * kused
-        kernel = "tc_candidates_kernel (tcgen05 bf16, K = %d per pair)" % kused
+        kernel = "tc_candidates_kernel (wgmma bf16, K = %d per pair)" % kused
 
     # ---- e2e: queries from host memory, keys + distances back to host, through the synchronous call (+ the exchange at N > 1)
     e2e = None
@@ -896,13 +948,15 @@ def run_dropin(env):
         for _ in range(50):
             call()
         env.sync()
-        reps = 2000
+        reps = env.K
         t0 = time.perf_counter()
         for _ in range(reps):
             rc = call()
         env.sync()
         sec = (time.perf_counter() - t0) / reps
         out[label] = {"us_per_block": sec * 1e6, "rows_per_s": n / sec, "rc": int(rc)}
+        if label == "host_pointers":
+            env.dump("dropin_sum", split_int64(keep))
         if "pinned" in label:
             env.check(lib.MoB200_ColumnCacheConfigure(0))
         if host:
@@ -920,7 +974,7 @@ def run_dropin(env):
     secb = (time.perf_counter() - t0) / 5
     out["host_pointers_1024_blocks_per_call"] = {"us_per_block": secb * 1e6 / 1024, "rows_per_s": nb / secb, "rc": 0}
     ok = ok and bool(np.array_equal(R, A + B))
-    res = {"value": out["host_pointers"]["rows_per_s"], "units_per_step": n, "timing": {"total_ms": out["host_pointers"]["us_per_block"] * 2.0, "ms_per_step": out["host_pointers"]["us_per_block"] * 1e-3, "launches": 2000, "steps": 2000, "warmup": 50, "clocks": None, "wall_ms": None},
+    res = {"value": out["host_pointers"]["rows_per_s"], "units_per_step": n, "timing": {"total_ms": out["host_pointers"]["us_per_block"] * 2.0, "ms_per_step": out["host_pointers"]["us_per_block"] * 1e-3, "launches": env.K, "steps": env.K, "warmup": 50, "clocks": None, "wall_ms": None},
            "kernel_ms": None, "kernel": "go_arith_kernel<int64, +>", "blocks": out, "e2e": {"value": out["host_pointers"]["rows_per_s"], "unit": "rows/s", "h2d_bytes_per_step": 16 * n, "d2h_bytes_per_step": 8 * n + n // 8, "host_memory": "pageable (numpy)"},
            "parity": {"bit_exact": ok, "ok": ok}, "parallelism": "1 OS thread, 1 block in flight"}
     if env.rank == 0 and not env.args.no_cpu:
@@ -942,11 +996,11 @@ def finish(env, w, r):
            "timer": "CUDA events on the library stream (MoB200_TimerStart/Stop) around exactly `steps` steps, barrier + synchronise on both sides, max over ranks",
            "wall_ms_rank0": t.get("wall_ms")}
     if w in ("q6", "q1"):
-        cfg["l2"] = "inputs (%.1f GB per GPU) are larger than the 126 MB L2; no flush needed" % (r["alg_bytes"] / 1e9)
+        cfg["l2"] = "inputs (%.1f GB per GPU) are larger than the 50 MB L2; no flush needed" % (r["alg_bytes"] / 1e9)
     elif w == "sum":
         cfg["l2"] = r["l2"]
     elif w in ("bruteforce", "ivf"):
-        cfg["l2"] = "the index (%.1f GB per GPU) is larger than the 126 MB L2; no flush needed" % (4.0 * r["rows_per_gpu"] * 768 / 1e9)
+        cfg["l2"] = "the index (%.1f GB per GPU) is larger than the 50 MB L2; no flush needed" % (4.0 * r["rows_per_gpu"] * 768 / 1e9)
         cfg["queries"] = r["queries"]; cfg["rows_total"] = r["rows_total"]; cfg["index_build_s"] = r["index_build_s"]
     line["config"] = cfg
     if r.get("alg_bytes") is not None and r.get("kernel_ms"):
@@ -963,7 +1017,7 @@ def finish(env, w, r):
         line["roofline"] = {"bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": traffic, "kernel": r["kernel"], "kernel_ms": r["kernel_ms"],
                             "algorithmic_flop_per_launch": r["alg_flop"], "peak_source": src, "traffic_source": tsrc, "tc_refined_queries": r["tc_refined_queries"],
                             "tc_fallback_queries": r["tc_fallback_queries"], "kernel_ms_source": "CUDA events around the candidate pass of the last timed step",
-                            "note": "useful flop only (tiles are padded to 128 queries x 256 rows)" if w == "ivf" else None}
+                            "note": "useful flop only (tiles are padded to 128 queries x 128 rows)" if w == "ivf" else None}
     else:
         line["roofline"] = None
     line["cpu_baseline"] = r.get("cpu_baseline")
@@ -989,6 +1043,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-pageable", action="store_true")
     ap.add_argument("--queries", type=int, default=10_000)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step of every workload as DIR/<name>.npy")
     ap.add_argument("--tune", action="append", default=[], metavar="NAME=VALUE",
                     help="kernel-variant knob passed to MoB200_SetTuning (experiments only; the default run uses none)")
     args = ap.parse_args()
@@ -1019,6 +1075,9 @@ def main():
         if len(lines) > 1:
             head["workloads"] = {w: lines[w] for w in names[1:] if w in lines}
         head["bench_seconds_total"] = time.time() - t_all0
+        if args.dump_outputs:
+            write_dumps(args.dump_outputs, env.dumps)
+            head["dumped_outputs"] = sorted(env.dumps)
         print(json.dumps(head))
     if env.dist is not None:
         env.dist.destroy_process_group()

@@ -1,5 +1,5 @@
 /*
- * mo_b200.h -- C-ABI of libmo_b200.so, the B200 (sm_100a) implementation of MatrixOne's per-block batch
+ * mo_b200.h -- C-ABI of libmo_b200.so, the H100 (sm_90a) implementation of MatrixOne's per-block batch
  * operators and vector-distance kernels.
  *
  * PART 1 is the reference's cgo surface, byte for byte the same prototypes as /root/reference/cgo/mo.h:24-73

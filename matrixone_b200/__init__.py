@@ -1,4 +1,4 @@
-"""matrixone_b200 -- B200 (sm_100a) batch operators and vector-distance kernels behind MatrixOne's cgo C-ABI.
+"""matrixone_b200 -- H100 (sm_90a) batch operators and vector-distance kernels behind MatrixOne's cgo C-ABI.
 
 The product is the shared library `libmo_b200.so` (include/mo_b200.h); this package is its Python harness:
   capi      ctypes prototypes of every exported symbol

@@ -1,4 +1,4 @@
-"""Build libmo_b200.so (the C-ABI library, include/mo_b200.h) with nvcc for sm_100a, in-tree.
+"""Build libmo_b200.so (the C-ABI library, include/mo_b200.h) with nvcc for sm_90a (H100), in-tree.
 
     python -m matrixone_b200.build [--force] [--verbose]
 
@@ -16,7 +16,7 @@ OUT = os.path.join(HERE, "libmo_b200.so")
 OBJ = os.path.join(HERE, "build")
 SOURCES = ["runtime.cu", "agg.cu", "tpch.cu", "elementwise.cu", "goelem.cu", "colops.cu", "join.cu", "kmeans.cu", "lz4.cu", "vecdecode.cu", "plan.cu", "decimal.cu", "bloom.cu", "distance.cu", "search.cu", "tcsearch.cu", "xcall.cu", "datagen.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -56,7 +56,7 @@ def build(force=False, verbose=False):
         with ThreadPoolExecutor(max_workers=min(8, len(todo))) as ex:
             list(ex.map(compile_one, todo))
     if todo or not os.path.exists(OUT):
-        _run([NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", OUT] + objs)
+        _run([NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", OUT] + objs)
     if verbose:
         for k, v in logs.items():
             print("==", k)

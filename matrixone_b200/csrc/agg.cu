@@ -4,7 +4,7 @@
 // minmax2.go:49-80.
 //
 // HBM-bound streaming reduction: every thread issues 4 independent 128-bit L1-bypassing loads per iteration
-// (grid = 148 SMs x CTAS_PER_SM persistent CTAs, grid-stride), the nulls word for 64 rows is a warp-broadcast
+// (grid = SMs x CTAS_PER_SM persistent CTAs, grid-stride), the nulls word for 64 rows is a warp-broadcast
 // load, partials are combined by warp shuffles -> shared memory -> one per-CTA record; the last CTA to finish
 // (atomicInc ticket) folds the per-CTA records in index order, so results are run-to-run deterministic.
 //

@@ -14,7 +14,7 @@
 
 namespace mob {
 
-constexpr int kSMs = 148;  // B200: 2 dies x 74 SMs; grids are sized in multiples of this
+constexpr int kSMs = 132;  // H100 SXM; grids are sized in multiples of the device's SM count (num_sms(), this until it is known)
 
 struct ArenaBlock { char *p; size_t size; };
 

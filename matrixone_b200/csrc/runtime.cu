@@ -246,7 +246,7 @@ int32_t MoB200_Init(int32_t device) {
     return MO_RC_SUCCESS;
 }
 
-const char *MoB200_Version(void) { return "mo_b200 0.1 (sm_100a)"; }
+const char *MoB200_Version(void) { return "mo_b200 0.1 (sm_90a)"; }
 
 int32_t MoB200_DeviceCount(void) {
     int n = 0;
@@ -418,7 +418,7 @@ int32_t MoB200_LastError(char *buf, uint64_t buflen) {
 int32_t MoB200_FlushL2(void) {
     REQUIRE_CTX(t);
     static thread_local void *buf = nullptr;
-    const size_t bytes = (size_t)256 << 20;  // 2x the 126 MB L2
+    const size_t bytes = (size_t)256 << 20;  // 5x the 50 MB L2
     if (!buf) MOB_CUDA_TRY(cudaMalloc(&buf, bytes));
     flush_l2_kernel<<<num_sms() * 4, 256, 0, t.stream>>>((int4 *)buf, bytes / 16);
     MOB_LAUNCH_CHECK();

@@ -1,18 +1,18 @@
-// tcsearch.cu -- tensor-core candidate generation for batched brute-force search (tcgen05 + TMEM + TMA, sm_100a).
+// tcsearch.cu -- tensor-core candidate generation for batched brute-force search (wgmma + TMA + mbarrier, sm_90a).
 //
-// The exact kernel in search.cu replays the Go distance loop (3 fp32 ops per element pair, ~33 T lane-ops/s ceiling on this
-// part).  For large query batches the L2 distance is a dense contraction, so candidates are generated on the 5th-gen tensor
-// cores and only the survivors are re-scored exactly:
+// The exact kernel in search.cu replays the Go distance loop (3 fp32 ops per element pair).  For large query batches the L2
+// distance is a dense contraction, so candidates are generated on the tensor cores and only the survivors are re-scored exactly:
 //
 //   1. split_kernel:   x (fp32) = hi + lo with hi = bf16(x), lo = bf16(x - hi); operands are stored K-concatenated,
 //                      A' = [q_hi | q_hi | q_lo], B' = [x_hi | x_lo | x_hi]  (K' = 3*dim, padded to a multiple of 64), so ONE
 //                      bf16 GEMM yields q_hi.x_hi + q_hi.x_lo + q_lo.x_hi = q.x up to ~2^-16 relative (the lo.lo term is
 //                      dropped); squared norms are computed in fp64 and rounded to fp32.
-//   2. tc_candidates_kernel: persistent, warp-specialised.  CTA tile 128 queries x 256 rows, K' streamed in 64-element
-//                      (128-byte, SWIZZLE_128B) slabs by TMA through a 4-stage mbarrier ring; one elected thread issues
-//                      tcgen05.mma.cta_group::1.kind::f16 (M128 N256 K16) into one of two 256-column TMEM accumulators; four
-//                      epilogue warps read the other accumulator with tcgen05.ld (each thread = one query row), form
-//                      d~ = |q|^2 + |x|^2 - 2 q.x and keep the KP smallest per (query, row range) in a thread-private shared-memory list.
+//   2. tc_candidates_kernel: persistent, warp-specialised.  CTA tile 128 queries x 128 rows, K' streamed in 64-element
+//                      (128-byte, SWIZZLE_128B) slabs by TMA through a 4-stage mbarrier ring; one warpgroup issues
+//                      wgmma.mma_async m64n128k16 (two per K16 step, one per 64 query rows) into registers and, once a tile is
+//                      complete, stores the accumulator to a shared-memory tile; four epilogue warps read that tile (each thread =
+//                      one query row) while the warpgroup already multiplies the next one, form d~ = |q|^2 + |x|^2 - 2 q.x and
+//                      keep the KP smallest per (query, row range) in registers.
 //   3. rescore (search.cu path): the approximate lists of all ranges are merged per query, the best KR candidates are
 //                      re-scored with the bit-exact Go-order distance, sorted by (distance, id), and the top k returned.
 //   4. proof of completeness: a row that was never a candidate has d~ >= t, the smallest "list-full threshold" of its
@@ -38,34 +38,33 @@ using namespace mob;
 
 namespace {
 
-constexpr int BM = 128, BN = 256, BK = 64;
+constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int KP = 16;                      // candidates kept per (query, row range)
 constexpr int KP_LONG = 32;                 // ... by the one-term pass over IVF lists (short ranges: the list threshold must sit well above the k-th result)
-constexpr int kTcThreads = 256;             // warp 0 TMA, warp 1 MMA, warp 2 TMEM alloc, warp 3 idle, warps 4-7 epilogue
+constexpr int kTcThreads = 288;             // warps 0-3 MMA warpgroup, warps 4-7 epilogue, warp 8 TMA
+constexpr int kStages = 4;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
+constexpr int B_STAGE_BYTES = BN * BK * 2;  // 16 KB
+constexpr int kAccStride = BM + 4;          // accumulator tile [row][query], padded so that the fragment stores are conflict-free
 
-// PAIR = false: one CTA per unit, tcgen05.mma.cta_group::1, M = 128: the CTA stages the whole 256-row B tile (48 KB per k-block).
-// PAIR = true : a cluster of two CTAs (one TPC) per unit, tcgen05.mma.cta_group::2, M = 256: each CTA stages its own 128 query
-//               rows and HALF of the B tile (32 KB per k-block for the same flop per SM) -- the candidate pass is bound by
-//               L2 -> SM bytes, so this is worth up to 1.5x where there are enough queries to fill 256-row tiles.
+// PAIR = false: one CTA per unit, 128 queries, the CTA loads the whole 128-row B tile.
+// PAIR = true : a cluster of two CTAs per unit (256 queries, 128 per CTA) that share the B tile: each CTA loads HALF of it with a
+//               TMA multicast into both CTAs' shared memory, so a k-block costs 24 instead of 32 KB of L2 -> SM traffic per CTA --
+//               the candidate pass is bound by those bytes where there are enough queries to fill 256-row units.
 template <bool PAIR>
 struct TcCfg {
-    static constexpr int kStages = PAIR ? 6 : 4;
-    static constexpr int kBRows = PAIR ? BN / 2 : BN;            // B rows staged per CTA per k-block
-    static constexpr int kBStageBytes = kBRows * BK * 2;         // 16 / 32 KB
+    static constexpr int kBRows = PAIR ? BN / 2 : BN;            // B rows each CTA loads per k-block
     static constexpr int kTileM = PAIR ? 2 * BM : BM;            // query rows per unit
 };
 
-template <bool PAIR>
-struct TcSmemT {
-    unsigned char a[TcCfg<PAIR>::kStages][A_STAGE_BYTES];                 // 1024-byte aligned (SWIZZLE_128B atoms)
-    unsigned char b[TcCfg<PAIR>::kStages][TcCfg<PAIR>::kBStageBytes];
-    float xn[2][BN];                          // |x|^2 of the current tile's rows (double buffered with the accumulators)
-    float scratch[32][BM];                    // epilogue slow path: a thread's 32 distances of the current chunk, [column][thread]
-    unsigned long long full[TcCfg<PAIR>::kStages], empty[TcCfg<PAIR>::kStages], tmem_full[2], tmem_empty[2];
+struct TcSmem {
+    unsigned char a[kStages][A_STAGE_BYTES];  // 1024-byte aligned (SWIZZLE_128B atoms)
+    unsigned char b[kStages][B_STAGE_BYTES];
+    float acc[BN][kAccStride];                // the finished accumulator of one tile, [row of the tile][query row of the CTA]
+    float xn[2][BN];                          // |x|^2 of the current tile's rows (double buffered across tiles)
+    unsigned long long full[kStages], empty[kStages], acc_full, acc_empty;
     unsigned long long sched_full[2], sched_empty[2];   // dynamic unit feed (single-CTA units): the producer publishes the next unit index
     int sched_unit[2];
-    unsigned tmem_base;
 };
 
 // ---- PTX wrappers ------------------------------------------------------------------------------------------------------
@@ -95,19 +94,11 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap *map, unsigned lon
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(unsigned long long *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// the box lands at the same shared-memory offset in every CTA of `mask` and completes bytes on the barrier at the same offset in each
+__device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap *map, unsigned long long *bar, void *dst, int c0, int c1, unsigned short mask) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask) : "memory");
 }
-__device__ __forceinline__ void tc_mma_bf16(unsigned tmem_d, unsigned long long desc_a, unsigned long long desc_b, unsigned idesc, unsigned accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// ---- CTA-pair (cta_group::2) variants.  Barrier operands that live in the LEADER CTA (rank 0) are addressed through mapa.
 __device__ __forceinline__ unsigned cluster_ctarank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ unsigned mapa_rank(unsigned local_addr, unsigned rank) {
     unsigned r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank)); return r;
@@ -115,51 +106,38 @@ __device__ __forceinline__ unsigned mapa_rank(unsigned local_addr, unsigned rank
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// both CTAs of the pair load into their OWN shared memory and signal the leader's barrier (cluster address)
-__device__ __forceinline__ void tma_load_2d_pair(const CUtensorMap *map, unsigned bar_cluster_addr, void *dst, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(smem_u32(dst)), "l"(map), "r"(bar_cluster_addr), "r"(c0), "r"(c1) : "memory");
-}
 __device__ __forceinline__ void mbar_arrive_cluster(unsigned bar_cluster_addr) {
     asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
 }
-// arrives on the barrier at the same shared-memory offset in both CTAs of the pair once the MMAs issued so far have completed
-__device__ __forceinline__ void tc_commit_pair(unsigned long long *bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((unsigned short)3) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// ties the accumulator registers to the preceding wait, so that no read of them is scheduled above it
+__device__ __forceinline__ void fence_operands(float *d) {
+#pragma unroll
+    for (int i = 0; i < 64; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_mma_bf16_pair(unsigned tmem_d, unsigned long long desc_a, unsigned long long desc_b, unsigned idesc, unsigned accumulate) {
+// D[64 x 128] (+)= A[64 x 16] . B[128 x 16]^T, both operands K-major in shared memory; scale_d = 0 overwrites D
+__device__ __forceinline__ void wgmma_m64n128k16(float *d, unsigned long long desc_a, unsigned long long desc_b, unsigned scale_d) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread = TMEM lane = query row).  The load is asynchronous:
-// tc_ld32_issue starts it, tc_ld32_wait (tcgen05.wait::ld) makes the registers valid; the "+f" operands tie every later use of
-// v[] to the wait so the compiler cannot schedule arithmetic on them above it.
-__device__ __forceinline__ void tc_ld32_issue(unsigned taddr, float *v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]), "=f"(v[8]), "=f"(v[9]), "=f"(v[10]), "=f"(v[11]), "=f"(v[12]), "=f"(v[13]), "=f"(v[14]), "=f"(v[15]), "=f"(v[16]), "=f"(v[17]), "=f"(v[18]), "=f"(v[19]), "=f"(v[20]), "=f"(v[21]), "=f"(v[22]), "=f"(v[23]), "=f"(v[24]), "=f"(v[25]), "=f"(v[26]), "=f"(v[27]), "=f"(v[28]), "=f"(v[29]), "=f"(v[30]), "=f"(v[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld32_wait(float *v) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-        : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7]), "+f"(v[8]), "+f"(v[9]), "+f"(v[10]), "+f"(v[11]), "+f"(v[12]), "+f"(v[13]), "+f"(v[14]), "+f"(v[15]), "+f"(v[16]), "+f"(v[17]), "+f"(v[18]), "+f"(v[19]), "+f"(v[20]), "+f"(v[21]), "+f"(v[22]), "+f"(v[23]), "+f"(v[24]), "+f"(v[25]), "+f"(v[26]), "+f"(v[27]), "+f"(v[28]), "+f"(v[29]), "+f"(v[30]), "+f"(v[31])
-        :: "memory");
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor):
-// start>>4 | LBO(=1, ignored for swizzled K-major)<<16 | SBO(=1024 B: 8 rows x 128 B)>>4 <<32 | version 1 <<46 | layout 2 <<61
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma: start>>4 | LBO(=1, unused for swizzled K-major)<<16 |
+// SBO(=1024 B: 8 rows x 128 B)>>4 <<32 | layout 1 (128-byte swizzle) <<62
 __device__ __forceinline__ unsigned long long make_desc(unsigned smem_addr) {
-    return (unsigned long long)((smem_addr & 0x3ffff) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+    return (unsigned long long)((smem_addr & 0x3ffff) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// instruction descriptor (UMMA::InstrDescriptor): D=F32 (bit 4), A=BF16 (bit 7), B=BF16 (bit 10), K-major both, N>>3 at 17, M>>4 at 24
-constexpr unsigned kIdesc = (1u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(BN >> 3) << 17) | ((unsigned)(BM >> 4) << 24);
-constexpr unsigned kIdescPair = (1u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(BN >> 3) << 17) | ((unsigned)((2 * BM) >> 4) << 24);
 
 // bound on |approximate - real| squared distance of one (query operand, row operand) pair, from the operand norms:
 //   three-term product: |2 q.x error| <= 2 (3 * 2^-16 [dropped lo.lo + bf16 residuals] + 144 * 2^-23 [fp32 accumulation over K'/16
@@ -190,137 +168,129 @@ tc_candidates_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                      // dynamic unit feed (nullptr: unit u = worker, worker + nworkers, ...): the producer thread takes the next unit from this
                      // counter when it has issued the last load of the current one, and hands the index to the MMA and epilogue warps through a
                      // two-slot shared-memory queue.  Units are ordered list-major, so the query tiles of one IVF list start within a few
-                     // microseconds of each other on different SMs and stream the list's B' tiles through L2 together (with the static deal they
-                     // drifted apart and every tile of a list re-read it from HBM: 2.5 x the algorithmic bytes), and the tail is balanced.
+                     // microseconds of each other on different SMs and stream the list's B' tiles through L2 together (with a static deal they
+                     // drift apart and every tile of a list re-reads it from HBM), and the tail is balanced.
                      int *sched) {
-    using Cfg = TcCfg<PAIR>;
     const bool dyn = !PAIR && sched != nullptr;
-    constexpr int STAGES = Cfg::kStages;
     extern __shared__ unsigned char smem_raw[];
     // SWIZZLE_128B atoms need 1024-byte alignment in the shared window: align by hand (the launch adds 1024 spare bytes)
-    TcSmemT<PAIR> &S = *reinterpret_cast<TcSmemT<PAIR> *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
+    TcSmem &S = *reinterpret_cast<TcSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const unsigned rank = PAIR ? cluster_ctarank() : 0u;            // 0 = leader: issues the MMAs, owns the full / tmem_empty barriers
+    const unsigned rank = PAIR ? cluster_ctarank() : 0u;            // a pair's CTAs take query rows rank*128.. of the unit and B half `rank`
     const int worker = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
     const int nworkers = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], 1); }
-        for (int a = 0; a < 2; a++) { mbar_init(&S.tmem_full[a], 1); mbar_init(&S.tmem_empty[a], PAIR ? 8 : 4); }
-        for (int a = 0; a < 2; a++) { mbar_init(&S.sched_full[a], 1); mbar_init(&S.sched_empty[a], 1 + 128); }   // readers: the MMA thread + 128 epilogue threads
+        // a stage is free again once the four MMA warps of this CTA -- and of the peer, whose half of B was multicast into it -- are done
+        for (int s = 0; s < kStages; s++) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], PAIR ? 8 : 4); }
+        mbar_init(&S.acc_full, 128); mbar_init(&S.acc_empty, 128);
+        for (int a = 0; a < 2; a++) { mbar_init(&S.sched_full[a], 1); mbar_init(&S.sched_empty[a], 128 + 128); }   // readers: the MMA warpgroup + the 128 epilogue threads
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    if (warp == 2) {   // TMEM: 512 columns = two 128 x 256 fp32 accumulators (per CTA)
-        if (PAIR) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&S.tmem_base)) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&S.tmem_base)) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tc_fence_before();
     __syncthreads();
     if (PAIR) cluster_sync_all();   // the peer's barriers must be initialised before anything signals them
-    tc_fence_after();
-    const unsigned tmem_base = S.tmem_base;
 
-    if (warp == 0) {
-        // ===== TMA producer (one thread; in a pair both CTAs run it, each for its own rows) =====
+    // the unit of iteration `it` (-1: done); the producer takes it from the counter, everybody else from the queue
+    auto unit_of = [&](int it, bool producer) -> int {
+        if (!dyn) { const int u = worker + it * nworkers; return u < nunits ? u : -1; }
+        const int slot = it & 1;
+        if (producer) {
+            mbar_wait(&S.sched_empty[slot], ((it >> 1) & 1) ^ 1);
+            int u = atomicAdd(sched, 1);
+            if (u >= nunits) u = -1;
+            *(volatile int *)&S.sched_unit[slot] = u;
+            mbar_arrive(&S.sched_full[slot]);        // release: the index is visible to whoever observes the phase
+            return u;
+        }
+        mbar_wait(&S.sched_full[slot], (it >> 1) & 1);
+        const int u = *(volatile int *)&S.sched_unit[slot];
+        mbar_arrive(&S.sched_empty[slot]);
+        return u;
+    };
+
+    if (warp == 8) {
+        // ===== TMA producer (one thread; in a pair both CTAs run it, each for its own query rows and its half of B) =====
         if (lane == 0) {
             int stage = 0; unsigned phase = 0;
             for (int it = 0;; it++) {
-                int u;
-                if (dyn) {
-                    const int slot = it & 1;
-                    mbar_wait(&S.sched_empty[slot], ((it >> 1) & 1) ^ 1);
-                    u = atomicAdd(sched, 1);
-                    if (u >= nunits) u = -1;
-                    *(volatile int *)&S.sched_unit[slot] = u;
-                    mbar_arrive(&S.sched_full[slot]);        // release: the index is visible to whoever observes the phase
-                } else {
-                    u = worker + it * nworkers;
-                    if (u >= nunits) u = -1;
-                }
+                const int u = unit_of(it, true);
                 if (u < 0) break;
                 const TcUnit U = units[u];
                 for (int n0 = U.n_begin; n0 < U.n_end; n0 += BN) {
                     for (int kb = 0; kb < nkb; kb++) {
                         mbar_wait(&S.empty[stage], phase ^ 1);
-                        if (PAIR) {
-                            // the leader's barrier collects the bytes of all four loads (two per CTA)
-                            if (rank == 0) mbar_expect_tx(&S.full[stage], 2 * (A_STAGE_BYTES + Cfg::kBStageBytes));
-                            const unsigned bar = mapa_rank(smem_u32(&S.full[stage]), 0);
-                            tma_load_2d_pair(&map_a, bar, S.a[stage], kb * BK, U.a_row0 + (int)rank * BM);
-                            tma_load_2d_pair(&map_b, bar, S.b[stage], kb * BK, n0 + (int)rank * Cfg::kBRows);
-                        } else {
-                            mbar_expect_tx(&S.full[stage], A_STAGE_BYTES + Cfg::kBStageBytes);
-                            tma_load_2d(&map_a, &S.full[stage], S.a[stage], kb * BK, U.a_row0);
-                            tma_load_2d(&map_b, &S.full[stage], S.b[stage], kb * BK, n0);
-                        }
-                        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                        mbar_expect_tx(&S.full[stage], A_STAGE_BYTES + B_STAGE_BYTES);   // a pair: own A + own B half + the peer's B half
+                        tma_load_2d(&map_a, &S.full[stage], S.a[stage], kb * BK, U.a_row0 + (int)rank * BM);
+                        if (PAIR) tma_load_2d_multicast(&map_b, &S.full[stage], S.b[stage] + rank * (B_STAGE_BYTES / 2), kb * BK, n0 + (int)rank * (BN / 2), 3);
+                        else tma_load_2d(&map_b, &S.full[stage], S.b[stage], kb * BK, n0);
+                        if (++stage == kStages) { stage = 0; phase ^= 1; }
                     }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one thread of the leader CTA) =====
-        if (lane == 0 && rank == 0) {
-            int stage = 0; unsigned phase = 0; unsigned tile = 0;
-            for (int it = 0;; it++) {
-                int u;
-                if (dyn) {
-                    const int slot = it & 1;
-                    mbar_wait(&S.sched_full[slot], (it >> 1) & 1);
-                    u = *(volatile int *)&S.sched_unit[slot];
-                    mbar_arrive(&S.sched_empty[slot]);
-                } else {
-                    u = worker + it * nworkers;
-                    if (u >= nunits) u = -1;
-                }
-                if (u < 0) break;
-                const TcUnit U = units[u];
-                for (int n0 = U.n_begin; n0 < U.n_end; n0 += BN, tile++) {
-                    const unsigned acc = tile & 1;
-                    mbar_wait(&S.tmem_empty[acc], ((tile >> 1) & 1) ^ 1);
-                    tc_fence_after();
-                    const unsigned tmem_d = tmem_base + acc * BN;
-                    for (int kb = 0; kb < nkb; kb++) {
-                        mbar_wait(&S.full[stage], phase);
-                        tc_fence_after();
-                        const unsigned long long da = make_desc(smem_u32(S.a[stage])), db = make_desc(smem_u32(S.b[stage]));
+    } else if (warp < 4) {
+        // ===== MMA warpgroup: 128 x 128 fp32 accumulator in registers (query rows 0-63 in d0, 64-127 in d1) =====
+        float d0[64], d1[64];
 #pragma unroll
-                        for (int k = 0; k < BK / 16; k++) {  // +32 bytes (= 2 in the >>4 address field) per K16 step inside the 128-B swizzle atom
-                            if (PAIR) tc_mma_bf16_pair(tmem_d, da + 2 * k, db + 2 * k, kIdescPair, (kb | k) != 0);
-                            else tc_mma_bf16(tmem_d, da + 2 * k, db + 2 * k, kIdesc, (kb | k) != 0);
-                        }
-                        if (PAIR) tc_commit_pair(&S.empty[stage]); else tc_commit(&S.empty[stage]);   // frees the smem slot(s) once these MMAs have read them
-                        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        for (int i = 0; i < 64; i++) { d0[i] = 0.f; d1[i] = 0.f; }
+        const unsigned peer = rank ^ 1u;
+        auto release = [&](int s) {   // every warp has waited for its wgmma groups that read stage s
+            __syncwarp();
+            if (lane == 0) {
+                mbar_arrive(&S.empty[s]);
+                if (PAIR) mbar_arrive_cluster(mapa_rank(smem_u32(&S.empty[s]), peer));
+            }
+        };
+        int stage = 0; unsigned phase = 0; unsigned tile = 0;
+        for (int it = 0;; it++) {
+            const int u = unit_of(it, false);
+            if (u < 0) break;
+            const TcUnit U = units[u];
+            for (int n0 = U.n_begin; n0 < U.n_end; n0 += BN, tile++) {
+                int prev = 0;
+                for (int kb = 0; kb < nkb; kb++) {
+                    mbar_wait(&S.full[stage], phase);
+                    __syncwarp();
+                    wgmma_fence();
+                    const unsigned long long da = make_desc(smem_u32(S.a[stage])), db = make_desc(smem_u32(S.b[stage]));
+#pragma unroll
+                    for (int k = 0; k < BK / 16; k++) {  // +32 bytes (= 2 in the >>4 address field) per K16 step inside the 128-B swizzle atom
+                        const unsigned acc = (kb | k) != 0;
+                        wgmma_m64n128k16(d0, da + 2 * k, db + 2 * k, acc);
+                        wgmma_m64n128k16(d1, da + 512 + 2 * k, db + 2 * k, acc);   // query rows 64..127: +8 KB
                     }
-                    if (PAIR) tc_commit_pair(&S.tmem_full[acc]); else tc_commit(&S.tmem_full[acc]);   // accumulator complete -> epilogue(s)
+                    wgmma_commit();
+                    if (kb > 0) { wgmma_wait<1>(); release(prev); }   // the previous k-block's MMAs have read their stage
+                    prev = stage;
+                    if (++stage == kStages) { stage = 0; phase ^= 1; }
                 }
+                wgmma_wait<0>();
+                fence_operands(d0); fence_operands(d1);
+                release(prev);
+                // accumulator -> shared tile (once the epilogue has finished reading the previous one).  Fragment of m64nNk16:
+                // d[4j + 2i + c] = (query row 16 warp + lane/4 + 8i, tile row 8j + 2 (lane%4) + c)
+                mbar_wait(&S.acc_empty, (tile & 1) ^ 1);
+                const int r0 = 16 * warp + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+                for (int j = 0; j < 16; j++)
+#pragma unroll
+                    for (int i = 0; i < 2; i++)
+#pragma unroll
+                        for (int c = 0; c < 2; c++) {
+                            S.acc[8 * j + c0 + c][r0 + 8 * i] = d0[4 * j + 2 * i + c];
+                            S.acc[8 * j + c0 + c][64 + r0 + 8 * i] = d1[4 * j + 2 * i + c];
+                        }
+                mbar_arrive(&S.acc_full);
             }
         }
-    } else if (warp >= 4) {
-        // ===== epilogue: thread e = query row of this CTA's half of the tile = TMEM lane =====
+    } else {
+        // ===== epilogue: thread e = query row of this CTA's 128 rows of the unit =====
         const int e = threadIdx.x - 128;
-        const int ew = warp - 4;                              // TMEM lane quarter 32*ew .. 32*ew+31
         const int row_in_unit = (int)rank * BM + e;
-        const unsigned tmem_empty_leader0 = PAIR ? mapa_rank(smem_u32(&S.tmem_empty[0]), 0) : 0u;
-        const unsigned tmem_empty_leader1 = PAIR ? mapa_rank(smem_u32(&S.tmem_empty[1]), 0) : 0u;
         unsigned tile = 0;
         for (int it = 0;; it++) {
-            int u;
-            if (dyn) {
-                const int slot = it & 1;
-                mbar_wait(&S.sched_full[slot], (it >> 1) & 1);
-                u = *(volatile int *)&S.sched_unit[slot];
-                mbar_arrive(&S.sched_empty[slot]);
-            } else {
-                u = worker + it * nworkers;
-                if (u >= nunits) u = -1;
-            }
+            const int u = unit_of(it, false);
             if (u < 0) break;
             const TcUnit U = units[u];
             const bool valid_row = row_in_unit < U.a_valid;
@@ -339,44 +309,40 @@ tc_candidates_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
             const float my_eps = share ? tc_eps(qn, one_term ? alonorm[U.a_row0 + row_in_unit] : 0.f, xmax2[0], one_term ? xmax2[1] : 0.f, one_term) : 0.f;
             float cap = INFINITY, published = INFINITY;
             for (int n0 = U.n_begin; n0 < U.n_end; n0 += BN, tile++) {
-                const unsigned acc = tile & 1;
-                // |x|^2 of this tile's rows -> shared (2 per thread); named barrier over the 128 epilogue threads
-                for (int j = e; j < BN; j += 128) S.xn[acc][j] = (n0 + j < U.n_end) ? xnorm[n0 + j] : INFINITY;
+                const unsigned xb = tile & 1;
+                // |x|^2 of this tile's rows -> shared (one per thread); named barrier over the 128 epilogue threads
+                for (int j = e; j < BN; j += 128) S.xn[xb][j] = (n0 + j < U.n_end) ? xnorm[n0 + j] : INFINITY;
                 asm volatile("bar.sync 1, 128;" ::: "memory");
-                mbar_wait(&S.tmem_full[acc], (tile >> 1) & 1);
-                tc_fence_after();
+                mbar_wait(&S.acc_full, tile & 1);
                 const int ncols = U.n_end - n0 < BN ? U.n_end - n0 : BN;
                 if (share) {
                     const float b = __ldcg(&qbound[qid]);
                     if (b < INFINITY) { cap = fminf(cap, b + my_eps + b * rel_margin + abs_margin + 1e-30f); thr = fminf(thr, cap); }
                 }
-                const unsigned trow = tmem_base + ((unsigned)(32 * ew) << 16) + acc * BN;
 #pragma unroll 1
                 for (int c = 0; c < ncols; c += 32) {
-                    float v[32];
-                    tc_ld32_issue(trow + c, v);
-                    tc_ld32_wait(v);
                     // fast path: 32 approximate distances and their minimum, branch-free (independent FADD/FFMA/FMNMX chains)
+                    float v[32];
                     float dmin = INFINITY;
 #pragma unroll
                     for (int j4 = 0; j4 < 32; j4 += 4) {
-                        const float4 xn4 = *reinterpret_cast<const float4 *>(&S.xn[acc][c + j4]);   // +inf for rows past the end
-                        v[j4 + 0] = fmaf(-2.0f, v[j4 + 0], qn + xn4.x); v[j4 + 1] = fmaf(-2.0f, v[j4 + 1], qn + xn4.y);
-                        v[j4 + 2] = fmaf(-2.0f, v[j4 + 2], qn + xn4.z); v[j4 + 3] = fmaf(-2.0f, v[j4 + 3], qn + xn4.w);
+                        const float4 xn4 = *reinterpret_cast<const float4 *>(&S.xn[xb][c + j4]);   // +inf for rows past the end
+                        v[j4 + 0] = fmaf(-2.0f, S.acc[c + j4 + 0][e], qn + xn4.x); v[j4 + 1] = fmaf(-2.0f, S.acc[c + j4 + 1][e], qn + xn4.y);
+                        v[j4 + 2] = fmaf(-2.0f, S.acc[c + j4 + 2][e], qn + xn4.z); v[j4 + 3] = fmaf(-2.0f, S.acc[c + j4 + 3][e], qn + xn4.w);
                         dmin = fminf(fminf(dmin, fminf(v[j4 + 0], v[j4 + 1])), fminf(v[j4 + 2], v[j4 + 3]));
                     }
                     // slow path (some element beats the list's worst entry): the insertion code exists ONCE -- the hits are walked
-                    // through a bit mask and fetched from a per-thread shared-memory column (dynamic register indexing is impossible,
+                    // through a bit mask and their distances recomputed from the shared tile (dynamic register indexing is impossible,
                     // and 32 unrolled copies of the sweep would not fit the instruction cache)
                     if (dmin < thr) {
                         unsigned hit = 0;
 #pragma unroll
-                        for (int j = 0; j < 32; j++) { S.scratch[j][e] = v[j]; hit |= (v[j] < thr) ? (1u << j) : 0u; }
+                        for (int j = 0; j < 32; j++) hit |= (v[j] < thr) ? (1u << j) : 0u;
 #pragma unroll 1
                         while (hit) {
                             const int j = __ffs((int)hit) - 1;
                             hit &= hit - 1;
-                            const float d = S.scratch[j][e];
+                            const float d = fmaf(-2.0f, S.acc[c + j][e], qn + S.xn[xb][c + j]);   // the same value as v[j]
                             if (d < thr) {   // thr may have dropped since the mask was taken
                                 const int id = n0 + c + j;
 #pragma unroll
@@ -392,18 +358,13 @@ tc_candidates_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                         }
                     }
                 }
+                mbar_arrive(&S.acc_empty);   // 128 arrivals release the shared tile to the MMA warpgroup
                 if (share && topk <= KPT) {   // the k best rows seen by this unit bound the query's k-th real distance from above
                     float kth = INFINITY;
 #pragma unroll
                     for (int j = 0; j < KPT; j++) if (j == topk - 1) kth = ld[j];
                     const float pb = fmaxf(kth + my_eps, 0.f);
                     if (pb < published) { published = pb; atomicMin(reinterpret_cast<int *>(&qbound[qid]), __float_as_int(pb)); }
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) {   // 4 (8 in a pair) arrivals, one per epilogue warp, release the accumulator to the MMA issuer
-                    if (PAIR) mbar_arrive_cluster(acc ? tmem_empty_leader1 : tmem_empty_leader0);
-                    else mbar_arrive(&S.tmem_empty[acc]);
                 }
             }
             if (valid_row) {
@@ -414,13 +375,8 @@ tc_candidates_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
             }
         }
     }
-    tc_fence_before();
     __syncthreads();
-    if (PAIR) cluster_sync_all();   // the leader's MMAs read the peer's shared memory and signal its barriers: leave together
-    if (warp == 2) {
-        if (PAIR) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-    }
+    if (PAIR) cluster_sync_all();   // the peer multicasts into this CTA's shared memory and arrives on its barriers: leave together
 }
 
 // ---- operand preparation -------------------------------------------------------------------------------------------------
@@ -881,7 +837,7 @@ static int tc_run_units(ThreadCtx &t, const TcOperand &A, int64_t a_rows, const 
     MOB_CUDA_TRY(cudaMemcpyAsync(dunits, units.data(), sizeof(TcUnit) * units.size(), cudaMemcpyHostToDevice, t.stream));
     MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
     static bool attr = false;
-    const size_t smem1 = sizeof(TcSmemT<false>) + 1024, smem2 = sizeof(TcSmemT<true>) + 1024;
+    const size_t smem1 = sizeof(TcSmem) + 1024, smem2 = smem1;
     if (!attr) {
         MOB_CUDA_TRY(cudaFuncSetAttribute(tc_candidates_kernel<false, KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
         MOB_CUDA_TRY(cudaFuncSetAttribute(tc_candidates_kernel<false, KP_LONG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
@@ -915,7 +871,7 @@ static int tc_run_units(ThreadCtx &t, const TcOperand &A, int64_t a_rows, const 
         else tc_candidates_kernel<false, KP><<<grid, kTcThreads, smem1, t.stream>>>(map_a, map_b, dunits, nunits, nkb, A.enorm ? A.enorm : A.norm, B.enorm ? B.enorm : B.norm, *part_d, *part_i, *part_thr, qbound, row_query, alonorm, xmax2, sh_one, sh_k, sh_rel, sh_abs, sched);
     } else {
         if (kp != KP) { set_error("tc search: CTA pairs keep %d candidates per list", KP); return MO_RC_INTERNAL_ERROR; }
-        // clusters of two CTAs (one TPC each): one persistent pair per two SMs
+        // clusters of two CTAs that share the B tile: one persistent pair per two SMs
         int pairs = num_sms() / 2;
         if (pairs > nunits) pairs = nunits;
         cudaLaunchConfig_t cfg = {};
@@ -1083,7 +1039,7 @@ static int bf_tc_level(ThreadCtx &t, int level, int metric, const float *ddata, 
     const bool one_term = level == 0;
     const int nkb = one_term ? (dim + BK - 1) / BK : A.kprime / BK;
     // work units: (query tile, row range); ranges sized so that units ~ a whole number of waves over the SMs
-    // enough queries to fill 256-row tiles: CTA pairs (cta_group::2) stage 1.5x fewer bytes per flop
+    // enough queries to fill 256-row units: CTA pairs share the B tile (TMA multicast) and load 1.33x fewer bytes per flop
     const bool pair = g_tc_pair_mode == 2 || (g_tc_pair_mode == 0 && nq >= 1024);
     const int tile_m = pair ? TcCfg<true>::kTileM : TcCfg<false>::kTileM;
     const int mt = (int)((nq + tile_m - 1) / tile_m);

@@ -11,7 +11,7 @@
 //
 // Mapping: a "pair" is two consecutive rows.  Lane l of a warp owns pair (w*32 + l), so one warp instruction reads
 // 64 consecutive rows: 256 B of the int32 column (LDG.64/lane) and 512 B of each float64 column (LDG.128/lane) --
-// whole 32-byte sectors, nothing fetched twice.  kUnroll pairs are in flight per thread; grid = 148 x CTAs/SM
+// whole 32-byte sectors, nothing fetched twice.  kUnroll pairs are in flight per thread; grid = SMs x CTAs/SM
 // persistent CTAs, grid-stride.  Products are rounded exactly as the reference's separate multiply / add nodes do
 // (__dmul_rn/__dadd_rn, no FMA contraction), so only the summation ORDER differs from the serial Go loop.
 // Reduction: registers -> warp shuffles -> shared memory -> per-CTA record; the last CTA (atomicInc ticket) folds

@@ -92,16 +92,16 @@ def build_usearch_ref(force=False):
 
 
 def build_mocl_ref(force=False):
-    """the reference's own CUDA kernels (cgo/cuda/mocl.cu:4-92: l2distance_f32/_f64[_const], one thread per row), compiled UNCHANGED for sm_100a into a
+    """the reference's own CUDA kernels (cgo/cuda/mocl.cu:4-92: l2distance_f32/_f64[_const], one thread per row), compiled UNCHANGED for sm_90a into a
     cubin.  The reference ships them as mocl_kernel64.fatbin loaded with cuModuleLoad (cgo/cuda/cuda.cpp:82-95); tools/ref_cuda_compare.py loads
     this cubin the same way and times the kernels next to ours (SURVEY.md section 2.3 bar (ii))."""
-    out = os.path.join(REF_DIR, "mocl_sm100a.cubin")
+    out = os.path.join(REF_DIR, "mocl_sm90a.cubin")
     src = os.path.join(REF, "cgo", "cuda", "mocl.cu")
     if not os.path.exists(src):
         return out if os.path.exists(out) else None
     if force or _newer(out, [src]):
         os.makedirs(REF_DIR, exist_ok=True)
-        _run([os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc"), "-cubin", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-o", out, src])
+        _run([os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc"), "-cubin", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-o", out, src])
     return out
 
 

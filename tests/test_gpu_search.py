@@ -121,10 +121,10 @@ def test_ivf_empty_lists_and_small_index(gpu):
 
 @pytest.mark.parametrize("n,dim,nq,k", [(20_000, 128, 300, 10), (9_000, 768, 257, 10), (5_000, 100, 130, 5), (70_000, 64, 1000, 16), (300, 32, 40, 3),
                                         (20_000, 96, 200, 32), (1_024, 64, 500, 25)])   # k > 16: the wide mode of centroid probes
-@pytest.mark.parametrize("pair", [1, 2])   # 1: single-CTA units (cta_group::1), 2: CTA pairs (cta_group::2, M = 256)
+@pytest.mark.parametrize("pair", [1, 2])   # 1: single-CTA units (128 queries), 2: CTA pairs (a cluster of two sharing the row tile, 256 queries)
 @pytest.mark.parametrize("ladder", [1, 2])  # 1: three-term product only, 2: hi-only level first, then three-term for the unproven
 def test_tensor_core_candidate_path_is_exact(gpu, n, dim, nq, k, pair, ladder):
-    """tcgen05 candidate generation + exact re-scoring + completeness proof (csrc/tcsearch.cu): the results must be the exact
+    """tensor-core (wgmma) candidate generation + exact re-scoring + completeness proof (csrc/tcsearch.cu): the results must be the exact
     answer (bit-exact distances), and the tensor path itself must be doing the work (few proof failures -> few fallbacks)."""
     ds = datagen.vectors_f32(40, 0, n, dim); qs = datagen.vectors_f32(41, 0, nq, dim)
     qs[:7] = ds[[0, 5, n // 2, n - 1, 17, 100, 255]]          # self matches: exact distance 0

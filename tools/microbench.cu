@@ -1,5 +1,5 @@
-// microbench.cu -- pipe-throughput probes for B200 (sm_100a): lane-ops per clock per SM for the arithmetic the kernels
-// lean on.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench tools/microbench.cu
+// microbench.cu -- pipe-throughput probes for H100 (sm_90a): lane-ops per clock per SM for the arithmetic the kernels
+// lean on.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench tools/microbench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,6 +1,6 @@
 """Resident-column timings of the operator kernels that have no bench.py workload of their own (generic fused plan, filter->sels, Shrink,
 first-seen group ids, grouped aggregates, decimal SUM): CUDA-event kernel time through MoB200_LastKernelMs, GB/s of ALGORITHMIC bytes.
-Also the command ncu captures are taken on (tools/profile_r02.sh).   python tools/profile_ops.py [rows] > gpurun_out/r02_ops.json"""
+    python tools/profile_ops.py [rows] > ops.json"""
 import ctypes as C
 import json
 import os

@@ -1,8 +1,8 @@
-"""Kernel-vs-kernel: the reference's OWN CUDA kernels (cgo/cuda/mocl.cu, compiled unchanged by oracle/build.py into oracle/_ref/mocl_sm100a.cubin)
+"""Kernel-vs-kernel: the reference's OWN CUDA kernels (cgo/cuda/mocl.cu, compiled unchanged by oracle/build.py into oracle/_ref/mocl_sm90a.cubin)
 against this library's row-distance kernel, both on RESIDENT data (the reference's shim additionally allocates + copies per call, cuda.cpp:123-201;
 that cost is not charged here).  2 M rows x 768-d f32, one side constant and both sides per-row; device time by CUDA events.
 
-    python tools/ref_cuda_compare.py > gpurun_out/ref_cuda_compare.json
+    python tools/ref_cuda_compare.py > ref_cuda_compare.json
 """
 import ctypes as C
 import json
@@ -34,7 +34,7 @@ def main():
     dev = ck(cu.cuDeviceGet(0))
     ctx = ck(cu.cuDevicePrimaryCtxRetain(dev))          # the runtime's primary context: the library's device pointers are valid in it
     ck(cu.cuCtxSetCurrent(ctx))
-    cubin = open(os.path.join(ROOT, "oracle", "_ref", "mocl_sm100a.cubin"), "rb").read()
+    cubin = open(os.path.join(ROOT, "oracle", "_ref", "mocl_sm90a.cubin"), "rb").read()
     mod = ck(cu.cuModuleLoadData(cubin))
     f_const = ck(cu.cuModuleGetFunction(mod, b"l2distance_f32_const"))
     f_vv = ck(cu.cuModuleGetFunction(mod, b"l2distance_f32"))

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""One-call kernel survey for a gpurun slot: every hot kernel at a bench-like size, variants side by side.
+"""One-call kernel survey on a GPU: every hot kernel at a bench-like size, variants side by side.
 Prints one JSON line per measurement (kernel-only CUDA-event time via MoB200_LastKernelMs, median of `reps`)."""
 import ctypes as C
 import json
