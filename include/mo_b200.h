@@ -313,18 +313,22 @@ typedef struct mo_dec_params_t { int32_t scale1, scale2; int64_t err_row; } mo_d
  * What the colexec pipeline runs per block as table_scan -> filter -> projection -> group (filter.go:87-153, evalExpression.go:575-640,
  * group/exec2.go:296-367, aggexec/*), described by a host-side mo_plan_t:
  *   columns      args[2 .. 2+ncols): fixed-width columns of col_type[c] (MO_T_*), each with an optional nulls bitmap
- *   predicates   conjunction of  col OP lo  (OP: 0 == 1 != 2 > 3 >= 4 < 5 <=)  or  col BETWEEN lo AND hi (op 6); a NULL operand rejects the row
+ *   predicates   conjunction of  col OP lo  (OP: 0 == 1 != 2 > 3 >= 4 < 5 <=)  or  col BETWEEN lo AND hi (op 6, inclusive); a NULL operand
+ *                rejects the row.  The column value is compared with the float64 constant exactly (integer columns of any magnitude, UINT64
+ *                unsigned), as the reference does once the constant is cast to the column type; a NaN constant: only != holds (IEEE)
  *   instructions SSA program: value slot ncols + i = COL(a) | CONST(imm) | slot a (+ - * /) slot b; slots 0..ncols-1 are the columns.  float64
  *                arithmetic, one rounding per instruction (the reference evaluates one node at a time); integer columns are converted (exact
- *                below 2^53); NULL in -> NULL out; x / 0 -> NULL
- *   keys         nkeys columns packed into <= 8 bytes exactly like fillKeys (inthashmap.go:92-183; has_null_keys: marker byte per column)
+ *                below 2^53; MIN / MAX of an integer column above 2^53 is of the rounded value); NULL in -> NULL out; x / 0 and x / -0.0 -> NULL
+ *   keys         nkeys columns packed into <= 8 bytes exactly like fillKeys (inthashmap.go:92-183; has_null_keys: marker byte per column, a NULL
+ *                key writes the marker 1 only; without has_null_keys a row with a NULL key joins no group, inthashmap.go:171-180)
  *   aggregates   kind MO_AGG_SUM / COUNT / MIN / MAX / AVG over value slot `value`; value = -1 with MO_AGG_COUNT is COUNT(*)
  * Result: mo_plan_result_header_t followed by ngroups records {mo_plan_group_t, naggs x mo_plan_agg_value_t}, groups in first-seen row order
  * (the reference's group-id order) when header.sorted (up to 8192 groups; beyond that in table order, first_row is there to sort by).  An
  * aggregate with count 0 is NULL.  No group-by (nkeys = 0): one group, present only if a row qualified.  header.overflow = more groups than the
  * result buffer holds (synchronous form: MO_RC_INVALID_ARGUMENT).  Device columns AND a device result: asynchronous form (as MO_XCALL_AGG).
- * float64 sums are accumulated with atomics: the association order is not fixed (agreement with the serial loop ~1e-13 relative); MIN / MAX
- * ignore NaN.  The TPC-H Q6 / Q1 shapes below are hand-specialised instances of this operator that reach the HBM roofline. */
+ * float64 sums are accumulated with atomics: the association order is not fixed (|sum - exact| <= count * 2^-52 * sum |x|); MIN / MAX
+ * ignore NaN (a group whose values are all NaN gives NaN with count > 0) and do not tell -0.0 from 0.0.  The specialised Q6 kernel reports
+ * first_row = -1.  The TPC-H Q6 / Q1 shapes below are hand-specialised instances of this operator that reach the HBM roofline. */
 #define MO_XCALL_PLAN 0x2100
 #define MO_PLAN_MAX_COLS 12
 #define MO_PLAN_MAX_PREDS 8

@@ -111,8 +111,12 @@ struct PlanAux {                       // host-prepared decode of the descriptor
     int sz[MO_PLAN_MAX_COLS];          // element width in bytes
     int ext[MO_PLAN_MAX_COLS];         // after the load: 0 nothing (zero-extended), 1 / 2 / 3 sign-extend from 8 / 16 / 32 bits
     int tof[MO_PLAN_MAX_COLS];         // then: 0 keep, 1 int64 -> float64, 2 uint64 -> float64, 3 float32 bits -> float64
-    int pred_int[MO_PLAN_MAX_PREDS];   // predicate compares in the integer domain (the slot holds a raw int64)
+    int pred_mode[MO_PLAN_MAX_PREDS];  // 0 float64 slot vs P.pred lo / hi, 1 raw int64 vs ilo / ihi, 2 raw uint64 vs ilo / ihi (unsigned),
+                                       // 3 never true, 4 true unless the operand is NULL
+    int pred_slot[MO_PLAN_MAX_PREDS];  // PHYSICAL slot the predicate reads
     long long ilo[MO_PLAN_MAX_PREDS], ihi[MO_PLAN_MAX_PREDS];
+    int raw_phys[MO_PLAN_MAX_COLS];    // -1, or a physical slot keeping the column's raw integer for predicates when its own slot turns float64
+    unsigned key_nulls;                // null bits of the nullable key columns (has_null_keys == 0: a row with a NULL key joins no group)
     int key_mode[MO_PLAN_MAX_KEYS];    // 0 raw integer slot, 1 float64 slot holding an integer (exact: < 8-byte types), 2 reload the 8 bytes from the column,
                                        // 3 float64 slot holding a float32 (key = its float32 bits), 4 float64 bits
     int key_shift[MO_PLAN_MAX_KEYS];   // bit offset of the column inside the packed key when has_null_keys == 0
@@ -203,6 +207,8 @@ plan_kernel(const mo_plan_t *__restrict__ Pg, const PlanAux *__restrict__ Ag, Pl
                     if (ext == 3) { PLAN_FORJ raw[g][j] = (unsigned long long)(long long)(int32_t)raw[g][j]; }
                     else if (ext == 2) { PLAN_FORJ raw[g][j] = (unsigned long long)(long long)(int16_t)raw[g][j]; }
                     else if (ext == 1) { PLAN_FORJ raw[g][j] = (unsigned long long)(long long)(int8_t)raw[g][j]; }
+                    const int rp = X.raw_phys[c];
+                    if (rp >= 0) { PLAN_FORJ PLAN_SLOT(rp, j) = raw[g][j]; }
                     if (tof == 1) { PLAN_FORJ raw[g][j] = (unsigned long long)__double_as_longlong((double)(long long)raw[g][j]); }
                     else if (tof == 2) { PLAN_FORJ raw[g][j] = (unsigned long long)__double_as_longlong((double)raw[g][j]); }
                     else if (tof == 3) { PLAN_FORJ raw[g][j] = (unsigned long long)__double_as_longlong((double)__uint_as_float((unsigned)raw[g][j])); }
@@ -213,7 +219,7 @@ plan_kernel(const mo_plan_t *__restrict__ Pg, const PlanAux *__restrict__ Ag, Pl
         }
         // ---- filter: conjunction; a NULL operand makes the conjunct not-true (filter.go:125-141 keeps rows with !null && true)
         for (int q = 0; q < P.npreds; q++) {
-            const int c = P.pred[q].col, op = P.pred[q].op, pc = X.phys[c];
+            const int c = P.pred[q].col, op = P.pred[q].op, pc = X.pred_slot[q], mode = X.pred_mode[q];
 #define PLAN_PRED(XT, LOADX, EXPR) PLAN_FORJ { const XT x = LOADX; ok[j] = ok[j] && (EXPR) && !((nb[j] >> c) & 1u); }
 #define PLAN_PRED_SWITCH(XT, LOADX)                                       \
             switch (op) {                                                 \
@@ -225,14 +231,21 @@ plan_kernel(const mo_plan_t *__restrict__ Pg, const PlanAux *__restrict__ Ag, Pl
             case 5: PLAN_PRED(XT, LOADX, x <= lo) break;                  \
             default: PLAN_PRED(XT, LOADX, x >= lo && x <= hi) break;      /* BETWEEN, inclusive (operator_between.go:138-199) */ \
             }
-            if (X.pred_int[q]) {
+            if (mode == 1) {
                 const long long lo = X.ilo[q], hi = X.ihi[q];
                 PLAN_PRED_SWITCH(long long, (long long)PLAN_SLOT(pc, j))
-            } else {
+            } else if (mode == 2) {
+                const unsigned long long lo = (unsigned long long)X.ilo[q], hi = (unsigned long long)X.ihi[q];
+                PLAN_PRED_SWITCH(unsigned long long, PLAN_SLOT(pc, j))
+            } else if (mode == 0) {
                 const double lo = P.pred[q].lo, hi = P.pred[q].hi;
                 PLAN_PRED_SWITCH(double, __longlong_as_double((long long)PLAN_SLOT(pc, j)))
+            } else {
+                const bool t = mode == 4;
+                PLAN_FORJ ok[j] = ok[j] && t && !((nb[j] >> c) & 1u);
             }
         }
+        if (!P.has_null_keys && X.key_nulls) { const unsigned kn = X.key_nulls; PLAN_FORJ ok[j] = ok[j] && !(nb[j] & kn); }   // fillKeys: zValues[i] = 0
         if (!(ok[0] | ok[1] | ok[2] | ok[3])) continue;
         // ---- group keys (fillKeys): one column at a time.  BEFORE the projection: keys only read column slots, which the expression nodes may reuse
         uint64_t keys[R];
@@ -288,10 +301,11 @@ plan_kernel(const mo_plan_t *__restrict__ Pg, const PlanAux *__restrict__ Ag, Pl
             ps[j] = -1;
             if (ok[j]) {
                 const uint64_t key = keys[j];
+                const bool sentinel = key == kEmptyKey;    // the all-ones key is also the empty-entry marker: it never gets private state
                 int p = -1;
 #pragma unroll
-                for (int g = 0; g < kPriv; g++) if (dk[g] == key) p = g;
-                if (p < 0 && !dict_full && key != kEmptyKey) {
+                for (int g = 0; g < kPriv; g++) if (dk[g] == key && !sentinel) p = g;
+                if (p < 0 && !dict_full && !sentinel) {
                     bool okc = false;
 #pragma unroll
                     for (int g = 0; g < kPriv; g++) {
@@ -667,7 +681,6 @@ int xcall_plan(mo_xcall_args_t *args, uint64_t len) {
     memset(&X, 0, sizeof X);
     {
         auto is_float = [](int T) { return T == MO_T_FLOAT32 || T == MO_T_FLOAT64; };
-        auto integral = [](double v) { return v == std::floor(v) && std::fabs(v) < 9007199254740992.0; };
         bool value_use[MO_PLAN_MAX_COLS] = {false}, f64dom[MO_PLAN_MAX_COLS];
         for (int i = 0; i < P.ninstr; i++) {
             const mo_plan_instr_t &in = P.instr[i];
@@ -676,18 +689,47 @@ int xcall_plan(mo_xcall_args_t *args, uint64_t len) {
             if (in.op >= MO_PLAN_OP_ADD && in.b < P.ncols) value_use[in.b] = true;
         }
         for (int a = 0; a < P.naggs; a++) if (P.agg[a].value >= 0 && P.agg[a].value < P.ncols) value_use[P.agg[a].value] = true;
-        bool intable[MO_PLAN_MAX_PREDS];
-        for (int c = 0; c < P.ncols; c++) f64dom[c] = is_float(P.col_type[c]) || value_use[c];
+        for (int c = 0; c < P.ncols; c++) { f64dom[c] = is_float(P.col_type[c]) || value_use[c]; X.raw_phys[c] = -1; }
+        // A predicate on an integer column compares the value with the float64 constant exactly (what the reference computes once the planner
+        // has cast the constant to the column type): x > c <=> x > floor(c), x >= c <=> x >= ceil(c), == a non-integral c never holds.  The
+        // integral bound is then compared in the 64-bit integer domain of the slot (unsigned for UINT64); a bound outside it decides the
+        // predicate for every row.  A NaN constant follows IEEE: only != holds.
+        const double two63 = 9223372036854775808.0, two64 = 18446744073709551616.0, two53 = 9007199254740992.0;
+        int nphys = P.ncols;
         for (int j = 0; j < P.npreds; j++) {
             const mo_plan_pred_t &q = P.pred[j];
-            intable[j] = !is_float(P.col_type[q.col]) && P.col_type[q.col] != MO_T_UINT64 && integral(q.lo) && (q.op != 6 || integral(q.hi));
-            if (!intable[j]) f64dom[q.col] = true;
+            const int c = q.col, T = P.col_type[c];
+            X.pred_slot[j] = c;
+            X.pred_mode[j] = 0;
+            if (is_float(T)) continue;
+            const bool uns = T == MO_T_UINT64;
+            const double dmin = uns ? 0.0 : -two63, dmax = uns ? two64 : two63;   // the domain is [dmin, dmax)
+            auto to_int = [&](double t) { return uns ? (long long)(unsigned long long)t : (long long)t; };
+            int mode = uns ? 2 : 1;
+            double lo = 0.0, hi = 0.0;
+            if (q.op == 6) {
+                lo = std::ceil(q.lo); hi = std::floor(q.hi);
+                if (q.lo != q.lo || q.hi != q.hi || lo >= dmax || hi < dmin) mode = 3;
+                else { lo = lo < dmin ? dmin : lo; X.ilo[j] = to_int(lo); X.ihi[j] = hi >= dmax ? (uns ? -1ll : 0x7fffffffffffffffll) : to_int(hi); }
+            } else if (q.lo != q.lo) {
+                mode = q.op == 1 ? 4 : 3;
+            } else {
+                lo = (q.op == 2 || q.op == 5) ? std::floor(q.lo) : (q.op == 3 || q.op == 4) ? std::ceil(q.lo) : q.lo;
+                if ((q.op == 0 || q.op == 1) && lo != std::floor(lo)) mode = q.op == 1 ? 4 : 3;     // == a non-integral constant
+                else if (lo >= dmax) mode = (q.op == 1 || q.op == 4 || q.op == 5) ? 4 : 3;            // above every value (also +inf)
+                else if (lo < dmin) mode = (q.op == 1 || q.op == 2 || q.op == 3) ? 4 : 3;             // below every value (also -inf)
+                else X.ilo[j] = to_int(lo);
+            }
+            X.pred_mode[j] = mode;
+            if (!f64dom[c] || mode > 2) continue;
+            // the column's slot holds float64(x): exact for a bound below 2^53 in magnitude (rounding is monotonic and c +- 1 are
+            // representable), so the float64 compare with the original constant is kept; larger bounds read a raw copy of the column
+            if (std::fabs(lo) < two53 && (q.op != 6 || std::fabs(hi) < two53)) { X.pred_mode[j] = 0; continue; }
+            if (X.raw_phys[c] < 0) X.raw_phys[c] = nphys++;
+            X.pred_slot[j] = X.raw_phys[c];
         }
-        for (int j = 0; j < P.npreds; j++) {
-            const mo_plan_pred_t &q = P.pred[j];
-            X.pred_int[j] = intable[j] && !f64dom[q.col];
-            if (X.pred_int[j]) { X.ilo[j] = (long long)q.lo; X.ihi[j] = q.op == 6 ? (long long)q.hi : 0; }
-        }
+        X.key_nulls = 0;
+        for (int k = 0; k < P.nkeys; k++) if (args[2 + P.key_col[k]].pnulls) X.key_nulls |= 1u << P.key_col[k];
         for (int c = 0; c < P.ncols; c++) {
             const int T = P.col_type[c];
             X.sz[c] = tbytes(T);
@@ -725,11 +767,13 @@ int xcall_plan(mo_xcall_args_t *args, uint64_t len) {
             if (in.op >= MO_PLAN_OP_ADD) use(in.b, 3 + i);
         }
         for (int a = 0; a < P.naggs; a++) use(P.agg[a].value, t_agg);
-        bool busy[MO_PLAN_MAX_COLS + MO_PLAN_MAX_INSTR] = {false};
+        bool busy[2 * MO_PLAN_MAX_COLS + MO_PLAN_MAX_INSTR] = {false};
         int nphys = P.ncols;
         for (int c = 0; c < P.ncols; c++) { X.phys[c] = c; busy[c] = true; }
+        for (int c = 0; c < P.ncols; c++) if (X.raw_phys[c] >= 0) { busy[X.raw_phys[c]] = true; nphys = std::max(nphys, X.raw_phys[c] + 1); }
         for (int i = 0; i < P.ninstr; i++) {
             const int now = 3 + i, dst = P.ncols + i;
+            if (i == 0) for (int c = 0; c < P.ncols; c++) if (X.raw_phys[c] >= 0) busy[X.raw_phys[c]] = false;   // raw copies die with the filter
             // values whose last reader is this node or an earlier phase give their slot back (a node may overwrite its own operand: every
             // (thread, row) cell is read before it is written)
             for (int v = 0; v < dst; v++) if (busy[X.phys[v]] && last[v] <= now) {
