@@ -120,6 +120,16 @@ __device__ __forceinline__ int2 ld_stream8(const void *p) {
     asm volatile("ld.global.nc.L1::no_allocate.v2.s32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
     return r;
 }
+// Two float64 through ld_stream16 under a per-lane predicate: +0.0 where `pred` is false, and no memory access.  One predicated
+// instruction, not a lane-dependent branch region (DESIGN 5.1).  Typed .f64: with .s32 outputs ptxas copied every result out of the
+// load's destination registers, which waits for the load.
+__device__ __forceinline__ double2 ld_stream16_f64_if(bool pred, const double *p) {
+    double2 r;
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\tmov.f64 %0, 0d0000000000000000;\n\tmov.f64 %1, 0d0000000000000000;\n\t"
+                 "@q ld.global.nc.L1::no_allocate.v2.f64 {%0, %1}, [%3];\n\t}"
+                 : "=d"(r.x), "=d"(r.y) : "r"((int)pred), "l"(p));
+    return r;
+}
 __device__ __forceinline__ void st_stream16(void *p, int4 v) {
     asm volatile("st.global.L1::no_allocate.v4.s32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w));
 }

@@ -3,9 +3,11 @@
 // The reference runs these as an operator chain that materialises a vector per expression node and compacts every
 // column after each conjunct (table_scan -> filter -> projection -> group: pkg/sql/colexec/filter/filter.go:87-153,
 // pkg/sql/colexec/group/exec2.go:296-367, aggexec/sumavg2.go:133-199).  Here each shape is ONE pass over the
-// columns: every byte is read from HBM exactly once, nothing is written but a few hundred bytes of partials.
+// columns, no byte is read twice, nothing is written but a few hundred bytes of partials.  Q1 reads every byte (~98 % of its
+// rows pass).  Q6 reads shipdate whole and each later column only in the DRAM blocks where a row is still alive after the earlier
+// conjuncts, like the reference's conjunct-by-conjunct filter: on TPC-H data 13 B/row at 64-byte blocks instead of 28 (DESIGN 5.1).
 //
-//   Q6  SUM(price*disc) WHERE date in [lo,hi) AND disc BETWEEN a AND b AND qty < c     28 B/row   (q6.sql:50-61)
+//   Q6  SUM(price*disc) WHERE date in [lo,hi) AND disc BETWEEN a AND b AND qty < c     28 B/row algorithmic (q6.sql:50-61)
 //   Q1  filter date <= cutoff, group by (returnflag, linestatus), 8 aggregates          38 B/row packed keys,
 //                                                                                        84 B/row varlena keys (q1.sql:1-21)
 //
@@ -34,54 +36,21 @@ struct Q6Rec { double sum; unsigned long long cnt; };
 // "no row qualified" -- the layout MO_XCALL_Q6_MERGE consumes
 struct Q6DevOut { double *res; uint64_t res_words; uint64_t *rnulls; };
 
-template <int UNROLL, int CTAS>
-__global__ void __launch_bounds__(kThreads, CTAS)
-q6_kernel(const int32_t *__restrict__ sd, const double *__restrict__ disc, const double *__restrict__ qty,
-          const double *__restrict__ price, uint64_t n, mo_q6_params_t P, Q6Rec *__restrict__ partials,
-          Q6Rec *__restrict__ out, unsigned *ticket, Q6DevOut dres) {
-    const uint64_t npairs = n >> 1;
-    const uint64_t tid = blockIdx.x * (uint64_t)kThreads + threadIdx.x;
-    const uint64_t nthreads = (uint64_t)gridDim.x * kThreads;
-    double s0 = 0.0, s1 = 0.0;
-    unsigned cnt = 0;  // a thread sees < 2^32 rows
+// SUM node over one row: the projection l_extendedprice * l_discount is added where the row passed all three conjuncts, +0.0 elsewhere
+// (s starts at +0.0 and can never become -0.0 under round-to-nearest, so s + 0.0 == s)
+__device__ __forceinline__ void q6_add(bool ok, double di, double pr, double &s, unsigned &cnt) {
+    double prod = __dmul_rn(pr, di);             // projection node l_extendedprice * l_discount
+    s = __dadd_rn(s, ok ? prod : 0.0);           // SUM node
+    cnt += ok;
+}
+__device__ __forceinline__ void q6_row(const mo_q6_params_t &P, int32_t d, double di, double q, double pr, double &s, unsigned &cnt) {
+    q6_add((d >= P.date_lo) & (d < P.date_hi) & (di >= P.disc_lo) & (di <= P.disc_hi) & (q < P.qty_hi), di, pr, s, cnt);
+}
 
-    auto row = [&](int32_t d, double di, double q, double pr, double &s) {
-        bool ok = (d >= P.date_lo) & (d < P.date_hi) & (di >= P.disc_lo) & (di <= P.disc_hi) & (q < P.qty_hi);
-        double prod = __dmul_rn(pr, di);             // projection node l_extendedprice * l_discount
-        s = __dadd_rn(s, ok ? prod : 0.0);           // SUM node; +0.0 leaves s unchanged (s is never -0.0)
-        cnt += ok;
-    };
-
-    uint64_t p = tid;
-    for (; p + (UNROLL - 1) * nthreads < npairs; p += UNROLL * nthreads) {
-        int2 d[UNROLL]; int4 a[UNROLL], b[UNROLL], c[UNROLL];
-#pragma unroll
-        for (int k = 0; k < UNROLL; k++) {
-            const uint64_t q = p + k * nthreads;
-            d[k] = ld_stream8(sd + 2 * q);
-            a[k] = ld_stream16(disc + 2 * q);
-            b[k] = ld_stream16(qty + 2 * q);
-            c[k] = ld_stream16(price + 2 * q);
-        }
-#pragma unroll
-        for (int k = 0; k < UNROLL; k++) {
-            double di[2], qq[2], pr[2];
-            memcpy(di, &a[k], 16); memcpy(qq, &b[k], 16); memcpy(pr, &c[k], 16);
-            row(d[k].x, di[0], qq[0], pr[0], s0);
-            row(d[k].y, di[1], qq[1], pr[1], s1);
-        }
-    }
-    for (; p < npairs; p += nthreads) {
-        int2 d = ld_stream8(sd + 2 * p);
-        int4 a = ld_stream16(disc + 2 * p), b = ld_stream16(qty + 2 * p), c = ld_stream16(price + 2 * p);
-        double di[2], qq[2], pr[2];
-        memcpy(di, &a, 16); memcpy(qq, &b, 16); memcpy(pr, &c, 16);
-        row(d.x, di[0], qq[0], pr[0], s0);
-        row(d.y, di[1], qq[1], pr[1], s1);
-    }
-    if ((n & 1) && tid == 0) row(sd[n - 1], disc[n - 1], qty[n - 1], price[n - 1], s0);  // odd tail row
-
-    // ---- deterministic reduction
+// deterministic reduction of the per-thread state: warp shuffles, shared memory, per-CTA record; the last CTA folds the records in
+// CTA-index order
+__device__ __forceinline__ void q6_finish(double s0, double s1, unsigned cnt, Q6Rec *__restrict__ partials, Q6Rec *__restrict__ out,
+                                          unsigned *ticket, Q6DevOut dres) {
     double s = __dadd_rn(s0, s1);
     unsigned long long c64 = cnt;
     s = warp_sum_f64(s);
@@ -122,6 +91,127 @@ q6_kernel(const int32_t *__restrict__ sd, const double *__restrict__ disc, const
             }
         }
     }
+}
+
+// Dense scan: all four columns of every pair.  Selected by q6_variant = 1: the arm the selective kernel is timed and tested against.
+template <int UNROLL, int CTAS>
+__global__ void __launch_bounds__(kThreads, CTAS)
+q6_kernel(const int32_t *__restrict__ sd, const double *__restrict__ disc, const double *__restrict__ qty,
+          const double *__restrict__ price, uint64_t n, mo_q6_params_t P, Q6Rec *__restrict__ partials,
+          Q6Rec *__restrict__ out, unsigned *ticket, Q6DevOut dres) {
+    const uint64_t npairs = n >> 1;
+    const uint64_t tid = blockIdx.x * (uint64_t)kThreads + threadIdx.x;
+    const uint64_t nthreads = (uint64_t)gridDim.x * kThreads;
+    double s0 = 0.0, s1 = 0.0;
+    unsigned cnt = 0;  // a thread sees < 2^32 rows
+
+    uint64_t p = tid;
+    for (; p + (UNROLL - 1) * nthreads < npairs; p += UNROLL * nthreads) {
+        int2 d[UNROLL]; int4 a[UNROLL], b[UNROLL], c[UNROLL];
+#pragma unroll
+        for (int k = 0; k < UNROLL; k++) {
+            const uint64_t q = p + k * nthreads;
+            d[k] = ld_stream8(sd + 2 * q);
+            a[k] = ld_stream16(disc + 2 * q);
+            b[k] = ld_stream16(qty + 2 * q);
+            c[k] = ld_stream16(price + 2 * q);
+        }
+#pragma unroll
+        for (int k = 0; k < UNROLL; k++) {
+            double di[2], qq[2], pr[2];
+            memcpy(di, &a[k], 16); memcpy(qq, &b[k], 16); memcpy(pr, &c[k], 16);
+            q6_row(P, d[k].x, di[0], qq[0], pr[0], s0, cnt);
+            q6_row(P, d[k].y, di[1], qq[1], pr[1], s1, cnt);
+        }
+    }
+    for (; p < npairs; p += nthreads) {
+        int2 d = ld_stream8(sd + 2 * p);
+        int4 a = ld_stream16(disc + 2 * p), b = ld_stream16(qty + 2 * p), c = ld_stream16(price + 2 * p);
+        double di[2], qq[2], pr[2];
+        memcpy(di, &a, 16); memcpy(qq, &b, 16); memcpy(pr, &c, 16);
+        q6_row(P, d.x, di[0], qq[0], pr[0], s0, cnt);
+        q6_row(P, d.y, di[1], qq[1], pr[1], s1, cnt);
+    }
+    if ((n & 1) && tid == 0) q6_row(P, sd[n - 1], disc[n - 1], qty[n - 1], price[n - 1], s0, cnt);  // odd tail row
+    q6_finish(s0, s1, cnt, partials, out, ticket, dres);
+}
+
+// Selective scan (the default): the columns are read in dependent rounds, in the reference's conjunct order (filter.go:87-153).
+// shipdate is read for every pair; a lane then reads its 16 B of discount only if a row of its pair is inside the date range, its
+// quantity only if a row also passed the discount test, and its price only if a row passed all three.  DRAM moves a block only if
+// one of its rows is still alive (DESIGN 5.1 has the byte model).  The next batch's shipdate is in flight while the current batch's
+// rounds run, so a batch costs three round trips.  Merging the quantity and price rounds measured slower for Q6: it reads more.
+// Same grid, pair -> thread mapping, per-thread order and s0 / s1 split as q6_kernel, and a row whose columns were not read adds +0.0
+// exactly as a failing row does there: the result is bit-identical to the dense kernel's.
+template <int UNROLL>
+__global__ void __launch_bounds__(kThreads, 4)
+q6_selective_kernel(const int32_t *__restrict__ sd, const double *__restrict__ disc, const double *__restrict__ qty,
+                    const double *__restrict__ price, uint64_t n, mo_q6_params_t P, Q6Rec *__restrict__ partials,
+                    Q6Rec *__restrict__ out, unsigned *ticket, Q6DevOut dres) {
+    const uint64_t npairs = n >> 1;
+    const uint64_t tid = blockIdx.x * (uint64_t)kThreads + threadIdx.x;
+    const uint64_t nthreads = (uint64_t)gridDim.x * kThreads;
+    const int lane = threadIdx.x & 31;
+    double s0 = 0.0, s1 = 0.0;
+    unsigned cnt = 0;  // a thread sees < 2^32 rows
+
+    // The batched loop runs while the warp's LAST lane has a whole batch, so its trip count is warp-uniform; what is left goes to the
+    // per-thread loop below, and every thread still visits its pairs in ascending order.
+    const uint64_t span = (uint64_t)(31 - lane) + (UNROLL - 1) * nthreads;
+    uint64_t p = tid;
+    bool more = p + span < npairs;
+    int2 dn[UNROLL];
+    if (more) {
+#pragma unroll
+        for (int k = 0; k < UNROLL; k++) dn[k] = ld_stream8(sd + 2 * (p + k * nthreads));
+    }
+    while (more) {
+        int2 d[UNROLL];
+#pragma unroll
+        for (int k = 0; k < UNROLL; k++) d[k] = dn[k];
+        const uint64_t pn = p + UNROLL * nthreads;
+        more = pn + span < npairs;
+        if (more) {
+#pragma unroll
+            for (int k = 0; k < UNROLL; k++) dn[k] = ld_stream8(sd + 2 * (pn + k * nthreads));
+        }
+        bool m0[UNROLL], m1[UNROLL];   // row still alive
+        double2 a[UNROLL], b[UNROLL], c[UNROLL];
+#pragma unroll
+        for (int k = 0; k < UNROLL; k++) {
+            m0[k] = (d[k].x >= P.date_lo) & (d[k].x < P.date_hi);
+            m1[k] = (d[k].y >= P.date_lo) & (d[k].y < P.date_hi);
+            a[k] = ld_stream16_f64_if(m0[k] | m1[k], disc + 2 * (p + k * nthreads));
+        }
+#pragma unroll
+        for (int k = 0; k < UNROLL; k++) {
+            m0[k] = m0[k] & (a[k].x >= P.disc_lo) & (a[k].x <= P.disc_hi);
+            m1[k] = m1[k] & (a[k].y >= P.disc_lo) & (a[k].y <= P.disc_hi);
+            b[k] = ld_stream16_f64_if(m0[k] | m1[k], qty + 2 * (p + k * nthreads));
+        }
+#pragma unroll
+        for (int k = 0; k < UNROLL; k++) {
+            m0[k] = m0[k] & (b[k].x < P.qty_hi);
+            m1[k] = m1[k] & (b[k].y < P.qty_hi);
+            c[k] = ld_stream16_f64_if(m0[k] | m1[k], price + 2 * (p + k * nthreads));
+        }
+#pragma unroll
+        for (int k = 0; k < UNROLL; k++) {   // a dead row's unread columns are +0.0; it adds +0.0 like any failing row
+            q6_add(m0[k], a[k].x, c[k].x, s0, cnt);
+            q6_add(m1[k], a[k].y, c[k].y, s1, cnt);
+        }
+        p = pn;
+    }
+    for (; p < npairs; p += nthreads) {
+        int2 d = ld_stream8(sd + 2 * p);
+        int4 a = ld_stream16(disc + 2 * p), b = ld_stream16(qty + 2 * p), c = ld_stream16(price + 2 * p);
+        double di[2], qq[2], pr[2];
+        memcpy(di, &a, 16); memcpy(qq, &b, 16); memcpy(pr, &c, 16);
+        q6_row(P, d.x, di[0], qq[0], pr[0], s0, cnt);
+        q6_row(P, d.y, di[1], qq[1], pr[1], s1, cnt);
+    }
+    if ((n & 1) && tid == 0) q6_row(P, sd[n - 1], disc[n - 1], qty[n - 1], price[n - 1], s0, cnt);  // odd tail row
+    q6_finish(s0, s1, cnt, partials, out, ticket, dres);
 }
 
 // =========================================================================================================
@@ -918,9 +1008,8 @@ static int launch_q6(ThreadCtx &t, const int32_t *sd, const double *disc, const 
     if (!aligned_to(sd, 8) || !aligned_to(disc, 16) || !aligned_to(qty, 16) || !aligned_to(price, 16)) {
         set_error("q6: columns must be 16-byte aligned (int32 column 8-byte)"); return MO_RC_INVALID_ARGUMENT;
     }
-    int variant = g_q6_variant;
-    int ctas = (variant == 1 || variant == 3) ? 2 : 4;
-    int grid = num_sms() * ctas;
+    const int variant = g_q6_variant;
+    int grid = num_sms() * 4;
     uint64_t work = (n / 2 + kThreads - 1) / kThreads;
     if ((uint64_t)grid > work) grid = work ? (int)work : 1;
     Q6Rec *partials = (Q6Rec *)arena_alloc(t, sizeof(Q6Rec) * (size_t)(grid + 1));
@@ -928,10 +1017,8 @@ static int launch_q6(ThreadCtx &t, const int32_t *sd, const double *disc, const 
     Q6Rec *out = partials + grid;
     cudaEventRecord(t.kev0, t.stream);
     switch (variant) {
-    case 1: q6_kernel<4, 2><<<grid, kThreads, 0, t.stream>>>(sd, disc, qty, price, n, P, partials, out, t.ctrl, dres); break;
-    case 2: q6_kernel<2, 4><<<grid, kThreads, 0, t.stream>>>(sd, disc, qty, price, n, P, partials, out, t.ctrl, dres); break;
-    case 3: q6_kernel<8, 2><<<grid, kThreads, 0, t.stream>>>(sd, disc, qty, price, n, P, partials, out, t.ctrl, dres); break;
-    default: q6_kernel<4, 4><<<grid, kThreads, 0, t.stream>>>(sd, disc, qty, price, n, P, partials, out, t.ctrl, dres); break;
+    case 1: q6_kernel<4, 4><<<grid, kThreads, 0, t.stream>>>(sd, disc, qty, price, n, P, partials, out, t.ctrl, dres); break;
+    default: q6_selective_kernel<3><<<grid, kThreads, 0, t.stream>>>(sd, disc, qty, price, n, P, partials, out, t.ctrl, dres); break;
     }
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();

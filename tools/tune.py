@@ -14,13 +14,53 @@ sys.path.insert(0, ROOT)
 from matrixone_b200 import capi, datagen, ops  # noqa: E402
 from matrixone_b200.vector import DeviceBuffer, Vector, varlena_column_from_matrix, xcall  # noqa: E402
 
-lib = capi.load_library()
-capi.check(lib.MoB200_Init(0), lib)
+lib = None
 PEAK = 6568.4
 try:
     PEAK = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:
     pass
+
+# Q6 selectivity sweep: (name, (date_lo, date_hi, disc_lo, disc_hi, qty_hi))
+Q6_SWEEP = (("q6", datagen.q6_params()),
+            ("every_row_passes", (-2**31, 2**31 - 1, -np.inf, np.inf, np.inf)),
+            ("discount_window_empty", (-2**31, 2**31 - 1, 1.0, 0.0, np.inf)),
+            ("no_row_passes", (0, 0, -np.inf, np.inf, np.inf)))
+Q6_GRAINS = (32, 64, 128)
+Q6_VARIANTS = (0, 1)   # selective (default), dense
+
+
+def q6_touched_bytes(shipdate, discount, quantity, params, grain):
+    """Bytes the selective Q6 kernel must read when DRAM is fetched in aligned `grain`-byte blocks: all of shipdate; discount in the
+    blocks holding a row inside the date range; quantity where a row also passed the discount test; price where a row passed all
+    three.  The columns start on a `grain` boundary (device allocations are 256-byte aligned), and the slice must too."""
+    date_lo, date_hi, disc_lo, disc_hi, qty_hi = params
+    alive = (shipdate >= date_lo) & (shipdate < date_hi)
+
+    def blocks(mask, width):
+        per = grain // width
+        m = np.zeros(-(-mask.size // per) * per, dtype=bool)
+        m[:mask.size] = mask
+        return int(m.reshape(-1, per).any(axis=1).sum()) * grain
+
+    total = blocks(np.ones(shipdate.size, dtype=bool), 4) + blocks(alive, 8)
+    alive &= (discount >= disc_lo) & (discount <= disc_hi)
+    total += blocks(alive, 8)
+    alive &= quantity < qty_hi
+    return total + blocks(alive, 8)
+
+
+def l2_fetch_granularity():
+    """cudaLimitMaxL2FetchGranularity as the CUDA runtime reports it, or None.  Read only: the limit is process-wide, and a library
+    embedded in a database must leave it to the host process."""
+    for name in ("libcudart.so", "libcudart.so.12", "/usr/local/cuda/lib64/libcudart.so"):
+        try:
+            rt = C.CDLL(name)
+        except OSError:
+            continue
+        v = C.c_size_t(0)
+        return v.value if rt.cudaDeviceGetLimit(C.byref(v), 5) == 0 else None   # 5 = cudaLimitMaxL2FetchGranularity
+    return None
 
 
 def kms():
@@ -48,7 +88,40 @@ def report(name, ms, best, nbytes=None, **kw):
     print(json.dumps(d), flush=True)
 
 
+def q6_sweep(b, n):
+    """selective (default) vs dense (q6_variant=1) Q6 kernel, timed alternately over parameter sets of falling selectivity, next to the
+    bytes each set makes the selective kernel read (counted from the columns)"""
+    print(json.dumps({"bench": "q6_env", "l2_fetch_granularity": l2_fetch_granularity()}), flush=True)
+    chunk = 1 << 24
+    for name, P in Q6_SWEEP:
+        touched = dict.fromkeys(Q6_GRAINS, 0)
+        for r0 in range(0, n, chunk):
+            m = min(chunk, n - r0)
+            sd = b["shipdate"].view(4 * m, 4 * r0).to_numpy(np.int32)
+            di = b["discount"].view(8 * m, 8 * r0).to_numpy(np.float64)
+            qt = b["quantity"].view(8 * m, 8 * r0).to_numpy(np.float64)
+            for g in Q6_GRAINS:
+                touched[g] += q6_touched_bytes(sd, di, qt, P, g)
+        times = {var: [] for var in Q6_VARIANTS}
+        results = {}
+        for _ in range(5):
+            for var in Q6_VARIANTS:
+                lib.MoB200_SetTuning(b"q6_variant", var)
+                ms, _best = timed(lambda: results.__setitem__(var, ops.q6_filter_sum(b["shipdate"], b["discount"], b["quantity"], b["extendedprice"], n, *P)), reps=3, warm=1)
+                times[var].append(ms)
+        lib.MoB200_SetTuning(b"q6_variant", 0)
+        for var in Q6_VARIANTS:
+            ms = statistics.median(times[var])
+            report("q6_sweep", ms, min(times[var]), 28.0 * n, params=name, variant=var, rows=n, kernel_ms_range=[round(min(times[var]), 4), round(max(times[var]), 4)],
+                   Grows_per_s=round(n / ms / 1e6, 2), qualifying_rows=results[var][1], same_as_dense=results[var][:2] == results[1][:2],
+                   touched_bytes_per_row={g: round(touched[g] / n, 3) for g in Q6_GRAINS},
+                   touched_GBps={g: round(touched[g] / ms / 1e6, 1) for g in Q6_GRAINS})
+
+
 def main():
+    global lib
+    lib = capi.load_library()
+    capi.check(lib.MoB200_Init(0), lib)
     which = set(sys.argv[1:]) or {"q6", "q1", "sum", "elem", "dist", "bf"}
     n = int(os.environ.get("TUNE_ROWS", 200_000_000))
     if which & {"q6", "q1"}:
@@ -57,13 +130,8 @@ def main():
         b = {k: DeviceBuffer(size.get(k, 8) * n, lib) for k in names}
         capi.check(lib.MoB200_GenLineitem(10, 0, n, b["shipdate"].ptr, b["quantity"].ptr, b["extendedprice"].ptr, b["discount"].ptr,
                                           b["tax"].ptr, b["returnflag"].ptr, b["linestatus"].ptr), lib)
-        P = datagen.q6_params()
         if "q6" in which:
-            for var in (0, 1, 2, 3):
-                lib.MoB200_SetTuning(b"q6_variant", var)
-                ms, best = timed(lambda: ops.q6_filter_sum(b["shipdate"], b["discount"], b["quantity"], b["extendedprice"], n, *P))
-                report("q6", ms, best, 28.0 * n, variant=var, rows=n, Grows_per_s=round(n / ms / 1e6, 2))
-            lib.MoB200_SetTuning(b"q6_variant", 0)
+            q6_sweep(b, n)
         if "q1" in which:
             for var in (0, 1, 3, 4):
                 lib.MoB200_SetTuning(b"q1_variant", var)
