@@ -463,8 +463,7 @@ uint64_t MoB200_KernelLaunchCount(void);      /* kernels launched by this librar
 int32_t MoB200_LastKernelMs(float *ms);       /* device time of the dominant kernel of the calling thread's last call (CUDA events) */
 int32_t MoB200_LastError(char *buf, uint64_t buflen);  /* thread-local last error text */
 int32_t MoB200_FlushL2(void);                 /* write a >L2-sized scratch buffer (bench hygiene) */
-int32_t MoB200_SetTuning(const char *name, int32_t value);
-void *MoB200_DebugBuffer(void);               /* per-CTA phase timestamps of the last Q1 launch when SetTuning("q1_debug",1) */  /* kernel-variant knobs used by tools/tune.py; returns 0 if known */
+int32_t MoB200_SetTuning(const char *name, int32_t value);  /* kernel-variant knobs used by tools/tune.py; returns 0 if name and value are known, else -1 */
 
 /* synthetic column generators used by bench.py / tests (counter-based, reproducible on the host: see
  * matrixone_b200/datagen.py).  All write DEVICE memory, rows [row0, row0+n). */

@@ -146,7 +146,7 @@ PROTOTYPES = {
     "MoB200_DownloadAsync": (_i32, [_vp, _vp, _u64]), "MoB200_UploadAsync": (_i32, [_vp, _vp, _u64]),
     "MoB200_Sync": (_i32, []), "MoB200_SetStream": (_i32, [_vp]), "MoB200_TimerStart": (_i32, []),
     "MoB200_TimerStop": (_i32, [C.POINTER(C.c_float)]), "MoB200_KernelLaunchCount": (_u64, []), "MoB200_LastKernelMs": (_i32, [C.POINTER(C.c_float)]),
-    "MoB200_LastError": (_i32, [C.c_char_p, _u64]), "MoB200_FlushL2": (_i32, []), "MoB200_SetTuning": (_i32, [C.c_char_p, _i32]), "MoB200_DebugBuffer": (_vp, []),
+    "MoB200_LastError": (_i32, [C.c_char_p, _u64]), "MoB200_FlushL2": (_i32, []), "MoB200_SetTuning": (_i32, [C.c_char_p, _i32]),
     "MoB200_GenLineitem": (_i32, [_u64, _u64, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "MoB200_GenInt64": (_i32, [_u64, _u64, _u64, _vp, _vp, C.c_uint32]),
     "MoB200_GenVectorsF32": (_i32, [_u64, _u64, _u64, _i64, _vp, _vp, _i64, C.c_float]),

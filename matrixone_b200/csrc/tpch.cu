@@ -18,6 +18,12 @@
 // (__dmul_rn/__dadd_rn, no FMA contraction), so only the summation ORDER differs from the serial Go loop.
 // Reduction: registers -> warp shuffles -> shared memory -> per-CTA record; the last CTA (atomicInc ticket) folds
 // the records in CTA-index order => bitwise run-to-run deterministic for a fixed grid.
+//
+// Q1 has one kernel per input class, chosen from the input (launch_q1):
+//   q1_tma_kernel<4>  packed keys, shipdate and key columns 16-byte aligned, n >= 64 tiles of 1024 rows: one producer warp per
+//                     CTA streams whole tiles into shared memory with cp.async.bulk, 16 consumer warps reduce them
+//   q1_kernel<4>      everything else (varlena keys, unaligned columns, fewer rows): the pair mapping above, loads into registers
+// A pass keeps at most 4 groups per CTA; when it sees more it reports overflow and q1_kernel<8> runs the input again.
 #include "common.cuh"
 #include <cstring>
 #include <atomic>
@@ -223,46 +229,10 @@ struct Q1Rec { Q1Slot slot[MO_Q1_MAX_GROUPS]; unsigned overflow; unsigned pad; }
 constexpr unsigned kEmptyKey = 0xffffffffu;
 constexpr int kQ1MaxGrid = 1024;  // upper bound on the grid (the last-CTA fold keeps a [grid][8] byte map in shared memory)
 
-// Shared state of one CTA: key -> slot dictionary (slots handed out first-come) + flags
+// Shared state of one CTA: key -> slot dictionary (slots handed out first-come) + overflow flag
 struct Q1Shared {
     unsigned dict[MO_Q1_MAX_GROUPS];
     unsigned overflow;
-    unsigned slow;   // debug: dictionary slow-path entries
-};
-
-// Shared-memory accumulators (staged kernels, G = 4): the per-thread state acc[slot][5], cnt[slot], first[slot] lives in shared memory,
-// slot-major ([(slot * 5 + j) * threads + tid]: conflict-free whatever slot each lane uses), so a row costs 5 x (LDS, DADD, STS) on ITS
-// slot instead of 20 indicator-FMAs over all four: ncu put the register version at 2.87 G warp instructions per SF100 pass with the
-// issue slots 70 % busy -- instruction-bound, not HBM-bound.  Branch-free like the register version: rows that do not qualify add 0.0 to
-// slot 0.  acc + v is the same single rounding as before, so results are bit-identical.
-template <int kT>
-struct Q1SmemAcc {
-    double *acc; unsigned *cnt; unsigned *first;   // bases already offset by tid
-    static constexpr size_t kBytes = (size_t)kT * 4 * (kQ1Vals * 8 + 4 + 4);
-    __device__ __forceinline__ void bind(unsigned char *base, int tid) {
-        acc = reinterpret_cast<double *>(base) + tid;
-        cnt = reinterpret_cast<unsigned *>(base + (size_t)kT * 4 * kQ1Vals * 8) + tid;
-        first = cnt + (size_t)kT * 4;
-#pragma unroll
-        for (int g = 0; g < 4; g++) {
-#pragma unroll
-            for (int j = 0; j < kQ1Vals; j++) acc[(g * kQ1Vals + j) * kT] = 0.0;
-            cnt[g * kT] = 0u; first[g * kT] = 0xffffffffu;
-        }
-    }
-    __device__ __forceinline__ void add(int slot, bool m, uint64_t r, double q, double pr, double t2, double t4, double di) {
-        const int s = m ? slot : 0;
-        double *a = acc + (size_t)s * kQ1Vals * kT;
-        a[0] = __dadd_rn(a[0], m ? q : 0.0);
-        a[kT] = __dadd_rn(a[kT], m ? pr : 0.0);
-        a[2 * kT] = __dadd_rn(a[2 * kT], m ? t2 : 0.0);
-        a[3 * kT] = __dadd_rn(a[3 * kT], m ? t4 : 0.0);
-        a[4 * kT] = __dadd_rn(a[4 * kT], m ? di : 0.0);
-        const unsigned c = cnt[s * kT];
-        cnt[s * kT] = c + (m ? 1u : 0u);
-        const unsigned f = first[s * kT];
-        first[s * kT] = (m && c == 0u) ? (unsigned)r : f;     // rows of one launch are numbered below 2^32 (checked by the launcher)
-    }
 };
 
 // Per-thread aggregation state (registers).  Control flow of every method is WARP-UNIFORM: all 32 lanes call row() together
@@ -277,10 +247,9 @@ struct Q1Thread {
     Q1Shared *S;
     int32_t cutoff;
     int lane;
-    bool dbg;
 
-    __device__ __forceinline__ void init(Q1Shared *s, int32_t cut, bool debug) {
-        S = s; cutoff = cut; lane = threadIdx.x & 31; dbg = debug;
+    __device__ __forceinline__ void init(Q1Shared *s, int32_t cut) {
+        S = s; cutoff = cut; lane = threadIdx.x & 31;
 #pragma unroll
         for (int g = 0; g < G; g++) {
             cnt[g] = 0; first[g] = ~0ull; dk[g] = kEmptyKey;
@@ -318,29 +287,6 @@ struct Q1Thread {
             miss = __ballot_sync(0xffffffffu, !settled);
         }
         return slot;
-    }
-
-    // shared-memory accumulator form of row(): same dictionary, same products, 15 accumulate instructions instead of ~44
-    template <int kT>
-    __device__ __forceinline__ void row_smem(Q1SmemAcc<kT> &A, uint64_t r, bool inb, int32_t d, double q, double pr, double di, double tx, unsigned key) {
-        const bool valid = inb && d <= cutoff;
-        const int slot = find_slot(key, valid);
-        const double t1 = __dsub_rn(1.0, di);
-        const double t2 = __dmul_rn(pr, t1);
-        const double t3 = __dadd_rn(1.0, tx);
-        const double t4 = __dmul_rn(t2, t3);
-        A.add(slot, valid && slot >= 0, r, q, pr, t2, t4, di);
-    }
-    template <int kT>
-    __device__ __forceinline__ void load_from(const Q1SmemAcc<kT> &A) {   // registers <- shared state, for the common epilogue (G >= 4)
-#pragma unroll
-        for (int g = 0; g < 4; g++) {
-#pragma unroll
-            for (int j = 0; j < kQ1Vals; j++) acc[g][j] = A.acc[(g * kQ1Vals + j) * kT];
-            cnt[g] = A.cnt[g * kT];
-            const unsigned f = A.first[g * kT];
-            first[g] = f == 0xffffffffu ? ~0ull : (unsigned long long)f;
-        }
     }
 
     // `inb` = the row exists; the shipdate filter is folded into `valid`.
@@ -395,19 +341,8 @@ __device__ __forceinline__ unsigned q1_key_scalar(const uint8_t *rf, const uint8
 
 // CTA reduction + last-CTA fold, shared by both kernels.  kT = threads per CTA.
 template <int G, int kT>
-__device__ void q1_epilogue(Q1Thread<G> &T, Q1Shared &S, Q1Rec *__restrict__ partials, Q1Rec *__restrict__ out, unsigned *ticket,
-                            unsigned long long *dbg) {
-    auto stamp = [&](int k) { if (dbg && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); dbg[blockIdx.x * 16 + k] = t; } };
-    stamp(1);
-    if (dbg && (threadIdx.x & 31) == 0 && (threadIdx.x >> 5) < 8) {
-        unsigned long long tt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tt));
-        unsigned sm; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
-        dbg[blockIdx.x * 16 + 8 + (threadIdx.x >> 5)] = tt;
-        if (threadIdx.x == 0) dbg[blockIdx.x * 16 + 5] = sm;
-    }
+__device__ void q1_epilogue(Q1Thread<G> &T, Q1Shared &S, Q1Rec *__restrict__ partials, Q1Rec *__restrict__ out, unsigned *ticket) {
     __syncthreads();  // dictionary final
-    stamp(2);
-    if (dbg && threadIdx.x == 0) dbg[blockIdx.x * 16 + 7] = S.slow;
     // Register slots are indexed by the CTA dictionary, identical for every thread of the CTA.
     constexpr int kW = kT / 32;
     __shared__ double sv[kW][G][kQ1Vals];
@@ -446,7 +381,6 @@ __device__ void q1_epilogue(Q1Thread<G> &T, Q1Shared &S, Q1Rec *__restrict__ par
         unsigned tk = atomicInc(ticket, gridDim.x - 1);
         last = (tk == gridDim.x - 1);
     }
-    stamp(3);
     __syncthreads();
     if (last) {
         // Fold the CTA records (MergeGroup: re-hash partial keys + BatchMerge, mergeGroup.go:132-247) with the whole CTA:
@@ -498,26 +432,24 @@ __device__ void q1_epilogue(Q1Thread<G> &T, Q1Shared &S, Q1Rec *__restrict__ par
             }
         }
         __syncthreads();
-        stamp(4);
     }
 }
 
-// ---- variant A: direct register-staged loads (pairs of rows, UNROLL pairs in flight per thread) -------------------------
+// ---- register kernel: direct loads into registers (pairs of rows, UNROLL pairs in flight per thread) ---------------------
 template <int G, int UNROLL, int CTAS, int KEYMODE>
 __global__ void __launch_bounds__(kThreads, CTAS)
 q1_kernel(const int32_t *__restrict__ sd, const double *__restrict__ qty, const double *__restrict__ price,
           const double *__restrict__ disc, const double *__restrict__ tax, const uint8_t *__restrict__ rf,
           const uint8_t *__restrict__ ls, uint64_t n, int32_t cutoff, Q1Rec *__restrict__ partials,
-          Q1Rec *__restrict__ out, unsigned *ticket, unsigned long long *dbg, const Q1Rec *gate) {
+          Q1Rec *__restrict__ out, unsigned *ticket, const Q1Rec *gate) {
     // asynchronous form: the 8-slot retry is enqueued behind the 4-slot pass and runs only if that pass overflowed its dictionary
     if (gate && !gate->overflow) return;
-    if (dbg && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); dbg[blockIdx.x * 16] = t; }
     __shared__ Q1Shared S;
     S.dict[threadIdx.x & (MO_Q1_MAX_GROUPS - 1)] = kEmptyKey;   // all threads write (same values): no lane-dependent branch
-    S.overflow = 0; S.slow = 0;
+    S.overflow = 0;
     __syncthreads();
     Q1Thread<G> T;
-    T.init(&S, cutoff, dbg != nullptr);
+    T.init(&S, cutoff);
     const int lane = threadIdx.x & 31;
 
     auto load_keys = [&](uint64_t pair, unsigned &k0, unsigned &k1) {
@@ -583,120 +515,19 @@ q1_kernel(const int32_t *__restrict__ sd, const double *__restrict__ qty, const 
         if (has) { key = q1_key_scalar<KEYMODE>(rf, ls, r); dd = sd[r]; v0 = qty[r]; v1 = price[r]; v2 = disc[r]; v3 = tax[r]; }
         T.row(r, has, dd, v0, v1, v2, v3, key);
     }
-    q1_epilogue<G, kThreads>(T, S, partials, out, ticket, dbg);
+    q1_epilogue<G, kThreads>(T, S, partials, out, ticket);
 }
 
-// ---- variant B: cp.async-staged tiles (packed keys only) ----------------------------------------------------------------
-// Each warp owns a ring of kStages tiles of 64 rows in shared memory.  The 64-row slices of the seven columns are copied with
-// per-lane cp.async (LDGSTS): 8 B/lane for the int32 column, 16 B/lane for each float64 column, 4 B/lane (half a warp) for each
-// key column -- every copy instruction covers whole 32-byte sectors.  Bytes in flight per SM = warps x kStages x 2432 B,
-// independent of the register file, so the loads of tile i+kStages-1 are in the air while tile i is reduced: the register
-// version above could keep only ~78 KB per SM in flight and stalled on HBM latency (profiles/r01_ncu_summary.md).
-// No CTA barriers in the steady state: a warp waits for ITS oldest copy group (cp.async.wait_group) and __syncwarp()s.
-constexpr int kTileRows = 64;
-constexpr int kTileBytes = kTileRows * 38;   // 256 (shipdate) + 4 x 512 + 2 x 64 = 2432
-constexpr int kStagedThreads = 512;
+// ---- TMA kernel: CTA-wide bulk-copy pipeline (packed keys) ---------------------------------------------------------------------------
+// ONE producer warp streams 1024-row tiles -- 7 bulk copies of 1-8 KB per tile, 4 tiles (156 KB) in flight per SM -- and the 16 consumer
+// warps share each tile: full[stage] (transaction count) / empty[stage] (one arrival per consumer warp) mbarriers, no CTA barrier in the
+// steady state.  Two staged designs lost to it (DESIGN 5.1): per-lane 16-byte cp.async (LDGSTS) into per-warp rings is not merged into
+// sector requests the way LDG.128 is, so every 32-byte sector crossed the L2 -> SM crossbar twice; per-warp rings filled with one
+// cp.async.bulk per 64-row column slice fixed that but drowned the TMA unit in tiny copies (7 per 64 rows).
+constexpr int kCtaTileRows = 1024, kCtaStages = 4, kCtaConsumers = 16;
+constexpr int kCtaTileBytes = kCtaTileRows * 38;   // 4096 shipdate + 4 x 8192 + 2 x 1024
+constexpr int kCtaThreads = (kCtaConsumers + 1) * 32;
 
-__device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async8(void *smem, const void *gmem) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async4(void *smem, const void *gmem) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-template <int G, int kStages, bool SMEMACC>
-__global__ void __launch_bounds__(kStagedThreads, 1)
-q1_staged_kernel(const int32_t *__restrict__ sd, const double *__restrict__ qty, const double *__restrict__ price,
-                 const double *__restrict__ disc, const double *__restrict__ tax, const uint8_t *__restrict__ rf,
-                 const uint8_t *__restrict__ ls, uint64_t n, int32_t cutoff, Q1Rec *__restrict__ partials,
-                 Q1Rec *__restrict__ out, unsigned *ticket, unsigned long long *dbg) {
-    extern __shared__ __align__(16) unsigned char ring[];   // [warp][stage][kTileBytes]
-    if (dbg && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); dbg[blockIdx.x * 16] = t; }
-    __shared__ Q1Shared S;
-    S.dict[threadIdx.x & (MO_Q1_MAX_GROUPS - 1)] = kEmptyKey;   // all threads write (same values): no lane-dependent branch
-    S.overflow = 0; S.slow = 0;
-    __syncthreads();
-    Q1Thread<G> T;
-    T.init(&S, cutoff, dbg != nullptr);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    constexpr int kWarps = kStagedThreads / 32;
-    unsigned char *wring = ring + (size_t)warp * kStages * kTileBytes;
-    Q1SmemAcc<kStagedThreads> A;
-    if (SMEMACC) A.bind(ring + (size_t)kWarps * kStages * kTileBytes, threadIdx.x);
-    const uint64_t ntiles = n / kTileRows;
-    const uint64_t gw = blockIdx.x * (uint64_t)kWarps + warp, nw = (uint64_t)gridDim.x * kWarps;
-
-    auto issue = [&](uint64_t tile, int stage) {   // all lanes; one commit group per tile
-        unsigned char *s = wring + stage * kTileBytes;
-        const uint64_t r0 = tile * kTileRows;
-        cp_async8(s + lane * 8, sd + r0 + lane * 2);
-        cp_async16(s + 256 + lane * 16, qty + r0 + lane * 2);
-        cp_async16(s + 768 + lane * 16, price + r0 + lane * 2);
-        cp_async16(s + 1280 + lane * 16, disc + r0 + lane * 2);
-        cp_async16(s + 1792 + lane * 16, tax + r0 + lane * 2);
-        // keys: lanes 0-15 copy the returnflag slice, lanes 16-31 the linestatus slice (address select, no branch); the
-        // linestatus area follows the returnflag area so one destination expression serves both
-        cp_async4(s + 2304 + lane * 4, (lane < 16 ? rf + r0 + lane * 4 : ls + r0 + (lane - 16) * 4));
-        cp_async_commit();
-    };
-
-    // prologue: kStages - 1 tiles in flight (empty groups keep the group arithmetic uniform when tiles run out)
-    uint64_t next = gw;
-#pragma unroll
-    for (int s = 0; s < kStages - 1; s++) {
-        if (next < ntiles) issue(next, s); else cp_async_commit();
-        next += nw;
-    }
-    int stage = 0;
-    for (uint64_t tile = gw; tile < ntiles; tile += nw) {
-        // refill the slot consumed in the previous iteration, then wait for the oldest group
-        const int fill = (stage + kStages - 1) % kStages;
-        if (next < ntiles) issue(next, fill); else cp_async_commit();
-        next += nw;
-        cp_async_wait<kStages - 1>();
-        __syncwarp();
-        const unsigned char *s = wring + stage * kTileBytes;
-        const uint64_t r0 = tile * kTileRows;
-#pragma unroll
-        for (int h = 0; h < 2; h++) {   // lane handles rows lane and lane + 32 of the tile: conflict-free LDS
-            const int rl = lane + 32 * h;
-            const int32_t d = *reinterpret_cast<const int32_t *>(s + rl * 4);
-            const double q = *reinterpret_cast<const double *>(s + 256 + rl * 8);
-            const double pr = *reinterpret_cast<const double *>(s + 768 + rl * 8);
-            const double di = *reinterpret_cast<const double *>(s + 1280 + rl * 8);
-            const double tx = *reinterpret_cast<const double *>(s + 1792 + rl * 8);
-            const unsigned key = (unsigned)s[2304 + rl] | ((unsigned)s[2368 + rl] << 8);
-            if (SMEMACC) T.row_smem(A, r0 + rl, true, d, q, pr, di, tx, key);
-            else T.row(r0 + rl, true, d, q, pr, di, tx, key);
-        }
-        __syncwarp();   // every lane is done with this slot before any lane's next cp.async overwrites it
-        stage = (stage + 1) % kStages;
-    }
-    cp_async_wait<0>();
-    // rows past the last full tile (< 64): warp 0 of CTA 0, direct loads
-    if (blockIdx.x == 0 && warp == 0) {
-        for (uint64_t r = ntiles * kTileRows + lane; r - lane < n; r += 32) {
-            const bool has = r < n;
-            unsigned key = 0; int32_t dd = 0; double v0 = 0, v1 = 0, v2 = 0, v3 = 0;
-            if (has) { key = q1_key_scalar<0>(rf, ls, r); dd = sd[r]; v0 = qty[r]; v1 = price[r]; v2 = disc[r]; v3 = tax[r]; }
-            if (SMEMACC) T.row_smem(A, r, has, dd, v0, v1, v2, v3, key);
-            else T.row(r, has, dd, v0, v1, v2, v3, key);
-        }
-    }
-    if (SMEMACC) T.load_from(A);
-    q1_epilogue<G, kStagedThreads>(T, S, partials, out, ticket, dbg);
-}
-
-// ---- variant C: bulk-copy (TMA 1-D) staged tiles ---------------------------------------------------------------------------------
-// Same per-warp ring as variant B, but every column slice of a tile is ONE cp.async.bulk (256 B shipdate, 4 x 512 B float64 columns,
-// 2 x 64 B key bytes) issued by lane 0 and completed on a per-(warp, stage) mbarrier: 7 copy instructions per 64-row tile instead of
-// 6 x 32 per-lane LDGSTS, nothing passes through L1, and the L2 -> SM crossbar moves every byte once (ncu on variant B:
-// l1tex__m_xbar2l1tex_read_bytes = 1.84 x the DRAM bytes, sector hit rate 49 %).
 __device__ __forceinline__ void q1_mbar_init(unsigned long long *bar, unsigned count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(count));
 }
@@ -713,95 +544,6 @@ __device__ __forceinline__ void q1_bulk_copy(void *smem, const void *gmem, unsig
                  ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem), "r"(bytes), "r"((unsigned)__cvta_generic_to_shared(bar)) : "memory");
 }
 
-template <int G, int kStages>
-__global__ void __launch_bounds__(kStagedThreads, 1)
-q1_bulk_kernel(const int32_t *__restrict__ sd, const double *__restrict__ qty, const double *__restrict__ price,
-               const double *__restrict__ disc, const double *__restrict__ tax, const uint8_t *__restrict__ rf,
-               const uint8_t *__restrict__ ls, uint64_t n, int32_t cutoff, Q1Rec *__restrict__ partials,
-               Q1Rec *__restrict__ out, unsigned *ticket, unsigned long long *dbg) {
-    extern __shared__ __align__(16) unsigned char ring[];   // [warp][stage][kTileBytes], then the mbarriers
-    if (dbg && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); dbg[blockIdx.x * 16] = t; }
-    __shared__ Q1Shared S;
-    S.dict[threadIdx.x & (MO_Q1_MAX_GROUPS - 1)] = kEmptyKey;
-    S.overflow = 0; S.slow = 0;
-    constexpr int kWarps = kStagedThreads / 32;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    unsigned char *wring = ring + (size_t)warp * kStages * kTileBytes;
-    unsigned long long *bars = reinterpret_cast<unsigned long long *>(ring + (size_t)kWarps * kStages * kTileBytes) + warp * kStages;
-    if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < kStages; s++) q1_mbar_init(&bars[s], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    Q1Thread<G> T;
-    T.init(&S, cutoff, dbg != nullptr);
-    const uint64_t ntiles = n / kTileRows;
-    const uint64_t gw = blockIdx.x * (uint64_t)kWarps + warp, nw = (uint64_t)gridDim.x * kWarps;
-
-    auto issue = [&](uint64_t tile, int stage) {   // lane 0 only
-        unsigned char *s = wring + stage * kTileBytes;
-        const uint64_t r0 = tile * kTileRows;
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the slot was last READ through the generic proxy
-        q1_mbar_expect_tx(&bars[stage], kTileBytes);
-        q1_bulk_copy(s, sd + r0, 256, &bars[stage]);
-        q1_bulk_copy(s + 256, qty + r0, 512, &bars[stage]);
-        q1_bulk_copy(s + 768, price + r0, 512, &bars[stage]);
-        q1_bulk_copy(s + 1280, disc + r0, 512, &bars[stage]);
-        q1_bulk_copy(s + 1792, tax + r0, 512, &bars[stage]);
-        q1_bulk_copy(s + 2304, rf + r0, 64, &bars[stage]);
-        q1_bulk_copy(s + 2368, ls + r0, 64, &bars[stage]);
-    };
-
-    uint64_t next = gw;
-    if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < kStages - 1; s++) { if (next < ntiles) issue(next, s); next += nw; }
-    } else next += (uint64_t)(kStages - 1) * nw;
-    int stage = 0; unsigned phase = 0;
-    for (uint64_t tile = gw; tile < ntiles; tile += nw) {
-        const int fill = (stage + kStages - 1) % kStages;
-        if (lane == 0 && next < ntiles) issue(next, fill);   // the slot consumed in the previous iteration (all lanes passed its __syncwarp)
-        next += nw;
-        q1_mbar_wait(&bars[stage], phase);
-        const unsigned char *s = wring + stage * kTileBytes;
-        const uint64_t r0 = tile * kTileRows;
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-            const int rl = lane + 32 * h;
-            const int32_t d = *reinterpret_cast<const int32_t *>(s + rl * 4);
-            const double q = *reinterpret_cast<const double *>(s + 256 + rl * 8);
-            const double pr = *reinterpret_cast<const double *>(s + 768 + rl * 8);
-            const double di = *reinterpret_cast<const double *>(s + 1280 + rl * 8);
-            const double tx = *reinterpret_cast<const double *>(s + 1792 + rl * 8);
-            const unsigned key = (unsigned)s[2304 + rl] | ((unsigned)s[2368 + rl] << 8);
-            T.row(r0 + rl, true, d, q, pr, di, tx, key);
-        }
-        __syncwarp();
-        stage = (stage + 1) % kStages;
-        if (stage == 0) phase ^= 1u;
-    }
-    if (blockIdx.x == 0 && warp == 0) {
-        for (uint64_t r = ntiles * kTileRows + lane; r - lane < n; r += 32) {
-            const bool has = r < n;
-            unsigned key = 0; int32_t dd = 0; double v0 = 0, v1 = 0, v2 = 0, v3 = 0;
-            if (has) { key = q1_key_scalar<0>(rf, ls, r); dd = sd[r]; v0 = qty[r]; v1 = price[r]; v2 = disc[r]; v3 = tax[r]; }
-            T.row(r, has, dd, v0, v1, v2, v3, key);
-        }
-    }
-    q1_epilogue<G, kStagedThreads>(T, S, partials, out, ticket, dbg);
-}
-
-// ---- variant D: CTA-wide TMA pipeline ------------------------------------------------------------------------------------------------
-// ncu on variant B shows every 32-byte sector requested twice from L2 (lts__t_sector_hit_rate 49 %, l1tex__m_xbar2l1tex_read_bytes = 1.84 x the
-// DRAM bytes): the per-lane 16-byte LDGSTS requests of a warp are not merged into sector requests the way LDG.128 is.  Variant C (per-warp bulk
-// copies of 64-512 bytes) fixed that but drowned the TMA unit in tiny copies (7 per 64 rows; 0.75 of the HBM rate).  Here ONE producer warp
-// streams 1024-row tiles -- 7 bulk copies of 1-8 KB per tile, 4 tiles (156 KB) in flight per SM -- and the 16 consumer warps share each tile:
-// full[stage] (transaction count) / empty[stage] (one arrival per consumer warp) mbarriers, no CTA barrier in the steady state.
-constexpr int kCtaTileRows = 1024, kCtaStages = 4, kCtaConsumers = 16;
-constexpr int kCtaTileBytes = kCtaTileRows * 38;   // 4096 shipdate + 4 x 8192 + 2 x 1024
-constexpr int kCtaThreads = (kCtaConsumers + 1) * 32;
-
 __device__ __forceinline__ void q1_mbar_arrive(unsigned long long *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"((unsigned)__cvta_generic_to_shared(bar)) : "memory");
 }
@@ -811,12 +553,11 @@ __global__ void __launch_bounds__(kCtaThreads, 1)
 q1_tma_kernel(const int32_t *__restrict__ sd, const double *__restrict__ qty, const double *__restrict__ price,
               const double *__restrict__ disc, const double *__restrict__ tax, const uint8_t *__restrict__ rf,
               const uint8_t *__restrict__ ls, uint64_t n, int32_t cutoff, Q1Rec *__restrict__ partials,
-              Q1Rec *__restrict__ out, unsigned *ticket, unsigned long long *dbg) {
+              Q1Rec *__restrict__ out, unsigned *ticket) {
     extern __shared__ __align__(16) unsigned char ring[];   // [stage][kCtaTileBytes], then full[] and empty[] mbarriers
-    if (dbg && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); dbg[blockIdx.x * 16] = t; }
     __shared__ Q1Shared S;
     S.dict[threadIdx.x & (MO_Q1_MAX_GROUPS - 1)] = kEmptyKey;
-    S.overflow = 0; S.slow = 0;
+    S.overflow = 0;
     unsigned long long *full = reinterpret_cast<unsigned long long *>(ring + (size_t)kCtaStages * kCtaTileBytes);
     unsigned long long *empty = full + kCtaStages;
     if (threadIdx.x == 0) {
@@ -826,7 +567,7 @@ q1_tma_kernel(const int32_t *__restrict__ sd, const double *__restrict__ qty, co
     }
     __syncthreads();
     Q1Thread<G> T;
-    T.init(&S, cutoff, dbg != nullptr);
+    T.init(&S, cutoff);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint64_t ntiles = n / kCtaTileRows;
     // tiles of this CTA: blockIdx.x, blockIdx.x + gridDim.x, ...
@@ -882,7 +623,7 @@ q1_tma_kernel(const int32_t *__restrict__ sd, const double *__restrict__ qty, co
             }
         }
     }
-    q1_epilogue<G, kCtaThreads>(T, S, partials, out, ticket, dbg);
+    q1_epilogue<G, kCtaThreads>(T, S, partials, out, ticket);
 }
 
 __host__ __device__ void q1_finalize(const Q1Rec &F, mo_q1_result_t *res, int64_t row_base = 0) {
@@ -961,14 +702,13 @@ __global__ void q6_merge_kernel(const double *parts, uint64_t nparts, Q6DevOut o
     if (o.rnulls) o.rnulls[0] = any ? 0ull : 1ull;
 }
 
-int g_q6_variant = 0, g_q1_variant = 0;  // tuning knobs (MoB200_SetTuning)
-unsigned long long *g_q1_dbg = nullptr;   // optional per-CTA phase timestamps (MoB200_SetTuning("q1_debug", 1))
+// kernel choice (MoB200_SetTuning): 0 = chosen from the input; 1 = the reference arm (dense q6_kernel, register q1_kernel)
+int g_q6_variant = 0, g_q1_variant = 0;
 
 }  // namespace
 
 namespace mob {
 
-unsigned long long *q1_debug_buffer() { return g_q1_dbg; }
 int g_plan_specialise = 1;
 int xcall_plan(mo_xcall_args_t *args, uint64_t len);
 
@@ -987,14 +727,9 @@ int tuning_set(const char *name, int value) {
     if (!strcmp(name, "get_tc_kused")) return g_last_tc_kused;
     if (!strcmp(name, "tc_share")) { g_tc_share_mode = (int)value; return 0; }
     if (!strcmp(name, "tc_sched")) { g_tc_sched_mode = (int)value; return 0; }
-    if (!strcmp(name, "q6_variant")) { g_q6_variant = value; return 0; }
+    if (!strcmp(name, "q6_variant")) { if (value != 0 && value != 1) return -1; g_q6_variant = value; return 0; }
     if (!strcmp(name, "plan_specialise")) { g_plan_specialise = value; return 0; }
-    if (!strcmp(name, "q1_variant")) { g_q1_variant = value; return 0; }
-    if (!strcmp(name, "q1_debug")) {
-        if (value && !g_q1_dbg) { if (cudaMalloc((void **)&g_q1_dbg, 8 * 16 * 1024) != cudaSuccess) return -1; cudaMemset(g_q1_dbg, 0, 8 * 16 * 1024); }
-        if (!value && g_q1_dbg) { cudaFree(g_q1_dbg); g_q1_dbg = nullptr; }
-        return 0;
-    }
+    if (!strcmp(name, "q1_variant")) { if (value != 0 && value != 1) return -1; g_q1_variant = value; return 0; }
     return -1;
 }
 
@@ -1002,6 +737,24 @@ int tuning_set(const char *name, int value) {
 static const uint64_t kHostChunkRows = 32ull << 20;
 
 static bool aligned_to(const void *p, uintptr_t a) { return (((uintptr_t)p) & (a - 1)) == 0; }
+
+// copy a host value into the caller's result buffer, which may be host or device memory
+static int write_result(ThreadCtx &t, void *dst, const void *src, size_t bytes) {
+    if (!is_device_ptr(dst)) { memcpy(dst, src, bytes); return MO_RC_SUCCESS; }
+    MOB_CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, t.stream));
+    MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
+    return MO_RC_SUCCESS;
+}
+
+// Q6 result: sum in word 0, qualifying rows in word 1 when the buffer holds 16 bytes, nulls word bit 0 = "no row qualified"
+static int write_q6_result(ThreadCtx &t, const mo_xcall_args_t &r, double sum, int64_t rows, bool any) {
+    unsigned char w[16];
+    memcpy(w, &sum, 8); memcpy(w + 8, &rows, 8);
+    int rc = write_result(t, r.pdata, w, r.dataSz >= 16 ? 16 : 8);
+    if (rc || !r.pnulls) return rc;
+    const uint64_t nullword = any ? 0ull : 1ull;
+    return write_result(t, r.pnulls, &nullword, 8);
+}
 
 static int launch_q6(ThreadCtx &t, const int32_t *sd, const double *disc, const double *qty, const double *price,
                      uint64_t n, const mo_q6_params_t &P, Q6Rec *hrec, Q6DevOut dres = Q6DevOut{nullptr, 0, nullptr}) {
@@ -1058,19 +811,7 @@ int xcall_q6(mo_xcall_args_t *args, uint64_t len) {
         int rc = xcall_plan(pa, len);
         if (rc) return rc;
         const bool any_ = R.h.ngroups > 0 && R.a.count > 0;
-        const double sum_ = any_ ? R.a.value : 0.0;
-        const int64_t rows_ = R.h.ngroups > 0 ? R.g.rows : 0;
-        const uint64_t nullword_ = any_ ? 0ull : 1ull;
-        if (is_device_ptr(args[0].pdata)) {
-            MOB_CUDA_TRY(cudaMemcpyAsync(args[0].pdata, &sum_, 8, cudaMemcpyHostToDevice, t.stream));
-            if (args[0].dataSz >= 16) MOB_CUDA_TRY(cudaMemcpyAsync(args[0].pdata + 8, &rows_, 8, cudaMemcpyHostToDevice, t.stream));
-            MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
-        } else { memcpy(args[0].pdata, &sum_, 8); if (args[0].dataSz >= 16) memcpy(args[0].pdata + 8, &rows_, 8); }
-        if (args[0].pnulls) {
-            if (is_device_ptr(args[0].pnulls)) { MOB_CUDA_TRY(cudaMemcpyAsync(args[0].pnulls, &nullword_, 8, cudaMemcpyHostToDevice, t.stream)); MOB_CUDA_TRY(cudaStreamSynchronize(t.stream)); }
-            else memcpy(args[0].pnulls, &nullword_, 8);
-        }
-        return MO_RC_SUCCESS;
+        return write_q6_result(t, args[0], any_ ? R.a.value : 0.0, R.h.ngroups > 0 ? R.g.rows : 0, any_);
     }
 
     const bool dev = is_device_ptr(args[1].pdata);
@@ -1113,66 +854,37 @@ int xcall_q6(mo_xcall_args_t *args, uint64_t len) {
         }
     }
     if (rc) return rc;
-    uint64_t nullword = any ? 0ull : 1ull;
-    int64_t c64 = (int64_t)cnt;
-    if (is_device_ptr(args[0].pdata)) {
-        MOB_CUDA_TRY(cudaMemcpyAsync(args[0].pdata, &sum, 8, cudaMemcpyHostToDevice, t.stream));
-        if (args[0].dataSz >= 16) MOB_CUDA_TRY(cudaMemcpyAsync(args[0].pdata + 8, &c64, 8, cudaMemcpyHostToDevice, t.stream));
-        MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
-    } else {
-        memcpy(args[0].pdata, &sum, 8);
-        if (args[0].dataSz >= 16) memcpy(args[0].pdata + 8, &c64, 8);
-    }
-    if (args[0].pnulls) {
-        if (is_device_ptr(args[0].pnulls)) { MOB_CUDA_TRY(cudaMemcpyAsync(args[0].pnulls, &nullword, 8, cudaMemcpyHostToDevice, t.stream)); MOB_CUDA_TRY(cudaStreamSynchronize(t.stream)); }
-        else memcpy(args[0].pnulls, &nullword, 8);
-    }
-    return MO_RC_SUCCESS;
+    return write_q6_result(t, args[0], sum, (int64_t)cnt, any);
 }
 
-template <int KEYMODE>
-static int launch_q1(ThreadCtx &t, const int32_t *sd, const double *qty, const double *price, const double *disc, const double *tax,
-                     const uint8_t *rf, const uint8_t *ls, uint64_t n, int32_t cutoff, Q1Rec *hrec, mo_q1_result_t *dres = nullptr, int64_t row_base = 0) {
-    if (!aligned_to(sd, 8) || !aligned_to(qty, 16) || !aligned_to(price, 16) || !aligned_to(disc, 16) || !aligned_to(tax, 16) ||
-        !aligned_to(rf, KEYMODE ? 8 : 2) || !aligned_to(ls, KEYMODE ? 8 : 2)) {
+// device addresses of the Q1 input columns; the key columns hold packed uint8 values or 24-byte varlena cells
+struct Q1Cols { const int32_t *sd; const double *qty, *price, *disc, *tax; const uint8_t *rf, *ls; };
+
+static int launch_q1(ThreadCtx &t, const Q1Cols &c, bool varlena, uint64_t n, int32_t cutoff, Q1Rec *hrec, mo_q1_result_t *dres = nullptr,
+                     int64_t row_base = 0) {
+    if (!aligned_to(c.sd, 8) || !aligned_to(c.qty, 16) || !aligned_to(c.price, 16) || !aligned_to(c.disc, 16) || !aligned_to(c.tax, 16) ||
+        !aligned_to(c.rf, varlena ? 8 : 2) || !aligned_to(c.ls, varlena ? 8 : 2)) {
         set_error("q1: columns must be 16-byte aligned (int32 column 8-byte, key columns 2/8-byte)"); return MO_RC_INVALID_ARGUMENT;
     }
-    // variant: 0 = auto (cp.async-staged kernel, 3 stages, for packed keys; register kernel otherwise), 1 = register kernel,
-    // 2 = register kernel with 8 group slots, 3 = staged with 4 stages, 4 = staged with 5 stages
-    const bool can_stage = KEYMODE == 0 && aligned_to(sd, 16) && aligned_to(rf, 16) && aligned_to(ls, 16) && n >= kTileRows;
+    // The TMA kernel bulk-copies 1024-row tiles of every column, so it needs packed keys and 16-byte aligned sources.  Below 64 tiles
+    // the register kernel serves: there the rows past the last whole tile (up to 1023, taken by one warp) cost the TMA kernel more than
+    // the register kernel's whole pass (DESIGN 5.1).  q1_variant = 1 forces the register kernel, the arm the TMA kernel is tested against.
+    const bool tma = !varlena && aligned_to(c.sd, 16) && aligned_to(c.rf, 16) && aligned_to(c.ls, 16) && n >= (uint64_t)kCtaTileRows * 64 &&
+                     g_q1_variant != 1;
     Q1Rec *first_out = nullptr;   // asynchronous form: result record of the 4-slot pass
     for (int attempt = 0; attempt < 2; attempt++) {
-        const bool wide = attempt == 1 || g_q1_variant == 2;
-        const bool staged = can_stage && !wide && g_q1_variant != 1;
-        int grid = num_sms() * (staged ? 1 : 2);
-        const int threads = staged ? kStagedThreads : kThreads;
-        uint64_t work = staged ? (n / kTileRows + (kStagedThreads / 32) - 1) / (kStagedThreads / 32) : (n / 2 + kThreads - 1) / kThreads;
+        const bool wide = attempt == 1;
+        const bool use_tma = tma && !wide;
+        // TMA kernel: one CTA per SM, each taking whole tiles; register kernel: two CTAs per SM, each thread at least one pair
+        const uint64_t work = use_tma ? n / kCtaTileRows : (n / 2 + kThreads - 1) / kThreads;
+        int grid = num_sms() * (use_tma ? 1 : 2);
         if ((uint64_t)grid > work) grid = work ? (int)work : 1;
         if (grid > kQ1MaxGrid) grid = kQ1MaxGrid;
-        (void)threads;
         Q1Rec *partials = (Q1Rec *)arena_alloc(t, sizeof(Q1Rec) * (size_t)(grid + 1));
         if (!partials) return MO_RC_INTERNAL_ERROR;
         Q1Rec *out = partials + grid;
         if (attempt == 0 || !dres) cudaEventRecord(t.kev0, t.stream);
-        if (staged && g_q1_variant >= 5 && g_q1_variant <= 7) {
-            const int stages = g_q1_variant == 5 ? 3 : (g_q1_variant == 6 ? 4 : 5);
-            const size_t smem = (size_t)(kStagedThreads / 32) * stages * kTileBytes + (size_t)(kStagedThreads / 32) * stages * 8;
-            static bool battr[3] = {false, false, false};
-            const int bi = g_q1_variant - 5;
-            if (!battr[bi]) {
-                cudaError_t e = stages == 3 ? cudaFuncSetAttribute(q1_bulk_kernel<4, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                              : stages == 4 ? cudaFuncSetAttribute(q1_bulk_kernel<4, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                                            : cudaFuncSetAttribute(q1_bulk_kernel<4, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                if (e != cudaSuccess) { set_error("q1: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return MO_RC_INTERNAL_ERROR; }
-                battr[bi] = true;
-            }
-            if (stages == 3) q1_bulk_kernel<4, 3><<<grid, kStagedThreads, smem, t.stream>>>(sd, qty, price, disc, tax, rf, ls, n, cutoff, partials, out, t.ctrl, g_q1_dbg);
-            else if (stages == 4) q1_bulk_kernel<4, 4><<<grid, kStagedThreads, smem, t.stream>>>(sd, qty, price, disc, tax, rf, ls, n, cutoff, partials, out, t.ctrl, g_q1_dbg);
-            else q1_bulk_kernel<4, 5><<<grid, kStagedThreads, smem, t.stream>>>(sd, qty, price, disc, tax, rf, ls, n, cutoff, partials, out, t.ctrl, g_q1_dbg);
-        } else if (staged && (g_q1_variant == 10 || g_q1_variant == 0) && n >= (uint64_t)kCtaTileRows * 64) {   // default for packed keys (measured 1.07 vs 0.83 of the HBM rate for variant B)
-            grid = num_sms();
-            const uint64_t nt = n / kCtaTileRows;
-            if ((uint64_t)grid > nt) grid = (int)nt;
+        if (use_tma) {
             const size_t smem = (size_t)kCtaStages * kCtaTileBytes + 2 * kCtaStages * 8;
             static bool tattr = false;
             if (!tattr) {
@@ -1180,38 +892,13 @@ static int launch_q1(ThreadCtx &t, const int32_t *sd, const double *qty, const d
                 if (e != cudaSuccess) { set_error("q1: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return MO_RC_INTERNAL_ERROR; }
                 tattr = true;
             }
-            q1_tma_kernel<4><<<grid, kCtaThreads, smem, t.stream>>>(sd, qty, price, disc, tax, rf, ls, n, cutoff, partials, out, t.ctrl, g_q1_dbg);
-        } else if (staged && (g_q1_variant == 8 || g_q1_variant == 9) && n < (1ull << 32)) {
-            // shared-memory accumulators: 8 = 3 stages, 9 = 2 stages
-            const int stages = g_q1_variant == 8 ? 3 : 2;
-            const size_t smem = (size_t)(kStagedThreads / 32) * stages * kTileBytes + Q1SmemAcc<kStagedThreads>::kBytes;
-            static bool sattr[2] = {false, false};
-            if (!sattr[stages - 2]) {
-                cudaError_t e = stages == 3 ? cudaFuncSetAttribute(q1_staged_kernel<4, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                                            : cudaFuncSetAttribute(q1_staged_kernel<4, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                if (e != cudaSuccess) { set_error("q1: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return MO_RC_INTERNAL_ERROR; }
-                sattr[stages - 2] = true;
-            }
-            if (stages == 3) q1_staged_kernel<4, 3, true><<<grid, kStagedThreads, smem, t.stream>>>(sd, qty, price, disc, tax, rf, ls, n, cutoff, partials, out, t.ctrl, g_q1_dbg);
-            else q1_staged_kernel<4, 2, true><<<grid, kStagedThreads, smem, t.stream>>>(sd, qty, price, disc, tax, rf, ls, n, cutoff, partials, out, t.ctrl, g_q1_dbg);
-        } else if (staged) {
-            const int stages = g_q1_variant == 3 ? 4 : (g_q1_variant == 4 ? 5 : 3);   // 3 stages measured best (tools/tune.py q1)
-            const size_t smem = (size_t)(kStagedThreads / 32) * stages * kTileBytes;
-            static bool attr_done[3] = {false, false, false};
-            if (!attr_done[stages - 3]) {
-                cudaError_t e = stages == 3 ? cudaFuncSetAttribute(q1_staged_kernel<4, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                              : stages == 4 ? cudaFuncSetAttribute(q1_staged_kernel<4, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                                            : cudaFuncSetAttribute(q1_staged_kernel<4, 5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                if (e != cudaSuccess) { set_error("q1: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return MO_RC_INTERNAL_ERROR; }
-                attr_done[stages - 3] = true;
-            }
-            if (stages == 3) q1_staged_kernel<4, 3, false><<<grid, kStagedThreads, smem, t.stream>>>(sd, qty, price, disc, tax, rf, ls, n, cutoff, partials, out, t.ctrl, g_q1_dbg);
-            else if (stages == 4) q1_staged_kernel<4, 4, false><<<grid, kStagedThreads, smem, t.stream>>>(sd, qty, price, disc, tax, rf, ls, n, cutoff, partials, out, t.ctrl, g_q1_dbg);
-            else q1_staged_kernel<4, 5, false><<<grid, kStagedThreads, smem, t.stream>>>(sd, qty, price, disc, tax, rf, ls, n, cutoff, partials, out, t.ctrl, g_q1_dbg);
+            q1_tma_kernel<4><<<grid, kCtaThreads, smem, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, out, t.ctrl);
         } else if (!wide) {
-            q1_kernel<4, 2, 2, KEYMODE><<<grid, kThreads, 0, t.stream>>>(sd, qty, price, disc, tax, rf, ls, n, cutoff, partials, out, t.ctrl, g_q1_dbg, nullptr);
+            if (varlena) q1_kernel<4, 2, 2, 1><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, out, t.ctrl, nullptr);
+            else q1_kernel<4, 2, 2, 0><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, out, t.ctrl, nullptr);
         } else {
-            q1_kernel<8, 2, 2, KEYMODE><<<grid, kThreads, 0, t.stream>>>(sd, qty, price, disc, tax, rf, ls, n, cutoff, partials, out, t.ctrl, g_q1_dbg, first_out);
+            if (varlena) q1_kernel<8, 2, 2, 1><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, out, t.ctrl, first_out);
+            else q1_kernel<8, 2, 2, 0><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, out, t.ctrl, first_out);
         }
         if (attempt == 0 || !dres) cudaEventRecord(t.kev1, t.stream);
         MOB_LAUNCH_CHECK();
@@ -1258,22 +945,22 @@ int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
     for (int i = 2; i <= 5; i++) if (args[i].dataSz < 8 * len) { set_error("q1: column %d shorter than len", i); return MO_RC_INVALID_ARGUMENT; }
     bool q1_nullable = false;
     for (int i = 1; i <= 7; i++) q1_nullable = q1_nullable || args[i].pnulls != nullptr;
-    int keymode;
-    if (args[6].dataSz == len && args[7].dataSz == len) keymode = 0;
-    else if (args[6].dataSz == 24 * len && args[7].dataSz == 24 * len) keymode = 1;
+    bool varlena;
+    if (args[6].dataSz == len && args[7].dataSz == len) varlena = false;
+    else if (args[6].dataSz == 24 * len && args[7].dataSz == 24 * len) varlena = true;
     else { set_error("q1: key columns must be packed uint8 (len bytes) or varlena cells (24*len bytes)"); return MO_RC_INVALID_ARGUMENT; }
     int32_t cutoff;
     if (is_device_ptr(args[8].pdata)) { int rc = read_back(t, &cutoff, args[8].pdata, 4); if (rc) return rc; }
     else memcpy(&cutoff, args[8].pdata, 4);
     const bool dev = is_device_ptr(args[1].pdata);
     for (int i = 2; i <= 7; i++) if (is_device_ptr(args[i].pdata) != dev) { set_error("q1: columns must all be host or all device"); return MO_RC_INVALID_ARGUMENT; }
-    const uint64_t ksz = keymode ? 24 : 1;
+    const uint64_t ksz = varlena ? 24 : 1;
     int64_t row_base = 0;   // optional: params = {int32 cutoff; int32 pad; int64 row_base} -> first_row values are global row numbers
     if (args[8].dataSz >= 16 && !is_device_ptr(args[8].pdata)) memcpy(&row_base, args[8].pdata + 8, 8);
     if (q1_nullable) {
         // nullable inputs: the generic fused operator (plan.cu).  NULL shipdate rejects the row; NULL values are skipped by their aggregates;
         // a NULL key is its own group (has_null_keys; its key byte reads 0 here).  Packed uint8 keys only.
-        if (keymode != 0) { set_error("q1: nullable columns need packed uint8 key columns"); return MO_RC_INVALID_ARGUMENT; }
+        if (varlena) { set_error("q1: nullable columns need packed uint8 key columns"); return MO_RC_INVALID_ARGUMENT; }
         mo_plan_t Q; memset(&Q, 0, sizeof Q);
         Q.ncols = 7; Q.col_type[0] = MO_T_DATE; for (int c = 1; c <= 4; c++) Q.col_type[c] = MO_T_FLOAT64; Q.col_type[5] = Q.col_type[6] = MO_T_UINT8;
         Q.row_base = row_base; Q.has_null_keys = (args[6].pnulls || args[7].pnulls) ? 1 : 0;
@@ -1314,16 +1001,14 @@ int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
             o.avg_disc = r.a[4].count ? r.a[4].value / (double)r.a[4].count : 0.0;
             o.count_order = r.a[5].count;
         }
-        if (is_device_ptr(args[0].pdata)) { MOB_CUDA_TRY(cudaMemcpyAsync(args[0].pdata, &res, sizeof res, cudaMemcpyHostToDevice, t.stream)); MOB_CUDA_TRY(cudaStreamSynchronize(t.stream)); }
-        else memcpy(args[0].pdata, &res, sizeof res);
-        return MO_RC_SUCCESS;
+        return write_result(t, args[0].pdata, &res, sizeof res);
     }
 
+    const Q1Cols cols{(const int32_t *)args[1].pdata, (const double *)args[2].pdata, (const double *)args[3].pdata, (const double *)args[4].pdata,
+                      (const double *)args[5].pdata, args[6].pdata, args[7].pdata};
     if (dev && len && is_device_ptr(args[0].pdata)) {
         // resident columns AND a device result: enqueue only (see xcall_q6)
-        mo_q1_result_t *dres = (mo_q1_result_t *)args[0].pdata;
-        int rc = keymode ? launch_q1<1>(t, (const int32_t *)args[1].pdata, (const double *)args[2].pdata, (const double *)args[3].pdata, (const double *)args[4].pdata, (const double *)args[5].pdata, args[6].pdata, args[7].pdata, len, cutoff, nullptr, dres, row_base)
-                         : launch_q1<0>(t, (const int32_t *)args[1].pdata, (const double *)args[2].pdata, (const double *)args[3].pdata, (const double *)args[4].pdata, (const double *)args[5].pdata, args[6].pdata, args[7].pdata, len, cutoff, nullptr, dres, row_base);
+        int rc = launch_q1(t, cols, varlena, len, cutoff, nullptr, (mo_q1_result_t *)args[0].pdata, row_base);
         arena_reset(t);
         return rc;
     }
@@ -1333,8 +1018,7 @@ int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
     if (dev || len == 0) {
         if (len) {
             Q1Rec R;
-            rc = keymode ? launch_q1<1>(t, (const int32_t *)args[1].pdata, (const double *)args[2].pdata, (const double *)args[3].pdata, (const double *)args[4].pdata, (const double *)args[5].pdata, args[6].pdata, args[7].pdata, len, cutoff, &R)
-                         : launch_q1<0>(t, (const int32_t *)args[1].pdata, (const double *)args[2].pdata, (const double *)args[3].pdata, (const double *)args[4].pdata, (const double *)args[5].pdata, args[6].pdata, args[7].pdata, len, cutoff, &R);
+            rc = launch_q1(t, cols, varlena, len, cutoff, &R);
             if (!rc) q1_merge_rec(F, R, first);
         }
         arena_reset(t);
@@ -1342,17 +1026,13 @@ int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
         for (uint64_t r0 = 0; r0 < len && rc == MO_RC_SUCCESS; r0 += kHostChunkRows) {
             uint64_t m = len - r0 < kHostChunkRows ? len - r0 : kHostChunkRows;
             Stager st(t);
-            const int32_t *d_sd = (const int32_t *)st.in(args[1].pdata + 4 * r0, 4 * m);
-            const double *d_q = (const double *)st.in(args[2].pdata + 8 * r0, 8 * m);
-            const double *d_p = (const double *)st.in(args[3].pdata + 8 * r0, 8 * m);
-            const double *d_d = (const double *)st.in(args[4].pdata + 8 * r0, 8 * m);
-            const double *d_t = (const double *)st.in(args[5].pdata + 8 * r0, 8 * m);
-            const uint8_t *d_rf = (const uint8_t *)st.in(args[6].pdata + ksz * r0, ksz * m);
-            const uint8_t *d_ls = (const uint8_t *)st.in(args[7].pdata + ksz * r0, ksz * m);
+            const Q1Cols d{(const int32_t *)st.in(args[1].pdata + 4 * r0, 4 * m), (const double *)st.in(args[2].pdata + 8 * r0, 8 * m),
+                           (const double *)st.in(args[3].pdata + 8 * r0, 8 * m), (const double *)st.in(args[4].pdata + 8 * r0, 8 * m),
+                           (const double *)st.in(args[5].pdata + 8 * r0, 8 * m), (const uint8_t *)st.in(args[6].pdata + ksz * r0, ksz * m),
+                           (const uint8_t *)st.in(args[7].pdata + ksz * r0, ksz * m)};
             if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
             Q1Rec R;
-            rc = keymode ? launch_q1<1>(t, d_sd, d_q, d_p, d_d, d_t, d_rf, d_ls, m, cutoff, &R)
-                         : launch_q1<0>(t, d_sd, d_q, d_p, d_d, d_t, d_rf, d_ls, m, cutoff, &R);
+            rc = launch_q1(t, d, varlena, m, cutoff, &R);
             if (!rc) {
                 for (int g = 0; g < MO_Q1_MAX_GROUPS; g++) if (R.slot[g].used && R.slot[g].cnt) R.slot[g].first_row += r0;
                 q1_merge_rec(F, R, first);
@@ -1365,11 +1045,7 @@ int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
     if (F.overflow) { set_error("q1: too many groups"); return MO_RC_INVALID_ARGUMENT; }
     mo_q1_result_t res;
     q1_finalize(F, &res, row_base);
-    if (is_device_ptr(args[0].pdata)) {
-        MOB_CUDA_TRY(cudaMemcpyAsync(args[0].pdata, &res, sizeof res, cudaMemcpyHostToDevice, t.stream));
-        MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
-    } else memcpy(args[0].pdata, &res, sizeof res);
-    return MO_RC_SUCCESS;
+    return write_result(t, args[0].pdata, &res, sizeof res);
 }
 
 // MO_XCALL_Q6_MERGE: args[0] = result as MO_XCALL_Q6_FILTER_SUM ; args[1] = len partial results of 16 bytes (sum f64, count i64)

@@ -32,7 +32,6 @@ int xcall_bruteforce(mo_xcall_args_t *args, uint64_t len);
 int xcall_ivf(mo_xcall_args_t *args, uint64_t len);
 int xcall_topk_merge(mo_xcall_args_t *args, uint64_t len);
 int tuning_set(const char *name, int value);
-unsigned long long *q1_debug_buffer();
 }  // namespace mob
 
 using namespace mob;
@@ -86,6 +85,3 @@ extern "C" int32_t XCall(int64_t runtimeId, int64_t funcId, uint8_t *errStr, uin
 }
 
 extern "C" int32_t MoB200_SetTuning(const char *name, int32_t value) { return tuning_set(name, value); }
-
-// debug aid for tools/q1_phases.py: device address of the per-CTA phase timestamps (8 x uint64 per CTA), or NULL
-extern "C" void *MoB200_DebugBuffer(void) { return q1_debug_buffer(); }

@@ -93,6 +93,20 @@ def _no_device_checks(lib):
     assert rc in (-1, capi.RC_INTERNAL_ERROR)
 
 
+def test_set_tuning_accepts_only_known_kernel_variants(lib):
+    """q1_variant and q6_variant take 0 (kernel chosen from the input) or 1 (the reference kernel); any other value, and an unknown
+    name, returns -1"""
+    try:
+        for name, bad in ((b"q1_variant", (2, 10, -1)), (b"q6_variant", (2, 3))):
+            for v in bad:
+                assert lib.MoB200_SetTuning(name, v) == -1, (name, v)
+            assert lib.MoB200_SetTuning(name, 1) == 0
+            assert lib.MoB200_SetTuning(name, 0) == 0
+        assert lib.MoB200_SetTuning(b"q1_debug", 1) == -1
+    finally:
+        lib.MoB200_SetTuning(b"q1_variant", 0); lib.MoB200_SetTuning(b"q6_variant", 0)
+
+
 def test_missing_library_raises_importerror(tmp_path):
     with pytest.raises(ImportError):
         capi.load_library(str(tmp_path / "libmo_b200.so"))
