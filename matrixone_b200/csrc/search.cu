@@ -446,6 +446,7 @@ int xcall_bruteforce(mo_xcall_args_t *args, uint64_t len) {
     int64_t *ok = (int64_t *)st.out(args[0].pdata, (size_t)P.nq * P.k * 8);
     double *od = (double *)st.out(args[1].pdata, (size_t)P.nq * P.k * 8);
     if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    g_last_tc_kused = 0; g_last_tc_fallbacks = -1;   // the statistics describe this search, also when it does not reach the tensor cores
     if (tc_search_applicable(P.n, (int)P.dim, P.nq, P.k, P.metric))
         rc = bruteforce_topk_tc_device(t, ddata, P.n, (int)P.dim, dq, P.nq, P.k, P.key_base, P.sqrt_out, ok, od, true, (int)P.metric);
     else
@@ -608,7 +609,7 @@ int xcall_ivf(mo_xcall_args_t *args, uint64_t len) {
     else memcpy(offsets.data(), args[6].pdata, offsets.size() * 8);
 
     IvfJob job{dcent, P.nlist, ddata, P.n, dim, &offsets, doffsets, drowids, (int)P.k, nprobe, (int)P.metric, (int)P.sqrt_out};
-    g_last_tc_fallbacks = -1; g_last_tc_refined = -1;
+    g_last_tc_fallbacks = -1; g_last_tc_refined = -1; g_last_tc_kused = 0; g_last_tc_probe_kused = 0;
     rc = ivf_search_level(t, job, 0, dq, P.nq, ok, od);
     int frc = st.finish();
     return rc ? rc : frc;
@@ -630,10 +631,12 @@ int ivf_make_plan(ThreadCtx &t, const float *dcent, int64_t nlist, int dim, cons
     plan.bucket_l = (int32_t *)arena_alloc(t, (size_t)npairs * 4);
     if (!plan.probes || !probe_d || !cnt || !plan.bucket_q || !plan.bucket_slot || !plan.pair_pos || !plan.bucket_l) return MO_RC_INTERNAL_ERROR;
     // exact either way: the tensor-core pass proves its top-nprobe complete or re-runs the query through the exact kernel
+    g_last_tc_pass_k = 0;
     int rc = tc_probe_applicable(nlist, dim, nq, nprobe, metric)
                  ? bruteforce_topk_tc_device(t, dcent, nlist, dim, dq, nq, nprobe, 0, 0, plan.probes, probe_d, false)
                  : bruteforce_topk_device(t, dcent, nlist, dim, dq, nq, nprobe, metric, 0, 0, plan.probes, probe_d);
     if (rc) return rc;
+    g_last_tc_probe_kused = g_last_tc_pass_k;
     int *dstart = cnt + nlist, *cursor = cnt + 2 * nlist;
     if (doffsets) { ivf_mask_empty_kernel<<<num_sms() * 4, 256, 0, t.stream>>>(plan.probes, npairs, doffsets); MOB_LAUNCH_CHECK(); }
     MOB_CUDA_TRY(cudaMemsetAsync(cnt, 0, (size_t)nlist * 4 * 3, t.stream));

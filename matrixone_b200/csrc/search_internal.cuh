@@ -45,5 +45,8 @@ void tc_one_term_report(int64_t nq, int64_t failed);
 
 extern thread_local int g_last_tc_fallbacks;   // queries of the last tensor-core search that ended in the exact kernel
 extern thread_local int g_last_tc_refined;     // IVF: queries of the last search that needed the sub-range refine pass
+extern thread_local int g_last_tc_kused;       // K columns the last search's candidate pass multiplied (0: it ran no candidate pass)
+extern thread_local int g_last_tc_pass_k;      // K columns of the last candidate pass launched on this thread (probe passes included)
+extern thread_local int g_last_tc_probe_kused; // K columns of the last IVF search's centroid probe pass (0: exact kernel)
 
 }  // namespace mob

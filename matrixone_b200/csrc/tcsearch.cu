@@ -140,16 +140,30 @@ __device__ __forceinline__ unsigned long long make_desc(unsigned smem_addr) {
 }
 
 // bound on |approximate - real| squared distance of one (query operand, row operand) pair, from the operand norms:
-//   three-term product: |2 q.x error| <= 2 (3 * 2^-16 [dropped lo.lo + bf16 residuals] + 144 * 2^-23 [fp32 accumulation over K'/16
-//     MMA steps]) |q||x| < 2^-12.8 |q||x|; 2^-12 is used
+//   fp32 accumulation: a pass of nkb k-blocks runs steps = 4 nkb k16 MMA steps.  The H100 aligns the 16 products of a step to
+//     the largest term (a product or the running sum) and truncates what falls below a few bits past that term's last fp32 bit,
+//     then truncates the sum (measured: sixteen products of just under 1/4 ulp of the running sum are all lost, so fewer than
+//     3 extra bits; tests/test_gpu_tcsearch_exact.py, hidden_neighbour_data).  Priced with no extra bit at all, each product
+//     loses less than one ulp of the largest term and the sum one more: 17 ulps a step.  Every term is at most
+//     sum |q_i x_i| <= |q||x|, so |q.x error| <= 17 steps 2^-23 |q||x| and the distance (2 q.x) carries 34 steps 2^-23 |q||x|
+//   three-term product (K' = 3 dim): 2 * 3 * 2^-16 [dropped lo.lo + bf16 residuals] + accumulation; up to 37 steps (dim <= 192)
+//     that stays under 2^-12, the coefficient used there
 //   one-term (hi-only) product: q.x - qh.xh = qh.xL + qL.xh + qL.xL with qL = q - qh, xL = x - xh known exactly, so
-//     |error| <= |q||xL| + |qL||x| + 3 |qL||xL|  (|qh| <= |q| + |qL|); fp32 accumulation over dim/16 MMA steps < 2^-17 |q||x|
+//     |error| <= |q||xL| + |qL||x| + 3 |qL||xL|  (|qh| <= |q| + |qL|), plus accumulation (at least 2^-16)
 //   both: norm / final-formula / residual-formation rounding 2^-20 (|q|^2 + |x|^2)
-// qn, ql = |q|^2, |q - hi(q)|^2 of the query operand; xm, xl = the largest |x|^2, |x - hi(x)|^2 over the row operand
-__device__ __forceinline__ float tc_eps(float qn, float ql, float xm, float xl, int one_term) {
+// qn, ql = |q|^2, |q - hi(q)|^2 of the query operand; xm, xl = the largest |x|^2, |x - hi(x)|^2 over the row operand;
+// nkb = the 64-column k-blocks the candidate pass ran.
+// sqrt(a b) of two squared norms; where a b leaves the normal fp32 range (rows scaled by 1e-18 or 1e18) it is taken as
+// sqrt(a) sqrt(b), so that the bound neither underflows to nothing nor overflows to infinity
+__device__ __forceinline__ float root_mul(float a, float b) {
+    const float p = a * b;
+    return p >= 1e-30f && p <= 1e30f ? sqrtf(p) : sqrtf(a) * sqrtf(b);
+}
+__device__ __forceinline__ float tc_eps(float qn, float ql, float xm, float xl, int one_term, int nkb) {
+    const float acc = (float)(4 * nkb) * 4.0531158447265625e-6f;   // 34 steps 2^-23
     if (one_term)
-        return 2.002f * (sqrtf(qn * xl) + sqrtf(ql * xm) + 3.0f * sqrtf(ql * xl)) + 1.52587890625e-5f * sqrtf(qn * xm) + 9.5367431640625e-7f * (qn + xm);
-    return 2.44140625e-4f * sqrtf(qn * xm) + 9.5367431640625e-7f * (qn + xm);
+        return 2.002f * (root_mul(qn, xl) + root_mul(ql, xm) + 3.0f * root_mul(ql, xl)) + fmaxf(1.52587890625e-5f, acc) * root_mul(qn, xm) + 9.5367431640625e-7f * (qn + xm);
+    return fmaxf(2.44140625e-4f, 9.1552734375e-5f + acc) * root_mul(qn, xm) + 9.5367431640625e-7f * (qn + xm);
 }
 
 // one work unit: up to kTileM rows of the A' operand (queries) x dataset rows [n_begin, n_end); lists are written at out_base + row
@@ -306,7 +320,7 @@ tc_candidates_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
             // above it cannot displace the k-th result, so they are excluded exactly like rows beyond a full list (thr only falls)
             const bool share = qbound != nullptr && valid_row;
             const int qid = share ? (row_query ? row_query[U.a_row0 + row_in_unit] : U.a_row0 + row_in_unit) : 0;
-            const float my_eps = share ? tc_eps(qn, one_term ? alonorm[U.a_row0 + row_in_unit] : 0.f, xmax2[0], one_term ? xmax2[1] : 0.f, one_term) : 0.f;
+            const float my_eps = share ? tc_eps(qn, one_term ? alonorm[U.a_row0 + row_in_unit] : 0.f, xmax2[0], one_term ? xmax2[1] : 0.f, one_term, nkb) : 0.f;
             float cap = INFINITY, published = INFINITY;
             for (int n0 = U.n_begin; n0 < U.n_end; n0 += BN, tile++) {
                 const unsigned xb = tile & 1;
@@ -460,6 +474,8 @@ __global__ void split_residual_kernel(const float *__restrict__ x, int64_t n, in
                 }
                 *reinterpret_cast<int4 *>(o + j) = *reinterpret_cast<const int4 *>(h);
             }
+            // the pass reads whole 64-column k-blocks: the columns from dim to the next multiple of 64 must be zero, not stale scratch
+            for (int j = dim + lane; j < kprime && j < (dim + BK - 1) / BK * BK; j += 32) o[j] = __float2bfloat16_rn(0.f);
             s = warp_sum_f64(s); sl = warp_sum_f64(sl);
             if (lane == 0) { norm[r] = (float)s; lonorm[r] = (float)sl; }
             continue;
@@ -524,13 +540,13 @@ constexpr int kMergeSlots = kMaxMergeLists / 32;
 __global__ void tc_merge_kernel(int nq, int R, const float *__restrict__ part_d, const int *__restrict__ part_i,
                                 const float *__restrict__ part_thr, const int *__restrict__ pos_map, int pos_cols, long long pos_stride,
                                 const float *__restrict__ pnorm, const float *__restrict__ plonorm, const float *__restrict__ xmax2, int one_term,
-                                const float *__restrict__ qnorm, const float *__restrict__ qlonorm, int k, int dim,
+                                const float *__restrict__ qnorm, const float *__restrict__ qlonorm, int k, int dim, int nkb,
                                 int kp, int kr, int *__restrict__ cand, float *__restrict__ t_excl) {
     const int lane = threadIdx.x & 31;
     const int q = (int)((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5);
     if (q >= nq) return;   // whole warps leave together
     // error bound of every list of this query when it does not depend on the list (brute force: one query operand)
-    const float eps_q = (!pnorm && qnorm) ? tc_eps(qnorm[q], one_term ? qlonorm[q] : 0.f, xmax2[0], one_term ? xmax2[1] : 0.f, one_term) : 0.f;
+    const float eps_q = (!pnorm && qnorm) ? tc_eps(qnorm[q], one_term ? qlonorm[q] : 0.f, xmax2[0], one_term ? xmax2[1] : 0.f, one_term, nkb) : 0.f;
     float sel_d0 = 0.f, sel_d1 = 0.f, sel_e0 = 0.f, sel_e1 = 0.f;   // approximate distance / bound of selections lane and lane + 32
     int nsel = 0;
     long long L[kMergeSlots]; int head[kMergeSlots]; float cur[kMergeSlots], tl[kMergeSlots], eps[kMergeSlots];
@@ -546,7 +562,7 @@ __global__ void tc_merge_kernel(int nq, int R, const float *__restrict__ part_d,
         if (l >= 0) {
             tl[i] = part_thr[l];
             if (part_i[(size_t)l * kp] >= 0) cur[i] = part_d[(size_t)l * kp];
-            if (pnorm && p >= 0) eps[i] = tc_eps(pnorm[p], plonorm[p], xmax2[0], xmax2[1], one_term);
+            if (pnorm && p >= 0) eps[i] = tc_eps(pnorm[p], plonorm[p], xmax2[0], xmax2[1], one_term, nkb);
         }
     }
     for (int j = 0; j < kr; j++) {
@@ -677,7 +693,7 @@ __global__ void tc_max_kernel(const float *__restrict__ v, int64_t n, float *out
 // prove completeness:  every excluded row has approximate distance >= t_excl, |approx - real| <= eps_tc, |real - go| <= eps_go,
 // so d_k + eps_tc + eps_go < t_excl  =>  no excluded row can displace the k-th result.  flag = 1 when the proof fails.
 template <int KRT>
-__global__ void tc_final_kernel(int nq, int k, int64_t n_rows, int dim, const int *__restrict__ cand, const float *__restrict__ exact,
+__global__ void tc_final_kernel(int nq, int k, int64_t n_rows, int dim, int nkb, const int *__restrict__ cand, const float *__restrict__ exact,
                                 const float *__restrict__ t_excl, const float *__restrict__ qnorm, const float *__restrict__ xnorm_max,
                                 const float *__restrict__ qlonorm, const float *__restrict__ xlonorm_max, int one_term, int eps_applied, int metric,
                                 const int64_t *__restrict__ id_map, int64_t key_base, int sqrt_out, int64_t *__restrict__ out_k,
@@ -708,11 +724,11 @@ __global__ void tc_final_kernel(int nq, int k, int64_t n_rows, int dim, const in
     else if (m < k) proven = false;
     else {
         // eps_applied: the merge already lowered t by every list's own bound (IVF residual operands)
-        const float eps_tc = eps_applied ? 0.f : scale * tc_eps(qnorm[q], one_term ? qlonorm[q] : 0.f, *xnorm_max, one_term ? *xlonorm_max : 0.f, one_term);
+        const float eps_tc = eps_applied ? 0.f : scale * tc_eps(qnorm[q], one_term ? qlonorm[q] : 0.f, *xnorm_max, one_term ? *xlonorm_max : 0.f, one_term, nkb);
         // |Go-order fp32 value - real value|: relative dim * 2^-23 for L2; absolute dim * 2^-23 |q||x| for the inner product;
         // for cosine 4 dim 2^-24 (dot product and both norms) + 2^-19 (normalisation of the operands of the candidate pass)
         float eps_go = (float)dim * 1.1920928955078125e-7f * t;
-        if (metric == MO_METRIC_IP) eps_go = (float)dim * 1.1920928955078125e-7f * sqrtf(qnorm[q] * *xnorm_max);
+        if (metric == MO_METRIC_IP) eps_go = (float)dim * 1.1920928955078125e-7f * root_mul(qnorm[q], *xnorm_max);
         if (metric == MO_METRIC_COS) eps_go = (float)dim * 2.384185791015625e-7f + 1.9073486328125e-6f;
         proven = d[k - 1] + eps_tc + eps_go < t;
     }
@@ -746,6 +762,8 @@ int g_tc_sched_mode = 0;         // 1 = static round-robin deal of the units of 
 int g_tc_share_mode = 0;         // 1 = no cross-unit threshold sharing (MoB200_SetTuning("tc_share"))
 int g_tc_ladder_mode = 0;        // 0 = auto (one-term level first unless it has been failing), 1 = never, 2 = always (MoB200_SetTuning("tc_ladder"))
 std::atomic<int> g_one_term_skip{0};   // searches left before the one-term level is tried again (shared by all callers: a property of the data)
+thread_local int g_last_tc_pass_k = 0;   // K elements per pair of the last candidate pass this thread launched, timed or not
+thread_local int g_last_tc_probe_kused = 0;   // ... of the centroid probe of the last IVF search (0: the probe ran on the exact kernel)
 thread_local int g_last_tc_kused = 0;   // (per calling thread, like the kernel timer) K elements per (query, row) pair the timed candidate pass multiplied (dim = one term, 3*dim = three)
 int g_tc_range_mb = 0;         // L2 budget of one row range of the brute-force candidate pass, MB (0 = ignore the L2)
 int g_tc_pair_mode = 0;          // 0 = auto, 1 = single-CTA units only, 2 = CTA pairs wherever the brute-force path runs (MoB200_SetTuning("tc_pair"))
@@ -834,6 +852,7 @@ static int tc_run_units(ThreadCtx &t, const TcOperand &A, int64_t a_rows, const 
     tc_fill_kernel<<<num_sms() * 4, 256, 0, t.stream>>>(*part_thr, *part_i, nlists, kp);
     MOB_LAUNCH_CHECK();
     if (units.empty()) return MO_RC_SUCCESS;
+    g_last_tc_pass_k = nkb * BK;
     MOB_CUDA_TRY(cudaMemcpyAsync(dunits, units.data(), sizeof(TcUnit) * units.size(), cudaMemcpyHostToDevice, t.stream));
     MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
     static bool attr = false;
@@ -899,7 +918,8 @@ static int tc_operand_max(ThreadCtx &t, const TcOperand &B, int64_t n, bool with
 }
 
 // merge approximate lists -> exact re-score -> final order + proof; returns the queries whose proof failed
-static int tc_finish(ThreadCtx &t, const float *ddata, int64_t n, int dim, const float *dq, int64_t nq, int k, int R, const int *pos_map,
+// nkb = the k-blocks the candidate pass ran (its error bound depends on them)
+static int tc_finish(ThreadCtx &t, const float *ddata, int64_t n, int dim, int nkb, const float *dq, int64_t nq, int k, int R, const int *pos_map,
                      int pos_cols, long long pos_stride, const float *part_d, const int *part_i, const float *part_thr, const float *qnorm, const float *xnorm,
                      const int64_t *id_map, int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d, std::vector<int> &redo,
                      const float *qlonorm = nullptr, const float *xlonorm = nullptr,   // both given: the candidate pass was hi-only (one term)
@@ -921,7 +941,7 @@ static int tc_finish(ThreadCtx &t, const float *ddata, int64_t n, int dim, const
         if (one_term) { tc_max_kernel<<<num_sms() * 2, 256, 0, t.stream>>>(xlonorm, n, xlomax); MOB_LAUNCH_CHECK(); }
     }
     if (R > kMaxMergeLists) { set_error("tc search: %d candidate lists per query exceed the merge limit %d", R, kMaxMergeLists); return MO_RC_INTERNAL_ERROR; }
-    tc_merge_kernel<<<(unsigned)((nq + 3) / 4), 128, 0, t.stream>>>((int)nq, R, part_d, part_i, part_thr, pos_map, pos_cols, pos_stride, pair_norm, pair_lonorm, xmax, one_term, qnorm, qlonorm, l2 ? k : (1 << 30) /* pruning bound is L2-specific */, dim, kp, kr, cand, t_excl);
+    tc_merge_kernel<<<(unsigned)((nq + 3) / 4), 128, 0, t.stream>>>((int)nq, R, part_d, part_i, part_thr, pos_map, pos_cols, pos_stride, pair_norm, pair_lonorm, xmax, one_term, qnorm, qlonorm, l2 ? k : (1 << 30) /* pruning bound is L2-specific */, dim, nkb, kp, kr, cand, t_excl);
     MOB_LAUNCH_CHECK();
     {
         const size_t smem = (size_t)(kRescoreThreads / 32) * godist::RingCfg<false>::kStages * godist::RingCfg<false>::kStageBytes;
@@ -939,8 +959,8 @@ static int tc_finish(ThreadCtx &t, const float *ddata, int64_t n, int dim, const
         else tc_rescore_kernel<MO_METRIC_L2SQ><<<(unsigned)blocks, kRescoreThreads, smem, t.stream>>>(ddata, dq, dim, (int)nq, kr, cand, exact);
         MOB_LAUNCH_CHECK();
     }
-    if (kr == KR) tc_final_kernel<KR><<<(unsigned)((nq + 127) / 128), 128, 0, t.stream>>>((int)nq, k, n, dim, cand, exact, t_excl, qnorm, xmax, qlonorm, xlomax, one_term, pair_norm ? 1 : 0, metric, id_map, key_base, sqrt_out, out_k, out_d, flags);
-    else tc_final_kernel<KR_WIDE><<<(unsigned)((nq + 127) / 128), 128, 0, t.stream>>>((int)nq, k, n, dim, cand, exact, t_excl, qnorm, xmax, qlonorm, xlomax, one_term, pair_norm ? 1 : 0, metric, id_map, key_base, sqrt_out, out_k, out_d, flags);
+    if (kr == KR) tc_final_kernel<KR><<<(unsigned)((nq + 127) / 128), 128, 0, t.stream>>>((int)nq, k, n, dim, nkb, cand, exact, t_excl, qnorm, xmax, qlonorm, xlomax, one_term, pair_norm ? 1 : 0, metric, id_map, key_base, sqrt_out, out_k, out_d, flags);
+    else tc_final_kernel<KR_WIDE><<<(unsigned)((nq + 127) / 128), 128, 0, t.stream>>>((int)nq, k, n, dim, nkb, cand, exact, t_excl, qnorm, xmax, qlonorm, xlomax, one_term, pair_norm ? 1 : 0, metric, id_map, key_base, sqrt_out, out_k, out_d, flags);
     MOB_LAUNCH_CHECK();
     std::vector<int> hflags((size_t)nq);
     MOB_CUDA_TRY(cudaMemcpyAsync(hflags.data(), flags, sizeof(int) * (size_t)nq, cudaMemcpyDeviceToHost, t.stream));
@@ -1077,7 +1097,7 @@ static int bf_tc_level(ThreadCtx &t, int level, int metric, const float *ddata, 
     rc = tc_run_units(t, A, nq, B, n, units, (int64_t)R * nq, &part_d, &part_i, &part_thr, timed, pair, nkb, KP, k <= KP ? &sh : nullptr);
     if (rc) return rc;
     std::vector<int> redo;
-    rc = tc_finish(t, ddata, n, dim, dq, nq, k, R, nullptr, 0, 0, part_d, part_i, part_thr, A.norm, B.norm, nullptr, key_base, sqrt_out, out_k, out_d, redo,
+    rc = tc_finish(t, ddata, n, dim, nkb, dq, nq, k, R, nullptr, 0, 0, part_d, part_i, part_thr, A.norm, B.norm, nullptr, key_base, sqrt_out, out_k, out_d, redo,
                    one_term ? A.lonorm : nullptr, one_term ? B.lonorm : nullptr, nullptr, nullptr, KP, metric, xmax2);
     if (rc) return rc;
     if (record_stats && level == 0) {
@@ -1223,11 +1243,12 @@ int ivf_tc_scan(ThreadCtx &t, const IvfPlan &plan, const float *ddata, int64_t n
         ivf_seed_bound_kernel<<<(unsigned)blocks, kRescoreThreads, smem, t.stream>>>(ddata, dq, dim, (int)nq, plan.nprobe, k, plan.probes, doffsets, sh.qbound);
         MOB_LAUNCH_CHECK();
     }
-    rc = tc_run_units(t, A, plan.npairs, B, n, units, plan.npairs * split, &part_d, &part_i, &part_thr, !refine, false, one_term ? (dim + BK - 1) / BK : 0, kp, &sh);
+    const int nkb = one_term ? (dim + BK - 1) / BK : A.kprime / BK;
+    rc = tc_run_units(t, A, plan.npairs, B, n, units, plan.npairs * split, &part_d, &part_i, &part_thr, !refine, false, nkb, kp, &sh);
     if (rc) return rc;
     // the approximate lists are indexed by bucket position; tc_finish walks them per query through pair_pos; the final keys are
     // the primary keys row_ids[local row]; every probed list's exclusion bound is lowered by the error bound of ITS operand pair
-    rc = tc_finish(t, ddata, n, dim, dq, nq, k, plan.nprobe * split, plan.pair_pos, plan.nprobe, plan.npairs, part_d, part_i, part_thr, nullptr, B.norm, drowids, 0,
+    rc = tc_finish(t, ddata, n, dim, nkb, dq, nq, k, plan.nprobe * split, plan.pair_pos, plan.nprobe, plan.npairs, part_d, part_i, part_thr, nullptr, B.norm, drowids, 0,
                    sqrt_out, ok, od, redo, nullptr, one_term ? B.lonorm : nullptr, A.norm, A.lonorm, kp, MO_METRIC_L2SQ, xmax2);
     return rc;
 }
