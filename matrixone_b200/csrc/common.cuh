@@ -45,6 +45,8 @@ bool is_device_ptr(const void *p);
 
 // prepared search operands (tcsearch.cu) that read [p, p + bytes) are dropped: called by every library entry point that WRITES device memory
 void search_invalidate(const void *p, uint64_t bytes);
+// MoB200_SetTuning names of the search module (tcsearch.cu): false for any other name, else *out = the answer (0 for a knob)
+bool search_tuning(const char *name, int value, int *out);
 
 // --- device scratch arena -------------------------------------------------------------------------------
 void *arena_alloc(ThreadCtx &t, size_t bytes);   // 256-byte aligned; nullptr on failure (error set)

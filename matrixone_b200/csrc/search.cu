@@ -296,6 +296,30 @@ __global__ void cos_norm_kernel(const float *__restrict__ v, int64_t n, int dim,
     }
 }
 
+// COS: the squared norms of the rows and of the queries that bf_topk_kernel divides by (other metrics: none)
+int cos_norms(ThreadCtx &t, int metric, const float *ddata, int64_t n, const float *dq, int64_t nq, int dim, float **xnorm, float **qnorm) {
+    *xnorm = *qnorm = nullptr;
+    if (metric != MO_METRIC_COS) return MO_RC_SUCCESS;
+    *xnorm = (float *)arena_alloc(t, sizeof(float) * (size_t)(n > 0 ? n : 1));
+    *qnorm = (float *)arena_alloc(t, sizeof(float) * (size_t)nq);
+    if (!*xnorm || !*qnorm) return MO_RC_INTERNAL_ERROR;
+    if (n > 0) { cos_norm_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(ddata, n, dim, *xnorm); MOB_LAUNCH_CHECK(); }
+    cos_norm_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(dq, nq, dim, *qnorm); MOB_LAUNCH_CHECK();
+    return MO_RC_SUCCESS;
+}
+
+__global__ void gather_rows_kernel(const float *__restrict__ src, const int *__restrict__ idx, int m, int dim, float *__restrict__ dst) {
+    for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < (int64_t)m * dim; e += (int64_t)gridDim.x * blockDim.x)
+        dst[e] = src[(int64_t)idx[e / dim] * dim + e % dim];
+}
+__global__ void scatter_results_kernel(const int64_t *__restrict__ sk, const double *__restrict__ sd, const int *__restrict__ idx, int m, int k,
+                                       int64_t *__restrict__ out_k, double *__restrict__ out_d) {
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < m * k; e += gridDim.x * blockDim.x) {
+        const int q = idx[e / k];
+        out_k[(size_t)q * k + e % k] = sk[e]; out_d[(size_t)q * k + e % k] = sd[e];
+    }
+}
+
 // merge nlists sorted (dist,id) lists of length k per query into the final keys/distances.
 // in_i holds LOCAL ids when id_map/key_base describe the translation, or final int64 keys when in_k is given.
 __global__ void topk_merge_kernel(int64_t nq, int k, int nlists, int64_t list_stride /* in queries */, const float *__restrict__ in_d,
@@ -395,14 +419,9 @@ int bruteforce_topk_device(ThreadCtx &t, const float *ddata, int64_t n, int dim,
     const int64_t tiles_per = (ntiles + R - 1) / R;
     R = n > 0 ? (ntiles + tiles_per - 1) / tiles_per : 1;
     const int nitems = (int)(R * nqt);
-    float *xnorm = nullptr, *qnorm = nullptr;
-    if (metric == MO_METRIC_COS) {
-        xnorm = (float *)arena_alloc(t, sizeof(float) * (size_t)(n > 0 ? n : 1));
-        qnorm = (float *)arena_alloc(t, sizeof(float) * (size_t)nq);
-        if (!xnorm || !qnorm) return MO_RC_INTERNAL_ERROR;
-        if (n > 0) { cos_norm_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(ddata, n, dim, xnorm); MOB_LAUNCH_CHECK(); }
-        cos_norm_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(dq, nq, dim, qnorm); MOB_LAUNCH_CHECK();
-    }
+    float *xnorm, *qnorm;
+    int rc = cos_norms(t, metric, ddata, n, dq, nq, dim, &xnorm, &qnorm);
+    if (rc) return rc;
     std::vector<WorkDesc> items((size_t)nitems);
     for (int64_t r = 0; r < R; r++)
         for (int qt = 0; qt < nqt; qt++) {
@@ -420,7 +439,7 @@ int bruteforce_topk_device(ThreadCtx &t, const float *ddata, int64_t n, int dim,
     if (!ditems || !part_d || !part_i) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemcpyAsync(ditems, items.data(), sizeof(WorkDesc) * (size_t)nitems, cudaMemcpyHostToDevice, t.stream));
     MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));   // items is pageable host memory about to go out of scope
-    int rc = launch_bf_metric(t, metric, ditems, nitems, dim, k, part_d, part_i);
+    rc = launch_bf_metric(t, metric, ditems, nitems, dim, k, part_d, part_i);
     if (rc) return rc;
     topk_merge_kernel<<<(unsigned)((nq + 127) / 128), 128, 0, t.stream>>>(nq, k, (int)R, nq, part_d, part_i, nullptr, nullptr, nullptr, key_base, sqrt_out, 0, out_k, out_d);
     MOB_LAUNCH_CHECK();
@@ -446,7 +465,7 @@ int xcall_bruteforce(mo_xcall_args_t *args, uint64_t len) {
     int64_t *ok = (int64_t *)st.out(args[0].pdata, (size_t)P.nq * P.k * 8);
     double *od = (double *)st.out(args[1].pdata, (size_t)P.nq * P.k * 8);
     if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
-    g_last_tc_kused = 0; g_last_tc_fallbacks = -1;   // the statistics describe this search, also when it does not reach the tensor cores
+    g_search_stats = SearchStats();   // the statistics describe this search, also when it does not reach the tensor cores
     if (tc_search_applicable(P.n, (int)P.dim, P.nq, P.k, P.metric))
         rc = bruteforce_topk_tc_device(t, ddata, P.n, (int)P.dim, dq, P.nq, P.k, P.key_base, P.sqrt_out, ok, od, true, (int)P.metric);
     else
@@ -513,21 +532,29 @@ __global__ void ivf_fill_kernel(const int64_t *probes, int64_t npairs, int nprob
     }
 }
 
-__global__ void ivf_gather_queries_kernel(const float *__restrict__ src, const int *__restrict__ idx, int m, int dim, float *__restrict__ dst) {
-    for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < (int64_t)m * dim; e += (int64_t)gridDim.x * blockDim.x)
-        dst[e] = src[(int64_t)idx[e / dim] * dim + e % dim];
-}
-__global__ void ivf_scatter_kernel(const int64_t *__restrict__ sk, const double *__restrict__ sd, const int *__restrict__ idx, int m, int k,
-                                   int64_t *__restrict__ out_k, double *__restrict__ out_d) {
-    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < m * k; e += gridDim.x * blockDim.x) {
-        const int q = idx[e / k];
-        out_k[(size_t)q * k + e % k] = sk[e]; out_d[(size_t)q * k + e % k] = sd[e];
-    }
-}
-
 }  // namespace
 
 namespace mob {
+
+int redo_queries(ThreadCtx &t, const std::vector<int> &redo, const float *dq, int dim, int k, int64_t *out_k, double *out_d,
+                 const std::function<int(const float *sub, int64_t m, int64_t *sk, double *sd)> &next) {
+    if (redo.empty()) return MO_RC_SUCCESS;
+    const int m = (int)redo.size();
+    int *didx = (int *)arena_alloc(t, sizeof(int) * (size_t)m);
+    float *sub = (float *)arena_alloc(t, sizeof(float) * (size_t)m * dim);
+    int64_t *sk = (int64_t *)arena_alloc(t, sizeof(int64_t) * (size_t)m * k);
+    double *sd = (double *)arena_alloc(t, sizeof(double) * (size_t)m * k);
+    if (!didx || !sub || !sk || !sd) return MO_RC_INTERNAL_ERROR;
+    MOB_CUDA_TRY(cudaMemcpyAsync(didx, redo.data(), sizeof(int) * (size_t)m, cudaMemcpyHostToDevice, t.stream));
+    MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
+    gather_rows_kernel<<<num_sms() * 4, 256, 0, t.stream>>>(dq, didx, m, dim, sub);
+    MOB_LAUNCH_CHECK();
+    int rc = next(sub, m, sk, sd);
+    if (rc) return rc;
+    scatter_results_kernel<<<(unsigned)((m * k + 255) / 256), 256, 0, t.stream>>>(sk, sd, didx, m, k, out_k, out_d);
+    MOB_LAUNCH_CHECK();
+    return MO_RC_SUCCESS;
+}
 
 struct IvfJob {
     const float *dcent; int64_t nlist; const float *ddata; int64_t n; int dim; const std::vector<int64_t> *offsets; const int64_t *doffsets;
@@ -544,7 +571,7 @@ static int ivf_search_level(ThreadCtx &t, const IvfJob &J, int level, const floa
     int rc = ivf_make_plan(t, J.dcent, J.nlist, J.dim, dq, nq, J.nprobe, J.metric, plan, J.doffsets);
     if (rc) return rc;
     if (level >= 2 || !tc_ivf_applicable(J.n, J.dim, nq, J.k, J.nprobe, J.metric, level == 1)) {
-        if (level > 0) g_last_tc_fallbacks = (int)nq;
+        if (level > 0) g_search_stats.fallbacks = (int)nq;
         return ivf_exact_scan(t, plan, J.ddata, J.n, J.dim, dq, nq, *J.offsets, J.drowids, J.k, J.metric, J.sqrt_out, ok, od);
     }
     std::vector<int> redo;
@@ -553,23 +580,10 @@ static int ivf_search_level(ThreadCtx &t, const IvfJob &J, int level, const floa
     rc = ivf_tc_scan(t, plan, J.ddata, J.n, J.dim, dq, nq, J.dcent, J.doffsets, *J.offsets, J.drowids, J.k, J.sqrt_out, pass, ok, od, redo, &nonfinite);
     if (!rc && pass == 0 && !nonfinite) tc_one_term_report(nq, (int64_t)redo.size());
     if (rc) return rc;
-    if (level == 0) { g_last_tc_refined = (int)redo.size(); g_last_tc_fallbacks = 0; }
-    if (redo.empty()) return MO_RC_SUCCESS;
-    const int m = (int)redo.size();
-    int *didx = (int *)arena_alloc(t, sizeof(int) * (size_t)m);
-    float *sub = (float *)arena_alloc(t, sizeof(float) * (size_t)m * J.dim);
-    int64_t *sk = (int64_t *)arena_alloc(t, sizeof(int64_t) * (size_t)m * J.k);
-    double *sd = (double *)arena_alloc(t, sizeof(double) * (size_t)m * J.k);
-    if (!didx || !sub || !sk || !sd) return MO_RC_INTERNAL_ERROR;
-    MOB_CUDA_TRY(cudaMemcpyAsync(didx, redo.data(), sizeof(int) * (size_t)m, cudaMemcpyHostToDevice, t.stream));
-    MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
-    ivf_gather_queries_kernel<<<num_sms() * 4, 256, 0, t.stream>>>(dq, didx, m, J.dim, sub);
-    MOB_LAUNCH_CHECK();
-    rc = ivf_search_level(t, J, nonfinite ? 2 : level + 1, sub, m, sk, sd);
-    if (rc) return rc;
-    ivf_scatter_kernel<<<(unsigned)((m * J.k + 255) / 256), 256, 0, t.stream>>>(sk, sd, didx, m, J.k, ok, od);
-    MOB_LAUNCH_CHECK();
-    return MO_RC_SUCCESS;
+    if (level == 0) { g_search_stats.refined = (int)redo.size(); g_search_stats.fallbacks = 0; }
+    return redo_queries(t, redo, dq, J.dim, J.k, ok, od, [&](const float *sub, int64_t m, int64_t *sk, double *sd) {
+        return ivf_search_level(t, J, nonfinite ? 2 : level + 1, sub, m, sk, sd);
+    });
 }
 
 // IvfflatSearchIndex.Search (pkg/vectorindex/ivfflat/search.go:509-630):
@@ -609,7 +623,7 @@ int xcall_ivf(mo_xcall_args_t *args, uint64_t len) {
     else memcpy(offsets.data(), args[6].pdata, offsets.size() * 8);
 
     IvfJob job{dcent, P.nlist, ddata, P.n, dim, &offsets, doffsets, drowids, (int)P.k, nprobe, (int)P.metric, (int)P.sqrt_out};
-    g_last_tc_fallbacks = -1; g_last_tc_refined = -1; g_last_tc_kused = 0; g_last_tc_probe_kused = 0;
+    g_search_stats = SearchStats();
     rc = ivf_search_level(t, job, 0, dq, P.nq, ok, od);
     int frc = st.finish();
     return rc ? rc : frc;
@@ -631,12 +645,14 @@ int ivf_make_plan(ThreadCtx &t, const float *dcent, int64_t nlist, int dim, cons
     plan.bucket_l = (int32_t *)arena_alloc(t, (size_t)npairs * 4);
     if (!plan.probes || !probe_d || !cnt || !plan.bucket_q || !plan.bucket_slot || !plan.pair_pos || !plan.bucket_l) return MO_RC_INTERNAL_ERROR;
     // exact either way: the tensor-core pass proves its top-nprobe complete or re-runs the query through the exact kernel
-    g_last_tc_pass_k = 0;
-    int rc = tc_probe_applicable(nlist, dim, nq, nprobe, metric)
-                 ? bruteforce_topk_tc_device(t, dcent, nlist, dim, dq, nq, nprobe, 0, 0, plan.probes, probe_d, false)
-                 : bruteforce_topk_device(t, dcent, nlist, dim, dq, nq, nprobe, metric, 0, 0, plan.probes, probe_d);
+    int rc;
+    if (tc_probe_applicable(nlist, dim, nq, nprobe, metric)) {
+        rc = bruteforce_topk_tc_device(t, dcent, nlist, dim, dq, nq, nprobe, 0, 0, plan.probes, probe_d, false);
+    } else {
+        g_search_stats.probe_kused = 0;   // (an earlier level of the ladder may have probed on the tensor cores)
+        rc = bruteforce_topk_device(t, dcent, nlist, dim, dq, nq, nprobe, metric, 0, 0, plan.probes, probe_d);
+    }
     if (rc) return rc;
-    g_last_tc_probe_kused = g_last_tc_pass_k;
     int *dstart = cnt + nlist, *cursor = cnt + 2 * nlist;
     if (doffsets) { ivf_mask_empty_kernel<<<num_sms() * 4, 256, 0, t.stream>>>(plan.probes, npairs, doffsets); MOB_LAUNCH_CHECK(); }
     MOB_CUDA_TRY(cudaMemsetAsync(cnt, 0, (size_t)nlist * 4 * 3, t.stream));
@@ -661,14 +677,9 @@ int ivf_exact_scan(ThreadCtx &t, const IvfPlan &plan, const float *ddata, int64_
                    const std::vector<int64_t> &offsets, const int64_t *drowids, int k, int metric, int sqrt_out, int64_t *ok, double *od) {
     const int64_t nlist = (int64_t)offsets.size() - 1;
     const int64_t npairs = plan.npairs;
-    float *xnorm = nullptr, *qnorm = nullptr;
-    if (metric == MO_METRIC_COS) {
-        xnorm = (float *)arena_alloc(t, sizeof(float) * (size_t)(n > 0 ? n : 1));
-        qnorm = (float *)arena_alloc(t, sizeof(float) * (size_t)nq);
-        if (!xnorm || !qnorm) return MO_RC_INTERNAL_ERROR;
-        if (n > 0) { cos_norm_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(ddata, n, dim, xnorm); MOB_LAUNCH_CHECK(); }
-        cos_norm_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(dq, nq, dim, qnorm); MOB_LAUNCH_CHECK();
-    }
+    float *xnorm, *qnorm;
+    int rc = cos_norms(t, metric, ddata, n, dq, nq, dim, &xnorm, &qnorm);
+    if (rc) return rc;
     std::vector<WorkDesc> items;
     for (int64_t l = 0; l < nlist; l++) {
         const int c = plan.hcnt[(size_t)l];
@@ -690,7 +701,7 @@ int ivf_exact_scan(ThreadCtx &t, const IvfPlan &plan, const float *ddata, int64_
     if (!items.empty()) {
         MOB_CUDA_TRY(cudaMemcpyAsync(ditems, items.data(), sizeof(WorkDesc) * items.size(), cudaMemcpyHostToDevice, t.stream));
         MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
-        int rc = launch_bf_metric(t, metric, ditems, (int)items.size(), dim, k, part_d, part_i);
+        rc = launch_bf_metric(t, metric, ditems, (int)items.size(), dim, k, part_d, part_i);
         if (rc) return rc;
     }
     topk_merge_kernel<<<(unsigned)((nq + 127) / 128), 128, 0, t.stream>>>(nq, k, plan.nprobe, nq, part_d, part_i, nullptr, nullptr, drowids, 0, sqrt_out, 1, ok, od);

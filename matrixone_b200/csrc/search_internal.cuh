@@ -1,6 +1,7 @@
 // search_internal.cuh -- declarations shared by search.cu (exact kernels) and tcsearch.cu (tensor-core candidate pass)
 #pragma once
 #include "common.cuh"
+#include <functional>
 #include <vector>
 
 namespace mob {
@@ -31,6 +32,7 @@ struct SearchReadGuard { SearchReadGuard(); ~SearchReadGuard(); SearchReadGuard(
 bool tc_search_applicable(int64_t n, int dim, int64_t nq, int k, int metric);
 bool tc_probe_applicable(int64_t nlist, int dim, int64_t nq, int nprobe, int metric);
 // record_stats = false: a helper search inside another call (IVF centroid probe) leaves the fallback counter and kernel timer alone
+// and records only probe_kused
 int bruteforce_topk_tc_device(ThreadCtx &t, const float *ddata, int64_t n, int dim, const float *dq, int64_t nq, int k,
                               int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d, bool record_stats = true, int metric = MO_METRIC_L2SQ);
 bool tc_ivf_applicable(int64_t n, int dim, int64_t nq, int k, int nprobe, int metric, bool refine);
@@ -43,10 +45,18 @@ int ivf_tc_scan(ThreadCtx &t, const IvfPlan &plan, const float *ddata, int64_t n
 bool tc_one_term_wanted(int k, bool record);   // ladder policy shared by brute force and IVF
 void tc_one_term_report(int64_t nq, int64_t failed);
 
-extern thread_local int g_last_tc_fallbacks;   // queries of the last tensor-core search that ended in the exact kernel
-extern thread_local int g_last_tc_refined;     // IVF: queries of the last search that needed the sub-range refine pass
-extern thread_local int g_last_tc_kused;       // K columns the last search's candidate pass multiplied (0: it ran no candidate pass)
-extern thread_local int g_last_tc_pass_k;      // K columns of the last candidate pass launched on this thread (probe passes included)
-extern thread_local int g_last_tc_probe_kused; // K columns of the last IVF search's centroid probe pass (0: exact kernel)
+// the next level of a precision ladder for the queries in `redo` (rows of dq): they are gathered into one sub-batch, next(sub, m, sk, sd)
+// answers it, and its keys and distances are scattered back into their rows of out_k / out_d
+int redo_queries(ThreadCtx &t, const std::vector<int> &redo, const float *dq, int dim, int k, int64_t *out_k, double *out_d,
+                 const std::function<int(const float *sub, int64_t m, int64_t *sk, double *sd)> &next);
+
+// statistics of the last search on this thread (MoB200_SetTuning "get_tc_*"); xcall_bruteforce and xcall_ivf reset them at entry
+struct SearchStats {
+    int kused = 0;        // K columns per (query, row) pair the search's first candidate pass multiplied (0: it ran no candidate pass)
+    int probe_kused = 0;  // IVF: K columns of the last pass of the centroid probe (0: the probe ran on the exact kernel)
+    int refined = -1;     // queries the first tensor-core level could not prove (brute force: only a one-term level records it)
+    int fallbacks = -1;   // queries that ended in the exact kernel (-1: the search did not reach the tensor cores)
+};
+extern thread_local SearchStats g_search_stats;
 
 }  // namespace mob

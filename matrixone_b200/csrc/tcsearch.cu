@@ -179,13 +179,13 @@ tc_candidates_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                      // different times; each publishes an upper bound of the query's k-th real distance and prunes with the best one
                      float *qbound, const int *__restrict__ row_query, const float *__restrict__ alonorm,
                      const float *__restrict__ xmax2, int one_term, int topk, float rel_margin, float abs_margin,
-                     // dynamic unit feed (nullptr: unit u = worker, worker + nworkers, ...): the producer thread takes the next unit from this
-                     // counter when it has issued the last load of the current one, and hands the index to the MMA and epilogue warps through a
-                     // two-slot shared-memory queue.  Units are ordered list-major, so the query tiles of one IVF list start within a few
-                     // microseconds of each other on different SMs and stream the list's B' tiles through L2 together (with a static deal they
-                     // drift apart and every tile of a list re-reads it from HBM), and the tail is balanced.
+                     // dynamic unit feed of single-CTA launches (CTA pairs: unit u = worker, worker + nworkers, ...): the producer thread takes
+                     // the next unit from this counter when it has issued the last load of the current one, and hands the index to the MMA and
+                     // epilogue warps through a two-slot shared-memory queue.  Units are ordered list-major, so the query tiles of one IVF list
+                     // start within a few microseconds of each other on different SMs and stream the list's B' tiles through L2 together (with a
+                     // static deal they drift apart and every tile of a list re-reads it from HBM), and the tail is balanced.
                      int *sched) {
-    const bool dyn = !PAIR && sched != nullptr;
+    constexpr bool dyn = !PAIR;
     extern __shared__ unsigned char smem_raw[];
     // SWIZZLE_128B atoms need 1024-byte alignment in the shared window: align by hand (the launch adds 1024 spare bytes)
     TcSmem &S = *reinterpret_cast<TcSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
@@ -394,10 +394,32 @@ tc_candidates_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
 }
 
 // ---- operand preparation -------------------------------------------------------------------------------------------------
-// mode 0: A' = [hi | hi | lo] (queries), mode 1: B' = [hi | lo | hi] (dataset).  One warp per row; pads K' with zeros.
+// one row of the split, by one warp: element j of the row is elem(j).  mode 0: A' = [hi | hi | lo] (queries), mode 1: B' =
+// [hi | lo | hi] (dataset); K' is padded with zeros.  norm = |v|^2, lonorm = |v - hi|^2 (the part of v a hi-only product does
+// not see), both accumulated in double; an Inf / NaN element raises *nonfinite (the caller falls back to the exact kernel).
+template <class Elem>
+__device__ __forceinline__ void split_row(Elem elem, int lane, int dim, int kprime, int mode, __nv_bfloat16 *__restrict__ o,
+                                          float *__restrict__ norm, float *__restrict__ lonorm, int *__restrict__ nonfinite) {
+    double s = 0.0, sl = 0.0;
+    for (int j = lane; j < dim; j += 32) {
+        const float v = elem(j);
+        const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+        const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
+        o[j] = hi;
+        o[dim + j] = mode == 0 ? hi : lo;
+        o[2 * dim + j] = mode == 0 ? lo : hi;
+        s += (double)v * (double)v;
+        const double l = (double)(v - __bfloat162float(hi));   // exact in fp32
+        sl += l * l;
+        if (!(fabsf(v) <= 3.0e38f)) *nonfinite = 1;
+    }
+    for (int j = 3 * dim + lane; j < kprime; j += 32) o[j] = __float2bfloat16_rn(0.f);
+    s = warp_sum_f64(s); sl = warp_sum_f64(sl);
+    if (lane == 0) { *norm = (float)s; *lonorm = (float)sl; }
+}
+
 __global__ void split_kernel(const float *__restrict__ x, int64_t n, int dim, int kprime, int mode, int normalize, __nv_bfloat16 *__restrict__ out,
                              float *__restrict__ norm, float *__restrict__ lonorm, int *__restrict__ nonfinite) {
-    // norm = |x|^2, lonorm = |x - hi|^2 (the part of x a hi-only product does not see); both accumulated in double.
     // normalize (cosine): the row is first divided by its length, so 1 - cos(q, x) = |q^ - x^|^2 / 2 and the L2 machinery applies;
     // a zero (or non-finite) row raises *nonfinite and the caller answers the whole call with the exact kernel.
     const int lane = threadIdx.x & 31;
@@ -413,22 +435,7 @@ __global__ void split_kernel(const float *__restrict__ x, int64_t n, int dim, in
             len = (float)sqrt(s0);
             if (!(len > 0.f && len <= 3.0e38f)) { if (lane == 0) *nonfinite = 1; len = 1.0f; }
         }
-        double s = 0.0, sl = 0.0;
-        for (int j = lane; j < dim; j += 32) {
-            const float v = normalize ? __fdiv_rn(p[j], len) : p[j];
-            const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-            const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-            o[j] = hi;
-            o[dim + j] = mode == 0 ? hi : lo;
-            o[2 * dim + j] = mode == 0 ? lo : hi;
-            s += (double)v * (double)v;
-            const double l = (double)(v - __bfloat162float(hi));   // exact in fp32
-            sl += l * l;
-            if (!(fabsf(v) <= 3.0e38f)) *nonfinite = 1;   // Inf / NaN: the caller falls back to the exact kernel
-        }
-        for (int j = 3 * dim + lane; j < kprime; j += 32) o[j] = __float2bfloat16_rn(0.f);
-        s = warp_sum_f64(s); sl = warp_sum_f64(sl);
-        if (lane == 0) { norm[r] = (float)s; lonorm[r] = (float)sl; }
+        split_row([&](int j) { return normalize ? __fdiv_rn(p[j], len) : p[j]; }, lane, dim, kprime, mode, o, norm + r, lonorm + r, nonfinite);
     }
 }
 
@@ -454,10 +461,10 @@ __global__ void split_residual_kernel(const float *__restrict__ x, int64_t n, in
         }
         const float *p = x + src * dim, *c = cent + l * dim;
         __nv_bfloat16 *o = out + r * kprime;
-        double s = 0.0, sl = 0.0;
         if (hi_only && (dim & 7) == 0 && (kprime & 7) == 0) {
             // one-term level: the candidate pass multiplies only the first `dim` columns (hi . hi), so only they are written -- a third
             // of the bytes; 8 elements per lane: two 128-bit loads per operand, one 128-bit store
+            double s = 0.0, sl = 0.0;
             for (int j = lane * 8; j < dim; j += 256) {
                 const float4 p0 = *reinterpret_cast<const float4 *>(p + j), p1 = *reinterpret_cast<const float4 *>(p + j + 4);
                 const float4 c0 = *reinterpret_cast<const float4 *>(c + j), c1 = *reinterpret_cast<const float4 *>(c + j + 4);
@@ -480,21 +487,7 @@ __global__ void split_residual_kernel(const float *__restrict__ x, int64_t n, in
             if (lane == 0) { norm[r] = (float)s; lonorm[r] = (float)sl; }
             continue;
         }
-        for (int j = lane; j < dim; j += 32) {
-            const float v = __fsub_rn(p[j], c[j]);
-            const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-            const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-            o[j] = hi;
-            o[dim + j] = mode == 0 ? hi : lo;
-            o[2 * dim + j] = mode == 0 ? lo : hi;
-            s += (double)v * (double)v;
-            const double d = (double)(v - __bfloat162float(hi));
-            sl += d * d;
-            if (!(fabsf(v) <= 3.0e38f)) *nonfinite = 1;
-        }
-        for (int j = 3 * dim + lane; j < kprime; j += 32) o[j] = __float2bfloat16_rn(0.f);
-        s = warp_sum_f64(s); sl = warp_sum_f64(sl);
-        if (lane == 0) { norm[r] = (float)s; lonorm[r] = (float)sl; }
+        split_row([&](int j) { return __fsub_rn(p[j], c[j]); }, lane, dim, kprime, mode, o, norm + r, lonorm + r, nonfinite);
     }
 }
 
@@ -693,7 +686,7 @@ __global__ void tc_max_kernel(const float *__restrict__ v, int64_t n, float *out
 // prove completeness:  every excluded row has approximate distance >= t_excl, |approx - real| <= eps_tc, |real - go| <= eps_go,
 // so d_k + eps_tc + eps_go < t_excl  =>  no excluded row can displace the k-th result.  flag = 1 when the proof fails.
 template <int KRT>
-__global__ void tc_final_kernel(int nq, int k, int64_t n_rows, int dim, int nkb, const int *__restrict__ cand, const float *__restrict__ exact,
+__global__ void tc_final_kernel(int nq, int k, int dim, int nkb, const int *__restrict__ cand, const float *__restrict__ exact,
                                 const float *__restrict__ t_excl, const float *__restrict__ qnorm, const float *__restrict__ xnorm_max,
                                 const float *__restrict__ qlonorm, const float *__restrict__ xlonorm_max, int one_term, int eps_applied, int metric,
                                 const int64_t *__restrict__ id_map, int64_t key_base, int sqrt_out, int64_t *__restrict__ out_k,
@@ -741,39 +734,54 @@ __global__ void tc_fill_kernel(float *thr, int *ids, int64_t nlists, int kp) {
         if (i < nlists) thr[i] = INFINITY;
     }
 }
-__global__ void gather_rows_kernel(const float *__restrict__ src, const int *__restrict__ idx, int m, int dim, float *__restrict__ dst) {
-    for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < (int64_t)m * dim; e += (int64_t)gridDim.x * blockDim.x)
-        dst[e] = src[(int64_t)idx[e / dim] * dim + e % dim];
-}
-__global__ void scatter_results_kernel(const int64_t *__restrict__ sk, const double *__restrict__ sd, const int *__restrict__ idx, int m, int k,
-                                       int64_t *__restrict__ out_k, double *__restrict__ out_d) {
-    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < m * k; e += gridDim.x * blockDim.x) {
-        const int q = idx[e / k];
-        out_k[(size_t)q * k + e % k] = sk[e]; out_d[(size_t)q * k + e % k] = sd[e];
-    }
-}
 
 }  // namespace
 
 namespace mob {
 
-int g_search_mode = 0;          // 0 = auto, 1 = exact kernel only, 2 = force the tensor-core path (MoB200_SetTuning("search_mode"))
-int g_tc_sched_mode = 0;         // 1 = static round-robin deal of the units of single-CTA launches (MoB200_SetTuning("tc_sched"))
-int g_tc_share_mode = 0;         // 1 = no cross-unit threshold sharing (MoB200_SetTuning("tc_share"))
-int g_tc_ladder_mode = 0;        // 0 = auto (one-term level first unless it has been failing), 1 = never, 2 = always (MoB200_SetTuning("tc_ladder"))
-std::atomic<int> g_one_term_skip{0};   // searches left before the one-term level is tried again (shared by all callers: a property of the data)
-thread_local int g_last_tc_pass_k = 0;   // K elements per pair of the last candidate pass this thread launched, timed or not
-thread_local int g_last_tc_probe_kused = 0;   // ... of the centroid probe of the last IVF search (0: the probe ran on the exact kernel)
-thread_local int g_last_tc_kused = 0;   // (per calling thread, like the kernel timer) K elements per (query, row) pair the timed candidate pass multiplied (dim = one term, 3*dim = three)
-int g_tc_range_mb = 0;         // L2 budget of one row range of the brute-force candidate pass, MB (0 = ignore the L2)
-int g_tc_pair_mode = 0;          // 0 = auto, 1 = single-CTA units only, 2 = CTA pairs wherever the brute-force path runs (MoB200_SetTuning("tc_pair"))
-thread_local int g_last_tc_refined = -1;
-thread_local int g_last_tc_fallbacks = -1;   // queries of the last tensor-core search that failed the completeness proof and were re-run exactly
+// knobs (MoB200_SetTuning): they reach paths that production selects from the input
+static int g_search_mode = 0;        // 0 = auto, 1 = exact kernel only, 2 = force the tensor-core path
+static int g_tc_pair_mode = 0;       // 0 = auto, 1 = single-CTA units only, 2 = CTA pairs wherever the brute-force path runs
+static int g_tc_ladder_mode = 0;     // 0 = auto (one-term level first unless it has been failing), 1 = never, 2 = always
+static int g_tc_share_mode = 0;      // 1 = no cross-unit threshold sharing
+static int g_tc_range_mb = 0;        // L2 budget of one row range of the brute-force candidate pass, MB (0 = ignore the L2)
+static std::atomic<int> g_one_term_skip{0};   // searches left before the one-term level is tried again (shared by all callers: a property of the data)
+thread_local SearchStats g_search_stats;
+
+bool search_tuning(const char *name, int value, int *out) {
+    static const struct { const char *name; int *knob; } knobs[] = {
+        {"search_mode", &g_search_mode}, {"tc_pair", &g_tc_pair_mode}, {"tc_ladder", &g_tc_ladder_mode}, {"tc_share", &g_tc_share_mode}, {"tc_range_mb", &g_tc_range_mb}};
+    for (const auto &k : knobs)
+        if (!strcmp(name, k.name)) {
+            *k.knob = value;
+            if (k.knob == &g_tc_ladder_mode) g_one_term_skip.store(0);
+            *out = 0;
+            return true;
+        }
+    const SearchStats &s = g_search_stats;
+    const struct { const char *name; int value; } stats[] = {
+        {"get_tc_kused", s.kused}, {"get_tc_probe_kused", s.probe_kused}, {"get_tc_refined", s.refined}, {"get_tc_fallbacks", s.fallbacks}};
+    for (const auto &st : stats)
+        if (!strcmp(name, st.name)) { *out = st.value; return true; }
+    return false;
+}
 
 struct TcOperand { __nv_bfloat16 *bf = nullptr; float *norm = nullptr; float *lonorm = nullptr; const float *enorm = nullptr; int kprime = 0; };   // enorm: what the epilogue adds (null = norm; zeros for inner product)   // norm = |x|^2, lonorm = |x - bf16(x)|^2 per row
 
+static int tc_kprime(int dim) { return ((3 * dim + BK - 1) / BK) * BK; }   // K' = 3 dim in whole k-blocks
+
+// an operand of `rows` rows in the call's arena
+static int tc_alloc(ThreadCtx &t, int64_t rows, int dim, TcOperand &op) {
+    const size_t r = (size_t)(rows > 0 ? rows : 1);
+    op.kprime = tc_kprime(dim);
+    op.bf = (__nv_bfloat16 *)arena_alloc(t, r * op.kprime * 2 + 1024);
+    op.norm = (float *)arena_alloc(t, r * 4);
+    op.lonorm = (float *)arena_alloc(t, r * 4);
+    return op.bf && op.norm && op.lonorm ? MO_RC_SUCCESS : MO_RC_INTERNAL_ERROR;
+}
+
 // datasets split once by MoB200_SearchPrepare (index load); looked up by (pointer, rows, dim)
-struct PreparedOperand { const float *x; int64_t n; int dim; int device; TcOperand op; const float *cent = nullptr; int64_t nlist = 0; int normalized = 0; const int64_t *offsets = nullptr; };   // cent != nullptr: IVF residual operand; normalized: cosine
+struct PreparedOperand { const float *x; int64_t n; int dim; TcOperand op; const float *cent = nullptr; int64_t nlist = 0; int normalized = 0; const int64_t *offsets = nullptr; };   // cent != nullptr: IVF residual operand; normalized: cosine
 static std::mutex g_prepared_mu;
 static std::vector<PreparedOperand> g_prepared;
 // A search holds this shared for its whole call (the kernels it launched have finished when it returns); whoever frees or rebuilds a
@@ -783,48 +791,52 @@ static std::shared_mutex g_search_rw;
 SearchReadGuard::SearchReadGuard() { g_search_rw.lock_shared(); }
 SearchReadGuard::~SearchReadGuard() { g_search_rw.unlock_shared(); }
 
-// split an fp32 row-major matrix into the K-concatenated bf16 operand; *nonfinite (device flag) is raised on Inf/NaN
-static int tc_prepare(ThreadCtx &t, const float *x, int64_t n, int dim, int mode, int *dnonfinite, TcOperand &op, int normalize = 0) {
-    // one API call may split the same matrix more than once (IVF refine pass): the operand lives in the call's arena, so it
-    // is reused while the arena epoch lasts.  A nonfinite input was already reported by the split that filled the cache.
-    struct Cached { const float *x = nullptr; int64_t n = 0; int dim = 0, mode = 0, normalize = 0; uint64_t epoch = ~0ull; const ThreadCtx *t = nullptr; TcOperand op; };
-    static thread_local Cached cache[2];
-    Cached &c = cache[mode & 1];
-    if (mode == 1) {
-        std::lock_guard<std::mutex> lk(g_prepared_mu);
-        for (const PreparedOperand &e : g_prepared) if (e.x == x && e.n == n && e.dim == dim && !e.cent && e.normalized == normalize) { op = e.op; return MO_RC_SUCCESS; }
-    }
-    if (c.t == &t && c.epoch == t.arena_epoch && c.x == x && c.n == n && c.dim == dim && c.mode == mode && c.normalize == normalize) { op = c.op; return MO_RC_SUCCESS; }
-    op.kprime = ((3 * dim + BK - 1) / BK) * BK;
-    op.bf = (__nv_bfloat16 *)arena_alloc(t, (size_t)(n > 0 ? n : 1) * op.kprime * 2 + 1024);
-    op.norm = (float *)arena_alloc(t, (size_t)(n > 0 ? n : 1) * 4);
-    op.lonorm = (float *)arena_alloc(t, (size_t)(n > 0 ? n : 1) * 4);
-    if (!op.bf || !op.norm || !op.lonorm) return MO_RC_INTERNAL_ERROR;
-    if (n > 0) { split_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(x, n, dim, op.kprime, mode, normalize, op.bf, op.norm, op.lonorm, dnonfinite); MOB_LAUNCH_CHECK(); }
-    c.x = x; c.n = n; c.dim = dim; c.mode = mode; c.normalize = normalize; c.epoch = t.arena_epoch; c.t = &t; c.op = op;
-    return MO_RC_SUCCESS;
-}
+static void free_prepared(const TcOperand &op) { cudaFree(op.bf); cudaFree(op.norm); }   // lonorm shares norm's allocation
 
-// IVF entries as residual operand (see split_residual_kernel); prepared at index load or once per call
-static int tc_prepare_ivf_entries(ThreadCtx &t, const float *x, int64_t n, int dim, const float *dcent, int64_t nlist, const int64_t *doffsets,
-                                  int *dnonfinite, TcOperand &op) {
+// frees and forgets every prepared operand for which pred holds.  The pre-check takes only the list mutex: most calls (scratch
+// uploads, generators) touch no prepared dataset and must not wait for running searches.
+template <class Pred>
+static void drop_prepared(Pred pred) {
     {
         std::lock_guard<std::mutex> lk(g_prepared_mu);
-        for (const PreparedOperand &e : g_prepared) if (e.x == x && e.n == n && e.dim == dim && e.cent == dcent && e.nlist == nlist && e.offsets == doffsets) { op = e.op; return MO_RC_SUCCESS; }
+        if (std::none_of(g_prepared.begin(), g_prepared.end(), pred)) return;
     }
-    struct Cached { const float *x = nullptr, *c = nullptr; int64_t n = 0; int dim = 0; uint64_t epoch = ~0ull; const ThreadCtx *t = nullptr; TcOperand op; };
-    static thread_local Cached c;
-    if (c.t == &t && c.epoch == t.arena_epoch && c.x == x && c.c == dcent && c.n == n && c.dim == dim) { op = c.op; return MO_RC_SUCCESS; }
-    op.kprime = ((3 * dim + BK - 1) / BK) * BK;
-    op.bf = (__nv_bfloat16 *)arena_alloc(t, (size_t)(n > 0 ? n : 1) * op.kprime * 2 + 1024);
-    op.norm = (float *)arena_alloc(t, (size_t)(n > 0 ? n : 1) * 4);
-    op.lonorm = (float *)arena_alloc(t, (size_t)(n > 0 ? n : 1) * 4);
-    if (!op.bf || !op.norm || !op.lonorm) return MO_RC_INTERNAL_ERROR;
+    std::unique_lock<std::shared_mutex> wr(g_search_rw);   // wait for running searches to finish before freeing their operand
+    std::lock_guard<std::mutex> lk(g_prepared_mu);
+    for (size_t i = 0; i < g_prepared.size();) {
+        if (pred(g_prepared[i])) { free_prepared(g_prepared[i].op); g_prepared.erase(g_prepared.begin() + (long)i); }
+        else i++;
+    }
+}
+
+// the operand of x prepared at index load: brute force (cent == nullptr) with normalisation `normalized`, or IVF residuals against
+// (cent, nlist, offsets)
+static bool find_prepared(const float *x, int64_t n, int dim, const float *cent, int64_t nlist, const int64_t *offsets, int normalized, TcOperand &op) {
+    std::lock_guard<std::mutex> lk(g_prepared_mu);
+    for (const PreparedOperand &e : g_prepared)
+        if (e.x == x && e.n == n && e.dim == dim && e.cent == cent && e.nlist == nlist && e.offsets == offsets && e.normalized == normalized) { op = e.op; return true; }
+    return false;
+}
+
+// split an fp32 row-major matrix into the K-concatenated bf16 operand: mode 0 = queries (A'), mode 1 = dataset (B'); cent != nullptr:
+// IVF entries as residuals against their list's centroid (see split_residual_kernel).  *nonfinite (device flag) is raised on Inf/NaN.
+static int tc_prepare(ThreadCtx &t, const float *x, int64_t n, int dim, int mode, int normalize, const float *cent, int64_t nlist,
+                      const int64_t *offsets, int *dnonfinite, TcOperand &op) {
+    if (mode == 1 && find_prepared(x, n, dim, cent, nlist, offsets, normalize, op)) return MO_RC_SUCCESS;
+    // one API call may split the same matrix more than once (the levels of a precision ladder): the operand lives in the call's
+    // arena, so it is reused while the arena epoch lasts.  A nonfinite input was already reported by the split that filled the cache.
+    struct Cached { const float *x = nullptr, *cent = nullptr; int64_t n = 0; int dim = 0, normalize = 0; uint64_t epoch = ~0ull; const ThreadCtx *t = nullptr; TcOperand op; };
+    static thread_local Cached cache[3];   // queries, dataset, IVF entries
+    Cached &c = cache[cent ? 2 : mode];
+    if (c.t == &t && c.epoch == t.arena_epoch && c.x == x && c.cent == cent && c.n == n && c.dim == dim && c.normalize == normalize) { op = c.op; return MO_RC_SUCCESS; }
+    int rc = tc_alloc(t, n, dim, op);
+    if (rc) return rc;
     if (n > 0) {
-        split_residual_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(x, n, dim, op.kprime, 1, dcent, doffsets, nlist, nullptr, nullptr, op.bf, op.norm, op.lonorm, dnonfinite, 0);
+        if (cent) split_residual_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(x, n, dim, op.kprime, 1, cent, offsets, nlist, nullptr, nullptr, op.bf, op.norm, op.lonorm, dnonfinite, 0);
+        else split_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(x, n, dim, op.kprime, mode, normalize, op.bf, op.norm, op.lonorm, dnonfinite);
         MOB_LAUNCH_CHECK();
     }
-    c.x = x; c.c = dcent; c.n = n; c.dim = dim; c.epoch = t.arena_epoch; c.t = &t; c.op = op;
+    c = Cached{x, cent, n, dim, normalize, t.arena_epoch, &t, op};
     return MO_RC_SUCCESS;
 }
 
@@ -835,10 +847,9 @@ __global__ void tc_fill_inf_kernel(float *p, int64_t n) {
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = INFINITY;
 }
 
+// nkb = the 64-column k-blocks of K' to multiply; a timed pass records its K in the search statistics
 static int tc_run_units(ThreadCtx &t, const TcOperand &A, int64_t a_rows, const TcOperand &B, int64_t b_rows, const std::vector<TcUnit> &units,
-                        int64_t nlists, float **part_d, int **part_i, float **part_thr, bool timed = true, bool pair = false, int nkb = 0, int kp = KP,
-                        const TcShare *share = nullptr) {
-    if (nkb <= 0 || nkb > A.kprime / BK) nkb = A.kprime / BK;   // 0 = the whole K' (three-term product)
+                        int64_t nlists, float **part_d, int **part_i, float **part_thr, bool timed, bool pair, int nkb, int kp, const TcShare *share) {
     CUtensorMap map_a, map_b;
     int rc = make_map(&map_a, A.bf, (uint64_t)a_rows, (uint64_t)A.kprime, BM);
     if (rc) return rc;
@@ -852,15 +863,14 @@ static int tc_run_units(ThreadCtx &t, const TcOperand &A, int64_t a_rows, const 
     tc_fill_kernel<<<num_sms() * 4, 256, 0, t.stream>>>(*part_thr, *part_i, nlists, kp);
     MOB_LAUNCH_CHECK();
     if (units.empty()) return MO_RC_SUCCESS;
-    g_last_tc_pass_k = nkb * BK;
     MOB_CUDA_TRY(cudaMemcpyAsync(dunits, units.data(), sizeof(TcUnit) * units.size(), cudaMemcpyHostToDevice, t.stream));
     MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
     static bool attr = false;
-    const size_t smem1 = sizeof(TcSmem) + 1024, smem2 = smem1;
+    const size_t smem = sizeof(TcSmem) + 1024;
     if (!attr) {
-        MOB_CUDA_TRY(cudaFuncSetAttribute(tc_candidates_kernel<false, KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
-        MOB_CUDA_TRY(cudaFuncSetAttribute(tc_candidates_kernel<false, KP_LONG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
-        MOB_CUDA_TRY(cudaFuncSetAttribute(tc_candidates_kernel<true, KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+        MOB_CUDA_TRY(cudaFuncSetAttribute(tc_candidates_kernel<false, KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        MOB_CUDA_TRY(cudaFuncSetAttribute(tc_candidates_kernel<false, KP_LONG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        MOB_CUDA_TRY(cudaFuncSetAttribute(tc_candidates_kernel<true, KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = true;
     }
     const int nunits = (int)units.size();
@@ -876,30 +886,30 @@ static int tc_run_units(ThreadCtx &t, const TcOperand &A, int64_t a_rows, const 
         }
         row_query = share->row_query; xmax2 = share->xmax2; sh_one = share->one_term; sh_k = share->topk; sh_rel = share->rel_margin; sh_abs = share->abs_margin;
     }
-    int *sched = nullptr;
-    if (!pair && g_tc_sched_mode == 0) {
+    int *sched = nullptr;   // the unit counter of single-CTA launches
+    if (!pair) {
         sched = (int *)arena_alloc(t, 4);
         if (!sched) return MO_RC_INTERNAL_ERROR;
         MOB_CUDA_TRY(cudaMemsetAsync(sched, 0, 4, t.stream));
     }
-    if (timed) { t.kev_prio = 2; g_last_tc_kused = nkb * BK; cudaEventRecord(t.kev0, t.stream); }   // MoB200_LastKernelMs reports the first (whole-list) pass, not the refine pass
+    if (timed) { t.kev_prio = 2; g_search_stats.kused = nkb * BK; cudaEventRecord(t.kev0, t.stream); }   // MoB200_LastKernelMs reports the first (whole-list) pass, not the refine pass
     if (!pair) {
         int grid = num_sms();
         if (grid > nunits) grid = nunits;
-        if (kp == KP_LONG) tc_candidates_kernel<false, KP_LONG><<<grid, kTcThreads, smem1, t.stream>>>(map_a, map_b, dunits, nunits, nkb, A.enorm ? A.enorm : A.norm, B.enorm ? B.enorm : B.norm, *part_d, *part_i, *part_thr, qbound, row_query, alonorm, xmax2, sh_one, sh_k, sh_rel, sh_abs, sched);
-        else tc_candidates_kernel<false, KP><<<grid, kTcThreads, smem1, t.stream>>>(map_a, map_b, dunits, nunits, nkb, A.enorm ? A.enorm : A.norm, B.enorm ? B.enorm : B.norm, *part_d, *part_i, *part_thr, qbound, row_query, alonorm, xmax2, sh_one, sh_k, sh_rel, sh_abs, sched);
+        if (kp == KP_LONG) tc_candidates_kernel<false, KP_LONG><<<grid, kTcThreads, smem, t.stream>>>(map_a, map_b, dunits, nunits, nkb, A.enorm ? A.enorm : A.norm, B.enorm ? B.enorm : B.norm, *part_d, *part_i, *part_thr, qbound, row_query, alonorm, xmax2, sh_one, sh_k, sh_rel, sh_abs, sched);
+        else tc_candidates_kernel<false, KP><<<grid, kTcThreads, smem, t.stream>>>(map_a, map_b, dunits, nunits, nkb, A.enorm ? A.enorm : A.norm, B.enorm ? B.enorm : B.norm, *part_d, *part_i, *part_thr, qbound, row_query, alonorm, xmax2, sh_one, sh_k, sh_rel, sh_abs, sched);
     } else {
         if (kp != KP) { set_error("tc search: CTA pairs keep %d candidates per list", KP); return MO_RC_INTERNAL_ERROR; }
         // clusters of two CTAs that share the B tile: one persistent pair per two SMs
         int pairs = num_sms() / 2;
         if (pairs > nunits) pairs = nunits;
         cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)(2 * pairs)); cfg.blockDim = dim3(kTcThreads); cfg.dynamicSmemBytes = smem2; cfg.stream = t.stream;
+        cfg.gridDim = dim3((unsigned)(2 * pairs)); cfg.blockDim = dim3(kTcThreads); cfg.dynamicSmemBytes = smem; cfg.stream = t.stream;
         cudaLaunchAttribute at[1];
         at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
-        const float *an = A.enorm ? A.enorm : A.norm, *bn = B.enorm ? B.enorm : B.norm; int kp = nkb;
-        MOB_CUDA_TRY(cudaLaunchKernelEx(&cfg, tc_candidates_kernel<true, KP>, map_a, map_b, (const TcUnit *)dunits, nunits, kp, an, bn, *part_d, *part_i, *part_thr, qbound, row_query, alonorm, xmax2, sh_one, sh_k, sh_rel, sh_abs, (int *)nullptr));
+        const float *an = A.enorm ? A.enorm : A.norm, *bn = B.enorm ? B.enorm : B.norm;
+        MOB_CUDA_TRY(cudaLaunchKernelEx(&cfg, tc_candidates_kernel<true, KP>, map_a, map_b, (const TcUnit *)dunits, nunits, nkb, an, bn, *part_d, *part_i, *part_thr, qbound, row_query, alonorm, xmax2, sh_one, sh_k, sh_rel, sh_abs, (int *)nullptr));
     }
     if (timed) cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
@@ -918,30 +928,24 @@ static int tc_operand_max(ThreadCtx &t, const TcOperand &B, int64_t n, bool with
 }
 
 // merge approximate lists -> exact re-score -> final order + proof; returns the queries whose proof failed
-// nkb = the k-blocks the candidate pass ran (its error bound depends on them)
-static int tc_finish(ThreadCtx &t, const float *ddata, int64_t n, int dim, int nkb, const float *dq, int64_t nq, int k, int R, const int *pos_map,
-                     int pos_cols, long long pos_stride, const float *part_d, const int *part_i, const float *part_thr, const float *qnorm, const float *xnorm,
-                     const int64_t *id_map, int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d, std::vector<int> &redo,
-                     const float *qlonorm = nullptr, const float *xlonorm = nullptr,   // both given: the candidate pass was hi-only (one term)
-                     const float *pair_norm = nullptr, const float *pair_lonorm = nullptr,   // IVF: operand norms per (query, list) pair
-                     int kp = KP, int metric = MO_METRIC_L2SQ, float *xmax2_in = nullptr) {
+// A = the query operand of the candidate pass, one row per query, or per (query, probed list) pair (IVF: pairs, lists found
+// through pos_map); nkb = the k-blocks the pass ran and one_term = it was hi-only (its error bound depends on both);
+// xmax2 = the largest |x|^2 and |x - hi(x)|^2 of the row operand (tc_operand_max)
+static int tc_finish(ThreadCtx &t, const float *ddata, int dim, const float *dq, int64_t nq, int k, int metric, const TcOperand &A, bool pairs,
+                     bool one_term, int nkb, const float *xmax2, int R, const int *pos_map, int pos_cols, long long pos_stride,
+                     const float *part_d, const int *part_i, const float *part_thr, int kp,
+                     const int64_t *id_map, int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d, std::vector<int> &redo) {
     const bool l2 = metric != MO_METRIC_IP && metric != MO_METRIC_COS;
-    const int one_term = xlonorm ? 1 : 0;
     const int kr = (k > KP || one_term) ? KR_WIDE : KR;   // a looser approximation needs more exact re-scores to prove the top k
     int *cand = (int *)arena_alloc(t, sizeof(int) * (size_t)nq * kr);
     float *exact = (float *)arena_alloc(t, sizeof(float) * (size_t)nq * kr);
-    float *t_excl = (float *)arena_alloc(t, sizeof(float) * (size_t)nq + 16);
+    float *t_excl = (float *)arena_alloc(t, sizeof(float) * (size_t)nq);
     int *flags = (int *)arena_alloc(t, sizeof(int) * (size_t)nq);
     if (!cand || !exact || !t_excl || !flags) return MO_RC_INTERNAL_ERROR;
-    float *xmax = xmax2_in ? xmax2_in : t_excl + nq, *xlomax = xmax + 1;
-    if (!xmax2_in) {
-        MOB_CUDA_TRY(cudaMemsetAsync(xmax, 0, 8, t.stream));
-        tc_max_kernel<<<num_sms() * 2, 256, 0, t.stream>>>(xnorm, n, xmax);
-        MOB_LAUNCH_CHECK();
-        if (one_term) { tc_max_kernel<<<num_sms() * 2, 256, 0, t.stream>>>(xlonorm, n, xlomax); MOB_LAUNCH_CHECK(); }
-    }
+    const float *qnorm = pairs ? nullptr : A.norm, *qlonorm = pairs ? nullptr : A.lonorm;
+    const float *pair_norm = pairs ? A.norm : nullptr, *pair_lonorm = pairs ? A.lonorm : nullptr;
     if (R > kMaxMergeLists) { set_error("tc search: %d candidate lists per query exceed the merge limit %d", R, kMaxMergeLists); return MO_RC_INTERNAL_ERROR; }
-    tc_merge_kernel<<<(unsigned)((nq + 3) / 4), 128, 0, t.stream>>>((int)nq, R, part_d, part_i, part_thr, pos_map, pos_cols, pos_stride, pair_norm, pair_lonorm, xmax, one_term, qnorm, qlonorm, l2 ? k : (1 << 30) /* pruning bound is L2-specific */, dim, nkb, kp, kr, cand, t_excl);
+    tc_merge_kernel<<<(unsigned)((nq + 3) / 4), 128, 0, t.stream>>>((int)nq, R, part_d, part_i, part_thr, pos_map, pos_cols, pos_stride, pair_norm, pair_lonorm, xmax2, one_term, qnorm, qlonorm, l2 ? k : (1 << 30) /* pruning bound is L2-specific */, dim, nkb, kp, kr, cand, t_excl);
     MOB_LAUNCH_CHECK();
     {
         const size_t smem = (size_t)(kRescoreThreads / 32) * godist::RingCfg<false>::kStages * godist::RingCfg<false>::kStageBytes;
@@ -959,8 +963,8 @@ static int tc_finish(ThreadCtx &t, const float *ddata, int64_t n, int dim, int n
         else tc_rescore_kernel<MO_METRIC_L2SQ><<<(unsigned)blocks, kRescoreThreads, smem, t.stream>>>(ddata, dq, dim, (int)nq, kr, cand, exact);
         MOB_LAUNCH_CHECK();
     }
-    if (kr == KR) tc_final_kernel<KR><<<(unsigned)((nq + 127) / 128), 128, 0, t.stream>>>((int)nq, k, n, dim, nkb, cand, exact, t_excl, qnorm, xmax, qlonorm, xlomax, one_term, pair_norm ? 1 : 0, metric, id_map, key_base, sqrt_out, out_k, out_d, flags);
-    else tc_final_kernel<KR_WIDE><<<(unsigned)((nq + 127) / 128), 128, 0, t.stream>>>((int)nq, k, n, dim, nkb, cand, exact, t_excl, qnorm, xmax, qlonorm, xlomax, one_term, pair_norm ? 1 : 0, metric, id_map, key_base, sqrt_out, out_k, out_d, flags);
+    if (kr == KR) tc_final_kernel<KR><<<(unsigned)((nq + 127) / 128), 128, 0, t.stream>>>((int)nq, k, dim, nkb, cand, exact, t_excl, qnorm, xmax2, qlonorm, xmax2 + 1, one_term, pairs, metric, id_map, key_base, sqrt_out, out_k, out_d, flags);
+    else tc_final_kernel<KR_WIDE><<<(unsigned)((nq + 127) / 128), 128, 0, t.stream>>>((int)nq, k, dim, nkb, cand, exact, t_excl, qnorm, xmax2, qlonorm, xmax2 + 1, one_term, pairs, metric, id_map, key_base, sqrt_out, out_k, out_d, flags);
     MOB_LAUNCH_CHECK();
     std::vector<int> hflags((size_t)nq);
     MOB_CUDA_TRY(cudaMemcpyAsync(hflags.data(), flags, sizeof(int) * (size_t)nq, cudaMemcpyDeviceToHost, t.stream));
@@ -1034,7 +1038,7 @@ void tc_one_term_report(int64_t nq, int64_t failed);
 static int bf_tc_level(ThreadCtx &t, int level, int metric, const float *ddata, int64_t n, int dim, const float *dq, int64_t nq, int k,
                        int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d, bool record_stats, bool timed) {
     if (level >= 2) {
-        if (record_stats) g_last_tc_fallbacks = (int)nq;
+        if (record_stats) g_search_stats.fallbacks = (int)nq;
         return bruteforce_topk_device(t, ddata, n, dim, dq, nq, k, metric, key_base, sqrt_out, out_k, out_d);
     }
     const int normalize = metric == MO_METRIC_COS ? 1 : 0;
@@ -1042,8 +1046,8 @@ static int bf_tc_level(ThreadCtx &t, int level, int metric, const float *ddata, 
     if (!dnonfinite) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(dnonfinite, 0, 4, t.stream));
     TcOperand A, B;
-    int rc = tc_prepare(t, dq, nq, dim, 0, dnonfinite, A, normalize);
-    if (!rc) rc = tc_prepare(t, ddata, n, dim, 1, dnonfinite, B, normalize);
+    int rc = tc_prepare(t, dq, nq, dim, 0, normalize, nullptr, 0, nullptr, dnonfinite, A);
+    if (!rc) rc = tc_prepare(t, ddata, n, dim, 1, normalize, nullptr, 0, nullptr, dnonfinite, B);
     if (rc) return rc;
     int hnonfinite = 0;
     rc = read_back(t, &hnonfinite, dnonfinite, 4);
@@ -1096,59 +1100,27 @@ static int bf_tc_level(ThreadCtx &t, int level, int metric, const float *ddata, 
                metric == MO_METRIC_COS ? 2.0f * ((float)dim * 4.76837158203125e-7f + 3.814697265625e-6f) : 0.f, xmax2};
     rc = tc_run_units(t, A, nq, B, n, units, (int64_t)R * nq, &part_d, &part_i, &part_thr, timed, pair, nkb, KP, k <= KP ? &sh : nullptr);
     if (rc) return rc;
+    if (!record_stats) g_search_stats.probe_kused = nkb * BK;   // an IVF centroid probe: the K of its last pass
     std::vector<int> redo;
-    rc = tc_finish(t, ddata, n, dim, nkb, dq, nq, k, R, nullptr, 0, 0, part_d, part_i, part_thr, A.norm, B.norm, nullptr, key_base, sqrt_out, out_k, out_d, redo,
-                   one_term ? A.lonorm : nullptr, one_term ? B.lonorm : nullptr, nullptr, nullptr, KP, metric, xmax2);
+    rc = tc_finish(t, ddata, dim, dq, nq, k, metric, A, false, one_term, nkb, xmax2, R, nullptr, 0, 0, part_d, part_i, part_thr, KP,
+                   nullptr, key_base, sqrt_out, out_k, out_d, redo);
     if (rc) return rc;
     if (record_stats && level == 0) {
-        g_last_tc_refined = (int)redo.size();
+        g_search_stats.refined = (int)redo.size();
         tc_one_term_report(nq, (int64_t)redo.size());
     }
-    if (redo.empty()) return MO_RC_SUCCESS;
-    // queries whose completeness could not be proven: next level, results scattered back
-    const int m = (int)redo.size();
-    int *didx = (int *)arena_alloc(t, sizeof(int) * (size_t)m);
-    float *sub = (float *)arena_alloc(t, sizeof(float) * (size_t)m * dim);
-    int64_t *sk = (int64_t *)arena_alloc(t, sizeof(int64_t) * (size_t)m * k);
-    double *sd = (double *)arena_alloc(t, sizeof(double) * (size_t)m * k);
-    if (!didx || !sub || !sk || !sd) return MO_RC_INTERNAL_ERROR;
-    MOB_CUDA_TRY(cudaMemcpyAsync(didx, redo.data(), sizeof(int) * (size_t)m, cudaMemcpyHostToDevice, t.stream));
-    MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
-    gather_rows_kernel<<<num_sms() * 4, 256, 0, t.stream>>>(dq, didx, m, dim, sub);
-    MOB_LAUNCH_CHECK();
-    rc = bf_tc_level(t, level + 1, metric, ddata, n, dim, sub, m, k, key_base, sqrt_out, sk, sd, record_stats, false);
-    if (rc) return rc;
-    scatter_results_kernel<<<(unsigned)((m * k + 255) / 256), 256, 0, t.stream>>>(sk, sd, didx, m, k, out_k, out_d);
-    MOB_LAUNCH_CHECK();
-    return MO_RC_SUCCESS;
+    // queries whose completeness could not be proven: next level
+    return redo_queries(t, redo, dq, dim, k, out_k, out_d, [&](const float *sub, int64_t m, int64_t *sk, double *sd) {
+        return bf_tc_level(t, level + 1, metric, ddata, n, dim, sub, m, k, key_base, sqrt_out, sk, sd, record_stats, false);
+    });
 }
 
 void search_invalidate(const void *p, uint64_t bytes) {
-    {   // cheap pre-check under the list mutex only: most writes (scratch uploads, generators) touch no prepared dataset
-        std::lock_guard<std::mutex> lk0(g_prepared_mu);
-        bool hit = false;
-        const char *lo0 = (const char *)p, *hi0 = lo0 + bytes;
-        for (const PreparedOperand &e : g_prepared) {
-            const char *xl = (const char *)e.x, *xh = xl + (size_t)e.n * e.dim * 4;
-            const char *cl = (const char *)e.cent, *ch = e.cent ? cl + (size_t)e.nlist * e.dim * 4 : cl;
-            const char *ol = (const char *)e.offsets, *oh = e.offsets ? ol + (size_t)(e.nlist + 1) * 8 : ol;   // the residual operand depends on the list boundaries too
-            if ((lo0 < xh && xl < hi0) || (e.cent && lo0 < ch && cl < hi0) || (e.offsets && lo0 < oh && ol < hi0)) hit = true;
-        }
-        if (!hit) return;
-    }
-    std::unique_lock<std::shared_mutex> wr(g_search_rw);   // wait for running searches to finish before freeing their operand
-    std::lock_guard<std::mutex> lk(g_prepared_mu);
     const char *lo = (const char *)p, *hi = lo + bytes;
-    for (size_t i = 0; i < g_prepared.size();) {
-        const PreparedOperand &e = g_prepared[i];
-        const char *xl = (const char *)e.x, *xh = xl + (size_t)e.n * e.dim * 4;
-        const char *cl = (const char *)e.cent, *ch = e.cent ? cl + (size_t)e.nlist * e.dim * 4 : cl;
-        const char *ol = (const char *)e.offsets, *oh = e.offsets ? ol + (size_t)(e.nlist + 1) * 8 : ol;
-        if ((lo < xh && xl < hi) || (e.cent && lo < ch && cl < hi) || (e.offsets && lo < oh && ol < hi)) {
-            cudaFree(e.op.bf); cudaFree(e.op.norm);
-            g_prepared.erase(g_prepared.begin() + (long)i);
-        } else i++;
-    }
+    auto overlaps = [&](const void *b, size_t len) { return b && lo < (const char *)b + len && (const char *)b < hi; };
+    drop_prepared([&](const PreparedOperand &e) {   // the residual operand depends on the centroids and the list boundaries too
+        return overlaps(e.x, (size_t)e.n * e.dim * 4) || overlaps(e.cent, (size_t)e.nlist * e.dim * 4) || overlaps(e.offsets, (size_t)(e.nlist + 1) * 8);
+    });
 }
 
 // the one-term level needs k <= KP (its proof re-scores 64 candidates) and is skipped while it has recently been failing
@@ -1164,7 +1136,7 @@ void tc_one_term_report(int64_t nq, int64_t failed) { if (nq >= 64 && failed * 5
 int bruteforce_topk_tc_device(ThreadCtx &t, const float *ddata, int64_t n, int dim, const float *dq, int64_t nq, int k,
                               int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d, bool record_stats, int metric) {
     const bool ladder = tc_one_term_wanted(k, record_stats);
-    if (record_stats) { g_last_tc_fallbacks = 0; g_last_tc_refined = -1; }
+    if (record_stats) g_search_stats.fallbacks = 0;   // the search reached the tensor cores
     if (metric == MO_METRIC_L2) metric = MO_METRIC_L2SQ;
     return bf_tc_level(t, ladder ? 0 : 1, metric, ddata, n, dim, dq, nq, k, key_base, sqrt_out, out_k, out_d, record_stats, record_stats);
 }
@@ -1194,13 +1166,9 @@ int ivf_tc_scan(ThreadCtx &t, const IvfPlan &plan, const float *ddata, int64_t n
     MOB_CUDA_TRY(cudaMemsetAsync(dnonfinite, 0, 4, t.stream));
     // operands are residuals against the list centroid: entries prepared at index load (or once per call), queries per (query, list) pair
     TcOperand B, A;
-    int rc = tc_prepare_ivf_entries(t, ddata, n, dim, dcent, nlist, doffsets, dnonfinite, B);
+    int rc = tc_prepare(t, ddata, n, dim, 1, 0, dcent, nlist, doffsets, dnonfinite, B);
+    if (!rc) rc = tc_alloc(t, plan.npairs, dim, A);
     if (rc) return rc;
-    A.kprime = B.kprime;
-    A.bf = (__nv_bfloat16 *)arena_alloc(t, (size_t)plan.npairs * A.kprime * 2 + 1024);
-    A.norm = (float *)arena_alloc(t, (size_t)plan.npairs * 4);
-    A.lonorm = (float *)arena_alloc(t, (size_t)plan.npairs * 4);
-    if (!A.bf || !A.norm || !A.lonorm) return MO_RC_INTERNAL_ERROR;
     split_residual_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(dq, plan.nvalid, dim, A.kprime, 0, dcent, nullptr, nlist, plan.bucket_q, plan.bucket_l,
                                                                A.bf, A.norm, A.lonorm, dnonfinite, one_term ? 1 : 0);
     MOB_LAUNCH_CHECK();
@@ -1248,15 +1216,41 @@ int ivf_tc_scan(ThreadCtx &t, const IvfPlan &plan, const float *ddata, int64_t n
     if (rc) return rc;
     // the approximate lists are indexed by bucket position; tc_finish walks them per query through pair_pos; the final keys are
     // the primary keys row_ids[local row]; every probed list's exclusion bound is lowered by the error bound of ITS operand pair
-    rc = tc_finish(t, ddata, n, dim, nkb, dq, nq, k, plan.nprobe * split, plan.pair_pos, plan.nprobe, plan.npairs, part_d, part_i, part_thr, nullptr, B.norm, drowids, 0,
-                   sqrt_out, ok, od, redo, nullptr, one_term ? B.lonorm : nullptr, A.norm, A.lonorm, kp, MO_METRIC_L2SQ, xmax2);
-    return rc;
+    return tc_finish(t, ddata, dim, dq, nq, k, MO_METRIC_L2SQ, A, true, one_term, nkb, xmax2, plan.nprobe * split, plan.pair_pos, plan.nprobe, plan.npairs,
+                     part_d, part_i, part_thr, kp, drowids, 0, sqrt_out, ok, od, redo);
+}
+
+// index load: split e's rows (e.cent != nullptr: IVF residuals) into an operand in device memory of its own and register it.  It
+// replaces only the operand of the same kind (brute force with the same normalisation, or IVF): preparing COS after L2, or IVF after
+// brute force, on one dataset keeps the earlier operand (ADVICE r01).  Rows with Inf/NaN values are left unprepared.
+static int32_t search_prepare(ThreadCtx &t, PreparedOperand e, const char *what) {
+    drop_prepared([&](const PreparedOperand &o) { return o.x == e.x && !o.cent == !e.cent && (e.cent || o.normalized == e.normalized); });
+    e.op.kprime = tc_kprime(e.dim);
+    MOB_CUDA_TRY(cudaMalloc((void **)&e.op.bf, (size_t)e.n * e.op.kprime * 2 + 1024));
+    if (cudaMalloc((void **)&e.op.norm, (size_t)e.n * 8) != cudaSuccess) { free_prepared(e.op); set_error("%s: out of device memory", what); return MO_RC_INTERNAL_ERROR; }
+    e.op.lonorm = e.op.norm + e.n;
+    int *dnonfinite = (int *)arena_alloc(t, 4);
+    int hnonfinite = 1;
+    int rc = dnonfinite ? MO_RC_SUCCESS : MO_RC_INTERNAL_ERROR;
+    if (!rc && cudaMemsetAsync(dnonfinite, 0, 4, t.stream) != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
+    if (!rc) {
+        if (e.cent) split_residual_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(e.x, e.n, e.dim, e.op.kprime, 1, e.cent, e.offsets, e.nlist, nullptr, nullptr,
+                                                                               e.op.bf, e.op.norm, e.op.lonorm, dnonfinite, 0);
+        else split_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(e.x, e.n, e.dim, e.op.kprime, 1, e.normalized, e.op.bf, e.op.norm, e.op.lonorm, dnonfinite);
+        g_launches++;
+        if (cudaGetLastError() != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
+    }
+    if (!rc) rc = read_back(t, &hnonfinite, dnonfinite, 4);
+    arena_reset(t);
+    if (rc || hnonfinite) { free_prepared(e.op); return rc; }
+    std::lock_guard<std::mutex> lk(g_prepared_mu);
+    g_prepared.push_back(e);
+    return MO_RC_SUCCESS;
 }
 
 }  // namespace mob
 
 extern "C" {
-static void release_same_kind(const void *data, bool ivf, int normalized);
 
 // Index load: split a RESIDENT dataset into the tensor-core operand once instead of once per search.  The rows must not change
 // until MoB200_SearchRelease(data).  Datasets the tensor-core path cannot serve (dim < 16, Inf/NaN values) are left unprepared:
@@ -1271,27 +1265,8 @@ int32_t MoB200_SearchPrepareMetric(const void *data, uint64_t n, int64_t dim, in
     if (metric != MO_METRIC_L2 && metric != MO_METRIC_L2SQ && metric != MO_METRIC_IP && metric != MO_METRIC_COS) return MO_RC_SUCCESS;
     if (!data || n == 0 || dim < 16 || n >= (1ull << 31) - BN) return MO_RC_SUCCESS;
     if (!is_device_ptr(data)) { set_error("SearchPrepare: the dataset must be device memory"); return MO_RC_INVALID_ARGUMENT; }
-    release_same_kind(data, false, metric == MO_METRIC_COS ? 1 : 0);
-    PreparedOperand e; e.x = (const float *)data; e.n = (int64_t)n; e.dim = (int)dim; e.device = 0; e.normalized = metric == MO_METRIC_COS ? 1 : 0;
-    e.op.kprime = ((3 * (int)dim + BK - 1) / BK) * BK;
-    MOB_CUDA_TRY(cudaMalloc((void **)&e.op.bf, (size_t)n * e.op.kprime * 2 + 1024));
-    if (cudaMalloc((void **)&e.op.norm, (size_t)n * 8) != cudaSuccess) { cudaFree(e.op.bf); set_error("SearchPrepare: out of device memory"); return MO_RC_INTERNAL_ERROR; }
-    e.op.lonorm = e.op.norm + n;
-    int *dnonfinite = (int *)arena_alloc(t, 4);
-    int hnonfinite = 1;
-    int rc = dnonfinite ? MO_RC_SUCCESS : MO_RC_INTERNAL_ERROR;
-    if (!rc && cudaMemsetAsync(dnonfinite, 0, 4, t.stream) != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
-    if (!rc) {
-        split_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(e.x, e.n, e.dim, e.op.kprime, 1, e.normalized, e.op.bf, e.op.norm, e.op.lonorm, dnonfinite);
-        g_launches++;
-        if (cudaGetLastError() != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
-    }
-    if (!rc) rc = read_back(t, &hnonfinite, dnonfinite, 4);
-    arena_reset(t);
-    if (rc || hnonfinite) { cudaFree(e.op.bf); cudaFree(e.op.norm); return rc; }
-    std::lock_guard<std::mutex> lk(g_prepared_mu);
-    g_prepared.push_back(e);
-    return MO_RC_SUCCESS;
+    PreparedOperand e; e.x = (const float *)data; e.n = (int64_t)n; e.dim = (int)dim; e.normalized = metric == MO_METRIC_COS ? 1 : 0;
+    return search_prepare(t, e, "SearchPrepare");
 }
 
 // Index load for an IVF-flat index: the list-ordered entries [n][dim] are split as RESIDUALS against their list's centroid
@@ -1302,66 +1277,13 @@ int32_t MoB200_SearchPrepareIvf(const void *data, uint64_t n, int64_t dim, const
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     if (!data || n == 0 || dim < 16 || n >= (1ull << 31) - BN || nlist == 0) return MO_RC_SUCCESS;
     if (!is_device_ptr(data) || !is_device_ptr(centroids) || !is_device_ptr(offsets)) { set_error("SearchPrepareIvf: entries, centroids and offsets must be device memory"); return MO_RC_INVALID_ARGUMENT; }
-    release_same_kind(data, true, 0);
-    PreparedOperand e; e.x = (const float *)data; e.n = (int64_t)n; e.dim = (int)dim; e.device = 0; e.cent = (const float *)centroids; e.nlist = (int64_t)nlist; e.offsets = (const int64_t *)offsets;
-    e.op.kprime = ((3 * (int)dim + BK - 1) / BK) * BK;
-    MOB_CUDA_TRY(cudaMalloc((void **)&e.op.bf, (size_t)n * e.op.kprime * 2 + 1024));
-    if (cudaMalloc((void **)&e.op.norm, (size_t)n * 8) != cudaSuccess) { cudaFree(e.op.bf); set_error("SearchPrepareIvf: out of device memory"); return MO_RC_INTERNAL_ERROR; }
-    e.op.lonorm = e.op.norm + n;
-    int *dnonfinite = (int *)arena_alloc(t, 4);
-    int hnonfinite = 1;
-    int rc = dnonfinite ? MO_RC_SUCCESS : MO_RC_INTERNAL_ERROR;
-    if (!rc && cudaMemsetAsync(dnonfinite, 0, 4, t.stream) != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
-    if (!rc) {
-        split_residual_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(e.x, e.n, e.dim, e.op.kprime, 1, e.cent, (const int64_t *)offsets, e.nlist, nullptr, nullptr,
-                                                                   e.op.bf, e.op.norm, e.op.lonorm, dnonfinite, 0);
-        g_launches++;
-        if (cudaGetLastError() != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
-    }
-    if (!rc) rc = read_back(t, &hnonfinite, dnonfinite, 4);
-    arena_reset(t);
-    if (rc || hnonfinite) { cudaFree(e.op.bf); cudaFree(e.op.norm); return rc; }
-    std::lock_guard<std::mutex> lk(g_prepared_mu);
-    g_prepared.push_back(e);
-    return MO_RC_SUCCESS;
+    PreparedOperand e; e.x = (const float *)data; e.n = (int64_t)n; e.dim = (int)dim; e.cent = (const float *)centroids; e.nlist = (int64_t)nlist; e.offsets = (const int64_t *)offsets;
+    return search_prepare(t, e, "SearchPrepareIvf");
 }
 
-// drop only the operand of the same kind (brute force with the same normalisation, or IVF): preparing COS after L2, or IVF after brute force,
-// on one dataset keeps the earlier operand (ADVICE r01)
-static void release_same_kind(const void *data, bool ivf, int normalized) {
-    using namespace mob;
-    {
-        std::lock_guard<std::mutex> lk0(g_prepared_mu);
-        bool hit = false;
-        for (const PreparedOperand &e : g_prepared) if (e.x == data && (e.cent != nullptr) == ivf && (ivf || e.normalized == normalized)) hit = true;
-        if (!hit) return;
-    }
-    std::unique_lock<std::shared_mutex> wr(g_search_rw);
-    std::lock_guard<std::mutex> lk(g_prepared_mu);
-    for (size_t i = 0; i < g_prepared.size();) {
-        const PreparedOperand &e = g_prepared[i];
-        if (e.x == data && (e.cent != nullptr) == ivf && (ivf || e.normalized == normalized)) { cudaFree(e.op.bf); cudaFree(e.op.norm); g_prepared.erase(g_prepared.begin() + (long)i); }
-        else i++;
-    }
-}
-
+// also drops IVF operands built against `data` as their centroid table (residuals would be stale)
 int32_t MoB200_SearchRelease(const void *data) {
-    using namespace mob;
-    {
-        std::lock_guard<std::mutex> lk0(g_prepared_mu);
-        bool hit = false;
-        for (const PreparedOperand &e : g_prepared) if (e.x == data || (e.cent && (const void *)e.cent == data)) hit = true;
-        if (!hit) return MO_RC_SUCCESS;
-    }
-    std::unique_lock<std::shared_mutex> wr(g_search_rw);   // running searches first
-    std::lock_guard<std::mutex> lk(g_prepared_mu);
-    // also drops IVF operands built against `data` as their centroid table (residuals would be stale)
-    for (size_t i = 0; i < g_prepared.size();) {
-        if (g_prepared[i].x == data || (g_prepared[i].cent && (const void *)g_prepared[i].cent == data)) {
-            cudaFree(g_prepared[i].op.bf); cudaFree(g_prepared[i].op.norm);
-            g_prepared.erase(g_prepared.begin() + (long)i);
-        } else i++;
-    }
+    mob::drop_prepared([&](const mob::PreparedOperand &e) { return e.x == data || (e.cent && (const void *)e.cent == data); });
     return MO_RC_SUCCESS;
 }
 

@@ -712,22 +712,9 @@ namespace mob {
 int g_plan_specialise = 1;
 int xcall_plan(mo_xcall_args_t *args, uint64_t len);
 
-extern int g_search_mode;
-extern thread_local int g_last_tc_fallbacks, g_last_tc_refined, g_last_tc_kused, g_last_tc_probe_kused;
-extern int g_tc_pair_mode, g_tc_range_mb, g_tc_ladder_mode, g_tc_share_mode, g_tc_sched_mode;
-extern std::atomic<int> g_one_term_skip;
-
 int tuning_set(const char *name, int value) {
-    if (!strcmp(name, "search_mode")) { g_search_mode = value; return 0; }
-    if (!strcmp(name, "get_tc_fallbacks")) return g_last_tc_fallbacks;
-    if (!strcmp(name, "get_tc_refined")) return g_last_tc_refined;
-    if (!strcmp(name, "tc_pair")) { g_tc_pair_mode = (int)value; return 0; }
-    if (!strcmp(name, "tc_range_mb")) { g_tc_range_mb = (int)value; return 0; }
-    if (!strcmp(name, "tc_ladder")) { g_tc_ladder_mode = (int)value; g_one_term_skip.store(0); return 0; }
-    if (!strcmp(name, "get_tc_kused")) return g_last_tc_kused;
-    if (!strcmp(name, "get_tc_probe_kused")) return g_last_tc_probe_kused;
-    if (!strcmp(name, "tc_share")) { g_tc_share_mode = (int)value; return 0; }
-    if (!strcmp(name, "tc_sched")) { g_tc_sched_mode = (int)value; return 0; }
+    int search_answer;
+    if (search_tuning(name, value, &search_answer)) return search_answer;
     if (!strcmp(name, "q6_variant")) { if (value != 0 && value != 1) return -1; g_q6_variant = value; return 0; }
     if (!strcmp(name, "plan_specialise")) { g_plan_specialise = value; return 0; }
     if (!strcmp(name, "q1_variant")) { if (value != 0 && value != 1) return -1; g_q1_variant = value; return 0; }

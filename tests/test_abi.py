@@ -95,7 +95,8 @@ def _no_device_checks(lib):
 
 def test_set_tuning_accepts_only_known_kernel_variants(lib):
     """q1_variant and q6_variant take 0 (kernel chosen from the input) or 1 (the reference kernel); any other value, and an unknown
-    name, returns -1"""
+    name, returns -1.  The search knobs are accepted; tc_sched (a deleted static deal of the tensor-core units) is unknown."""
+    search_knobs = (b"search_mode", b"tc_pair", b"tc_ladder", b"tc_share", b"tc_range_mb")
     try:
         for name, bad in ((b"q1_variant", (2, 10, -1)), (b"q6_variant", (2, 3))):
             for v in bad:
@@ -103,8 +104,15 @@ def test_set_tuning_accepts_only_known_kernel_variants(lib):
             assert lib.MoB200_SetTuning(name, 1) == 0
             assert lib.MoB200_SetTuning(name, 0) == 0
         assert lib.MoB200_SetTuning(b"q1_debug", 1) == -1
+        assert lib.MoB200_SetTuning(b"tc_sched", 1) == -1
+        assert lib.MoB200_SetTuning(b"tc_sched", 0) == -1
+        for name in search_knobs:
+            assert lib.MoB200_SetTuning(name, 1) == 0, name
+            assert lib.MoB200_SetTuning(name, 0) == 0, name
     finally:
         lib.MoB200_SetTuning(b"q1_variant", 0); lib.MoB200_SetTuning(b"q6_variant", 0)
+        for name in search_knobs:
+            lib.MoB200_SetTuning(name, 0)
 
 
 def test_missing_library_raises_importerror(tmp_path):

@@ -242,6 +242,29 @@ def test_ivf_refine_pass_resolves_crowded_lists(gpu):
     assert fallbacks <= refined
 
 
+def test_search_statistics_describe_only_the_last_search(gpu):
+    """get_tc_* after a brute-force search on the exact kernel describe that search, not the IVF search before it, whose centroid
+    probe and list scan ran on the tensor cores"""
+    nlist, dim, n, nq, k, nprobe = 300, 64, 9_000, 200, 4, 9
+    centers = datagen.vectors_f32(30, 0, nlist, dim) * 4
+    data = datagen.vectors_f32(31, 0, n, dim, centers, 1.0)
+    qs = datagen.vectors_f32(32, 0, nq, dim, centers, 1.0)
+    ivf = ops.IvfflatSearchIndex(data, np.arange(n) % nlist, centers)
+    bf = ops.BruteForceIndex(data[:1000], dim)
+    stats = lambda: tuple(gpu.MoB200_SetTuning(b"get_tc_" + s, 0) for s in (b"kused", b"probe_kused", b"refined", b"fallbacks"))
+    try:
+        gpu.MoB200_SetTuning(b"search_mode", 2)
+        ivf.search(qs, k, nprobe)
+        kused, probe_kused, refined, fallbacks = stats()
+        assert kused > 0 and probe_kused > 0 and refined >= 0 and fallbacks >= 0, stats()
+        gpu.MoB200_SetTuning(b"search_mode", 1)
+        bf.search(qs, k)
+        assert stats() == (0, 0, -1, -1)
+    finally:
+        gpu.MoB200_SetTuning(b"search_mode", 0)
+        ivf.destroy(); bf.destroy()
+
+
 @pytest.mark.gpu
 def test_prepared_operand_is_dropped_when_the_dataset_is_overwritten(gpu):
     """MoB200_SearchPrepare caches the split operand of a resident dataset; a library write into that buffer (Upload) must

@@ -14,7 +14,7 @@ from matrixone_b200.vector import DeviceBuffer, Vector, xcall
 pytestmark = pytest.mark.gpu
 
 L2, IP, COS = capi.METRIC_L2, capi.METRIC_IP, capi.METRIC_COS
-KNOBS = ("tc_pair", "tc_ladder", "tc_sched", "tc_share", "tc_range_mb")
+KNOBS = ("tc_pair", "tc_ladder", "tc_share", "tc_range_mb")
 
 
 def _stat(gpu, name):
@@ -74,19 +74,19 @@ def did_the_work(kused, fallbacks, nq, dim, k, ladder):
 # tc_range_mb=1 at dim 1024 over 40,000 rows makes 79 row ranges (more than 64 merge lists per query)
 GRID = [
     (16, 128, 1, 1, L2, dict(tc_pair=1, tc_ladder=1), True, False, 0),
-    (17, 129, 127, 16, L2, dict(tc_ladder=2, tc_sched=1), False, False, 0),
+    (17, 129, 127, 16, L2, dict(tc_ladder=2), False, False, 0),
     (33, 1023, 128, 16, IP, dict(tc_ladder=2, tc_share=1), True, True, 0),
     (100, 1024, 129, 17, L2, dict(tc_pair=2, tc_ladder=1), True, False, 0),
     (129, 20_001, 255, 32, COS, dict(tc_ladder=1), True, False, 0),
     (1024, 20_001, 256, 16, L2, dict(tc_pair=2, tc_ladder=2), False, False, 0),
-    (1536, 1024, 257, 1, COS, dict(tc_pair=2, tc_ladder=2, tc_sched=1), True, True, 0),
+    (1536, 1024, 257, 1, COS, dict(tc_pair=2, tc_ladder=2), True, True, 0),
     (3072, 1023, 1000, 16, L2, dict(tc_pair=1, tc_ladder=2, tc_share=1), True, False, 0),
     (4096, 20_001, 129, 16, IP, dict(tc_ladder=2), True, False, 0),
     (4096, 1024, 257, 32, L2, dict(tc_pair=2, tc_ladder=1), False, True, 0),
     (1024, 40_000, 257, 10, L2, dict(tc_ladder=2, tc_range_mb=1), True, False, 0),
-    (100, 20_001, 1000, 16, L2, dict(tc_pair=2, tc_ladder=1, tc_sched=1, tc_share=1), True, False, 0),
+    (100, 20_001, 1000, 16, L2, dict(tc_pair=2, tc_ladder=1, tc_share=1), True, False, 0),
     (33, 1024, 256, 32, IP, dict(tc_pair=2, tc_ladder=1), True, False, 0),
-    (17, 20_001, 257, 17, COS, dict(tc_ladder=2, tc_sched=1, tc_share=1), False, False, 1 << 33),
+    (17, 20_001, 257, 17, COS, dict(tc_ladder=2, tc_share=1), False, False, 1 << 33),
     (129, 128, 255, 1, L2, dict(tc_pair=2, tc_ladder=2), True, True, 7),
     (16, 1023, 128, 16, L2, dict(tc_ladder=1), False, False, 1 << 40),
     (1536, 20_001, 127, 16, COS, dict(tc_ladder=2), True, False, 0),
