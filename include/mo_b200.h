@@ -424,6 +424,27 @@ typedef struct mo_search_params_t {
  * [4] params mo_search_params_t (n = nshards, nq, k). */
 #define MO_XCALL_TOPK_MERGE 0x3002
 
+/* Filtered search: the unfiltered entry point run over the ADMITTED rows only, with the original keys.
+ * MO_XCALL_BRUTEFORCE_TOPK_FILTERED_F32: args [0..4] as MO_XCALL_BRUTEFORCE_TOPK_F32, [5] filter: pdata -> mo_search_filter_t.
+ *   The key of a row is key_base + row ordinal.
+ * MO_XCALL_IVF_TOPK_FILTERED_F32: args [0..7] as MO_XCALL_IVF_TOPK_F32, [8] filter: pdata -> mo_search_filter_t.
+ *   The key of a row is row_ids[row] (the primary key); the probes are those of the unfiltered search.
+ * Admission: KEY_BITMAP admits a key whose bit is set (bitmap_test_with_len, cgo/bitmap.h:55-63; a key at or past 64 * nwords, or
+ * negative, is rejected); KEY_BLOOM admits a key for which bloomfilter_test of its 8 little-endian bytes is true (the filter's
+ * current bits, including those added on the device).  Fewer than k admitted rows: front padding (key -1, distance 0); brute force
+ * with k = 1 and no admitted row: key -1, distance MaxFloat32 (brute_force.go:289-331).  An unknown kind, a null filter or a
+ * descriptor shorter than mo_search_filter_t: MO_RC_INVALID_ARGUMENT. */
+#define MO_XCALL_BRUTEFORCE_TOPK_FILTERED_F32 0x3003
+#define MO_XCALL_IVF_TOPK_FILTERED_F32 0x3004
+#define MO_SEARCH_FILTER_KEY_BITMAP 1
+#define MO_SEARCH_FILTER_KEY_BLOOM 2
+typedef struct mo_search_filter_t {
+    int32_t kind;          /* MO_SEARCH_FILTER_KEY_BITMAP | MO_SEARCH_FILTER_KEY_BLOOM */
+    int32_t pad;
+    const void *filter;    /* KEY_BITMAP: uint64_t words (host or device); KEY_BLOOM: bloomfilter_t * of mo_b200_bloom.h */
+    uint64_t nwords;       /* KEY_BITMAP only: length in 64-bit words */
+} mo_search_filter_t;
+
 /* ======================================================================================================
  * PART 3 -- runtime / residency extension
  * ==================================================================================================== */
@@ -463,7 +484,8 @@ uint64_t MoB200_KernelLaunchCount(void);      /* kernels launched by this librar
 int32_t MoB200_LastKernelMs(float *ms);       /* device time of the dominant kernel of the calling thread's last call (CUDA events) */
 int32_t MoB200_LastError(char *buf, uint64_t buflen);  /* thread-local last error text */
 int32_t MoB200_FlushL2(void);                 /* write a >L2-sized scratch buffer (bench hygiene) */
-int32_t MoB200_SetTuning(const char *name, int32_t value);  /* kernel-variant knobs used by tools/tune.py; returns 0 if name and value are known, else -1 */
+int32_t MoB200_SetTuning(const char *name, int32_t value);  /* kernel-variant knobs used by tools/tune.py; returns 0 if name and value are known, else -1
+                                                             * (search_filter_path: 0 auto, 1 masked scan, 2 compacted admitted rows) */
 
 /* synthetic column generators used by bench.py / tests (counter-based, reproducible on the host: see
  * matrixone_b200/datagen.py).  All write DEVICE memory, rows [row0, row0+n). */

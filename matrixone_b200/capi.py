@@ -70,6 +70,9 @@ AGG_STATE_BYTES = 24
 XCALL_BRUTEFORCE_TOPK_F32 = 0x3000
 XCALL_IVF_TOPK_F32 = 0x3001
 XCALL_TOPK_MERGE = 0x3002
+XCALL_BRUTEFORCE_TOPK_FILTERED_F32 = 0x3003
+XCALL_IVF_TOPK_FILTERED_F32 = 0x3004
+SEARCH_FILTER_KEY_BITMAP, SEARCH_FILTER_KEY_BLOOM = 1, 2
 METRIC_L2, METRIC_IP, METRIC_COS, METRIC_L1, METRIC_L2SQ = 0, 1, 2, 3, 4
 
 
@@ -122,6 +125,11 @@ class Q1Params(C.Structure):
 class SearchParams(C.Structure):
     _fields_ = [("n", C.c_int64), ("dim", C.c_int64), ("nq", C.c_int64), ("k", C.c_int32), ("metric", C.c_int32),
                 ("nprobe", C.c_int32), ("sqrt_out", C.c_int32), ("nlist", C.c_int64), ("key_base", C.c_int64)]
+
+
+class SearchFilter(C.Structure):
+    """mo_search_filter_t: which rows a filtered search may return (by key)"""
+    _fields_ = [("kind", C.c_int32), ("pad", C.c_int32), ("filter", C.c_void_p), ("nwords", C.c_uint64)]
 
 
 _vp, _u64, _i32, _i64 = C.c_void_p, C.c_uint64, C.c_int32, C.c_int64

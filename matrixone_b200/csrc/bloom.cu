@@ -18,7 +18,7 @@
 //   Kernel shape: one thread per key; the filter words are random 8-byte reads (L2-resident for filters up to ~100 MB), keys stream coalesced.
 //   Algorithmic bytes per key: elemsz + 1 result byte + k x 32-byte sectors of the filter.
 #include "common.cuh"
-#include "xxh3_128.cuh"
+#include "bloom_internal.cuh"
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -27,8 +27,6 @@
 #include <vector>
 
 using namespace mob;
-
-#include "../../include/mo_b200_bloom.h"
 
 namespace {
 
@@ -65,17 +63,6 @@ uint64_t *mirror_of(ThreadCtx &t, const bloomfilter_t *bf, bool will_write) {
     return m.dbits;
 }
 
-__device__ __forceinline__ xxh3::Hash128 key_hash(const uint8_t *p, size_t len, uint64_t seed) {
-    // bloom_calculate_hash, bloom.c:43-66: narrow integers are widened so that equal values of different widths share their hash
-    switch (len) {
-    case 1: return xxh3::hash_u64((uint64_t)(int64_t)(int8_t)p[0], seed);
-    case 2: return xxh3::hash_u64((uint64_t)(int64_t)(int16_t)((uint16_t)p[0] | ((uint16_t)p[1] << 8)), seed);
-    case 4: return xxh3::hash_u64((uint64_t)(int64_t)(int32_t)xxh3::rd32(p), seed);
-    case 8: return xxh3::hash_u64(xxh3::rd64(p), seed);
-    default: return xxh3::hash_bytes(p, len, seed);
-    }
-}
-
 struct KeySrc {   // where row i's key bytes are
     const uint8_t *keys; uint64_t len; uint64_t elemsz;      // fixed: keys + i * elemsz ; varlena: 24-byte cells (elemsz = stride)
     const uint8_t *area; uint64_t area_len; int varlena;     // varlena: big cells point into area
@@ -109,7 +96,7 @@ bloom_kernel(uint64_t *__restrict__ bits, uint64_t nbits, uint32_t k, uint64_t s
         if (!have) continue;                                                    // rows past the end of the key buffer are not touched (bloom.c loop bounds)
         const bool isnull = nullmap && ((nullmap[i >> 6] >> (i & 63)) & 1ull);
         if (isnull || nbits == 0) { if (MODE == 1) result[i] = 0; continue; }
-        const xxh3::Hash128 h = key_hash(p, n, seed);
+        const xxh3::Hash128 h = bloom_key_hash(p, n, seed);
         if (MODE == 0) {
             for (uint32_t j = 0; j < k; j++) {
                 const uint64_t pos = (h.lo + (uint64_t)j * h.hi) & (nbits - 1);
@@ -117,12 +104,7 @@ bloom_kernel(uint64_t *__restrict__ bits, uint64_t nbits, uint32_t k, uint64_t s
                 if (!(bits[pos >> 6] & bit)) atomicOr((unsigned long long *)&bits[pos >> 6], (unsigned long long)bit);
             }
         } else {
-            bool all = true;   // (issuing all k probes before looking at any was measured: 6 % slower -- the early exit saves more sectors than the overlap gains)
-            for (uint32_t j = 0; j < k && all; j++) {
-                const uint64_t pos = (h.lo + (uint64_t)j * h.hi) & (nbits - 1);
-                all = (__ldg(&bits[pos >> 6]) >> (pos & 63)) & 1ull;
-            }
-            result[i] = all ? 1 : 0;
+            result[i] = bloom_test_hash(bits, nbits, k, h) ? 1 : 0;
         }
     }
 }
@@ -138,7 +120,7 @@ taa_insert_kernel(const uint64_t *__restrict__ bits, uint64_t nbits, uint32_t k,
         const uint8_t *p; uint64_t n;
         if (!key_of(K, i, &p, &n)) continue;
         if (nbits == 0 || (nullmap && ((nullmap[i >> 6] >> (i & 63)) & 1ull))) continue;
-        const xxh3::Hash128 h = key_hash(p, n, seed);
+        const xxh3::Hash128 h = bloom_key_hash(p, n, seed);
         for (uint32_t j = 0; j < k; j++) {
             const uint64_t pos = (h.lo + (uint64_t)j * h.hi) & (nbits - 1);
             // the entry's key carries the position's bit BEFORE the call in its top bit (the filter is not modified by this kernel, so every
@@ -164,7 +146,7 @@ taa_finish_kernel(uint64_t *__restrict__ bits, uint64_t nbits, uint32_t k, uint6
         if (!key_of(K, i, &p, &n)) continue;
         if (nullmap && ((nullmap[i >> 6] >> (i & 63)) & 1ull)) { result[i] = 0; continue; }
         if (nbits == 0) { result[i] = 0; continue; }
-        const xxh3::Hash128 h = key_hash(p, n, seed);
+        const xxh3::Hash128 h = bloom_key_hash(p, n, seed);
         bool all = true;
         for (uint32_t j = 0; j < k; j++) {
             const uint64_t pos = (h.lo + (uint64_t)j * h.hi) & (nbits - 1);
@@ -256,6 +238,8 @@ void run(const char *what, int op, int fmt, const bloomfilter_t *bf, const void 
 }
 
 }  // namespace
+
+uint64_t *mob::bloom_mirror(ThreadCtx &t, const bloomfilter_t *bf, bool will_write) { return mirror_of(t, bf, will_write); }
 
 // ---- the reference's symbols (cgo/bloom.h) -------------------------------------------------------------------------------------------------
 extern "C" {

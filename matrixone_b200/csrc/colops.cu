@@ -44,7 +44,8 @@ __device__ __forceinline__ uint64_t mix64(uint64_t x) {
 constexpr int kSelThreads = 256, kSelRows = 32, kSelTile = kSelThreads * kSelRows;   // 8192 rows per tile = one MatrixOne block
 constexpr unsigned long long kFlagA = 1ull << 62, kFlagP = 2ull << 62, kValMask = (1ull << 62) - 1;
 
-template <typename OutT>
+// BITS: the flags are a bitmap (bit j of 32-bit word w = row 32 w + j, zero past n) instead of one byte per row
+template <typename OutT, bool BITS = false>
 __global__ void __launch_bounds__(kSelThreads)
 select_kernel(const uint8_t *__restrict__ v, const uint64_t *__restrict__ nulls, uint64_t n, OutT *__restrict__ sels,
               unsigned long long *status, unsigned *ticket, unsigned long long *total, int aligned) {
@@ -57,7 +58,9 @@ select_kernel(const uint8_t *__restrict__ v, const uint64_t *__restrict__ nulls,
     const uint64_t ntiles = (n + kSelTile - 1) / kSelTile;
     const uint64_t row0 = (uint64_t)tile * kSelTile + (uint64_t)threadIdx.x * kSelRows;
     unsigned mask = 0;
-    if (row0 + kSelRows <= n && aligned) {
+    if (BITS) {
+        if (row0 < n) mask = reinterpret_cast<const uint32_t *>(v)[row0 >> 5];
+    } else if (row0 + kSelRows <= n && aligned) {
         const int4 x0 = ld_stream16(v + row0), x1 = ld_stream16(v + row0 + 16);
         const unsigned w[8] = {(unsigned)x0.x, (unsigned)x0.y, (unsigned)x0.z, (unsigned)x0.w, (unsigned)x1.x, (unsigned)x1.y, (unsigned)x1.z, (unsigned)x1.w};
 #pragma unroll
@@ -107,7 +110,7 @@ select_kernel(const uint8_t *__restrict__ v, const uint64_t *__restrict__ nulls,
 }
 
 // launches the compaction; *dtotal (device) receives the count.  status/ticket scratch comes from the arena.
-template <typename OutT>
+template <typename OutT, bool BITS = false>
 int launch_select(ThreadCtx &t, const uint8_t *v, const uint64_t *nulls, uint64_t n, OutT *sels, unsigned long long *dtotal) {
     if (n == 0) { MOB_CUDA_TRY(cudaMemsetAsync(dtotal, 0, 8, t.stream)); return MO_RC_SUCCESS; }
     const uint64_t ntiles = (n + kSelTile - 1) / kSelTile;
@@ -115,10 +118,20 @@ int launch_select(ThreadCtx &t, const uint8_t *v, const uint64_t *nulls, uint64_
     if (!status) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(status, 0, ntiles * 8 + 16, t.stream));
     unsigned *ticket = (unsigned *)(status + ntiles);
-    select_kernel<OutT><<<(unsigned)ntiles, kSelThreads, 0, t.stream>>>(v, nulls, n, sels, status, ticket, dtotal, (((uintptr_t)v) & 15) == 0 ? 1 : 0);
+    select_kernel<OutT, BITS><<<(unsigned)ntiles, kSelThreads, 0, t.stream>>>(v, nulls, n, sels, status, ticket, dtotal, (((uintptr_t)v) & 15) == 0 ? 1 : 0);
     MOB_LAUNCH_CHECK();
     return MO_RC_SUCCESS;
 }
+
+}  // namespace
+
+namespace mob {
+int compact_bits(ThreadCtx &t, const uint32_t *bits, uint64_t n, int32_t *sels, unsigned long long *dtotal) {
+    return launch_select<int32_t, true>(t, reinterpret_cast<const uint8_t *>(bits), nullptr, n, sels, dtotal);
+}
+}  // namespace mob
+
+namespace {
 
 // =========================================================================================================
 // gather (Shrink / Union / FixedLengthShuffle) with nulls.Filter fused: dst[i] = src[sels[i]], dst null bit i = src null bit sels[i]

@@ -19,6 +19,7 @@
 // Work per launch: Q*N*dim element-pairs, 3 fp32 ops each (sub, mul, add) => 3*Q*N*dim flop; bytes N*dim*4 + Q*dim*4.
 #include "common.cuh"
 #include "search_internal.cuh"
+#include "bloom_internal.cuh"
 #include <cstring>
 #include <cfloat>
 #include <cmath>
@@ -90,6 +91,7 @@ struct WorkDesc {
     const int64_t *slot_of;                  // local query -> output slot (nullptr: range*nq_total + q)
     int64_t range;
     const float *xnorm, *qnorm;              // COS: squared norms (exact Go order)
+    const uint32_t *admit;                   // nullable: bit r of word r / 32 = row r may be listed (filtered search)
 };
 
 template <int METRIC>
@@ -221,7 +223,7 @@ bf_topk_kernel(const WorkDesc *__restrict__ items, int dim, int k, float *__rest
             for (int b = 0; b < 4; b++) {
                 const int rl = 4 * tx + b;
                 const int64_t row = row0 + rl;
-                if (row >= W.row_end) continue;
+                if (row >= W.row_end || (W.admit && !((W.admit[row >> 5] >> (row & 31)) & 1u))) continue;
                 float d = acc[a][b];
                 if (METRIC == MO_METRIC_IP) d = -d;
                 if (METRIC == MO_METRIC_COS) {     // distance_func.go:264-284
@@ -320,6 +322,44 @@ __global__ void scatter_results_kernel(const int64_t *__restrict__ sk, const dou
     }
 }
 
+// ---- filtered search ---------------------------------------------------------------------------------------------------------
+// admission mask: bit r of 32-bit word r / 32 = row r is admitted; one lane per row, one ballot per word, the admitted rows are
+// counted in the same pass.  The key of row r is row_ids[r] (IVF: the primary key) or key_base + r (brute force).
+//   KEY_BITMAP: bitmap_test_with_len (cgo/bitmap.h:55-63): bit `key` of words[0, nwords) -- a key at or past 64 * nwords (or < 0) is rejected
+//   KEY_BLOOM:  bloomfilter_test of the key's 8 little-endian bytes against the filter's device mirror
+__global__ void filter_admit_kernel(int kind, const uint64_t *__restrict__ words, uint64_t nwords, uint64_t nbits, uint32_t nhash, uint64_t seed,
+                                    int64_t n, int64_t key_base, const int64_t *__restrict__ row_ids, uint32_t *__restrict__ admit,
+                                    unsigned long long *count) {
+    const int lane = threadIdx.x & 31;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r - lane < n; r += stride) {   // r - lane: the warp's first row, uniform
+        bool ok = false;
+        if (r < n) {
+            const int64_t key = row_ids ? row_ids[r] : key_base + r;
+            if (kind == MO_SEARCH_FILTER_KEY_BITMAP) ok = ((uint64_t)key >> 6) < nwords && ((words[(uint64_t)key >> 6] >> (key & 63)) & 1ull);
+            else ok = nbits != 0 && bloom_test_hash(words, nbits, nhash, bloom_key_hash(reinterpret_cast<const uint8_t *>(&key), 8, seed));
+        }
+        const unsigned w = __ballot_sync(0xffffffffu, ok);
+        if (lane == 0) { admit[(r - lane) >> 5] = w; if (w) atomicAdd(count, (unsigned long long)__popc(w)); }
+    }
+}
+// compacted set: local row -> key (brute force; the compaction keeps the row order, so the key order of ties is the local order)
+__global__ void filter_remap_keys_kernel(int64_t *keys, int64_t cnt, const int32_t *__restrict__ idx, int64_t key_base) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < cnt; i += (int64_t)gridDim.x * blockDim.x)
+        if (keys[i] >= 0) keys[i] = key_base + idx[keys[i]];
+}
+__global__ void filter_gather_ids_kernel(const int64_t *__restrict__ src, const int32_t *__restrict__ idx, int64_t m, int64_t *__restrict__ dst) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) dst[i] = src[idx[i]];
+}
+// IVF list boundaries of the compacted entries: list l starts at the number of admitted rows before offsets[l] (idx is ascending)
+__global__ void filter_offsets_kernel(const int64_t *__restrict__ offsets, int64_t nlist, const int32_t *__restrict__ idx, int64_t m, int64_t *__restrict__ out) {
+    for (int64_t l = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; l <= nlist; l += (int64_t)gridDim.x * blockDim.x) {
+        int64_t lo = 0, hi = m;
+        while (lo < hi) { const int64_t mid = (lo + hi) >> 1; if (idx[mid] < offsets[l]) lo = mid + 1; else hi = mid; }
+        out[l] = lo;
+    }
+}
+
 // merge nlists sorted (dist,id) lists of length k per query into the final keys/distances.
 // in_i holds LOCAL ids when id_map/key_base describe the translation, or final int64 keys when in_k is given.
 __global__ void topk_merge_kernel(int64_t nq, int k, int nlists, int64_t list_stride /* in queries */, const float *__restrict__ in_d,
@@ -399,6 +439,62 @@ int read_params(ThreadCtx &t, const mo_xcall_args_t &a, mo_search_params_t *P) {
     return MO_RC_SUCCESS;
 }
 
+int read_filter(ThreadCtx &t, const mo_xcall_args_t &a, mo_search_filter_t *F) {
+    if (!a.pdata || a.dataSz < sizeof(mo_search_filter_t)) { set_error("filtered search: filter descriptor missing or shorter than %zu bytes", sizeof(mo_search_filter_t)); return MO_RC_INVALID_ARGUMENT; }
+    if (is_device_ptr(a.pdata)) { int rc = read_back(t, F, a.pdata, sizeof *F); if (rc) return rc; }
+    else memcpy(F, a.pdata, sizeof *F);
+    if (F->kind != MO_SEARCH_FILTER_KEY_BITMAP && F->kind != MO_SEARCH_FILTER_KEY_BLOOM) { set_error("filtered search: unknown filter kind %d", F->kind); return MO_RC_INVALID_ARGUMENT; }
+    if (!F->filter) { set_error("filtered search: null filter"); return MO_RC_INVALID_ARGUMENT; }
+    if (F->kind == MO_SEARCH_FILTER_KEY_BLOOM) {
+        const bloomfilter_t *bf = (const bloomfilter_t *)F->filter;
+        if (memcmp(bf->magic, "XXBF", 4) != 0 || bf->k > MAX_K_SEED) { set_error("filtered search: not a bloom filter (bad magic or k)"); return MO_RC_INVALID_ARGUMENT; }
+    }
+    return MO_RC_SUCCESS;
+}
+
+// the admission mask of n rows (keys: row_ids[r], or key_base + r without row_ids) in the call's arena, and the admitted count
+int filter_admission(ThreadCtx &t, Stager &st, const mo_search_filter_t &F, int64_t n, int64_t key_base, const int64_t *row_ids,
+                     uint32_t **admit, int64_t *admitted) {
+    const uint64_t *words; uint64_t nwords = 0, nbits = 0, seed = 0; uint32_t nhash = 0;
+    if (F.kind == MO_SEARCH_FILTER_KEY_BITMAP) {
+        nwords = F.nwords;
+        words = nwords ? (const uint64_t *)st.in(F.filter, (size_t)nwords * 8) : nullptr;   // no words: every key is rejected
+    } else {   // the filter's own device mirror: bits added on the device are seen
+        const bloomfilter_t *bf = (const bloomfilter_t *)F.filter;
+        words = bloom_mirror(t, bf, false);
+        if (!words) return MO_RC_INTERNAL_ERROR;
+        nbits = bf->nbits; nhash = bf->k; seed = bf->seed;
+    }
+    *admit = (uint32_t *)arena_alloc(t, (size_t)((n + 31) / 32 + 1) * 4);
+    unsigned long long *dcount = (unsigned long long *)arena_alloc(t, 8);
+    if (st.failed || !*admit || !dcount) return MO_RC_INTERNAL_ERROR;
+    MOB_CUDA_TRY(cudaMemsetAsync(dcount, 0, 8, t.stream));
+    if (n > 0) {
+        int64_t grid = (n + 255) / 256;
+        if (grid > num_sms() * 8ll) grid = num_sms() * 8ll;
+        filter_admit_kernel<<<(unsigned)grid, 256, 0, t.stream>>>(F.kind, words, nwords, nbits, nhash, seed, n, key_base, row_ids, *admit, dcount);
+        MOB_LAUNCH_CHECK();
+    }
+    unsigned long long h = 0;
+    int rc = read_back(t, &h, dcount, 8);
+    *admitted = (int64_t)h;
+    g_search_stats.filter_admitted = (int)h;
+    return rc;
+}
+
+// the admitted rows of ddata, in order: *idx = their row numbers, *sub = the rows
+int filter_gather(ThreadCtx &t, const float *ddata, int64_t n, int dim, const uint32_t *admit, int64_t m, int32_t **idx, float **sub) {
+    *idx = (int32_t *)arena_alloc(t, (size_t)(m > 0 ? m : 1) * 4);
+    *sub = (float *)arena_alloc(t, (size_t)(m > 0 ? m : 1) * dim * 4);
+    unsigned long long *dtotal = (unsigned long long *)arena_alloc(t, 8);
+    if (!*idx || !*sub || !dtotal) return MO_RC_INTERNAL_ERROR;
+    int rc = compact_bits(t, admit, (uint64_t)n, *idx, dtotal);
+    if (rc) return rc;
+    if (m > 0) { gather_rows_kernel<<<num_sms() * 8, 256, 0, t.stream>>>(ddata, *idx, (int)m, dim, *sub); MOB_LAUNCH_CHECK(); }
+    g_search_stats.filter_compacted = 1;
+    return MO_RC_SUCCESS;
+}
+
 }  // namespace
 
 namespace mob {
@@ -406,7 +502,7 @@ namespace mob {
 // Core: brute-force top-k of nq queries against rows [0,n) of ddata, results (keys + key_base, float64 distances) to
 // device buffers out_k/out_d (nq*k).  All pointers are device pointers.
 int bruteforce_topk_device(ThreadCtx &t, const float *ddata, int64_t n, int dim, const float *dq, int64_t nq, int k, int metric,
-                           int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d) {
+                           int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d, const uint32_t *admit) {
     if (k <= 0 || nq <= 0) return MO_RC_SUCCESS;
     if (k > KMAX) { set_error("search: k=%d exceeds the fused kernel limit %d", k, KMAX); return MO_RC_INVALID_ARGUMENT; }
     if (n >= (1ll << 31)) { set_error("search: more than 2^31 rows per shard"); return MO_RC_INVALID_ARGUMENT; }
@@ -431,7 +527,7 @@ int bruteforce_topk_device(ThreadCtx &t, const float *ddata, int64_t n, int dim,
             if (w.row_begin > n) w.row_begin = n;
             w.queries = dq; w.nq_total = nq; w.qidx = nullptr; w.q0 = (int64_t)qt * TQ;
             w.nq_local = (int)(nq - w.q0 < TQ ? nq - w.q0 : TQ);
-            w.slot_of = nullptr; w.range = r; w.xnorm = xnorm; w.qnorm = qnorm;
+            w.slot_of = nullptr; w.range = r; w.xnorm = xnorm; w.qnorm = qnorm; w.admit = admit;
         }
     WorkDesc *ditems = (WorkDesc *)arena_alloc(t, sizeof(WorkDesc) * (size_t)nitems);
     float *part_d = (float *)arena_alloc(t, sizeof(float) * (size_t)(R * nq * k));
@@ -446,7 +542,16 @@ int bruteforce_topk_device(ThreadCtx &t, const float *ddata, int64_t n, int dim,
     return MO_RC_SUCCESS;
 }
 
-int xcall_bruteforce(mo_xcall_args_t *args, uint64_t len) {
+// the tensor-core path where it applies, else the exact kernel; admit (nullable) restricts the rows that may be listed
+static int bruteforce_search(ThreadCtx &t, const mo_search_params_t &P, const float *ddata, int64_t n, const float *dq, int64_t key_base,
+                             int64_t *ok, double *od, const uint32_t *admit) {
+    if (tc_search_applicable(n, (int)P.dim, P.nq, P.k, P.metric))
+        return bruteforce_topk_tc_device(t, ddata, n, (int)P.dim, dq, P.nq, P.k, key_base, P.sqrt_out, ok, od, true, (int)P.metric, admit);
+    return bruteforce_topk_device(t, ddata, n, (int)P.dim, dq, P.nq, P.k, P.metric, key_base, P.sqrt_out, ok, od, admit);
+}
+
+// MO_XCALL_BRUTEFORCE_TOPK_F32 (farg == nullptr) and MO_XCALL_BRUTEFORCE_TOPK_FILTERED_F32 (farg = the filter descriptor)
+static int bruteforce_call(mo_xcall_args_t *args, uint64_t len, const mo_xcall_args_t *farg) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     SearchReadGuard guard;   // prepared operands stay alive until this call returns
@@ -459,6 +564,8 @@ int xcall_bruteforce(mo_xcall_args_t *args, uint64_t len) {
         args[0].dataSz < (uint64_t)P.nq * P.k * 8 || args[1].dataSz < (uint64_t)P.nq * P.k * 8) {
         set_error("search: buffer sizes do not match params"); return MO_RC_INVALID_ARGUMENT;
     }
+    mo_search_filter_t F;
+    if (farg && (rc = read_filter(t, *farg, &F)) != 0) return rc;
     Stager st(t);
     const float *ddata = (const float *)st.in(args[2].pdata, (size_t)P.n * P.dim * 4);
     const float *dq = (const float *)st.in(args[3].pdata, (size_t)P.nq * P.dim * 4);
@@ -466,13 +573,32 @@ int xcall_bruteforce(mo_xcall_args_t *args, uint64_t len) {
     double *od = (double *)st.out(args[1].pdata, (size_t)P.nq * P.k * 8);
     if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
     g_search_stats = SearchStats();   // the statistics describe this search, also when it does not reach the tensor cores
-    if (tc_search_applicable(P.n, (int)P.dim, P.nq, P.k, P.metric))
-        rc = bruteforce_topk_tc_device(t, ddata, P.n, (int)P.dim, dq, P.nq, P.k, P.key_base, P.sqrt_out, ok, od, true, (int)P.metric);
-    else
-        rc = bruteforce_topk_device(t, ddata, P.n, (int)P.dim, dq, P.nq, P.k, P.metric, P.key_base, P.sqrt_out, ok, od);
+    if (!farg) {
+        rc = bruteforce_search(t, P, ddata, P.n, dq, P.key_base, ok, od, nullptr);
+    } else {
+        uint32_t *admit; int64_t m = 0;
+        rc = filter_admission(t, st, F, P.n, P.key_base, nullptr, &admit, &m);
+        if (!rc && filter_compact_wanted(P.n, m, false)) {
+            // few admitted rows: search the gathered rows (local ids 0..m-1), then local id -> key
+            int32_t *idx; float *sub;
+            rc = filter_gather(t, ddata, P.n, (int)P.dim, admit, m, &idx, &sub);
+            if (!rc) rc = bruteforce_search(t, P, sub, m, dq, 0, ok, od, nullptr);
+            if (!rc) {
+                filter_remap_keys_kernel<<<num_sms() * 4, 256, 0, t.stream>>>(ok, P.nq * P.k, idx, P.key_base);
+                if (cudaGetLastError() != cudaSuccess) { set_error("filtered search: key remap launch failed"); rc = MO_RC_INTERNAL_ERROR; }
+                g_launches++;
+            }
+        } else if (!rc) {
+            g_search_stats.filter_compacted = 0;
+            rc = bruteforce_search(t, P, ddata, P.n, dq, P.key_base, ok, od, admit);
+        }
+    }
     int frc = st.finish();
     return rc ? rc : frc;
 }
+
+int xcall_bruteforce(mo_xcall_args_t *args, uint64_t len) { return bruteforce_call(args, len, nullptr); }
+int xcall_bruteforce_filtered(mo_xcall_args_t *args, uint64_t len) { return bruteforce_call(args, len, &args[5]); }
 
 // merge of per-shard lists: in keys/dists are [nshards][nq][k] (final keys, f64 distances, -1 = missing)
 int xcall_topk_merge(mo_xcall_args_t *args, uint64_t len) {
@@ -560,6 +686,7 @@ struct IvfJob {
     const float *dcent; int64_t nlist; const float *ddata; int64_t n; int dim; const std::vector<int64_t> *offsets; const int64_t *doffsets;
     const int64_t *drowids;
     int k, nprobe, metric, sqrt_out;
+    const uint32_t *admit;   // filtered search, masked scan: admitted list-ordered rows (nullptr: all)
 };
 
 // level 0: tensor-core candidate pass over whole lists (one-term product when the ladder allows it, else three-term), level 1: the
@@ -572,12 +699,12 @@ static int ivf_search_level(ThreadCtx &t, const IvfJob &J, int level, const floa
     if (rc) return rc;
     if (level >= 2 || !tc_ivf_applicable(J.n, J.dim, nq, J.k, J.nprobe, J.metric, level == 1)) {
         if (level > 0) g_search_stats.fallbacks = (int)nq;
-        return ivf_exact_scan(t, plan, J.ddata, J.n, J.dim, dq, nq, *J.offsets, J.drowids, J.k, J.metric, J.sqrt_out, ok, od);
+        return ivf_exact_scan(t, plan, J.ddata, J.n, J.dim, dq, nq, *J.offsets, J.drowids, J.k, J.metric, J.sqrt_out, ok, od, J.admit);
     }
     std::vector<int> redo;
     bool nonfinite = false;
     const int pass = level == 1 ? 2 : (tc_one_term_wanted(J.k, true) ? 0 : 1);
-    rc = ivf_tc_scan(t, plan, J.ddata, J.n, J.dim, dq, nq, J.dcent, J.doffsets, *J.offsets, J.drowids, J.k, J.sqrt_out, pass, ok, od, redo, &nonfinite);
+    rc = ivf_tc_scan(t, plan, J.ddata, J.n, J.dim, dq, nq, J.dcent, J.doffsets, *J.offsets, J.drowids, J.k, J.sqrt_out, pass, ok, od, redo, &nonfinite, J.admit);
     if (!rc && pass == 0 && !nonfinite) tc_one_term_report(nq, (int64_t)redo.size());
     if (rc) return rc;
     if (level == 0) { g_search_stats.refined = (int)redo.size(); g_search_stats.fallbacks = 0; }
@@ -590,7 +717,7 @@ static int ivf_search_level(ThreadCtx &t, const IvfJob &J, int level, const floa
 //   findCentroids (:292-311)  = exact top-nprobe over the centroid table (same kernel, k = nprobe)
 //   list scan + ORDER BY LIMIT (:572-592) = exact top-k over the rows of the probed lists
 // args: see MO_XCALL_IVF_TOPK_F32 in include/mo_b200.h.
-int xcall_ivf(mo_xcall_args_t *args, uint64_t len) {
+static int ivf_call(mo_xcall_args_t *args, uint64_t len, const mo_xcall_args_t *farg) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     SearchReadGuard guard;
@@ -609,6 +736,8 @@ int xcall_ivf(mo_xcall_args_t *args, uint64_t len) {
         args[0].dataSz < (uint64_t)P.nq * P.k * 8 || args[1].dataSz < (uint64_t)P.nq * P.k * 8) {
         set_error("ivf: buffer sizes do not match params"); return MO_RC_INVALID_ARGUMENT;
     }
+    mo_search_filter_t F;
+    if (farg && (rc = read_filter(t, *farg, &F)) != 0) return rc;
     Stager st(t);
     const float *ddata = (const float *)st.in(args[2].pdata, (size_t)P.n * dim * 4);
     const float *dq = (const float *)st.in(args[3].pdata, (size_t)P.nq * dim * 4);
@@ -622,12 +751,45 @@ int xcall_ivf(mo_xcall_args_t *args, uint64_t len) {
     if (is_device_ptr(args[6].pdata)) { MOB_CUDA_TRY(cudaMemcpyAsync(offsets.data(), args[6].pdata, offsets.size() * 8, cudaMemcpyDeviceToHost, t.stream)); MOB_CUDA_TRY(cudaStreamSynchronize(t.stream)); }
     else memcpy(offsets.data(), args[6].pdata, offsets.size() * 8);
 
-    IvfJob job{dcent, P.nlist, ddata, P.n, dim, &offsets, doffsets, drowids, (int)P.k, nprobe, (int)P.metric, (int)P.sqrt_out};
+    IvfJob job{dcent, P.nlist, ddata, P.n, dim, &offsets, doffsets, drowids, (int)P.k, nprobe, (int)P.metric, (int)P.sqrt_out, nullptr};
     g_search_stats = SearchStats();
-    rc = ivf_search_level(t, job, 0, dq, P.nq, ok, od);
+    if (!farg) {
+        rc = ivf_search_level(t, job, 0, dq, P.nq, ok, od);
+    } else {
+        // the probes depend only on the centroids: both paths probe the lists the unfiltered search probes
+        uint32_t *admit; int64_t m = 0;
+        rc = filter_admission(t, st, F, P.n, 0, drowids, &admit, &m);
+        std::vector<int64_t> sub_offsets((size_t)P.nlist + 1);
+        if (!rc && filter_compact_wanted(P.n, m, true)) {
+            // few admitted rows: a compacted index -- the admitted entries in list order, their primary keys, and list boundaries
+            // rebuilt from them (lists without an admitted row become empty, and their probes are dropped)
+            int32_t *idx; float *sub;
+            int64_t *sub_ids = (int64_t *)arena_alloc(t, (size_t)(m > 0 ? m : 1) * 8), *dsub_off = (int64_t *)arena_alloc(t, sub_offsets.size() * 8);
+            rc = sub_ids && dsub_off ? filter_gather(t, ddata, P.n, dim, admit, m, &idx, &sub) : MO_RC_INTERNAL_ERROR;
+            if (!rc) {
+                if (m > 0) filter_gather_ids_kernel<<<num_sms() * 4, 256, 0, t.stream>>>(drowids, idx, m, sub_ids);
+                filter_offsets_kernel<<<(unsigned)((P.nlist + 256) / 256), 256, 0, t.stream>>>(doffsets, P.nlist, idx, m, dsub_off);
+                g_launches += m > 0 ? 2 : 1;
+                if (cudaGetLastError() != cudaSuccess) { set_error("filtered search: compaction launch failed"); rc = MO_RC_INTERNAL_ERROR; }
+            }
+            if (!rc && (cudaMemcpyAsync(sub_offsets.data(), dsub_off, sub_offsets.size() * 8, cudaMemcpyDeviceToHost, t.stream) != cudaSuccess ||
+                        cudaStreamSynchronize(t.stream) != cudaSuccess)) { set_error("filtered search: list boundaries download failed"); rc = MO_RC_INTERNAL_ERROR; }
+            if (!rc) {
+                IvfJob sj{dcent, P.nlist, sub, m, dim, &sub_offsets, dsub_off, sub_ids, (int)P.k, nprobe, (int)P.metric, (int)P.sqrt_out, nullptr};
+                rc = ivf_search_level(t, sj, 0, dq, P.nq, ok, od);
+            }
+        } else if (!rc) {
+            g_search_stats.filter_compacted = 0;
+            job.admit = admit;
+            rc = ivf_search_level(t, job, 0, dq, P.nq, ok, od);
+        }
+    }
     int frc = st.finish();
     return rc ? rc : frc;
 }
+
+int xcall_ivf(mo_xcall_args_t *args, uint64_t len) { return ivf_call(args, len, nullptr); }
+int xcall_ivf_filtered(mo_xcall_args_t *args, uint64_t len) { return ivf_call(args, len, &args[8]); }
 
 // 1. probes[q][rank] = list id by ascending centroid distance (findCentroids, ivfflat/search.go:292-311): the exact top-nprobe kernel
 // 2. invert: list -> bucket of (query, slot) pairs
@@ -674,7 +836,8 @@ int ivf_make_plan(ThreadCtx &t, const float *dcent, int64_t nlist, int dim, cons
 // 3. (list, 64-query tile) work items through the exact kernel; 4. merge the nprobe partial lists of each query, local row -> primary
 // key through row_ids, optional sqrt (DistanceTransformIvfflat)
 int ivf_exact_scan(ThreadCtx &t, const IvfPlan &plan, const float *ddata, int64_t n, int dim, const float *dq, int64_t nq,
-                   const std::vector<int64_t> &offsets, const int64_t *drowids, int k, int metric, int sqrt_out, int64_t *ok, double *od) {
+                   const std::vector<int64_t> &offsets, const int64_t *drowids, int k, int metric, int sqrt_out, int64_t *ok, double *od,
+                   const uint32_t *admit) {
     const int64_t nlist = (int64_t)offsets.size() - 1;
     const int64_t npairs = plan.npairs;
     float *xnorm, *qnorm;
@@ -689,7 +852,7 @@ int ivf_exact_scan(ThreadCtx &t, const IvfPlan &plan, const float *ddata, int64_
             w.data = ddata; w.n = n; w.row_begin = offsets[(size_t)l]; w.row_end = offsets[(size_t)l + 1];
             w.queries = dq; w.nq_total = nq; w.qidx = plan.bucket_q + plan.hstart[(size_t)l] + q0; w.q0 = 0;
             w.nq_local = c - q0 < TQ ? c - q0 : TQ;
-            w.slot_of = plan.bucket_slot + plan.hstart[(size_t)l] + q0; w.range = 0; w.xnorm = xnorm; w.qnorm = qnorm;
+            w.slot_of = plan.bucket_slot + plan.hstart[(size_t)l] + q0; w.range = 0; w.xnorm = xnorm; w.qnorm = qnorm; w.admit = admit;
             items.push_back(w);
         }
     }

@@ -652,7 +652,8 @@ tc_rescore_kernel(const float *__restrict__ data, const float *__restrict__ quer
 // first tile on.  One warp per query, lane = row, through the same batch machinery as the re-score.
 __global__ void __launch_bounds__(kRescoreThreads)
 ivf_seed_bound_kernel(const float *__restrict__ data, const float *__restrict__ queries, int dim, int nq, int nprobe, int k,
-                      const int64_t *__restrict__ probes, const int64_t *__restrict__ offsets, float *__restrict__ qbound) {
+                      const int64_t *__restrict__ probes, const int64_t *__restrict__ offsets, float *__restrict__ qbound,
+                      const uint32_t *__restrict__ admit /* filtered search: only admitted rows seed the bound */) {
     using Cfg = godist::RingCfg<false>;
     extern __shared__ __align__(16) unsigned char rescore_smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -662,7 +663,7 @@ ivf_seed_bound_kernel(const float *__restrict__ data, const float *__restrict__ 
         int64_t l = -1;   // the nearest probed list that has rows here (a list-sharded index holds only some of them)
         for (int r = 0; r < nprobe && l < 0; r++) { const int64_t c = probes[q * nprobe + r]; if (c >= 0 && offsets[c + 1] > offsets[c]) l = c; }
         const int64_t b = l >= 0 ? offsets[l] : 0, e = l >= 0 ? offsets[l + 1] : 0;
-        const bool good = b + lane < e;
+        const bool good = b + lane < e && (!admit || ((admit[(b + lane) >> 5] >> ((b + lane) & 31)) & 1u));
         const uint8_t *px = good ? reinterpret_cast<const uint8_t *>(data + (b + lane) * dim) : nullptr;
         const uint8_t *pq = reinterpret_cast<const uint8_t *>(queries + q * dim);
         const godist::RowAcc<float, godist::K_GO_L2SQ> acc = godist::row_batch<float, godist::K_GO_L2SQ, false>(ring, lane, px, pq, dim, good);
@@ -706,7 +707,10 @@ __global__ void tc_final_kernel(int nq, int k, int dim, int nkb, const int *__re
     const int total = m < k ? m : k;
     const int pad = k - total;
     int64_t *ok = out_k + (size_t)q * k; double *od = out_d + (size_t)q * k;
-    for (int j = 0; j < pad; j++) { ok[j] = -1; od[j] = 0.0; }
+    // padding (fewer than k rows exist -- with a filter, fewer than k admitted): key -1, distance 0; brute force with k = 1 and no row
+    // leaves the running minimum untouched: MaxFloat32 (brute_force.go:289-331).  eps_applied = the IVF list scan, which pads with 0.
+    const double pad_d = (k == 1 && !eps_applied) ? (double)3.40282346638528859811704183484516925440e+38f : 0.0;
+    for (int j = 0; j < pad; j++) { ok[j] = -1; od[j] = pad_d; }
     for (int j = 0; j < total; j++) { ok[pad + j] = id[j]; od[pad + j] = sqrt_out ? sqrt((double)d[j]) : (double)d[j]; }
     // the candidate kernel works in units of |q|^2 + |x|^2 - 2 q.x: that IS the L2 distance; for inner product (norms left out)
     // and cosine (normalised operands) it is twice the metric's distance
@@ -745,12 +749,13 @@ static int g_tc_pair_mode = 0;       // 0 = auto, 1 = single-CTA units only, 2 =
 static int g_tc_ladder_mode = 0;     // 0 = auto (one-term level first unless it has been failing), 1 = never, 2 = always
 static int g_tc_share_mode = 0;      // 1 = no cross-unit threshold sharing
 static int g_tc_range_mb = 0;        // L2 budget of one row range of the brute-force candidate pass, MB (0 = ignore the L2)
+static int g_filter_path = 0;        // filtered search: 0 = auto (from the admitted count), 1 = masked scan, 2 = compacted admitted rows
 static std::atomic<int> g_one_term_skip{0};   // searches left before the one-term level is tried again (shared by all callers: a property of the data)
 thread_local SearchStats g_search_stats;
 
 bool search_tuning(const char *name, int value, int *out) {
     static const struct { const char *name; int *knob; } knobs[] = {
-        {"search_mode", &g_search_mode}, {"tc_pair", &g_tc_pair_mode}, {"tc_ladder", &g_tc_ladder_mode}, {"tc_share", &g_tc_share_mode}, {"tc_range_mb", &g_tc_range_mb}};
+        {"search_mode", &g_search_mode}, {"search_filter_path", &g_filter_path}, {"tc_pair", &g_tc_pair_mode}, {"tc_ladder", &g_tc_ladder_mode}, {"tc_share", &g_tc_share_mode}, {"tc_range_mb", &g_tc_range_mb}};
     for (const auto &k : knobs)
         if (!strcmp(name, k.name)) {
             *k.knob = value;
@@ -760,7 +765,8 @@ bool search_tuning(const char *name, int value, int *out) {
         }
     const SearchStats &s = g_search_stats;
     const struct { const char *name; int value; } stats[] = {
-        {"get_tc_kused", s.kused}, {"get_tc_probe_kused", s.probe_kused}, {"get_tc_refined", s.refined}, {"get_tc_fallbacks", s.fallbacks}};
+        {"get_tc_kused", s.kused}, {"get_tc_probe_kused", s.probe_kused}, {"get_tc_refined", s.refined}, {"get_tc_fallbacks", s.fallbacks},
+        {"get_filter_admitted", s.filter_admitted}, {"get_filter_compacted", s.filter_compacted}};
     for (const auto &st : stats)
         if (!strcmp(name, st.name)) { *out = st.value; return true; }
     return false;
@@ -876,7 +882,7 @@ static int tc_run_units(ThreadCtx &t, const TcOperand &A, int64_t a_rows, const 
     const int nunits = (int)units.size();
     float *qbound = nullptr; const int *row_query = nullptr; const float *alonorm = A.lonorm, *xmax2 = nullptr;
     int sh_one = 0, sh_k = 0; float sh_rel = 0.f, sh_abs = 0.f;
-    if (share && !A.enorm && !B.enorm && g_tc_share_mode != 1) {   // inner product leaves the norms out of the epilogue: no sharing there
+    if (share && !A.enorm && g_tc_share_mode != 1) {   // inner product leaves the norms out of the epilogue (A.enorm = zeros): no sharing there
         qbound = share->qbound;
         if (!qbound) {
             qbound = (float *)arena_alloc(t, (size_t)share->nq * 4);
@@ -924,6 +930,20 @@ static int tc_operand_max(ThreadCtx &t, const TcOperand &B, int64_t n, bool with
     tc_max_kernel<<<num_sms() * 2, 256, 0, t.stream>>>(B.norm, n, *xmax2);
     MOB_LAUNCH_CHECK();
     if (with_lo) { tc_max_kernel<<<num_sms() * 2, 256, 0, t.stream>>>(B.lonorm, n, *xmax2 + 1); MOB_LAUNCH_CHECK(); }
+    return MO_RC_SUCCESS;
+}
+
+// filtered search, masked scan: the norms the epilogue adds become +inf for rows that are not admitted, so every approximate distance
+// of such a row is +inf -- it is never listed and never lowers a list's threshold (DESIGN.md section 5.7)
+__global__ void tc_mask_norms_kernel(const float *__restrict__ norm, const uint32_t *__restrict__ admit, int64_t n, float *__restrict__ out) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        out[i] = ((admit[i >> 5] >> (i & 31)) & 1u) ? norm[i] : INFINITY;
+}
+static int tc_mask_norms(ThreadCtx &t, TcOperand &B, int64_t n, const uint32_t *admit) {
+    float *masked = (float *)arena_alloc(t, (size_t)(n > 0 ? n : 1) * 4);
+    if (!masked) return MO_RC_INTERNAL_ERROR;
+    if (n > 0) { tc_mask_norms_kernel<<<num_sms() * 4, 256, 0, t.stream>>>(B.enorm ? B.enorm : B.norm, admit, n, masked); MOB_LAUNCH_CHECK(); }
+    B.enorm = masked;
     return MO_RC_SUCCESS;
 }
 
@@ -1002,6 +1022,15 @@ static int plan_ranges(int64_t ntiles, int mt, int workers, int rmin, int rcap) 
     return best;
 }
 
+// the masked scan costs what the unfiltered search costs; the compacted search costs the gather of the admitted rows plus a search
+// over them whose operand is split per call, not prepared.  Measured crossover (DESIGN.md section 5.12): brute force between 1/2 and
+// all rows admitted, IVF between 1/10 and 1/2 (the unfiltered IVF scan is cheap next to the per-call residual split).
+bool filter_compact_wanted(int64_t n, int64_t admitted, bool ivf) {
+    if (g_filter_path == 1) return false;
+    if (g_filter_path == 2) return true;
+    return ivf ? admitted * 5 <= n : admitted * 4 <= 3 * n;
+}
+
 bool tc_search_applicable(int64_t n, int dim, int64_t nq, int k, int metric) {
     if (g_search_mode == 1) return false;
     // k <= KP: one candidate list per (query, row range); KP < k <= KW ("wide", centroid probes): ranges of >= 128 rows, at least 8 of them
@@ -1036,10 +1065,10 @@ bool tc_ivf_applicable(int64_t n, int dim, int64_t nq, int k, int nprobe, int me
 // still unproven goes to the exact kernel.  Every level answers its queries exactly or hands them down.
 void tc_one_term_report(int64_t nq, int64_t failed);
 static int bf_tc_level(ThreadCtx &t, int level, int metric, const float *ddata, int64_t n, int dim, const float *dq, int64_t nq, int k,
-                       int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d, bool record_stats, bool timed) {
+                       int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d, bool record_stats, bool timed, const uint32_t *admit) {
     if (level >= 2) {
         if (record_stats) g_search_stats.fallbacks = (int)nq;
-        return bruteforce_topk_device(t, ddata, n, dim, dq, nq, k, metric, key_base, sqrt_out, out_k, out_d);
+        return bruteforce_topk_device(t, ddata, n, dim, dq, nq, k, metric, key_base, sqrt_out, out_k, out_d, admit);
     }
     const int normalize = metric == MO_METRIC_COS ? 1 : 0;
     int *dnonfinite = (int *)arena_alloc(t, 4);
@@ -1053,12 +1082,16 @@ static int bf_tc_level(ThreadCtx &t, int level, int metric, const float *ddata, 
     rc = read_back(t, &hnonfinite, dnonfinite, 4);
     if (rc) return rc;
     if (hnonfinite)   // the error bound of the tensor-core pass does not apply to Inf/NaN inputs (cosine: nor to zero vectors)
-        return bf_tc_level(t, 2, metric, ddata, n, dim, dq, nq, k, key_base, sqrt_out, out_k, out_d, record_stats, false);
+        return bf_tc_level(t, 2, metric, ddata, n, dim, dq, nq, k, key_base, sqrt_out, out_k, out_d, record_stats, false, admit);
     if (metric == MO_METRIC_IP) {   // -q.x: the epilogue adds no norms (the candidate kernel then works in units of -2 q.x)
         float *zeros = (float *)arena_alloc(t, (size_t)(n > nq ? n : nq) * 4);
         if (!zeros) return MO_RC_INTERNAL_ERROR;
         MOB_CUDA_TRY(cudaMemsetAsync(zeros, 0, (size_t)(n > nq ? n : nq) * 4, t.stream));
         A.enorm = zeros; B.enorm = zeros;
+    }
+    if (admit) {   // filtered search: the prepared operand is used as it is; only the norms its epilogue adds are masked
+        int rc2 = tc_mask_norms(t, B, n, admit);
+        if (rc2) return rc2;
     }
     const bool one_term = level == 0;
     const int nkb = one_term ? (dim + BK - 1) / BK : A.kprime / BK;
@@ -1111,7 +1144,7 @@ static int bf_tc_level(ThreadCtx &t, int level, int metric, const float *ddata, 
     }
     // queries whose completeness could not be proven: next level
     return redo_queries(t, redo, dq, dim, k, out_k, out_d, [&](const float *sub, int64_t m, int64_t *sk, double *sd) {
-        return bf_tc_level(t, level + 1, metric, ddata, n, dim, sub, m, k, key_base, sqrt_out, sk, sd, record_stats, false);
+        return bf_tc_level(t, level + 1, metric, ddata, n, dim, sub, m, k, key_base, sqrt_out, sk, sd, record_stats, false, admit);
     });
 }
 
@@ -1134,18 +1167,18 @@ bool tc_one_term_wanted(int k, bool record) {
 void tc_one_term_report(int64_t nq, int64_t failed) { if (nq >= 64 && failed * 5 > nq * 2) g_one_term_skip.store(16); }
 
 int bruteforce_topk_tc_device(ThreadCtx &t, const float *ddata, int64_t n, int dim, const float *dq, int64_t nq, int k,
-                              int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d, bool record_stats, int metric) {
+                              int64_t key_base, int sqrt_out, int64_t *out_k, double *out_d, bool record_stats, int metric, const uint32_t *admit) {
     const bool ladder = tc_one_term_wanted(k, record_stats);
     if (record_stats) g_search_stats.fallbacks = 0;   // the search reached the tensor cores
     if (metric == MO_METRIC_L2) metric = MO_METRIC_L2SQ;
-    return bf_tc_level(t, ladder ? 0 : 1, metric, ddata, n, dim, dq, nq, k, key_base, sqrt_out, out_k, out_d, record_stats, record_stats);
+    return bf_tc_level(t, ladder ? 0 : 1, metric, ddata, n, dim, dq, nq, k, key_base, sqrt_out, out_k, out_d, record_stats, record_stats, admit);
 }
 
 // IVF list scan on the tensor cores: the queries probing a list are gathered (as split bf16 rows) next to each other, so
 // a (list, 128-query tile) pair is one work unit of the same candidate kernel; every (query, probe rank) pair owns one list.
 int ivf_tc_scan(ThreadCtx &t, const IvfPlan &plan, const float *ddata, int64_t n, int dim, const float *dq, int64_t nq,
                 const float *dcent, const int64_t *doffsets, const std::vector<int64_t> &offsets, const int64_t *drowids, int k, int sqrt_out,
-                int pass, int64_t *ok, double *od, std::vector<int> &redo, bool *nonfinite) {
+                int pass, int64_t *ok, double *od, std::vector<int> &redo, bool *nonfinite, const uint32_t *admit) {
     // pass 0: hi-only product over whole lists (one term), pass 1: three-term product over whole lists, pass 2 (refine): three-term
     // product with every list cut into sub-ranges of `chunk` rows, each keeping its own KP candidates, so the excluded-row
     // threshold of a (query, list) pair moves far away from the k-th result
@@ -1176,6 +1209,7 @@ int ivf_tc_scan(ThreadCtx &t, const IvfPlan &plan, const float *ddata, int64_t n
     rc = read_back(t, &hnonfinite, dnonfinite, 4);
     if (rc) return rc;
     if (hnonfinite) { *nonfinite = true; redo.resize((size_t)nq); for (int64_t q = 0; q < nq; q++) redo[(size_t)q] = (int)q; return MO_RC_SUCCESS; }
+    if (admit && (rc = tc_mask_norms(t, B, n, admit)) != 0) return rc;
     std::vector<TcUnit> units;
     for (int64_t l = 0; l < nlist; l++) {
         const int c = plan.hcnt[(size_t)l];
@@ -1208,7 +1242,7 @@ int ivf_tc_scan(ThreadCtx &t, const IvfPlan &plan, const float *ddata, int64_t n
         if (!attr) { MOB_CUDA_TRY(cudaFuncSetAttribute(ivf_seed_bound_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
         int64_t blocks = (nq + kRescoreThreads / 32 - 1) / (kRescoreThreads / 32);
         if (blocks > 2ll * num_sms()) blocks = 2ll * num_sms();
-        ivf_seed_bound_kernel<<<(unsigned)blocks, kRescoreThreads, smem, t.stream>>>(ddata, dq, dim, (int)nq, plan.nprobe, k, plan.probes, doffsets, sh.qbound);
+        ivf_seed_bound_kernel<<<(unsigned)blocks, kRescoreThreads, smem, t.stream>>>(ddata, dq, dim, (int)nq, plan.nprobe, k, plan.probes, doffsets, sh.qbound, admit);
         MOB_LAUNCH_CHECK();
     }
     const int nkb = one_term ? (dim + BK - 1) / BK : A.kprime / BK;

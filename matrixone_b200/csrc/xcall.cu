@@ -30,6 +30,8 @@ int xcall_join_probe(mo_xcall_args_t *args, uint64_t len);
 int xcall_group_agg(int op, int T, mo_xcall_args_t *args, uint64_t len);
 int xcall_bruteforce(mo_xcall_args_t *args, uint64_t len);
 int xcall_ivf(mo_xcall_args_t *args, uint64_t len);
+int xcall_bruteforce_filtered(mo_xcall_args_t *args, uint64_t len);
+int xcall_ivf_filtered(mo_xcall_args_t *args, uint64_t len);
 int xcall_topk_merge(mo_xcall_args_t *args, uint64_t len);
 int tuning_set(const char *name, int value);
 }  // namespace mob
@@ -79,6 +81,8 @@ extern "C" int32_t XCall(int64_t runtimeId, int64_t funcId, uint8_t *errStr, uin
     else if (funcId == MO_XCALL_BRUTEFORCE_TOPK_F32) rc = xcall_bruteforce(a, len);
     else if (funcId == MO_XCALL_IVF_TOPK_F32) rc = xcall_ivf(a, len);
     else if (funcId == MO_XCALL_TOPK_MERGE) rc = xcall_topk_merge(a, len);
+    else if (funcId == MO_XCALL_BRUTEFORCE_TOPK_FILTERED_F32) rc = xcall_bruteforce_filtered(a, len);
+    else if (funcId == MO_XCALL_IVF_TOPK_FILTERED_F32) rc = xcall_ivf_filtered(a, len);
     else return -1;  // unknown funcId, cgo/mo.c:64-67
     if (rc != 0) fill_err(errStr, rc);
     return rc;

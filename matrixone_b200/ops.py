@@ -234,6 +234,23 @@ def _search_params(n, dim, nq, k, metric, nprobe=0, sqrt_out=0, nlist=0, key_bas
     return capi.SearchParams(n, dim, nq, k, metric, nprobe, sqrt_out, nlist, key_base)
 
 
+def _filter_vec(filt):
+    """the mo_search_filter_t argument of a filtered search.  filt: key bitmap words (numpy uint64, host) or a DeviceBuffer of them
+    (bit `key` set = admitted), or a bloom filter handle (bloomfilter_t * from the library's bloomfilter_* symbols, as int / c_void_p)"""
+    if isinstance(filt, DeviceBuffer):
+        d = capi.SearchFilter(capi.SEARCH_FILTER_KEY_BITMAP, 0, filt.ptr, filt.nbytes // 8)
+        return _params_vec(d), None
+    if isinstance(filt, np.ndarray):
+        w = np.ascontiguousarray(filt, dtype=np.uint64).reshape(-1)
+        d = capi.SearchFilter(capi.SEARCH_FILTER_KEY_BITMAP, 0, w.ctypes.data, w.size)
+        return _params_vec(d), w
+    if isinstance(filt, C.c_void_p):
+        filt = filt.value
+    if isinstance(filt, int):
+        return _params_vec(capi.SearchFilter(capi.SEARCH_FILTER_KEY_BLOOM, 0, filt, 0)), None
+    raise TypeError("filter: numpy uint64 key bitmap, DeviceBuffer key bitmap, or bloom filter handle")
+
+
 class BruteForceIndex:
     """brute_force.GoBruteForceIndex: NewBruteForceIndex(dataset, dim, metric) keeps the dataset RESIDENT in HBM
     (the reference keeps it in C-malloc memory, brute_force.go:104-123); Search returns (keys int64[nq*limit],
@@ -257,9 +274,10 @@ class BruteForceIndex:
         if self.prepared:
             capi.check(self.lib.MoB200_SearchPrepareMetric(self.buf.ptr, self.n, self.dim, self.metric), self.lib)
 
-    def search(self, queries, limit, out_device=False, out=None):
+    def search(self, queries, limit, out_device=False, out=None, filter=None):
         """out = (keys_device_ptr, distances_device_ptr): results stay in caller-owned device memory (int64 / float64, nq*limit
-        each) and nothing is returned -- the form a multi-GPU caller hands straight to NCCL"""
+        each) and nothing is returned -- the form a multi-GPU caller hands straight to NCCL.
+        filter: search only the rows whose key (key_base + row) the filter admits (see _filter_vec)"""
         if isinstance(queries, DeviceBuffer):
             nq = queries.nbytes // (4 * self.dim)
             qv = Vector(data_ptr=queries.ptr, data_nbytes=queries.nbytes, length=nq)
@@ -271,14 +289,19 @@ class BruteForceIndex:
             return np.zeros(0, dtype=np.int64), np.zeros(0, dtype=np.float64)
         p = _search_params(self.n, self.dim, nq, limit, self.metric, key_base=self.key_base)
         dv = Vector(data_ptr=self.buf.ptr, data_nbytes=self.n * self.dim * 4, length=self.n)
+        fid, extra, keep = capi.XCALL_BRUTEFORCE_TOPK_F32, [], None
+        if filter is not None:
+            fv, keep = _filter_vec(filter)
+            fid, extra = capi.XCALL_BRUTEFORCE_TOPK_FILTERED_F32, [fv]
         if out is not None:
             kv = Vector(data_ptr=out[0], data_nbytes=nq * limit * 8, length=nq)
             dvv = Vector(data_ptr=out[1], data_nbytes=nq * limit * 8, length=nq)
-            xcall(capi.XCALL_BRUTEFORCE_TOPK_F32, [kv, dvv, dv, qv, _params_vec(p)], nq)
+            xcall(fid, [kv, dvv, dv, qv, _params_vec(p)] + extra, nq)
             return None
         keys = np.zeros(nq * limit, dtype=np.int64)
         dists = np.zeros(nq * limit, dtype=np.float64)
-        xcall(capi.XCALL_BRUTEFORCE_TOPK_F32, [Vector(data=keys, length=nq), Vector(data=dists, length=nq), dv, qv, _params_vec(p)], nq)
+        xcall(fid, [Vector(data=keys, length=nq), Vector(data=dists, length=nq), dv, qv, _params_vec(p)] + extra, nq)
+        del keep
         return keys, dists
 
     def destroy(self):
@@ -370,7 +393,8 @@ class IvfflatSearchIndex:
         ix.d_ids.free(); ix.d_ids = DeviceBuffer.from_numpy(ix.row_ids, lib)
         return ix
 
-    def search(self, queries, limit, nprobe, sqrt_out=False, out=None):
+    def search(self, queries, limit, nprobe, sqrt_out=False, out=None, filter=None):
+        """filter: search only the entries whose primary key (row id) the filter admits, in the lists the unfiltered search probes"""
         if isinstance(queries, DeviceBuffer):
             nq = queries.nbytes // (4 * self.dim)
             qvec = Vector(data_ptr=queries.ptr, data_nbytes=queries.nbytes, length=nq)
@@ -387,13 +411,18 @@ class IvfflatSearchIndex:
             dists = np.zeros(nq * limit, dtype=np.float64)
             kv, dvv = Vector(data=keys, length=nq), Vector(data=dists, length=nq)
         p = _search_params(self.n, self.dim, nq, limit, self.metric, nprobe=nprobe, sqrt_out=int(sqrt_out), nlist=self.nlist)
-        xcall(capi.XCALL_IVF_TOPK_F32, [
+        fid, extra, keep = capi.XCALL_IVF_TOPK_F32, [], None
+        if filter is not None:
+            fv, keep = _filter_vec(filter)
+            fid, extra = capi.XCALL_IVF_TOPK_FILTERED_F32, [fv]
+        xcall(fid, [
             kv, dvv,
             Vector(data_ptr=self.d_data.ptr, data_nbytes=self.d_data.nbytes, length=self.n),
             qvec, _params_vec(p),
             Vector(data_ptr=self.d_cent.ptr, data_nbytes=self.d_cent.nbytes, length=self.nlist),
             Vector(data_ptr=self.d_off.ptr, data_nbytes=self.d_off.nbytes, length=self.nlist + 1),
-            Vector(data_ptr=self.d_ids.ptr, data_nbytes=self.d_ids.nbytes, length=self.n)], nq)
+            Vector(data_ptr=self.d_ids.ptr, data_nbytes=self.d_ids.nbytes, length=self.n)] + extra, nq)
+        del keep
         return keys, dists
 
     def destroy(self):
