@@ -369,16 +369,6 @@ int run_minmax(ThreadCtx &t, const void *dcol, const uint64_t *dnulls, uint64_t 
     return MO_RC_SUCCESS;
 }
 
-int type_size(int T) {
-    switch (T) {
-    case MO_T_BOOL: case MO_T_INT8: case MO_T_UINT8: return 1;
-    case MO_T_INT16: case MO_T_UINT16: return 2;
-    case MO_T_INT32: case MO_T_UINT32: case MO_T_FLOAT32: case MO_T_DATE: return 4;
-    case MO_T_INT64: case MO_T_UINT64: case MO_T_FLOAT64: case MO_T_TIME: case MO_T_DATETIME: case MO_T_TIMESTAMP: return 8;
-    }
-    return 0;
-}
-
 __global__ void popcount_kernel(const uint64_t *p, uint64_t nbits, unsigned long long *out) {
     // count set bits among the first nbits (last word masked, cgo/bitmap.h:110-131)
     uint64_t nw = (nbits + 63) >> 6;

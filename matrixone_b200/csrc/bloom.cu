@@ -19,6 +19,7 @@
 //   Algorithmic bytes per key: elemsz + 1 result byte + k x 32-byte sectors of the filter.
 #include "common.cuh"
 #include "bloom_internal.cuh"
+#include "keytable.cuh"
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -110,9 +111,9 @@ bloom_kernel(uint64_t *__restrict__ bits, uint64_t nbits, uint32_t k, uint64_t s
 }
 
 // ---- test_and_add ------------------------------------------------------------------------------------------------------------------------
-constexpr uint64_t kEmpty = ~0ull;
-__device__ __forceinline__ uint64_t mix64(uint64_t x) { x ^= x >> 33; x *= 0xff51afd7ed558ccdull; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull; return x ^ (x >> 33); }
-
+// The scratch table is a keytable.cuh table (keys and rows filled with 0xff bytes).  An entry's key is the position with the position's bit
+// before the call in bit 63, so it is never all ones; it is probed from the slot of the position alone, because taa_finish_kernel looks it up
+// without knowing that bit.  The table is at most half full, so kt_insert_from always finds a slot.
 __global__ void __launch_bounds__(256)
 taa_insert_kernel(const uint64_t *__restrict__ bits, uint64_t nbits, uint32_t k, uint64_t seed, KeySrc K, uint64_t nitem, const uint64_t *__restrict__ nullmap,
                   uint64_t *__restrict__ tkey, unsigned *__restrict__ trow, uint64_t tmask) {
@@ -127,13 +128,7 @@ taa_insert_kernel(const uint64_t *__restrict__ bits, uint64_t nbits, uint32_t k,
             // inserter of a position builds the same key)
             const uint64_t was = (bits[pos >> 6] >> (pos & 63)) & 1ull;
             const uint64_t key = pos | (was << 63);
-            uint64_t s = mix64(pos) & tmask;
-            for (;;) {
-                uint64_t cur = tkey[s];
-                if (cur == kEmpty) cur = atomicCAS((unsigned long long *)&tkey[s], (unsigned long long)kEmpty, (unsigned long long)key);
-                if (cur == kEmpty || cur == key) { atomicMin(&trow[s], (unsigned)i); break; }
-                s = (s + 1) & tmask;
-            }
+            atomicMin(&trow[kt_insert_from(tkey, tmask, key, mix64(pos) & tmask)], (unsigned)i);
         }
     }
 }
@@ -158,10 +153,6 @@ taa_finish_kernel(uint64_t *__restrict__ bits, uint64_t nbits, uint32_t k, uint6
         }
         result[i] = all ? 1 : 0;
     }
-}
-
-__global__ void taa_init_kernel(uint64_t *tkey, unsigned *trow, uint64_t slots) {
-    for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < slots; s += (uint64_t)gridDim.x * blockDim.x) { tkey[s] = kEmpty; trow[s] = 0xffffffffu; }
 }
 
 // offsets of a [u32 length][payload] stream (bloom.c:159-176): inherently sequential; one thread walks it (this format is not used by the Go side)
@@ -224,13 +215,15 @@ void run(const char *what, int op, int fmt, const bloomfilter_t *bf, const void 
     } else {
         uint64_t slots = 1024;
         while (slots < 2 * (uint64_t)nitem * (bf->k ? bf->k : 1)) slots <<= 1;
-        uint64_t *tkey = (uint64_t *)st.tmp(slots * 8);
-        unsigned *trow = (unsigned *)st.tmp(slots * 4);
+        uint64_t *tkey = (uint64_t *)st.tmp(slots * 12);   // then trow: both start as all ones, so one memset sets up the table
+        unsigned *trow = (unsigned *)(tkey + slots);
         if (st.failed) { st.finish(); bloom_fatal(what); }
-        taa_init_kernel<<<num_sms() * 4, 256, 0, t.stream>>>(tkey, trow, slots);
+        if (cudaMemsetAsync(tkey, 0xff, slots * 12, t.stream) != cudaSuccess) {
+            set_error("bloom: scratch table initialisation failed"); st.finish(); bloom_fatal(what);
+        }
         taa_insert_kernel<<<grid, 256, 0, t.stream>>>(bits, bf->nbits, bf->k, bf->seed, K, nitem, nm, tkey, trow, slots - 1);
         taa_finish_kernel<<<grid, 256, 0, t.stream>>>(bits, bf->nbits, bf->k, bf->seed, K, nitem, nm, tkey, trow, slots - 1, res);
-        g_launches.fetch_add(3, std::memory_order_relaxed);
+        g_launches.fetch_add(2, std::memory_order_relaxed);
     }
     cudaEventRecord(t.kev1, t.stream);
     if (cudaGetLastError() != cudaSuccess) { set_error("bloom: kernel launch failed"); st.finish(); bloom_fatal(what); }

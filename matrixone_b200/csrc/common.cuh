@@ -102,6 +102,17 @@ struct Stager {
 // read one small device value back through the pinned staging buffer (synchronises the stream)
 int read_back(ThreadCtx &t, void *host_dst, const void *dev_src, size_t bytes);
 
+// element width in bytes of a fixed-width MO_T_* type, 0 for any other type
+inline int type_size(int T) {
+    switch (T) {
+    case MO_T_BOOL: case MO_T_INT8: case MO_T_UINT8: return 1;
+    case MO_T_INT16: case MO_T_UINT16: return 2;
+    case MO_T_INT32: case MO_T_UINT32: case MO_T_FLOAT32: case MO_T_DATE: return 4;
+    case MO_T_INT64: case MO_T_UINT64: case MO_T_FLOAT64: case MO_T_TIME: case MO_T_DATETIME: case MO_T_TIMESTAMP: return 8;
+    }
+    return 0;
+}
+
 }  // namespace mob
 
 // =========================================================================================================
@@ -137,6 +148,18 @@ __device__ __forceinline__ void st_stream16(void *p, int4 v) {
 }
 
 __device__ __forceinline__ bool bm_test(const uint64_t *p, uint64_t i) { return p && ((p[i >> 6] >> (i & 63)) & 1ull); }
+
+// total order on non-NaN doubles as unsigned integers, so that MIN / MAX states can use the integer atomics; -0.0 is folded onto +0.0 (they
+// compare equal in the reference too)
+__device__ __forceinline__ unsigned long long flt_key(double d) {
+    if (d == 0.0) d = 0.0;
+    unsigned long long b = (unsigned long long)__double_as_longlong(d);
+    return (b >> 63) ? ~b : (b | (1ull << 63));
+}
+__device__ __forceinline__ double flt_unkey(unsigned long long k) {
+    const unsigned long long b = (k >> 63) ? (k & ~(1ull << 63)) : ~k;
+    return __longlong_as_double((long long)b);
+}
 
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v) {

@@ -15,6 +15,7 @@
 //   call (O(groups)) unless it was prepared with MoB200_JoinMapPrepare (cached per table_keys pointer).
 // All passes stream their inputs once; algorithmic bytes per probe row: 8 (key) + 16 per emitted pair + one random 8-byte table probe.
 #include "common.cuh"
+#include "keytable.cuh"
 #include <cstring>
 #include <mutex>
 #include <shared_mutex>
@@ -25,9 +26,6 @@ namespace mob {
 namespace {
 
 constexpr int kThreads = 256;
-constexpr uint64_t kEmptyKey = 0xffffffffffffffffull;
-
-__device__ __forceinline__ uint64_t mix64(uint64_t x) { x ^= x >> 33; x *= 0xff51afd7ed558ccdull; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull; return x ^ (x >> 33); }
 
 inline unsigned grid_for(uint64_t items, int per_block = kThreads) {
     uint64_t g = (items + per_block - 1) / per_block;
@@ -172,43 +170,28 @@ __global__ void __launch_bounds__(kThreads) copy_rows_kernel(const uint32_t *__r
     if (blockIdx.x == 0 && threadIdx.x == 0) *count_out = (int64_t)m;
 }
 
-// ---- the probe-side hash table -----------------------------------------------------------------------------------------------------------------------
-struct JoinTable { uint64_t *key; uint32_t *id; uint64_t mask; uint32_t sentinel_id; /* id of the key 0xff..ff (stored outside the table) */ };
-
-__global__ void __launch_bounds__(kThreads) jt_init_kernel(uint64_t *key, uint32_t *id, uint64_t slots) {
-    for (uint64_t s = blockIdx.x * (uint64_t)kThreads + threadIdx.x; s < slots; s += (uint64_t)gridDim.x * kThreads) { key[s] = kEmptyKey; id[s] = 0; }
-}
-__global__ void __launch_bounds__(kThreads) jt_build_kernel(const uint64_t *__restrict__ table_keys, uint64_t ngroups, uint64_t *key, uint32_t *id, uint64_t mask, uint32_t *sentinel_id) {
+// ---- the probe-side hash table: a keytable.cuh table, key[slots + 1] and id[slots + 1] (the id of the all-ones key, or 0, in id[slots]) -----------
+__global__ void __launch_bounds__(kThreads) jt_build_kernel(const uint64_t *__restrict__ table_keys, uint64_t ngroups, uint64_t *key, uint32_t *id, uint64_t mask) {
     for (uint64_t g = blockIdx.x * (uint64_t)kThreads + threadIdx.x; g < ngroups; g += (uint64_t)gridDim.x * kThreads) {
-        const uint64_t k = table_keys[g];
-        if (k == kEmptyKey) { *sentinel_id = (uint32_t)(g + 1); continue; }
-        uint64_t s = mix64(k) & mask;
-        for (;;) {
-            const uint64_t cur = atomicCAS((unsigned long long *)&key[s], (unsigned long long)kEmptyKey, (unsigned long long)k);
-            if (cur == kEmptyKey || cur == k) { id[s] = (uint32_t)(g + 1); break; }   // table_keys are distinct: one writer per slot
-            s = (s + 1) & mask;
-        }
+        // the table is at most half full, so a slot is always found; table_keys are distinct: one writer per slot
+        uint64_t s;
+        kt_insert(key, mask, table_keys[g], s);
+        id[s] = (uint32_t)(g + 1);
     }
 }
-__device__ __forceinline__ uint32_t jt_find(const uint64_t *__restrict__ key, const uint32_t *__restrict__ id, uint64_t mask, const uint32_t *sentinel_id, uint64_t k) {
-    if (k == kEmptyKey) return *sentinel_id;
-    uint64_t s = mix64(k) & mask;
-    for (;;) {
-        const uint64_t cur = key[s];
-        if (cur == k) return id[s];
-        if (cur == kEmptyKey) return 0;
-        s = (s + 1) & mask;
-    }
+__device__ __forceinline__ uint32_t jt_find(const uint64_t *__restrict__ key, const uint32_t *__restrict__ id, uint64_t mask, uint64_t k) {
+    uint64_t s;
+    return kt_find(key, mask, k, s) ? id[s] : 0u;
 }
 __global__ void __launch_bounds__(kThreads) jt_find_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ knulls, uint64_t n, const uint64_t *__restrict__ tkey,
-                                                           const uint32_t *__restrict__ tid, uint64_t mask, const uint32_t *sentinel_id, uint64_t *__restrict__ vals) {
+                                                           const uint32_t *__restrict__ tid, uint64_t mask, uint64_t *__restrict__ vals) {
     for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
         const bool isnull = knulls && ((knulls[i >> 6] >> (i & 63)) & 1ull);
-        vals[i] = isnull ? 0ull : (uint64_t)jt_find(tkey, tid, mask, sentinel_id, keys[i]);
+        vals[i] = isnull ? 0ull : (uint64_t)jt_find(tkey, tid, mask, keys[i]);
     }
 }
 
-struct DevTable { uint64_t *key = nullptr; uint32_t *id = nullptr; uint32_t *sentinel = nullptr; uint64_t mask = 0; uint64_t ngroups = 0; bool cached = false; };
+struct DevTable { uint64_t *key = nullptr; uint32_t *id = nullptr; uint64_t mask = 0; uint64_t ngroups = 0; bool cached = false; };
 std::shared_mutex g_jm_mu;
 std::unordered_map<const void *, DevTable> g_jm;   // prepared join maps, by table_keys pointer
 
@@ -217,22 +200,20 @@ int build_table(ThreadCtx &t, const uint64_t *dkeys, uint64_t ngroups, bool pers
     while (slots < 2 * ngroups) slots <<= 1;
     DevTable T;
     if (persistent) {
-        if (cudaMalloc(&T.key, slots * 8) != cudaSuccess || cudaMalloc(&T.id, slots * 4) != cudaSuccess || cudaMalloc(&T.sentinel, 4) != cudaSuccess) {
+        if (cudaMalloc(&T.key, (slots + 1) * 8) != cudaSuccess || cudaMalloc(&T.id, (slots + 1) * 4) != cudaSuccess) {
             set_error("join map: cudaMalloc of a %llu-slot table failed", (unsigned long long)slots);
             if (T.key) cudaFree(T.key);
-            if (T.id) cudaFree(T.id);
             return MO_RC_INTERNAL_ERROR;
         }
     } else {
-        T.key = (uint64_t *)arena_alloc(t, slots * 8); T.id = (uint32_t *)arena_alloc(t, slots * 4); T.sentinel = (uint32_t *)arena_alloc(t, 4);
-        if (!T.key || !T.id || !T.sentinel) return MO_RC_INTERNAL_ERROR;
+        T.key = (uint64_t *)arena_alloc(t, (slots + 1) * 8); T.id = (uint32_t *)arena_alloc(t, (slots + 1) * 4);
+        if (!T.key || !T.id) return MO_RC_INTERNAL_ERROR;
     }
     T.mask = slots - 1; T.ngroups = ngroups; T.cached = persistent;
-    MOB_CUDA_TRY(cudaMemsetAsync(T.sentinel, 0, 4, t.stream));
-    jt_init_kernel<<<grid_for(slots), kThreads, 0, t.stream>>>(T.key, T.id, slots);
-    MOB_LAUNCH_CHECK();
+    MOB_CUDA_TRY(cudaMemsetAsync(T.key, 0xff, (slots + 1) * 8, t.stream));   // every slot empty
+    MOB_CUDA_TRY(cudaMemsetAsync(T.id, 0, (slots + 1) * 4, t.stream));
     if (ngroups) {
-        jt_build_kernel<<<grid_for(ngroups), kThreads, 0, t.stream>>>(dkeys, ngroups, T.key, T.id, T.mask, T.sentinel);
+        jt_build_kernel<<<grid_for(ngroups), kThreads, 0, t.stream>>>(dkeys, ngroups, T.key, T.id, T.mask);
         MOB_LAUNCH_CHECK();
     }
     *out = T;
@@ -253,11 +234,11 @@ int table_for(ThreadCtx &t, Stager &st, const mo_xcall_args_t &a, DevTable *T, s
 
 // ---- JOIN_PROBE -----------------------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads) probe_count_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ knulls, uint64_t n, const uint64_t *__restrict__ tkey,
-                                                               const uint32_t *__restrict__ tid, uint64_t mask, const uint32_t *sentinel_id, const int32_t *__restrict__ offsets,
+                                                               const uint32_t *__restrict__ tid, uint64_t mask, const int32_t *__restrict__ offsets,
                                                                int join_type, uint32_t *__restrict__ vals, uint64_t *__restrict__ cnt) {
     for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
         const bool isnull = knulls && ((knulls[i >> 6] >> (i & 63)) & 1ull);
-        const uint32_t v = isnull ? 0u : jt_find(tkey, tid, mask, sentinel_id, keys[i]);
+        const uint32_t v = isnull ? 0u : jt_find(tkey, tid, mask, keys[i]);
         uint64_t m = 0;
         if (v) m = offsets ? (uint64_t)(offsets[v] - offsets[v - 1]) : 1ull;
         uint64_t c;
@@ -389,7 +370,7 @@ int xcall_join_find(mo_xcall_args_t *args, uint64_t len) {
     const uint64_t *kn = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? ((len + 63) / 64) * 8 : 0);
     if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
     cudaEventRecord(t.kev0, t.stream);
-    jt_find_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(keys, kn, len, T.key, T.id, T.mask, T.sentinel, vals);
+    jt_find_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(keys, kn, len, T.key, T.id, T.mask, vals);
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
     return st.finish();
@@ -426,7 +407,7 @@ int xcall_join_probe(mo_xcall_args_t *args, uint64_t len) {
     uint64_t *total = (uint64_t *)st.tmp(8);
     if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
     cudaEventRecord(t.kev0, t.stream);
-    probe_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(keys, kn, len, T.key, T.id, T.mask, T.sentinel, offsets, P.join_type, vals, cnt);
+    probe_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(keys, kn, len, T.key, T.id, T.mask, offsets, P.join_type, vals, cnt);
     MOB_LAUNCH_CHECK();
     rc = exclusive_scan(t, cnt, len, cnt, total);
     if (rc) { st.finish(); return rc; }
@@ -454,10 +435,10 @@ extern "C" int32_t MoB200_JoinMapPrepare(const void *table_keys, uint64_t ngroup
     DevTable T;
     int rc = build_table(t, dkeys, ngroups, true, &T);
     int frc = st.finish();
-    if (rc || frc) { if (!rc) { cudaFree(T.key); cudaFree(T.id); cudaFree(T.sentinel); } return rc ? rc : frc; }
+    if (rc || frc) { if (!rc) { cudaFree(T.key); cudaFree(T.id); } return rc ? rc : frc; }
     std::unique_lock<std::shared_mutex> lk(g_jm_mu);
     auto it = g_jm.find(table_keys);
-    if (it != g_jm.end()) { cudaFree(it->second.key); cudaFree(it->second.id); cudaFree(it->second.sentinel); }
+    if (it != g_jm.end()) { cudaFree(it->second.key); cudaFree(it->second.id); }
     g_jm[table_keys] = T;
     return MO_RC_SUCCESS;
 }
@@ -468,7 +449,7 @@ extern "C" int32_t MoB200_JoinMapRelease(const void *table_keys) {
     auto it = g_jm.find(table_keys);
     if (it == g_jm.end()) return MO_RC_SUCCESS;
     // (probes hold the shared lock until their stream has drained, so nothing is reading the table once the unique lock is ours)
-    cudaFree(it->second.key); cudaFree(it->second.id); cudaFree(it->second.sentinel);
+    cudaFree(it->second.key); cudaFree(it->second.id);
     g_jm.erase(it);
     return MO_RC_SUCCESS;
 }

@@ -18,6 +18,7 @@
 // converted to float64 (exact below 2^53); each instruction rounds once like the reference's separate nodes (no FMA contraction).
 // Group sums are accumulated with atomics: the association order is not fixed (results agree with the serial loop to ~1e-13).
 #include "common.cuh"
+#include "keytable.cuh"
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -29,7 +30,6 @@ namespace {
 constexpr int kThreads = 128;
 constexpr int kCtaSlots = 32;           // per-CTA group table (shared atomics)
 constexpr int kPriv = 4;               // groups whose state every thread keeps PRIVATELY in shared memory (no atomics, no shuffles)
-constexpr uint64_t kEmptyKey = 0xffffffffffffffffull;
 
 struct PlanCols { const uint8_t *data[MO_PLAN_MAX_COLS]; const uint64_t *nulls[MO_PLAN_MAX_COLS]; };
 
@@ -37,23 +37,10 @@ struct PlanCols { const uint8_t *data[MO_PLAN_MAX_COLS]; const uint64_t *nulls[M
 struct PlanGlobal {
     uint64_t *key; unsigned long long *first_row; unsigned long long *rows;   // [cap]
     double *acc; unsigned long long *cnt;                                      // [cap][naggs]
-    uint64_t mask;                                                             // cap - 1
+    uint64_t mask;                                                             // cap - 1: a keytable.cuh table of cap + 1 slots
     unsigned *overflow;
 };
 
-__device__ __forceinline__ uint64_t mix64(uint64_t x) {
-    x ^= x >> 33; x *= 0xff51afd7ed558ccdull; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull; x ^= x >> 33;
-    return x;
-}
-__device__ __forceinline__ unsigned long long flt_key(double d) {
-    if (d == 0.0) d = 0.0;
-    unsigned long long b = (unsigned long long)__double_as_longlong(d);
-    return (b >> 63) ? ~b : (b | (1ull << 63));
-}
-__device__ __forceinline__ double flt_unkey(unsigned long long k) {
-    const unsigned long long b = (k >> 63) ? (k & ~(1ull << 63)) : ~k;
-    return __longlong_as_double((long long)b);
-}
 __device__ __forceinline__ double agg_identity(int kind) {
     if (kind == MO_AGG_MIN) return __longlong_as_double((long long)~0ull);   // ordered-key domain: all ones
     if (kind == MO_AGG_MAX) return __longlong_as_double(0ll);
@@ -73,19 +60,10 @@ __device__ __forceinline__ void agg_fold(int kind, double *a, double p) {
 }
 
 
-__device__ __forceinline__ uint64_t global_find(PlanGlobal &G, uint64_t key) {
-    if (key == kEmptyKey) { G.key[G.mask + 1] = key; return G.mask + 1; }
-    uint64_t s = mix64(key) & G.mask, probes = 0;
-    for (;;) {
-        uint64_t cur = G.key[s];
-        if (cur == key) return s;
-        if (cur == kEmptyKey) {
-            cur = atomicCAS((unsigned long long *)&G.key[s], (unsigned long long)kEmptyKey, (unsigned long long)key);
-            if (cur == kEmptyKey || cur == key) return s;
-        }
-        s = (s + 1) & G.mask;
-        if (++probes > G.mask) { *G.overflow = 1; return ~0ull; }
-    }
+__device__ __forceinline__ bool global_find(PlanGlobal &G, uint64_t key, uint64_t &slot) {
+    if (kt_insert(G.key, G.mask, key, slot)) return true;
+    *G.overflow = 1;
+    return false;
 }
 
 __global__ void plan_init_kernel(PlanGlobal G, int naggs, const mo_plan_t *P) {
@@ -351,28 +329,20 @@ plan_kernel(const mo_plan_t *__restrict__ Pg, const PlanAux *__restrict__ Ag, Pl
                 const uint64_t key = keys[j];
                 const uint64_t grow = (uint64_t)P.row_base + r0 + (uint64_t)j * kThreads;
                 int slot = -1;
-                if (key != kEmptyKey) {
-                    unsigned s = (unsigned)mix64(key) & (kCtaSlots - 1);
-                    for (int probes = 0; probes < kCtaSlots; probes++) {
-                        uint64_t cur = tkey[s];
-                        if (cur == key) { slot = (int)s; break; }
-                        if (cur == kEmptyKey) {
-                            cur = atomicCAS((unsigned long long *)&tkey[s], (unsigned long long)kEmptyKey, (unsigned long long)key);
-                            if (cur == kEmptyKey || cur == key) { slot = (int)s; break; }
-                        }
-                        s = (s + 1) & (kCtaSlots - 1);
-                    }
+                if (key != kEmptyKey) {   // the CTA table has no all-ones key slot: that key goes to the global table
+                    unsigned s;
+                    if (kt_insert(tkey, (unsigned)(kCtaSlots - 1), key, s)) slot = (int)s;
                 }
                 unsigned long long *first_p = slot >= 0 ? &tfirst[slot] : nullptr, *rows_p = slot >= 0 ? &trows[slot] : nullptr;
                 double *acc_p = slot >= 0 ? &tacc[slot * naggs] : nullptr; unsigned long long *cnt_p = slot >= 0 ? &tcnt[slot * naggs] : nullptr;
                 bool have = true;
                 if (slot < 0) {
-                    const uint64_t gs = global_find(G, key);
-                    if (gs == ~0ull) have = false;
+                    uint64_t gs;
+                    if (!global_find(G, key, gs)) have = false;
                     else { first_p = &G.first_row[gs]; rows_p = &G.rows[gs]; acc_p = &G.acc[gs * naggs]; cnt_p = &G.cnt[gs * naggs]; }
                 }
                 if (have) {
-                    if (*((volatile unsigned long long *)first_p) > grow) atomicMin(first_p, (unsigned long long)grow);
+                    first_row_min(first_p, grow);
                     atomicAdd(rows_p, 1ull);
                     for (int a = 0; a < naggs; a++) {
                         const int vs = P.agg[a].value;
@@ -404,8 +374,8 @@ plan_kernel(const mo_plan_t *__restrict__ Pg, const PlanAux *__restrict__ Ag, Pl
             else if (kind == MO_AGG_MAX) { if ((unsigned long long)__double_as_longlong(v) > (unsigned long long)__double_as_longlong(acc)) acc = v; }
         }
         if (cnt == 0) continue;
-        const uint64_t gs = global_find(G, pk);
-        if (gs == ~0ull) continue;
+        uint64_t gs;
+        if (!global_find(G, pk, gs)) continue;
         agg_fold(kind, &G.acc[gs * naggs + a], acc);
         atomicAdd(&G.cnt[gs * naggs + a], cnt);
     }
@@ -415,16 +385,16 @@ plan_kernel(const mo_plan_t *__restrict__ Pg, const PlanAux *__restrict__ Ag, Pl
         unsigned long long rows = 0, first = ~0ull;
         for (int t = 0; t < kThreads; t++) { rows += prows0[g * kThreads + t]; const unsigned long long f = pfirst0[g * kThreads + t]; if (f < first) first = f; }
         if (rows == 0) continue;
-        const uint64_t gs = global_find(G, pk);
-        if (gs == ~0ull) continue;
+        uint64_t gs;
+        if (!global_find(G, pk, gs)) continue;
         atomicMin(&G.first_row[gs], first);
         atomicAdd(&G.rows[gs], rows);
     }
     // ---- and the shared CTA table
     for (int s = threadIdx.x; s < kCtaSlots; s += kThreads) {
         if (tkey[s] == kEmptyKey || trows[s] == 0) continue;
-        const uint64_t gs = global_find(G, tkey[s]);
-        if (gs == ~0ull) continue;
+        uint64_t gs;
+        if (!global_find(G, tkey[s], gs)) continue;
         atomicMin(&G.first_row[gs], tfirst[s]);
         atomicAdd(&G.rows[gs], trows[s]);
         for (int a = 0; a < naggs; a++) {
