@@ -31,7 +31,7 @@ enum Kind { K_SUM_SIGNED = 0, K_SUM_UNSIGNED = 1, K_SUM_FLOAT = 2, K_MIN = 3, K_
 //  all         : cnt = non-null rows
 struct Rec { uint64_t w0, w1, w2, w3; double d; uint64_t cnt; uint64_t pad0, pad1; };
 // signed SUM: can a prefix of the serial sum leave int64?  Not if every |v| <= INT64_MAX / rows (then even the sum of all magnitudes fits).
-__host__ __device__ __forceinline__ bool sum_check_needed(const Rec &r) { return r.cnt != 0 && r.w2 > (uint64_t)INT64_MAX / r.cnt; }
+__device__ __forceinline__ bool sum_check_needed(const Rec &r) { return r.cnt != 0 && r.w2 > (uint64_t)INT64_MAX / r.cnt; }
 
 __device__ __forceinline__ void add128(uint64_t &lo, uint64_t &hi, uint64_t x) { lo += x; hi += (lo < x); }
 __device__ __forceinline__ void add128p(uint64_t &lo, uint64_t &hi, uint64_t lo2, uint64_t hi2) {
@@ -134,11 +134,12 @@ __device__ Rec block_reduce(Rec r) {
 
 struct Seg { __int128 total, maxp, minp; };
 enum Cls { C_SIGNED = 0, C_UNSIGNED = 1, C_FLOAT = 2, C_MINMAX = 3, C_COUNT = 4 };
-// asynchronous form: the last CTA writes the caller's device-resident result / partial state itself (no second launch)
-struct AggStateOut { uint64_t *res; uint64_t res_words; uint64_t *rnulls; int op; int cls; };
+// the result / partial state in device memory (the caller's, or staged for a host result): the last CTA writes it itself (no second
+// launch); rc, when set, receives the state's rc word for the synchronous form to return
+struct AggStateOut { uint64_t *res; uint64_t res_words; uint64_t *rnulls; int64_t *rc; int op; int cls; };
 
 __device__ __forceinline__ void write_agg_state(const Rec &rec, const AggStateOut &so, int32_t ov) {
-    uint64_t bits = 0, cnt = rec.cnt; int64_t rc = MO_RC_SUCCESS; const bool isnull = cnt == 0;
+    uint64_t bits = 0, cnt = rec.cnt; int64_t rc = MO_RC_SUCCESS; const bool isnull = cnt == 0 && so.cls != C_COUNT;
     double dsum = 0.0;
     if (so.cls == C_SIGNED) { bits = rec.w0; dsum = (double)(int64_t)rec.w0; if (ov) rc = MO_RC_OUT_OF_RANGE; }
     else if (so.cls == C_UNSIGNED) { bits = rec.w0; dsum = (double)rec.w0; if (rec.w1) rc = MO_RC_OUT_OF_RANGE; }
@@ -150,6 +151,7 @@ __device__ __forceinline__ void write_agg_state(const Rec &rec, const AggStateOu
     if (so.res_words >= 2) so.res[1] = cnt;
     if (so.res_words >= 3) so.res[2] = (uint64_t)rc;
     if (so.rnulls) so.rnulls[0] = isnull ? 1ull : 0ull;
+    if (so.rc) *so.rc = rc;
 }
 
 // col must be 16-byte aligned for the vector path (vec = true); rows are [0, n).
@@ -255,44 +257,8 @@ agg_kernel(const T *__restrict__ col, const uint64_t *__restrict__ nulls, uint64
     }
 }
 
-// ---- exact serial-order overflow check for SUM over signed ints (slow path, rare) ---------------------------------
-// Go errors at the first row whose running sum leaves int64 (int64OfCheck, sumavg2.go:89-94).  Each thread summarises a
-// contiguous segment as (total, max prefix, min prefix) in 128-bit; segments are then folded in row order.
-
-// `gate` (async path): the aggregate record of the same call; when its magnitude sum fits int64 no prefix can overflow and the
-// whole grid returns at once
-__device__ __forceinline__ bool prefix_check_needed(const Rec *gate) { return !gate || sum_check_needed(*gate); }
-
-template <typename T>
-__global__ void prefix_seg_kernel(const T *__restrict__ col, const uint64_t *__restrict__ nulls, uint64_t n, uint64_t seg_rows, uint64_t nseg,
-                                  Seg *segs, const Rec *gate) {
-    if (!prefix_check_needed(gate)) return;
-    uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-    if (s >= nseg) return;   // the grid is rounded up to whole CTAs: surplus threads own no segment
-    uint64_t r0 = s * seg_rows, r1 = r0 + seg_rows;
-    if (r1 > n) r1 = n;
-    __int128 tot = 0, mx = 0, mn = 0;
-    for (uint64_t i = r0; i < r1; i++) {
-        if (bm_test(nulls, i)) continue;
-        tot += (__int128)(int64_t)col[i];
-        if (tot > mx) mx = tot;
-        if (tot < mn) mn = tot;
-    }
-    segs[s].total = tot; segs[s].maxp = mx; segs[s].minp = mn;
-}
-__global__ void prefix_fold_kernel(const Seg *segs, uint64_t nseg, int32_t *overflow, const Rec *gate) {
-    if (!prefix_check_needed(gate)) { *overflow = 0; return; }
-    __int128 run = 0; int32_t ov = 0;
-    const __int128 hi = (__int128)INT64_MAX, lo = (__int128)INT64_MIN;
-    for (uint64_t s = 0; s < nseg; s++) {
-        if (run + segs[s].maxp > hi || run + segs[s].minp < lo) { ov = 1; break; }
-        run += segs[s].total;
-    }
-    *overflow = ov;
-}
-
 template <typename T, int KIND>
-int launch_agg(ThreadCtx &t, const void *dcol, const uint64_t *dnulls, uint64_t n, Rec *hrec, Rec **drec = nullptr, AggStateOut so = AggStateOut{nullptr, 0, nullptr, 0, 0}) {
+int launch_agg(ThreadCtx &t, const void *dcol, const uint64_t *dnulls, uint64_t n, const AggStateOut &so) {
     int grid = num_sms() * kCtasPerSm;
     uint64_t work = (n + (16 / sizeof(T)) * kThreads - 1) / ((16 / sizeof(T)) * kThreads);
     if ((uint64_t)grid > work) grid = work ? (int)work : 1;
@@ -304,69 +270,16 @@ int launch_agg(ThreadCtx &t, const void *dcol, const uint64_t *dnulls, uint64_t 
     agg_kernel<T, KIND><<<grid, kThreads, 0, t.stream>>>((const T *)dcol, dnulls, n, vec, partials, out, t.ctrl, so);
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
-    if (drec) { *drec = out; return MO_RC_SUCCESS; }   // async: the record stays on the device
-    return read_back(t, hrec, out, sizeof(Rec));
-}
-
-template <typename T>
-int signed_prefix_overflow(ThreadCtx &t, const void *dcol, const uint64_t *dnulls, uint64_t n, int32_t *ov, const Rec *gate = nullptr,
-                           int32_t **dov_out = nullptr) {
-    const uint64_t nseg_target = (uint64_t)num_sms() * 256;
-    uint64_t seg_rows = (n + nseg_target - 1) / nseg_target;
-    if (seg_rows < 64) seg_rows = 64;
-    uint64_t nseg = (n + seg_rows - 1) / seg_rows;
-    Seg *segs = (Seg *)arena_alloc(t, sizeof(Seg) * nseg + 16);
-    if (!segs) return MO_RC_INTERNAL_ERROR;
-    int32_t *dov = (int32_t *)(segs + nseg);
-    prefix_seg_kernel<T><<<(unsigned)((nseg + 255) / 256), 256, 0, t.stream>>>((const T *)dcol, dnulls, n, seg_rows, nseg, segs, gate);
-    MOB_LAUNCH_CHECK();
-    prefix_fold_kernel<<<1, 1, 0, t.stream>>>(segs, nseg, dov, gate);
-    MOB_LAUNCH_CHECK();
-    if (dov_out) { *dov_out = dov; return MO_RC_SUCCESS; }   // async: the flag stays on the device
-    return read_back(t, ov, dov, 4);
-}
-
-template <typename T>
-int run_sum_signed(ThreadCtx &t, const void *dcol, const uint64_t *dnulls, uint64_t n, int64_t *sum, uint64_t *cnt) {
-    Rec r;
-    int rc = launch_agg<T, K_SUM_SIGNED>(t, dcol, dnulls, n, &r);
-    if (rc) return rc;
-    *cnt = r.cnt;
-    // |every prefix| <= sum of |v|: if that fits int64 nothing can overflow and the wrapping sum is the exact sum
-    *sum = (int64_t)r.w0;
-    if (!sum_check_needed(r)) return MO_RC_SUCCESS;
-    // otherwise decide with the exact serial-order prefix check; when it passes, the total fits and the wrapping sum is exact
-    int32_t ov = 0;
-    rc = signed_prefix_overflow<T>(t, dcol, dnulls, n, &ov);
-    if (rc) return rc;
-    return ov ? MO_RC_OUT_OF_RANGE : MO_RC_SUCCESS;
-}
-
-template <typename T>
-int run_sum_unsigned(ThreadCtx &t, const void *dcol, const uint64_t *dnulls, uint64_t n, uint64_t *sum, uint64_t *cnt) {
-    Rec r;
-    int rc = launch_agg<T, K_SUM_UNSIGNED>(t, dcol, dnulls, n, &r);
-    if (rc) return rc;
-    *cnt = r.cnt; *sum = r.w0;
-    return r.w1 ? MO_RC_OUT_OF_RANGE : MO_RC_SUCCESS;  // prefixes are monotone: overflow iff the exact total exceeds 2^64-1
-}
-
-template <typename T>
-int run_sum_float(ThreadCtx &t, const void *dcol, const uint64_t *dnulls, uint64_t n, double *sum, uint64_t *cnt) {
-    Rec r;
-    int rc = launch_agg<T, K_SUM_FLOAT>(t, dcol, dnulls, n, &r);
-    if (rc) return rc;
-    *cnt = r.cnt; *sum = r.d;
     return MO_RC_SUCCESS;
 }
 
-template <typename T, int KIND>
-int run_minmax(ThreadCtx &t, const void *dcol, const uint64_t *dnulls, uint64_t n, uint64_t *bits, uint64_t *cnt) {
-    Rec r;
-    int rc = launch_agg<T, KIND>(t, dcol, dnulls, n, &r);
-    if (rc) return rc;
-    *cnt = r.cnt; *bits = r.w0;
-    return MO_RC_SUCCESS;
+template <typename T>
+int launch_agg_typed(ThreadCtx &t, const void *dcol, const uint64_t *dnulls, uint64_t n, const AggStateOut &so) {
+    if (so.op == MO_AGG_MIN) return launch_agg<T, K_MIN>(t, dcol, dnulls, n, so);
+    if (so.op == MO_AGG_MAX) return launch_agg<T, K_MAX>(t, dcol, dnulls, n, so);
+    if (so.cls == C_FLOAT) return launch_agg<T, K_SUM_FLOAT>(t, dcol, dnulls, n, so);
+    if (so.cls == C_UNSIGNED) return launch_agg<T, K_SUM_UNSIGNED>(t, dcol, dnulls, n, so);
+    return launch_agg<T, K_SUM_SIGNED>(t, dcol, dnulls, n, so);
 }
 
 __global__ void popcount_kernel(const uint64_t *p, uint64_t nbits, unsigned long long *out) {
@@ -382,104 +295,22 @@ __global__ void popcount_kernel(const uint64_t *p, uint64_t nbits, unsigned long
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
 }
 
-// ---- device-resident results (the asynchronous form) ----------------------------------------------------------------------------
-// When the column AND the result vector live in device memory the call only enqueues work on the calling thread's stream: no host
-// read-back, no synchronisation.  A 1-thread kernel turns the aggregate record into the caller's result words.  This is what lets a
-// multi-GPU caller hand the partial state straight to NCCL (MergeGroup seam, mergeGroup.go:132-247) and merge on the device.
-__global__ void agg_state_kernel(const Rec *rec, int op, int cls, uint64_t len, const unsigned long long *nullcount, const Seg *segs, uint64_t nseg,
-                                 uint64_t *res, uint64_t res_words, uint64_t *rnulls) {
-    uint64_t bits = 0, cnt = 0; int64_t rc = MO_RC_SUCCESS; bool isnull = false;
-    // signed SUM whose magnitudes do not fit int64: fold the serial-order segment summaries (prefix_seg_kernel ran behind the same gate)
-    int32_t ov = 0;
-    if (cls == C_SIGNED && segs && prefix_check_needed(rec)) {
-        __int128 run = 0;
-        const __int128 hi = (__int128)INT64_MAX, lo = (__int128)INT64_MIN;
-        for (uint64_t s = 0; s < nseg; s++) {
-            if (run + segs[s].maxp > hi || run + segs[s].minp < lo) { ov = 1; break; }
-            run += segs[s].total;
-        }
-    }
-    const int32_t *ovflag = &ov;
-    if (cls == C_COUNT) { cnt = len - (nullcount ? *nullcount : 0ull); bits = cnt; }
-    else {
-        cnt = rec->cnt; isnull = cnt == 0;
-        double dsum = 0.0;
-        if (cls == C_SIGNED) {
-            bits = rec->w0; dsum = (double)(int64_t)rec->w0;
-            if (sum_check_needed(*rec) && ovflag && *ovflag) rc = MO_RC_OUT_OF_RANGE;
-        } else if (cls == C_UNSIGNED) { bits = rec->w0; dsum = (double)rec->w0; if (rec->w1) rc = MO_RC_OUT_OF_RANGE; }
-        else if (cls == C_FLOAT) { dsum = rec->d; memcpy(&bits, &dsum, 8); }
-        else bits = rec->w0;
-        // a 1-word result of AVG is the final value; a 3-word result is the partial STATE (sum in the SUM return type, count, rc) and AVG divides at the merge
-        if (op == MO_AGG_AVG && res_words < 3 && !isnull) { double avg = dsum / (double)cnt; memcpy(&bits, &avg, 8); }
-    }
-    res[0] = bits;
-    if (res_words >= 2) res[1] = cnt;
-    if (res_words >= 3) res[2] = (uint64_t)rc;
-    if (rnulls) rnulls[0] = isnull ? 1ull : 0ull;
-}
-
-template <typename T>
-static int agg_async_typed(ThreadCtx &t, int op, int cls, const void *dcol, const uint64_t *dnulls, uint64_t n, Rec **drec, AggStateOut so) {
-    // ONE launch: the last CTA of the aggregate kernel writes the caller's result / state (and, for a signed SUM whose magnitudes do not fit
-    // int64, runs the exact serial-order check itself)
-    if (op == MO_AGG_MIN) return launch_agg<T, K_MIN>(t, dcol, dnulls, n, nullptr, drec, so);
-    if (op == MO_AGG_MAX) return launch_agg<T, K_MAX>(t, dcol, dnulls, n, nullptr, drec, so);
-    if (cls == C_FLOAT) return launch_agg<T, K_SUM_FLOAT>(t, dcol, dnulls, n, nullptr, drec, so);
-    if (cls == C_UNSIGNED) return launch_agg<T, K_SUM_UNSIGNED>(t, dcol, dnulls, n, nullptr, drec, so);
-    return launch_agg<T, K_SUM_SIGNED>(t, dcol, dnulls, n, nullptr, drec, so);
-}
-
-static int xcall_agg_async(ThreadCtx &t, int op, int T, mo_xcall_args_t *args, uint64_t len) {
-    const void *dcol = args[1].pdata;
-    const uint64_t *dnulls = args[1].pnulls;
-    const bool is_signed = T >= MO_T_INT8 && T <= MO_T_INT64, is_unsigned = T >= MO_T_UINT8 && T <= MO_T_UINT64;
-    const bool is_float = T == MO_T_FLOAT32 || T == MO_T_FLOAT64;
-    Rec *drec = nullptr; unsigned long long *dcount = nullptr;
-    bool state_written = false;
-    int cls, rc = MO_RC_SUCCESS;
-    Rec *zero = (Rec *)arena_alloc(t, sizeof(Rec));
-    if (!zero) return MO_RC_INTERNAL_ERROR;
-    if (op == MO_AGG_COUNT) {
-        cls = C_COUNT;
-        if (dnulls && len) {
-            dcount = (unsigned long long *)arena_alloc(t, 8);
-            if (!dcount) return MO_RC_INTERNAL_ERROR;
-            MOB_CUDA_TRY(cudaMemsetAsync(dcount, 0, 8, t.stream));
-            uint64_t nw = (len + 63) >> 6;
-            int grid = (int)((nw + 255) / 256);
-            if (grid > num_sms() * 8) grid = num_sms() * 8;
-            popcount_kernel<<<grid, 256, 0, t.stream>>>(dnulls, len, dcount);
-            MOB_LAUNCH_CHECK();
-        }
-    } else if (op == MO_AGG_MIN || op == MO_AGG_MAX || op == MO_AGG_SUM || op == MO_AGG_AVG) {
-        const bool mm = op == MO_AGG_MIN || op == MO_AGG_MAX;
-        cls = mm ? C_MINMAX : is_signed ? C_SIGNED : is_unsigned ? C_UNSIGNED : C_FLOAT;
-        if (!mm && !is_signed && !is_unsigned && !is_float) { set_error("sum: unsupported type %d", T); return MO_RC_INVALID_ARGUMENT; }
-        const AggStateOut so{(uint64_t *)args[0].pdata, args[0].dataSz / 8, args[0].pnulls, op, cls};
-        state_written = len != 0;
-        if (len == 0) { MOB_CUDA_TRY(cudaMemsetAsync(zero, 0, sizeof(Rec), t.stream)); drec = zero; }
-        else switch (T) {
-        case MO_T_BOOL: case MO_T_UINT8: rc = agg_async_typed<uint8_t>(t, op, cls, dcol, dnulls, len, &drec, so); break;
-        case MO_T_INT8: rc = agg_async_typed<int8_t>(t, op, cls, dcol, dnulls, len, &drec, so); break;
-        case MO_T_INT16: rc = agg_async_typed<int16_t>(t, op, cls, dcol, dnulls, len, &drec, so); break;
-        case MO_T_UINT16: rc = agg_async_typed<uint16_t>(t, op, cls, dcol, dnulls, len, &drec, so); break;
-        case MO_T_INT32: case MO_T_DATE: rc = agg_async_typed<int32_t>(t, op, cls, dcol, dnulls, len, &drec, so); break;
-        case MO_T_UINT32: rc = agg_async_typed<uint32_t>(t, op, cls, dcol, dnulls, len, &drec, so); break;
-        case MO_T_INT64: case MO_T_TIME: case MO_T_DATETIME: case MO_T_TIMESTAMP: rc = agg_async_typed<int64_t>(t, op, cls, dcol, dnulls, len, &drec, so); break;
-        case MO_T_UINT64: rc = agg_async_typed<uint64_t>(t, op, cls, dcol, dnulls, len, &drec, so); break;
-        case MO_T_FLOAT32: rc = agg_async_typed<float>(t, op, cls, dcol, dnulls, len, &drec, so); break;
-        case MO_T_FLOAT64: rc = agg_async_typed<double>(t, op, cls, dcol, dnulls, len, &drec, so); break;
-        default: set_error("agg: unsupported type %d", T); return MO_RC_INVALID_ARGUMENT;
-        }
-        if (rc) return rc;
-    } else { set_error("agg: unknown op %d", op); return MO_RC_INVALID_ARGUMENT; }
-    if (!state_written) {   // COUNT, or an empty column
-        agg_state_kernel<<<1, 1, 0, t.stream>>>(drec, op, cls, len, dcount, nullptr, 0, (uint64_t *)args[0].pdata, args[0].dataSz / 8, args[0].pnulls);
-        MOB_LAUNCH_CHECK();
-    }
-    arena_reset(t);   // stream order protects the scratch: the next call's kernels queue behind these
+// *dout = set bits among the first nbits of dp (nbits > 0), in stream order
+int launch_popcount(ThreadCtx &t, const uint64_t *dp, uint64_t nbits, unsigned long long *dout) {
+    MOB_CUDA_TRY(cudaMemsetAsync(dout, 0, 8, t.stream));
+    uint64_t nw = (nbits + 63) >> 6;
+    int grid = (int)((nw + 255) / 256);
+    if (grid > num_sms() * 8) grid = num_sms() * 8;
+    popcount_kernel<<<grid, 256, 0, t.stream>>>(dp, nbits, dout);
+    MOB_LAUNCH_CHECK();
     return MO_RC_SUCCESS;
+}
+
+// COUNT, or an empty column: the state without a column scan (COUNT subtracts the null count popcount_kernel left in *nullcount)
+__global__ void agg_state_kernel(uint64_t len, const unsigned long long *nullcount, AggStateOut so) {
+    Rec r{};
+    if (so.cls == C_COUNT) r.w0 = r.cnt = len - (nullcount ? *nullcount : 0ull);
+    write_agg_state(r, so, 0);
 }
 
 // ---- MergeGroup for H0 aggregates: fold `n` partial states (value bits, non-null count, rc) in order (BatchMerge, sumavg2.go:205-248,
@@ -572,16 +403,14 @@ int bitmap_count_device(ThreadCtx &t, const uint64_t *dp, uint64_t nbits, uint64
     if (nbits == 0 || !dp) { *count = 0; return MO_RC_SUCCESS; }
     unsigned long long *dout = (unsigned long long *)arena_alloc(t, 8);
     if (!dout) return MO_RC_INTERNAL_ERROR;
-    MOB_CUDA_TRY(cudaMemsetAsync(dout, 0, 8, t.stream));
-    uint64_t nw = (nbits + 63) >> 6;
-    int grid = (int)((nw + 255) / 256);
-    if (grid > num_sms() * 8) grid = num_sms() * 8;
-    popcount_kernel<<<grid, 256, 0, t.stream>>>(dp, nbits, dout);
-    MOB_LAUNCH_CHECK();
-    return read_back(t, count, dout, 8);
+    int rc = launch_popcount(t, dp, nbits, dout);
+    return rc ? rc : read_back(t, count, dout, 8);
 }
 
 // XCall family MO_XCALL_AGG(op, T): args[0] = result, args[1] = column.  See include/mo_b200.h.
+// When the column AND the result live in device memory the call only enqueues work on the calling thread's stream: no read-back, no
+// synchronisation.  This is what lets a multi-GPU caller hand the partial state straight to NCCL (MergeGroup seam, mergeGroup.go:132-247)
+// and merge on the device.  Otherwise the same kernels write staged buffers, and the call returns the state's rc.
 int xcall_agg(int op, int T, mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
@@ -589,82 +418,56 @@ int xcall_agg(int op, int T, mo_xcall_args_t *args, uint64_t len) {
     if (!sz || T == MO_T_BOOL && op != MO_AGG_COUNT && op != MO_AGG_MIN && op != MO_AGG_MAX) { set_error("agg: unsupported type %d", T); return MO_RC_INVALID_ARGUMENT; }
     if (!args[0].pdata || args[0].dataSz < 8) { set_error("agg: result vector must hold 8 bytes"); return MO_RC_INVALID_ARGUMENT; }
     if (args[1].dataSz < (uint64_t)sz * len) { set_error("agg: column shorter than len"); return MO_RC_INVALID_ARGUMENT; }
-    if (is_device_ptr(args[0].pdata) && (len == 0 || is_device_ptr(args[1].pdata)) && (!args[0].pnulls || is_device_ptr(args[0].pnulls)) &&
-        (!args[1].pnulls || is_device_ptr(args[1].pnulls)))
-        return xcall_agg_async(t, op, T, args, len);
+    if (op < 0 || op > MO_AGG_AVG) { set_error("agg: unknown op %d", op); return MO_RC_INVALID_ARGUMENT; }
+    const bool is_signed = T >= MO_T_INT8 && T <= MO_T_INT64, is_unsigned = T >= MO_T_UINT8 && T <= MO_T_UINT64;
+    const int cls = op == MO_AGG_COUNT ? C_COUNT : (op == MO_AGG_MIN || op == MO_AGG_MAX) ? C_MINMAX : is_signed ? C_SIGNED : is_unsigned ? C_UNSIGNED : C_FLOAT;
+    if (cls == C_FLOAT && T != MO_T_FLOAT32 && T != MO_T_FLOAT64) { set_error("sum: unsupported type %d", T); return MO_RC_INVALID_ARGUMENT; }
+    const bool async = is_device_ptr(args[0].pdata) && (len == 0 || is_device_ptr(args[1].pdata)) && (!args[0].pnulls || is_device_ptr(args[0].pnulls)) &&
+                       (!args[1].pnulls || is_device_ptr(args[1].pnulls));
     Stager st(t);
     const void *dcol = st.in(args[1].pdata, (size_t)sz * len);
     const uint64_t *dnulls = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? ((len + 63) / 64) * 8 : 0);
+    // 1 word: the value; 2: + non-null rows; 3: + rc (the partial state MO_XCALL_AGG_MERGE folds)
+    const uint64_t words = args[0].dataSz >= 24 ? 3 : args[0].dataSz / 8;
+    // the synchronous form stages the host results and the rc word as one block: one copy back, as for an 8192-row call it is most of the cost
+    struct { uint64_t words[3], nulls; int64_t rc; } h{};
+    uint64_t *dh = async ? nullptr : (uint64_t *)st.out(&h, sizeof h);
+    const bool hres = !async && !is_device_ptr(args[0].pdata), hnulls = !async && args[0].pnulls && !is_device_ptr(args[0].pnulls);
+    const AggStateOut so{hres ? dh : (uint64_t *)args[0].pdata, words, hnulls ? dh + 3 : args[0].pnulls, async ? nullptr : (int64_t *)dh + 4, op, cls};
     if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
-
-    uint64_t bits = 0, cnt = 0; int rc = MO_RC_SUCCESS; bool isnull = false;
-    const bool is_signed = T >= MO_T_INT8 && T <= MO_T_INT64, is_unsigned = T >= MO_T_UINT8 && T <= MO_T_UINT64;
-    const bool is_float = T == MO_T_FLOAT32 || T == MO_T_FLOAT64;
-    if (len == 0) { isnull = (op != MO_AGG_COUNT); }
-    else if (op == MO_AGG_COUNT) {
-        uint64_t nn = 0;
-        rc = bitmap_count_device(t, dnulls, dnulls ? len : 0, &nn);
-        bits = len - nn;
-    } else if (op == MO_AGG_SUM || op == MO_AGG_AVG) {
-        double dsum = 0; int64_t isum = 0; uint64_t usum = 0;
-        if (is_signed) {
-            switch (sz) {
-            case 1: rc = run_sum_signed<int8_t>(t, dcol, dnulls, len, &isum, &cnt); break;
-            case 2: rc = run_sum_signed<int16_t>(t, dcol, dnulls, len, &isum, &cnt); break;
-            case 4: rc = run_sum_signed<int32_t>(t, dcol, dnulls, len, &isum, &cnt); break;
-            default: rc = run_sum_signed<int64_t>(t, dcol, dnulls, len, &isum, &cnt); break;
-            }
-            memcpy(&bits, &isum, 8); dsum = (double)isum;
-        } else if (is_unsigned) {
-            switch (sz) {
-            case 1: rc = run_sum_unsigned<uint8_t>(t, dcol, dnulls, len, &usum, &cnt); break;
-            case 2: rc = run_sum_unsigned<uint16_t>(t, dcol, dnulls, len, &usum, &cnt); break;
-            case 4: rc = run_sum_unsigned<uint32_t>(t, dcol, dnulls, len, &usum, &cnt); break;
-            default: rc = run_sum_unsigned<uint64_t>(t, dcol, dnulls, len, &usum, &cnt); break;
-            }
-            bits = usum; dsum = (double)usum;
-        } else if (is_float) {
-            if (sz == 4) rc = run_sum_float<float>(t, dcol, dnulls, len, &dsum, &cnt);
-            else rc = run_sum_float<double>(t, dcol, dnulls, len, &dsum, &cnt);
-            memcpy(&bits, &dsum, 8);
-        } else { set_error("sum: unsupported type %d", T); rc = MO_RC_INVALID_ARGUMENT; }
-        isnull = cnt == 0;
-        if (op == MO_AGG_AVG && args[0].dataSz >= 24) { /* partial STATE: the raw sum, the merge divides */ }
-        else if (op == MO_AGG_AVG && !isnull) { double avg = dsum / (double)cnt; memcpy(&bits, &avg, 8); }  // sumavg2.go:331
-    } else if (op == MO_AGG_MIN || op == MO_AGG_MAX) {
-#define MM(TT) (op == MO_AGG_MIN ? run_minmax<TT, K_MIN>(t, dcol, dnulls, len, &bits, &cnt) : run_minmax<TT, K_MAX>(t, dcol, dnulls, len, &bits, &cnt))
+    int rc = MO_RC_SUCCESS;
+    if (op == MO_AGG_COUNT || len == 0) {
+        unsigned long long *dcount = nullptr;
+        if (op == MO_AGG_COUNT && dnulls && len) {
+            dcount = (unsigned long long *)st.tmp(8);
+            if (st.failed) return MO_RC_INTERNAL_ERROR;
+            rc = launch_popcount(t, dnulls, len, dcount);
+            if (rc) return rc;
+        }
+        agg_state_kernel<<<1, 1, 0, t.stream>>>(len, dcount, so);
+        MOB_LAUNCH_CHECK();
+    } else {
         switch (T) {
-        case MO_T_BOOL: case MO_T_UINT8: rc = MM(uint8_t); break;
-        case MO_T_INT8: rc = MM(int8_t); break;
-        case MO_T_INT16: rc = MM(int16_t); break;
-        case MO_T_UINT16: rc = MM(uint16_t); break;
-        case MO_T_INT32: case MO_T_DATE: rc = MM(int32_t); break;
-        case MO_T_UINT32: rc = MM(uint32_t); break;
-        case MO_T_INT64: case MO_T_TIME: case MO_T_DATETIME: case MO_T_TIMESTAMP: rc = MM(int64_t); break;
-        case MO_T_UINT64: rc = MM(uint64_t); break;
-        case MO_T_FLOAT32: rc = MM(float); break;
-        case MO_T_FLOAT64: rc = MM(double); break;
-        default: rc = MO_RC_INVALID_ARGUMENT;
+        case MO_T_BOOL: case MO_T_UINT8: rc = launch_agg_typed<uint8_t>(t, dcol, dnulls, len, so); break;
+        case MO_T_INT8: rc = launch_agg_typed<int8_t>(t, dcol, dnulls, len, so); break;
+        case MO_T_INT16: rc = launch_agg_typed<int16_t>(t, dcol, dnulls, len, so); break;
+        case MO_T_UINT16: rc = launch_agg_typed<uint16_t>(t, dcol, dnulls, len, so); break;
+        case MO_T_INT32: case MO_T_DATE: rc = launch_agg_typed<int32_t>(t, dcol, dnulls, len, so); break;
+        case MO_T_UINT32: rc = launch_agg_typed<uint32_t>(t, dcol, dnulls, len, so); break;
+        case MO_T_INT64: case MO_T_TIME: case MO_T_DATETIME: case MO_T_TIMESTAMP: rc = launch_agg_typed<int64_t>(t, dcol, dnulls, len, so); break;
+        case MO_T_UINT64: rc = launch_agg_typed<uint64_t>(t, dcol, dnulls, len, so); break;
+        case MO_T_FLOAT32: rc = launch_agg_typed<float>(t, dcol, dnulls, len, so); break;
+        case MO_T_FLOAT64: rc = launch_agg_typed<double>(t, dcol, dnulls, len, so); break;
+        default: set_error("agg: unsupported type %d", T); return MO_RC_INVALID_ARGUMENT;
         }
-#undef MM
-        isnull = cnt == 0;
-    } else { set_error("agg: unknown op %d", op); rc = MO_RC_INVALID_ARGUMENT; }
-
-    // write the result (host memory directly; device memory through the stream)
-    if (rc == MO_RC_SUCCESS || rc == MO_RC_OUT_OF_RANGE) {
-        uint64_t nullword = isnull ? 1ull : 0ull;
-        if (op == MO_AGG_COUNT) cnt = bits;
-        uint64_t words[3] = {bits, cnt, (uint64_t)(int64_t)rc};
-        const size_t wb = args[0].dataSz >= 24 ? 24 : args[0].dataSz >= 16 ? 16 : 8;   // 8: value; 16: + non-null rows; 24: + rc (partial state)
-        if (is_device_ptr(args[0].pdata)) cudaMemcpyAsync(args[0].pdata, words, wb, cudaMemcpyHostToDevice, t.stream);
-        else memcpy(args[0].pdata, words, wb);
-        if (args[0].pnulls) {
-            if (is_device_ptr(args[0].pnulls)) cudaMemcpyAsync(args[0].pnulls, &nullword, 8, cudaMemcpyHostToDevice, t.stream);
-            else memcpy(args[0].pnulls, &nullword, 8);
-        }
+        if (rc) return rc;
     }
-    int frc = st.finish();
-    return rc ? rc : frc;
+    if (async) { st.release_async(); return MO_RC_SUCCESS; }   // the state's rc word carries errors
+    rc = st.finish();
+    if (rc) return rc;
+    if (hres) memcpy(args[0].pdata, h.words, 8 * words);
+    if (hnulls) memcpy(args[0].pnulls, &h.nulls, 8);
+    return (int)h.rc;
 }
 
 }  // namespace mob

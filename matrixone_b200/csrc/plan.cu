@@ -21,7 +21,7 @@
 #include "keytable.cuh"
 #include <cmath>
 #include <cstring>
-#include <vector>
+#include <algorithm>
 
 using namespace mob;
 
@@ -506,78 +506,51 @@ static bool is_q1_shape(const mo_plan_t &P) {
 
 namespace mob {
 
-int xcall_q6(mo_xcall_args_t *args, uint64_t len);
-int xcall_q1(mo_xcall_args_t *args, uint64_t len);
+int q6_run(ThreadCtx &t, Stager &st, const uint8_t *const cols[4], uint64_t len, const mo_q6_params_t &P, double *res, uint64_t res_words,
+           uint64_t *rnulls);
+int q1_run(ThreadCtx &t, Stager &st, const uint8_t *const cols[7], bool varlena, uint64_t len, int32_t cutoff, int64_t row_base,
+           mo_q1_result_t *res);
 extern int g_plan_specialise;   // MoB200_SetTuning("plan_specialise", 0) forces the interpreter (tests, profiling)
 
-// returns 1 when a specialised kernel answered (rc in *rc), 0 when the interpreter must run
-static int plan_try_specialised(ThreadCtx &t, const mo_plan_t &P, mo_xcall_args_t *args, uint64_t len, uint64_t res_groups, int *rc) {
-    if (!g_plan_specialise || len == 0) return 0;
-    for (int c = 0; c < P.ncols; c++) if (args[2 + c].pnulls) return 0;
+// Runs the specialised kernel when the descriptor is the Q6 or Q1 shape over non-nullable columns and sets *answered; otherwise (and when
+// the Q1 scan finds more groups than the result can take) the interpreter must run.
+static int plan_try_specialised(ThreadCtx &t, const mo_plan_t &P, mo_xcall_args_t *args, uint64_t len, uint64_t res_groups, bool *answered) {
+    *answered = false;
+    if (!g_plan_specialise || len == 0) return MO_RC_SUCCESS;
+    for (int c = 0; c < P.ncols; c++) if (args[2 + c].pnulls) return MO_RC_SUCCESS;
     const bool q6 = is_q6_shape(P), q1 = !q6 && is_q1_shape(P);
-    if (!q6 && !q1) return 0;
-    const bool dev_res = is_device_ptr(args[0].pdata);
-    bool dev_cols = true;
-    for (int c = 0; c < P.ncols; c++) dev_cols = dev_cols && is_device_ptr(args[2 + c].pdata);
-    const bool async = dev_res && dev_cols;
-    mo_xcall_args_t a[9]; memset(a, 0, sizeof a);
+    if (!q6 && !q1) return MO_RC_SUCCESS;
+    bool async = is_device_ptr(args[0].pdata);
+    const uint8_t *cols[7];
+    for (int c = 0; c < P.ncols; c++) { cols[c] = args[2 + c].pdata; async = async && is_device_ptr(cols[c]); }
+    // the kernels below write the header and the groups they found: the rest of a host result is uploaded first so that the copy-back keeps it
+    const uint64_t ngroups_max = q6 ? 1 : std::min<uint64_t>(res_groups, MO_Q1_MAX_GROUPS);
+    Stager st(t);
+    uint8_t *dres = (uint8_t *)st.out(args[0].pdata, sizeof(mo_plan_result_header_t) + (sizeof(mo_plan_group_t) + sizeof(mo_plan_agg_value_t) * P.naggs) * ngroups_max, true);
+    void *dq = st.tmp(q6 ? sizeof(Q6Out) : sizeof(mo_q1_result_t));
+    int *dflag = (int *)st.tmp(4);
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     if (q6) {
-        mo_q6_params_t Q{(int32_t)P.pred[0].lo, (int32_t)P.pred[1].lo, P.pred[2].lo, P.pred[2].hi, P.pred[3].lo};
-        Q6Out hq{0.0, 0};
-        Q6Out *dq = async ? (Q6Out *)arena_alloc(t, sizeof(Q6Out)) : nullptr;
-        if (async && !dq) { *rc = MO_RC_INTERNAL_ERROR; return 1; }
-        a[0].pdata = async ? (uint8_t *)dq : (uint8_t *)&hq; a[0].dataSz = 16;
-        a[1] = args[2]; a[2] = args[3]; a[3] = args[4]; a[4] = args[5];
-        a[5].pdata = (uint8_t *)&Q; a[5].dataSz = sizeof Q;
-        *rc = xcall_q6(a, len);
-        if (*rc) return 1;
-        if (async) { plan_from_q6_kernel<<<1, 1, 0, t.stream>>>(dq, args[0].pdata); g_launches.fetch_add(1); return 1; }   // dq: arena memory, stream ordered
-        mo_plan_result_header_t H{hq.rows ? 1 : 0, 1, 0, 0};
-        struct { mo_plan_result_header_t h; mo_plan_group_t g; mo_plan_agg_value_t v; } R{H, {0, -1, hq.rows}, {hq.sum, hq.rows}};
-        const size_t bytes = hq.rows ? sizeof R : sizeof H;
-        if (dev_res) { *rc = cudaMemcpyAsync(args[0].pdata, &R, bytes, cudaMemcpyHostToDevice, t.stream) == cudaSuccess && cudaStreamSynchronize(t.stream) == cudaSuccess ? 0 : MO_RC_INTERNAL_ERROR; }
-        else memcpy(args[0].pdata, &R, bytes);
-        return 1;
+        const mo_q6_params_t Q{(int32_t)P.pred[0].lo, (int32_t)P.pred[1].lo, P.pred[2].lo, P.pred[2].hi, P.pred[3].lo};
+        const int rc = q6_run(t, st, cols, len, Q, (double *)dq, 2, nullptr);
+        if (rc) return rc;
+        plan_from_q6_kernel<<<1, 1, 0, t.stream>>>((const Q6Out *)dq, dres);
+        MOB_LAUNCH_CHECK();
+    } else {
+        int rc = q1_run(t, st, cols, false, len, (int32_t)P.pred[0].lo, P.row_base, (mo_q1_result_t *)dq);
+        if (rc == MO_RC_INVALID_ARGUMENT && !async) return st.finish();   // host columns with device ones, or unaligned: the interpreter takes them
+        if (rc) return rc;
+        plan_from_q1_kernel<<<1, 1, 0, t.stream>>>((const mo_q1_result_t *)dq, dres, res_groups, dflag);
+        MOB_LAUNCH_CHECK();
+        // more than the result's groups cannot be known without this read-back
+        int fallback = 0;
+        rc = read_back(t, &fallback, dflag, 4);
+        if (rc) return rc;
+        if (fallback) return st.finish();
     }
-    if (res_groups < 1) return 0;
-    mo_q1_params_t Q{(int32_t)P.pred[0].lo, 0, P.row_base};
-    mo_q1_result_t hq; memset(&hq, 0, sizeof hq);
-    mo_q1_result_t *dq = async ? (mo_q1_result_t *)arena_alloc(t, sizeof(mo_q1_result_t) + 16) : nullptr;
-    if (async && !dq) { *rc = MO_RC_INTERNAL_ERROR; return 1; }
-    a[0].pdata = async ? (uint8_t *)dq : (uint8_t *)&hq; a[0].dataSz = sizeof(mo_q1_result_t);
-    for (int c = 0; c < 7; c++) a[1 + c] = args[2 + c];
-    a[6].dataSz = len; a[7].dataSz = len;     // packed uint8 keys: exactly len bytes (the Q1 entry point tells key layouts apart by size)
-    a[8].pdata = (uint8_t *)&Q; a[8].dataSz = sizeof Q;
-    *rc = xcall_q1(a, len);
-    if (async) {
-        if (*rc) return 1;
-        // more than 8 groups cannot be known without a read-back: the asynchronous form keeps the specialised kernel only when the caller's
-        // buffer could not hold more groups than it anyway; otherwise the interpreter runs
-        int *dflag = (int *)(dq + 1);
-        plan_from_q1_kernel<<<1, 1, 0, t.stream>>>(dq, args[0].pdata, res_groups, dflag);
-        g_launches.fetch_add(1);
-        int hflag = 0;
-        *rc = read_back(t, &hflag, dflag, 4);
-        return (*rc || !hflag) ? 1 : 0;
-    }
-    if (*rc == MO_RC_INVALID_ARGUMENT) { *rc = 0; return 0; }          // > 8 groups: the generic path answers
-    if (*rc) return 1;
-    if ((uint64_t)hq.ngroups > res_groups) { *rc = 0; return 0; }
-    const size_t rec = sizeof(mo_plan_group_t) + 8 * sizeof(mo_plan_agg_value_t);
-    std::vector<uint8_t> buf(sizeof(mo_plan_result_header_t) + rec * (size_t)hq.ngroups);
-    mo_plan_result_header_t H{hq.ngroups, 1, 0, 0};
-    memcpy(buf.data(), &H, sizeof H);
-    for (int64_t i = 0; i < hq.ngroups; i++) {
-        const mo_q1_group_t &s = hq.groups[i];
-        mo_plan_group_t g{(uint64_t)s.returnflag | ((uint64_t)s.linestatus << 8), s.first_row, s.count_order};
-        const double v[8] = {s.sum_qty, s.sum_base_price, s.sum_disc_price, s.sum_charge, s.avg_qty, s.avg_price, s.avg_disc, (double)s.count_order};
-        uint8_t *p = buf.data() + sizeof H + rec * (size_t)i;
-        memcpy(p, &g, sizeof g);
-        for (int k = 0; k < 8; k++) { mo_plan_agg_value_t av{v[k], s.count_order}; memcpy(p + sizeof g + k * sizeof av, &av, sizeof av); }
-    }
-    if (dev_res) { *rc = cudaMemcpyAsync(args[0].pdata, buf.data(), buf.size(), cudaMemcpyHostToDevice, t.stream) == cudaSuccess && cudaStreamSynchronize(t.stream) == cudaSuccess ? 0 : MO_RC_INTERNAL_ERROR; }
-    else memcpy(args[0].pdata, buf.data(), buf.size());
-    return 1;
+    *answered = true;
+    if (async) { st.release_async(); return MO_RC_SUCCESS; }
+    return st.finish();
 }
 
 // MO_XCALL_PLAN: args [0] result buffer ; [1] mo_plan_t (host) ; [2 .. 2 + ncols) the columns (+pnulls).  len = rows.  See include/mo_b200.h.
@@ -616,7 +589,11 @@ int xcall_plan(mo_xcall_args_t *args, uint64_t len) {
     const size_t rec = sizeof(mo_plan_group_t) + sizeof(mo_plan_agg_value_t) * (size_t)P.naggs;
     if (!args[0].pdata || args[0].dataSz < sizeof(mo_plan_result_header_t) + rec) { set_error("plan: result buffer too small for one group"); return MO_RC_INVALID_ARGUMENT; }
     const uint64_t res_groups = (args[0].dataSz - sizeof(mo_plan_result_header_t)) / rec;
-    { int src = 0; if (plan_try_specialised(t, P, args, len, res_groups, &src)) return src; }
+    {
+        bool answered = false;
+        const int rc = plan_try_specialised(t, P, args, len, res_groups, &answered);
+        if (rc || answered) return rc;
+    }
     const bool dev_res = is_device_ptr(args[0].pdata);
     bool dev_cols = true;
     for (int c = 0; c < P.ncols; c++) dev_cols = dev_cols && (len == 0 || is_device_ptr(args[2 + c].pdata)) && (!args[2 + c].pnulls || is_device_ptr(args[2 + c].pnulls));

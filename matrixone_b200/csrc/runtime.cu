@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <vector>
 #include <mutex>
 #include <map>
 #include <list>
@@ -194,14 +195,22 @@ void *Stager::out(void *p, size_t bytes, bool preload) {
 
 int Stager::finish() {
     int rc = failed ? MO_RC_INTERNAL_ERROR : MO_RC_SUCCESS;
+    // outputs that fit go through the pinned staging buffer: a copy into pageable memory waits for the stream by itself, and a call with
+    // a few small results (an aggregate's words and nulls word) would pay that wait once per result
+    size_t pinned_used = 0;
+    std::vector<size_t> at(backs.size(), SIZE_MAX);
     if (!failed) {
-        for (auto &b : backs) {
-            cudaError_t e = cudaMemcpyAsync(b.host, b.dev, b.bytes, cudaMemcpyDeviceToHost, t.stream);
+        for (size_t i = 0; i < backs.size(); i++) {
+            const Back &b = backs[i];
+            if (pinned_used + b.bytes <= t.pinned_sz) { at[i] = pinned_used; pinned_used += b.bytes; }
+            cudaError_t e = cudaMemcpyAsync(at[i] == SIZE_MAX ? b.host : t.pinned + at[i], b.dev, b.bytes, cudaMemcpyDeviceToHost, t.stream);
             if (e != cudaSuccess) { set_error("D2H copy failed: %s", cudaGetErrorString(e)); rc = MO_RC_INTERNAL_ERROR; break; }
         }
     }
     cudaError_t e = cudaStreamSynchronize(t.stream);
     if (e != cudaSuccess) { set_error("stream synchronize failed: %s", cudaGetErrorString(e)); rc = MO_RC_INTERNAL_ERROR; }
+    if (rc == MO_RC_SUCCESS)
+        for (size_t i = 0; i < backs.size(); i++) if (at[i] != SIZE_MAX) memcpy(backs[i].host, t.pinned + at[i], backs[i].bytes);
     backs.clear();
     pins.clear();   // the stream is idle: cached blocks may be evicted now
     arena_reset(t);

@@ -25,6 +25,7 @@
 //   q1_kernel<4>      everything else (varlena keys, unaligned columns, fewer rows): the pair mapping above, loads into registers
 // A pass keeps at most 4 groups per CTA; when it sees more it reports overflow and q1_kernel<8> runs the input again.
 #include "common.cuh"
+#include <algorithm>
 #include <cstring>
 #include <atomic>
 
@@ -38,8 +39,8 @@ constexpr int kThreads = 256;
 // Q6
 // =========================================================================================================
 struct Q6Rec { double sum; unsigned long long cnt; };
-// caller-owned device result (asynchronous form): sum at res[0], qualifying rows at res[1] when res_words >= 2, nulls word bit 0 =
-// "no row qualified" -- the layout MO_XCALL_Q6_MERGE consumes
+// device result (the caller's, or staged for a host result): sum at res[0], qualifying rows at res[1] when res_words >= 2, nulls word
+// bit 0 = "no row qualified" -- the layout MO_XCALL_Q6_MERGE consumes
 struct Q6DevOut { double *res; uint64_t res_words; uint64_t *rnulls; };
 
 // SUM node over one row: the projection l_extendedprice * l_discount is added where the row passed all three conjuncts, +0.0 elsewhere
@@ -442,7 +443,7 @@ q1_kernel(const int32_t *__restrict__ sd, const double *__restrict__ qty, const 
           const double *__restrict__ disc, const double *__restrict__ tax, const uint8_t *__restrict__ rf,
           const uint8_t *__restrict__ ls, uint64_t n, int32_t cutoff, Q1Rec *__restrict__ partials,
           Q1Rec *__restrict__ out, unsigned *ticket, const Q1Rec *gate) {
-    // asynchronous form: the 8-slot retry is enqueued behind the 4-slot pass and runs only if that pass overflowed its dictionary
+    // the 8-slot retry is enqueued behind the 4-slot pass and runs only if that pass overflowed its dictionary
     if (gate && !gate->overflow) return;
     __shared__ Q1Shared S;
     S.dict[threadIdx.x & (MO_Q1_MAX_GROUPS - 1)] = kEmptyKey;   // all threads write (same values): no lane-dependent branch
@@ -626,7 +627,7 @@ q1_tma_kernel(const int32_t *__restrict__ sd, const double *__restrict__ qty, co
     q1_epilogue<G, kCtaThreads>(T, S, partials, out, ticket);
 }
 
-__host__ __device__ void q1_finalize(const Q1Rec &F, mo_q1_result_t *res, int64_t row_base = 0) {
+__device__ void q1_finalize(const Q1Rec &F, mo_q1_result_t *res, int64_t row_base) {
     memset(res, 0, sizeof *res);
     int order[MO_Q1_MAX_GROUPS], ng = 0;
     for (int g = 0; g < MO_Q1_MAX_GROUPS; g++) if (F.slot[g].used && F.slot[g].cnt) order[ng++] = g;
@@ -645,8 +646,8 @@ __host__ __device__ void q1_finalize(const Q1Rec &F, mo_q1_result_t *res, int64_
     }
 }
 
-// asynchronous form: pick the pass that did not overflow, order the groups, write the caller's device result.  ngroups = -1 reports
-// "more than MO_Q1_MAX_GROUPS distinct keys" (the synchronous form returns MO_RC_INVALID_ARGUMENT for that).
+// pick the pass that did not overflow, order the groups, write the device result.  ngroups = -1 reports "more than MO_Q1_MAX_GROUPS
+// distinct keys" (the synchronous form returns MO_RC_INVALID_ARGUMENT for that).
 __global__ void q1_finalize_kernel(const Q1Rec *narrow, const Q1Rec *wide, mo_q1_result_t *res, int64_t row_base) {
     const Q1Rec *F = (narrow && !narrow->overflow) ? narrow : wide;
     if (!F || F->overflow) { memset(res, 0, sizeof *res); res->ngroups = -1; return; }
@@ -734,18 +735,8 @@ static int write_result(ThreadCtx &t, void *dst, const void *src, size_t bytes) 
     return MO_RC_SUCCESS;
 }
 
-// Q6 result: sum in word 0, qualifying rows in word 1 when the buffer holds 16 bytes, nulls word bit 0 = "no row qualified"
-static int write_q6_result(ThreadCtx &t, const mo_xcall_args_t &r, double sum, int64_t rows, bool any) {
-    unsigned char w[16];
-    memcpy(w, &sum, 8); memcpy(w + 8, &rows, 8);
-    int rc = write_result(t, r.pdata, w, r.dataSz >= 16 ? 16 : 8);
-    if (rc || !r.pnulls) return rc;
-    const uint64_t nullword = any ? 0ull : 1ull;
-    return write_result(t, r.pnulls, &nullword, 8);
-}
-
 static int launch_q6(ThreadCtx &t, const int32_t *sd, const double *disc, const double *qty, const double *price,
-                     uint64_t n, const mo_q6_params_t &P, Q6Rec *hrec, Q6DevOut dres = Q6DevOut{nullptr, 0, nullptr}) {
+                     uint64_t n, const mo_q6_params_t &P, Q6DevOut dres) {
     if (!aligned_to(sd, 8) || !aligned_to(disc, 16) || !aligned_to(qty, 16) || !aligned_to(price, 16)) {
         set_error("q6: columns must be 16-byte aligned (int32 column 8-byte)"); return MO_RC_INVALID_ARGUMENT;
     }
@@ -763,8 +754,46 @@ static int launch_q6(ThreadCtx &t, const int32_t *sd, const double *disc, const 
     }
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
-    if (dres.res) return MO_RC_SUCCESS;   // asynchronous form: the last CTA wrote the caller's device result
-    return read_back(t, hrec, out, sizeof(Q6Rec));
+    return MO_RC_SUCCESS;
+}
+
+// Chunks of a scan: device columns are one chunk; host columns are staged kHostChunkRows rows at a time inside the caller's Stager, each
+// chunk's scratch handed back before the next chunk is staged (its copies queue behind the previous kernel on the same stream).
+static uint64_t scan_chunks(bool dev, uint64_t len) { return dev ? (len ? 1 : 0) : (len + kHostChunkRows - 1) / kHostChunkRows; }
+
+// columns [0, ncols) all host or all device; false (error set) otherwise
+static bool same_residency(const char *what, const uint8_t *const *cols, int ncols, bool *dev) {
+    *dev = is_device_ptr(cols[0]);
+    for (int i = 1; i < ncols; i++) if (is_device_ptr(cols[i]) != *dev) { set_error("%s: columns must all be host or all device", what); return false; }
+    return true;
+}
+
+// The Q6 scan of host or device columns {shipdate, discount, quantity, price} into a caller-layout device result.  Partial results of
+// several chunks are merged in chunk order exactly like per-pipeline partials in MergeGroup (BatchMerge, sumavg2.go:222-236); with no
+// rows the merge of zero partials writes the empty (NULL) result.
+int q6_run(ThreadCtx &t, Stager &st, const uint8_t *const cols[4], uint64_t len, const mo_q6_params_t &P, double *res, uint64_t res_words,
+           uint64_t *rnulls) {
+    bool dev;
+    if (!same_residency("q6", cols, 4, &dev)) return MO_RC_INVALID_ARGUMENT;
+    const Q6DevOut dres{res, res_words, rnulls};
+    const uint64_t nchunks = scan_chunks(dev, len);
+    double *parts = nchunks == 1 ? nullptr : (double *)st.tmp(16 * nchunks);
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    for (uint64_t i = 0; i < nchunks; i++) {
+        const uint64_t r0 = i * kHostChunkRows, m = nchunks == 1 ? len : std::min(kHostChunkRows, len - r0);
+        const ArenaMark mark = arena_mark(t);
+        const void *c[4] = {st.in(cols[0] + 4 * r0, 4 * m), st.in(cols[1] + 8 * r0, 8 * m), st.in(cols[2] + 8 * r0, 8 * m), st.in(cols[3] + 8 * r0, 8 * m)};
+        if (st.failed) return MO_RC_INTERNAL_ERROR;
+        const int rc = launch_q6(t, (const int32_t *)c[0], (const double *)c[1], (const double *)c[2], (const double *)c[3], m, P,
+                                 nchunks == 1 ? dres : Q6DevOut{parts + 2 * i, 2, nullptr});
+        if (rc) return rc;
+        arena_rewind(t, mark);
+    }
+    if (nchunks != 1) {
+        q6_merge_kernel<<<1, 1, 0, t.stream>>>(parts, nchunks, dres);
+        MOB_LAUNCH_CHECK();
+    }
+    return MO_RC_SUCCESS;
 }
 
 int xcall_q6(mo_xcall_args_t *args, uint64_t len) {
@@ -798,58 +827,38 @@ int xcall_q6(mo_xcall_args_t *args, uint64_t len) {
         pa[2] = args[1]; pa[3] = args[2]; pa[4] = args[3]; pa[5] = args[4];
         int rc = xcall_plan(pa, len);
         if (rc) return rc;
-        const bool any_ = R.h.ngroups > 0 && R.a.count > 0;
-        return write_q6_result(t, args[0], any_ ? R.a.value : 0.0, R.h.ngroups > 0 ? R.g.rows : 0, any_);
+        // sum in word 0, qualifying rows in word 1 when the buffer holds 16 bytes, nulls word bit 0 = "no row qualified"
+        const bool any = R.h.ngroups > 0 && R.a.count > 0;
+        const double sum = any ? R.a.value : 0.0;
+        const int64_t rows = R.h.ngroups > 0 ? R.g.rows : 0;
+        unsigned char w[16];
+        memcpy(w, &sum, 8); memcpy(w + 8, &rows, 8);
+        rc = write_result(t, args[0].pdata, w, args[0].dataSz >= 16 ? 16 : 8);
+        if (rc || !args[0].pnulls) return rc;
+        const uint64_t nullword = any ? 0ull : 1ull;
+        return write_result(t, args[0].pnulls, &nullword, 8);
     }
 
-    const bool dev = is_device_ptr(args[1].pdata);
-    for (int i = 2; i <= 4; i++) if (is_device_ptr(args[i].pdata) != dev) { set_error("q6: columns must all be host or all device"); return MO_RC_INVALID_ARGUMENT; }
-
-    double sum = 0.0; unsigned long long cnt = 0; bool any = false;
-    int rc = MO_RC_SUCCESS;
-    if (dev && len && is_device_ptr(args[0].pdata) && (!args[0].pnulls || is_device_ptr(args[0].pnulls))) {
-        // resident columns AND a device result: enqueue only (no read-back, no synchronisation); the result is ordered on the calling
-        // thread's stream, ready for NCCL + MO_XCALL_Q6_MERGE or a later MoB200_Download
-        rc = launch_q6(t, (const int32_t *)args[1].pdata, (const double *)args[2].pdata, (const double *)args[3].pdata,
-                       (const double *)args[4].pdata, len, P, nullptr, Q6DevOut{(double *)args[0].pdata, args[0].dataSz / 8, args[0].pnulls});
-        arena_reset(t);
-        return rc;
-    }
-    if (dev || len == 0) {
-        if (len) {
-            Q6Rec r;
-            rc = launch_q6(t, (const int32_t *)args[1].pdata, (const double *)args[2].pdata, (const double *)args[3].pdata,
-                           (const double *)args[4].pdata, len, P, &r);
-            sum = r.sum; cnt = r.cnt; any = r.cnt != 0;
-        }
-        arena_reset(t);
-    } else {
-        // host-resident columns: stream block ranges through the arena; partial sums are merged in chunk order
-        // exactly like per-pipeline partials in MergeGroup (BatchMerge, sumavg2.go:222-236)
-        for (uint64_t r0 = 0; r0 < len && rc == MO_RC_SUCCESS; r0 += kHostChunkRows) {
-            uint64_t m = len - r0 < kHostChunkRows ? len - r0 : kHostChunkRows;
-            Stager st(t);
-            const int32_t *d_sd = (const int32_t *)st.in(args[1].pdata + 4 * r0, 4 * m);
-            const double *d_di = (const double *)st.in(args[2].pdata + 8 * r0, 8 * m);
-            const double *d_q = (const double *)st.in(args[3].pdata + 8 * r0, 8 * m);
-            const double *d_p = (const double *)st.in(args[4].pdata + 8 * r0, 8 * m);
-            if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
-            Q6Rec r;
-            rc = launch_q6(t, d_sd, d_di, d_q, d_p, m, P, &r);
-            if (rc == MO_RC_SUCCESS && r.cnt) { sum = any ? sum + r.sum : r.sum; any = true; cnt += r.cnt; }
-            int frc = st.finish();
-            if (!rc) rc = frc;
-        }
-    }
+    // resident columns AND a device result: enqueue only (no read-back, no synchronisation); the result is ordered on the calling thread's
+    // stream, ready for NCCL + MO_XCALL_Q6_MERGE or a later MoB200_Download
+    const bool async = len && is_device_ptr(args[1].pdata) && is_device_ptr(args[0].pdata) && (!args[0].pnulls || is_device_ptr(args[0].pnulls));
+    Stager st(t);
+    double *dres = (double *)st.out(args[0].pdata, args[0].dataSz >= 16 ? 16 : 8);
+    uint64_t *dn = (uint64_t *)st.out(args[0].pnulls, args[0].pnulls ? 8 : 0);
+    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    const uint8_t *cols[4] = {args[1].pdata, args[2].pdata, args[3].pdata, args[4].pdata};
+    const int rc = q6_run(t, st, cols, len, P, dres, args[0].dataSz / 8, dn);
     if (rc) return rc;
-    return write_q6_result(t, args[0], sum, (int64_t)cnt, any);
+    if (async) { st.release_async(); return MO_RC_SUCCESS; }
+    return st.finish();
 }
 
 // device addresses of the Q1 input columns; the key columns hold packed uint8 values or 24-byte varlena cells
 struct Q1Cols { const int32_t *sd; const double *qty, *price, *disc, *tax; const uint8_t *rf, *ls; };
 
-static int launch_q1(ThreadCtx &t, const Q1Cols &c, bool varlena, uint64_t n, int32_t cutoff, Q1Rec *hrec, mo_q1_result_t *dres = nullptr,
-                     int64_t row_base = 0) {
+// the 4-slot pass, the 8-slot pass that runs only if the 4-slot pass overflowed its dictionary, and q1_finalize_kernel, which writes the
+// caller-layout result of the pass that did not overflow (ngroups = -1 when both did)
+static int launch_q1(ThreadCtx &t, const Q1Cols &c, bool varlena, uint64_t n, int32_t cutoff, mo_q1_result_t *dres, int64_t row_base) {
     if (!aligned_to(c.sd, 8) || !aligned_to(c.qty, 16) || !aligned_to(c.price, 16) || !aligned_to(c.disc, 16) || !aligned_to(c.tax, 16) ||
         !aligned_to(c.rf, varlena ? 8 : 2) || !aligned_to(c.ls, varlena ? 8 : 2)) {
         set_error("q1: columns must be 16-byte aligned (int32 column 8-byte, key columns 2/8-byte)"); return MO_RC_INVALID_ARGUMENT;
@@ -859,69 +868,73 @@ static int launch_q1(ThreadCtx &t, const Q1Cols &c, bool varlena, uint64_t n, in
     // the register kernel's whole pass (DESIGN 5.1).  q1_variant = 1 forces the register kernel, the arm the TMA kernel is tested against.
     const bool tma = !varlena && aligned_to(c.sd, 16) && aligned_to(c.rf, 16) && aligned_to(c.ls, 16) && n >= (uint64_t)kCtaTileRows * 64 &&
                      g_q1_variant != 1;
-    Q1Rec *first_out = nullptr;   // asynchronous form: result record of the 4-slot pass
-    for (int attempt = 0; attempt < 2; attempt++) {
-        const bool wide = attempt == 1;
-        const bool use_tma = tma && !wide;
-        // TMA kernel: one CTA per SM, each taking whole tiles; register kernel: two CTAs per SM, each thread at least one pair
+    // TMA kernel: one CTA per SM, each taking whole tiles; register kernel: two CTAs per SM, each thread at least one pair
+    auto grid_of = [&](bool use_tma) {
         const uint64_t work = use_tma ? n / kCtaTileRows : (n / 2 + kThreads - 1) / kThreads;
         int grid = num_sms() * (use_tma ? 1 : 2);
         if ((uint64_t)grid > work) grid = work ? (int)work : 1;
-        if (grid > kQ1MaxGrid) grid = kQ1MaxGrid;
-        Q1Rec *partials = (Q1Rec *)arena_alloc(t, sizeof(Q1Rec) * (size_t)(grid + 1));
-        if (!partials) return MO_RC_INTERNAL_ERROR;
-        Q1Rec *out = partials + grid;
-        if (attempt == 0 || !dres) cudaEventRecord(t.kev0, t.stream);
-        if (use_tma) {
-            const size_t smem = (size_t)kCtaStages * kCtaTileBytes + 2 * kCtaStages * 8;
-            static bool tattr = false;
-            if (!tattr) {
-                cudaError_t e = cudaFuncSetAttribute(q1_tma_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                if (e != cudaSuccess) { set_error("q1: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return MO_RC_INTERNAL_ERROR; }
-                tattr = true;
-            }
-            q1_tma_kernel<4><<<grid, kCtaThreads, smem, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, out, t.ctrl);
-        } else if (!wide) {
-            if (varlena) q1_kernel<4, 2, 2, 1><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, out, t.ctrl, nullptr);
-            else q1_kernel<4, 2, 2, 0><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, out, t.ctrl, nullptr);
-        } else {
-            if (varlena) q1_kernel<8, 2, 2, 1><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, out, t.ctrl, first_out);
-            else q1_kernel<8, 2, 2, 0><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, out, t.ctrl, first_out);
+        return grid > kQ1MaxGrid ? kQ1MaxGrid : grid;
+    };
+    int grid = grid_of(tma);
+    Q1Rec *partials = (Q1Rec *)arena_alloc(t, sizeof(Q1Rec) * (size_t)(grid + 1));
+    if (!partials) return MO_RC_INTERNAL_ERROR;
+    Q1Rec *narrow = partials + grid;
+    cudaEventRecord(t.kev0, t.stream);
+    if (tma) {
+        const size_t smem = (size_t)kCtaStages * kCtaTileBytes + 2 * kCtaStages * 8;
+        static bool tattr = false;
+        if (!tattr) {
+            cudaError_t e = cudaFuncSetAttribute(q1_tma_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (e != cudaSuccess) { set_error("q1: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return MO_RC_INTERNAL_ERROR; }
+            tattr = true;
         }
-        if (attempt == 0 || !dres) cudaEventRecord(t.kev1, t.stream);
-        MOB_LAUNCH_CHECK();
-        if (dres) {
-            // no read-back: enqueue the gated 8-slot retry behind a 4-slot pass, then the finalize kernel
-            if (!wide) { first_out = out; continue; }
-            q1_finalize_kernel<<<1, 1, 0, t.stream>>>(first_out, out, dres, row_base);
-            MOB_LAUNCH_CHECK();
-            return MO_RC_SUCCESS;
-        }
-        int rc = read_back(t, hrec, out, sizeof(Q1Rec));
-        if (rc) return rc;
-        if (!hrec->overflow) return MO_RC_SUCCESS;
-        if (wide) break;  // more than MO_Q1_MAX_GROUPS distinct keys
+        q1_tma_kernel<4><<<grid, kCtaThreads, smem, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, narrow, t.ctrl);
+    } else if (varlena) {
+        q1_kernel<4, 2, 2, 1><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, narrow, t.ctrl, nullptr);
+    } else {
+        q1_kernel<4, 2, 2, 0><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, narrow, t.ctrl, nullptr);
     }
-    set_error("q1: more than %d distinct group keys; the fused small-cardinality kernel does not apply", MO_Q1_MAX_GROUPS);
-    return MO_RC_INVALID_ARGUMENT;
+    cudaEventRecord(t.kev1, t.stream);
+    MOB_LAUNCH_CHECK();
+    grid = grid_of(false);
+    partials = (Q1Rec *)arena_alloc(t, sizeof(Q1Rec) * (size_t)(grid + 1));
+    if (!partials) return MO_RC_INTERNAL_ERROR;
+    Q1Rec *wide = partials + grid;
+    if (varlena) q1_kernel<8, 2, 2, 1><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, wide, t.ctrl, narrow);
+    else q1_kernel<8, 2, 2, 0><<<grid, kThreads, 0, t.stream>>>(c.sd, c.qty, c.price, c.disc, c.tax, c.rf, c.ls, n, cutoff, partials, wide, t.ctrl, narrow);
+    MOB_LAUNCH_CHECK();
+    q1_finalize_kernel<<<1, 1, 0, t.stream>>>(narrow, wide, dres, row_base);
+    MOB_LAUNCH_CHECK();
+    return MO_RC_SUCCESS;
 }
 
-static void q1_merge_rec(Q1Rec &F, const Q1Rec &R, bool &first) {
-    if (first) { F = R; first = false; return; }
-    for (int g = 0; g < MO_Q1_MAX_GROUPS; g++) {
-        const Q1Slot &s = R.slot[g];
-        if (!s.used || s.cnt == 0) continue;
-        int dst = -1;
-        for (int x = 0; x < MO_Q1_MAX_GROUPS; x++) {
-            if (F.slot[x].used && F.slot[x].key == s.key) { dst = x; break; }
-            if (!F.slot[x].used || F.slot[x].key == kEmptyKey) { dst = x; F.slot[x].key = s.key; F.slot[x].used = 1; F.slot[x].cnt = 0; F.slot[x].first_row = ~0ull; for (int j = 0; j < kQ1Vals; j++) F.slot[x].v[j] = 0; break; }
-        }
-        if (dst < 0) { F.overflow = 1; continue; }
-        Q1Slot &D = F.slot[dst];
-        D.cnt += s.cnt;
-        if (s.first_row < D.first_row) D.first_row = s.first_row;
-        for (int j = 0; j < kQ1Vals; j++) D.v[j] = D.v[j] + s.v[j];
+// The Q1 scan of host or device columns {shipdate, quantity, extendedprice, discount, tax, returnflag, linestatus} into a device
+// mo_q1_result_t (first_row offset by row_base).  Chunks as q6_run; their results are merged in chunk order by q1_merge_kernel.
+int q1_run(ThreadCtx &t, Stager &st, const uint8_t *const cols[7], bool varlena, uint64_t len, int32_t cutoff, int64_t row_base,
+           mo_q1_result_t *res) {
+    bool dev;
+    if (!same_residency("q1", cols, 7, &dev)) return MO_RC_INVALID_ARGUMENT;
+    const uint64_t ksz = varlena ? 24 : 1;
+    const uint64_t nchunks = scan_chunks(dev, len);
+    mo_q1_result_t *parts = nchunks == 1 ? nullptr : (mo_q1_result_t *)st.tmp(sizeof(mo_q1_result_t) * nchunks);
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    for (uint64_t i = 0; i < nchunks; i++) {
+        const uint64_t r0 = i * kHostChunkRows, m = nchunks == 1 ? len : std::min(kHostChunkRows, len - r0);
+        const ArenaMark mark = arena_mark(t);
+        const Q1Cols d{(const int32_t *)st.in(cols[0] + 4 * r0, 4 * m), (const double *)st.in(cols[1] + 8 * r0, 8 * m),
+                       (const double *)st.in(cols[2] + 8 * r0, 8 * m), (const double *)st.in(cols[3] + 8 * r0, 8 * m),
+                       (const double *)st.in(cols[4] + 8 * r0, 8 * m), (const uint8_t *)st.in(cols[5] + ksz * r0, ksz * m),
+                       (const uint8_t *)st.in(cols[6] + ksz * r0, ksz * m)};
+        if (st.failed) return MO_RC_INTERNAL_ERROR;
+        const int rc = launch_q1(t, d, varlena, m, cutoff, nchunks == 1 ? res : parts + i, row_base + (int64_t)r0);
+        if (rc) return rc;
+        arena_rewind(t, mark);
     }
+    if (nchunks != 1) {
+        q1_merge_kernel<<<1, 1, 0, t.stream>>>(parts, nchunks, res);
+        MOB_LAUNCH_CHECK();
+    }
+    return MO_RC_SUCCESS;
 }
 
 int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
@@ -942,7 +955,6 @@ int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
     else memcpy(&cutoff, args[8].pdata, 4);
     const bool dev = is_device_ptr(args[1].pdata);
     for (int i = 2; i <= 7; i++) if (is_device_ptr(args[i].pdata) != dev) { set_error("q1: columns must all be host or all device"); return MO_RC_INVALID_ARGUMENT; }
-    const uint64_t ksz = varlena ? 24 : 1;
     int64_t row_base = 0;   // optional: params = {int32 cutoff; int32 pad; int64 row_base} -> first_row values are global row numbers
     if (args[8].dataSz >= 16 && !is_device_ptr(args[8].pdata)) memcpy(&row_base, args[8].pdata + 8, 8);
     if (q1_nullable) {
@@ -992,48 +1004,24 @@ int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
         return write_result(t, args[0].pdata, &res, sizeof res);
     }
 
-    const Q1Cols cols{(const int32_t *)args[1].pdata, (const double *)args[2].pdata, (const double *)args[3].pdata, (const double *)args[4].pdata,
-                      (const double *)args[5].pdata, args[6].pdata, args[7].pdata};
-    if (dev && len && is_device_ptr(args[0].pdata)) {
-        // resident columns AND a device result: enqueue only (see xcall_q6)
-        int rc = launch_q1(t, cols, varlena, len, cutoff, nullptr, (mo_q1_result_t *)args[0].pdata, row_base);
-        arena_reset(t);
-        return rc;
-    }
-
-    Q1Rec F; memset(&F, 0, sizeof F); bool first = true; int rc = MO_RC_SUCCESS;
-    for (int g = 0; g < MO_Q1_MAX_GROUPS; g++) F.slot[g].key = kEmptyKey;
-    if (dev || len == 0) {
-        if (len) {
-            Q1Rec R;
-            rc = launch_q1(t, cols, varlena, len, cutoff, &R);
-            if (!rc) q1_merge_rec(F, R, first);
-        }
-        arena_reset(t);
-    } else {
-        for (uint64_t r0 = 0; r0 < len && rc == MO_RC_SUCCESS; r0 += kHostChunkRows) {
-            uint64_t m = len - r0 < kHostChunkRows ? len - r0 : kHostChunkRows;
-            Stager st(t);
-            const Q1Cols d{(const int32_t *)st.in(args[1].pdata + 4 * r0, 4 * m), (const double *)st.in(args[2].pdata + 8 * r0, 8 * m),
-                           (const double *)st.in(args[3].pdata + 8 * r0, 8 * m), (const double *)st.in(args[4].pdata + 8 * r0, 8 * m),
-                           (const double *)st.in(args[5].pdata + 8 * r0, 8 * m), (const uint8_t *)st.in(args[6].pdata + ksz * r0, ksz * m),
-                           (const uint8_t *)st.in(args[7].pdata + ksz * r0, ksz * m)};
-            if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
-            Q1Rec R;
-            rc = launch_q1(t, d, varlena, m, cutoff, &R);
-            if (!rc) {
-                for (int g = 0; g < MO_Q1_MAX_GROUPS; g++) if (R.slot[g].used && R.slot[g].cnt) R.slot[g].first_row += r0;
-                q1_merge_rec(F, R, first);
-            }
-            int frc = st.finish();
-            if (!rc) rc = frc;
-        }
-    }
+    const uint8_t *cols[7] = {args[1].pdata, args[2].pdata, args[3].pdata, args[4].pdata, args[5].pdata, args[6].pdata, args[7].pdata};
+    const bool async = dev && len && is_device_ptr(args[0].pdata);   // resident columns AND a device result: enqueue only (see xcall_q6)
+    Stager st(t);
+    mo_q1_result_t *dres = (mo_q1_result_t *)st.out(args[0].pdata, sizeof(mo_q1_result_t));
+    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    int rc = q1_run(t, st, cols, varlena, len, cutoff, row_base, dres);
     if (rc) return rc;
-    if (F.overflow) { set_error("q1: too many groups"); return MO_RC_INVALID_ARGUMENT; }
-    mo_q1_result_t res;
-    q1_finalize(F, &res, row_base);
-    return write_result(t, args[0].pdata, &res, sizeof res);
+    if (async) { st.release_async(); return MO_RC_SUCCESS; }   // more than MO_Q1_MAX_GROUPS keys: ngroups = -1 in the result
+    rc = st.finish();
+    if (rc) return rc;
+    int64_t ngroups;
+    if (is_device_ptr(args[0].pdata)) { rc = read_back(t, &ngroups, args[0].pdata, 8); if (rc) return rc; }
+    else ngroups = ((const mo_q1_result_t *)args[0].pdata)->ngroups;
+    if (ngroups < 0) {
+        set_error("q1: more than %d distinct group keys; the fused small-cardinality kernel does not apply", MO_Q1_MAX_GROUPS);
+        return MO_RC_INVALID_ARGUMENT;
+    }
+    return MO_RC_SUCCESS;
 }
 
 // MO_XCALL_Q6_MERGE: args[0] = result as MO_XCALL_Q6_FILTER_SUM ; args[1] = len partial results of 16 bytes (sum f64, count i64)
