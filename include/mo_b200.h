@@ -395,6 +395,41 @@ typedef struct mo_q1_result_t {
     mo_q1_group_t groups[MO_Q1_MAX_GROUPS];
 } mo_q1_result_t;
 
+/* --- new: fused TPC-H Q6 over DECIMAL(15,2) columns (the reference's own lineitem schema), exact to the digit.
+ * args: [0] result: pdata -> mo_q6_dec_result_t, pnulls (optional) -> nulls word, bit 0 = no row qualified ; [1] shipdate int32 ;
+ * [2] discount ; [3] quantity ; [4] extendedprice (Decimal64 = int64 unscaled, all of one scale) ; [5] params: pdata -> mo_q6_dec_params_t.
+ * The result equals the reference's operator chain: filter (date_lo <= d < date_hi, disc_lo <= discount <= disc_hi, quantity < qty_hi, the
+ * constants already cast to the column scale, so each compare is an int64 compare), Shrink, d64Mul(extendedprice, discount) -> Decimal128 at
+ * scale 2 * scale, SUM with the checked Add128 of sumDecimal128FastExec.  The sum is exact and independent of the summation order.
+ * scale must be 0..4 (every product then keeps its full scale); other scales and columns with a nulls bitmap (the schema's columns are
+ * NOT NULL) are rejected with MO_RC_INVALID_ARGUMENT -- the decimal operator chain (DEC_ARITH, DEC_SUM) serves them.
+ * Errors: the call fails iff one pipeline over the qualifying rows in row order would fail, i.e. the running sum leaves int128 at some row:
+ * rc = MO_RC_INVALID_ARGUMENT ("Decimal128 Add overflow") and err_row = the lowest such row, params.row_base included.  The reference's message names the values, not
+ * the row, and which of several errors it raises first depends on its batch order.  Asynchronous form (device columns AND a device result:
+ * enqueue only) as for Q6_FILTER_SUM: the call returns MO_RC_SUCCESS and the failure is reported in result.rc / result.err_row.
+ * MO_XCALL_Q6_DEC_MERGE (MergeGroup): args [0] result as above ; [1] len partial mo_q6_dec_result_t, folded in order: an empty partial
+ * (count 0) is skipped, a failing partial fails the merge with the lowest err_row of the failing partials (global rows when each range was
+ * scanned with its row_base), the sum is checked as BatchMerge does (an overflow there, or partials of different scales, with no failing
+ * partial: rc = MO_RC_INVALID_ARGUMENT with err_row = -1). */
+#define MO_XCALL_Q6_DEC_FILTER_SUM 0x2004
+#define MO_XCALL_Q6_DEC_MERGE 0x2006
+typedef struct mo_dec128_t { uint64_t lo, hi; } mo_dec128_t;   /* Decimal128: two's complement {B0_63, B64_127} */
+typedef struct mo_q6_dec_params_t {
+    int32_t date_lo, date_hi;           /* date_lo <= d < date_hi */
+    int64_t disc_lo, disc_hi;           /* disc_lo <= discount <= disc_hi (BETWEEN), unscaled at `scale` */
+    int64_t qty_hi;                     /* quantity < qty_hi, unscaled at `scale` */
+    int32_t scale;                      /* scale of the four Decimal64 measures, 0..4 */
+    int32_t reserved;
+    int64_t row_base;                   /* added to err_row: the global row of this range's first row */
+} mo_q6_dec_params_t;
+typedef struct mo_q6_dec_result_t {
+    mo_dec128_t revenue;                /* SUM(l_extendedprice * l_discount), Decimal128 at scale `scale` */
+    int64_t count;                      /* qualifying rows */
+    int64_t err_row;                    /* lowest failing row, -1 when rc == 0 */
+    int32_t rc;                         /* MO_RC_SUCCESS or MO_RC_INVALID_ARGUMENT */
+    int32_t scale;                      /* 2 * params.scale */
+} mo_q6_dec_result_t;
+
 /* --- new: brute-force top-k (GoBruteForceIndex.Search, pkg/vectorindex/brute_force/brute_force.go:248-341).
  * args: [0] result keys int64[nq*k] ; [1] result distances f64[nq*k] ; [2] dataset f32 row-major (dataSz = n*dim*4)
  * ; [3] queries f32 row-major (dataSz = nq*dim*4) ; [4] params: pdata -> mo_search_params_t.  len = nq.

@@ -66,6 +66,8 @@ XCALL_Q6_FILTER_SUM = 0x2000
 XCALL_Q1_GROUP_AGG = 0x2001
 XCALL_Q6_MERGE = 0x2002
 XCALL_Q1_MERGE = 0x2003
+XCALL_Q6_DEC_FILTER_SUM = 0x2004
+XCALL_Q6_DEC_MERGE = 0x2006
 AGG_STATE_BYTES = 24
 XCALL_BRUTEFORCE_TOPK_F32 = 0x3000
 XCALL_IVF_TOPK_F32 = 0x3001
@@ -105,6 +107,18 @@ class XCallArgs(C.Structure):
 class Q6Params(C.Structure):
     _fields_ = [("date_lo", C.c_int32), ("date_hi", C.c_int32), ("disc_lo", C.c_double), ("disc_hi", C.c_double),
                 ("qty_hi", C.c_double)]
+
+
+class Q6DecParams(C.Structure):
+    """mo_q6_dec_params_t: constants unscaled at `scale`, the scale of the four Decimal64 measures, row_base added to err_row"""
+    _fields_ = [("date_lo", C.c_int32), ("date_hi", C.c_int32), ("disc_lo", C.c_int64), ("disc_hi", C.c_int64),
+                ("qty_hi", C.c_int64), ("scale", C.c_int32), ("reserved", C.c_int32), ("row_base", C.c_int64)]
+
+
+class Q6DecResult(C.Structure):
+    """mo_q6_dec_result_t: revenue Decimal128 {lo, hi} at scale `scale`"""
+    _fields_ = [("revenue_lo", C.c_uint64), ("revenue_hi", C.c_uint64), ("count", C.c_int64), ("err_row", C.c_int64),
+                ("rc", C.c_int32), ("scale", C.c_int32)]
 
 
 class Q1Group(C.Structure):

@@ -143,6 +143,14 @@ __device__ __forceinline__ double2 ld_stream16_f64_if(bool pred, const double *p
                  : "=d"(r.x), "=d"(r.y) : "r"((int)pred), "l"(p));
     return r;
 }
+// the int64 twin (Decimal64 columns): 0 where `pred` is false
+__device__ __forceinline__ longlong2 ld_stream16_s64_if(bool pred, const int64_t *p) {
+    longlong2 r;
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\tmov.b64 %0, 0;\n\tmov.b64 %1, 0;\n\t"
+                 "@q ld.global.nc.L1::no_allocate.v2.s64 {%0, %1}, [%3];\n\t}"
+                 : "=l"(r.x), "=l"(r.y) : "r"((int)pred), "l"(p));
+    return r;
+}
 __device__ __forceinline__ void st_stream16(void *p, int4 v) {
     asm volatile("st.global.L1::no_allocate.v4.s32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w));
 }

@@ -38,40 +38,101 @@ constexpr int kThreads = 256;
 // =========================================================================================================
 // Q6
 // =========================================================================================================
-struct Q6Rec { double sum; unsigned long long cnt; };
+typedef unsigned __int128 u128;
+
 // device result (the caller's, or staged for a host result): sum at res[0], qualifying rows at res[1] when res_words >= 2, nulls word
 // bit 0 = "no row qualified" -- the layout MO_XCALL_Q6_MERGE consumes
 struct Q6DevOut { double *res; uint64_t res_words; uint64_t *rnulls; };
 
-// SUM node over one row: the projection l_extendedprice * l_discount is added where the row passed all three conjuncts, +0.0 elsewhere
-// (s starts at +0.0 and can never become -0.0 under round-to-nearest, so s + 0.0 == s)
-__device__ __forceinline__ void q6_add(bool ok, double di, double pr, double &s, unsigned &cnt) {
-    double prod = __dmul_rn(pr, di);             // projection node l_extendedprice * l_discount
-    s = __dadd_rn(s, ok ? prod : 0.0);           // SUM node
+// Value domains of the Q6 scan.  The pair mapping, the conjunct-order loads and the reduction below are shared; a domain supplies the
+// column type, the SUM node over one row and the sum's reduction.
+//   Q6F64  float64 columns: product and every addition rounded as the reference's separate nodes (__dmul_rn / __dadd_rn)
+//   Q6Dec  Decimal64 columns of one scale s <= 4 (int64 unscaled): the exact d64Mul product (Decimal128 at scale 2s, never rounded) summed
+//          modulo 2^128, and the OR of the product magnitudes, whose bit length bounds every running sum (q6_dec_rare)
+struct Q6F64 {
+    typedef double V; typedef double2 V2; typedef double Sum; typedef mo_q6_params_t Params;
+    static __device__ __forceinline__ V2 load2_if(bool p, const V *a) { return ld_stream16_f64_if(p, a); }
+    static __device__ __forceinline__ Sum zero() { return 0.0; }
+    static __device__ __forceinline__ Sum plus(Sum a, Sum b) { return __dadd_rn(a, b); }
+    static __device__ __forceinline__ Sum warp_sum(Sum s) { return warp_sum_f64(s); }
+    // s starts at +0.0 and can never become -0.0 under round-to-nearest, so s + 0.0 == s
+    static __device__ __forceinline__ void add(bool ok, V di, V pr, Sum &s) {
+        double prod = __dmul_rn(pr, di);         // projection node l_extendedprice * l_discount
+        s = __dadd_rn(s, ok ? prod : 0.0);       // SUM node
+    }
+    static __device__ __forceinline__ Sum &odd(Sum &, Sum &s1) { return s1; }
+    static __device__ __forceinline__ void write(Q6DevOut o, Sum f, unsigned long long fc) {
+        if (!o.res) return;
+        o.res[0] = f;
+        if (o.res_words >= 2) reinterpret_cast<long long *>(o.res)[1] = (long long)fc;
+        if (o.rnulls) o.rnulls[0] = fc ? 0ull : 1ull;
+    }
+};
+// mag: OR over the rows of (high word of |product|) | (low word != 0), so |product| < 2^(64 + bit length of mag) -- a bound on every
+// product that costs one 64-bit register
+struct DecSum { u128 s; uint64_t mag; };
+struct Q6Dec {
+    typedef int64_t V; typedef longlong2 V2; typedef DecSum Sum; typedef mo_q6_dec_params_t Params;
+    static __device__ __forceinline__ V2 load2_if(bool p, const V *a) { return ld_stream16_s64_if(p, a); }
+    static __device__ __forceinline__ Sum zero() { return DecSum{0, 0}; }
+    static __device__ __forceinline__ Sum plus(Sum a, Sum b) { return DecSum{a.s + b.s, a.mag | b.mag}; }
+    static __device__ __forceinline__ Sum warp_sum(Sum v) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const uint64_t sl = __shfl_xor_sync(0xffffffffu, (uint64_t)v.s, o), sh = __shfl_xor_sync(0xffffffffu, (uint64_t)(v.s >> 64), o);
+            v.s += ((u128)sh << 64) | sl;
+            v.mag |= __shfl_xor_sync(0xffffffffu, v.mag, o);
+        }
+        return v;
+    }
+    // d64Mul (arith_decimal_fast.go): |pr| * |di| < 2^126, so the 128-bit product is exact; the sign is applied after
+    static __device__ __forceinline__ void add(bool ok, V di, V pr, Sum &s) {
+        const uint64_t ap = pr < 0 ? 0ull - (uint64_t)pr : (uint64_t)pr, ad = di < 0 ? 0ull - (uint64_t)di : (uint64_t)di;
+        const uint64_t lo = ap * ad, hi = __umul64hi(ap, ad);
+        const u128 m = ((u128)hi << 64) | lo;
+        const u128 v = (pr < 0) != (di < 0) ? (u128)0 - m : m;
+        s.s += ok ? v : (u128)0;
+        s.mag |= ok ? (hi | (uint64_t)(lo != 0)) : 0ull;
+    }
+    static __device__ __forceinline__ void write(Q6DevOut, Sum, unsigned long long) {}   // q6_dec_fold_kernel writes the result
+    // integer addition is associative: the odd rows share the even rows' accumulator (the float64 domain keeps two for its fixed order)
+    static __device__ __forceinline__ Sum &odd(Sum &s0, Sum &) { return s0; }
+};
+
+template <class D> struct Q6Rec { typename D::Sum sum; unsigned long long cnt; };
+
+// SUM node over one row: the projection l_extendedprice * l_discount is added where the row passed all three conjuncts, 0 elsewhere
+template <class D>
+__device__ __forceinline__ void q6_add(bool ok, typename D::V di, typename D::V pr, typename D::Sum &s, unsigned &cnt) {
+    D::add(ok, di, pr, s);
     cnt += ok;
 }
-__device__ __forceinline__ void q6_row(const mo_q6_params_t &P, int32_t d, double di, double q, double pr, double &s, unsigned &cnt) {
-    q6_add((d >= P.date_lo) & (d < P.date_hi) & (di >= P.disc_lo) & (di <= P.disc_hi) & (q < P.qty_hi), di, pr, s, cnt);
+template <class D>
+__device__ __forceinline__ void q6_row(const typename D::Params &P, int32_t d, typename D::V di, typename D::V q, typename D::V pr,
+                                       typename D::Sum &s, unsigned &cnt) {
+    q6_add<D>((d >= P.date_lo) & (d < P.date_hi) & (di >= P.disc_lo) & (di <= P.disc_hi) & (q < P.qty_hi), di, pr, s, cnt);
 }
 
 // deterministic reduction of the per-thread state: warp shuffles, shared memory, per-CTA record; the last CTA folds the records in
 // CTA-index order
-__device__ __forceinline__ void q6_finish(double s0, double s1, unsigned cnt, Q6Rec *__restrict__ partials, Q6Rec *__restrict__ out,
-                                          unsigned *ticket, Q6DevOut dres) {
-    double s = __dadd_rn(s0, s1);
+template <class D>
+__device__ __forceinline__ void q6_finish(typename D::Sum s0, typename D::Sum s1, unsigned cnt, Q6Rec<D> *__restrict__ partials,
+                                          Q6Rec<D> *__restrict__ out, unsigned *ticket, Q6DevOut dres) {
+    typedef typename D::Sum Sum;
+    Sum s = D::plus(s0, s1);
     unsigned long long c64 = cnt;
-    s = warp_sum_f64(s);
+    s = D::warp_sum(s);
     c64 = warp_sum(c64);
-    __shared__ double ss[kThreads / 32];
+    __shared__ Sum ss[kThreads / 32];
     __shared__ unsigned long long sc[kThreads / 32];
     __shared__ bool last;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (lane == 0) { ss[warp] = s; sc[warp] = c64; }
     __syncthreads();
     if (threadIdx.x == 0) {
-        double t = 0.0; unsigned long long tc = 0;
+        Sum t = D::zero(); unsigned long long tc = 0;
 #pragma unroll
-        for (int w = 0; w < kThreads / 32; w++) { t = __dadd_rn(t, ss[w]); tc += sc[w]; }
+        for (int w = 0; w < kThreads / 32; w++) { t = D::plus(t, ss[w]); tc += sc[w]; }
         partials[blockIdx.x].sum = t; partials[blockIdx.x].cnt = tc;
         __threadfence();
         unsigned tk = atomicInc(ticket, gridDim.x - 1);
@@ -80,36 +141,33 @@ __device__ __forceinline__ void q6_finish(double s0, double s1, unsigned cnt, Q6
     __syncthreads();
     if (last) {
         __threadfence();
-        double t = 0.0; unsigned long long tc = 0;
-        for (unsigned bIdx = threadIdx.x; bIdx < gridDim.x; bIdx += kThreads) { t = __dadd_rn(t, partials[bIdx].sum); tc += partials[bIdx].cnt; }
-        t = warp_sum_f64(t); tc = warp_sum(tc);
+        Sum t = D::zero(); unsigned long long tc = 0;
+        for (unsigned bIdx = threadIdx.x; bIdx < gridDim.x; bIdx += kThreads) { t = D::plus(t, partials[bIdx].sum); tc += partials[bIdx].cnt; }
+        t = D::warp_sum(t); tc = warp_sum(tc);
         __syncthreads();
         if (lane == 0) { ss[warp] = t; sc[warp] = tc; }
         __syncthreads();
         if (threadIdx.x == 0) {
-            double f = 0.0; unsigned long long fc = 0;
+            Sum f = D::zero(); unsigned long long fc = 0;
 #pragma unroll
-            for (int w = 0; w < kThreads / 32; w++) { f = __dadd_rn(f, ss[w]); fc += sc[w]; }
+            for (int w = 0; w < kThreads / 32; w++) { f = D::plus(f, ss[w]); fc += sc[w]; }
             out->sum = f; out->cnt = fc;
-            if (dres.res) {
-                dres.res[0] = f;
-                if (dres.res_words >= 2) reinterpret_cast<long long *>(dres.res)[1] = (long long)fc;
-                if (dres.rnulls) dres.rnulls[0] = fc ? 0ull : 1ull;
-            }
+            D::write(dres, f, fc);
         }
     }
 }
 
 // Dense scan: all four columns of every pair.  Selected by q6_variant = 1: the arm the selective kernel is timed and tested against.
-template <int UNROLL, int CTAS>
+template <class D, int UNROLL, int CTAS>
 __global__ void __launch_bounds__(kThreads, CTAS)
-q6_kernel(const int32_t *__restrict__ sd, const double *__restrict__ disc, const double *__restrict__ qty,
-          const double *__restrict__ price, uint64_t n, mo_q6_params_t P, Q6Rec *__restrict__ partials,
-          Q6Rec *__restrict__ out, unsigned *ticket, Q6DevOut dres) {
+q6_kernel(const int32_t *__restrict__ sd, const typename D::V *__restrict__ disc, const typename D::V *__restrict__ qty,
+          const typename D::V *__restrict__ price, uint64_t n, typename D::Params P, Q6Rec<D> *__restrict__ partials,
+          Q6Rec<D> *__restrict__ out, unsigned *ticket, Q6DevOut dres) {
+    typedef typename D::V V;
     const uint64_t npairs = n >> 1;
     const uint64_t tid = blockIdx.x * (uint64_t)kThreads + threadIdx.x;
     const uint64_t nthreads = (uint64_t)gridDim.x * kThreads;
-    double s0 = 0.0, s1 = 0.0;
+    typename D::Sum s0 = D::zero(), s1 = D::zero();
     unsigned cnt = 0;  // a thread sees < 2^32 rows
 
     uint64_t p = tid;
@@ -125,22 +183,22 @@ q6_kernel(const int32_t *__restrict__ sd, const double *__restrict__ disc, const
         }
 #pragma unroll
         for (int k = 0; k < UNROLL; k++) {
-            double di[2], qq[2], pr[2];
+            V di[2], qq[2], pr[2];
             memcpy(di, &a[k], 16); memcpy(qq, &b[k], 16); memcpy(pr, &c[k], 16);
-            q6_row(P, d[k].x, di[0], qq[0], pr[0], s0, cnt);
-            q6_row(P, d[k].y, di[1], qq[1], pr[1], s1, cnt);
+            q6_row<D>(P, d[k].x, di[0], qq[0], pr[0], s0, cnt);
+            q6_row<D>(P, d[k].y, di[1], qq[1], pr[1], D::odd(s0, s1), cnt);
         }
     }
     for (; p < npairs; p += nthreads) {
         int2 d = ld_stream8(sd + 2 * p);
         int4 a = ld_stream16(disc + 2 * p), b = ld_stream16(qty + 2 * p), c = ld_stream16(price + 2 * p);
-        double di[2], qq[2], pr[2];
+        V di[2], qq[2], pr[2];
         memcpy(di, &a, 16); memcpy(qq, &b, 16); memcpy(pr, &c, 16);
-        q6_row(P, d.x, di[0], qq[0], pr[0], s0, cnt);
-        q6_row(P, d.y, di[1], qq[1], pr[1], s1, cnt);
+        q6_row<D>(P, d.x, di[0], qq[0], pr[0], s0, cnt);
+        q6_row<D>(P, d.y, di[1], qq[1], pr[1], D::odd(s0, s1), cnt);
     }
-    if ((n & 1) && tid == 0) q6_row(P, sd[n - 1], disc[n - 1], qty[n - 1], price[n - 1], s0, cnt);  // odd tail row
-    q6_finish(s0, s1, cnt, partials, out, ticket, dres);
+    if ((n & 1) && tid == 0) q6_row<D>(P, sd[n - 1], disc[n - 1], qty[n - 1], price[n - 1], s0, cnt);  // odd tail row
+    q6_finish<D>(s0, s1, cnt, partials, out, ticket, dres);
 }
 
 // Selective scan (the default): the columns are read in dependent rounds, in the reference's conjunct order (filter.go:87-153).
@@ -150,16 +208,17 @@ q6_kernel(const int32_t *__restrict__ sd, const double *__restrict__ disc, const
 // rounds run, so a batch costs three round trips.  Merging the quantity and price rounds measured slower for Q6: it reads more.
 // Same grid, pair -> thread mapping, per-thread order and s0 / s1 split as q6_kernel, and a row whose columns were not read adds +0.0
 // exactly as a failing row does there: the result is bit-identical to the dense kernel's.
-template <int UNROLL>
+template <class D, int UNROLL>
 __global__ void __launch_bounds__(kThreads, 4)
-q6_selective_kernel(const int32_t *__restrict__ sd, const double *__restrict__ disc, const double *__restrict__ qty,
-                    const double *__restrict__ price, uint64_t n, mo_q6_params_t P, Q6Rec *__restrict__ partials,
-                    Q6Rec *__restrict__ out, unsigned *ticket, Q6DevOut dres) {
+q6_selective_kernel(const int32_t *__restrict__ sd, const typename D::V *__restrict__ disc, const typename D::V *__restrict__ qty,
+                    const typename D::V *__restrict__ price, uint64_t n, typename D::Params P, Q6Rec<D> *__restrict__ partials,
+                    Q6Rec<D> *__restrict__ out, unsigned *ticket, Q6DevOut dres) {
+    typedef typename D::V V;
     const uint64_t npairs = n >> 1;
     const uint64_t tid = blockIdx.x * (uint64_t)kThreads + threadIdx.x;
     const uint64_t nthreads = (uint64_t)gridDim.x * kThreads;
     const int lane = threadIdx.x & 31;
-    double s0 = 0.0, s1 = 0.0;
+    typename D::Sum s0 = D::zero(), s1 = D::zero();
     unsigned cnt = 0;  // a thread sees < 2^32 rows
 
     // The batched loop runs while the warp's LAST lane has a whole batch, so its trip count is warp-uniform; what is left goes to the
@@ -183,42 +242,42 @@ q6_selective_kernel(const int32_t *__restrict__ sd, const double *__restrict__ d
             for (int k = 0; k < UNROLL; k++) dn[k] = ld_stream8(sd + 2 * (pn + k * nthreads));
         }
         bool m0[UNROLL], m1[UNROLL];   // row still alive
-        double2 a[UNROLL], b[UNROLL], c[UNROLL];
+        typename D::V2 a[UNROLL], b[UNROLL], c[UNROLL];
 #pragma unroll
         for (int k = 0; k < UNROLL; k++) {
             m0[k] = (d[k].x >= P.date_lo) & (d[k].x < P.date_hi);
             m1[k] = (d[k].y >= P.date_lo) & (d[k].y < P.date_hi);
-            a[k] = ld_stream16_f64_if(m0[k] | m1[k], disc + 2 * (p + k * nthreads));
+            a[k] = D::load2_if(m0[k] | m1[k], disc + 2 * (p + k * nthreads));
         }
 #pragma unroll
         for (int k = 0; k < UNROLL; k++) {
             m0[k] = m0[k] & (a[k].x >= P.disc_lo) & (a[k].x <= P.disc_hi);
             m1[k] = m1[k] & (a[k].y >= P.disc_lo) & (a[k].y <= P.disc_hi);
-            b[k] = ld_stream16_f64_if(m0[k] | m1[k], qty + 2 * (p + k * nthreads));
+            b[k] = D::load2_if(m0[k] | m1[k], qty + 2 * (p + k * nthreads));
         }
 #pragma unroll
         for (int k = 0; k < UNROLL; k++) {
             m0[k] = m0[k] & (b[k].x < P.qty_hi);
             m1[k] = m1[k] & (b[k].y < P.qty_hi);
-            c[k] = ld_stream16_f64_if(m0[k] | m1[k], price + 2 * (p + k * nthreads));
+            c[k] = D::load2_if(m0[k] | m1[k], price + 2 * (p + k * nthreads));
         }
 #pragma unroll
-        for (int k = 0; k < UNROLL; k++) {   // a dead row's unread columns are +0.0; it adds +0.0 like any failing row
-            q6_add(m0[k], a[k].x, c[k].x, s0, cnt);
-            q6_add(m1[k], a[k].y, c[k].y, s1, cnt);
+        for (int k = 0; k < UNROLL; k++) {   // a dead row's unread columns are 0; it adds 0 like any failing row
+            q6_add<D>(m0[k], a[k].x, c[k].x, s0, cnt);
+            q6_add<D>(m1[k], a[k].y, c[k].y, D::odd(s0, s1), cnt);
         }
         p = pn;
     }
     for (; p < npairs; p += nthreads) {
         int2 d = ld_stream8(sd + 2 * p);
         int4 a = ld_stream16(disc + 2 * p), b = ld_stream16(qty + 2 * p), c = ld_stream16(price + 2 * p);
-        double di[2], qq[2], pr[2];
+        V di[2], qq[2], pr[2];
         memcpy(di, &a, 16); memcpy(qq, &b, 16); memcpy(pr, &c, 16);
-        q6_row(P, d.x, di[0], qq[0], pr[0], s0, cnt);
-        q6_row(P, d.y, di[1], qq[1], pr[1], s1, cnt);
+        q6_row<D>(P, d.x, di[0], qq[0], pr[0], s0, cnt);
+        q6_row<D>(P, d.y, di[1], qq[1], pr[1], D::odd(s0, s1), cnt);
     }
-    if ((n & 1) && tid == 0) q6_row(P, sd[n - 1], disc[n - 1], qty[n - 1], price[n - 1], s0, cnt);  // odd tail row
-    q6_finish(s0, s1, cnt, partials, out, ticket, dres);
+    if ((n & 1) && tid == 0) q6_row<D>(P, sd[n - 1], disc[n - 1], qty[n - 1], price[n - 1], s0, cnt);  // odd tail row
+    q6_finish<D>(s0, s1, cnt, partials, out, ticket, dres);
 }
 
 // =========================================================================================================
@@ -703,6 +762,141 @@ __global__ void q6_merge_kernel(const double *parts, uint64_t nparts, Q6DevOut o
     if (o.rnulls) o.rnulls[0] = any ? 0ull : 1ull;
 }
 
+// ---- Q6 over Decimal64 ------------------------------------------------------------------------------------------------------------------
+// Running state of one MO_XCALL_Q6_DEC_FILTER_SUM call across its chunks (device scratch, zeroed before the first chunk)
+struct Q6DecRun { u128 sum; unsigned long long mag, cnt, err1; };   // err1 = failing row + 1, 0 = none
+
+// bit length of the largest |product| a DecSum.mag admits
+__device__ __forceinline__ int dec_mag_bits(uint64_t mag) { return mag ? 128 - __clzll((long long)mag) : 0; }
+// z = x + y; true when the checked Add128 fails (decimal.go Add128: equal signs in, the other sign out)
+__device__ __forceinline__ bool add128_overflows(u128 x, u128 y, u128 &z) {
+    z = x + y;
+    const bool sx = (x >> 127) != 0, sy = (y >> 127) != 0, sz = (z >> 127) != 0;
+    return sx == sy && sz != sx;
+}
+__device__ __forceinline__ u128 dec128_get(mo_dec128_t v) { return ((u128)v.hi << 64) | v.lo; }
+__device__ __forceinline__ mo_dec128_t dec128_put(u128 x) { return mo_dec128_t{(uint64_t)x, (uint64_t)(x >> 64)}; }
+
+// row r of a chunk passes the three conjuncts: its d64Mul product in v
+__device__ __forceinline__ bool q6_dec_row(const mo_q6_dec_params_t &P, const int32_t *sd, const int64_t *disc, const int64_t *qty,
+                                           const int64_t *price, uint64_t r, u128 &v) {
+    if (!(sd[r] >= P.date_lo && sd[r] < P.date_hi && disc[r] >= P.disc_lo && disc[r] <= P.disc_hi && qty[r] < P.qty_hi)) return false;
+    DecSum s = Q6Dec::zero();
+    Q6Dec::add(true, disc[r], price[r], s);
+    v = s.s;
+    return true;
+}
+
+// Every running sum of the call is below 2^dec_mag_bits(bound) times the call's row count 2^lg_rows.  While that stays under 2^127 no
+// prefix can overflow (on TPC-H data by more than 30 bits) and the chunk is only folded into the running state.  Otherwise -- the rare
+// path -- the three q6_dec_walk kernels find the first row of the chunk where the row-order running sum, continued from the exact sum of
+// the earlier chunks as the reference's SUM runs it, leaves int128.
+__device__ __forceinline__ bool q6_dec_rare(const Q6DecRun *run, const Q6Rec<Q6Dec> *chunk, int lg_rows) {
+    return !run->err1 && dec_mag_bits(run->mag | chunk->sum.mag) + lg_rows > 127;
+}
+// 192-bit two's complement: an int128 prefix plus fewer than 2^63 products below 2^126 stays inside it
+struct W192 { u128 lo; int64_t hi; };
+__device__ __forceinline__ void w192_add(W192 &w, u128 v) {      // w += v, v a sign-extended int128
+    const u128 z = w.lo + v;
+    w.hi += (int64_t)(z < w.lo) - (int64_t)(v >> 127);
+    w.lo = z;
+}
+__device__ __forceinline__ bool w192_in_i128(const W192 &w) { return w.hi == -(int64_t)(w.lo >> 127); }
+
+constexpr int kWalkCtas = 128, kWalkSegs = kWalkCtas * kThreads;   // contiguous row segments of the rare-path walk, one per thread
+__device__ __forceinline__ void walk_segment(uint64_t m, uint64_t &r, uint64_t &end) {
+    const uint64_t t = blockIdx.x * (uint64_t)kThreads + threadIdx.x, per = (m + kWalkSegs - 1) / kWalkSegs;
+    r = t * per < m ? t * per : m;
+    end = r + per < m ? r + per : m;
+}
+// walk 1: the exact sum of each segment's qualifying products
+__global__ void __launch_bounds__(kThreads)
+q6_dec_walk_sums(const int32_t *sd, const int64_t *disc, const int64_t *qty, const int64_t *price, uint64_t m, mo_q6_dec_params_t P,
+                 const Q6Rec<Q6Dec> *chunk, const Q6DecRun *run, int lg_rows, W192 *seg) {
+    if (!q6_dec_rare(run, chunk, lg_rows)) return;
+    uint64_t r, end;
+    walk_segment(m, r, end);
+    W192 w{0, 0};
+    u128 v;
+    for (; r < end; r++) if (q6_dec_row(P, sd, disc, qty, price, r, v)) w192_add(w, v);
+    seg[blockIdx.x * kThreads + threadIdx.x] = w;
+}
+// walk 2 (one thread): exclusive prefix of the segment sums, from the running sum of the earlier chunks
+__global__ void q6_dec_walk_scan(W192 *seg, const Q6Rec<Q6Dec> *chunk, const Q6DecRun *run, int lg_rows) {
+    if (!q6_dec_rare(run, chunk, lg_rows)) return;
+    W192 acc{run->sum, -(int64_t)(run->sum >> 127)};
+    for (int t = 0; t < kWalkSegs; t++) {
+        const W192 s = seg[t];
+        seg[t] = acc;
+        const u128 lo = acc.lo + s.lo;
+        acc.hi += s.hi + (int64_t)(lo < acc.lo);
+        acc.lo = lo;
+    }
+}
+// walk 3: each segment continues the running sum from its prefix in row order; the lowest row where it leaves int128 fails the call.  A
+// segment whose prefix is already outside int128 holds no first failure: an earlier segment's walk finds it.
+__global__ void __launch_bounds__(kThreads)
+q6_dec_walk_find(const int32_t *sd, const int64_t *disc, const int64_t *qty, const int64_t *price, uint64_t m, uint64_t r0,
+                 mo_q6_dec_params_t P, const W192 *seg, const Q6Rec<Q6Dec> *chunk, const Q6DecRun *run, int lg_rows,
+                 unsigned long long *fail_row) {
+    if (!q6_dec_rare(run, chunk, lg_rows)) return;
+    uint64_t r, end;
+    walk_segment(m, r, end);
+    W192 w = seg[blockIdx.x * kThreads + threadIdx.x];
+    if (!w192_in_i128(w)) return;
+    u128 v;
+    for (; r < end; r++) {
+        if (!q6_dec_row(P, sd, disc, qty, price, r, v)) continue;
+        w192_add(w, v);
+        if (!w192_in_i128(w)) { atomicMin(fail_row, (unsigned long long)(P.row_base + (int64_t)(r0 + r))); return; }
+    }
+}
+
+// After the scan of one chunk (rows [r0, r0 + m) of the call) and its rare-path walk: the chunk's sum (modulo 2^128: exact whenever no
+// prefix overflowed) and the walk's failing row join the running state; after the last chunk (res != NULL) the caller-layout result is written.
+__global__ void q6_dec_fold_kernel(mo_q6_dec_params_t P, const Q6Rec<Q6Dec> *chunk, const unsigned long long *fail_row, Q6DecRun *run,
+                                   mo_q6_dec_result_t *res, uint64_t *rnulls) {
+    Q6DecRun R = *run;
+    if (chunk) {
+        R.mag |= chunk->sum.mag;
+        if (!R.err1 && *fail_row != ~0ull) R.err1 = *fail_row + 1;
+        R.sum += chunk->sum.s;
+        R.cnt += chunk->cnt;
+    }
+    *run = R;
+    if (!res) return;
+    res->revenue = dec128_put(R.sum);
+    res->count = (int64_t)R.cnt;
+    res->err_row = R.err1 ? (int64_t)R.err1 - 1 : -1;
+    res->rc = R.err1 ? MO_RC_INVALID_ARGUMENT : MO_RC_SUCCESS;
+    res->scale = 2 * P.scale;
+    if (rnulls) rnulls[0] = R.cnt ? 0ull : 1ull;
+}
+
+// MergeGroup of Q6_DEC partials in order: empty partials skipped; a failing partial fails the merge with the lowest err_row among the failing
+// partials; otherwise the sum is checked as BatchMerge's Add128 (sum_decimal_fast.go), and an overflow there or a partial of another scale
+// fails the merge with err_row = -1
+__global__ void q6_dec_merge_kernel(const mo_q6_dec_result_t *parts, uint64_t nparts, mo_q6_dec_result_t *res, uint64_t *rnulls) {
+    u128 sum = 0; long long cnt = 0, perr = -1; int prc = MO_RC_SUCCESS, scale = -1; bool bad = false;
+    for (uint64_t p = 0; p < nparts; p++) {
+        const mo_q6_dec_result_t &P = parts[p];
+        if (P.rc != MO_RC_SUCCESS) {
+            if (prc == MO_RC_SUCCESS) prc = P.rc;
+            if (P.err_row >= 0 && (perr < 0 || P.err_row < perr)) perr = P.err_row;
+        }
+        if (P.count == 0) continue;
+        if (scale < 0) scale = P.scale;
+        bad = add128_overflows(sum, dec128_get(P.revenue), sum) || P.scale != scale || bad;
+        cnt += P.count;
+    }
+    res->revenue = dec128_put(sum);
+    res->count = cnt;
+    res->rc = prc != MO_RC_SUCCESS ? prc : (bad ? MO_RC_INVALID_ARGUMENT : MO_RC_SUCCESS);
+    res->err_row = prc != MO_RC_SUCCESS ? perr : -1;
+    res->scale = scale >= 0 ? scale : (nparts ? parts[0].scale : 0);
+    if (rnulls) rnulls[0] = cnt ? 0ull : 1ull;
+}
+
 // kernel choice (MoB200_SetTuning): 0 = chosen from the input; 1 = the reference arm (dense q6_kernel, register q1_kernel)
 int g_q6_variant = 0, g_q1_variant = 0;
 
@@ -735,8 +929,10 @@ static int write_result(ThreadCtx &t, void *dst, const void *src, size_t bytes) 
     return MO_RC_SUCCESS;
 }
 
-static int launch_q6(ThreadCtx &t, const int32_t *sd, const double *disc, const double *qty, const double *price,
-                     uint64_t n, const mo_q6_params_t &P, Q6DevOut dres) {
+// The Q6 scan of one chunk in domain D; the whole-chunk record lands in *rec (arena memory, valid until the caller rewinds the arena)
+template <class D>
+static int launch_q6(ThreadCtx &t, const int32_t *sd, const typename D::V *disc, const typename D::V *qty, const typename D::V *price,
+                     uint64_t n, const typename D::Params &P, Q6DevOut dres, Q6Rec<D> **rec = nullptr) {
     if (!aligned_to(sd, 8) || !aligned_to(disc, 16) || !aligned_to(qty, 16) || !aligned_to(price, 16)) {
         set_error("q6: columns must be 16-byte aligned (int32 column 8-byte)"); return MO_RC_INVALID_ARGUMENT;
     }
@@ -744,13 +940,14 @@ static int launch_q6(ThreadCtx &t, const int32_t *sd, const double *disc, const 
     int grid = num_sms() * 4;
     uint64_t work = (n / 2 + kThreads - 1) / kThreads;
     if ((uint64_t)grid > work) grid = work ? (int)work : 1;
-    Q6Rec *partials = (Q6Rec *)arena_alloc(t, sizeof(Q6Rec) * (size_t)(grid + 1));
+    Q6Rec<D> *partials = (Q6Rec<D> *)arena_alloc(t, sizeof(Q6Rec<D>) * (size_t)(grid + 1));
     if (!partials) return MO_RC_INTERNAL_ERROR;
-    Q6Rec *out = partials + grid;
+    Q6Rec<D> *out = partials + grid;
+    if (rec) *rec = out;
     cudaEventRecord(t.kev0, t.stream);
     switch (variant) {
-    case 1: q6_kernel<4, 4><<<grid, kThreads, 0, t.stream>>>(sd, disc, qty, price, n, P, partials, out, t.ctrl, dres); break;
-    default: q6_selective_kernel<3><<<grid, kThreads, 0, t.stream>>>(sd, disc, qty, price, n, P, partials, out, t.ctrl, dres); break;
+    case 1: q6_kernel<D, 4, 4><<<grid, kThreads, 0, t.stream>>>(sd, disc, qty, price, n, P, partials, out, t.ctrl, dres); break;
+    default: q6_selective_kernel<D, 3><<<grid, kThreads, 0, t.stream>>>(sd, disc, qty, price, n, P, partials, out, t.ctrl, dres); break;
     }
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
@@ -784,8 +981,8 @@ int q6_run(ThreadCtx &t, Stager &st, const uint8_t *const cols[4], uint64_t len,
         const ArenaMark mark = arena_mark(t);
         const void *c[4] = {st.in(cols[0] + 4 * r0, 4 * m), st.in(cols[1] + 8 * r0, 8 * m), st.in(cols[2] + 8 * r0, 8 * m), st.in(cols[3] + 8 * r0, 8 * m)};
         if (st.failed) return MO_RC_INTERNAL_ERROR;
-        const int rc = launch_q6(t, (const int32_t *)c[0], (const double *)c[1], (const double *)c[2], (const double *)c[3], m, P,
-                                 nchunks == 1 ? dres : Q6DevOut{parts + 2 * i, 2, nullptr});
+        const int rc = launch_q6<Q6F64>(t, (const int32_t *)c[0], (const double *)c[1], (const double *)c[2], (const double *)c[3], m, P,
+                                        nchunks == 1 ? dres : Q6DevOut{parts + 2 * i, 2, nullptr});
         if (rc) return rc;
         arena_rewind(t, mark);
     }
@@ -851,6 +1048,106 @@ int xcall_q6(mo_xcall_args_t *args, uint64_t len) {
     if (rc) return rc;
     if (async) { st.release_async(); return MO_RC_SUCCESS; }
     return st.finish();
+}
+
+// The Q6 scan of Decimal64 columns (host or device) into a device mo_q6_dec_result_t.  Chunks as q6_run; while a chunk's columns are still
+// staged, the rare-path walk kernels (which return at once while the magnitude bound holds) check it and q6_dec_fold_kernel folds it into
+// the call's running state in chunk order.
+static int q6_dec_run(ThreadCtx &t, Stager &st, const uint8_t *const cols[4], uint64_t len, const mo_q6_dec_params_t &P,
+                      mo_q6_dec_result_t *res, uint64_t *rnulls) {
+    bool dev;
+    if (!same_residency("q6 dec", cols, 4, &dev)) return MO_RC_INVALID_ARGUMENT;
+    const uint64_t nchunks = scan_chunks(dev, len);
+    Q6DecRun *run = (Q6DecRun *)st.tmp(sizeof(Q6DecRun));
+    unsigned long long *fail_row = (unsigned long long *)st.tmp(8);
+    W192 *seg = (W192 *)st.tmp(sizeof(W192) * kWalkSegs);
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    MOB_CUDA_TRY(cudaMemsetAsync(run, 0, sizeof(Q6DecRun), t.stream));
+    MOB_CUDA_TRY(cudaMemsetAsync(fail_row, 0xff, 8, t.stream));
+    int lg_rows = 0;
+    while (lg_rows < 64 && (1ull << lg_rows) < len) lg_rows++;
+    if (nchunks == 0) {
+        q6_dec_fold_kernel<<<1, 1, 0, t.stream>>>(P, nullptr, fail_row, run, res, rnulls);
+        MOB_LAUNCH_CHECK();
+    }
+    for (uint64_t i = 0; i < nchunks; i++) {
+        const uint64_t r0 = i * kHostChunkRows, m = nchunks == 1 ? len : std::min(kHostChunkRows, len - r0);
+        const ArenaMark mark = arena_mark(t);
+        const void *c[4] = {st.in(cols[0] + 4 * r0, 4 * m), st.in(cols[1] + 8 * r0, 8 * m), st.in(cols[2] + 8 * r0, 8 * m), st.in(cols[3] + 8 * r0, 8 * m)};
+        if (st.failed) return MO_RC_INTERNAL_ERROR;
+        const int32_t *sd = (const int32_t *)c[0];
+        const int64_t *disc = (const int64_t *)c[1], *qty = (const int64_t *)c[2], *price = (const int64_t *)c[3];
+        Q6Rec<Q6Dec> *rec = nullptr;
+        const int rc = launch_q6<Q6Dec>(t, sd, disc, qty, price, m, P, Q6DevOut{nullptr, 0, nullptr}, &rec);
+        if (rc) return rc;
+        q6_dec_walk_sums<<<kWalkCtas, kThreads, 0, t.stream>>>(sd, disc, qty, price, m, P, rec, run, lg_rows, seg);
+        q6_dec_walk_scan<<<1, 1, 0, t.stream>>>(seg, rec, run, lg_rows);
+        q6_dec_walk_find<<<kWalkCtas, kThreads, 0, t.stream>>>(sd, disc, qty, price, m, r0, P, seg, rec, run, lg_rows, fail_row);
+        const bool last = i + 1 == nchunks;
+        q6_dec_fold_kernel<<<1, 1, 0, t.stream>>>(P, rec, fail_row, run, last ? res : nullptr, last ? rnulls : nullptr);
+        MOB_LAUNCH_CHECK();
+        arena_rewind(t, mark);
+    }
+    return MO_RC_SUCCESS;
+}
+
+// rc / err_row of a Q6_DEC result that the synchronous form returns
+static int q6_dec_status(ThreadCtx &t, const void *res, const char *what) {
+    mo_q6_dec_result_t R;
+    if (is_device_ptr(res)) { const int rc = read_back(t, &R, res, sizeof R); if (rc) return rc; }
+    else memcpy(&R, res, sizeof R);
+    if (R.rc == MO_RC_SUCCESS) return MO_RC_SUCCESS;
+    if (R.err_row >= 0) set_error("%s: invalid input: Decimal128 Add overflow at row %lld", what, (long long)R.err_row);
+    else set_error("%s: invalid input: Decimal128 Add overflow or partials of different scales", what);
+    return R.rc;
+}
+
+// MO_XCALL_Q6_DEC_FILTER_SUM: see include/mo_b200.h
+int xcall_q6_dec(mo_xcall_args_t *args, uint64_t len) {
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    if (!args[5].pdata || args[5].dataSz < sizeof(mo_q6_dec_params_t)) { set_error("q6 dec: params missing"); return MO_RC_INVALID_ARGUMENT; }
+    if (!args[0].pdata || args[0].dataSz < sizeof(mo_q6_dec_result_t)) { set_error("q6 dec: result must hold a mo_q6_dec_result_t"); return MO_RC_INVALID_ARGUMENT; }
+    if (args[1].dataSz < 4 * len || args[2].dataSz < 8 * len || args[3].dataSz < 8 * len || args[4].dataSz < 8 * len) {
+        set_error("q6 dec: column shorter than len"); return MO_RC_INVALID_ARGUMENT;
+    }
+    for (int i = 1; i <= 4; i++)
+        if (args[i].pnulls) { set_error("q6 dec: the DECIMAL(15,2) lineitem columns are NOT NULL; column %d has a nulls bitmap", i); return MO_RC_INVALID_ARGUMENT; }
+    mo_q6_dec_params_t P;
+    if (is_device_ptr(args[5].pdata)) { int rc = read_back(t, &P, args[5].pdata, sizeof P); if (rc) return rc; }
+    else memcpy(&P, args[5].pdata, sizeof P);
+    if (P.scale < 0 || P.scale > 4) { set_error("q6 dec: scale %d outside 0..4", (int)P.scale); return MO_RC_INVALID_ARGUMENT; }
+    const bool async = len && is_device_ptr(args[1].pdata) && is_device_ptr(args[0].pdata) && (!args[0].pnulls || is_device_ptr(args[0].pnulls));
+    Stager st(t);
+    mo_q6_dec_result_t *dres = (mo_q6_dec_result_t *)st.out(args[0].pdata, sizeof(mo_q6_dec_result_t));
+    uint64_t *dn = (uint64_t *)st.out(args[0].pnulls, args[0].pnulls ? 8 : 0);
+    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    const uint8_t *cols[4] = {args[1].pdata, args[2].pdata, args[3].pdata, args[4].pdata};
+    int rc = q6_dec_run(t, st, cols, len, P, dres, dn);
+    if (rc) return rc;
+    if (async) { st.release_async(); return MO_RC_SUCCESS; }
+    rc = st.finish();
+    return rc ? rc : q6_dec_status(t, args[0].pdata, "q6 dec");
+}
+
+// MO_XCALL_Q6_DEC_MERGE: args[0] = result as MO_XCALL_Q6_DEC_FILTER_SUM ; args[1] = len partial mo_q6_dec_result_t
+int xcall_q6_dec_merge(mo_xcall_args_t *args, uint64_t len) {
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    if (!args[0].pdata || args[0].dataSz < sizeof(mo_q6_dec_result_t) || args[1].dataSz < sizeof(mo_q6_dec_result_t) * len) {
+        set_error("q6 dec merge: result and partials are mo_q6_dec_result_t"); return MO_RC_INVALID_ARGUMENT;
+    }
+    const bool async = is_device_ptr(args[0].pdata) && (len == 0 || is_device_ptr(args[1].pdata)) && (!args[0].pnulls || is_device_ptr(args[0].pnulls));
+    Stager st(t);
+    const mo_q6_dec_result_t *dparts = (const mo_q6_dec_result_t *)st.in(args[1].pdata, sizeof(mo_q6_dec_result_t) * len);
+    mo_q6_dec_result_t *dres = (mo_q6_dec_result_t *)st.out(args[0].pdata, sizeof(mo_q6_dec_result_t));
+    uint64_t *dn = (uint64_t *)st.out(args[0].pnulls, args[0].pnulls ? 8 : 0);
+    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    q6_dec_merge_kernel<<<1, 1, 0, t.stream>>>(dparts, len, dres, dn);
+    MOB_LAUNCH_CHECK();
+    if (async) { st.release_async(); return MO_RC_SUCCESS; }
+    const int rc = st.finish();
+    return rc ? rc : q6_dec_status(t, args[0].pdata, "q6 dec merge");
 }
 
 // device addresses of the Q1 input columns; the key columns hold packed uint8 values or 24-byte varlena cells

@@ -13,6 +13,8 @@ int xcall_go_elementwise(int64_t funcId, mo_xcall_args_t *args, uint64_t len);
 int xcall_q1(mo_xcall_args_t *args, uint64_t len);
 int xcall_q6_merge(mo_xcall_args_t *args, uint64_t len);
 int xcall_q1_merge(mo_xcall_args_t *args, uint64_t len);
+int xcall_q6_dec(mo_xcall_args_t *args, uint64_t len);
+int xcall_q6_dec_merge(mo_xcall_args_t *args, uint64_t len);
 int xcall_agg_merge(int op, int T, mo_xcall_args_t *args, uint64_t len);
 int xcall_plan(mo_xcall_args_t *args, uint64_t len);
 int xcall_dec_arith(int op, int width, mo_xcall_args_t *args, uint64_t len);
@@ -78,6 +80,8 @@ extern "C" int32_t XCall(int64_t runtimeId, int64_t funcId, uint8_t *errStr, uin
     else if (funcId >= 0x4000 && funcId < 0x5800) rc = xcall_go_elementwise(funcId, a, len);
     else if (funcId == MO_XCALL_Q6_FILTER_SUM) rc = xcall_q6(a, len);
     else if (funcId == MO_XCALL_Q1_GROUP_AGG) rc = xcall_q1(a, len);
+    else if (funcId == MO_XCALL_Q6_DEC_FILTER_SUM) rc = xcall_q6_dec(a, len);
+    else if (funcId == MO_XCALL_Q6_DEC_MERGE) rc = xcall_q6_dec_merge(a, len);
     else if (funcId == MO_XCALL_BRUTEFORCE_TOPK_F32) rc = xcall_bruteforce(a, len);
     else if (funcId == MO_XCALL_IVF_TOPK_F32) rc = xcall_ivf(a, len);
     else if (funcId == MO_XCALL_TOPK_MERGE) rc = xcall_topk_merge(a, len);

@@ -129,6 +129,64 @@ def q6_merge(parts):
     return float(res[0]), int(res.view(np.int64)[1]), bool(rn[0] & np.uint64(1))
 
 
+Q6_DEC_RESULT_BYTES = C.sizeof(capi.Q6DecResult)
+
+
+def q6_dec_result_from_bytes(raw, null_word=None):
+    """mo_q6_dec_result_t bytes -> dict: revenue (Python int, unscaled at `scale`), scale, count, rc, err_row, is_null"""
+    r = capi.Q6DecResult.from_buffer_copy(bytes(raw)[:Q6_DEC_RESULT_BYTES])
+    rev = r.revenue_lo | (r.revenue_hi << 64)
+    return {"revenue": rev - (1 << 128) if rev >> 127 else rev, "scale": r.scale, "count": r.count, "rc": r.rc, "err_row": r.err_row,
+            "is_null": r.count == 0 if null_word is None else bool(int(null_word) & 1)}
+
+
+def _q6_dec_args(rv, shipdate, discount, quantity, extendedprice, n, date_lo, date_hi, disc_lo, disc_hi, qty_hi, scale, row_base):
+    p = capi.Q6DecParams(date_lo, date_hi, disc_lo, disc_hi, qty_hi, scale, 0, row_base)
+    return [rv, _vec(shipdate, n), _vec(discount, n), _vec(quantity, n), _vec(extendedprice, n), _params_vec(p)]
+
+
+def q6_dec_filter_sum(shipdate, discount, quantity, extendedprice, n, date_lo, date_hi, disc_lo, disc_hi, qty_hi, scale, row_base=0):
+    """TPC-H Q6 over DECIMAL columns: shipdate int32 days, the three measures Decimal64 (int64 unscaled) at `scale` (0..4), the constants
+    already unscaled at `scale`.  Returns the q6_dec_result_from_bytes dict; a Decimal128 Add overflow comes back as rc / err_row (the
+    failing row + row_base)."""
+    res = np.zeros(Q6_DEC_RESULT_BYTES, dtype=np.uint8)
+    rn = np.zeros(1, dtype=np.uint64)
+    rc, msg = xcall(capi.XCALL_Q6_DEC_FILTER_SUM, _q6_dec_args(Vector(data=res, nulls=rn, length=1), shipdate, discount, quantity, extendedprice,
+                                                               n, date_lo, date_hi, disc_lo, disc_hi, qty_hi, scale, row_base), n,
+                    raise_on_error=False)
+    if rc not in (0, capi.RC_INVALID_ARGUMENT):
+        raise capi.MoError(rc, msg)
+    out = q6_dec_result_from_bytes(res.tobytes(), rn[0])
+    if rc and out["rc"] == 0:      # rejected before the scan (bad scale, nulls bitmap, short or misaligned column)
+        raise capi.MoError(rc, msg)
+    return out
+
+
+def q6_dec_filter_sum_device(shipdate, discount, quantity, extendedprice, n, date_lo, date_hi, disc_lo, disc_hi, qty_hi, scale, out_ptr,
+                             out_nulls_ptr=None, row_base=0):
+    """asynchronous form: resident columns, mo_q6_dec_result_t written to DEVICE memory at out_ptr, nothing read back or synchronised"""
+    rv = Vector(data_ptr=out_ptr, data_nbytes=Q6_DEC_RESULT_BYTES, nulls_ptr=out_nulls_ptr, length=1)
+    xcall(capi.XCALL_Q6_DEC_FILTER_SUM, _q6_dec_args(rv, shipdate, discount, quantity, extendedprice, n, date_lo, date_hi, disc_lo, disc_hi,
+                                                     qty_hi, scale, row_base), n)
+
+
+def q6_dec_merge(parts_bytes, nparts):
+    """MergeGroup of nparts concatenated mo_q6_dec_result_t, in order -> the q6_dec_result_from_bytes dict"""
+    buf = np.frombuffer(bytes(parts_bytes), dtype=np.uint8).copy()
+    res = np.zeros(Q6_DEC_RESULT_BYTES, dtype=np.uint8)
+    rn = np.zeros(1, dtype=np.uint64)
+    rc, msg = xcall(capi.XCALL_Q6_DEC_MERGE, [Vector(data=res, nulls=rn, length=1), Vector(data=buf, length=nparts)], nparts,
+                    raise_on_error=False)
+    if rc not in (0, capi.RC_INVALID_ARGUMENT):
+        raise capi.MoError(rc, msg)
+    return q6_dec_result_from_bytes(res.tobytes(), rn[0])
+
+
+def q6_dec_merge_device(parts_ptr, nparts, out_ptr, out_nulls_ptr=None):
+    xcall(capi.XCALL_Q6_DEC_MERGE, [Vector(data_ptr=out_ptr, data_nbytes=Q6_DEC_RESULT_BYTES, nulls_ptr=out_nulls_ptr, length=1),
+                                    Vector(data_ptr=parts_ptr, data_nbytes=Q6_DEC_RESULT_BYTES * nparts, length=nparts)], nparts)
+
+
 def _q1_groups(r):
     out = []
     for g in range(r.ngroups):
