@@ -248,7 +248,8 @@ typedef struct { int32_t div0_null; int32_t reserved; int64_t err_row; } mo_go_p
 /* ---- LZ4 block decompression of column blocks (csrc/lz4.cu): compress.Decompress = lz4.UncompressBlock (pkg/compress/compress.go:37-47), one
  * warp per block.  args: [0] dst bytes ; [1] src bytes ; [2] int64[4 * len] descriptors {src_off, src_len, dst_off, dst_len} per block (dst_len = the
  * decoded size the object metadata records; a block that decodes to anything else, or is malformed, fails the call with MO_RC_INVALID_ARGUMENT and
- * the block number in the error text).  len = number of blocks. */
+ * the LOWEST such block number in the error text).  len = number of blocks.  Like the Go decoder, it does not enforce the format's end-of-block
+ * rules (last 5 bytes literals, no match in the last 12): a block that ends in a match decodes by the sequence rules, where liblz4 rejects it. */
 #define MO_XCALL_LZ4_DECODE 0x6030
 /* ---- a decompressed column block -> a resident vector (csrc/vecdecode.cu): Vector.UnmarshalBinary (pkg/container/vector/vector.go:766-819) on the device.
  * args: [0] mo_vector_view_t (out) ; [1] data bytes (out: capacity >= dataLen, aligned) ; [2] area bytes (out) ; [3] nulls uint64 words (out:

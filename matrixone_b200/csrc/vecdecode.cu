@@ -49,7 +49,9 @@ __global__ void vec_parse_kernel(const uint8_t *__restrict__ src, uint64_t n, mo
             else {
                 V.null_count = (int64_t)rd_u64(src + o);
                 const uint64_t bytes = rd_u64(src + o + 16);
-                if (24 + bytes > nsp_len || (bytes & 7)) bad = true;
+                // compared as bytes > nsp_len - 24 (nsp_len >= 24 here): 24 + bytes wraps for a size field near 2^64 and would pass a bitmap
+                // that runs far past its section
+                if (bytes > nsp_len - 24 || (bytes & 7)) bad = true;
                 else { s.words_off = o + 24; s.words_len = bytes / 8; }
             }
         }
