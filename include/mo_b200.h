@@ -128,6 +128,8 @@ typedef struct mo_xcall_args_t {
 #define MO_T_TIME 51
 #define MO_T_DATETIME 52
 #define MO_T_TIMESTAMP 53
+#define MO_T_DECIMAL64 32
+#define MO_T_DECIMAL128 33
 
 /* reference funcIds, cgo/mo.c:49-52 == cxcall.go:33-38.  args: [0] f64 result, [1] vec col, [2] vec col
  * (varlena cells; either side may be const: dataSz == 24).  Semantics of cgo/xcall.c:23-134:
@@ -293,6 +295,31 @@ typedef struct mo_join_params_t { int32_t join_type; int32_t reserved; } mo_join
 #define MO_XCALL_JOIN_FIND 0x6011
 #define MO_XCALL_JOIN_PROBE 0x6012
 #define MO_XCALL_GROUP_AGG(op, T) (0x6400 + ((op) << 8) + (T))
+/* ---- ORDER BY / ORDER BY ... LIMIT (csrc/order.cu): the sels of the Order operator (order.go:103) or the first `limit` of them for Top
+ * (top.go:445); payload columns are then reordered with MO_XCALL_SHUFFLE, as Batch.Shuffle(sels) does.
+ *   args: [0] sels int64[min(limit, len)] (out: indices into this call's rows) ; [1] host mo_order_params_t ; [2 .. 2+nkeys) key columns of
+ *         key[k].col_type (+pnulls; a 1-element vector is a const key) ; [2+nkeys] int64 row ids [len] when has_row_ids.  len = rows (< 2^32).
+ *   limit < 0 or >= len: the whole order; otherwise the first `limit` rows.
+ *   Keys compare left to right as compare.New(type, desc, nullsLast) (pkg/compare/compare.go:24-115): flags = the OrderBySpec flag word
+ *   (MO_ORDER_DESC, MO_ORDER_NULLS_FIRST, MO_ORDER_NULLS_LAST; neither NULLS flag: nullsLast = desc); two NULLs are equal; -0.0 == +0.0; NaN is
+ *   above every number and equal to every NaN.  Ties break by ascending row id (row_ids[i], or the row index; then the row index): a total,
+ *   stable order.  Against the reference (unstable pdqsort in Order, a heap in Top) the output key tuples are identical, and the rows are
+ *   wherever all key tuples are distinct.  Key types: bool, int8-64, uint8-64, float32/64, DATE, TIME, DATETIME, TIMESTAMP, DECIMAL64,
+ *   DECIMAL128.  MergeOrder / MergeTop: each shard's keys gathered with SHUFFLE, its row ids base + sels, all shards in one call with row ids.
+ *   Another type, nkeys outside 1..MO_ORDER_MAX_KEYS, short buffers or len >= 2^32: MO_RC_INVALID_ARGUMENT.  Device sels, key columns, nulls
+ *   and row ids: asynchronous form (enqueue only). */
+#define MO_XCALL_ORDER_SELS 0x6040
+#define MO_ORDER_MAX_KEYS 8
+#define MO_ORDER_DESC 2          /* pkg/pb/plan/plan.pb.go:419-424 */
+#define MO_ORDER_NULLS_FIRST 4
+#define MO_ORDER_NULLS_LAST 8
+typedef struct mo_order_key_t { int32_t col_type; int32_t flags; } mo_order_key_t;
+typedef struct mo_order_params_t {
+    int32_t nkeys;
+    int32_t has_row_ids;
+    int64_t limit;
+    mo_order_key_t key[MO_ORDER_MAX_KEYS];
+} mo_order_params_t;
 
 /* ---- Decimal64 / Decimal128 (csrc/decimal.cu): the reference's native TPC-H column type is DECIMAL(15,2).  Decimal64 = int64 unscaled value,
  * Decimal128 = 16 bytes two's complement {B0_63, B64_127}; scales travel in the parameter block.  Conventions of the Go engine (as GO_ARITH).

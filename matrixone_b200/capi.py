@@ -52,6 +52,20 @@ XCALL_KMEANS_ELKAN_F32, XCALL_KMEANS_ELKAN_F64 = 0x6020, 0x6021
 XCALL_LZ4_DECODE = 0x6030
 XCALL_VECTOR_UNMARSHAL = 0x6031
 JOIN_INNER, JOIN_LEFT, JOIN_SEMI, JOIN_ANTI = 0, 1, 2, 3
+# ORDER BY / ORDER BY ... LIMIT (csrc/order.cu); flags = the planner's OrderBySpec flag word (plan.pb.go:419-424)
+XCALL_ORDER_SELS = 0x6040
+ORDER_MAX_KEYS = 8
+ORDER_DESC, ORDER_NULLS_FIRST, ORDER_NULLS_LAST = 2, 4, 8
+T_DECIMAL64, T_DECIMAL128 = 32, 33
+
+
+class OrderKey(C.Structure):
+    _fields_ = [("col_type", C.c_int32), ("flags", C.c_int32)]
+
+
+class OrderParams(C.Structure):
+    """mo_order_params_t: limit < 0 = the whole order"""
+    _fields_ = [("nkeys", C.c_int32), ("has_row_ids", C.c_int32), ("limit", C.c_int64), ("key", OrderKey * ORDER_MAX_KEYS)]
 
 
 def XCALL_SHUFFLE(szof):

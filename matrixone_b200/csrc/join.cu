@@ -4,8 +4,8 @@
 //   build side   GROUP_IDS over the build keys (IntHashMap insert, first-seen ids) gives vals[i]; JOIN_SELS turns them into the JoinMap's GroupSels:
 //                offsets int32[groupCount + 2], vals int32[n] -- rows of group k (0-based) at vals[offsets[k] .. offsets[k + 1]), ASCENDING row ids,
 //                exactly what GroupSels.Insert + Finalize (joinMapMsg.go:72-125: count, prefix sum, stable scatter) leave behind.
-//                Here: order-preserving compaction of the rows with an id, then a stable LSD radix sort by group id (8 bits per pass, one warp per
-//                1024-row tile ranks with __match_any_sync so equal digits keep their order), offsets from a histogram + exclusive scan.
+//                Here: order-preserving compaction of the rows with an id, then the stable radix sort of order.cu by group id (sort_u32_pairs),
+//                offsets from a histogram + exclusive scan.
 //   probe side   JOIN_FIND = intHashMapIterator.Find (vals[i] = group id or 0; a NULL key never matches, zvals == 0).
 //                JOIN_PROBE = the emission loop of container.probe for the equality-only joins: per probe row the matched build rows in sels order
 //                (unique maps: build row = id - 1), for inner / left outer / left semi / left anti.  Output pairs (probe row, build row | -1) in
@@ -23,13 +23,15 @@
 
 namespace mob {
 
+int sort_u32_pairs(ThreadCtx &t, uint32_t *k0, uint32_t *v0, uint32_t *k1, uint32_t *v1, const uint64_t *m_ptr, uint64_t cap);   // order.cu
+
 namespace {
 
 constexpr int kThreads = 256;
 
-inline unsigned grid_for(uint64_t items, int per_block = kThreads) {
-    uint64_t g = (items + per_block - 1) / per_block;
-    const uint64_t mx = (uint64_t)num_sms() * (per_block == 1 ? 32 : 16);
+inline unsigned grid_for(uint64_t items) {
+    uint64_t g = (items + kThreads - 1) / kThreads;
+    const uint64_t mx = (uint64_t)num_sms() * 16;
     return (unsigned)(g > mx ? mx : (g ? g : 1));
 }
 
@@ -111,52 +113,6 @@ __global__ void __launch_bounds__(kThreads) sels_compact_kernel(const uint64_t *
     for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
         const uint64_t g = groups[i];
         if (g && g <= ngroups) { key[pos[i]] = (uint32_t)(g - 1); row[pos[i]] = (uint32_t)i; }
-    }
-}
-// one radix pass, 8 bits at `shift`: tiles of 1024 items, ONE WARP per tile
-constexpr int kRadixTile = 1024;
-__global__ void __launch_bounds__(32) radix_hist_kernel(const uint32_t *__restrict__ key, const uint64_t *__restrict__ m_ptr, int shift, uint64_t *__restrict__ hist, uint64_t nblocks_cap) {
-    __shared__ unsigned h[256];
-    const uint64_t m = *m_ptr;
-    const uint64_t nblocks = (m + kRadixTile - 1) / kRadixTile;
-    for (uint64_t b = blockIdx.x; b < nblocks_cap; b += gridDim.x) {
-        for (int d = threadIdx.x; d < 256; d += 32) h[d] = 0;
-        __syncwarp();
-        if (b < nblocks) {
-            for (int r = 0; r < kRadixTile / 32; r++) {
-                const uint64_t i = b * kRadixTile + (uint64_t)r * 32 + threadIdx.x;
-                if (i < m) atomicAdd(&h[(key[i] >> shift) & 255u], 1u);
-            }
-        }
-        __syncwarp();
-        for (int d = threadIdx.x; d < 256; d += 32) hist[(uint64_t)d * nblocks_cap + b] = h[d];   // digit-major: the scan orders (digit, tile)
-        __syncwarp();
-    }
-}
-__global__ void __launch_bounds__(32) radix_scatter_kernel(const uint32_t *__restrict__ key, const uint32_t *__restrict__ row, const uint64_t *__restrict__ m_ptr, int shift,
-                                                           const uint64_t *__restrict__ base, uint64_t nblocks_cap, uint32_t *__restrict__ okey, uint32_t *__restrict__ orow) {
-    __shared__ uint64_t run[256];
-    const uint64_t m = *m_ptr;
-    const uint64_t nblocks = (m + kRadixTile - 1) / kRadixTile;
-    const unsigned lane = threadIdx.x;
-    for (uint64_t b = blockIdx.x; b < nblocks; b += gridDim.x) {
-        for (int d = lane; d < 256; d += 32) run[d] = base[(uint64_t)d * nblocks_cap + b];
-        __syncwarp();
-        for (int r = 0; r < kRadixTile / 32; r++) {
-            const uint64_t i = b * kRadixTile + (uint64_t)r * 32 + lane;
-            const bool live = i < m;
-            const uint32_t k = live ? key[i] : 0u, rw = live ? row[i] : 0u;
-            const unsigned d = live ? ((k >> shift) & 255u) : 256u;            // 256: the dead lanes of the last round match only each other
-            const unsigned peers = __match_any_sync(0xffffffffu, d);
-            const unsigned rank = __popc(peers & ((1u << lane) - 1u));
-            uint64_t pos = 0;
-            if (live) pos = run[d] + rank;
-            __syncwarp();
-            if (live && rank == 0) run[d] += __popc(peers);                  // the lowest lane of every digit class advances its cursor
-            __syncwarp();
-            if (live) { okey[pos] = k; orow[pos] = rw; }
-        }
-        __syncwarp();
     }
 }
 __global__ void __launch_bounds__(kThreads) sels_offsets_kernel(const uint64_t *__restrict__ starts, uint64_t ngroups, const uint64_t *__restrict__ total, int32_t *__restrict__ offsets) {
@@ -293,10 +249,8 @@ __global__ void __launch_bounds__(kThreads) probe_emit_kernel(uint64_t n, const 
 int group_rows_stable(ThreadCtx &t, const uint64_t *groups, uint64_t len, uint64_t ngroups, uint64_t **starts, uint32_t **rows, uint64_t **scal_out) {
     uint64_t *flag = (uint64_t *)arena_alloc(t, (len + 1) * 8), *cnt = (uint64_t *)arena_alloc(t, (ngroups + 1) * 8);
     uint32_t *k0 = (uint32_t *)arena_alloc(t, len * 4 + 4), *r0 = (uint32_t *)arena_alloc(t, len * 4 + 4), *k1 = (uint32_t *)arena_alloc(t, len * 4 + 4), *r1 = (uint32_t *)arena_alloc(t, len * 4 + 4);
-    const uint64_t nblocks_cap = (len + kRadixTile - 1) / kRadixTile + 1;
-    uint64_t *hist = (uint64_t *)arena_alloc(t, 256 * nblocks_cap * 8);
     uint64_t *scal = (uint64_t *)arena_alloc(t, 32);     // [0] rows with a group, [1] scratch total, [2] bad flag
-    if (!flag || !cnt || !k0 || !r0 || !k1 || !r1 || !hist || !scal) return MO_RC_INTERNAL_ERROR;
+    if (!flag || !cnt || !k0 || !r0 || !k1 || !r1 || !scal) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(cnt, 0, (ngroups + 1) * 8, t.stream));
     MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, 32, t.stream));
     sels_flag_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(groups, len, ngroups, flag, cnt, (unsigned *)(scal + 2));
@@ -305,23 +259,12 @@ int group_rows_stable(ThreadCtx &t, const uint64_t *groups, uint64_t len, uint64
     if (rc) return rc;
     sels_compact_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(groups, flag, len, ngroups, k0, r0);
     MOB_LAUNCH_CHECK();
-    int bits = 0;
-    while (bits < 32 && (1ull << bits) < ngroups) bits++;
-    uint32_t *ka = k0, *ra = r0, *kb = k1, *rb = r1;
-    for (int shift = 0; shift < bits; shift += 8) {
-        const unsigned g = grid_for(nblocks_cap, 1);
-        radix_hist_kernel<<<g, 32, 0, t.stream>>>(ka, scal, shift, hist, nblocks_cap);
-        MOB_LAUNCH_CHECK();
-        rc = exclusive_scan(t, hist, 256 * nblocks_cap, hist, scal + 1);
-        if (rc) return rc;
-        radix_scatter_kernel<<<g, 32, 0, t.stream>>>(ka, ra, scal, shift, hist, nblocks_cap, kb, rb);
-        MOB_LAUNCH_CHECK();
-        uint32_t *x = ka; ka = kb; kb = x; x = ra; ra = rb; rb = x;
-    }
+    rc = sort_u32_pairs(t, k0, r0, k1, r1, scal, len);                // stable by group id: rows ascending inside every group, in r0
+    if (rc) return rc;
     rc = exclusive_scan(t, cnt, ngroups, cnt, scal + 1);               // cnt[k] -> start of group k
     if (rc) return rc;
     MOB_CUDA_TRY(cudaMemcpyAsync(cnt + ngroups, scal, 8, cudaMemcpyDeviceToDevice, t.stream));   // starts[ngroups] = m
-    *starts = cnt; *rows = ra; *scal_out = scal;
+    *starts = cnt; *rows = r0; *scal_out = scal;
     return MO_RC_SUCCESS;
 }
 

@@ -35,6 +35,7 @@ int xcall_ivf(mo_xcall_args_t *args, uint64_t len);
 int xcall_bruteforce_filtered(mo_xcall_args_t *args, uint64_t len);
 int xcall_ivf_filtered(mo_xcall_args_t *args, uint64_t len);
 int xcall_topk_merge(mo_xcall_args_t *args, uint64_t len);
+int xcall_order_sels(mo_xcall_args_t *args, uint64_t len);
 int tuning_set(const char *name, int value);
 }  // namespace mob
 
@@ -73,6 +74,7 @@ extern "C" int32_t XCall(int64_t runtimeId, int64_t funcId, uint8_t *errStr, uin
     else if (funcId == MO_XCALL_KMEANS_ELKAN_F32 || funcId == MO_XCALL_KMEANS_ELKAN_F64) rc = xcall_kmeans(funcId, a, len);
     else if (funcId == MO_XCALL_JOIN_FIND) rc = xcall_join_find(a, len);
     else if (funcId == MO_XCALL_JOIN_PROBE) rc = xcall_join_probe(a, len);
+    else if (funcId == MO_XCALL_ORDER_SELS) rc = xcall_order_sels(a, len);
     else if (funcId > 0x6100 && funcId <= 0x6100 + 24) rc = xcall_shuffle((int)(funcId - 0x6100), a, len);
     else if (funcId >= 0x6400 && funcId < 0x6400 + (5 << 8)) rc = xcall_group_agg((int)((funcId - 0x6400) >> 8), (int)((funcId - 0x6400) & 0xff), a, len);
     else if (funcId == MO_XCALL_Q6_MERGE) rc = xcall_q6_merge(a, len);

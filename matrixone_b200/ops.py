@@ -551,6 +551,55 @@ def shuffle(src, sels, src_nulls=None, want_nulls=False):
     return (dst, dn) if want_nulls else dst
 
 
+_T_OF_DTYPE = {np.dtype(np.bool_): capi.T_BOOL, np.dtype(np.int8): capi.T_INT8, np.dtype(np.int16): capi.T_INT16,
+               np.dtype(np.int32): capi.T_INT32, np.dtype(np.int64): capi.T_INT64, np.dtype(np.uint8): capi.T_UINT8,
+               np.dtype(np.uint16): capi.T_UINT16, np.dtype(np.uint32): capi.T_UINT32, np.dtype(np.uint64): capi.T_UINT64,
+               np.dtype(np.float32): capi.T_FLOAT32, np.dtype(np.float64): capi.T_FLOAT64}
+
+
+def _order_params(types, flags, limit, has_row_ids):
+    if len(types) != len(flags):
+        raise ValueError("one flag word per key")
+    p = capi.OrderParams()
+    p.nkeys, p.has_row_ids, p.limit = len(types), 1 if has_row_ids else 0, -1 if limit is None else int(limit)
+    for k, (T, f) in enumerate(zip(types[:capi.ORDER_MAX_KEYS], flags)):
+        p.key[k].col_type, p.key[k].flags = int(T), int(f)
+    return p
+
+
+def order_sels(cols, nulls, flags, limit=None, row_ids=None, types=None, length=None):
+    """Order / Top (order.go:103, top.go:445): the row permutation by the key columns, or its first `limit` rows; reorder payload columns
+    with shuffle().  cols: numpy key columns (a 1-element array = const key; DECIMAL128 as uint64[n, 2] {lo, hi}); nulls: per key bitmap
+    words or None; flags: per key ORDER_DESC | ORDER_NULLS_FIRST | ORDER_NULLS_LAST; types: MO_T_* per key (default: from the dtype, so
+    DATE / DECIMAL64 and friends order as their storage type).  row_ids (int64[n]): the merge form -- ties break by them.  Returns int64 sels."""
+    cols = [np.ascontiguousarray(c) for c in cols]
+    types = list(types) if types is not None else [capi.T_DECIMAL128 if c.ndim == 2 else _T_OF_DTYPE[c.dtype] for c in cols]
+    nulls = list(nulls) if nulls is not None else [None] * len(cols)
+    n = length if length is not None else (len(row_ids) if row_ids is not None else max(c.shape[0] for c in cols))
+    nout = n if limit is None or limit < 0 or limit >= n else int(limit)
+    sels = np.zeros(max(nout, 1), dtype=np.int64)
+    vecs = [Vector(data=sels[:nout], length=nout), _params_vec(_order_params(types, flags, limit, row_ids is not None))]
+    for c, nl in zip(cols, nulls):
+        vecs.append(Vector(data=c.view(np.uint8).reshape(-1), nulls=nl, length=c.shape[0]))
+    if row_ids is not None:
+        vecs.append(Vector(data=np.ascontiguousarray(row_ids, dtype=np.int64), length=n))
+    xcall(capi.XCALL_ORDER_SELS, vecs, n)
+    return sels[:nout]
+
+
+def order_sels_device(cols, nulls, types, flags, n, sels_ptr, limit=None, row_ids=None):
+    """asynchronous form on resident vectors (DeviceBuffer key columns, nulls and row ids): enqueues the order and returns; sels_ptr
+    (device, int64[min(limit, n)]) holds the result once the calling thread's stream has run it"""
+    nulls = list(nulls) if nulls is not None else [None] * len(cols)
+    nout = n if limit is None or limit < 0 or limit >= n else int(limit)
+    vecs = [Vector(data_ptr=sels_ptr, data_nbytes=8 * nout, length=nout), _params_vec(_order_params(types, flags, limit, row_ids is not None))]
+    for c, nl in zip(cols, nulls):
+        vecs.append(Vector(data_ptr=c.ptr, data_nbytes=c.nbytes, nulls_ptr=nl.ptr if nl is not None else None, length=n))
+    if row_ids is not None:
+        vecs.append(Vector(data_ptr=row_ids.ptr, data_nbytes=8 * n, length=n))
+    xcall(capi.XCALL_ORDER_SELS, vecs, n)
+
+
 def pack_keys(cols, nulls=None, has_null=True, length=None):
     """fillKeys (inthashmap.go:92-183): <= 8 key bytes per row.  cols: list of fixed-width numpy columns (a 1-element array = const vector).
     Returns (keys uint64[n], skip bitmap words or None)"""
