@@ -130,6 +130,18 @@ typedef struct mo_xcall_args_t {
 #define MO_T_TIMESTAMP 53
 #define MO_T_DECIMAL64 32
 #define MO_T_DECIMAL128 33
+#define MO_T_BIT 11
+#define MO_T_YEAR 55
+#define MO_T_UUID 63
+#define MO_T_ENUM 66
+/* varlena types: 24-byte cells + area (cgo/xcall.h:47-61) */
+#define MO_T_CHAR 60
+#define MO_T_VARCHAR 61
+#define MO_T_BINARY 64
+#define MO_T_VARBINARY 65
+#define MO_T_BLOB 70
+#define MO_T_TEXT 71
+#define MO_T_DATALINK 72
 
 /* reference funcIds, cgo/mo.c:49-52 == cxcall.go:33-38.  args: [0] f64 result, [1] vec col, [2] vec col
  * (varlena cells; either side may be const: dataSz == 24).  Semantics of cgo/xcall.c:23-134:
@@ -305,11 +317,24 @@ typedef struct mo_join_params_t { int32_t join_type; int32_t reserved; } mo_join
  *   above every number and equal to every NaN.  Ties break by ascending row id (row_ids[i], or the row index; then the row index): a total,
  *   stable order.  Against the reference (unstable pdqsort in Order, a heap in Top) the output key tuples are identical, and the rows are
  *   wherever all key tuples are distinct.  Key types: bool, int8-64, uint8-64, float32/64, DATE, TIME, DATETIME, TIMESTAMP, DECIMAL64,
- *   DECIMAL128.  MergeOrder / MergeTop: each shard's keys gathered with SHUFFLE, its row ids base + sels, all shards in one call with row ids.
- *   Another type, nkeys outside 1..MO_ORDER_MAX_KEYS, short buffers or len >= 2^32: MO_RC_INVALID_ARGUMENT.  Device sels, key columns, nulls
- *   and row ids: asynchronous form (enqueue only). */
+ *   DECIMAL128, BIT (uint64), YEAR (int16), ENUM (uint16), UUID (16 bytes compared byte by byte, types.CompareUuid), and the varlena types
+ *   CHAR, VARCHAR, BINARY, VARBINARY, BLOB, TEXT, DATALINK.
+ *   Varlena keys: the argument is what Vector.FillRawPtrLen gives -- pdata = 24-byte cells (dataSz = 24 * len; dataSz == 24 with len != 1 is
+ *   a const key), parea / areaSz = the area.  Values compare as Go's string `<` (bytes.Compare; sort.go varlenaLess, compare/strcompare.go):
+ *   unsigned bytes, a proper prefix sorts first, the empty value below every other.  Cells of NULL rows are never read.  A non-inline cell
+ *   that points outside [0, areaSz), or any non-inline cell when there is no area, fails the call with MO_RC_INVALID_ARGUMENT; the error
+ *   names the key and the lowest such row.  So does a value longer than MO_ORDER_MAX_VARLENA bytes.
+ *   MergeOrder / MergeTop: each shard's keys gathered with SHUFFLE, its row ids base + sels, all shards in one call with row ids.  A varlena
+ *   key of a merge is one cells vector with ONE area: the shards' cells concatenated, the offsets of their non-inline cells rebased into the
+ *   concatenation of their areas (what Vector.UnionBatch produces).  Varlena payload columns are reordered with SHUFFLE(24); its output cells
+ *   still point into the source area, so that area must outlive them.
+ *   Another type, nkeys outside 1..MO_ORDER_MAX_KEYS, short buffers or len >= 2^32: MO_RC_INVALID_ARGUMENT.  Device sels, key columns, nulls,
+ *   areas and row ids: asynchronous form (enqueue only) -- except that a call with varlena keys first reads back one small record (the
+ *   longest value of every varlena key and its lowest bad cell), which synchronises the calling thread's stream once.  Calls with only
+ *   fixed-width keys never synchronise. */
 #define MO_XCALL_ORDER_SELS 0x6040
 #define MO_ORDER_MAX_KEYS 8
+#define MO_ORDER_MAX_VARLENA 65535   /* longest varlena key value in bytes (MatrixOne's VARCHAR limit) */
 #define MO_ORDER_DESC 2          /* pkg/pb/plan/plan.pb.go:419-424 */
 #define MO_ORDER_NULLS_FIRST 4
 #define MO_ORDER_NULLS_LAST 8

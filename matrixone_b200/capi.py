@@ -56,7 +56,12 @@ JOIN_INNER, JOIN_LEFT, JOIN_SEMI, JOIN_ANTI = 0, 1, 2, 3
 XCALL_ORDER_SELS = 0x6040
 ORDER_MAX_KEYS = 8
 ORDER_DESC, ORDER_NULLS_FIRST, ORDER_NULLS_LAST = 2, 4, 8
+ORDER_MAX_VARLENA = 65535
 T_DECIMAL64, T_DECIMAL128 = 32, 33
+T_BIT, T_YEAR, T_UUID, T_ENUM = 11, 55, 63, 66
+# varlena types (24-byte cells + area)
+T_CHAR, T_VARCHAR, T_BINARY, T_VARBINARY, T_BLOB, T_TEXT, T_DATALINK = 60, 61, 64, 65, 70, 71, 72
+T_VARLENA = (T_CHAR, T_VARCHAR, T_BINARY, T_VARBINARY, T_BLOB, T_TEXT, T_DATALINK)
 
 
 class OrderKey(C.Structure):

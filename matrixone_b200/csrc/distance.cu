@@ -27,22 +27,7 @@ constexpr int kThreads = 128;   // 4 warps; every warp owns a shared-memory ring
 
 constexpr unsigned ST_DIM = 1u, ST_AREA = 2u, ST_ZERO = 4u, ST_EMPTY = 8u;
 
-struct Ref { const uint8_t *ptr; uint32_t len; bool ok; };
-
-// varlena decode, cgo/xcall.h:47-61 (== pkg/container/types/bytes.go:61-115)
-__device__ __forceinline__ Ref varlena_ref(const uint8_t *cells, uint64_t i, const uint8_t *area, uint64_t areaSz) {
-    const uint8_t *c = cells + 24 * i;
-    Ref r; r.ok = true;
-    const uint8_t b0 = c[0];
-    if (b0 <= MO_VARLENA_INLINE_SZ) { r.ptr = c + 1; r.len = b0; }
-    else {
-        uint32_t off, len;
-        memcpy(&off, c + 4, 4); memcpy(&len, c + 8, 4);
-        r.ptr = area + off; r.len = len;
-        if (!area || (uint64_t)off + len > areaSz) r.ok = false;
-    }
-    return r;
-}
+using Ref = VarlenaRef;
 
 using namespace mob::godist;
 

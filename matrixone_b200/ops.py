@@ -15,7 +15,7 @@ import ctypes as C
 import numpy as np
 
 from . import capi
-from .vector import DeviceBuffer, Vector, xcall
+from .vector import DeviceBuffer, Vector, varlena_bytes_column, xcall
 
 
 def _vec(x, length=None, itemsize=None):
@@ -571,16 +571,27 @@ def order_sels(cols, nulls, flags, limit=None, row_ids=None, types=None, length=
     """Order / Top (order.go:103, top.go:445): the row permutation by the key columns, or its first `limit` rows; reorder payload columns
     with shuffle().  cols: numpy key columns (a 1-element array = const key; DECIMAL128 as uint64[n, 2] {lo, hi}); nulls: per key bitmap
     words or None; flags: per key ORDER_DESC | ORDER_NULLS_FIRST | ORDER_NULLS_LAST; types: MO_T_* per key (default: from the dtype, so
-    DATE / DECIMAL64 and friends order as their storage type).  row_ids (int64[n]): the merge form -- ties break by them.  Returns int64 sels."""
-    cols = [np.ascontiguousarray(c) for c in cols]
-    types = list(types) if types is not None else [capi.T_DECIMAL128 if c.ndim == 2 else _T_OF_DTYPE[c.dtype] for c in cols]
+    DATE / DECIMAL64 and friends order as their storage type).  A varlena key (CHAR, VARCHAR, TEXT, BLOB ...; its type must be given, or
+    VARCHAR is assumed) is a list of bytes or a (cells, area) pair of uint8 arrays in the vector layout (vector.varlena_bytes_column).
+    row_ids (int64[n]): the merge form -- ties break by them.  Returns int64 sels."""
+    keys = []                                    # (data bytes, area or None, rows)
+    for c in cols:
+        if isinstance(c, list):
+            c = varlena_bytes_column(c)
+        if isinstance(c, tuple):
+            cells, area = np.ascontiguousarray(c[0], dtype=np.uint8).reshape(-1), c[1]
+            keys.append((cells, None if area is None else np.ascontiguousarray(area, dtype=np.uint8), cells.shape[0] // 24, capi.T_VARCHAR))
+        else:
+            c = np.ascontiguousarray(c)
+            keys.append((c.view(np.uint8).reshape(-1), None, c.shape[0], capi.T_DECIMAL128 if c.ndim == 2 else _T_OF_DTYPE.get(c.dtype)))
+    types = list(types) if types is not None else [k[3] for k in keys]
     nulls = list(nulls) if nulls is not None else [None] * len(cols)
-    n = length if length is not None else (len(row_ids) if row_ids is not None else max(c.shape[0] for c in cols))
+    n = length if length is not None else (len(row_ids) if row_ids is not None else max(k[2] for k in keys))
     nout = n if limit is None or limit < 0 or limit >= n else int(limit)
     sels = np.zeros(max(nout, 1), dtype=np.int64)
     vecs = [Vector(data=sels[:nout], length=nout), _params_vec(_order_params(types, flags, limit, row_ids is not None))]
-    for c, nl in zip(cols, nulls):
-        vecs.append(Vector(data=c.view(np.uint8).reshape(-1), nulls=nl, length=c.shape[0]))
+    for (data, area, rows, _), nl in zip(keys, nulls):
+        vecs.append(Vector(data=data, nulls=nl, area=area, length=rows))
     if row_ids is not None:
         vecs.append(Vector(data=np.ascontiguousarray(row_ids, dtype=np.int64), length=n))
     xcall(capi.XCALL_ORDER_SELS, vecs, n)
@@ -589,12 +600,15 @@ def order_sels(cols, nulls, flags, limit=None, row_ids=None, types=None, length=
 
 def order_sels_device(cols, nulls, types, flags, n, sels_ptr, limit=None, row_ids=None):
     """asynchronous form on resident vectors (DeviceBuffer key columns, nulls and row ids): enqueues the order and returns; sels_ptr
-    (device, int64[min(limit, n)]) holds the result once the calling thread's stream has run it"""
+    (device, int64[min(limit, n)]) holds the result once the calling thread's stream has run it.  A varlena key is a (cells, area)
+    pair of DeviceBuffers (area None: every value inline); such a call reads back one small record first, so it synchronises once."""
     nulls = list(nulls) if nulls is not None else [None] * len(cols)
     nout = n if limit is None or limit < 0 or limit >= n else int(limit)
     vecs = [Vector(data_ptr=sels_ptr, data_nbytes=8 * nout, length=nout), _params_vec(_order_params(types, flags, limit, row_ids is not None))]
     for c, nl in zip(cols, nulls):
-        vecs.append(Vector(data_ptr=c.ptr, data_nbytes=c.nbytes, nulls_ptr=nl.ptr if nl is not None else None, length=n))
+        c, area = c if isinstance(c, tuple) else (c, None)
+        vecs.append(Vector(data_ptr=c.ptr, data_nbytes=c.nbytes, nulls_ptr=nl.ptr if nl is not None else None, length=n,
+                           area_ptr=area.ptr if area is not None else None, area_nbytes=area.nbytes if area is not None else 0))
     if row_ids is not None:
         vecs.append(Vector(data_ptr=row_ids.ptr, data_nbytes=8 * n, length=n))
     xcall(capi.XCALL_ORDER_SELS, vecs, n)

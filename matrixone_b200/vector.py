@@ -77,6 +77,30 @@ def varlena_column_from_matrix(mat):
     return cells.view(np.uint8).reshape(-1), mat.view(np.uint8).reshape(-1)
 
 
+def varlena_bytes_column(values):
+    """Build (cells uint8[n*24], area uint8[]) for a list of bytes values (CHAR / VARCHAR / TEXT / BLOB ...), MatrixOne layout; the
+    non-inline values go into the area in row order."""
+    n = len(values)
+    lens = np.fromiter((len(v) for v in values), dtype=np.int64, count=n)
+    flat = np.frombuffer(b"".join(values), dtype=np.uint8)
+    starts = np.cumsum(lens) - lens
+    cells = np.zeros((n, VARLENA_SZ), dtype=np.uint8)
+    inl = lens <= VARLENA_INLINE
+    il = lens[inl]
+    rows = np.repeat(np.flatnonzero(inl), il)
+    j = np.arange(rows.size) - np.repeat(np.cumsum(il) - il, il)
+    cells[rows, 1 + j] = flat[np.repeat(starts[inl], il) + j]
+    cells[inl, 0] = il
+    big = ~inl
+    bl = lens[big]
+    u32 = cells.view(np.uint32)
+    u32[big, 0] = 0xFFFFFFFF
+    u32[big, 1] = (np.cumsum(bl) - bl).astype(np.uint32)
+    u32[big, 2] = bl.astype(np.uint32)
+    area = flat[np.repeat(big, lens)] if bl.size else np.zeros(0, dtype=np.uint8)
+    return cells.reshape(-1), np.ascontiguousarray(area)
+
+
 def varlena_char1_column(chars):
     """char(1)/varchar(1) column (TPC-H l_returnflag / l_linestatus): every cell inline, len 1."""
     chars = np.asarray(chars, dtype=np.uint8)

@@ -1,8 +1,11 @@
 #!/usr/bin/env python
 """ORDER BY / ORDER BY ... LIMIT (MO_XCALL_ORDER_SELS) against torch.sort(stable=True) and torch.topk on the same tensors, and JOIN_SELS on
-this library against another build of it (--other-lib, e.g. the parent commit's), one GPU, one process.
+this library against another build of it (--other-lib, e.g. the parent commit's; the fixed-width orders too, with their launch counts and
+whether the sels are identical), one GPU, one process.  String keys (--only varlena): VARCHAR(25) `Customer#%09d` names (ORDER and Top 100),
+random 8-100-byte TEXT, 1 KB TEXT with and without a common prefix, and the (l_returnflag, l_linestatus) pair, each beside the int64
+torch.sort of the same row count; pyarrow.compute.sort_indices on the CPU when pyarrow is installed.
 
-    python tools/order_bench.py [--rows N ...] [--runs R] [--other-lib PATH]
+    python tools/order_bench.py [--rows N ...] [--runs R] [--other-lib PATH] [--only fixed|varlena]
 
 Every case alternates the library call and its yardstick --runs times after --warmup rounds and reports medians of the time between CUDA
 events on the library's stream (asynchronous form on resident columns, then a synchronise), and G rows/s.  Results are checked once per case:
@@ -82,21 +85,163 @@ def order_case(lib, name, cols, nulls, types, flags, n, limit, yard, runs, warmu
             "lib_grows_s": round(n / lib_t / 1e6, 2), "yardstick_grows_s": round(n / yard_t / 1e6, 2), "checked": ok}
 
 
+def order_ab(libs, name, cols, nulls, types, flags, n, limit, runs, warmup):
+    """one fixed-width order on this build and on --other-lib, alternating: times, launch counts and whether the sels are identical"""
+    nout = n if limit is None else limit
+    outs = {tag: torch.empty(max(nout, 1), dtype=torch.int64, device="cuda") for tag, _ in libs}
+    launches = {}
+
+    def run(tag, L):
+        vecs = [Vector(data_ptr=outs[tag].data_ptr(), data_nbytes=8 * nout, length=nout), ops._params_vec(ops._order_params(types, flags, limit, False))]
+        for c, nl in zip(cols, nulls or [None] * len(cols)):
+            vecs.append(Vector(data_ptr=c.ptr, data_nbytes=c.nbytes, nulls_ptr=nl.ptr if nl is not None else None, length=n))
+        c0 = L.MoB200_KernelLaunchCount()
+        ms = lib_ms(L, lambda: xcall(capi.XCALL_ORDER_SELS, vecs, n, lib=L))
+        launches[tag] = L.MoB200_KernelLaunchCount() - c0
+        return ms
+    (t0, L0), (t1, L1) = libs
+    a, b = alternate(runs, warmup, lambda: run(t0, L0), lambda: run(t1, L1))
+    same = bool(torch.equal(outs[t0][:nout], outs[t1][:nout]))
+    del outs
+    torch.cuda.empty_cache()
+    return {"case": name, "rows": n, "limit": limit, "this_ms": round(a, 3), "other_ms": round(b, 3), "this_launches": launches[t0],
+            "other_launches": launches[t1], "identical_sels": same}
+
+
+def customer_cells(ids):
+    """VARCHAR(25) 'Customer#%09d' names as inline 24-byte cells, built on the device"""
+    n = ids.numel()
+    cells = torch.zeros((n, 24), dtype=torch.uint8, device="cuda")
+    cells[:, 0] = 18
+    cells[:, 1:10] = torch.tensor(list(b"Customer#"), dtype=torch.uint8, device="cuda")
+    d = ids.clone()
+    for j in range(9):
+        cells[:, 18 - j] = (48 + d % 10).to(torch.uint8)
+        d //= 10
+    return cells
+
+
+def area_cells(lens):
+    """non-inline cells over one area: row i's value at offset sum(lens[:i]) mod 2^32 (the cell's offset field has 32 bits, so rows past
+    4 GB of area read bytes of earlier rows; every cell stays inside the area), length lens[i]"""
+    n = lens.numel()
+    cells = torch.zeros((n, 6), dtype=torch.int32, device="cuda")
+    cells[:, 0] = -1
+    cells[:, 1] = (torch.cumsum(lens, 0) - lens).to(torch.int32)
+    cells[:, 2] = lens.to(torch.int32)
+    return cells.view(torch.uint8)
+
+
+def varlena_cases(lib, res, a, g):
+    """string keys: each case against the int64 torch.sort of the same row count, for scale"""
+    def int64_sort(n):
+        k = torch.randint(-2 ** 62, 2 ** 62, (n,), device="cuda", generator=g)
+        return k, lambda: torch.sort(k, stable=True)
+
+    def case(name, cols, types, flags, n, limit=None, check=None):
+        k, yard = int64_sort(n)
+        r = order_case(lib, name, cols, None, types, flags, n, limit, yard, a.runs, a.warmup, check)
+        r["yardstick"] = "torch.sort int64, %d rows" % n
+        res["cases"].append(r)
+        del k
+
+    n = a.varlena_rows
+    ids = torch.randperm(n, device="cuda", generator=g) + 1
+    cells = customer_cells(ids)
+    want = torch.sort(ids, stable=True)[1]
+    case("varchar25_customer_names", [(Dev(cells), None)], [capi.T_VARCHAR], [0], n, check=lambda s: bool(torch.equal(s, want)))
+    case("varchar25_customer_names_top100", [(Dev(cells), None)], [capi.T_VARCHAR], [0], n, limit=100, check=lambda s: bool(torch.equal(s, want[:100])))
+    del ids, cells, want
+    torch.cuda.empty_cache()
+
+    lens = torch.randint(8, 101, (n,), device="cuda", generator=g)
+    area = torch.randint(0, 256, (int(lens.sum()),), device="cuda", dtype=torch.uint8, generator=g)
+    cells = area_cells(lens)
+    case("text_random_8_100_bytes", [(Dev(cells), Dev(area))], [capi.T_TEXT], [0], n)
+    del lens, area, cells
+    torch.cuda.empty_cache()
+
+    n1k = a.kb_rows
+    for prefix in (0, 16):
+        area = torch.randint(0, 256, (n1k, 1000), device="cuda", dtype=torch.uint8, generator=g)
+        if prefix:
+            area[:, :prefix] = 0x41
+        cells = area_cells(torch.full((n1k,), 1000, device="cuda", dtype=torch.int64))
+        area = area.reshape(-1)
+        case("text_1kb_common_prefix_%d" % prefix, [(Dev(cells), Dev(area))], [capi.T_TEXT], [0], n1k)
+        del area, cells
+        torch.cuda.empty_cache()
+
+    n = a.flag_rows
+    rf = torch.zeros((n, 24), dtype=torch.uint8, device="cuda")
+    ls = torch.zeros((n, 24), dtype=torch.uint8, device="cuda")
+    rf[:, 0] = 1
+    ls[:, 0] = 1
+    rf[:, 1] = torch.tensor(list(b"ANR"), dtype=torch.uint8, device="cuda")[torch.randint(0, 3, (n,), device="cuda", generator=g)]
+    ls[:, 1] = torch.tensor(list(b"FO"), dtype=torch.uint8, device="cuda")[torch.randint(0, 2, (n,), device="cuda", generator=g)]
+    case("returnflag_linestatus", [(Dev(rf), None), (Dev(ls), None)], [capi.T_VARCHAR, capi.T_VARCHAR], [0, 0], n)
+    del rf, ls
+    torch.cuda.empty_cache()
+    res["pyarrow"] = pyarrow_sort(a.varlena_rows // 10)
+
+
+def pyarrow_sort(n):
+    """pyarrow.compute.sort_indices over Customer#%09d strings on the CPU, when pyarrow is installed"""
+    try:
+        import time
+
+        import numpy as np
+        import pyarrow as pa
+        import pyarrow.compute as pc
+    except ImportError:
+        return "not installed"
+    ids = np.random.default_rng(1).permutation(n) + 1
+    arr = pa.array(np.char.add("Customer#", np.char.zfill(ids.astype(str), 9)))
+    t0 = time.perf_counter()
+    pc.sort_indices(arr)
+    return {"case": "varchar25_customer_names", "rows": n, "ms": round((time.perf_counter() - t0) * 1e3, 1)}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, nargs="+", default=[100_000_000, 600_000_000])
     ap.add_argument("--top-rows", type=int, default=600_000_000)
     ap.add_argument("--join-rows", type=int, default=100_000_000)
+    ap.add_argument("--varlena-rows", type=int, default=100_000_000)
+    ap.add_argument("--kb-rows", type=int, default=10_000_000, help="rows of the 1 KB TEXT cases")
+    ap.add_argument("--flag-rows", type=int, default=600_000_000, help="rows of the (l_returnflag, l_linestatus) case")
     ap.add_argument("--runs", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--other-lib", default=None, help="another build of libmo_b200.so to time JOIN_SELS against")
+    ap.add_argument("--other-lib", default=None, help="another build of libmo_b200.so to time JOIN_SELS and the fixed-width orders against")
+    ap.add_argument("--only", choices=["fixed", "varlena"], default=None)
     a = ap.parse_args()
     lib = capi.load_library()
     capi.check(lib.MoB200_Init(0), lib)
     name, power = card()
     res = {"card": name, "power_limit": power, "runs": a.runs, "cases": []}
     g = torch.Generator(device="cuda").manual_seed(1)
+    if a.only != "fixed":
+        varlena_cases(lib, res, a, g)
+        if a.only == "varlena":
+            print(json.dumps(res))
+            return
+    if a.other_lib:
+        other = capi.load_library(a.other_lib)
+        capi.check(other.MoB200_Init(0), other)
+        ab = [("this", lib), ("other", other)]
+        res["fixed_width_ab"] = []
     for n in a.rows:
+        if a.other_lib:
+            k = torch.randint(-2 ** 62, 2 ** 62, (n,), device="cuda", generator=g)
+            s = torch.randint(0, 1000, (n,), device="cuda", generator=g)
+            d = torch.randint(8000, 11000, (n,), device="cuda", dtype=torch.int32, generator=g)
+            res["fixed_width_ab"].append(order_ab(ab, "int64_uniform", [Dev(k)], None, [capi.T_INT64], [0], n, None, a.runs, a.warmup))
+            res["fixed_width_ab"].append(order_ab(ab, "int64_small_range", [Dev(s)], None, [capi.T_INT64], [0], n, None, a.runs, a.warmup))
+            res["fixed_width_ab"].append(order_ab(ab, "date_desc_int64", [Dev(d), Dev(k)], None, [capi.T_DATE, capi.T_INT64], [capi.ORDER_DESC, 0], n,
+                                                  None, a.runs, a.warmup))
+            res["fixed_width_ab"].append(order_ab(ab, "top100_int64", [Dev(k)], None, [capi.T_INT64], [0], n, 100, a.runs, a.warmup))
+            del k, s, d
+            torch.cuda.empty_cache()
         for kind in ("uniform", "small_range"):
             k = torch.randint(-2 ** 62, 2 ** 62, (n,), device="cuda", generator=g) if kind == "uniform" else torch.randint(0, 1000, (n,), device="cuda", generator=g)
             yard = lambda: torch.sort(k, stable=True)  # noqa: E731
