@@ -306,6 +306,41 @@ typedef struct mo_join_params_t { int32_t join_type; int32_t reserved; } mo_join
 #define MO_XCALL_JOIN_SELS 0x6010
 #define MO_XCALL_JOIN_FIND 0x6011
 #define MO_XCALL_JOIN_PROBE 0x6012
+/* ---- byte-string keys: StrHashMap (pkg/common/hashmap/strhashmap.go), for keys wider than 8 bytes and for varlena keys (csrc/colops.cu,
+ * csrc/join.cu).  A key is a byte string; two rows are in one group exactly when their key bytes are equal (the reference compares 192-bit
+ * hashes of them), so -0.0 and +0.0 are two groups and NaN payloads stay distinct.
+ *   PACK_STR_KEYS    strHashmapIterator.encodeHashKeys (strhashmap.go:92-385): per row the concatenation over the key columns of -- fixed width:
+ *                    [0x00 marker when has_null] + the value's storage bytes ; varlena (CHAR, VARCHAR, BINARY, VARBINARY, BLOB, TEXT, DATALINK):
+ *                    [0x00 marker when has_null] + uint16 little-endian length + the bytes ; NULL: 0x01 alone when has_null, else the row joins no
+ *                    group (empty key, bit set in args[1].pnulls).  The reference pads keys shorter than 16 bytes with zeros; the codes are
+ *                    self-delimiting, so the padding never makes two keys equal and is left out.  The ROLLUP marker 0x02 is not built.
+ *                    args: [0] key bytes u8[cap] (out) ; [1] offsets uint64[len + 1] (out: row i's key is bytes[off[i], off[i + 1]); +pnulls out,
+ *                    has_null = 0 only: rows that join no group) ; [2] host mo_strkey_params_t ; [3 .. 3+ncols) key columns of col_type[k]: fixed
+ *                    width (the key types of ORDER_SELS, by storage size) or varlena cells + area as ORDER_SELS takes them (+pnulls; one element =
+ *                    const).  cap too small: MO_RC_OUT_OF_RANGE and off[len] = the bytes needed.  A cell outside its area or a value longer than
+ *                    MO_ORDER_MAX_VARLENA bytes: MO_RC_INVALID_ARGUMENT naming the column and its lowest such row.  Reads back one record (the byte
+ *                    total, the lowest bad cell per column): one synchronise.
+ *   STR_GROUP_IDS    StrHashMap insert as Group.buildOneBatch drives it (exec2.go:325-362): GROUP_IDS over byte-string keys, 1-based ids in
+ *                    first-seen order, persisting across calls through (ngroups, table bytes, table offsets), which the caller owns.
+ *                    args: [0] groups uint64[len] ; [1] int64 ngroups (in/out) ; [2] table bytes u8[cap_bytes] ; [3] table offsets
+ *                    uint64[cap_groups + 1]: group g is bytes[off[g - 1], off[g]) (off[0] = 0 for an empty table; in: groups 1..ngroups, out: + the
+ *                    new groups) ; [4] key bytes ; [5] key offsets uint64[len + 1] (PACK_STR_KEYS's; +pnulls: those rows get id 0) ; [6] first rows
+ *                    int64[len] (out, pdata NULL when not wanted): the batch row that created each new group, in id order.  More groups or bytes
+ *                    than the table holds: MO_RC_INVALID_ARGUMENT stating both capacities needed, with ngroups and the table untouched -- grow the
+ *                    table and repeat the call.  len + ngroups < 2^31.  Reads back its overflow record (a device ngroups is read first, as GROUP_IDS does).
+ *   STR_JOIN_FIND    strHashmapIterator.Find: vals[i] = 1-based id of probe key i in a table STR_GROUP_IDS built, 0 = absent or skipped.
+ *                    args: [0] vals uint64[len] ; [1] host int64 ngroups ; [2] table bytes ; [3] table offsets ; [4] probe key bytes ; [5] probe key
+ *                    offsets (+pnulls).  The device table is rebuilt per call (O(build groups)) unless MoB200_StrJoinMapPrepare cached it, keyed by
+ *                    the table offsets pointer.  Device pointers: enqueue only.
+ *   JOIN_PROBE_GIDS  JOIN_PROBE with each probe row's group id given (JOIN_FIND's or STR_JOIN_FIND's vals) instead of its key: the same pairs, in
+ *                    the same order.  args [0..3], [5], [6] as JOIN_PROBE ; [4] host int64 ngroups ; [7] vals uint64[len] (an id above ngroups:
+ *                    MO_RC_INVALID_ARGUMENT). */
+#define MO_XCALL_PACK_STR_KEYS 0x6003
+#define MO_XCALL_STR_GROUP_IDS 0x6004
+#define MO_XCALL_STR_JOIN_FIND 0x6013
+#define MO_XCALL_JOIN_PROBE_GIDS 0x6014
+#define MO_STRKEY_MAX_COLS 8
+typedef struct mo_strkey_params_t { int32_t ncols; int32_t has_null; int32_t col_type[MO_STRKEY_MAX_COLS]; } mo_strkey_params_t;
 #define MO_XCALL_GROUP_AGG(op, T) (0x6400 + ((op) << 8) + (T))
 /* ---- ORDER BY / ORDER BY ... LIMIT (csrc/order.cu): the sels of the Order operator (order.go:103) or the first `limit` of them for Top
  * (top.go:445); payload columns are then reordered with MO_XCALL_SHUFFLE, as Batch.Shuffle(sels) does.
@@ -563,7 +598,9 @@ int32_t MoB200_ColumnCacheStats(uint64_t *hits, uint64_t *misses, uint64_t *byte
 /* prepared join maps: build the probe-side device hash table of a JoinMap once (the JoinMap message lives for the whole probe phase,
  * pkg/vm/message/joinMapMsg.go:127-160); JOIN_FIND / JOIN_PROBE calls whose table_keys pointer equals `table_keys` reuse it. */
 int32_t MoB200_JoinMapPrepare(const void *table_keys, uint64_t ngroups);
-int32_t MoB200_JoinMapRelease(const void *table_keys);
+/* the same for a STR_GROUP_IDS table (copied to the device): STR_JOIN_FIND calls whose table offsets pointer equals `table_offsets` reuse it */
+int32_t MoB200_StrJoinMapPrepare(const void *table_bytes, const void *table_offsets, uint64_t ngroups);
+int32_t MoB200_JoinMapRelease(const void *table_keys);   /* either kind: table_keys, or the table_offsets of a string map */
 int32_t MoB200_Sync(void);                    /* synchronize the calling thread's stream */
 int32_t MoB200_SetStream(void *cuda_stream);  /* adopt an external cudaStream_t for the calling thread (NULL = own) */
 int32_t MoB200_TimerStart(void);              /* CUDA event on the calling thread's stream */
@@ -573,7 +610,9 @@ int32_t MoB200_LastKernelMs(float *ms);       /* device time of the dominant ker
 int32_t MoB200_LastError(char *buf, uint64_t buflen);  /* thread-local last error text */
 int32_t MoB200_FlushL2(void);                 /* write a >L2-sized scratch buffer (bench hygiene) */
 int32_t MoB200_SetTuning(const char *name, int32_t value);  /* kernel-variant knobs used by tools/tune.py; returns 0 if name and value are known, else -1
-                                                             * (search_filter_path: 0 auto, 1 masked scan, 2 compacted admitted rows) */
+                                                             * (search_filter_path: 0 auto, 1 masked scan, 2 compacted admitted rows;
+                                                             * strkey_hash_bits, test only: string-key hashes keep their low 1..63 bits, 0 = all,
+                                                             * so that hash tags collide and the key byte compare is exercised) */
 
 /* synthetic column generators used by bench.py / tests (counter-based, reproducible on the host: see
  * matrixone_b200/datagen.py).  All write DEVICE memory, rows [row0, row0+n). */

@@ -52,6 +52,15 @@ XCALL_KMEANS_ELKAN_F32, XCALL_KMEANS_ELKAN_F64 = 0x6020, 0x6021
 XCALL_LZ4_DECODE = 0x6030
 XCALL_VECTOR_UNMARSHAL = 0x6031
 JOIN_INNER, JOIN_LEFT, JOIN_SEMI, JOIN_ANTI = 0, 1, 2, 3
+# byte-string keys (StrHashMap): encoder, group ids, join lookup, and the join emission over given group ids
+XCALL_PACK_STR_KEYS, XCALL_STR_GROUP_IDS = 0x6003, 0x6004
+XCALL_STR_JOIN_FIND, XCALL_JOIN_PROBE_GIDS = 0x6013, 0x6014
+STRKEY_MAX_COLS = 8
+
+
+class StrKeyParams(C.Structure):
+    """mo_strkey_params_t: col_type = MO_T_* per key column"""
+    _fields_ = [("ncols", C.c_int32), ("has_null", C.c_int32), ("col_type", C.c_int32 * STRKEY_MAX_COLS)]
 # ORDER BY / ORDER BY ... LIMIT (csrc/order.cu); flags = the planner's OrderBySpec flag word (plan.pb.go:419-424)
 XCALL_ORDER_SELS = 0x6040
 ORDER_MAX_KEYS = 8
@@ -184,6 +193,7 @@ PROTOTYPES = {
     "MoB200_ColumnCacheConfigure": (_i32, [_u64]), "MoB200_ColumnPin": (_i32, [_vp, _u64, _u64]), "MoB200_ColumnUnpin": (_i32, [_vp]),
     "MoB200_ColumnCacheStats": (_i32, [C.POINTER(_u64), C.POINTER(_u64), C.POINTER(_u64)]),
     "MoB200_JoinMapPrepare": (_i32, [_vp, _u64]), "MoB200_JoinMapRelease": (_i32, [_vp]),
+    "MoB200_StrJoinMapPrepare": (_i32, [_vp, _vp, _u64]),
     "MoB200_DownloadAsync": (_i32, [_vp, _vp, _u64]), "MoB200_UploadAsync": (_i32, [_vp, _vp, _u64]),
     "MoB200_Sync": (_i32, []), "MoB200_SetStream": (_i32, [_vp]), "MoB200_TimerStart": (_i32, []),
     "MoB200_TimerStop": (_i32, [C.POINTER(C.c_float)]), "MoB200_KernelLaunchCount": (_u64, []), "MoB200_LastKernelMs": (_i32, [C.POINTER(C.c_float)]),

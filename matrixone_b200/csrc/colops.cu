@@ -7,6 +7,8 @@
 //   MO_XCALL_PACK_KEYS        intHashMapIterator.encodeHashKeys / fillKeys (<= 8 key bytes)       pkg/common/hashmap/inthashmap.go:92-183
 //   MO_XCALL_GROUP_IDS        IntHashMap insert: 1-based group ids in FIRST-SEEN order            pkg/common/hashmap/iterator.go:127-148,
 //                                                                                                 pkg/container/hashtable/int64_hash_map.go:92-158
+//   MO_XCALL_PACK_STR_KEYS    strHashmapIterator.encodeHashKeys (byte-string keys)                pkg/common/hashmap/strhashmap.go:92-385
+//   MO_XCALL_STR_GROUP_IDS    StrHashMap insert: GROUP_IDS over byte-string keys                  pkg/container/hashtable/string_hash_map.go:97-158
 //   MO_XCALL_GROUP_AGG(op,T)  sumAvgExec / countColumnExec / minMaxExecFixed .BatchFill           pkg/sql/colexec/aggexec/{sumavg2,count2,minmax2}.go
 //
 // These are what the fused plans (tpch.cu, plan.cu) are built from; exposed on their own they make every operator of the chain
@@ -14,7 +16,13 @@
 // ballots for bitmaps, a single-pass decoupled look-back scan for the order-preserving compaction.
 #include "common.cuh"
 #include "keytable.cuh"
+#include "varlena.cuh"
 #include <cstring>
+
+namespace mob {
+int exclusive_scan(ThreadCtx &t, const uint64_t *in, uint64_t n, uint64_t *out, uint64_t *total);   // join.cu
+int g_strkey_hash_bits = 0;
+}
 
 using namespace mob;
 
@@ -179,6 +187,66 @@ pack_keys_kernel(uint64_t *__restrict__ keys, uint32_t *__restrict__ skip32, uin
 }
 
 // =========================================================================================================
+// byte-string keys (strHashmapIterator.encodeHashKeys): per column [marker byte (has_null mode)] + the value's storage bytes, or for a varlena
+// column its uint16 little-endian length + its bytes; a NULL is the marker 1 alone (has_null) or makes the row's key empty and skipped
+// =========================================================================================================
+static_assert(MO_STRKEY_MAX_COLS <= MO_ORDER_MAX_KEYS, "one VarlenaStat entry per key column");
+struct StrKeyCols {
+    const uint8_t *col[MO_STRKEY_MAX_COLS]; const uint64_t *nulls[MO_STRKEY_MAX_COLS]; const uint8_t *area[MO_STRKEY_MAX_COLS];
+    uint64_t area_sz[MO_STRKEY_MAX_COLS]; int size[MO_STRKEY_MAX_COLS] /* 0 = varlena cells */; int cst[MO_STRKEY_MAX_COLS]; int n;
+};
+
+// the length of row i's key; its bytes too when out is set.  skip = a NULL in has_null = 0 mode (the key is then empty).
+__device__ __forceinline__ uint64_t strkey_row(const StrKeyCols &K, uint64_t i, int has_null, uint8_t *out, bool &skip) {
+    uint64_t off = 0;
+    skip = false;
+    for (int k = 0; k < K.n; k++) {
+        const uint64_t r = K.cst[k] ? 0 : i;
+        const bool isnull = bm_test(K.nulls[k], r);
+        if (has_null) {
+            if (out) out[off] = isnull ? 1 : 0;
+            off++;
+            if (isnull) continue;
+        } else if (isnull) { skip = true; return 0; }
+        if (K.size[k]) {
+            const uint8_t *p = K.col[k] + r * (uint64_t)K.size[k];
+            if (out) for (int b = 0; b < K.size[k]; b++) out[off + b] = p[b];
+            off += K.size[k];
+        } else {
+            const VarlenaRef v = varlena_ref(K.col[k], r, K.area[k], K.area_sz[k]);
+            if (out) {
+                out[off] = (uint8_t)v.len; out[off + 1] = (uint8_t)(v.len >> 8);
+                for (uint32_t b = 0; b < v.len; b++) out[off + 2 + b] = v.ptr[b];
+            }
+            off += 2 + (uint64_t)v.len;
+        }
+    }
+    return off;
+}
+
+__global__ void __launch_bounds__(kThreads)
+strkey_len_kernel(StrKeyCols K, uint64_t n, int has_null, uint64_t *__restrict__ lens, uint32_t *__restrict__ skip32) {
+    const uint64_t n64 = (n + 63) & ~63ull;
+    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n64; i += (uint64_t)gridDim.x * kThreads) {
+        bool skip = false;
+        if (i < n) lens[i] = strkey_row(K, i, has_null, nullptr, skip);
+        if (skip32) {
+            const unsigned m = __ballot_sync(0xffffffffu, skip);
+            if ((threadIdx.x & 31) == 0) skip32[i >> 5] = m;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kThreads)
+strkey_write_kernel(StrKeyCols K, uint64_t n, int has_null, const uint64_t *__restrict__ off, uint8_t *__restrict__ bytes) {
+    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
+        if (off[i + 1] == off[i]) continue;   // a skipped row (every other key has at least one byte): it must not write the columns before its NULL
+        bool skip;
+        strkey_row(K, i, has_null, bytes + off[i], skip);
+    }
+}
+
+// =========================================================================================================
 // group ids in first-seen order
 // =========================================================================================================
 // "virtual row" v: v < nexist is existing group v (its key comes from table_keys), v >= nexist is batch row v - nexist.  Every
@@ -221,16 +289,74 @@ gid_flag_kernel(uint64_t total, GidTable T, const uint32_t *__restrict__ rowslot
     }
 }
 
+// where assign writes a new group's key: the key word of an 8-byte key (GROUP_IDS) ...
+struct KeyWordSink {
+    uint64_t *table_keys; uint64_t table_cap; unsigned *overflow;
+    __device__ __forceinline__ bool fits(uint64_t) const { return true; }
+    __device__ __forceinline__ void put(uint64_t j, uint32_t, uint32_t s, const GidTable &T) const {
+        if (j < table_cap) table_keys[j] = T.key[s]; else *overflow = 2;
+    }
+};
+// ... or the bytes of a byte-string key (STR_GROUP_IDS), at offset toff[nexist] + pos[j - nexist] (an exclusive scan of the new groups'
+// lengths), with the batch row that created the group.  Nothing is written, ngroups included, unless every new group fits.
+struct StrBytesSink {
+    StrKeys K; uint8_t *tbytes; uint64_t *toff; uint64_t cap_groups, cap_bytes; const uint64_t *pos, *pos_total; int64_t *first_rows; unsigned *overflow;
+    __device__ __forceinline__ bool fits(uint64_t cnt) const {
+        const bool ok = *overflow == 0 && cnt <= cap_groups && toff[K.nexist] + *pos_total <= cap_bytes;
+        if (!ok && blockIdx.x == 0 && threadIdx.x == 0) *overflow |= 2;
+        return ok;
+    }
+    __device__ __forceinline__ void put(uint64_t j, uint32_t first, uint32_t, const GidTable &) const {
+        const ByteKey k = K.at(first);
+        const uint64_t at = toff[K.nexist] + pos[j - K.nexist];
+        for (uint64_t b = 0; b < k.n; b++) tbytes[at + b] = k.p[b];
+        toff[j + 1] = at + k.n;
+        if (first_rows) first_rows[j - K.nexist] = (int64_t)(first - K.nexist);
+    }
+};
+
+template <class Sink>
 __global__ void __launch_bounds__(kThreads)
 gid_assign_kernel(const uint32_t *__restrict__ firsts, const unsigned long long *count, GidTable T, const uint32_t *__restrict__ rowslot,
-                  uint64_t *__restrict__ table_keys, uint64_t table_cap, uint64_t nexist, int64_t *ngroups_out, unsigned *overflow) {
+                  Sink sink, uint64_t nexist, int64_t *ngroups_out) {
     const uint64_t cnt = *count;
+    const bool fits = sink.fits(cnt);
     for (uint64_t j = blockIdx.x * (uint64_t)kThreads + threadIdx.x; j < cnt; j += (uint64_t)gridDim.x * kThreads) {
-        const uint32_t s = rowslot[firsts[j]];
+        const uint32_t f = firsts[j];
+        const uint32_t s = rowslot[f];
         T.id[s] = j + 1;
-        if (j >= nexist) { if (j < table_cap) table_keys[j] = T.key[s]; else *overflow = 2; }
+        if (j >= nexist && fits) sink.put(j, f, s, T);
     }
-    if (blockIdx.x == 0 && threadIdx.x == 0) *ngroups_out = (int64_t)cnt;
+    if (blockIdx.x == 0 && threadIdx.x == 0 && fits) *ngroups_out = (int64_t)cnt;
+}
+
+// the byte-string twin of gid_insert_kernel: virtual rows as there, keys compared by their bytes (keytable.cuh)
+__global__ void __launch_bounds__(kThreads)
+sgid_insert_kernel(StrKeys K, const uint64_t *__restrict__ knulls, uint64_t n, GidTable T, uint64_t hash_mask, uint32_t *__restrict__ rowslot,
+                   unsigned *overflow) {
+    const uint64_t total = n + K.nexist;
+    for (uint64_t v = blockIdx.x * (uint64_t)kThreads + threadIdx.x; v < total; v += (uint64_t)gridDim.x * kThreads) {
+        if (v >= K.nexist && bm_test(knulls, v - K.nexist)) { rowslot[v] = kNoRowSlot; continue; }
+        const ByteKey k = K.at(v);
+        const uint64_t h = str_hash(k, hash_mask);
+        const uint64_t slot = kt_insert_str(T.key, T.mask, h, str_word(h, v), [&](uint32_t r) { return bytes_equal(K.at(r), k); });
+        if (slot == kNoSlot) { *overflow = 1; rowslot[v] = kNoRowSlot; continue; }
+        first_row_min(&T.minrow[slot], v);
+        rowslot[v] = (uint32_t)slot;
+    }
+}
+
+// lens[i] = the key length of new group nexist + i (0 past the last one): exclusive_scan turns it into the group's offset among the new bytes
+__global__ void __launch_bounds__(kThreads)
+sgid_len_kernel(const uint32_t *__restrict__ firsts, const unsigned long long *count, uint64_t nexist, const uint64_t *__restrict__ koff, uint64_t n,
+                uint64_t *__restrict__ lens) {
+    const uint64_t cnt = *count;
+    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
+        const uint64_t j = nexist + i;
+        uint64_t l = 0;
+        if (j < cnt) { const uint64_t r = firsts[j] - nexist; l = koff[r + 1] - koff[r]; }
+        lens[i] = l;
+    }
 }
 
 __global__ void __launch_bounds__(kThreads)
@@ -622,7 +748,7 @@ int xcall_group_ids(mo_xcall_args_t *args, uint64_t len) {
     MOB_LAUNCH_CHECK();
     int rc = launch_select<uint32_t>(t, isfirst, nullptr, total, firsts, dcount);
     if (rc) { st.finish(); return rc; }
-    gid_assign_kernel<<<grid_for(total < 1 ? 1 : (total < (1u << 20) ? total : (1u << 20))), kThreads, 0, t.stream>>>(firsts, dcount, T, rowslot, table_keys, table_cap, (uint64_t)nexist, dng, overflow);
+    gid_assign_kernel<<<grid_for(total < 1 ? 1 : (total < (1u << 20) ? total : (1u << 20))), kThreads, 0, t.stream>>>(firsts, dcount, T, rowslot, KeyWordSink{table_keys, table_cap, overflow}, (uint64_t)nexist, dng);
     MOB_LAUNCH_CHECK();
     gid_emit_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(groups, len, (uint64_t)nexist, T, rowslot);
     MOB_LAUNCH_CHECK();
@@ -631,6 +757,171 @@ int xcall_group_ids(mo_xcall_args_t *args, uint64_t len) {
     int frc = st.finish();
     if (rc) return rc;
     if (hov) { set_error("group ids: more distinct keys than the key table holds (%llu)", (unsigned long long)table_cap); return MO_RC_INVALID_ARGUMENT; }
+    return frc;
+}
+
+// MO_XCALL_PACK_STR_KEYS: args [0] key bytes u8[cap] ; [1] offsets uint64[len + 1] (+pnulls out: rows that join no group, has_null = 0) ;
+// [2] host mo_strkey_params_t ; [3 .. 3+ncols) key columns (fixed width or varlena cells + area; +pnulls; one element = const)
+int xcall_pack_str_keys(mo_xcall_args_t *args, uint64_t len) {
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    if (!args[2].pdata || args[2].dataSz < sizeof(mo_strkey_params_t) || is_device_ptr(args[2].pdata)) { set_error("pack str keys: host mo_strkey_params_t missing"); return MO_RC_INVALID_ARGUMENT; }
+    mo_strkey_params_t P;
+    memcpy(&P, args[2].pdata, sizeof P);
+    if (P.ncols < 1 || P.ncols > MO_STRKEY_MAX_COLS) { set_error("pack str keys: %d key columns (1..%d)", P.ncols, MO_STRKEY_MAX_COLS); return MO_RC_INVALID_ARGUMENT; }
+    if (!args[1].pdata || args[1].dataSz < 8 * (len + 1)) { set_error("pack str keys: the offsets need len + 1 entries"); return MO_RC_INVALID_ARGUMENT; }
+    bool dev = is_device_ptr(args[1].pdata) && (!args[1].pnulls || is_device_ptr(args[1].pnulls)) && (!args[0].pdata || is_device_ptr(args[0].pdata));
+    Stager st(t);
+    StrKeyCols K;
+    memset(&K, 0, sizeof K);
+    K.n = P.ncols;
+    for (int k = 0; k < K.n; k++) {
+        const mo_xcall_args_t &a = args[3 + k];
+        const int T = P.col_type[k];
+        const bool var = is_varlena(T);
+        const uint64_t esz = var ? MO_VARLENA_SZ : (uint64_t)key_type_size(T);
+        if (!esz) { st.finish(); set_error("pack str keys: column %d has unsupported type %d", k, T); return MO_RC_INVALID_ARGUMENT; }
+        const bool cst = len != 1 && a.dataSz == esz;
+        if (!cst && a.dataSz < esz * len) { st.finish(); set_error("pack str keys: column %d holds %llu bytes, %llu needed", k, (unsigned long long)a.dataSz, (unsigned long long)(esz * len)); return MO_RC_INVALID_ARGUMENT; }
+        if ((len || cst) && !a.pdata) { st.finish(); set_error("pack str keys: column %d has no data", k); return MO_RC_INVALID_ARGUMENT; }
+        const uint64_t rows = cst ? 1 : len;
+        K.col[k] = (const uint8_t *)st.in(a.pdata, rows * esz);
+        K.nulls[k] = (const uint64_t *)st.in(a.pnulls, a.pnulls ? ((rows + 63) / 64) * 8 : 0);
+        K.size[k] = var ? 0 : (int)esz;
+        K.cst[k] = cst ? 1 : 0;
+        if (a.pdata && rows) dev = dev && is_device_ptr(a.pdata);
+        if (a.pnulls) dev = dev && is_device_ptr(a.pnulls);
+        if (var && a.parea && a.areaSz) {
+            K.area[k] = (const uint8_t *)st.in(a.parea, a.areaSz);
+            K.area_sz[k] = a.areaSz;
+            dev = dev && is_device_ptr(a.parea);
+        }
+    }
+    uint64_t *off = (uint64_t *)st.out(args[1].pdata, 8 * (len + 1));
+    uint32_t *skip = (uint32_t *)st.out(args[1].pnulls, args[1].pnulls ? ((len + 63) / 64) * 8 : 0);
+    struct Rec { VarlenaStat vs; uint64_t total; };
+    Rec *rec = (Rec *)st.tmp(sizeof(Rec));
+    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    MOB_CUDA_TRY(cudaMemsetAsync(rec, 0, sizeof(Rec), t.stream));
+    for (int k = 0; k < K.n; k++) {
+        if (K.size[k] || !len) continue;
+        int rc = varlena_stat(t, K.col[k], K.nulls[k], K.area[k], K.area_sz[k], K.cst[k] ? 1 : len, &rec->vs, k);
+        if (rc) { st.finish(); return rc; }
+    }
+    int grid = num_sms() * 8;
+    const uint64_t work = (len + kThreads - 1) / kThreads;
+    if ((uint64_t)grid > work) grid = (int)(work ? work : 1);
+    cudaEventRecord(t.kev0, t.stream);
+    if (len) {
+        strkey_len_kernel<<<grid, kThreads, 0, t.stream>>>(K, len, P.has_null, off, skip);
+        MOB_LAUNCH_CHECK();
+    }
+    int rc = exclusive_scan(t, off, len, off, off + len);   // off[len] = the bytes needed
+    if (rc) { st.finish(); return rc; }
+    MOB_CUDA_TRY(cudaMemcpyAsync(&rec->total, off + len, 8, cudaMemcpyDeviceToDevice, t.stream));
+    Rec h;
+    rc = read_back(t, &h, rec, sizeof h);
+    if (rc) { st.finish(); return rc; }
+    rc = varlena_stat_error(h.vs, K.n, "pack str keys: column");
+    if (rc) { st.finish(); return rc; }
+    if (h.total > args[0].dataSz) {
+        int frc = st.finish();
+        if (frc) return frc;
+        set_error("pack str keys: the keys take %llu bytes, the buffer holds %llu (offsets[len] holds the size needed)", (unsigned long long)h.total, (unsigned long long)args[0].dataSz);
+        return MO_RC_OUT_OF_RANGE;
+    }
+    uint8_t *bytes = (uint8_t *)st.out(args[0].pdata, h.total);
+    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (len) {
+        strkey_write_kernel<<<grid, kThreads, 0, t.stream>>>(K, len, P.has_null, off, bytes);
+        MOB_LAUNCH_CHECK();
+    }
+    cudaEventRecord(t.kev1, t.stream);
+    if (dev) { st.release_async(); return MO_RC_SUCCESS; }
+    return st.finish();
+}
+
+// MO_XCALL_STR_GROUP_IDS: args [0] groups uint64[len] ; [1] int64 ngroups (in/out) ; [2] table bytes u8[cap_bytes] ; [3] table offsets
+// uint64[cap_groups + 1] ; [4] key bytes ; [5] key offsets uint64[len + 1] (+pnulls: rows that get id 0) ; [6] first rows int64[len] (out; pdata
+// NULL: not wanted)
+int xcall_str_group_ids(mo_xcall_args_t *args, uint64_t len) {
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    if (!args[1].pdata || args[1].dataSz < 8 || args[0].dataSz < 8 * len || !args[3].pdata || args[3].dataSz < 8 || args[5].dataSz < 8 * (len + 1) || !args[5].pdata) {
+        set_error("str group ids: buffers too small (groups len, ngroups 8 bytes, table offsets >= 1 entry, key offsets len + 1)"); return MO_RC_INVALID_ARGUMENT;
+    }
+    const bool want_first = args[6].pdata != nullptr;
+    if (want_first && args[6].dataSz < 8 * len) { set_error("str group ids: the first rows need len entries"); return MO_RC_INVALID_ARGUMENT; }
+    if (!is_device_ptr(args[5].pdata)) {   // host key offsets: they must lie inside the key bytes (device offsets are the caller's to keep right)
+        const uint64_t *ko = (const uint64_t *)args[5].pdata;
+        if (ko[len] > args[4].dataSz || ko[0] > ko[len]) { set_error("str group ids: key offsets end at %llu, the key bytes hold %llu", (unsigned long long)ko[len], (unsigned long long)args[4].dataSz); return MO_RC_INVALID_ARGUMENT; }
+    }
+    int64_t nexist = 0;
+    if (is_device_ptr(args[1].pdata)) { int rc = read_back(t, &nexist, args[1].pdata, 8); if (rc) return rc; } else memcpy(&nexist, args[1].pdata, 8);
+    const uint64_t cap_groups = args[3].dataSz / 8 - 1, cap_bytes = args[2].dataSz;
+    if (nexist < 0 || (uint64_t)nexist > cap_groups) { set_error("str group ids: ngroups %lld exceeds the table (%llu groups)", (long long)nexist, (unsigned long long)cap_groups); return MO_RC_INVALID_ARGUMENT; }
+    if (!is_device_ptr(args[3].pdata) && ((const uint64_t *)args[3].pdata)[nexist] > cap_bytes) {
+        set_error("str group ids: table offsets end at %llu, the table bytes hold %llu", (unsigned long long)((const uint64_t *)args[3].pdata)[nexist], (unsigned long long)cap_bytes); return MO_RC_INVALID_ARGUMENT;
+    }
+    const uint64_t total = len + (uint64_t)nexist;
+    if (total >= 0x7fffffffull) { set_error("str group ids: at most 2^31 rows plus groups per call"); return MO_RC_INVALID_ARGUMENT; }
+    uint64_t want = total < cap_groups ? total : cap_groups;   // as GROUP_IDS: more distinct keys than that fail the call anyway
+    if (want < 16) want = 16;
+    uint64_t cap = 32;
+    while (cap < 2 * want) cap <<= 1;
+    // asynchronous only when every output is device memory: a host ngroups must be copied back, so such a call finishes synchronously
+    const bool dev = is_device_ptr(args[0].pdata) && is_device_ptr(args[1].pdata) && is_device_ptr(args[2].pdata) && is_device_ptr(args[3].pdata) &&
+                     is_device_ptr(args[5].pdata) && (len == 0 || is_device_ptr(args[4].pdata)) && (!args[5].pnulls || is_device_ptr(args[5].pnulls)) && (!want_first || is_device_ptr(args[6].pdata));
+    Stager st(t);
+    uint64_t *groups = (uint64_t *)st.out(args[0].pdata, 8 * len);
+    int64_t *dng = (int64_t *)st.out(args[1].pdata, 8, true);
+    uint8_t *tbytes = (uint8_t *)st.out(args[2].pdata, cap_bytes, true);
+    uint64_t *toff = (uint64_t *)st.out(args[3].pdata, (cap_groups + 1) * 8, true);
+    const uint8_t *kbytes = (const uint8_t *)st.in(args[4].pdata, args[4].dataSz);
+    const uint64_t *koff = (const uint64_t *)st.in(args[5].pdata, 8 * (len + 1));
+    const uint64_t *knulls = (const uint64_t *)st.in(args[5].pnulls, args[5].pnulls ? ((len + 63) / 64) * 8 : 0);
+    int64_t *first_rows = want_first ? (int64_t *)st.out(args[6].pdata, 8 * len, true) : nullptr;
+    GidTable T;
+    T.key = (uint64_t *)st.tmp((cap + 1) * 16); T.minrow = (unsigned long long *)(T.key + cap + 1); T.id = (uint64_t *)st.tmp((cap + 1) * 8);
+    T.mask = cap - 1;
+    uint32_t *rowslot = (uint32_t *)st.tmp(total * 4 + 16);
+    uint8_t *isfirst = (uint8_t *)st.tmp(total + 16);
+    uint32_t *firsts = (uint32_t *)st.tmp(total * 4 + 16);
+    uint64_t *lens = (uint64_t *)st.tmp(len * 8 + 16);
+    unsigned long long *rec = (unsigned long long *)st.tmp(32);   // [0] groups after the call, [1] overflow bits, [2] new key bytes, [3] toff[nexist]
+    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    unsigned *overflow = (unsigned *)(rec + 1);
+    MOB_CUDA_TRY(cudaMemsetAsync(rec, 0, 32, t.stream));
+    MOB_CUDA_TRY(cudaMemsetAsync(T.id, 0, (cap + 1) * 8, t.stream));
+    MOB_CUDA_TRY(cudaMemsetAsync(T.key, 0xff, (cap + 1) * 16, t.stream));
+    auto grid_for = [&](uint64_t items) { uint64_t g = (items + kThreads - 1) / kThreads; uint64_t mx = (uint64_t)num_sms() * 8; return (unsigned)(g > mx ? mx : (g ? g : 1)); };
+    const StrKeys K{tbytes, toff, kbytes, koff, (uint64_t)nexist};
+    cudaEventRecord(t.kev0, t.stream);
+    sgid_insert_kernel<<<grid_for(total), kThreads, 0, t.stream>>>(K, knulls, len, T, strkey_hash_mask(), rowslot, overflow);
+    cudaEventRecord(t.kev1, t.stream);
+    MOB_LAUNCH_CHECK();
+    gid_flag_kernel<<<grid_for(total), kThreads, 0, t.stream>>>(total, T, rowslot, isfirst);
+    MOB_LAUNCH_CHECK();
+    int rc = launch_select<uint32_t>(t, isfirst, nullptr, total, firsts, rec);
+    if (rc) { st.finish(); return rc; }
+    sgid_len_kernel<<<grid_for(len), kThreads, 0, t.stream>>>(firsts, rec, (uint64_t)nexist, koff, len, lens);
+    MOB_LAUNCH_CHECK();
+    rc = exclusive_scan(t, lens, len, lens, (uint64_t *)(rec + 2));
+    if (rc) { st.finish(); return rc; }
+    MOB_CUDA_TRY(cudaMemcpyAsync(rec + 3, toff + nexist, 8, cudaMemcpyDeviceToDevice, t.stream));
+    const StrBytesSink sink{K, tbytes, toff, cap_groups, cap_bytes, lens, (const uint64_t *)(rec + 2), first_rows, overflow};
+    gid_assign_kernel<<<grid_for(total < 1 ? 1 : (total < (1u << 20) ? total : (1u << 20))), kThreads, 0, t.stream>>>(firsts, rec, T, rowslot, sink, (uint64_t)nexist, dng);
+    MOB_LAUNCH_CHECK();
+    gid_emit_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(groups, len, (uint64_t)nexist, T, rowslot);
+    MOB_LAUNCH_CHECK();
+    unsigned long long h[4];
+    rc = read_back(t, h, rec, sizeof h);
+    if (rc) { st.finish(); return rc; }
+    const unsigned hov = (unsigned)h[1];
+    if (!hov && dev) { st.release_async(); return MO_RC_SUCCESS; }
+    int frc = st.finish();
+    if (hov & 1) { set_error("str group ids: more than %llu distinct keys; the table holds %llu groups and %llu bytes (capacity)", (unsigned long long)cap, (unsigned long long)cap_groups, (unsigned long long)cap_bytes); return MO_RC_INVALID_ARGUMENT; }
+    if (hov) { set_error("str group ids: the groups need %llu groups and %llu bytes; the table holds %llu groups and %llu bytes (capacity)", h[0], h[3] + h[2], (unsigned long long)cap_groups, (unsigned long long)cap_bytes); return MO_RC_INVALID_ARGUMENT; }
     return frc;
 }
 

@@ -48,6 +48,10 @@ bool is_device_ptr(const void *p);
 void search_invalidate(const void *p, uint64_t bytes);
 // MoB200_SetTuning names of the search module (tcsearch.cu): false for any other name, else *out = the answer (0 for a knob)
 bool search_tuning(const char *name, int value, int *out);
+// MoB200_SetTuning("strkey_hash_bits", b), test only (colops.cu): string-key hashes keep their low b bits (1..63; 0 = all 64), so that hash tags
+// collide and the byte compare of the key table runs
+extern int g_strkey_hash_bits;
+inline uint64_t strkey_hash_mask() { const int b = g_strkey_hash_bits; return b <= 0 || b >= 64 ? ~0ull : (1ull << b) - 1; }
 
 // --- device scratch arena -------------------------------------------------------------------------------
 void *arena_alloc(ThreadCtx &t, size_t bytes);   // 256-byte aligned; nullptr on failure (error set)

@@ -11,6 +11,8 @@
 //                (unique maps: build row = id - 1), for inner / left outer / left semi / left anti.  Output pairs (probe row, build row | -1) in
 //                exactly the order the reference appends them: probe rows ascending, within a row the sels ascending.  Counts -> exclusive scan ->
 //                positions; rows with >= 32 matches are written by their whole warp.
+//   byte-string keys   STR_JOIN_FIND = strHashmapIterator.Find over a STR_GROUP_IDS table (keytable.cuh's byte-string slots);
+//                JOIN_PROBE_GIDS = JOIN_PROBE's counting and emission over the group ids JOIN_FIND or STR_JOIN_FIND returned.
 //   The hash table itself is not observable in the reference (random seeds): ids and pairs are.  The device table is rebuilt from table_keys per
 //   call (O(groups)) unless it was prepared with MoB200_JoinMapPrepare (cached per table_keys pointer).
 // All passes stream their inputs once; algorithmic bytes per probe row: 8 (key) + 16 per emitted pair + one random 8-byte table probe.
@@ -85,7 +87,9 @@ __global__ void __launch_bounds__(kThreads) scan_apply_kernel(const uint64_t *__
     for (int w = 0; w < warp; w++) run += sw[w];
     for (int j = 0; j < 8; j++) { if (base + j < n) out[base + j] = run; run += v[j]; }
 }
-// out[i] = sum of in[0 .. i); *total (device) = sum of all.  in == out allowed.  sums scratch from the arena.
+}  // namespace
+
+// out[i] = sum of in[0 .. i); *total (device) = sum of all.  in == out allowed.  sums scratch from the arena.  Also used by colops.cu.
 int exclusive_scan(ThreadCtx &t, const uint64_t *in, uint64_t n, uint64_t *out, uint64_t *total) {
     if (n == 0) { MOB_CUDA_TRY(cudaMemsetAsync(total, 0, 8, t.stream)); return MO_RC_SUCCESS; }
     const uint64_t nb = (n + kScanTile - 1) / kScanTile;
@@ -99,6 +103,8 @@ int exclusive_scan(ThreadCtx &t, const uint64_t *in, uint64_t n, uint64_t *out, 
     MOB_LAUNCH_CHECK();
     return MO_RC_SUCCESS;
 }
+
+namespace {
 
 // ---- JOIN_SELS ------------------------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads) sels_flag_kernel(const uint64_t *__restrict__ groups, uint64_t n, uint64_t ngroups, uint64_t *__restrict__ flag, uint64_t *__restrict__ cnt, unsigned *bad) {
@@ -147,9 +153,37 @@ __global__ void __launch_bounds__(kThreads) jt_find_kernel(const uint64_t *__res
     }
 }
 
-struct DevTable { uint64_t *key = nullptr; uint32_t *id = nullptr; uint64_t mask = 0; uint64_t ngroups = 0; bool cached = false; };
+// ---- the string twin (STR_JOIN_FIND): keytable.cuh's byte-string slots over the table's bytes; slot row g is group g + 1 -------------------
+__global__ void __launch_bounds__(kThreads) sjt_build_kernel(StrKeys K, uint64_t ngroups, uint64_t *slots, uint64_t mask, uint64_t hash_mask) {
+    for (uint64_t g = blockIdx.x * (uint64_t)kThreads + threadIdx.x; g < ngroups; g += (uint64_t)gridDim.x * kThreads) {
+        // the groups' keys are distinct and the table at most half full: every group claims the first empty slot of its probe
+        const uint64_t h = str_hash(K.at(g), hash_mask);
+        kt_insert_str(slots, mask, h, str_word(h, g), [](uint32_t) { return false; });
+    }
+}
+__global__ void __launch_bounds__(kThreads) sjt_find_kernel(StrKeys K, const uint64_t *__restrict__ knulls, uint64_t n, const uint64_t *__restrict__ slots,
+                                                            uint64_t mask, uint64_t hash_mask, uint64_t *__restrict__ vals) {
+    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
+        uint64_t v = 0;
+        if (!bm_test(knulls, i)) {
+            const ByteKey k = K.at(K.nexist + i);
+            uint32_t row;
+            if (kt_find_str(slots, mask, str_hash(k, hash_mask), [&](uint32_t r) { return bytes_equal(K.at(r), k); }, row)) v = (uint64_t)row + 1;
+        }
+        vals[i] = v;
+    }
+}
+
+// a device join table: the 8-byte one (key, id), or a string one (key = its slots; sbytes / soff = the table's bytes and offsets)
+struct DevTable { uint64_t *key = nullptr; uint32_t *id = nullptr; uint64_t mask = 0; uint64_t ngroups = 0; bool cached = false;
+                  bool str = false; const uint8_t *sbytes = nullptr; const uint64_t *soff = nullptr; };
 std::shared_mutex g_jm_mu;
-std::unordered_map<const void *, DevTable> g_jm;   // prepared join maps, by table_keys pointer
+std::unordered_map<const void *, DevTable> g_jm;   // prepared join maps, by table_keys pointer (string maps: by table offsets pointer)
+
+void free_table(DevTable &T) {
+    cudaFree(T.key); cudaFree(T.id);
+    cudaFree((void *)T.sbytes); cudaFree((void *)T.soff);
+}
 
 int build_table(ThreadCtx &t, const uint64_t *dkeys, uint64_t ngroups, bool persistent, DevTable *out) {
     uint64_t slots = 64;
@@ -181,20 +215,76 @@ int table_for(ThreadCtx &t, Stager &st, const mo_xcall_args_t &a, DevTable *T, s
     const uint64_t ngroups = a.dataSz / 8;
     lk = std::shared_lock<std::shared_mutex>(g_jm_mu);
     auto it = g_jm.find(a.pdata);
-    if (it != g_jm.end() && it->second.ngroups == ngroups) { *T = it->second; return MO_RC_SUCCESS; }
+    if (it != g_jm.end() && it->second.ngroups == ngroups && !it->second.str) { *T = it->second; return MO_RC_SUCCESS; }
     lk.unlock();
     const uint64_t *dkeys = (const uint64_t *)st.in(a.pdata, ngroups * 8);
     if (st.failed) return MO_RC_INTERNAL_ERROR;
     return build_table(t, dkeys, ngroups, false, T);
 }
 
-// ---- JOIN_PROBE -----------------------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads) probe_count_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ knulls, uint64_t n, const uint64_t *__restrict__ tkey,
-                                                               const uint32_t *__restrict__ tid, uint64_t mask, const int32_t *__restrict__ offsets,
+// the string table of groups 1..ngroups whose bytes / offsets are on the device; persistent: slots from cudaMalloc (the caller owns the rest)
+int build_str_table(ThreadCtx &t, const uint8_t *dbytes, const uint64_t *doff, uint64_t ngroups, bool persistent, DevTable *out) {
+    uint64_t slots = 64;
+    while (slots < 2 * ngroups) slots <<= 1;
+    DevTable T;
+    if (persistent) {
+        if (cudaMalloc(&T.key, slots * 8) != cudaSuccess) { set_error("join map: cudaMalloc of a %llu-slot table failed", (unsigned long long)slots); return MO_RC_INTERNAL_ERROR; }
+    } else {
+        T.key = (uint64_t *)arena_alloc(t, slots * 8);
+        if (!T.key) return MO_RC_INTERNAL_ERROR;
+    }
+    T.mask = slots - 1; T.ngroups = ngroups; T.cached = persistent; T.str = true; T.sbytes = dbytes; T.soff = doff;
+    const cudaError_t e = cudaMemsetAsync(T.key, 0xff, slots * 8, t.stream);
+    if (e != cudaSuccess) {
+        set_error("join map: clearing a %llu-slot table failed: %s", (unsigned long long)slots, cudaGetErrorString(e));
+        if (persistent) cudaFree(T.key);
+        return MO_RC_INTERNAL_ERROR;
+    }
+    if (ngroups) {
+        sjt_build_kernel<<<grid_for(ngroups), kThreads, 0, t.stream>>>(StrKeys{dbytes, doff, nullptr, nullptr, ngroups}, ngroups, T.key, T.mask, strkey_hash_mask());
+        MOB_LAUNCH_CHECK();
+    }
+    *out = T;
+    return MO_RC_SUCCESS;
+}
+
+// the prepared string table keyed by the table offsets pointer, or a scratch one
+int str_table_for(ThreadCtx &t, Stager &st, const mo_xcall_args_t &bytes, const mo_xcall_args_t &offs, uint64_t ngroups, DevTable *T,
+                  std::shared_lock<std::shared_mutex> &lk) {
+    lk = std::shared_lock<std::shared_mutex>(g_jm_mu);
+    auto it = g_jm.find(offs.pdata);
+    if (it != g_jm.end() && it->second.ngroups == ngroups && it->second.str) { *T = it->second; return MO_RC_SUCCESS; }
+    lk.unlock();
+    const uint8_t *db = (const uint8_t *)st.in(bytes.pdata, bytes.dataSz);
+    const uint64_t *doff = (const uint64_t *)st.in(offs.pdata, (ngroups + 1) * 8);
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    return build_str_table(t, db, doff, ngroups, false, T);
+}
+
+// ---- JOIN_PROBE / JOIN_PROBE_GIDS ---------------------------------------------------------------------------------------------------------------
+// the group id of probe row i: looked up by its key (JOIN_PROBE) ...
+struct KeyLookup {
+    const uint64_t *__restrict__ keys; const uint64_t *__restrict__ knulls; const uint64_t *__restrict__ tkey; const uint32_t *__restrict__ tid; uint64_t mask;
+    __device__ __forceinline__ uint32_t operator()(uint64_t i) const {
+        const bool isnull = knulls && ((knulls[i >> 6] >> (i & 63)) & 1ull);
+        return isnull ? 0u : jt_find(tkey, tid, mask, keys[i]);
+    }
+};
+// ... or given (JOIN_PROBE_GIDS); an id above ngroups sets *bad
+struct GidLookup {
+    const uint64_t *__restrict__ gids; uint64_t ngroups; unsigned *bad;
+    __device__ __forceinline__ uint32_t operator()(uint64_t i) const {
+        const uint64_t g = gids[i];
+        if (g > ngroups) { *bad = 1; return 0u; }
+        return (uint32_t)g;
+    }
+};
+
+template <class Lookup>
+__global__ void __launch_bounds__(kThreads) probe_count_kernel(Lookup lookup, uint64_t n, const int32_t *__restrict__ offsets,
                                                                int join_type, uint32_t *__restrict__ vals, uint64_t *__restrict__ cnt) {
     for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
-        const bool isnull = knulls && ((knulls[i >> 6] >> (i & 63)) & 1ull);
-        const uint32_t v = isnull ? 0u : jt_find(tkey, tid, mask, keys[i]);
+        const uint32_t v = lookup(i);
         uint64_t m = 0;
         if (v) m = offsets ? (uint64_t)(offsets[v] - offsets[v - 1]) : 1ull;
         uint64_t c;
@@ -239,6 +329,47 @@ __global__ void __launch_bounds__(kThreads) probe_emit_kernel(uint64_t n, const 
         }
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) *count_out = (int64_t)*total;
+}
+
+// the output side shared by JOIN_PROBE and JOIN_PROBE_GIDS: args [0] probe_rows, [1] build_rows, [2] count, [5] / [6] sels; reads back the result
+// count and *bad (scal[1], set by the lookup) in one record
+template <class Lookup>
+int run_probe(ThreadCtx &t, Stager &st, mo_xcall_args_t *args, uint64_t len, int join_type, uint64_t ngroups, Lookup lookup, uint64_t *scal) {
+    const uint64_t cap = args[0].dataSz / 8;
+    const bool multi = args[5].pdata != nullptr;
+    int64_t *out_probe = (int64_t *)st.out(args[0].pdata, cap * 8);
+    int64_t *out_build = (int64_t *)st.out(args[1].pdata, cap * 8);
+    int64_t *count = (int64_t *)st.out(args[2].pdata, 8);
+    const int32_t *offsets = multi ? (const int32_t *)st.in(args[5].pdata, (ngroups + 2) * 4) : nullptr;
+    const int32_t *sels = multi ? (const int32_t *)st.in(args[6].pdata, args[6].dataSz) : nullptr;
+    uint32_t *vals = (uint32_t *)st.tmp(len * 4 + 4);
+    uint64_t *cnt = (uint64_t *)st.tmp((len + 1) * 8);
+    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    cudaEventRecord(t.kev0, t.stream);
+    probe_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(lookup, len, offsets, join_type, vals, cnt);
+    MOB_LAUNCH_CHECK();
+    int rc = exclusive_scan(t, cnt, len, cnt, scal);
+    if (rc) { st.finish(); return rc; }
+    probe_emit_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(len, vals, cnt, scal, offsets, sels, join_type, cap, out_probe, out_build, count);
+    cudaEventRecord(t.kev1, t.stream);
+    MOB_LAUNCH_CHECK();
+    uint64_t h[2] = {0, 0};
+    rc = read_back(t, h, scal, sizeof h);
+    int frc = st.finish();
+    if (rc) return rc;
+    if (h[1]) { set_error("join probe: a group id exceeds the group count (%llu)", (unsigned long long)ngroups); return MO_RC_INVALID_ARGUMENT; }
+    if (h[0] > cap) { set_error("join probe: %lld result rows exceed the output capacity (%llu); the count is reported, call again with larger buffers", (long long)h[0], (unsigned long long)cap); return MO_RC_OUT_OF_RANGE; }
+    return frc;
+}
+
+// a host int64 argument (ngroups of STR_JOIN_FIND / JOIN_PROBE_GIDS)
+bool host_i64(const mo_xcall_args_t &a, uint64_t *v) {
+    int64_t x;
+    if (!a.pdata || a.dataSz < 8 || is_device_ptr(a.pdata)) return false;
+    memcpy(&x, a.pdata, 8);
+    if (x < 0) return false;
+    *v = (uint64_t)x;
+    return true;
 }
 
 }  // namespace
@@ -331,38 +462,72 @@ int xcall_join_probe(mo_xcall_args_t *args, uint64_t len) {
     const uint64_t cap = args[0].dataSz / 8;
     if (args[1].dataSz / 8 < cap || !args[2].pdata || args[2].dataSz < 8 || args[7].dataSz < 8 * len) { set_error("join probe: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
     const uint64_t ngroups = args[4].dataSz / 8;
-    const bool multi = args[5].pdata != nullptr;
-    if (multi && args[5].dataSz < (ngroups + 2) * 4) { set_error("join probe: sels offsets shorter than the group count + 2"); return MO_RC_INVALID_ARGUMENT; }
+    if (args[5].pdata && args[5].dataSz < (ngroups + 2) * 4) { set_error("join probe: sels offsets shorter than the group count + 2"); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);
     DevTable T;
     std::shared_lock<std::shared_mutex> lk;
     int rc = table_for(t, st, args[4], &T, lk);
     if (rc) { st.finish(); return rc; }
-    int64_t *out_probe = (int64_t *)st.out(args[0].pdata, cap * 8);
-    int64_t *out_build = (int64_t *)st.out(args[1].pdata, cap * 8);
-    int64_t *count = (int64_t *)st.out(args[2].pdata, 8);
-    const int32_t *offsets = multi ? (const int32_t *)st.in(args[5].pdata, (ngroups + 2) * 4) : nullptr;
-    const int32_t *sels = multi ? (const int32_t *)st.in(args[6].pdata, args[6].dataSz) : nullptr;
     const uint64_t *keys = (const uint64_t *)st.in(args[7].pdata, 8 * len);
     const uint64_t *kn = (const uint64_t *)st.in(args[7].pnulls, args[7].pnulls ? ((len + 63) / 64) * 8 : 0);
-    uint32_t *vals = (uint32_t *)st.tmp(len * 4 + 4);
-    uint64_t *cnt = (uint64_t *)st.tmp((len + 1) * 8);
-    uint64_t *total = (uint64_t *)st.tmp(8);
+    uint64_t *scal = (uint64_t *)st.tmp(16);
+    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, 16, t.stream));
+    return run_probe(t, st, args, len, P.join_type, ngroups, KeyLookup{keys, kn, T.key, T.id, T.mask}, scal);
+}
+
+// MO_XCALL_JOIN_PROBE_GIDS: args [0..3], [5], [6] as JOIN_PROBE ; [4] host int64 ngroups ; [7] vals uint64[len] (group ids, 0 = no match)
+int xcall_join_probe_gids(mo_xcall_args_t *args, uint64_t len) {
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    if (!args[3].pdata || args[3].dataSz < sizeof(mo_join_params_t) || is_device_ptr(args[3].pdata)) { set_error("join probe gids: host mo_join_params_t missing"); return MO_RC_INVALID_ARGUMENT; }
+    mo_join_params_t P;
+    memcpy(&P, args[3].pdata, sizeof P);
+    if (P.join_type < MO_JOIN_INNER || P.join_type > MO_JOIN_ANTI) { set_error("join probe gids: join type %d", P.join_type); return MO_RC_INVALID_ARGUMENT; }
+    uint64_t ngroups;
+    if (!host_i64(args[4], &ngroups)) { set_error("join probe gids: [4] must be a host int64 ngroups >= 0"); return MO_RC_INVALID_ARGUMENT; }
+    const uint64_t cap = args[0].dataSz / 8;
+    if (args[1].dataSz / 8 < cap || !args[2].pdata || args[2].dataSz < 8 || args[7].dataSz < 8 * len) { set_error("join probe gids: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
+    if (args[5].pdata && args[5].dataSz < (ngroups + 2) * 4) { set_error("join probe gids: sels offsets shorter than the group count + 2"); return MO_RC_INVALID_ARGUMENT; }
+    Stager st(t);
+    const uint64_t *gids = (const uint64_t *)st.in(args[7].pdata, 8 * len);
+    uint64_t *scal = (uint64_t *)st.tmp(16);
+    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, 16, t.stream));
+    return run_probe(t, st, args, len, P.join_type, ngroups, GidLookup{gids, ngroups, (unsigned *)(scal + 1)}, scal);
+}
+
+// MO_XCALL_STR_JOIN_FIND: args [0] vals uint64[len] ; [1] host int64 ngroups ; [2] table bytes ; [3] table offsets uint64[ngroups + 1] ; [4] probe key
+// bytes ; [5] probe key offsets uint64[len + 1] (+pnulls)
+int xcall_str_join_find(mo_xcall_args_t *args, uint64_t len) {
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    uint64_t ngroups;
+    if (!host_i64(args[1], &ngroups)) { set_error("str join find: [1] must be a host int64 ngroups >= 0"); return MO_RC_INVALID_ARGUMENT; }
+    if (args[0].dataSz < 8 * len || !args[3].pdata || args[3].dataSz < 8 * (ngroups + 1) || !args[5].pdata || args[5].dataSz < 8 * (len + 1)) { set_error("str join find: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
+    if (ngroups >= 0x7fffffffull) { set_error("str join find: at most 2^31 groups"); return MO_RC_INVALID_ARGUMENT; }
+    // host offsets must lie inside their bytes (device offsets are the caller's to keep right)
+    if (!is_device_ptr(args[3].pdata) && ((const uint64_t *)args[3].pdata)[ngroups] > args[2].dataSz) { set_error("str join find: table offsets end past the table bytes (%llu)", (unsigned long long)args[2].dataSz); return MO_RC_INVALID_ARGUMENT; }
+    if (!is_device_ptr(args[5].pdata) && ((const uint64_t *)args[5].pdata)[len] > args[4].dataSz) { set_error("str join find: probe key offsets end past the key bytes (%llu)", (unsigned long long)args[4].dataSz); return MO_RC_INVALID_ARGUMENT; }
+    const bool dev = is_device_ptr(args[0].pdata) && is_device_ptr(args[3].pdata) && is_device_ptr(args[5].pdata) && (!args[2].pdata || is_device_ptr(args[2].pdata)) &&
+                     (!args[4].pdata || is_device_ptr(args[4].pdata)) && (!args[5].pnulls || is_device_ptr(args[5].pnulls));
+    Stager st(t);
+    DevTable T;
+    std::shared_lock<std::shared_mutex> lk;
+    int rc = str_table_for(t, st, args[2], args[3], ngroups, &T, lk);
+    if (rc) { st.finish(); return rc; }
+    uint64_t *vals = (uint64_t *)st.out(args[0].pdata, 8 * len);
+    const uint8_t *kbytes = (const uint8_t *)st.in(args[4].pdata, args[4].dataSz);
+    const uint64_t *koff = (const uint64_t *)st.in(args[5].pdata, 8 * (len + 1));
+    const uint64_t *kn = (const uint64_t *)st.in(args[5].pnulls, args[5].pnulls ? ((len + 63) / 64) * 8 : 0);
     if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
     cudaEventRecord(t.kev0, t.stream);
-    probe_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(keys, kn, len, T.key, T.id, T.mask, offsets, P.join_type, vals, cnt);
-    MOB_LAUNCH_CHECK();
-    rc = exclusive_scan(t, cnt, len, cnt, total);
-    if (rc) { st.finish(); return rc; }
-    probe_emit_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(len, vals, cnt, total, offsets, sels, P.join_type, cap, out_probe, out_build, count);
+    sjt_find_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(StrKeys{T.sbytes, T.soff, kbytes, koff, ngroups}, kn, len, T.key, T.mask, strkey_hash_mask(), vals);
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
-    int64_t produced = 0;
-    rc = read_back(t, &produced, total, 8);
-    int frc = st.finish();
-    if (rc) return rc;
-    if ((uint64_t)produced > cap) { set_error("join probe: %lld result rows exceed the output capacity (%llu); the count is reported, call again with larger buffers", (long long)produced, (unsigned long long)cap); return MO_RC_OUT_OF_RANGE; }
-    return frc;
+    // asynchronous form: a prepared table may be released while this kernel still reads it; its cudaFree waits for the device's pending work
+    if (dev) { st.release_async(); return MO_RC_SUCCESS; }
+    return st.finish();
 }
 
 }  // namespace mob
@@ -378,11 +543,48 @@ extern "C" int32_t MoB200_JoinMapPrepare(const void *table_keys, uint64_t ngroup
     DevTable T;
     int rc = build_table(t, dkeys, ngroups, true, &T);
     int frc = st.finish();
-    if (rc || frc) { if (!rc) { cudaFree(T.key); cudaFree(T.id); } return rc ? rc : frc; }
+    if (rc || frc) { if (!rc) free_table(T); return rc ? rc : frc; }
     std::unique_lock<std::shared_mutex> lk(g_jm_mu);
     auto it = g_jm.find(table_keys);
-    if (it != g_jm.end()) { cudaFree(it->second.key); cudaFree(it->second.id); }
+    if (it != g_jm.end()) free_table(it->second);
     g_jm[table_keys] = T;
+    return MO_RC_SUCCESS;
+}
+
+// the string map: the table's bytes and offsets are copied to the device with it, so the caller may change or free its copy
+extern "C" int32_t MoB200_StrJoinMapPrepare(const void *table_bytes, const void *table_offsets, uint64_t ngroups) {
+    using namespace mob;
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    if (!table_offsets || ngroups >= 0x7fffffffull) { set_error("str join map: table offsets missing or more than 2^31 groups"); return MO_RC_INVALID_ARGUMENT; }
+    uint64_t nbytes = 0;
+    if (is_device_ptr(table_offsets)) { int rc = read_back(t, &nbytes, (const uint64_t *)table_offsets + ngroups, 8); if (rc) return rc; }
+    else memcpy(&nbytes, (const uint64_t *)table_offsets + ngroups, 8);
+    if (nbytes && !table_bytes) { set_error("str join map: table bytes missing"); return MO_RC_INVALID_ARGUMENT; }
+    uint8_t *db = nullptr;
+    uint64_t *doff = nullptr;
+    if (cudaMalloc(&db, nbytes ? nbytes : 1) != cudaSuccess || cudaMalloc(&doff, (ngroups + 1) * 8) != cudaSuccess) {
+        set_error("str join map: cudaMalloc of %llu bytes failed", (unsigned long long)nbytes);
+        cudaFree(db);
+        return MO_RC_INTERNAL_ERROR;
+    }
+    DevTable T;
+    int rc = MO_RC_SUCCESS;
+    if (nbytes && cudaMemcpyAsync(db, table_bytes, nbytes, cudaMemcpyDefault, t.stream) != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
+    if (!rc && cudaMemcpyAsync(doff, table_offsets, (ngroups + 1) * 8, cudaMemcpyDefault, t.stream) != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
+    if (!rc) rc = build_str_table(t, db, doff, ngroups, true, &T);
+    if (!rc && cudaStreamSynchronize(t.stream) != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
+    arena_reset(t);
+    if (rc) {
+        if (!t.err[0]) set_error("str join map: copying the table to the device failed");
+        if (T.key) cudaFree(T.key);
+        cudaFree(db); cudaFree(doff);
+        return rc;
+    }
+    std::unique_lock<std::shared_mutex> lk(g_jm_mu);
+    auto it = g_jm.find(table_offsets);
+    if (it != g_jm.end()) free_table(it->second);
+    g_jm[table_offsets] = T;
     return MO_RC_SUCCESS;
 }
 
@@ -391,8 +593,9 @@ extern "C" int32_t MoB200_JoinMapRelease(const void *table_keys) {
     std::unique_lock<std::shared_mutex> lk(g_jm_mu);
     auto it = g_jm.find(table_keys);
     if (it == g_jm.end()) return MO_RC_SUCCESS;
-    // (probes hold the shared lock until their stream has drained, so nothing is reading the table once the unique lock is ours)
-    cudaFree(it->second.key); cudaFree(it->second.id);
+    // (8-byte probes hold the shared lock until their stream has drained, so nothing is reading the table once the unique lock is ours; an
+    // asynchronous STR_JOIN_FIND may still be reading, and cudaFree waits for it)
+    free_table(it->second);
     g_jm.erase(it);
     return MO_RC_SUCCESS;
 }

@@ -43,6 +43,7 @@
 // makes that set approach len: correct, no faster than the full sort.  String keys with a common leading prefix of 8 bytes or more (or 7 after
 // a NULL flag) are such a case.
 #include "common.cuh"
+#include "varlena.cuh"
 #include <cstring>
 
 namespace mob {
@@ -452,12 +453,7 @@ __global__ void __launch_bounds__(kThreads) select_flag_kernel(OrderSpec S, uint
     }
 }
 
-// ---- varlena keys: the one read-back record, and the run numbers of a sort by rounds ------------------------------------------------------
-struct VarlenaStat {
-    unsigned long long bad_inv[MO_ORDER_MAX_KEYS];   // ~(lowest row whose cell points outside the area), 0 = none
-    unsigned maxlen[MO_ORDER_MAX_KEYS];              // longest non-NULL value
-};
-
+// ---- varlena keys: the one read-back record (varlena.cuh), and the run numbers of a sort by rounds -----------------------------------------
 __global__ void __launch_bounds__(kThreads)
 varlena_stat_kernel(const uint8_t *__restrict__ cells, const uint64_t *__restrict__ nulls, const uint8_t *area, uint64_t area_sz, uint64_t n,
                     VarlenaStat *vs, int k) {
@@ -553,28 +549,25 @@ run_number_kernel(Pairs<uint64_t> B, const uint64_t *__restrict__ m_ptr, const R
     }
 }
 
-int segment_bits(int T) {
-    switch (T) {
-    case MO_T_BOOL: case MO_T_INT8: case MO_T_UINT8: return 8;
-    case MO_T_INT16: case MO_T_UINT16: case MO_T_YEAR: case MO_T_ENUM: return 16;
-    case MO_T_INT32: case MO_T_UINT32: case MO_T_FLOAT32: case MO_T_DATE: return 32;
-    case MO_T_INT64: case MO_T_UINT64: case MO_T_FLOAT64: case MO_T_TIME: case MO_T_DATETIME: case MO_T_TIMESTAMP: case MO_T_DECIMAL64: case MO_T_BIT:
-        return 64;
-    case MO_T_DECIMAL128: case MO_T_UUID: return 128;
-    }
-    return 0;
-}
-
-bool is_varlena(int T) {
-    switch (T) {
-    case MO_T_CHAR: case MO_T_VARCHAR: case MO_T_BINARY: case MO_T_VARBINARY: case MO_T_BLOB: case MO_T_TEXT: case MO_T_DATALINK: return true;
-    }
-    return false;
-}
+int segment_bits(int T) { return 8 * key_type_size(T); }
 
 }  // namespace
 
 namespace mob {
+
+int varlena_stat(ThreadCtx &t, const uint8_t *cells, const uint64_t *nulls, const uint8_t *area, uint64_t area_sz, uint64_t n, VarlenaStat *vs, int k) {
+    varlena_stat_kernel<<<grid_for(n), kThreads, 0, t.stream>>>(cells, nulls, area, area_sz, n, vs, k);
+    MOB_LAUNCH_CHECK();
+    return MO_RC_SUCCESS;
+}
+
+int varlena_stat_error(const VarlenaStat &vs, int ncols, const char *what) {
+    for (int k = 0; k < ncols; k++) {
+        if (vs.bad_inv[k]) { set_error("%s %d row %llu: the varlena cell points outside the area", what, k, ~vs.bad_inv[k]); return MO_RC_INVALID_ARGUMENT; }
+        if (vs.maxlen[k] > MO_ORDER_MAX_VARLENA) { set_error("%s %d has a %u-byte value, at most %d supported", what, k, vs.maxlen[k], MO_ORDER_MAX_VARLENA); return MO_RC_INVALID_ARGUMENT; }
+    }
+    return MO_RC_SUCCESS;
+}
 
 // Stable sort of m (device count, <= cap) pairs (k[0][i], v[0][i]) by the 32-bit key; the sorted rows end in v[0].  Used by JOIN_SELS and
 // the k-means centroid update (group_rows_stable, join.cu).
@@ -651,15 +644,13 @@ int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
         for (int k = 0; k < P.nkeys; k++) {
             if (!is_varlena(base[k].type)) continue;
             const uint64_t rows = base[k].cst ? 1 : len;
-            varlena_stat_kernel<<<grid_for(rows), kThreads, 0, t.stream>>>(base[k].col, base[k].nulls, base[k].area, base[k].area_sz, rows, vs, k);
-            MOB_LAUNCH_CHECK();
+            int rc = varlena_stat(t, base[k].col, base[k].nulls, base[k].area, base[k].area_sz, rows, vs, k);
+            if (rc) { st.finish(); return rc; }
         }
         int rc = read_back(t, &vstat, vs, sizeof vstat);
         if (rc) { st.finish(); return rc; }
-        for (int k = 0; k < P.nkeys; k++) {
-            if (vstat.bad_inv[k]) { st.finish(); set_error("order sels: key %d row %llu: the varlena cell points outside the area", k, ~vstat.bad_inv[k]); return MO_RC_INVALID_ARGUMENT; }
-            if (vstat.maxlen[k] > MO_ORDER_MAX_VARLENA) { st.finish(); set_error("order sels: key %d has a %u-byte value, at most %d supported", k, vstat.maxlen[k], MO_ORDER_MAX_VARLENA); return MO_RC_INVALID_ARGUMENT; }
-        }
+        rc = varlena_stat_error(vstat, P.nkeys, "order sels: key");
+        if (rc) { st.finish(); return rc; }
     }
     for (int k = 0; k < P.nkeys; k++) {
         const OrderSeg &b = base[k];

@@ -913,6 +913,7 @@ int tuning_set(const char *name, int value) {
     if (!strcmp(name, "q6_variant")) { if (value != 0 && value != 1) return -1; g_q6_variant = value; return 0; }
     if (!strcmp(name, "plan_specialise")) { g_plan_specialise = value; return 0; }
     if (!strcmp(name, "q1_variant")) { if (value != 0 && value != 1) return -1; g_q1_variant = value; return 0; }
+    if (!strcmp(name, "strkey_hash_bits")) { if (value < 0 || value > 63) return -1; g_strkey_hash_bits = value; return 0; }
     return -1;
 }
 

@@ -651,6 +651,121 @@ class GroupTable:
                                      Vector(data_ptr=keys_dev.ptr, data_nbytes=8 * n, length=n)], n)
 
 
+def _strkey_params(types, has_null):
+    if not 1 <= len(types) <= capi.STRKEY_MAX_COLS:
+        raise ValueError("1..%d key columns" % capi.STRKEY_MAX_COLS)
+    p = capi.StrKeyParams()
+    p.ncols, p.has_null = len(types), 1 if has_null else 0
+    for k, T in enumerate(types):
+        p.col_type[k] = int(T)
+    return p
+
+
+def pack_str_keys(cols, types, nulls=None, has_null=True, length=None, capacity=None):
+    """strHashmapIterator.encodeHashKeys (strhashmap.go:92-385): the byte-string key of every row.  cols: per key column a numpy array (fixed
+    width; a 1-element array = const), or for a varlena type a list of bytes or a (cells, area) pair in the vector layout; types: MO_T_* per
+    column; nulls: per column bitmap words or None.  Returns (key bytes uint8[], offsets uint64[n + 1], skip bitmap words or None): row i's key is
+    bytes[off[i]:off[i + 1]]; skip (has_null=False) marks the rows that join no group."""
+    data = []
+    for c in cols:
+        if isinstance(c, list):
+            c = varlena_bytes_column(c)
+        if isinstance(c, tuple):
+            cells = np.ascontiguousarray(c[0], dtype=np.uint8).reshape(-1)
+            data.append((cells, None if c[1] is None else np.ascontiguousarray(c[1], dtype=np.uint8), cells.shape[0] // 24))
+        else:
+            c = np.ascontiguousarray(c)
+            data.append((c.view(np.uint8).reshape(-1), None, c.shape[0]))
+    n = length if length is not None else max(d[2] for d in data)
+    nulls = list(nulls) if nulls is not None else [None] * len(cols)
+    off = np.zeros(n + 1, dtype=np.uint64)
+    skip = None if has_null else np.zeros((n + 63) // 64, dtype=np.uint64)
+    cap = capacity if capacity is not None else 16 * n
+    prm = _params_vec(_strkey_params(types, has_null))
+    while True:
+        out = np.zeros(max(cap, 1), dtype=np.uint8)
+        vecs = [Vector(data=out[:cap], length=cap), Vector(data=off, nulls=skip, length=n), prm]
+        vecs += [Vector(data=d, nulls=nl, area=a, length=rows) for (d, a, rows), nl in zip(data, nulls)]
+        rc, msg = xcall(capi.XCALL_PACK_STR_KEYS, vecs, n, raise_on_error=False)
+        if rc == capi.RC_OUT_OF_RANGE and capacity is None:       # off[n] holds the size needed
+            cap = int(off[n])
+            continue
+        if rc:
+            raise capi.MoError(rc, msg)
+        return out[:int(off[n])], off, skip
+
+
+def pack_str_keys_device(cols, nulls, types, n, bytes_dev, offsets_dev, skip_dev=None, has_null=True):
+    """the form on resident vectors: cols are DeviceBuffers or, for varlena types, (cells, area) DeviceBuffer pairs (area None: every value
+    inline); key bytes go to bytes_dev (its whole size is the capacity), offsets (uint64[n + 1]) to offsets_dev.  Reads back one record."""
+    nulls = list(nulls) if nulls is not None else [None] * len(cols)
+    vecs = [Vector(data_ptr=bytes_dev.ptr, data_nbytes=bytes_dev.nbytes, length=n),
+            Vector(data_ptr=offsets_dev.ptr, data_nbytes=8 * (n + 1), nulls_ptr=skip_dev.ptr if skip_dev is not None else None, length=n),
+            _params_vec(_strkey_params(types, has_null))]
+    for c, nl in zip(cols, nulls):
+        c, area = c if isinstance(c, tuple) else (c, None)
+        vecs.append(Vector(data_ptr=c.ptr, data_nbytes=c.nbytes, nulls_ptr=nl.ptr if nl is not None else None, length=n,
+                           area_ptr=area.ptr if area is not None else None, area_nbytes=area.nbytes if area is not None else 0))
+    xcall(capi.XCALL_PACK_STR_KEYS, vecs, n)
+
+
+class StrGroupTable:
+    """StrHashMap as the group operator sees it (the twin of GroupTable): insert(key bytes, offsets) -> 1-based group ids in first-seen order.
+    Owns the table: bytes, offsets (group g is bytes[offsets[g - 1]:offsets[g]]) and ngroups, and grows them when a batch does not fit."""
+
+    def __init__(self, capacity_groups=1024, capacity_bytes=1 << 16):
+        self.bytes = np.zeros(max(capacity_bytes, 1), dtype=np.uint8)
+        self.offsets = np.zeros(capacity_groups + 1, dtype=np.uint64)
+        self.ngroups = np.zeros(1, dtype=np.int64)
+
+    def _grow(self, groups, nbytes):
+        g = int(self.ngroups[0])
+        if groups + 1 > self.offsets.shape[0]:
+            o = np.zeros(groups + 1, dtype=np.uint64); o[:g + 1] = self.offsets[:g + 1]; self.offsets = o
+        if nbytes > self.bytes.shape[0]:
+            b = np.zeros(nbytes, dtype=np.uint8); used = int(self.offsets[g]); b[:used] = self.bytes[:used]; self.bytes = b
+
+    def insert(self, key_bytes, key_offsets, skip=None, first_rows=False):
+        """groups uint64[n] (0 = skipped row), and with first_rows the batch row that created each new group, in id order"""
+        kb = np.ascontiguousarray(key_bytes, dtype=np.uint8)
+        ko = np.ascontiguousarray(key_offsets, dtype=np.uint64)
+        n = ko.shape[0] - 1
+        groups = np.zeros(n, dtype=np.uint64)
+        fr = np.zeros(max(n, 1), dtype=np.int64) if first_rows else None
+        before = int(self.ngroups[0])
+        for attempt in range(2):
+            vecs = [Vector(data=groups, length=n), Vector(data=self.ngroups, length=1), Vector(data=self.bytes, length=self.bytes.shape[0]),
+                    Vector(data=self.offsets, length=self.offsets.shape[0]), Vector(data=kb, length=kb.shape[0]), Vector(data=ko, nulls=skip, length=n),
+                    Vector(data=fr, length=n) if first_rows else Vector(length=0)]
+            rc, msg = xcall(capi.XCALL_STR_GROUP_IDS, vecs, n, raise_on_error=False)
+            if rc == capi.RC_INVALID_ARGUMENT and "capacity" in msg and attempt == 0:
+                # at most n new groups and their bytes: this size always fits
+                used = int(self.offsets[before])
+                self._grow(max(2 * (self.offsets.shape[0] - 1), before + n), max(2 * self.bytes.shape[0], used + int(ko[n] - ko[0]) if n else used))
+                continue
+            if rc:
+                raise capi.MoError(rc, msg)
+            break
+        if first_rows:
+            return groups, fr[:int(self.ngroups[0]) - before]
+        return groups
+
+    def insert_device(self, bytes_dev, offsets_dev, n, groups_dev, d_ngroups, table_bytes_dev, table_offsets_dev, first_rows_dev=None, skip_dev=None):
+        """every vector resident (DeviceBuffer; d_ngroups may be a host int64[1] array instead); the table is the caller's and does not grow"""
+        ngv = Vector(data=d_ngroups, length=1) if isinstance(d_ngroups, np.ndarray) else Vector(data_ptr=d_ngroups.ptr, data_nbytes=8, length=1)
+        vecs = [Vector(data_ptr=groups_dev.ptr, data_nbytes=8 * n, length=n), ngv,
+                Vector(data_ptr=table_bytes_dev.ptr, data_nbytes=table_bytes_dev.nbytes, length=1),
+                Vector(data_ptr=table_offsets_dev.ptr, data_nbytes=table_offsets_dev.nbytes, length=1),
+                Vector(data_ptr=bytes_dev.ptr, data_nbytes=bytes_dev.nbytes, length=n),
+                Vector(data_ptr=offsets_dev.ptr, data_nbytes=8 * (n + 1), nulls_ptr=skip_dev.ptr if skip_dev is not None else None, length=n),
+                Vector(data_ptr=first_rows_dev.ptr, data_nbytes=8 * n, length=n) if first_rows_dev is not None else Vector(length=0)]
+        xcall(capi.XCALL_STR_GROUP_IDS, vecs, n)
+
+    def keys(self):
+        g, o = int(self.ngroups[0]), self.offsets
+        return [self.bytes[int(o[j]):int(o[j + 1])].tobytes() for j in range(g)]
+
+
 def group_agg(op, T, state, state_nulls, counts, groups, col, col_nulls=None, length=None):
     """BatchFill of one aggregate into caller-owned state arrays (numpy, modified in place): state uint64/int64/float64[ngroups] (8-byte slots),
     state_nulls bitmap words (group is NULL), counts int64[ngroups] or None.  Returns rc (0 or RC_OUT_OF_RANGE)."""
@@ -831,6 +946,119 @@ def normalize_l2(cells, area, length, dtype=np.float32, nulls=None):
 
 
 # ---------------------------------------------------------------------------------------------- hash join (csrc/join.cu)
+def _group_sels(groups, ngroups, nbuild):
+    """JOIN_SELS: (offsets, sels) of the build rows by group, or (None, None) when GroupSels.Finalize keeps none (joinMapMsg.go:83-89): every
+    group has one row, or nothing was inserted (every key NULL)"""
+    if ngroups == nbuild:
+        return None, None
+    offsets = np.zeros(ngroups + 2, dtype=np.int32)
+    sels = np.zeros(max(nbuild, 1), dtype=np.int32)
+    cnt = np.zeros(1, dtype=np.int64)
+    xcall(capi.XCALL_JOIN_SELS, [Vector(data=offsets, length=ngroups + 2), Vector(data=sels, length=nbuild), Vector(data=cnt, length=1),
+                                 Vector(data=groups, length=nbuild)], nbuild)
+    if int(cnt[0]) == 0:
+        return None, None
+    return offsets, sels[:int(cnt[0])]
+
+
+def _probe_with(call, n, capacity):
+    """the JOIN_PROBE capacity protocol: call(op, ob, cnt) -> (rc, msg); a too-small buffer reports the count and the call is repeated"""
+    cap = capacity if capacity is not None else max(2 * n, 1024)
+    while True:
+        op, ob, cnt = np.zeros(cap, np.int64), np.zeros(cap, np.int64), np.zeros(1, np.int64)
+        rc, msg = call(op, ob, cnt)
+        if rc == capi.RC_OUT_OF_RANGE and capacity is None:
+            cap = int(cnt[0])
+            continue
+        if rc:
+            raise capi.MoError(rc, msg)
+        return op[:int(cnt[0])], ob[:int(cnt[0])]
+
+
+class StrJoinMap:
+    """message.JoinMap over byte-string keys (the twin of JoinMap; HashmapBuilder with varlena or wide keys, hashbuild/hashmap.go:110-116,258-275):
+    the build side's StrHashMap (StrGroupTable) and its GroupSels.  Keys are PACK_STR_KEYS bytes + offsets; probe = STR_JOIN_FIND + JOIN_PROBE_GIDS."""
+
+    def __init__(self, build_bytes, build_offsets, skip=None, prepare=True):
+        ko = np.ascontiguousarray(build_offsets, dtype=np.uint64)
+        self.nbuild = ko.shape[0] - 1
+        tab = StrGroupTable(max(self.nbuild, 1), max(int(ko[-1] - ko[0]), 1))
+        groups = tab.insert(build_bytes, ko, skip)
+        self.ngroups = int(tab.ngroups[0])
+        self.table_offsets = tab.offsets[:self.ngroups + 1].copy()
+        self.table_bytes = tab.bytes[:int(self.table_offsets[-1])].copy()
+        self.offsets, self.sels = _group_sels(groups, self.ngroups, self.nbuild)
+        self.prepared = False
+        if prepare and self.ngroups:
+            lib = capi.load_library()
+            capi.check(lib.MoB200_StrJoinMapPrepare(self.table_bytes.ctypes.data, self.table_offsets.ctypes.data, self.ngroups), lib)
+            self.prepared = True
+
+    def hash_on_unique(self):
+        return self.offsets is None
+
+    def _table(self):
+        return [Vector(data=np.array([self.ngroups], np.int64), length=1), Vector(data=self.table_bytes, length=len(self.table_bytes)),
+                Vector(data=self.table_offsets, length=self.ngroups + 1)]
+
+    def find(self, key_bytes, key_offsets, nulls=None):
+        """strHashmapIterator.Find: 1-based group id per probe key, 0 = no match"""
+        ko = np.ascontiguousarray(key_offsets, dtype=np.uint64)
+        n = ko.shape[0] - 1
+        vals = np.zeros(n, dtype=np.uint64)
+        kb = np.ascontiguousarray(key_bytes, dtype=np.uint8)
+        xcall(capi.XCALL_STR_JOIN_FIND, [Vector(data=vals, length=n)] + self._table() + [Vector(data=kb, length=len(kb)), Vector(data=ko, nulls=nulls, length=n)], n)
+        return vals
+
+    def probe(self, key_bytes, key_offsets, join_type=capi.JOIN_INNER, nulls=None, capacity=None):
+        """(probe rows, build rows) of the join result in the reference's emission order, as JoinMap.probe"""
+        return probe_gids(self.find(key_bytes, key_offsets, nulls), self.ngroups, self.offsets, self.sels, join_type, capacity)
+
+    def release(self):
+        if self.prepared:
+            lib = capi.load_library()
+            lib.MoB200_JoinMapRelease(self.table_offsets.ctypes.data)
+            self.prepared = False
+
+
+def str_join_find_device(vals_dev, n, ngroups, table_bytes_dev, table_offsets_dev, bytes_dev, offsets_dev, nulls_dev=None):
+    """STR_JOIN_FIND on resident vectors (DeviceBuffers): enqueues the lookup of n probe keys (bytes_dev, offsets_dev uint64[n + 1]) in a table
+    STR_GROUP_IDS built (ngroups is a host int); vals_dev (uint64[n]) holds the ids once the calling thread's stream has run it"""
+    xcall(capi.XCALL_STR_JOIN_FIND, [Vector(data_ptr=vals_dev.ptr, data_nbytes=8 * n, length=n), Vector(data=np.array([ngroups], np.int64), length=1),
+                                     Vector(data_ptr=table_bytes_dev.ptr, data_nbytes=table_bytes_dev.nbytes, length=1),
+                                     Vector(data_ptr=table_offsets_dev.ptr, data_nbytes=8 * (ngroups + 1), length=1),
+                                     Vector(data_ptr=bytes_dev.ptr, data_nbytes=bytes_dev.nbytes, length=n),
+                                     Vector(data_ptr=offsets_dev.ptr, data_nbytes=8 * (n + 1), nulls_ptr=nulls_dev.ptr if nulls_dev is not None else None, length=n)], n)
+
+
+def probe_gids_device(vals_dev, n, ngroups, offsets_dev, sels_dev, join_type, out_probe_dev, out_build_dev, count_dev):
+    """JOIN_PROBE_GIDS on resident vectors: the pairs go to out_probe_dev / out_build_dev (int64, their size is the capacity) and their count to
+    count_dev; offsets_dev / sels_dev None = unique map.  Reads the count back (RC_OUT_OF_RANGE: the buffers are too small, the count is written)."""
+    prm = np.array([join_type, 0], dtype=np.int32)
+    vecs = [Vector(data_ptr=out_probe_dev.ptr, data_nbytes=out_probe_dev.nbytes, length=1), Vector(data_ptr=out_build_dev.ptr, data_nbytes=out_build_dev.nbytes, length=1),
+            Vector(data_ptr=count_dev.ptr, data_nbytes=8, length=1), Vector(data=prm.view(np.uint8), length=1), Vector(data=np.array([ngroups], np.int64), length=1),
+            Vector(data_ptr=offsets_dev.ptr, data_nbytes=offsets_dev.nbytes, length=ngroups + 2) if offsets_dev is not None else Vector(length=0),
+            Vector(data_ptr=sels_dev.ptr, data_nbytes=sels_dev.nbytes, length=1) if sels_dev is not None else Vector(length=0),
+            Vector(data_ptr=vals_dev.ptr, data_nbytes=8 * n, length=n)]
+    xcall(capi.XCALL_JOIN_PROBE_GIDS, vecs, n)
+
+
+def probe_gids(vals, ngroups, offsets, sels, join_type=capi.JOIN_INNER, capacity=None):
+    """JOIN_PROBE_GIDS: the JOIN_PROBE emission over given group ids (JOIN_FIND's or STR_JOIN_FIND's vals); offsets / sels None = unique map"""
+    v = np.ascontiguousarray(vals, dtype=np.uint64)
+    n = v.shape[0]
+    prm = np.array([join_type, 0], dtype=np.int32)
+
+    def call(op, ob, cnt):
+        vecs = [Vector(data=op, length=len(op)), Vector(data=ob, length=len(ob)), Vector(data=cnt, length=1), Vector(data=prm.view(np.uint8), length=1),
+                Vector(data=np.array([ngroups], np.int64), length=1),
+                Vector(data=offsets, length=ngroups + 2) if offsets is not None else Vector(length=0),
+                Vector(data=sels, length=len(sels)) if sels is not None else Vector(length=0),
+                Vector(data=v, length=n)]
+        return xcall(capi.XCALL_JOIN_PROBE_GIDS, vecs, n, raise_on_error=False)
+    return _probe_with(call, n, capacity)
+
+
 class JoinMap:
     """message.JoinMap for equality joins over <= 8-byte packed keys (pkg/vm/message/joinMapMsg.go:127-210): the build side's IntHashMap
     (GroupTable: first-seen group ids + key table) and its GroupSels.  HashOnUnique (every build row its own group) keeps no sels."""
@@ -842,16 +1070,7 @@ class JoinMap:
         groups = tab.insert(k, skip)                                   # HashmapBuilder.BuildHashmap: itr.Insert (hashmap.go:340-360)
         self.ngroups = int(tab.ngroups[0])
         self.table_keys = np.ascontiguousarray(tab.keys[:max(self.ngroups, 1)])[:self.ngroups].copy() if self.ngroups else np.zeros(0, np.uint64)
-        self.offsets = self.sels = None
-        if self.ngroups != self.nbuild:                                 # GroupSels.Finalize keeps sels only when some group has != 1 row (joinMapMsg.go:83-89)
-            self.offsets = np.zeros(self.ngroups + 2, dtype=np.int32)
-            self.sels = np.zeros(max(self.nbuild, 1), dtype=np.int32)
-            cnt = np.zeros(1, dtype=np.int64)
-            xcall(capi.XCALL_JOIN_SELS, [Vector(data=self.offsets, length=self.ngroups + 2), Vector(data=self.sels, length=self.nbuild), Vector(data=cnt, length=1),
-                                         Vector(data=groups, length=self.nbuild)], self.nbuild)
-            self.sels = self.sels[:int(cnt[0])]
-            if int(cnt[0]) == 0:                                       # nothing inserted (every key NULL): Finalize keeps no sels (joinMapMsg.go:83-89)
-                self.offsets = self.sels = None
+        self.offsets, self.sels = _group_sels(groups, self.ngroups, self.nbuild)
         self.prepared = False
         if prepare and self.ngroups:
             lib = capi.load_library()
@@ -873,22 +1092,16 @@ class JoinMap:
         """(probe rows, build rows) of the join result in the reference's emission order; build row -1 = no build side (left outer / semi / anti)"""
         k = np.ascontiguousarray(keys, dtype=np.uint64)
         n = k.shape[0]
-        cap = capacity if capacity is not None else max(2 * n, 1024)
         prm = np.array([join_type, 0], dtype=np.int32)
-        while True:
-            op, ob, cnt = np.zeros(cap, np.int64), np.zeros(cap, np.int64), np.zeros(1, np.int64)
-            vecs = [Vector(data=op, length=cap), Vector(data=ob, length=cap), Vector(data=cnt, length=1), Vector(data=prm.view(np.uint8), length=1),
+
+        def call(op, ob, cnt):
+            vecs = [Vector(data=op, length=len(op)), Vector(data=ob, length=len(ob)), Vector(data=cnt, length=1), Vector(data=prm.view(np.uint8), length=1),
                     Vector(data=self.table_keys, length=self.ngroups),
                     Vector(data=self.offsets, length=self.ngroups + 2) if self.offsets is not None else Vector(length=0),
                     Vector(data=self.sels, length=len(self.sels)) if self.sels is not None else Vector(length=0),
                     Vector(data=k, nulls=nulls, length=n)]
-            rc, msg = xcall(capi.XCALL_JOIN_PROBE, vecs, n, raise_on_error=False)
-            if rc == capi.RC_OUT_OF_RANGE and capacity is None:       # the count was reported: size the buffers and ask again
-                cap = int(cnt[0])
-                continue
-            if rc:
-                raise capi.MoError(rc, msg)
-            return op[:int(cnt[0])], ob[:int(cnt[0])]
+            return xcall(capi.XCALL_JOIN_PROBE, vecs, n, raise_on_error=False)
+        return _probe_with(call, n, capacity)
 
     def release(self):
         if self.prepared:
