@@ -190,12 +190,13 @@ typedef struct mo_xcall_args_t {
 /* Wider results: dataSz >= 16 adds the non-null row count at pdata+8; dataSz >= 24 makes the result a PARTIAL STATE
  * mo_agg_state_t {value bits (SUM/AVG: the sum in the SUM return type; AVG is NOT divided yet), non-null rows, rc} -- what a partial
  * Group hands to MergeGroup (pkg/sql/colexec/group/mergeGroup.go:132-247).
- * Asynchronous form: when the column AND the result (pdata, pnulls) are DEVICE pointers the call only enqueues work on the calling
- * thread's stream and returns MO_RC_SUCCESS at once; errors detected on the device (SUM overflow) are reported in state.rc. */
+ * Asynchronous form: when the column, its nulls bitmap and the result (pdata, pnulls) are all DEVICE pointers (or NULL) the call only
+ * enqueues work on the calling thread's stream and returns MO_RC_SUCCESS at once; errors detected on the device (SUM overflow) are
+ * reported in state.rc.  Any host pointer among them, a column-cache hit included, makes the call synchronous. */
 typedef struct mo_agg_state_t { uint64_t bits; int64_t count; int64_t rc; } mo_agg_state_t;
 /* MergeGroup for these aggregates: args [0] result (8 / 16 / 24 bytes as above, + nulls word) ; [1] len partial states (24 bytes each),
  * folded in order with the reference's BatchMerge rules (sumavg2.go:205-248 incl. int64OfCheck / uint64OfCheck, minmax2.go:90-110).
- * Device pointers on both sides: asynchronous as above. */
+ * Device partials and a device result (pdata and pnulls): asynchronous as above. */
 #define MO_XCALL_AGG_MERGE(op, T) (0x1800 + ((op) << 8) + (T))
 
 /* --- new: fused TPC-H Q6 shape  SUM(a*b) WHERE d in [d_lo,d_hi) AND b BETWEEN b_lo AND b_hi AND c < c_hi
@@ -226,8 +227,9 @@ typedef struct { int32_t div0_null; int32_t reserved; int64_t err_row; } mo_go_p
 #define MO_XCALL_GO_MULTI_AND 0x5100
 #define MO_XCALL_GO_MULTI_OR 0x5101
 
-/* ---- the standalone column operators of the colexec pipeline (csrc/colops.cu).  Host or device pointers; with device pointers on
- * every vector FILTER_SELS and SHUFFLE only enqueue work (asynchronous form, as MO_XCALL_AGG).
+/* ---- the standalone column operators of the colexec pipeline (csrc/colops.cu).  Host or device pointers; when every data pointer and
+ * nulls bitmap of every vector is a device pointer (or NULL) FILTER_SELS and SHUFFLE only enqueue work (asynchronous form, as
+ * MO_XCALL_AGG).
  *
  * FILTER_SELS  Filter.Call inner loop (filter.go:116-152): rows with (!null && true), ascending.
  *              args: [0] sels int64[] (a host buffer only has to hold the selected rows) ; [1] count int64[1] ; [2] bool vector (+pnulls).  len = rows
@@ -453,9 +455,9 @@ typedef struct mo_q6_params_t {
 } mo_q6_params_t;
 
 /* Asynchronous form: device columns AND a device result (pdata 16 bytes = {f64 sum, i64 qualifying rows}, pnulls device or NULL): the
- * call enqueues the kernel on the calling thread's stream and returns at once.
+ * call enqueues the kernel on the calling thread's stream and returns at once.  A host column or result word makes it synchronous.
  * MO_XCALL_Q6_MERGE (MergeGroup): args [0] result as above ; [1] len partial results of 16 bytes each, added in order; an empty partial
- * (count 0) is NULL and skipped (sumavg2.go:222-236). */
+ * (count 0) is NULL and skipped (sumavg2.go:222-236).  Asynchronous when the partials, pdata and pnulls are device pointers. */
 #define MO_XCALL_Q6_MERGE 0x2002
 
 /* --- new: fused TPC-H Q1 shape: filter d <= cutoff, group by two 1-byte keys, 8 aggregates (q1.sql:5-12).

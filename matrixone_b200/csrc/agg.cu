@@ -380,23 +380,21 @@ int xcall_agg_merge(int op, int T, mo_xcall_args_t *args, uint64_t len) {
     if (!args[0].pdata || args[0].dataSz < 8 || args[1].dataSz < 24 * len) { set_error("agg merge: result needs 8 bytes, partial states 24 bytes each"); return MO_RC_INVALID_ARGUMENT; }
     const bool is_signed = T >= MO_T_INT8 && T <= MO_T_INT64, is_unsigned = T >= MO_T_UINT8 && T <= MO_T_UINT64;
     const int cls = op == MO_AGG_COUNT ? C_COUNT : (op == MO_AGG_MIN || op == MO_AGG_MAX) ? C_MINMAX : is_signed ? C_SIGNED : is_unsigned ? C_UNSIGNED : C_FLOAT;
-    const bool async = is_device_ptr(args[0].pdata) && (len == 0 || is_device_ptr(args[1].pdata));
     Stager st(t);
     const uint64_t *dparts = (const uint64_t *)st.in(args[1].pdata, 24 * len);
     uint64_t *dres = (uint64_t *)st.out(args[0].pdata, args[0].dataSz >= 24 ? 24 : args[0].dataSz >= 16 ? 16 : 8);
     uint64_t *dn = (uint64_t *)st.out(args[0].pnulls, args[0].pnulls ? 8 : 0);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
-    int64_t *drc = async ? nullptr : (int64_t *)st.tmp(8);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    // the asynchronous form leaves errors in the merged state's rc word; the synchronous form copies the rc back with the results
+    const bool async = st.resident();
+    int64_t hrc = 0;
+    int64_t *drc = async ? nullptr : (int64_t *)st.out(&hrc, 8);
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     agg_merge_kernel<<<1, 1, 0, t.stream>>>(dparts, len, op, T, cls, dres, args[0].dataSz / 8, dn, drc);
     MOB_LAUNCH_CHECK();
-    if (async) { st.release_async(); return MO_RC_SUCCESS; }   // the merged state's rc word carries errors
-    int rc = MO_RC_SUCCESS;
-    int64_t hrc = 0;
-    int r2 = read_back(t, &hrc, drc, 8);
-    if (r2) rc = r2; else if (hrc) { rc = (int)hrc; set_error("data out of range: merged SUM overflows its 64-bit state"); }
-    int frc = st.finish();
-    return rc ? rc : frc;
+    const int rc = st.complete();
+    if (rc || async) return rc;
+    if (hrc) set_error("data out of range: merged SUM overflows its 64-bit state");
+    return (int)hrc;
 }
 
 int bitmap_count_device(ThreadCtx &t, const uint64_t *dp, uint64_t nbits, uint64_t *count) {
@@ -408,7 +406,7 @@ int bitmap_count_device(ThreadCtx &t, const uint64_t *dp, uint64_t nbits, uint64
 }
 
 // XCall family MO_XCALL_AGG(op, T): args[0] = result, args[1] = column.  See include/mo_b200.h.
-// When the column AND the result live in device memory the call only enqueues work on the calling thread's stream: no read-back, no
+// When the column, the result and their nulls words live in device memory the call only enqueues work on the calling thread's stream: no read-back, no
 // synchronisation.  This is what lets a multi-GPU caller hand the partial state straight to NCCL (MergeGroup seam, mergeGroup.go:132-247)
 // and merge on the device.  Otherwise the same kernels write staged buffers, and the call returns the state's rc.
 int xcall_agg(int op, int T, mo_xcall_args_t *args, uint64_t len) {
@@ -422,19 +420,18 @@ int xcall_agg(int op, int T, mo_xcall_args_t *args, uint64_t len) {
     const bool is_signed = T >= MO_T_INT8 && T <= MO_T_INT64, is_unsigned = T >= MO_T_UINT8 && T <= MO_T_UINT64;
     const int cls = op == MO_AGG_COUNT ? C_COUNT : (op == MO_AGG_MIN || op == MO_AGG_MAX) ? C_MINMAX : is_signed ? C_SIGNED : is_unsigned ? C_UNSIGNED : C_FLOAT;
     if (cls == C_FLOAT && T != MO_T_FLOAT32 && T != MO_T_FLOAT64) { set_error("sum: unsupported type %d", T); return MO_RC_INVALID_ARGUMENT; }
-    const bool async = is_device_ptr(args[0].pdata) && (len == 0 || is_device_ptr(args[1].pdata)) && (!args[0].pnulls || is_device_ptr(args[0].pnulls)) &&
-                       (!args[1].pnulls || is_device_ptr(args[1].pnulls));
     Stager st(t);
     const void *dcol = st.in(args[1].pdata, (size_t)sz * len);
     const uint64_t *dnulls = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? ((len + 63) / 64) * 8 : 0);
     // 1 word: the value; 2: + non-null rows; 3: + rc (the partial state MO_XCALL_AGG_MERGE folds)
     const uint64_t words = args[0].dataSz >= 24 ? 3 : args[0].dataSz / 8;
     // the synchronous form stages the host results and the rc word as one block: one copy back, as for an 8192-row call it is most of the cost
+    const bool hres = !st.device(args[0].pdata), hnulls = !st.device(args[0].pnulls);
+    const bool async = st.resident();
     struct { uint64_t words[3], nulls; int64_t rc; } h{};
     uint64_t *dh = async ? nullptr : (uint64_t *)st.out(&h, sizeof h);
-    const bool hres = !async && !is_device_ptr(args[0].pdata), hnulls = !async && args[0].pnulls && !is_device_ptr(args[0].pnulls);
     const AggStateOut so{hres ? dh : (uint64_t *)args[0].pdata, words, hnulls ? dh + 3 : args[0].pnulls, async ? nullptr : (int64_t *)dh + 4, op, cls};
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     int rc = MO_RC_SUCCESS;
     if (op == MO_AGG_COUNT || len == 0) {
         unsigned long long *dcount = nullptr;
@@ -462,9 +459,8 @@ int xcall_agg(int op, int T, mo_xcall_args_t *args, uint64_t len) {
         }
         if (rc) return rc;
     }
-    if (async) { st.release_async(); return MO_RC_SUCCESS; }   // the state's rc word carries errors
-    rc = st.finish();
-    if (rc) return rc;
+    rc = st.complete();
+    if (rc || async) return rc;   // the asynchronous form leaves errors in the state's rc word
     if (hres) memcpy(args[0].pdata, h.words, 8 * words);
     if (hnulls) memcpy(args[0].pnulls, &h.nulls, 8);
     return (int)h.rc;

@@ -540,7 +540,7 @@ int run_group_agg(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len, int is_avg)
     const T *col = (const T *)st.in(args[3].pdata, KIND == G_COUNT ? 0 : len * sizeof(T));
     const uint64_t *nulls = (const uint64_t *)st.in(args[3].pnulls, args[3].pnulls ? nwords * 8 : 0);
     unsigned long long *tmp = (unsigned long long *)st.tmp(ngroups * 8 * 4 + ngroups + 64);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     AggTemp A{tmp, tmp + ngroups, tmp + 2 * ngroups, tmp + 3 * ngroups};
     uint8_t *needs_serial = (uint8_t *)(tmp + 4 * ngroups);
     unsigned long long *status = (unsigned long long *)(needs_serial + ((ngroups + 15) & ~15ull));
@@ -609,20 +609,19 @@ int xcall_filter_sels(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     if (!args[1].pdata || args[1].dataSz < 8 || args[2].dataSz < len) { set_error("filter sels: count needs 8 bytes, the bool vector len bytes"); return MO_RC_INVALID_ARGUMENT; }
-    const bool dev = is_device_ptr(args[0].pdata) && is_device_ptr(args[1].pdata) && (len == 0 || is_device_ptr(args[2].pdata));
     Stager st(t);
     const uint8_t *v = (const uint8_t *)st.in(args[2].pdata, len);
     const uint64_t *nulls = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? ((len + 63) / 64) * 8 : 0);
     // a host caller's sels buffer only has to hold the selected rows: compact into scratch, copy back `count` entries
-    const bool host_out = !is_device_ptr(args[0].pdata);
+    const bool host_out = !st.device(args[0].pdata);
     int64_t *sels = host_out ? (int64_t *)st.tmp(len * 8 + 8) : (int64_t *)args[0].pdata;
     unsigned long long *dcount = (unsigned long long *)st.out(args[1].pdata, 8);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     cudaEventRecord(t.kev0, t.stream);
     int rc = launch_select<int64_t>(t, v, nulls, len, sels, dcount);
     cudaEventRecord(t.kev1, t.stream);
     if (rc) { st.finish(); return rc; }
-    if (dev) { st.release_async(); return MO_RC_SUCCESS; }   // asynchronous form: everything stays on the device
+    if (st.resident()) return st.complete();   // asynchronous form: everything stays on the device
     unsigned long long cnt = 0;
     rc = read_back(t, &cnt, dcount, 8);
     if (rc) { st.finish(); return rc; }
@@ -630,7 +629,7 @@ int xcall_filter_sels(mo_xcall_args_t *args, uint64_t len) {
         if (cnt * 8 > args[0].dataSz) { st.finish(); set_error("filter sels: %llu rows selected, the sels buffer holds %llu", cnt, (unsigned long long)(args[0].dataSz / 8)); return MO_RC_INVALID_ARGUMENT; }
         if (cnt) MOB_CUDA_TRY(cudaMemcpyAsync(args[0].pdata, sels, cnt * 8, cudaMemcpyDeviceToHost, t.stream));
     }
-    return st.finish();
+    return st.complete();
 }
 
 // MO_XCALL_SHUFFLE(szof): args [0] dst (szof bytes x len, + pnulls out) ; [1] src (+pnulls, nullCnt = its bit length) ; [2] sels int64[len]
@@ -640,7 +639,6 @@ int xcall_shuffle(int szof, mo_xcall_args_t *args, uint64_t len) {
     if (szof != 1 && szof != 2 && szof != 4 && szof != 8 && szof != 16 && szof != 24) { set_error("shuffle: element size %d (1, 2, 4, 8, 16 or 24 = varlena cell)", szof); return MO_RC_INVALID_ARGUMENT; }
     if (args[0].dataSz < (uint64_t)szof * len || args[2].dataSz < 8 * len) { set_error("shuffle: dst / sels shorter than len"); return MO_RC_INVALID_ARGUMENT; }
     if (len == 0) return MO_RC_SUCCESS;
-    const bool dev = is_device_ptr(args[0].pdata) && is_device_ptr(args[1].pdata) && is_device_ptr(args[2].pdata);
     Stager st(t);
     void *dst = st.out(args[0].pdata, (size_t)szof * len);
     const void *src = st.in(args[1].pdata, args[1].dataSz);
@@ -649,7 +647,7 @@ int xcall_shuffle(int szof, mo_xcall_args_t *args, uint64_t len) {
     const uint64_t *snulls = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? ((snull_bits + 63) / 64) * 8 : 0);
     const int64_t *sels = (const int64_t *)st.in(args[2].pdata, 8 * len);
     uint32_t *dnulls = (uint32_t *)st.out(args[0].pnulls, args[0].pnulls ? ((len + 63) / 64) * 8 : 0);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     int grid = num_sms() * 8;
     const uint64_t work = (len + kThreads - 1) / kThreads;
     if ((uint64_t)grid > work) grid = (int)work;
@@ -664,8 +662,7 @@ int xcall_shuffle(int szof, mo_xcall_args_t *args, uint64_t len) {
     }
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
-    if (dev) { st.release_async(); return MO_RC_SUCCESS; }
-    return st.finish();
+    return st.complete();
 }
 
 // MO_XCALL_PACK_KEYS: args [0] keys uint64[len] (+ pnulls out: rows that join no group, has_null = 0 only) ; [1] params {int32 ncols, int32 has_null} ;
@@ -695,7 +692,7 @@ int xcall_pack_keys(mo_xcall_args_t *args, uint64_t len) {
     if (total > 8) { st.finish(); set_error("pack keys: %d key bytes exceed the 8-byte IntHashMap key (group/exec2.go:73-118)", total); return MO_RC_INVALID_ARGUMENT; }
     uint64_t *keys = (uint64_t *)st.out(args[0].pdata, 8 * len);
     uint32_t *skip = (uint32_t *)st.out(args[0].pnulls, args[0].pnulls ? ((len + 63) / 64) * 8 : 0);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     int grid = num_sms() * 8;
     const uint64_t work = (len + kThreads - 1) / kThreads;
     if ((uint64_t)grid > work) grid = (int)work;
@@ -733,7 +730,7 @@ int xcall_group_ids(mo_xcall_args_t *args, uint64_t len) {
     uint8_t *isfirst = (uint8_t *)st.tmp(total + 16);
     uint32_t *firsts = (uint32_t *)st.tmp(total * 4 + 16);
     unsigned long long *dcount = (unsigned long long *)st.tmp(16);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     unsigned *overflow = (unsigned *)(dcount + 1);
     MOB_CUDA_TRY(cudaMemsetAsync(dcount, 0, 16, t.stream));
     // id first: the keys and first rows the insert kernel reads are then the most recently written lines in L2
@@ -770,7 +767,6 @@ int xcall_pack_str_keys(mo_xcall_args_t *args, uint64_t len) {
     memcpy(&P, args[2].pdata, sizeof P);
     if (P.ncols < 1 || P.ncols > MO_STRKEY_MAX_COLS) { set_error("pack str keys: %d key columns (1..%d)", P.ncols, MO_STRKEY_MAX_COLS); return MO_RC_INVALID_ARGUMENT; }
     if (!args[1].pdata || args[1].dataSz < 8 * (len + 1)) { set_error("pack str keys: the offsets need len + 1 entries"); return MO_RC_INVALID_ARGUMENT; }
-    bool dev = is_device_ptr(args[1].pdata) && (!args[1].pnulls || is_device_ptr(args[1].pnulls)) && (!args[0].pdata || is_device_ptr(args[0].pdata));
     Stager st(t);
     StrKeyCols K;
     memset(&K, 0, sizeof K);
@@ -789,19 +785,16 @@ int xcall_pack_str_keys(mo_xcall_args_t *args, uint64_t len) {
         K.nulls[k] = (const uint64_t *)st.in(a.pnulls, a.pnulls ? ((rows + 63) / 64) * 8 : 0);
         K.size[k] = var ? 0 : (int)esz;
         K.cst[k] = cst ? 1 : 0;
-        if (a.pdata && rows) dev = dev && is_device_ptr(a.pdata);
-        if (a.pnulls) dev = dev && is_device_ptr(a.pnulls);
         if (var && a.parea && a.areaSz) {
             K.area[k] = (const uint8_t *)st.in(a.parea, a.areaSz);
             K.area_sz[k] = a.areaSz;
-            dev = dev && is_device_ptr(a.parea);
         }
     }
     uint64_t *off = (uint64_t *)st.out(args[1].pdata, 8 * (len + 1));
     uint32_t *skip = (uint32_t *)st.out(args[1].pnulls, args[1].pnulls ? ((len + 63) / 64) * 8 : 0);
     struct Rec { VarlenaStat vs; uint64_t total; };
     Rec *rec = (Rec *)st.tmp(sizeof(Rec));
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(rec, 0, sizeof(Rec), t.stream));
     for (int k = 0; k < K.n; k++) {
         if (K.size[k] || !len) continue;
@@ -831,14 +824,13 @@ int xcall_pack_str_keys(mo_xcall_args_t *args, uint64_t len) {
         return MO_RC_OUT_OF_RANGE;
     }
     uint8_t *bytes = (uint8_t *)st.out(args[0].pdata, h.total);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     if (len) {
         strkey_write_kernel<<<grid, kThreads, 0, t.stream>>>(K, len, P.has_null, off, bytes);
         MOB_LAUNCH_CHECK();
     }
     cudaEventRecord(t.kev1, t.stream);
-    if (dev) { st.release_async(); return MO_RC_SUCCESS; }
-    return st.finish();
+    return st.complete();
 }
 
 // MO_XCALL_STR_GROUP_IDS: args [0] groups uint64[len] ; [1] int64 ngroups (in/out) ; [2] table bytes u8[cap_bytes] ; [3] table offsets
@@ -869,9 +861,6 @@ int xcall_str_group_ids(mo_xcall_args_t *args, uint64_t len) {
     if (want < 16) want = 16;
     uint64_t cap = 32;
     while (cap < 2 * want) cap <<= 1;
-    // asynchronous only when every output is device memory: a host ngroups must be copied back, so such a call finishes synchronously
-    const bool dev = is_device_ptr(args[0].pdata) && is_device_ptr(args[1].pdata) && is_device_ptr(args[2].pdata) && is_device_ptr(args[3].pdata) &&
-                     is_device_ptr(args[5].pdata) && (len == 0 || is_device_ptr(args[4].pdata)) && (!args[5].pnulls || is_device_ptr(args[5].pnulls)) && (!want_first || is_device_ptr(args[6].pdata));
     Stager st(t);
     uint64_t *groups = (uint64_t *)st.out(args[0].pdata, 8 * len);
     int64_t *dng = (int64_t *)st.out(args[1].pdata, 8, true);
@@ -889,7 +878,7 @@ int xcall_str_group_ids(mo_xcall_args_t *args, uint64_t len) {
     uint32_t *firsts = (uint32_t *)st.tmp(total * 4 + 16);
     uint64_t *lens = (uint64_t *)st.tmp(len * 8 + 16);
     unsigned long long *rec = (unsigned long long *)st.tmp(32);   // [0] groups after the call, [1] overflow bits, [2] new key bytes, [3] toff[nexist]
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     unsigned *overflow = (unsigned *)(rec + 1);
     MOB_CUDA_TRY(cudaMemsetAsync(rec, 0, 32, t.stream));
     MOB_CUDA_TRY(cudaMemsetAsync(T.id, 0, (cap + 1) * 8, t.stream));
@@ -918,8 +907,7 @@ int xcall_str_group_ids(mo_xcall_args_t *args, uint64_t len) {
     rc = read_back(t, h, rec, sizeof h);
     if (rc) { st.finish(); return rc; }
     const unsigned hov = (unsigned)h[1];
-    if (!hov && dev) { st.release_async(); return MO_RC_SUCCESS; }
-    int frc = st.finish();
+    int frc = st.complete();
     if (hov & 1) { set_error("str group ids: more than %llu distinct keys; the table holds %llu groups and %llu bytes (capacity)", (unsigned long long)cap, (unsigned long long)cap_groups, (unsigned long long)cap_bytes); return MO_RC_INVALID_ARGUMENT; }
     if (hov) { set_error("str group ids: the groups need %llu groups and %llu bytes; the table holds %llu groups and %llu bytes (capacity)", h[0], h[3] + h[2], (unsigned long long)cap_groups, (unsigned long long)cap_bytes); return MO_RC_INVALID_ARGUMENT; }
     return frc;

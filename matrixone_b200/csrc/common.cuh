@@ -62,6 +62,8 @@ inline ArenaMark arena_mark(ThreadCtx &t) { return ArenaMark{t.cur_block, t.cur_
 inline void arena_rewind(ThreadCtx &t, ArenaMark m) { t.cur_block = m.block; t.cur_off = m.off; }
 
 // --- Stager: makes every pointer argument a device pointer for the duration of one call -------------------
+// It also decides how the call completes: a call that met only device memory is asynchronous (complete() enqueues nothing more and does
+// not synchronise); a call that met any host range, a column-cache hit included, copies back and synchronises once.
 struct Stager {
     ThreadCtx &t;
     struct Back { void *host; const void *dev; size_t bytes; };
@@ -75,13 +77,20 @@ struct Stager {
     // output: device pointers pass through; host pointers get an arena buffer that is copied back by finish().
     // preload=true first uploads the host content (needed when the kernel writes only some rows).
     void *out(void *p, size_t bytes, bool preload = false);
+    // classify a pointer the call reads or writes without staging it (a null pointer names no memory); a host answer counts as in() / out()
+    bool device(const void *p) { if (!p || is_device_ptr(p)) return true; host_seen = true; return false; }
+    // no host range met so far
+    bool resident() const { return !host_seen; }
     // device temp
     void *tmp(size_t bytes) { void *q = arena_alloc(t, bytes); if (!q) failed = true; return q; }
     // copy-backs + stream sync + arena reset. Returns MO_RC_SUCCESS or MO_RC_INTERNAL_ERROR.
     int finish();
-    // asynchronous form (every pointer was a device pointer): nothing to copy back, no synchronise; the scratch is handed back in stream order
-    void release_async() { backs.clear(); arena_reset(t); finished = true; }   // (no cached host blocks on this path: every pointer was a device pointer)
+    // the end of a call with an asynchronous form: finish() once a host range was met, else hand the scratch back in stream order and return
+    // without synchronising (there is then nothing to copy back and no cache block to keep)
+    int complete();
     ~Stager();
+private:
+    bool host_seen = false;
 };
 
 #define MOB_CUDA_TRY(expr)                                                                    \

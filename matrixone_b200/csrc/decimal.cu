@@ -192,7 +192,7 @@ int run_dec_arith(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
     const uint64_t *n1 = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? (c1 ? 8 : nwords * 8) : 0);
     const uint64_t *n2 = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? (c2 ? 8 : nwords * 8) : 0);
     unsigned long long *dbad = (unsigned long long *)st.tmp(8);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     uint64_t h1 = 0, h2 = 0;
     if (c1 && n1) { int rc = read_back(t, &h1, n1, 8); if (rc) { st.finish(); return rc; } }
     if (c2 && n2) { int rc = read_back(t, &h2, n2, 8); if (rc) { st.finish(); return rc; } }
@@ -235,7 +235,7 @@ int run_dec_sum(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
     const void *col = st.in(args[3].pdata, in_sz * len);
     const uint64_t *nulls = (const uint64_t *)st.in(args[3].pnulls, args[3].pnulls ? ((len + 63) / 64) * 8 : 0);
     unsigned *dbad = (unsigned *)st.tmp(4);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(dbad, 0, 4, t.stream));
     if (len) {
         int grid = num_sms() * 8;

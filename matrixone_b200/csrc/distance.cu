@@ -129,7 +129,7 @@ int run_rowdist(mo_xcall_args_t *args, uint64_t len) {
     const uint64_t *rn = (const uint64_t *)st.in(args[0].pnulls, args[0].pnulls ? ((len + 63) / 64) * 8 : 0);
     double *res = (double *)st.out(args[0].pdata, 8 * len, args[0].pnulls != nullptr);
     unsigned *dstatus = (unsigned *)st.tmp(4);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(dstatus, 0, 4, t.stream));
     const bool two = !c1 && !c2;
     const uint64_t warps = (len + 31) / 32;
@@ -239,7 +239,7 @@ int run_normalize(mo_xcall_args_t *args, uint64_t len) {
     uint8_t *oarea = args[1].areaSz ? (uint8_t *)st.out(args[0].parea, args[1].areaSz, true) : nullptr;
     double *norms = (double *)st.tmp(8 * len);
     unsigned *dstatus = (unsigned *)st.tmp(4);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(dstatus, 0, 4, t.stream));
     const uint64_t warps = (len + 31) / 32;
     uint64_t blocks = (warps + kThreads / 32 - 1) / (kThreads / 32);

@@ -266,7 +266,7 @@ int run_arith(void *r, void *a, void *b, uint64_t n, uint64_t *nulls, int32_t fl
     const bool partial = nulls != nullptr || OP == AR_DIV || OP == AR_MOD || OP == AR_INTDIV;
     R *dr = (R *)st.out(r, sizeof(R) * n, partial);
     unsigned *dstatus = (unsigned *)st.tmp(4);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(dstatus, 0, 4, t.stream));
     const bool vec = al16(dr) && (as || al16(da)) && (bs || al16(db));
     arith_kernel<T, R, OP><<<grid_for((n + 16 / sizeof(T) - 1) / (16 / sizeof(T))), kThreads, 0, t.stream>>>(dr, da, db, n, dn, flag, vec, dstatus);
@@ -325,7 +325,7 @@ int run_compare(void *r, void *a, void *b, uint64_t n, uint64_t *nulls, int32_t 
     const T *db = (const T *)st.in(b, sizeof(T) * (bs ? 1 : n));
     const uint64_t *dn = (const uint64_t *)st.in(nulls, nulls ? ((n + 63) / 64) * 8 : 0);
     uint8_t *dr = (uint8_t *)st.out(r, n, nulls != nullptr);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     const bool vec = al16(dr) && (as || al16(da)) && (bs || al16(db));
     compare_kernel<T, OP, ISBOOL><<<grid_for((n + 16 / sizeof(T) - 1) / (16 / sizeof(T))), kThreads, 0, t.stream>>>(dr, da, db, n, dn, flag, vec);
     MOB_LAUNCH_CHECK();
@@ -365,7 +365,7 @@ int run_logic(void *r, void *a, void *b, uint64_t n, uint64_t *anulls, uint64_t 
     const uint64_t *dbn = (const uint64_t *)st.in(bnulls, bnulls ? nb : 0);
     uint64_t *drn = (uint64_t *)st.out(rnulls, rnulls ? nb : 0, true);
     uint8_t *dr = (uint8_t *)st.out(r, n, false);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     logic_kernel<OP><<<grid_for((n + 63) / 64), kThreads, 0, t.stream>>>(dr, da, db, n, dan, dbn, drn, flag);
     MOB_LAUNCH_CHECK();
     return st.finish();

@@ -271,7 +271,7 @@ int run_go_arith(ThreadCtx &t, int Tid, mo_xcall_args_t *args, uint64_t len) {
     const uint64_t *n1 = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? (c1 ? 8 : nwords * 8) : 0);
     const uint64_t *n2 = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? (c2 ? 8 : nwords * 8) : 0);
     unsigned long long *dbad = (unsigned long long *)st.tmp(16);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     // const NULL operand: every row is NULL (baseTemplate.go:600-700)
     uint64_t h1 = 0, h2 = 0;
     if (c1 && n1) { int rc = read_back(t, &h1, n1, 8); if (rc) { st.finish(); return rc; } }
@@ -338,7 +338,7 @@ int run_go_compare(ThreadCtx &t, int op, mo_xcall_args_t *args, uint64_t len, do
     const T *b = (const T *)st.in(args[2].pdata, c2 ? sizeof(T) : sizeof(T) * len);
     const uint64_t *n1 = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? (c1 ? 8 : nwords * 8) : 0);
     const uint64_t *n2 = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? (c2 ? 8 : nwords * 8) : 0);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     uint64_t h1 = 0, h2 = 0;
     if (c1 && n1) { int rc = read_back(t, &h1, n1, 8); if (rc) { st.finish(); return rc; } }
     if (c2 && n2) { int rc = read_back(t, &h2, n2, 8); if (rc) { st.finish(); return rc; } }
@@ -369,7 +369,7 @@ int run_go_between(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
     uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, true);
     const T *col = (const T *)st.in(args[1].pdata, sizeof(T) * len);
     const uint64_t *nulls = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? nwords * 8 : 0);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     cudaEventRecord(t.kev0, t.stream);
     go_between_kernel<T><<<grid_rows(len), kThreads, 0, t.stream>>>(r, col, lo, hi, len, nulls, reinterpret_cast<uint32_t *>(rn));
     cudaEventRecord(t.kev1, t.stream);
@@ -402,7 +402,7 @@ int run_go_multi_logic(ThreadCtx &t, int is_or, mo_xcall_args_t *args, uint64_t 
             if (h & 1) P.p[k].kind = 2;
         }
     }
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(rn, 0, nwords * 8, t.stream));
     cudaEventRecord(t.kev0, t.stream);
     go_multi_logic_kernel<<<grid_rows(len), kThreads, 0, t.stream>>>(r, reinterpret_cast<uint32_t *>(rn), len, P, is_or, 0);

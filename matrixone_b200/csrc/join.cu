@@ -253,7 +253,12 @@ int str_table_for(ThreadCtx &t, Stager &st, const mo_xcall_args_t &bytes, const 
                   std::shared_lock<std::shared_mutex> &lk) {
     lk = std::shared_lock<std::shared_mutex>(g_jm_mu);
     auto it = g_jm.find(offs.pdata);
-    if (it != g_jm.end() && it->second.ngroups == ngroups && it->second.str) { *T = it->second; return MO_RC_SUCCESS; }
+    if (it != g_jm.end() && it->second.ngroups == ngroups && it->second.str) {
+        // nothing is staged, but a table prepared from host memory keeps the call synchronous, as a staged one does
+        st.device(bytes.pdata); st.device(offs.pdata);
+        *T = it->second;
+        return MO_RC_SUCCESS;
+    }
     lk.unlock();
     const uint8_t *db = (const uint8_t *)st.in(bytes.pdata, bytes.dataSz);
     const uint64_t *doff = (const uint64_t *)st.in(offs.pdata, (ngroups + 1) * 8);
@@ -344,7 +349,7 @@ int run_probe(ThreadCtx &t, Stager &st, mo_xcall_args_t *args, uint64_t len, int
     const int32_t *sels = multi ? (const int32_t *)st.in(args[6].pdata, args[6].dataSz) : nullptr;
     uint32_t *vals = (uint32_t *)st.tmp(len * 4 + 4);
     uint64_t *cnt = (uint64_t *)st.tmp((len + 1) * 8);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     cudaEventRecord(t.kev0, t.stream);
     probe_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(lookup, len, offsets, join_type, vals, cnt);
     MOB_LAUNCH_CHECK();
@@ -411,7 +416,7 @@ int xcall_join_sels(mo_xcall_args_t *args, uint64_t len) {
     int32_t *vals = (int32_t *)st.out(args[1].pdata, 4 * len);
     int64_t *count = (int64_t *)st.out(args[2].pdata, 8);
     const uint64_t *groups = (const uint64_t *)st.in(args[3].pdata, 8 * len);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     cudaEventRecord(t.kev0, t.stream);
     uint64_t *starts, *scal; uint32_t *rows;
     int rc = group_rows_stable(t, groups, len, ngroups, &starts, &rows, &scal);
@@ -442,7 +447,7 @@ int xcall_join_find(mo_xcall_args_t *args, uint64_t len) {
     uint64_t *vals = (uint64_t *)st.out(args[0].pdata, 8 * len);
     const uint64_t *keys = (const uint64_t *)st.in(args[2].pdata, 8 * len);
     const uint64_t *kn = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? ((len + 63) / 64) * 8 : 0);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     cudaEventRecord(t.kev0, t.stream);
     jt_find_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(keys, kn, len, T.key, T.id, T.mask, vals);
     cudaEventRecord(t.kev1, t.stream);
@@ -471,7 +476,7 @@ int xcall_join_probe(mo_xcall_args_t *args, uint64_t len) {
     const uint64_t *keys = (const uint64_t *)st.in(args[7].pdata, 8 * len);
     const uint64_t *kn = (const uint64_t *)st.in(args[7].pnulls, args[7].pnulls ? ((len + 63) / 64) * 8 : 0);
     uint64_t *scal = (uint64_t *)st.tmp(16);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, 16, t.stream));
     return run_probe(t, st, args, len, P.join_type, ngroups, KeyLookup{keys, kn, T.key, T.id, T.mask}, scal);
 }
@@ -492,7 +497,7 @@ int xcall_join_probe_gids(mo_xcall_args_t *args, uint64_t len) {
     Stager st(t);
     const uint64_t *gids = (const uint64_t *)st.in(args[7].pdata, 8 * len);
     uint64_t *scal = (uint64_t *)st.tmp(16);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, 16, t.stream));
     return run_probe(t, st, args, len, P.join_type, ngroups, GidLookup{gids, ngroups, (unsigned *)(scal + 1)}, scal);
 }
@@ -509,8 +514,6 @@ int xcall_str_join_find(mo_xcall_args_t *args, uint64_t len) {
     // host offsets must lie inside their bytes (device offsets are the caller's to keep right)
     if (!is_device_ptr(args[3].pdata) && ((const uint64_t *)args[3].pdata)[ngroups] > args[2].dataSz) { set_error("str join find: table offsets end past the table bytes (%llu)", (unsigned long long)args[2].dataSz); return MO_RC_INVALID_ARGUMENT; }
     if (!is_device_ptr(args[5].pdata) && ((const uint64_t *)args[5].pdata)[len] > args[4].dataSz) { set_error("str join find: probe key offsets end past the key bytes (%llu)", (unsigned long long)args[4].dataSz); return MO_RC_INVALID_ARGUMENT; }
-    const bool dev = is_device_ptr(args[0].pdata) && is_device_ptr(args[3].pdata) && is_device_ptr(args[5].pdata) && (!args[2].pdata || is_device_ptr(args[2].pdata)) &&
-                     (!args[4].pdata || is_device_ptr(args[4].pdata)) && (!args[5].pnulls || is_device_ptr(args[5].pnulls));
     Stager st(t);
     DevTable T;
     std::shared_lock<std::shared_mutex> lk;
@@ -520,14 +523,13 @@ int xcall_str_join_find(mo_xcall_args_t *args, uint64_t len) {
     const uint8_t *kbytes = (const uint8_t *)st.in(args[4].pdata, args[4].dataSz);
     const uint64_t *koff = (const uint64_t *)st.in(args[5].pdata, 8 * (len + 1));
     const uint64_t *kn = (const uint64_t *)st.in(args[5].pnulls, args[5].pnulls ? ((len + 63) / 64) * 8 : 0);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     cudaEventRecord(t.kev0, t.stream);
     sjt_find_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(StrKeys{T.sbytes, T.soff, kbytes, koff, ngroups}, kn, len, T.key, T.mask, strkey_hash_mask(), vals);
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
     // asynchronous form: a prepared table may be released while this kernel still reads it; its cudaFree waits for the device's pending work
-    if (dev) { st.release_async(); return MO_RC_SUCCESS; }
-    return st.finish();
+    return st.complete();
 }
 
 }  // namespace mob
@@ -539,7 +541,7 @@ extern "C" int32_t MoB200_JoinMapPrepare(const void *table_keys, uint64_t ngroup
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     Stager st(t);
     const uint64_t *dkeys = (const uint64_t *)st.in(table_keys, ngroups * 8);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     DevTable T;
     int rc = build_table(t, dkeys, ngroups, true, &T);
     int frc = st.finish();

@@ -207,7 +207,7 @@ int run_kmeans(mo_xcall_args_t *args) {
     int64_t *rnd_base = (int64_t *)st.tmp((size_t)k * 8);
     unsigned long long *dchanges = (unsigned long long *)st.tmp(16);
     int *dstatus = (int *)(dchanges + 1);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(half, 0, (size_t)(k * k) * sizeof(T), t.stream));
     MOB_CUDA_TRY(cudaMemsetAsync(dchanges, 0, 16, t.stream));
     cudaEventRecord(t.kev0, t.stream);

@@ -127,7 +127,7 @@ int xcall_lz4_decode(mo_xcall_args_t *args, uint64_t len) {
     const uint8_t *src = (const uint8_t *)st.in(args[1].pdata, args[1].dataSz);
     const int64_t *desc = (const int64_t *)st.in(args[2].pdata, 32 * len);
     unsigned long long *dbad = (unsigned long long *)st.tmp(8);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(dbad, 0xff, 8, t.stream));
     uint64_t ctas = (len + kWarpsPerCta - 1) / kWarpsPerCta;
 

@@ -602,7 +602,6 @@ int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
     OrderSpec spec;
     memset(&spec, 0, sizeof spec);
     int bit = 0, ns = 0;
-    bool dev = is_device_ptr(args[0].pdata) || nout == 0;
     Stager st(t);
     OrderSeg base[MO_ORDER_MAX_KEYS];
     bool has_var = false, ext = false;   // ext: a varlena or UUID key, order_word<true>
@@ -621,8 +620,6 @@ int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
         const uint64_t rows = cst ? 1 : len;
         const uint8_t *col = (const uint8_t *)st.in(a.pdata, cst ? esz : esz * len);
         const uint64_t *nulls = (const uint64_t *)st.in(a.pnulls, a.pnulls ? ((rows + 63) / 64) * 8 : 0);
-        if (a.pdata && (len || cst)) dev = dev && is_device_ptr(a.pdata);
-        if (a.pnulls) dev = dev && is_device_ptr(a.pnulls);
         OrderSeg &b = base[k];
         b = OrderSeg{};
         // BIT, YEAR and ENUM order as their storage types uint64, int16 and uint16
@@ -630,7 +627,6 @@ int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
         if (var && a.parea && a.areaSz) {
             b.area = (const uint8_t *)st.in(a.parea, a.areaSz);
             b.area_sz = a.areaSz;
-            dev = dev && is_device_ptr(a.parea);
         }
         has_var = has_var || var;
         ext = ext || var || T == MO_T_UUID;
@@ -639,7 +635,7 @@ int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
     VarlenaStat vstat{};
     if (has_var && len) {
         VarlenaStat *vs = (VarlenaStat *)st.tmp(sizeof(VarlenaStat));
-        if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+        if (st.failed) return MO_RC_INTERNAL_ERROR;
         MOB_CUDA_TRY(cudaMemsetAsync(vs, 0, sizeof(VarlenaStat), t.stream));
         for (int k = 0; k < P.nkeys; k++) {
             if (!is_varlena(base[k].type)) continue;
@@ -672,25 +668,24 @@ int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
         s.col = (const uint8_t *)st.in(rid->pdata, 8 * len); s.kind = SEG_ROWID; s.bits = 64; s.off = 64 * nwords;
         spec.seg[ns++] = s;
         nwords++;
-        if (len) dev = dev && is_device_ptr(rid->pdata);
     }
     if (!nwords) nwords = 1;   // only varlena keys whose every value is empty or NULL: one all-zero word keeps the rows in order
     spec.nsegs = ns; spec.nwords = nwords;
     int64_t *sels = (int64_t *)st.out(args[0].pdata, 8 * nout);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
-    if (nout == 0) { if (dev) { st.release_async(); return MO_RC_SUCCESS; } return st.finish(); }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    if (nout == 0) return st.complete();
 
     // Top: the candidate rows of the limit-th first word, in row order; Order: every row
     const bool top = nout < len / 8;
     const uint32_t *cand = nullptr;
     uint64_t *m_ptr = (uint64_t *)st.tmp(16);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     cudaEventRecord(t.kev0, t.stream);
     if (top) {
         SelectState *ss = (SelectState *)st.tmp(sizeof(SelectState));
         uint32_t *bits = (uint32_t *)st.tmp(((len + 63) / 64) * 8);
         uint32_t *c = (uint32_t *)st.tmp(len * 4 + 16);
-        if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+        if (st.failed) return MO_RC_INTERNAL_ERROR;
         SelectState init{};
         init.k = nout - 1; init.shift = 56;
         MOB_CUDA_TRY(cudaMemcpyAsync(ss, &init, sizeof init, cudaMemcpyHostToDevice, t.stream));
@@ -713,7 +708,7 @@ int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
     Pairs<uint64_t> B;
     B.k[0] = (uint64_t *)st.tmp(len * 8); B.k[1] = (uint64_t *)st.tmp(len * 8);
     B.v[0] = (uint32_t *)st.tmp(len * 4); B.v[1] = (uint32_t *)st.tmp(len * 4);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     // One LSD round over every word, or -- varlena keys with a long image -- rounds of kRoundWords words, most significant first: each round
     // after the first sorts by (run number, its words), and the device stops sorting once every run holds one row.
     const bool rounds = has_var && nwords > kRoundWords;
@@ -731,7 +726,7 @@ int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
         uint8_t *flag = (uint8_t *)st.tmp(len);
         unsigned long long *cnt = (unsigned long long *)st.tmp(kRunBlocks * 8);
         uint32_t *run = (uint32_t *)st.tmp(len * 4);
-        if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+        if (st.failed) return MO_RC_INTERNAL_ERROR;
         OrderSpec runspec;
         memset(&runspec, 0, sizeof runspec);
         runspec.seg[0].col = (const uint8_t *)run; runspec.seg[0].kind = SEG_RUN; runspec.seg[0].bits = 32;
@@ -758,8 +753,7 @@ int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
     sels_out_kernel<<<grid_for(nout), kThreads, 0, t.stream>>>(B.v[0], B.v[1], S.st, nout, sels);
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
-    if (dev) { st.release_async(); return MO_RC_SUCCESS; }
-    return st.finish();
+    return st.complete();
 }
 
 }  // namespace mob

@@ -520,12 +520,11 @@ static int plan_try_specialised(ThreadCtx &t, const mo_plan_t &P, mo_xcall_args_
     for (int c = 0; c < P.ncols; c++) if (args[2 + c].pnulls) return MO_RC_SUCCESS;
     const bool q6 = is_q6_shape(P), q1 = !q6 && is_q1_shape(P);
     if (!q6 && !q1) return MO_RC_SUCCESS;
-    bool async = is_device_ptr(args[0].pdata);
+    Stager st(t);
     const uint8_t *cols[7];
-    for (int c = 0; c < P.ncols; c++) { cols[c] = args[2 + c].pdata; async = async && is_device_ptr(cols[c]); }
+    for (int c = 0; c < P.ncols; c++) { cols[c] = args[2 + c].pdata; st.device(cols[c]); }   // residency decides the Q1 fallback below
     // the kernels below write the header and the groups they found: the rest of a host result is uploaded first so that the copy-back keeps it
     const uint64_t ngroups_max = q6 ? 1 : std::min<uint64_t>(res_groups, MO_Q1_MAX_GROUPS);
-    Stager st(t);
     uint8_t *dres = (uint8_t *)st.out(args[0].pdata, sizeof(mo_plan_result_header_t) + (sizeof(mo_plan_group_t) + sizeof(mo_plan_agg_value_t) * P.naggs) * ngroups_max, true);
     void *dq = st.tmp(q6 ? sizeof(Q6Out) : sizeof(mo_q1_result_t));
     int *dflag = (int *)st.tmp(4);
@@ -538,7 +537,7 @@ static int plan_try_specialised(ThreadCtx &t, const mo_plan_t &P, mo_xcall_args_
         MOB_LAUNCH_CHECK();
     } else {
         int rc = q1_run(t, st, cols, false, len, (int32_t)P.pred[0].lo, P.row_base, (mo_q1_result_t *)dq);
-        if (rc == MO_RC_INVALID_ARGUMENT && !async) return st.finish();   // host columns with device ones, or unaligned: the interpreter takes them
+        if (rc == MO_RC_INVALID_ARGUMENT && !st.resident()) return st.finish();   // host columns with device ones, or unaligned: the interpreter takes them
         if (rc) return rc;
         plan_from_q1_kernel<<<1, 1, 0, t.stream>>>((const mo_q1_result_t *)dq, dres, res_groups, dflag);
         MOB_LAUNCH_CHECK();
@@ -549,8 +548,7 @@ static int plan_try_specialised(ThreadCtx &t, const mo_plan_t &P, mo_xcall_args_
         if (fallback) return st.finish();
     }
     *answered = true;
-    if (async) { st.release_async(); return MO_RC_SUCCESS; }
-    return st.finish();
+    return st.complete();
 }
 
 // MO_XCALL_PLAN: args [0] result buffer ; [1] mo_plan_t (host) ; [2 .. 2 + ncols) the columns (+pnulls).  len = rows.  See include/mo_b200.h.
@@ -594,10 +592,6 @@ int xcall_plan(mo_xcall_args_t *args, uint64_t len) {
         const int rc = plan_try_specialised(t, P, args, len, res_groups, &answered);
         if (rc || answered) return rc;
     }
-    const bool dev_res = is_device_ptr(args[0].pdata);
-    bool dev_cols = true;
-    for (int c = 0; c < P.ncols; c++) dev_cols = dev_cols && (len == 0 || is_device_ptr(args[2 + c].pdata)) && (!args[2 + c].pnulls || is_device_ptr(args[2 + c].pnulls));
-
     Stager st(t);
     PlanCols C;
     for (int c = 0; c < MO_PLAN_MAX_COLS; c++) { C.data[c] = nullptr; C.nulls[c] = nullptr; }
@@ -617,7 +611,7 @@ int xcall_plan(mo_xcall_args_t *args, uint64_t len) {
     unsigned long long *nused = (unsigned long long *)st.tmp(16);
     mo_plan_t *dP = (mo_plan_t *)st.tmp(sizeof(mo_plan_t));
     PlanAux *dX = (PlanAux *)st.tmp(sizeof(PlanAux));
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     G.overflow = (unsigned *)(nused + 1);
     MOB_CUDA_TRY(cudaMemsetAsync(nused, 0, 16, t.stream));
     // the descriptor travels through the thread's pinned staging buffer (the caller's copy may be pageable and short-lived)
@@ -761,10 +755,10 @@ int xcall_plan(mo_xcall_args_t *args, uint64_t len) {
     MOB_LAUNCH_CHECK();
     plan_emit_kernel<<<num_sms() * 2, 256, 0, t.stream>>>(G, dP, used, nused, dres, res_groups, 8192);
     MOB_LAUNCH_CHECK();
-    if (dev_res && dev_cols) { st.release_async(); return MO_RC_SUCCESS; }   // asynchronous form: header.overflow reports a full table
+    if (st.resident()) return st.complete();   // asynchronous form: header.overflow reports a full table
     mo_plan_result_header_t H;
     int rc = read_back(t, &H, dres, sizeof H);
-    int frc = st.finish();
+    int frc = st.complete();
     if (rc) return rc;
     if (H.overflow) { set_error("plan: more groups (%lld) than the result buffer holds (%llu)", (long long)H.ngroups, (unsigned long long)res_groups); return MO_RC_INVALID_ARGUMENT; }
     return frc;

@@ -168,6 +168,7 @@ static const void *cache_lookup(const void *p, size_t bytes, std::shared_ptr<Dev
 const void *Stager::in(const void *p, size_t bytes) {
     if (!p || bytes == 0) return p;
     if (is_device_ptr(p)) return p;
+    host_seen = true;
     {
         std::shared_ptr<DevBlock> keep;
         const void *c = cache_lookup(p, bytes, keep);
@@ -183,6 +184,7 @@ const void *Stager::in(const void *p, size_t bytes) {
 void *Stager::out(void *p, size_t bytes, bool preload) {
     if (!p || bytes == 0) return p;
     if (is_device_ptr(p)) return p;
+    host_seen = true;
     void *d = arena_alloc(t, bytes);
     if (!d) { failed = true; return nullptr; }
     if (preload) {
@@ -216,6 +218,13 @@ int Stager::finish() {
     arena_reset(t);
     finished = true;
     return rc;
+}
+
+int Stager::complete() {
+    if (failed || host_seen) return finish();
+    arena_reset(t);
+    finished = true;
+    return MO_RC_SUCCESS;
 }
 
 Stager::~Stager() {

@@ -571,7 +571,7 @@ static int bruteforce_call(mo_xcall_args_t *args, uint64_t len, const mo_xcall_a
     const float *dq = (const float *)st.in(args[3].pdata, (size_t)P.nq * P.dim * 4);
     int64_t *ok = (int64_t *)st.out(args[0].pdata, (size_t)P.nq * P.k * 8);
     double *od = (double *)st.out(args[1].pdata, (size_t)P.nq * P.k * 8);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     g_search_stats = SearchStats();   // the statistics describe this search, also when it does not reach the tensor cores
     if (!farg) {
         rc = bruteforce_search(t, P, ddata, P.n, dq, P.key_base, ok, od, nullptr);
@@ -616,7 +616,7 @@ int xcall_topk_merge(mo_xcall_args_t *args, uint64_t len) {
     const double *id = (const double *)st.in(args[3].pdata, per * nshards);
     int64_t *ok = (int64_t *)st.out(args[0].pdata, per);
     double *od = (double *)st.out(args[1].pdata, per);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     topk_merge_kernel<<<(unsigned)((P.nq + 127) / 128), 128, 0, t.stream>>>(P.nq, P.k, (int)nshards, P.nq, nullptr, nullptr, id, ik, nullptr, 0, 0, 0, ok, od);
     MOB_LAUNCH_CHECK();
     return st.finish();
@@ -746,7 +746,7 @@ static int ivf_call(mo_xcall_args_t *args, uint64_t len, const mo_xcall_args_t *
     const int64_t *doffsets = (const int64_t *)st.in(args[6].pdata, (size_t)(P.nlist + 1) * 8);
     int64_t *ok = (int64_t *)st.out(args[0].pdata, (size_t)P.nq * P.k * 8);
     double *od = (double *)st.out(args[1].pdata, (size_t)P.nq * P.k * 8);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     std::vector<int64_t> offsets((size_t)P.nlist + 1);
     if (is_device_ptr(args[6].pdata)) { MOB_CUDA_TRY(cudaMemcpyAsync(offsets.data(), args[6].pdata, offsets.size() * 8, cudaMemcpyDeviceToHost, t.stream)); MOB_CUDA_TRY(cudaStreamSynchronize(t.stream)); }
     else memcpy(offsets.data(), args[6].pdata, offsets.size() * 8);

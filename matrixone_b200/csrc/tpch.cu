@@ -1037,18 +1037,16 @@ int xcall_q6(mo_xcall_args_t *args, uint64_t len) {
         return write_result(t, args[0].pnulls, &nullword, 8);
     }
 
-    // resident columns AND a device result: enqueue only (no read-back, no synchronisation); the result is ordered on the calling thread's
-    // stream, ready for NCCL + MO_XCALL_Q6_MERGE or a later MoB200_Download
-    const bool async = len && is_device_ptr(args[1].pdata) && is_device_ptr(args[0].pdata) && (!args[0].pnulls || is_device_ptr(args[0].pnulls));
+    // resident columns AND a device result and nulls word: enqueue only (no read-back, no synchronisation); the result is ordered on the
+    // calling thread's stream, ready for NCCL + MO_XCALL_Q6_MERGE or a later MoB200_Download
     Stager st(t);
     double *dres = (double *)st.out(args[0].pdata, args[0].dataSz >= 16 ? 16 : 8);
     uint64_t *dn = (uint64_t *)st.out(args[0].pnulls, args[0].pnulls ? 8 : 0);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     const uint8_t *cols[4] = {args[1].pdata, args[2].pdata, args[3].pdata, args[4].pdata};
     const int rc = q6_run(t, st, cols, len, P, dres, args[0].dataSz / 8, dn);
     if (rc) return rc;
-    if (async) { st.release_async(); return MO_RC_SUCCESS; }
-    return st.finish();
+    return st.complete();
 }
 
 // The Q6 scan of Decimal64 columns (host or device) into a device mo_q6_dec_result_t.  Chunks as q6_run; while a chunk's columns are still
@@ -1118,17 +1116,17 @@ int xcall_q6_dec(mo_xcall_args_t *args, uint64_t len) {
     if (is_device_ptr(args[5].pdata)) { int rc = read_back(t, &P, args[5].pdata, sizeof P); if (rc) return rc; }
     else memcpy(&P, args[5].pdata, sizeof P);
     if (P.scale < 0 || P.scale > 4) { set_error("q6 dec: scale %d outside 0..4", (int)P.scale); return MO_RC_INVALID_ARGUMENT; }
-    const bool async = len && is_device_ptr(args[1].pdata) && is_device_ptr(args[0].pdata) && (!args[0].pnulls || is_device_ptr(args[0].pnulls));
     Stager st(t);
     mo_q6_dec_result_t *dres = (mo_q6_dec_result_t *)st.out(args[0].pdata, sizeof(mo_q6_dec_result_t));
     uint64_t *dn = (uint64_t *)st.out(args[0].pnulls, args[0].pnulls ? 8 : 0);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     const uint8_t *cols[4] = {args[1].pdata, args[2].pdata, args[3].pdata, args[4].pdata};
     int rc = q6_dec_run(t, st, cols, len, P, dres, dn);
     if (rc) return rc;
-    if (async) { st.release_async(); return MO_RC_SUCCESS; }
-    rc = st.finish();
-    return rc ? rc : q6_dec_status(t, args[0].pdata, "q6 dec");
+    const bool async = st.resident();
+    rc = st.complete();
+    if (rc || async) return rc;
+    return q6_dec_status(t, args[0].pdata, "q6 dec");
 }
 
 // MO_XCALL_Q6_DEC_MERGE: args[0] = result as MO_XCALL_Q6_DEC_FILTER_SUM ; args[1] = len partial mo_q6_dec_result_t
@@ -1138,17 +1136,17 @@ int xcall_q6_dec_merge(mo_xcall_args_t *args, uint64_t len) {
     if (!args[0].pdata || args[0].dataSz < sizeof(mo_q6_dec_result_t) || args[1].dataSz < sizeof(mo_q6_dec_result_t) * len) {
         set_error("q6 dec merge: result and partials are mo_q6_dec_result_t"); return MO_RC_INVALID_ARGUMENT;
     }
-    const bool async = is_device_ptr(args[0].pdata) && (len == 0 || is_device_ptr(args[1].pdata)) && (!args[0].pnulls || is_device_ptr(args[0].pnulls));
     Stager st(t);
     const mo_q6_dec_result_t *dparts = (const mo_q6_dec_result_t *)st.in(args[1].pdata, sizeof(mo_q6_dec_result_t) * len);
     mo_q6_dec_result_t *dres = (mo_q6_dec_result_t *)st.out(args[0].pdata, sizeof(mo_q6_dec_result_t));
     uint64_t *dn = (uint64_t *)st.out(args[0].pnulls, args[0].pnulls ? 8 : 0);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     q6_dec_merge_kernel<<<1, 1, 0, t.stream>>>(dparts, len, dres, dn);
     MOB_LAUNCH_CHECK();
-    if (async) { st.release_async(); return MO_RC_SUCCESS; }
-    const int rc = st.finish();
-    return rc ? rc : q6_dec_status(t, args[0].pdata, "q6 dec merge");
+    const bool async = st.resident();
+    const int rc = st.complete();
+    if (rc || async) return rc;
+    return q6_dec_status(t, args[0].pdata, "q6 dec merge");
 }
 
 // device addresses of the Q1 input columns; the key columns hold packed uint8 values or 24-byte varlena cells
@@ -1303,15 +1301,14 @@ int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
     }
 
     const uint8_t *cols[7] = {args[1].pdata, args[2].pdata, args[3].pdata, args[4].pdata, args[5].pdata, args[6].pdata, args[7].pdata};
-    const bool async = dev && len && is_device_ptr(args[0].pdata);   // resident columns AND a device result: enqueue only (see xcall_q6)
     Stager st(t);
     mo_q1_result_t *dres = (mo_q1_result_t *)st.out(args[0].pdata, sizeof(mo_q1_result_t));
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     int rc = q1_run(t, st, cols, varlena, len, cutoff, row_base, dres);
     if (rc) return rc;
-    if (async) { st.release_async(); return MO_RC_SUCCESS; }   // more than MO_Q1_MAX_GROUPS keys: ngroups = -1 in the result
-    rc = st.finish();
-    if (rc) return rc;
+    const bool async = st.resident();   // resident columns AND a device result: enqueue only (see xcall_q6)
+    rc = st.complete();
+    if (rc || async) return rc;   // more than MO_Q1_MAX_GROUPS keys: ngroups = -1 in the result
     int64_t ngroups;
     if (is_device_ptr(args[0].pdata)) { rc = read_back(t, &ngroups, args[0].pdata, 8); if (rc) return rc; }
     else ngroups = ((const mo_q1_result_t *)args[0].pdata)->ngroups;
@@ -1327,16 +1324,14 @@ int xcall_q6_merge(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     if (!args[0].pdata || args[0].dataSz < 8 || args[1].dataSz < 16 * len) { set_error("q6 merge: result needs 8 bytes, partials 16 bytes each"); return MO_RC_INVALID_ARGUMENT; }
-    const bool async = is_device_ptr(args[0].pdata) && (len == 0 || is_device_ptr(args[1].pdata));
     Stager st(t);
     const double *dparts = (const double *)st.in(args[1].pdata, 16 * len);
     double *dres = (double *)st.out(args[0].pdata, args[0].dataSz >= 16 ? 16 : 8);
     uint64_t *dn = (uint64_t *)st.out(args[0].pnulls, args[0].pnulls ? 8 : 0);
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     q6_merge_kernel<<<1, 1, 0, t.stream>>>(dparts, len, Q6DevOut{dres, args[0].dataSz / 8, dn});
     MOB_LAUNCH_CHECK();
-    if (async) { st.release_async(); return MO_RC_SUCCESS; }
-    return st.finish();
+    return st.complete();
 }
 
 // MO_XCALL_Q1_MERGE: args[0] = mo_q1_result_t ; args[1] = len partial mo_q1_result_t (first_row already global: row_base param)
@@ -1344,17 +1339,17 @@ int xcall_q1_merge(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     if (!args[0].pdata || args[0].dataSz < sizeof(mo_q1_result_t) || args[1].dataSz < sizeof(mo_q1_result_t) * len) { set_error("q1 merge: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
-    const bool async = is_device_ptr(args[0].pdata) && (len == 0 || is_device_ptr(args[1].pdata));
     Stager st(t);
     const mo_q1_result_t *dparts = (const mo_q1_result_t *)st.in(args[1].pdata, sizeof(mo_q1_result_t) * len);
     mo_q1_result_t *dres = (mo_q1_result_t *)st.out(args[0].pdata, sizeof(mo_q1_result_t));
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     q1_merge_kernel<<<1, 1, 0, t.stream>>>(dparts, len, dres);
     MOB_LAUNCH_CHECK();
-    if (async) { st.release_async(); return MO_RC_SUCCESS; }
-    int rc = st.finish();
-    if (!rc && !is_device_ptr(args[0].pdata) && ((mo_q1_result_t *)args[0].pdata)->ngroups < 0) { set_error("q1 merge: more than %d distinct group keys", MO_Q1_MAX_GROUPS); return MO_RC_INVALID_ARGUMENT; }
-    return rc;
+    const bool async = st.resident();
+    const int rc = st.complete();
+    if (rc || async) return rc;
+    if (!is_device_ptr(args[0].pdata) && ((mo_q1_result_t *)args[0].pdata)->ngroups < 0) { set_error("q1 merge: more than %d distinct group keys", MO_Q1_MAX_GROUPS); return MO_RC_INVALID_ARGUMENT; }
+    return MO_RC_SUCCESS;
 }
 
 }  // namespace mob

@@ -115,7 +115,7 @@ int xcall_vector_unmarshal(mo_xcall_args_t *args, uint64_t len) {
     Sections *S = (Sections *)st.tmp(sizeof(Sections));
     int *overflow = (int *)st.tmp(8);
     mo_vector_view_t *dview = (mo_vector_view_t *)st.tmp(sizeof(mo_vector_view_t));
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(overflow, 0, 8, t.stream));
     vec_parse_kernel<<<1, 32, 0, t.stream>>>(src, args[4].dataSz, dview, S);
     MOB_LAUNCH_CHECK();
