@@ -162,6 +162,28 @@ int run_rowdist(mo_xcall_args_t *args, uint64_t len) {
 // result: the cell of row i has the SAME (offset, length) as the input's cell -- the result area mirrors the input area, inline cells stay
 // inline -- so no prefix sum over lengths is needed and a const input yields a const-shaped result (every cell points at the one vector).
 // Algorithmic bytes per row: 2 reads + 1 write of dim * sizeof(T) (the second read is served from L2 when the rows are short), 48 of cells.
+//
+// Whether a row below i is not NULL (the warp of row i asks; all lanes get the answer).  A const input's vector is written by the first
+// row that is not NULL: row 0 may be NULL.  The words below i are scanned downwards from i, so over all rows of a call the scans read
+// each bitmap word about once.
+__device__ __forceinline__ bool live_below(const uint64_t *rnulls, uint64_t i, int lane) {
+    if (i == 0) return false;
+    if (!rnulls) return true;
+    const uint64_t top = (i - 1) >> 6;
+    for (uint64_t b = 0; b <= top; b += 32) {
+        bool hit = false;
+        if (b + lane <= top) {
+            const uint64_t w = top - b - lane;
+            uint64_t live = ~rnulls[w];
+            const uint64_t below = i - (w << 6);          // rows of word w that are below i
+            if (below < 64) live &= (1ull << below) - 1;
+            hit = live != 0;
+        }
+        if (__any_sync(FULL, hit)) return true;
+    }
+    return false;
+}
+
 template <typename T>
 __global__ void __launch_bounds__(256)
 normalize_write_kernel(uint8_t *__restrict__ ocells, uint8_t *__restrict__ oarea, const uint64_t *__restrict__ rnulls, uint64_t n,
@@ -192,7 +214,7 @@ normalize_write_kernel(uint8_t *__restrict__ ocells, uint8_t *__restrict__ oarea
             continue;
         }
         if (lane < 24) oc[lane] = c[lane];
-        if (cst && i != 0) continue;                                                 // a const input: one vector, written once
+        if (cst && live_below(rnulls, i, lane)) continue;                           // a const input: one vector, written once
         uint8_t *dst = oarea + (a.ptr - area);
         if (((((uintptr_t)a.ptr) | ((uintptr_t)dst)) & 15) == 0) {
             constexpr int EPV = 16 / (int)sizeof(T);
