@@ -198,6 +198,11 @@ typedef struct mo_agg_state_t { uint64_t bits; int64_t count; int64_t rc; } mo_a
  * folded in order with the reference's BatchMerge rules (sumavg2.go:205-248 incl. int64OfCheck / uint64OfCheck, minmax2.go:90-110).
  * Device partials and a device result (pdata and pnulls): asynchronous as above. */
 #define MO_XCALL_AGG_MERGE(op, T) (0x1800 + ((op) << 8) + (T))
+/* Parameter blocks and scalar arguments -- every mo_*_params_t, mo_plan_t, mo_search_filter_t, mo_go_params_t, the BETWEEN bounds, the
+ * MULTI_AND / MULTI_OR operand count and ngroups -- may be host or device memory at every entry point.  A host block is copied and does not
+ * count toward the asynchronous form.  A device block is read back once before the call enqueues work, so the call waits for the work
+ * already on the calling thread's stream; apart from that the call completes exactly as it does with a host block.  Words a call writes
+ * into its block (err_row, the k-means iteration count) hold their value when a synchronous call returns. */
 
 /* --- new: fused TPC-H Q6 shape  SUM(a*b) WHERE d in [d_lo,d_hi) AND b BETWEEN b_lo AND b_hi AND c < c_hi
  * args: [0] result f64 (+ 1-word nulls bitmap, bit0 = no row qualified) ; [1] d int32/DATE col ; [2] b f64 col
@@ -238,7 +243,7 @@ typedef struct { int32_t div0_null; int32_t reserved; int64_t err_row; } mo_go_p
  *              args: [0] dst (+pnulls out) ; [1] src (+pnulls, nullCnt = its length in bits) ; [2] sels int64[len].  len = selected rows
  * PACK_KEYS    intHashMapIterator.encodeHashKeys / fillKeys (inthashmap.go:92-183): up to 8 key bytes per row from fixed-width columns, in
  *              has_null mode a marker byte (0 / 1) precedes every column's value bytes and a NULL contributes the marker only.
- *              args: [0] keys uint64[len] (+pnulls out, has_null = 0: rows with a NULL key join no group) ; [1] host params {int32 ncols, int32 has_null}
+ *              args: [0] keys uint64[len] (+pnulls out, has_null = 0: rows with a NULL key join no group) ; [1] params {int32 ncols, int32 has_null}
  *              ; [2 .. 2+ncols) key columns (+pnulls; a const vector holds one element)
  * GROUP_IDS    IntHashMap insert as driven by Group.buildOneBatch (exec2.go:325-362): 1-based group ids in FIRST-SEEN order; the table persists across
  *              calls through (ngroups, table_keys).  The hash function is not observable (random seeds, hashtable/hash.go:41-47), the ids are.
@@ -258,7 +263,7 @@ typedef struct { int32_t div0_null; int32_t reserved; int64_t err_row; } mo_go_p
  * (pkg/vectorindex/ivfflat/kmeans/elkans/clusterer.go:330-392; distance = metric.L2Distance for every metric, distance_func.go:452-476).
  * Centroids bit for bit, assignments and iteration count as the reference computes them (serial row-order sums, Go-order distances).
  * InitCentroids (initializer.go: draws from Go's PCG) stays with the caller.  args: [0] centroids T[k * dim] (in: initial, out: final) ;
- * [1] assignments int64[n] (out) ; [2] int64 iterations (out) ; [3] host mo_kmeans_params_t ; [4] vectors T[n * dim] ;
+ * [1] assignments int64[n] (out) ; [2] int64 iterations (out) ; [3] mo_kmeans_params_t ; [4] vectors T[n * dim] ;
  * [5] rnd float32[] (optional): the rnd.Float32() stream an EMPTY cluster re-seeds its centroid from (clusterer.go:700-707), consumed in
  * cluster order, dim values per empty cluster; running out of it fails the call with MO_RC_INVALID_ARGUMENT. */
 /* ---- LZ4 block decompression of column blocks (csrc/lz4.cu): compress.Decompress = lz4.UncompressBlock (pkg/compress/compress.go:37-47), one
@@ -297,7 +302,7 @@ typedef struct mo_kmeans_params_t { int64_t n, dim, k, max_iter; } mo_kmeans_par
  *               as (probe row, build row) pairs in the reference's order -- probe rows ascending, per probe row its group's sels ascending.
  *               join_type INNER: matches only; LEFT: + (row, -1) for a probe row without a match; SEMI: (row, -1) once per matching probe row;
  *               ANTI: (row, -1) per probe row WITHOUT a match.  args: [0] probe_rows int64[cap] ; [1] build_rows int64[cap] ; [2] int64 count (out; when
- *               it exceeds cap the call fails with MO_RC_OUT_OF_RANGE and the count is still written) ; [3] host mo_join_params_t ; [4] table_keys ;
+ *               it exceeds cap the call fails with MO_RC_OUT_OF_RANGE and the count is still written) ; [3] mo_join_params_t ; [4] table_keys ;
  *               [5] sels offsets int32[ngroups + 2] (pdata NULL: unique map, build row = id - 1) ; [6] sels vals int32[] ; [7] probe keys uint64[len] (+pnulls)
  * The device hash table is rebuilt from table_keys per call unless MoB200_JoinMapPrepare(table_keys, ngroups) cached it (keyed by that pointer). */
 #define MO_JOIN_INNER 0
@@ -317,7 +322,7 @@ typedef struct mo_join_params_t { int32_t join_type; int32_t reserved; } mo_join
  *                    group (empty key, bit set in args[1].pnulls).  The reference pads keys shorter than 16 bytes with zeros; the codes are
  *                    self-delimiting, so the padding never makes two keys equal and is left out.  The ROLLUP marker 0x02 is not built.
  *                    args: [0] key bytes u8[cap] (out) ; [1] offsets uint64[len + 1] (out: row i's key is bytes[off[i], off[i + 1]); +pnulls out,
- *                    has_null = 0 only: rows that join no group) ; [2] host mo_strkey_params_t ; [3 .. 3+ncols) key columns of col_type[k]: fixed
+ *                    has_null = 0 only: rows that join no group) ; [2] mo_strkey_params_t ; [3 .. 3+ncols) key columns of col_type[k]: fixed
  *                    width (the key types of ORDER_SELS, by storage size) or varlena cells + area as ORDER_SELS takes them (+pnulls; one element =
  *                    const).  cap too small: MO_RC_OUT_OF_RANGE and off[len] = the bytes needed.  A cell outside its area or a value longer than
  *                    MO_ORDER_MAX_VARLENA bytes: MO_RC_INVALID_ARGUMENT naming the column and its lowest such row.  Reads back one record (the byte
@@ -331,11 +336,11 @@ typedef struct mo_join_params_t { int32_t join_type; int32_t reserved; } mo_join
  *                    than the table holds: MO_RC_INVALID_ARGUMENT stating both capacities needed, with ngroups and the table untouched -- grow the
  *                    table and repeat the call.  len + ngroups < 2^31.  Reads back its overflow record (a device ngroups is read first, as GROUP_IDS does).
  *   STR_JOIN_FIND    strHashmapIterator.Find: vals[i] = 1-based id of probe key i in a table STR_GROUP_IDS built, 0 = absent or skipped.
- *                    args: [0] vals uint64[len] ; [1] host int64 ngroups ; [2] table bytes ; [3] table offsets ; [4] probe key bytes ; [5] probe key
+ *                    args: [0] vals uint64[len] ; [1] int64 ngroups ; [2] table bytes ; [3] table offsets ; [4] probe key bytes ; [5] probe key
  *                    offsets (+pnulls).  The device table is rebuilt per call (O(build groups)) unless MoB200_StrJoinMapPrepare cached it, keyed by
  *                    the table offsets pointer.  Device pointers: enqueue only.
  *   JOIN_PROBE_GIDS  JOIN_PROBE with each probe row's group id given (JOIN_FIND's or STR_JOIN_FIND's vals) instead of its key: the same pairs, in
- *                    the same order.  args [0..3], [5], [6] as JOIN_PROBE ; [4] host int64 ngroups ; [7] vals uint64[len] (an id above ngroups:
+ *                    the same order.  args [0..3], [5], [6] as JOIN_PROBE ; [4] int64 ngroups ; [7] vals uint64[len] (an id above ngroups:
  *                    MO_RC_INVALID_ARGUMENT). */
 #define MO_XCALL_PACK_STR_KEYS 0x6003
 #define MO_XCALL_STR_GROUP_IDS 0x6004
@@ -346,7 +351,7 @@ typedef struct mo_strkey_params_t { int32_t ncols; int32_t has_null; int32_t col
 #define MO_XCALL_GROUP_AGG(op, T) (0x6400 + ((op) << 8) + (T))
 /* ---- ORDER BY / ORDER BY ... LIMIT (csrc/order.cu): the sels of the Order operator (order.go:103) or the first `limit` of them for Top
  * (top.go:445); payload columns are then reordered with MO_XCALL_SHUFFLE, as Batch.Shuffle(sels) does.
- *   args: [0] sels int64[min(limit, len)] (out: indices into this call's rows) ; [1] host mo_order_params_t ; [2 .. 2+nkeys) key columns of
+ *   args: [0] sels int64[min(limit, len)] (out: indices into this call's rows) ; [1] mo_order_params_t ; [2 .. 2+nkeys) key columns of
  *         key[k].col_type (+pnulls; a 1-element vector is a const key) ; [2+nkeys] int64 row ids [len] when has_row_ids.  len = rows (< 2^32).
  *   limit < 0 or >= len: the whole order; otherwise the first `limit` rows.
  *   Keys compare left to right as compare.New(type, desc, nullsLast) (pkg/compare/compare.go:24-115): flags = the OrderBySpec flag word
@@ -390,7 +395,7 @@ typedef struct mo_order_params_t {
  *                         scale = max(scale1, scale2), result type = operand type; * : result Decimal128 with scale
  *                         min(scale1 + scale2, max(12, scale1, scale2)), scaled down with round-half-up when that is smaller than scale1 + scale2.
  *                         The first row that overflows fails the call with MO_RC_INVALID_ARGUMENT (moerr ErrInvalidInput) and err_row is set.
- *                         args: [0] result (+pnulls in/out) ; [1] a ; [2] b (const = one element) ; [3] host mo_dec_params_t
+ *                         args: [0] result (+pnulls in/out) ; [1] a ; [2] b (const = one element) ; [3] mo_dec_params_t
  *   DEC_SUM(width)        SUM / AVG accumulation of a decimal column into Decimal128 sums + int64 counts per group (count 0 = NULL; AVG divides at
  *                         Flush), sumDecimal64FastExec / sumDecimal128FastExec.batchFill, pkg/sql/colexec/aggexec/sum_decimal_fast.go -- exact and
  *                         order independent.  args: [0] sums Decimal128 per group (in/out) ; [1] counts int64 per group (in/out) ;
@@ -401,7 +406,7 @@ typedef struct mo_dec_params_t { int32_t scale1, scale2; int64_t err_row; } mo_d
 
 /* ---- the generic fused operator: scan -> filter -> project -> (hash) group -> aggregate in ONE pass over the columns (csrc/plan.cu).
  * What the colexec pipeline runs per block as table_scan -> filter -> projection -> group (filter.go:87-153, evalExpression.go:575-640,
- * group/exec2.go:296-367, aggexec/*), described by a host-side mo_plan_t:
+ * group/exec2.go:296-367, aggexec/*), described by a mo_plan_t:
  *   columns      args[2 .. 2+ncols): fixed-width columns of col_type[c] (MO_T_*), each with an optional nulls bitmap
  *   predicates   conjunction of  col OP lo  (OP: 0 == 1 != 2 > 3 >= 4 < 5 <=)  or  col BETWEEN lo AND hi (op 6, inclusive); a NULL operand
  *                rejects the row.  The column value is compared with the float64 constant exactly (integer columns of any magnitude, UINT64

@@ -671,8 +671,7 @@ int xcall_pack_keys(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     int32_t prm[2] = {0, 1};
-    if (!args[1].pdata || args[1].dataSz < 4 || is_device_ptr(args[1].pdata)) { set_error("pack keys: host params {ncols, has_null} missing"); return MO_RC_INVALID_ARGUMENT; }
-    memcpy(prm, args[1].pdata, args[1].dataSz >= 8 ? 8 : 4);
+    if (int rc = read_param(t, args[1], prm, 4, 8, "pack keys: params {ncols, has_null}")) return rc;
     if (prm[0] < 1 || prm[0] > kMaxKeyCols || args[0].dataSz < 8 * len) { set_error("pack keys: 1..%d key columns, keys buffer of 8*len bytes", kMaxKeyCols); return MO_RC_INVALID_ARGUMENT; }
     if (len == 0) return MO_RC_SUCCESS;
     Stager st(t);
@@ -708,7 +707,7 @@ int xcall_group_ids(mo_xcall_args_t *args, uint64_t len) {
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     if (!args[1].pdata || args[1].dataSz < 8 || args[0].dataSz < 8 * len || args[3].dataSz < 8 * len) { set_error("group ids: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
     int64_t nexist = 0;
-    if (is_device_ptr(args[1].pdata)) { int rc = read_back(t, &nexist, args[1].pdata, 8); if (rc) return rc; } else memcpy(&nexist, args[1].pdata, 8);
+    if (int rc = read_param(t, args[1], &nexist, 8, 8, "group ids: ngroups")) return rc;
     const uint64_t table_cap = args[2].dataSz / 8;
     if (nexist < 0 || (uint64_t)nexist > table_cap) { set_error("group ids: ngroups %lld exceeds the key table (%llu)", (long long)nexist, (unsigned long long)table_cap); return MO_RC_INVALID_ARGUMENT; }
     const uint64_t total = len + (uint64_t)nexist;
@@ -758,13 +757,12 @@ int xcall_group_ids(mo_xcall_args_t *args, uint64_t len) {
 }
 
 // MO_XCALL_PACK_STR_KEYS: args [0] key bytes u8[cap] ; [1] offsets uint64[len + 1] (+pnulls out: rows that join no group, has_null = 0) ;
-// [2] host mo_strkey_params_t ; [3 .. 3+ncols) key columns (fixed width or varlena cells + area; +pnulls; one element = const)
+// [2] mo_strkey_params_t ; [3 .. 3+ncols) key columns (fixed width or varlena cells + area; +pnulls; one element = const)
 int xcall_pack_str_keys(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
-    if (!args[2].pdata || args[2].dataSz < sizeof(mo_strkey_params_t) || is_device_ptr(args[2].pdata)) { set_error("pack str keys: host mo_strkey_params_t missing"); return MO_RC_INVALID_ARGUMENT; }
     mo_strkey_params_t P;
-    memcpy(&P, args[2].pdata, sizeof P);
+    if (int rc = read_param(t, args[2], &P, sizeof P, sizeof P, "pack str keys: mo_strkey_params_t")) return rc;
     if (P.ncols < 1 || P.ncols > MO_STRKEY_MAX_COLS) { set_error("pack str keys: %d key columns (1..%d)", P.ncols, MO_STRKEY_MAX_COLS); return MO_RC_INVALID_ARGUMENT; }
     if (!args[1].pdata || args[1].dataSz < 8 * (len + 1)) { set_error("pack str keys: the offsets need len + 1 entries"); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);
@@ -849,7 +847,7 @@ int xcall_str_group_ids(mo_xcall_args_t *args, uint64_t len) {
         if (ko[len] > args[4].dataSz || ko[0] > ko[len]) { set_error("str group ids: key offsets end at %llu, the key bytes hold %llu", (unsigned long long)ko[len], (unsigned long long)args[4].dataSz); return MO_RC_INVALID_ARGUMENT; }
     }
     int64_t nexist = 0;
-    if (is_device_ptr(args[1].pdata)) { int rc = read_back(t, &nexist, args[1].pdata, 8); if (rc) return rc; } else memcpy(&nexist, args[1].pdata, 8);
+    if (int rc = read_param(t, args[1], &nexist, 8, 8, "str group ids: ngroups")) return rc;
     const uint64_t cap_groups = args[3].dataSz / 8 - 1, cap_bytes = args[2].dataSz;
     if (nexist < 0 || (uint64_t)nexist > cap_groups) { set_error("str group ids: ngroups %lld exceeds the table (%llu groups)", (long long)nexist, (unsigned long long)cap_groups); return MO_RC_INVALID_ARGUMENT; }
     if (!is_device_ptr(args[3].pdata) && ((const uint64_t *)args[3].pdata)[nexist] > cap_bytes) {

@@ -116,6 +116,14 @@ private:
 // read one small device value back through the pinned staging buffer (synchronises the stream)
 int read_back(ThreadCtx &t, void *host_dst, const void *dev_src, size_t bytes);
 
+// A parameter block or scalar argument, host or device memory (include/mo_b200.h): copies min(a.dataSz, max) bytes to dst, reading a device
+// block back behind the work already on t.stream.  A missing block or one shorter than min bytes fails with "<what> missing".
+int read_param(ThreadCtx &t, const mo_xcall_args_t &a, void *dst, size_t min, size_t max, const char *what);
+// stores a host value into a word of the caller's, host or device memory (a parameter block's out word, a result computed on the host); a
+// device word is written on t.stream and holds the value when this returns
+
+int write_param(ThreadCtx &t, void *dst, const void *src, size_t bytes);
+
 // element width in bytes of a fixed-width MO_T_* type, 0 for any other type
 inline int type_size(int T) {
     switch (T) {

@@ -175,11 +175,11 @@ int run_dec_arith(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
     const size_t in_sz = W / 8, out_sz = (OP == 2 || W == 128) ? 16 : 8;
     const uint64_t nwords = (len + 63) / 64;
     const bool c1 = args[1].dataSz == in_sz && len > 1, c2 = args[2].dataSz == in_sz && len > 1;
-    if ((!c1 && args[1].dataSz < in_sz * len) || (!c2 && args[2].dataSz < in_sz * len) || args[0].dataSz < out_sz * len || !args[0].pnulls ||
-        !args[3].pdata || args[3].dataSz < sizeof(DecParams) || is_device_ptr(args[3].pdata)) {
-        set_error("decimal arith: vectors shorter than len, result without a null bitmap, or host params {scale1, scale2, err_row} missing"); return MO_RC_INVALID_ARGUMENT;
+    if ((!c1 && args[1].dataSz < in_sz * len) || (!c2 && args[2].dataSz < in_sz * len) || args[0].dataSz < out_sz * len || !args[0].pnulls) {
+        set_error("decimal arith: vectors shorter than len, or result without a null bitmap"); return MO_RC_INVALID_ARGUMENT;
     }
-    DecParams P; memcpy(&P, args[3].pdata, sizeof P);
+    DecParams P;
+    if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "decimal arith: params {scale1, scale2, err_row}")) return rc;
     int d1 = 0, d2 = 0, adj = 0;
     if (OP == 2) { int d = 12; if (P.scale1 > d) d = P.scale1; if (P.scale2 > d) d = P.scale2; if (P.scale1 + P.scale2 < d) d = P.scale1 + P.scale2; adj = d - P.scale1 - P.scale2; }
     else { d1 = P.scale2 > P.scale1 ? P.scale2 - P.scale1 : 0; d2 = P.scale1 > P.scale2 ? P.scale1 - P.scale2 : 0; }
@@ -214,8 +214,8 @@ int run_dec_arith(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
     if (rc) { st.finish(); return rc; }
     int frc = st.finish();
     P.err_row = bad == kNoRow ? -1 : (int64_t)bad;
-    memcpy(args[3].pdata, &P, sizeof P);
-    if (frc) return frc;
+    const int wrc = write_param(t, args[3].pdata, &P, sizeof P);
+    if (frc || wrc) return frc ? frc : wrc;
     if (bad == kNoRow) return MO_RC_SUCCESS;
     set_error("invalid input: Decimal%d %s overflow at row %llu", W, OP == 0 ? "Add" : (OP == 1 ? "Sub" : "Mul"), bad);
     return MO_RC_INVALID_ARGUMENT;

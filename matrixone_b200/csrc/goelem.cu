@@ -259,10 +259,8 @@ int run_go_arith(ThreadCtx &t, int Tid, mo_xcall_args_t *args, uint64_t len) {
         set_error("go arithmetic: vectors shorter than len, or the result has no null bitmap"); return MO_RC_INVALID_ARGUMENT;
     }
     GoParams P{0, 0, -1};
-    if (args[3].pdata && args[3].dataSz >= sizeof(GoParams)) {
-        if (is_device_ptr(args[3].pdata)) { int rc = read_back(t, &P, args[3].pdata, sizeof P); if (rc) return rc; }
-        else memcpy(&P, args[3].pdata, sizeof P);
-    }
+    const bool has_params = args[3].pdata && args[3].dataSz >= sizeof P;   // optional
+    if (has_params) { int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "go arithmetic: params"); if (rc) return rc; }
     Stager st(t);
     T *r = (T *)st.out(args[0].pdata, sizeof(T) * len, true);
     uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, true);
@@ -297,10 +295,7 @@ int run_go_arith(ThreadCtx &t, int Tid, mo_xcall_args_t *args, uint64_t len) {
     int frc = st.finish();
     if (frc) return frc;
     P.err_row = bad == kNoRow ? -1 : (int64_t)bad;
-    if (args[3].pdata && args[3].dataSz >= sizeof(GoParams)) {
-        if (is_device_ptr(args[3].pdata)) { MOB_CUDA_TRY(cudaMemcpyAsync(args[3].pdata, &P, sizeof P, cudaMemcpyHostToDevice, t.stream)); MOB_CUDA_TRY(cudaStreamSynchronize(t.stream)); }
-        else memcpy(args[3].pdata, &P, sizeof P);
-    }
+    if (has_params) { frc = write_param(t, args[3].pdata, &P, sizeof P); if (frc) return frc; }
     if (bad == kNoRow) return MO_RC_SUCCESS;
     if (OP == OP_DIV || OP == OP_MOD) { set_error("division by zero"); return MO_RC_DIVISION_BY_ZERO; }
     char sa[48], sb[48];
@@ -362,8 +357,8 @@ int run_go_between(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
         set_error("go between: vectors shorter than len, bounds missing, or the result has no null bitmap"); return MO_RC_INVALID_ARGUMENT;
     }
     T lo, hi;
-    if (is_device_ptr(args[2].pdata)) { int rc = read_back(t, &lo, args[2].pdata, sizeof(T)); if (rc) return rc; } else memcpy(&lo, args[2].pdata, sizeof(T));
-    if (is_device_ptr(args[3].pdata)) { int rc = read_back(t, &hi, args[3].pdata, sizeof(T)); if (rc) return rc; } else memcpy(&hi, args[3].pdata, sizeof(T));
+    if (int rc = read_param(t, args[2], &lo, sizeof lo, sizeof lo, "go between: lo")) return rc;
+    if (int rc = read_param(t, args[3], &hi, sizeof hi, sizeof hi, "go between: hi")) return rc;
     Stager st(t);
     uint8_t *r = (uint8_t *)st.out(args[0].pdata, len, false);
     uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, true);
@@ -380,8 +375,7 @@ int run_go_between(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
 int run_go_multi_logic(ThreadCtx &t, int is_or, mo_xcall_args_t *args, uint64_t len) {
     const uint64_t nwords = (len + 63) / 64;
     int32_t nparams = 0;
-    if (!args[1].pdata || args[1].dataSz < 4) { set_error("go logic: parameter count missing"); return MO_RC_INVALID_ARGUMENT; }
-    if (is_device_ptr(args[1].pdata)) { int rc = read_back(t, &nparams, args[1].pdata, 4); if (rc) return rc; } else memcpy(&nparams, args[1].pdata, 4);
+    if (int rc = read_param(t, args[1], &nparams, 4, 4, "go logic: parameter count")) return rc;
     if (nparams < 1 || nparams > kMaxLogicParams) { set_error("go logic: 1..%d operands", kMaxLogicParams); return MO_RC_INVALID_ARGUMENT; }
     if (args[0].dataSz < len || !args[0].pnulls) { set_error("go logic: result shorter than len, or without a null bitmap"); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);

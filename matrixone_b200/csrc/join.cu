@@ -367,16 +367,6 @@ int run_probe(ThreadCtx &t, Stager &st, mo_xcall_args_t *args, uint64_t len, int
     return frc;
 }
 
-// a host int64 argument (ngroups of STR_JOIN_FIND / JOIN_PROBE_GIDS)
-bool host_i64(const mo_xcall_args_t &a, uint64_t *v) {
-    int64_t x;
-    if (!a.pdata || a.dataSz < 8 || is_device_ptr(a.pdata)) return false;
-    memcpy(&x, a.pdata, 8);
-    if (x < 0) return false;
-    *v = (uint64_t)x;
-    return true;
-}
-
 }  // namespace
 
 // Stable grouping of rows by their 1-based group id (0 = the row takes no part): *starts = uint64[ngroups + 1] (start of every 0-based group in
@@ -455,14 +445,13 @@ int xcall_join_find(mo_xcall_args_t *args, uint64_t len) {
     return st.finish();
 }
 
-// MO_XCALL_JOIN_PROBE: args [0] probe_rows int64[cap] ; [1] build_rows int64[cap] ; [2] int64 count (out) ; [3] host mo_join_params_t ; [4] table_keys uint64[ngroups]
+// MO_XCALL_JOIN_PROBE: args [0] probe_rows int64[cap] ; [1] build_rows int64[cap] ; [2] int64 count (out) ; [3] mo_join_params_t ; [4] table_keys uint64[ngroups]
 // ; [5] sels offsets int32[ngroups + 2] (pdata NULL: unique map, build row = id - 1) ; [6] sels vals int32[] ; [7] probe keys uint64[len] (+pnulls)
 int xcall_join_probe(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
-    if (!args[3].pdata || args[3].dataSz < sizeof(mo_join_params_t) || is_device_ptr(args[3].pdata)) { set_error("join probe: host mo_join_params_t missing"); return MO_RC_INVALID_ARGUMENT; }
     mo_join_params_t P;
-    memcpy(&P, args[3].pdata, sizeof P);
+    if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "join probe: mo_join_params_t")) return rc;
     if (P.join_type < MO_JOIN_INNER || P.join_type > MO_JOIN_ANTI) { set_error("join probe: join type %d", P.join_type); return MO_RC_INVALID_ARGUMENT; }
     const uint64_t cap = args[0].dataSz / 8;
     if (args[1].dataSz / 8 < cap || !args[2].pdata || args[2].dataSz < 8 || args[7].dataSz < 8 * len) { set_error("join probe: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
@@ -481,16 +470,17 @@ int xcall_join_probe(mo_xcall_args_t *args, uint64_t len) {
     return run_probe(t, st, args, len, P.join_type, ngroups, KeyLookup{keys, kn, T.key, T.id, T.mask}, scal);
 }
 
-// MO_XCALL_JOIN_PROBE_GIDS: args [0..3], [5], [6] as JOIN_PROBE ; [4] host int64 ngroups ; [7] vals uint64[len] (group ids, 0 = no match)
+// MO_XCALL_JOIN_PROBE_GIDS: args [0..3], [5], [6] as JOIN_PROBE ; [4] int64 ngroups ; [7] vals uint64[len] (group ids, 0 = no match)
 int xcall_join_probe_gids(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
-    if (!args[3].pdata || args[3].dataSz < sizeof(mo_join_params_t) || is_device_ptr(args[3].pdata)) { set_error("join probe gids: host mo_join_params_t missing"); return MO_RC_INVALID_ARGUMENT; }
     mo_join_params_t P;
-    memcpy(&P, args[3].pdata, sizeof P);
+    if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "join probe gids: mo_join_params_t")) return rc;
     if (P.join_type < MO_JOIN_INNER || P.join_type > MO_JOIN_ANTI) { set_error("join probe gids: join type %d", P.join_type); return MO_RC_INVALID_ARGUMENT; }
-    uint64_t ngroups;
-    if (!host_i64(args[4], &ngroups)) { set_error("join probe gids: [4] must be a host int64 ngroups >= 0"); return MO_RC_INVALID_ARGUMENT; }
+    int64_t ng;
+    if (int rc = read_param(t, args[4], &ng, 8, 8, "join probe gids: [4] int64 ngroups")) return rc;
+    if (ng < 0) { set_error("join probe gids: [4] must be an int64 ngroups >= 0"); return MO_RC_INVALID_ARGUMENT; }
+    const uint64_t ngroups = (uint64_t)ng;
     const uint64_t cap = args[0].dataSz / 8;
     if (args[1].dataSz / 8 < cap || !args[2].pdata || args[2].dataSz < 8 || args[7].dataSz < 8 * len) { set_error("join probe gids: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
     if (args[5].pdata && args[5].dataSz < (ngroups + 2) * 4) { set_error("join probe gids: sels offsets shorter than the group count + 2"); return MO_RC_INVALID_ARGUMENT; }
@@ -502,13 +492,15 @@ int xcall_join_probe_gids(mo_xcall_args_t *args, uint64_t len) {
     return run_probe(t, st, args, len, P.join_type, ngroups, GidLookup{gids, ngroups, (unsigned *)(scal + 1)}, scal);
 }
 
-// MO_XCALL_STR_JOIN_FIND: args [0] vals uint64[len] ; [1] host int64 ngroups ; [2] table bytes ; [3] table offsets uint64[ngroups + 1] ; [4] probe key
+// MO_XCALL_STR_JOIN_FIND: args [0] vals uint64[len] ; [1] int64 ngroups ; [2] table bytes ; [3] table offsets uint64[ngroups + 1] ; [4] probe key
 // bytes ; [5] probe key offsets uint64[len + 1] (+pnulls)
 int xcall_str_join_find(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
-    uint64_t ngroups;
-    if (!host_i64(args[1], &ngroups)) { set_error("str join find: [1] must be a host int64 ngroups >= 0"); return MO_RC_INVALID_ARGUMENT; }
+    int64_t ng;
+    if (int rc = read_param(t, args[1], &ng, 8, 8, "str join find: [1] int64 ngroups")) return rc;
+    if (ng < 0) { set_error("str join find: [1] must be an int64 ngroups >= 0"); return MO_RC_INVALID_ARGUMENT; }
+    const uint64_t ngroups = (uint64_t)ng;
     if (args[0].dataSz < 8 * len || !args[3].pdata || args[3].dataSz < 8 * (ngroups + 1) || !args[5].pdata || args[5].dataSz < 8 * (len + 1)) { set_error("str join find: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
     if (ngroups >= 0x7fffffffull) { set_error("str join find: at most 2^31 groups"); return MO_RC_INVALID_ARGUMENT; }
     // host offsets must lie inside their bytes (device offsets are the caller's to keep right)

@@ -187,9 +187,8 @@ template <typename T>
 int run_kmeans(mo_xcall_args_t *args) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
-    if (!args[3].pdata || args[3].dataSz < sizeof(mo_kmeans_params_t) || is_device_ptr(args[3].pdata)) { set_error("kmeans: host mo_kmeans_params_t missing"); return MO_RC_INVALID_ARGUMENT; }
     mo_kmeans_params_t P;
-    memcpy(&P, args[3].pdata, sizeof P);
+    if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "kmeans: mo_kmeans_params_t")) return rc;
     const int64_t n = P.n, dim = P.dim, k = P.k;
     if (n < 1 || dim < 1 || k < 1 || k > n || dim > (1 << 20) || k > (1 << 20) || P.max_iter < 1) { set_error("kmeans: bad shape n=%lld dim=%lld k=%lld max_iter=%lld", (long long)n, (long long)dim, (long long)k, (long long)P.max_iter); return MO_RC_INVALID_ARGUMENT; }
     if (args[0].dataSz < (uint64_t)(k * dim) * sizeof(T) || args[1].dataSz < (uint64_t)n * 8 || !args[2].pdata || args[2].dataSz < 8 || args[4].dataSz < (uint64_t)(n * dim) * sizeof(T)) { set_error("kmeans: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
@@ -261,15 +260,13 @@ int run_kmeans(mo_xcall_args_t *args) {
     int frc = st.finish();
     if (frc) return frc;
     const int64_t iters = iter + 1;
-    if (is_device_ptr(args[2].pdata)) { if (cudaMemcpy(args[2].pdata, &iters, 8, cudaMemcpyHostToDevice) != cudaSuccess) return MO_RC_INTERNAL_ERROR; }
-    else memcpy(args[2].pdata, &iters, 8);
-    return MO_RC_SUCCESS;
+    return write_param(t, args[2].pdata, &iters, 8);
 }
 
 }  // namespace
 
 // MO_XCALL_KMEANS_ELKAN_F32 / _F64: args [0] centroids T[k * dim] (in: initial, out: final) ; [1] assignments int64[n] (out) ; [2] int64 iterations (out) ;
-// [3] host mo_kmeans_params_t ; [4] vectors T[n * dim] ; [5] rnd float32[] (optional: the rnd.Float32() stream empty clusters draw from)
+// [3] mo_kmeans_params_t ; [4] vectors T[n * dim] ; [5] rnd float32[] (optional: the rnd.Float32() stream empty clusters draw from)
 int xcall_kmeans(int64_t funcId, mo_xcall_args_t *args, uint64_t len) {
     (void)len;
     return funcId == MO_XCALL_KMEANS_ELKAN_F32 ? run_kmeans<float>(args) : run_kmeans<double>(args);

@@ -585,14 +585,13 @@ int sort_u32_pairs(ThreadCtx &t, uint32_t *k0, uint32_t *v0, uint32_t *k1, uint3
     return MO_RC_SUCCESS;
 }
 
-// MO_XCALL_ORDER_SELS: args [0] sels int64[min(limit, len)] ; [1] host mo_order_params_t ; [2 .. 2+nkeys) key columns (+pnulls; one element =
+// MO_XCALL_ORDER_SELS: args [0] sels int64[min(limit, len)] ; [1] mo_order_params_t ; [2 .. 2+nkeys) key columns (+pnulls; one element =
 // const) ; [2+nkeys] int64 row ids [len] when has_row_ids.  len = rows.
 int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
-    if (!args[1].pdata || args[1].dataSz < sizeof(mo_order_params_t) || is_device_ptr(args[1].pdata)) { set_error("order sels: host mo_order_params_t missing"); return MO_RC_INVALID_ARGUMENT; }
     mo_order_params_t P;
-    memcpy(&P, args[1].pdata, sizeof P);
+    if (int rc = read_param(t, args[1], &P, sizeof P, sizeof P, "order sels: mo_order_params_t")) return rc;
     if (P.nkeys < 1 || P.nkeys > MO_ORDER_MAX_KEYS) { set_error("order sels: %d keys (1..%d)", P.nkeys, MO_ORDER_MAX_KEYS); return MO_RC_INVALID_ARGUMENT; }
     if (len >= (1ull << 32)) { set_error("order sels: %llu rows, at most 2^32 - 1 per call", (unsigned long long)len); return MO_RC_INVALID_ARGUMENT; }
     const uint64_t nout = (P.limit < 0 || (uint64_t)P.limit >= len) ? len : (uint64_t)P.limit;

@@ -551,13 +551,12 @@ static int plan_try_specialised(ThreadCtx &t, const mo_plan_t &P, mo_xcall_args_
     return st.complete();
 }
 
-// MO_XCALL_PLAN: args [0] result buffer ; [1] mo_plan_t (host) ; [2 .. 2 + ncols) the columns (+pnulls).  len = rows.  See include/mo_b200.h.
+// MO_XCALL_PLAN: args [0] result buffer ; [1] mo_plan_t ; [2 .. 2 + ncols) the columns (+pnulls).  len = rows.  See include/mo_b200.h.
 int xcall_plan(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
-    if (!args[1].pdata || args[1].dataSz < sizeof(mo_plan_t) || is_device_ptr(args[1].pdata)) { set_error("plan: host mo_plan_t descriptor missing"); return MO_RC_INVALID_ARGUMENT; }
     mo_plan_t P;
-    memcpy(&P, args[1].pdata, sizeof P);
+    if (int rc = read_param(t, args[1], &P, sizeof P, sizeof P, "plan: mo_plan_t descriptor")) return rc;
     if (P.ncols < 1 || P.ncols > MO_PLAN_MAX_COLS || P.npreds < 0 || P.npreds > MO_PLAN_MAX_PREDS || P.ninstr < 0 || P.ninstr > MO_PLAN_MAX_INSTR ||
         P.nkeys < 0 || P.nkeys > MO_PLAN_MAX_KEYS || P.naggs < 1 || P.naggs > MO_PLAN_MAX_AGGS) { set_error("plan: descriptor counts out of range"); return MO_RC_INVALID_ARGUMENT; }
     int keybytes = 0;

@@ -241,6 +241,21 @@ int read_back(ThreadCtx &t, void *host_dst, const void *dev_src, size_t bytes) {
     return MO_RC_SUCCESS;
 }
 
+int read_param(ThreadCtx &t, const mo_xcall_args_t &a, void *dst, size_t min, size_t max, const char *what) {
+    if (!a.pdata || a.dataSz < min) { set_error("%s missing", what); return MO_RC_INVALID_ARGUMENT; }
+    const size_t bytes = a.dataSz < max ? (size_t)a.dataSz : max;
+    if (is_device_ptr(a.pdata)) return read_back(t, dst, a.pdata, bytes);
+    memcpy(dst, a.pdata, bytes);
+    return MO_RC_SUCCESS;
+}
+
+int write_param(ThreadCtx &t, void *dst, const void *src, size_t bytes) {
+    if (!is_device_ptr(dst)) { memcpy(dst, src, bytes); return MO_RC_SUCCESS; }
+    MOB_CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, t.stream));
+    MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
+    return MO_RC_SUCCESS;
+}
+
 }  // namespace mob
 
 using namespace mob;

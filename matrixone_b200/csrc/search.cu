@@ -432,17 +432,8 @@ int launch_bf_metric(ThreadCtx &t, int metric, const WorkDesc *ditems, int nitem
     return MO_RC_INVALID_ARGUMENT;
 }
 
-int read_params(ThreadCtx &t, const mo_xcall_args_t &a, mo_search_params_t *P) {
-    if (!a.pdata || a.dataSz < sizeof(mo_search_params_t)) { set_error("search: params missing"); return MO_RC_INVALID_ARGUMENT; }
-    if (is_device_ptr(a.pdata)) return read_back(t, P, a.pdata, sizeof *P);
-    memcpy(P, a.pdata, sizeof *P);
-    return MO_RC_SUCCESS;
-}
-
 int read_filter(ThreadCtx &t, const mo_xcall_args_t &a, mo_search_filter_t *F) {
-    if (!a.pdata || a.dataSz < sizeof(mo_search_filter_t)) { set_error("filtered search: filter descriptor missing or shorter than %zu bytes", sizeof(mo_search_filter_t)); return MO_RC_INVALID_ARGUMENT; }
-    if (is_device_ptr(a.pdata)) { int rc = read_back(t, F, a.pdata, sizeof *F); if (rc) return rc; }
-    else memcpy(F, a.pdata, sizeof *F);
+    if (int rc = read_param(t, a, F, sizeof *F, sizeof *F, "filtered search: filter descriptor")) return rc;
     if (F->kind != MO_SEARCH_FILTER_KEY_BITMAP && F->kind != MO_SEARCH_FILTER_KEY_BLOOM) { set_error("filtered search: unknown filter kind %d", F->kind); return MO_RC_INVALID_ARGUMENT; }
     if (!F->filter) { set_error("filtered search: null filter"); return MO_RC_INVALID_ARGUMENT; }
     if (F->kind == MO_SEARCH_FILTER_KEY_BLOOM) {
@@ -556,7 +547,7 @@ static int bruteforce_call(mo_xcall_args_t *args, uint64_t len, const mo_xcall_a
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     SearchReadGuard guard;   // prepared operands stay alive until this call returns
     mo_search_params_t P;
-    int rc = read_params(t, args[4], &P);
+    int rc = read_param(t, args[4], &P, sizeof P, sizeof P, "search: params");
     if (rc) return rc;
     if (P.nq != (int64_t)len) { set_error("search: len != params.nq"); return MO_RC_INVALID_ARGUMENT; }
     if (P.k == 0 || P.nq == 0) return MO_RC_SUCCESS;   // brute_force.go:262-264
@@ -605,7 +596,7 @@ int xcall_topk_merge(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     mo_search_params_t P;
-    int rc = read_params(t, args[4], &P);
+    int rc = read_param(t, args[4], &P, sizeof P, sizeof P, "search: params");
     if (rc) return rc;
     const int64_t nshards = P.n;
     if (P.nq != (int64_t)len || nshards < 1 || nshards > 64) { set_error("merge: bad params"); return MO_RC_INVALID_ARGUMENT; }
@@ -722,7 +713,7 @@ static int ivf_call(mo_xcall_args_t *args, uint64_t len, const mo_xcall_args_t *
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     SearchReadGuard guard;
     mo_search_params_t P;
-    int rc = read_params(t, args[4], &P);
+    int rc = read_param(t, args[4], &P, sizeof P, sizeof P, "search: params");
     if (rc) return rc;
     if (P.nq != (int64_t)len) { set_error("ivf: len != params.nq"); return MO_RC_INVALID_ARGUMENT; }
     if (P.k == 0 || P.nq == 0) return MO_RC_SUCCESS;

@@ -922,14 +922,6 @@ static const uint64_t kHostChunkRows = 32ull << 20;
 
 static bool aligned_to(const void *p, uintptr_t a) { return (((uintptr_t)p) & (a - 1)) == 0; }
 
-// copy a host value into the caller's result buffer, which may be host or device memory
-static int write_result(ThreadCtx &t, void *dst, const void *src, size_t bytes) {
-    if (!is_device_ptr(dst)) { memcpy(dst, src, bytes); return MO_RC_SUCCESS; }
-    MOB_CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, t.stream));
-    MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
-    return MO_RC_SUCCESS;
-}
-
 // The Q6 scan of one chunk in domain D; the whole-chunk record lands in *rec (arena memory, valid until the caller rewinds the arena)
 template <class D>
 static int launch_q6(ThreadCtx &t, const int32_t *sd, const typename D::V *disc, const typename D::V *qty, const typename D::V *price,
@@ -997,14 +989,12 @@ int q6_run(ThreadCtx &t, Stager &st, const uint8_t *const cols[4], uint64_t len,
 int xcall_q6(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
-    if (!args[5].pdata || args[5].dataSz < sizeof(mo_q6_params_t)) { set_error("q6: params missing"); return MO_RC_INVALID_ARGUMENT; }
     if (!args[0].pdata || args[0].dataSz < 8) { set_error("q6: result must hold 8 bytes"); return MO_RC_INVALID_ARGUMENT; }
     if (args[1].dataSz < 4 * len || args[2].dataSz < 8 * len || args[3].dataSz < 8 * len || args[4].dataSz < 8 * len) {
         set_error("q6: column shorter than len"); return MO_RC_INVALID_ARGUMENT;
     }
     mo_q6_params_t P;
-    if (is_device_ptr(args[5].pdata)) { int rc = read_back(t, &P, args[5].pdata, sizeof P); if (rc) return rc; }
-    else memcpy(&P, args[5].pdata, sizeof P);
+    if (int rc = read_param(t, args[5], &P, sizeof P, sizeof P, "q6: params")) return rc;
     bool nullable = false;
     for (int i = 1; i <= 4; i++) nullable = nullable || args[i].pnulls != nullptr;
     if (nullable) {
@@ -1031,10 +1021,10 @@ int xcall_q6(mo_xcall_args_t *args, uint64_t len) {
         const int64_t rows = R.h.ngroups > 0 ? R.g.rows : 0;
         unsigned char w[16];
         memcpy(w, &sum, 8); memcpy(w + 8, &rows, 8);
-        rc = write_result(t, args[0].pdata, w, args[0].dataSz >= 16 ? 16 : 8);
+        rc = write_param(t, args[0].pdata, w, args[0].dataSz >= 16 ? 16 : 8);
         if (rc || !args[0].pnulls) return rc;
         const uint64_t nullword = any ? 0ull : 1ull;
-        return write_result(t, args[0].pnulls, &nullword, 8);
+        return write_param(t, args[0].pnulls, &nullword, 8);
     }
 
     // resident columns AND a device result and nulls word: enqueue only (no read-back, no synchronisation); the result is ordered on the
@@ -1105,7 +1095,6 @@ static int q6_dec_status(ThreadCtx &t, const void *res, const char *what) {
 int xcall_q6_dec(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
-    if (!args[5].pdata || args[5].dataSz < sizeof(mo_q6_dec_params_t)) { set_error("q6 dec: params missing"); return MO_RC_INVALID_ARGUMENT; }
     if (!args[0].pdata || args[0].dataSz < sizeof(mo_q6_dec_result_t)) { set_error("q6 dec: result must hold a mo_q6_dec_result_t"); return MO_RC_INVALID_ARGUMENT; }
     if (args[1].dataSz < 4 * len || args[2].dataSz < 8 * len || args[3].dataSz < 8 * len || args[4].dataSz < 8 * len) {
         set_error("q6 dec: column shorter than len"); return MO_RC_INVALID_ARGUMENT;
@@ -1113,8 +1102,7 @@ int xcall_q6_dec(mo_xcall_args_t *args, uint64_t len) {
     for (int i = 1; i <= 4; i++)
         if (args[i].pnulls) { set_error("q6 dec: the DECIMAL(15,2) lineitem columns are NOT NULL; column %d has a nulls bitmap", i); return MO_RC_INVALID_ARGUMENT; }
     mo_q6_dec_params_t P;
-    if (is_device_ptr(args[5].pdata)) { int rc = read_back(t, &P, args[5].pdata, sizeof P); if (rc) return rc; }
-    else memcpy(&P, args[5].pdata, sizeof P);
+    if (int rc = read_param(t, args[5], &P, sizeof P, sizeof P, "q6 dec: params")) return rc;
     if (P.scale < 0 || P.scale > 4) { set_error("q6 dec: scale %d outside 0..4", (int)P.scale); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);
     mo_q6_dec_result_t *dres = (mo_q6_dec_result_t *)st.out(args[0].pdata, sizeof(mo_q6_dec_result_t));
@@ -1237,7 +1225,6 @@ int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     if (!args[0].pdata || args[0].dataSz < sizeof(mo_q1_result_t)) { set_error("q1: result buffer too small"); return MO_RC_INVALID_ARGUMENT; }
-    if (!args[8].pdata || args[8].dataSz < 4) { set_error("q1: cutoff param missing"); return MO_RC_INVALID_ARGUMENT; }
     if (args[1].dataSz < 4 * len) { set_error("q1: shipdate shorter than len"); return MO_RC_INVALID_ARGUMENT; }
     for (int i = 2; i <= 5; i++) if (args[i].dataSz < 8 * len) { set_error("q1: column %d shorter than len", i); return MO_RC_INVALID_ARGUMENT; }
     bool q1_nullable = false;
@@ -1246,21 +1233,18 @@ int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
     if (args[6].dataSz == len && args[7].dataSz == len) varlena = false;
     else if (args[6].dataSz == 24 * len && args[7].dataSz == 24 * len) varlena = true;
     else { set_error("q1: key columns must be packed uint8 (len bytes) or varlena cells (24*len bytes)"); return MO_RC_INVALID_ARGUMENT; }
-    int32_t cutoff;
-    if (is_device_ptr(args[8].pdata)) { int rc = read_back(t, &cutoff, args[8].pdata, 4); if (rc) return rc; }
-    else memcpy(&cutoff, args[8].pdata, 4);
+    mo_q1_params_t P{0, 0, 0};   // an int32 cutoff alone, or the whole block: row_base makes first_row values global row numbers
+    if (int rc = read_param(t, args[8], &P, 4, sizeof P, "q1: cutoff param")) return rc;
     const bool dev = is_device_ptr(args[1].pdata);
     for (int i = 2; i <= 7; i++) if (is_device_ptr(args[i].pdata) != dev) { set_error("q1: columns must all be host or all device"); return MO_RC_INVALID_ARGUMENT; }
-    int64_t row_base = 0;   // optional: params = {int32 cutoff; int32 pad; int64 row_base} -> first_row values are global row numbers
-    if (args[8].dataSz >= 16 && !is_device_ptr(args[8].pdata)) memcpy(&row_base, args[8].pdata + 8, 8);
     if (q1_nullable) {
         // nullable inputs: the generic fused operator (plan.cu).  NULL shipdate rejects the row; NULL values are skipped by their aggregates;
         // a NULL key is its own group (has_null_keys; its key byte reads 0 here).  Packed uint8 keys only.
         if (varlena) { set_error("q1: nullable columns need packed uint8 key columns"); return MO_RC_INVALID_ARGUMENT; }
         mo_plan_t Q; memset(&Q, 0, sizeof Q);
         Q.ncols = 7; Q.col_type[0] = MO_T_DATE; for (int c = 1; c <= 4; c++) Q.col_type[c] = MO_T_FLOAT64; Q.col_type[5] = Q.col_type[6] = MO_T_UINT8;
-        Q.row_base = row_base; Q.has_null_keys = (args[6].pnulls || args[7].pnulls) ? 1 : 0;
-        Q.npreds = 1; Q.pred[0] = mo_plan_pred_t{0, 5, (double)cutoff, 0.0};
+        Q.row_base = P.row_base; Q.has_null_keys = (args[6].pnulls || args[7].pnulls) ? 1 : 0;
+        Q.npreds = 1; Q.pred[0] = mo_plan_pred_t{0, 5, (double)P.cutoff, 0.0};
         Q.ninstr = 5;
         Q.instr[0] = mo_plan_instr_t{MO_PLAN_OP_CONST, 0, 0, 0, 1.0};        // slot 7: 1
         Q.instr[1] = mo_plan_instr_t{MO_PLAN_OP_SUB, 7, 3, 0, 0.0};          // slot 8: 1 - l_discount
@@ -1297,14 +1281,14 @@ int xcall_q1(mo_xcall_args_t *args, uint64_t len) {
             o.avg_disc = r.a[4].count ? r.a[4].value / (double)r.a[4].count : 0.0;
             o.count_order = r.a[5].count;
         }
-        return write_result(t, args[0].pdata, &res, sizeof res);
+        return write_param(t, args[0].pdata, &res, sizeof res);
     }
 
     const uint8_t *cols[7] = {args[1].pdata, args[2].pdata, args[3].pdata, args[4].pdata, args[5].pdata, args[6].pdata, args[7].pdata};
     Stager st(t);
     mo_q1_result_t *dres = (mo_q1_result_t *)st.out(args[0].pdata, sizeof(mo_q1_result_t));
     if (st.failed) return MO_RC_INTERNAL_ERROR;
-    int rc = q1_run(t, st, cols, varlena, len, cutoff, row_base, dres);
+    int rc = q1_run(t, st, cols, varlena, len, P.cutoff, P.row_base, dres);
     if (rc) return rc;
     const bool async = st.resident();   // resident columns AND a device result: enqueue only (see xcall_q6)
     rc = st.complete();
