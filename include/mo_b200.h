@@ -240,6 +240,8 @@ typedef struct { int32_t div0_null; int32_t reserved; int64_t err_row; } mo_go_p
  *              args: [0] sels int64[] (a host buffer only has to hold the selected rows) ; [1] count int64[1] ; [2] bool vector (+pnulls).  len = rows
  * SHUFFLE(sz)  Vector.Shrink / Union / shuffle.FixedLengthShuffle (vector.go:1014,2583 ; shuffle.go:21-26) with nulls.Filter
  *              (nulls.go:237-281) fused: dst[i] = src[sels[i]], dst null bit i = src null bit sels[i].  sz = element bytes: 1, 2, 4, 8, 16, 24 (varlena cell).
+ *              A negative sel gathers a NULL row: zero value bytes (a 24-byte cell: the empty inline value) and the null bit set -- the side of an
+ *              outer join's result row that has no match.  Without a dst bitmap the zero bytes are still written.
  *              args: [0] dst (+pnulls out) ; [1] src (+pnulls, nullCnt = its length in bits) ; [2] sels int64[len].  len = selected rows
  * PACK_KEYS    intHashMapIterator.encodeHashKeys / fillKeys (inthashmap.go:92-183): up to 8 key bytes per row from fixed-width columns, in
  *              has_null mode a marker byte (0 / 1) precedes every column's value bytes and a NULL contributes the marker only.
@@ -309,6 +311,39 @@ typedef struct mo_kmeans_params_t { int64_t n, dim, k, max_iter; } mo_kmeans_par
 #define MO_JOIN_LEFT 1
 #define MO_JOIN_SEMI 2
 #define MO_JOIN_ANTI 3
+/* ---- right-flavoured and single joins (hashjoin types.go:317-381: JoinType + IsRightJoin; FULL OUTER always runs right-flavoured).  JOIN_PROBE
+ * and JOIN_PROBE_GIDS take these types too, with the same capacity protocol, count read-back and bad-group-id error:
+ *   SINGLE        LEFT SINGLE: the LEFT pairs; a probe row whose group has more than one build row fails the call (join.go:504-507).
+ *   RIGHT         the INNER pairs, and every emitted build row is marked in the matched bitmap.
+ *   FULL          the LEFT pairs, marked as RIGHT.
+ *   RIGHT_SEMI    no pairs (count 0): only marks the matched build rows.
+ *   RIGHT_ANTI    no pairs: marks as RIGHT_SEMI.
+ *   RIGHT_SINGLE  the INNER pairs, marked as RIGHT; a build row matched a second time, in this call or an earlier one, fails the call.
+ * Types 5..9 take args[8]: the matched bitmap (rightRowsMatched, join.go:461-467,539-547), uint64[(nbuild + 63) / 64], LSB-first, one bit per build
+ * row (NULL-key rows included; they are never matched), in/out.  The caller zeroes it once per join and passes the same words to every probe
+ * batch.  Missing, or too short for the rows the map names: MO_RC_INVALID_ARGUMENT.  Types that emit pairs mark only when the result fits the
+ * output, so a call that fails with MO_RC_OUT_OF_RANGE leaves the bitmap untouched and its repeat is safe.  A SINGLE failure is
+ * MO_RC_INTERNAL_ERROR "scalar subquery returns more than 1 row" naming the lowest offending probe row (SINGLE) or the lowest build row matched
+ * twice in this call (RIGHT_SINGLE; which rows fail does not depend on the probe order).  Neither adds a synchronise: both come back in the
+ * record the probe already reads.
+ *   JOIN_MATCHED_MERGE  syncBitmap across workers or shards (join.go:650-676): out = the OR of n bitmaps.  args: [0] out uint64[(len + 63) / 64]
+ *                 (may be one of the inputs) ; [1] int32 n (1..MO_JOIN_MERGE_MAX) ; [2] mo_join_params_t (a type 5..9) ; [3 .. 3 + n) input
+ *                 bitmaps.  len = build rows.  RIGHT_SINGLE: a bit set in two inputs fails the call as above, naming the lowest such row, and
+ *                 the call reads back that one word; the other types only enqueue work when every bitmap is device memory.
+ *   JOIN_BUILD_ROWS     finalize (join.go:682-727): the build rows whose bit is CLEAR (RIGHT, FULL, RIGHT_ANTI, RIGHT_SINGLE) or SET (RIGHT_SEMI),
+ *                 ascending -- each is one result row whose probe-side columns are NULL.  Output contract of FILTER_SELS.  args: [0] sels
+ *                 int64[] (a host buffer only has to hold the rows found) ; [1] count int64[1] ; [2] matched bitmap ; [3] mo_join_params_t.
+ *                 len = build rows.
+ * The probe-side columns of those rows, and the build-side columns of a LEFT / FULL / SINGLE pair (row, -1), come from SHUFFLE with sel -1. */
+#define MO_JOIN_SINGLE 4
+#define MO_JOIN_RIGHT 5
+#define MO_JOIN_FULL 6
+#define MO_JOIN_RIGHT_SEMI 7
+#define MO_JOIN_RIGHT_ANTI 8
+#define MO_JOIN_RIGHT_SINGLE 9
+#define MO_JOIN_MERGE_MAX 64
+#define MO_XCALL_JOIN_MATCHED_MERGE 0x6015
+#define MO_XCALL_JOIN_BUILD_ROWS 0x6016
 typedef struct mo_join_params_t { int32_t join_type; int32_t reserved; } mo_join_params_t;
 #define MO_XCALL_JOIN_SELS 0x6010
 #define MO_XCALL_JOIN_FIND 0x6011

@@ -55,6 +55,10 @@ JOIN_INNER, JOIN_LEFT, JOIN_SEMI, JOIN_ANTI = 0, 1, 2, 3
 # byte-string keys (StrHashMap): encoder, group ids, join lookup, and the join emission over given group ids
 XCALL_PACK_STR_KEYS, XCALL_STR_GROUP_IDS = 0x6003, 0x6004
 XCALL_STR_JOIN_FIND, XCALL_JOIN_PROBE_GIDS = 0x6013, 0x6014
+# right-flavoured and single joins (hashjoin types.go:317-381): types 5..9 mark the build side's matched-row bitmap; merge and finalize it
+JOIN_SINGLE, JOIN_RIGHT, JOIN_FULL, JOIN_RIGHT_SEMI, JOIN_RIGHT_ANTI, JOIN_RIGHT_SINGLE = 4, 5, 6, 7, 8, 9
+XCALL_JOIN_MATCHED_MERGE, XCALL_JOIN_BUILD_ROWS = 0x6015, 0x6016
+JOIN_MERGE_MAX = 64
 STRKEY_MAX_COLS = 8
 
 

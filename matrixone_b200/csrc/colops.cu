@@ -1,6 +1,7 @@
 // colops.cu -- the standalone column operators of the colexec pipeline, one kernel family per reference operator:
 //
 //   MO_XCALL_FILTER_SELS      Filter.Call inner loop: bool vector (+nulls) -> ascending sels     pkg/sql/colexec/filter/filter.go:116-152
+//   MO_XCALL_JOIN_BUILD_ROWS  hashjoin finalize: the build rows a right-flavoured join adds         pkg/sql/colexec/hashjoin/join.go:682-727
 //   MO_XCALL_SHUFFLE(szof)    Vector.Shrink / Union / shuffle.FixedLengthShuffle + nulls.Filter   pkg/container/vector/vector.go:1014,2583,
 //                                                                                                 pkg/vectorize/shuffle/shuffle.go:21-26,
 //                                                                                                 pkg/container/nulls/nulls.go:237-281
@@ -38,11 +39,12 @@ constexpr int kThreads = 256;
 constexpr int kSelThreads = 256, kSelRows = 32, kSelTile = kSelThreads * kSelRows;   // 8192 rows per tile = one MatrixOne block
 constexpr unsigned long long kFlagA = 1ull << 62, kFlagP = 2ull << 62, kValMask = (1ull << 62) - 1;
 
-// BITS: the flags are a bitmap (bit j of 32-bit word w = row 32 w + j, zero past n) instead of one byte per row
+// BITS: the flags are a bitmap (bit j of 32-bit word w = row 32 w + j) instead of one byte per row, XORed with `flip` (~0u: the clear bits are
+// the flagged rows); bits past n are ignored
 template <typename OutT, bool BITS = false>
 __global__ void __launch_bounds__(kSelThreads)
 select_kernel(const uint8_t *__restrict__ v, const uint64_t *__restrict__ nulls, uint64_t n, OutT *__restrict__ sels,
-              unsigned long long *status, unsigned *ticket, unsigned long long *total, int aligned) {
+              unsigned long long *status, unsigned *ticket, unsigned long long *total, int aligned, unsigned flip) {
     __shared__ unsigned s_tile;
     __shared__ unsigned s_warp[kSelThreads / 32];
     __shared__ unsigned long long s_prefix;
@@ -53,7 +55,10 @@ select_kernel(const uint8_t *__restrict__ v, const uint64_t *__restrict__ nulls,
     const uint64_t row0 = (uint64_t)tile * kSelTile + (uint64_t)threadIdx.x * kSelRows;
     unsigned mask = 0;
     if (BITS) {
-        if (row0 < n) mask = reinterpret_cast<const uint32_t *>(v)[row0 >> 5];
+        if (row0 < n) {
+            mask = reinterpret_cast<const uint32_t *>(v)[row0 >> 5] ^ flip;
+            if (n - row0 < 32) mask &= (1u << (n - row0)) - 1u;
+        }
     } else if (row0 + kSelRows <= n && aligned) {
         const int4 x0 = ld_stream16(v + row0), x1 = ld_stream16(v + row0 + 16);
         const unsigned w[8] = {(unsigned)x0.x, (unsigned)x0.y, (unsigned)x0.z, (unsigned)x0.w, (unsigned)x1.x, (unsigned)x1.y, (unsigned)x1.z, (unsigned)x1.w};
@@ -105,14 +110,14 @@ select_kernel(const uint8_t *__restrict__ v, const uint64_t *__restrict__ nulls,
 
 // launches the compaction; *dtotal (device) receives the count.  status/ticket scratch comes from the arena.
 template <typename OutT, bool BITS = false>
-int launch_select(ThreadCtx &t, const uint8_t *v, const uint64_t *nulls, uint64_t n, OutT *sels, unsigned long long *dtotal) {
+int launch_select(ThreadCtx &t, const uint8_t *v, const uint64_t *nulls, uint64_t n, OutT *sels, unsigned long long *dtotal, unsigned flip = 0) {
     if (n == 0) { MOB_CUDA_TRY(cudaMemsetAsync(dtotal, 0, 8, t.stream)); return MO_RC_SUCCESS; }
     const uint64_t ntiles = (n + kSelTile - 1) / kSelTile;
     unsigned long long *status = (unsigned long long *)arena_alloc(t, ntiles * 8 + 16);
     if (!status) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(status, 0, ntiles * 8 + 16, t.stream));
     unsigned *ticket = (unsigned *)(status + ntiles);
-    select_kernel<OutT, BITS><<<(unsigned)ntiles, kSelThreads, 0, t.stream>>>(v, nulls, n, sels, status, ticket, dtotal, (((uintptr_t)v) & 15) == 0 ? 1 : 0);
+    select_kernel<OutT, BITS><<<(unsigned)ntiles, kSelThreads, 0, t.stream>>>(v, nulls, n, sels, status, ticket, dtotal, (((uintptr_t)v) & 15) == 0 ? 1 : 0, flip);
     MOB_LAUNCH_CHECK();
     return MO_RC_SUCCESS;
 }
@@ -128,7 +133,8 @@ int compact_bits(ThreadCtx &t, const uint32_t *bits, uint64_t n, int32_t *sels, 
 namespace {
 
 // =========================================================================================================
-// gather (Shrink / Union / FixedLengthShuffle) with nulls.Filter fused: dst[i] = src[sels[i]], dst null bit i = src null bit sels[i]
+// gather (Shrink / Union / FixedLengthShuffle) with nulls.Filter fused: dst[i] = src[sels[i]], dst null bit i = src null bit sels[i]; a negative
+// sel is a NULL row (zero bytes, null bit set): the missing side of an outer join's result row
 // =========================================================================================================
 template <typename E>
 __global__ void __launch_bounds__(kThreads)
@@ -138,9 +144,15 @@ gather_kernel(E *__restrict__ dst, const E *__restrict__ src, const int64_t *__r
     for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n64; i += (uint64_t)gridDim.x * kThreads) {
         bool isnull = false;
         if (i < nsel) {
-            const uint64_t s = (uint64_t)sels[i];
-            dst[i] = src[s];
-            isnull = snulls && s < snull_bits && ((snulls[s >> 6] >> (s & 63)) & 1ull);
+            const int64_t si = sels[i];
+            const uint64_t s = (uint64_t)si;
+            E e{};
+            isnull = si < 0;
+            if (!isnull) {
+                e = src[s];
+                isnull = snulls && s < snull_bits && ((snulls[s >> 6] >> (s & 63)) & 1ull);
+            }
+            dst[i] = e;
         }
         if (dnulls32) {
             const unsigned m = __ballot_sync(0xffffffffu, isnull);
@@ -604,6 +616,29 @@ int dispatch_minmax(ThreadCtx &t, int T, mo_xcall_args_t *args, uint64_t len) {
 
 namespace mob {
 
+// the output side of FILTER_SELS and JOIN_BUILD_ROWS: args [0] sels int64[] (device: >= len entries; host: >= count) ; [1] count int64[1].
+// launch(sels, dcount) enqueues the compaction.  Device outputs: asynchronous form; a host sels buffer gets the count read back and `count` rows.
+template <class Launch>
+int sels_result(ThreadCtx &t, Stager &st, mo_xcall_args_t *args, uint64_t len, const char *what, Launch launch) {
+    const bool host_out = !st.device(args[0].pdata);
+    int64_t *sels = host_out ? (int64_t *)st.tmp(len * 8 + 8) : (int64_t *)args[0].pdata;
+    unsigned long long *dcount = (unsigned long long *)st.out(args[1].pdata, 8);
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    cudaEventRecord(t.kev0, t.stream);
+    int rc = launch(sels, dcount);
+    cudaEventRecord(t.kev1, t.stream);
+    if (rc) { st.finish(); return rc; }
+    if (st.resident()) return st.complete();   // asynchronous form: everything stays on the device
+    unsigned long long cnt = 0;
+    rc = read_back(t, &cnt, dcount, 8);
+    if (rc) { st.finish(); return rc; }
+    if (host_out) {
+        if (cnt * 8 > args[0].dataSz) { st.finish(); set_error("%s: %llu rows selected, the sels buffer holds %llu", what, cnt, (unsigned long long)(args[0].dataSz / 8)); return MO_RC_INVALID_ARGUMENT; }
+        if (cnt) MOB_CUDA_TRY(cudaMemcpyAsync(args[0].pdata, sels, cnt * 8, cudaMemcpyDeviceToHost, t.stream));
+    }
+    return st.complete();
+}
+
 // MO_XCALL_FILTER_SELS: args [0] sels int64[>= count] ; [1] count int64[1] ; [2] bool vector (+pnulls).  len = rows.
 int xcall_filter_sels(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
@@ -612,24 +647,26 @@ int xcall_filter_sels(mo_xcall_args_t *args, uint64_t len) {
     Stager st(t);
     const uint8_t *v = (const uint8_t *)st.in(args[2].pdata, len);
     const uint64_t *nulls = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? ((len + 63) / 64) * 8 : 0);
-    // a host caller's sels buffer only has to hold the selected rows: compact into scratch, copy back `count` entries
-    const bool host_out = !st.device(args[0].pdata);
-    int64_t *sels = host_out ? (int64_t *)st.tmp(len * 8 + 8) : (int64_t *)args[0].pdata;
-    unsigned long long *dcount = (unsigned long long *)st.out(args[1].pdata, 8);
-    if (st.failed) return MO_RC_INTERNAL_ERROR;
-    cudaEventRecord(t.kev0, t.stream);
-    int rc = launch_select<int64_t>(t, v, nulls, len, sels, dcount);
-    cudaEventRecord(t.kev1, t.stream);
-    if (rc) { st.finish(); return rc; }
-    if (st.resident()) return st.complete();   // asynchronous form: everything stays on the device
-    unsigned long long cnt = 0;
-    rc = read_back(t, &cnt, dcount, 8);
-    if (rc) { st.finish(); return rc; }
-    if (host_out) {
-        if (cnt * 8 > args[0].dataSz) { st.finish(); set_error("filter sels: %llu rows selected, the sels buffer holds %llu", cnt, (unsigned long long)(args[0].dataSz / 8)); return MO_RC_INVALID_ARGUMENT; }
-        if (cnt) MOB_CUDA_TRY(cudaMemcpyAsync(args[0].pdata, sels, cnt * 8, cudaMemcpyDeviceToHost, t.stream));
-    }
-    return st.complete();
+    return sels_result(t, st, args, len, "filter sels", [&](int64_t *sels, unsigned long long *dcount) { return launch_select<int64_t>(t, v, nulls, len, sels, dcount); });
+}
+
+// MO_XCALL_JOIN_BUILD_ROWS (hashjoin syncBitmap + finalize, join.go:682-727): args [0] sels, [1] count as FILTER_SELS ; [2] matched bitmap uint64[(len + 63) / 64] ;
+// [3] mo_join_params_t.  The rows whose bit is set (RIGHT SEMI) or clear (the other right-flavoured types), ascending: the FILTER_SELS compaction
+// over the bitmap words, inverted or not.  len = build rows.
+int xcall_join_build_rows(mo_xcall_args_t *args, uint64_t len) {
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    mo_join_params_t P;
+    if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "join build rows: mo_join_params_t")) return rc;
+    if (P.join_type < MO_JOIN_RIGHT || P.join_type > MO_JOIN_RIGHT_SINGLE) { set_error("join build rows: join type %d (a right-flavoured type, 5..9)", P.join_type); return MO_RC_INVALID_ARGUMENT; }
+    const uint64_t words = (len + 63) / 64;
+    if (!args[1].pdata || args[1].dataSz < 8 || (words && !args[2].pdata) || args[2].dataSz < 8 * words) { set_error("join build rows: count needs 8 bytes, the matched bitmap (len + 63) / 64 words"); return MO_RC_INVALID_ARGUMENT; }
+    Stager st(t);
+    const uint32_t *bits = (const uint32_t *)st.in(args[2].pdata, 8 * words);
+    const unsigned flip = P.join_type == MO_JOIN_RIGHT_SEMI ? 0u : ~0u;   // syncBitmap negates the bitmap unless the join is a semi join (join.go:682-684)
+    return sels_result(t, st, args, len, "join build rows", [&](int64_t *sels, unsigned long long *dcount) {
+        return launch_select<int64_t, true>(t, reinterpret_cast<const uint8_t *>(bits), nullptr, len, sels, dcount, flip);
+    });
 }
 
 // MO_XCALL_SHUFFLE(szof): args [0] dst (szof bytes x len, + pnulls out) ; [1] src (+pnulls, nullCnt = its bit length) ; [2] sels int64[len]

@@ -10,7 +10,9 @@
 //                JOIN_PROBE = the emission loop of container.probe for the equality-only joins: per probe row the matched build rows in sels order
 //                (unique maps: build row = id - 1), for inner / left outer / left semi / left anti.  Output pairs (probe row, build row | -1) in
 //                exactly the order the reference appends them: probe rows ascending, within a row the sels ascending.  Counts -> exclusive scan ->
-//                positions; rows with >= 32 matches are written by their whole warp.
+//                positions; rows with >= 32 matches are written by their whole warp.  Left single, right, full, right semi / anti and right single
+//                (join.go:450-567) also mark the build side's matched-row bitmap or check the single-row rule.
+//   JOIN_MATCHED_MERGE = syncBitmap's OR over the workers' bitmaps (join.go:650-676); JOIN_BUILD_ROWS (colops.cu) = finalize's row list.
 //   byte-string keys   STR_JOIN_FIND = strHashmapIterator.Find over a STR_GROUP_IDS table (keytable.cuh's byte-string slots);
 //                JOIN_PROBE_GIDS = JOIN_PROBE's counting and emission over the group ids JOIN_FIND or STR_JOIN_FIND returned.
 //   The hash table itself is not observable in the reference (random seeds): ids and pairs are.  The device table is rebuilt from table_keys per
@@ -285,40 +287,86 @@ struct GidLookup {
     }
 };
 
+// ---- the build side's matched-row bitmap (rightRowsMatched, join.go:461-467,539-547) ------------------------------------------------------------
+// One bit per build row, LSB-first uint64 words, set with atomicOr.  RIGHT SINGLE looks at the bit it replaces: a build row whose bit was already
+// set is matched a second time, whichever pass or batch set it first, so the lowest such row of a call does not depend on the probe order.  A row
+// at or past the bitmap's last bit is not marked; the lowest one is recorded and fails the call.  A recorded row is kept as ~row with atomicMax,
+// so 0 means none and the whole record starts as zeros (one memset).
+struct Marks {
+    unsigned long long *words = nullptr; uint64_t nbits = 0; bool single = false;
+    unsigned long long *twice = nullptr, *past = nullptr;    // ~(lowest build row) matched twice (RIGHT SINGLE) / lying past the bitmap
+    __device__ __forceinline__ void mark(uint64_t r) const {
+        if (r >= nbits) { atomicMax(past, ~(unsigned long long)r); return; }
+        const unsigned long long bit = 1ull << (r & 63);
+        if (single) { if (atomicOr(&words[r >> 6], bit) & bit) atomicMax(twice, ~(unsigned long long)r); }
+        else if (!(words[r >> 6] & bit)) atomicOr(&words[r >> 6], bit);   // bits only ever go from 0 to 1: a set bit needs no atomic
+    }
+};
+// the record a probe reads back in one copy: [0] result count, [1] a group id above ngroups, [2] ~(lowest LEFT SINGLE probe row with more than one
+// match), [3] ~(lowest build row matched twice), [4] ~(lowest build row past the bitmap); 0 = none
+constexpr int kRecWords = 5;
+
+// counts per probe row of the pairs it emits.  RIGHT SEMI and RIGHT ANTI emit nothing: they mark here (groups of >= 32 sels by the whole warp)
+// and the call skips the scan and the emit pass (cnt == nullptr).  The types that emit pairs mark in the emit pass, once the result is known to
+// fit, so a call that fails with MO_RC_OUT_OF_RANGE leaves the bitmap as it was and its repeat marks each pair once.
 template <class Lookup>
-__global__ void __launch_bounds__(kThreads) probe_count_kernel(Lookup lookup, uint64_t n, const int32_t *__restrict__ offsets,
-                                                               int join_type, uint32_t *__restrict__ vals, uint64_t *__restrict__ cnt) {
-    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
-        const uint32_t v = lookup(i);
+__global__ void __launch_bounds__(kThreads) probe_count_kernel(Lookup lookup, uint64_t n, const int32_t *__restrict__ offsets, const int32_t *__restrict__ sels,
+                                                               int join_type, uint32_t *__restrict__ vals, uint64_t *__restrict__ cnt, Marks M,
+                                                               unsigned long long *single_row) {
+    const unsigned lane = threadIdx.x & 31;
+    const bool mark_here = join_type == MO_JOIN_RIGHT_SEMI || join_type == MO_JOIN_RIGHT_ANTI;
+    for (uint64_t i0 = blockIdx.x * (uint64_t)kThreads + (threadIdx.x & ~31u); i0 < n; i0 += (uint64_t)gridDim.x * kThreads) {
+        const uint64_t i = i0 + lane;                    // the loop is warp-uniform: whole warps mark heavy groups
+        uint32_t v = 0;
         uint64_t m = 0;
-        if (v) m = offsets ? (uint64_t)(offsets[v] - offsets[v - 1]) : 1ull;
-        uint64_t c;
-        switch (join_type) {
-        case MO_JOIN_INNER: c = m; break;
-        case MO_JOIN_LEFT: c = m ? m : 1; break;        // EmitUnmatchedProbe: one row with the build side NULL
-        case MO_JOIN_SEMI: c = m ? 1 : 0; break;
-        default: c = m ? 0 : 1; break;                   // anti
+        if (i < n) {
+            v = lookup(i);
+            if (v) m = offsets ? (uint64_t)(offsets[v] - offsets[v - 1]) : 1ull;
+            uint64_t c;
+            switch (join_type) {
+            case MO_JOIN_INNER: case MO_JOIN_RIGHT: case MO_JOIN_RIGHT_SINGLE: c = m; break;
+            case MO_JOIN_LEFT: case MO_JOIN_FULL: c = m ? m : 1; break;      // EmitUnmatchedProbe: one row with the build side NULL
+            case MO_JOIN_SINGLE: c = m ? m : 1; if (m > 1) atomicMax(single_row, ~(unsigned long long)i); break;   // join.go:504-507
+            case MO_JOIN_SEMI: c = m ? 1 : 0; break;
+            case MO_JOIN_ANTI: c = m ? 0 : 1; break;
+            default: c = 0; break;                       // right semi / right anti: marks only (join.go:452,549)
+            }
+            if (cnt) { vals[i] = m ? v : 0u; cnt[i] = c; }
         }
-        vals[i] = m ? v : 0u;
-        cnt[i] = c;
+        if (mark_here) {
+            const int32_t s0 = (m && offsets) ? offsets[v - 1] : 0;
+            if (m && m < 32) for (uint64_t j = 0; j < m; j++) M.mark(offsets ? (uint64_t)sels[s0 + j] : (uint64_t)v - 1);
+            unsigned heavy = __ballot_sync(0xffffffffu, m >= 32);
+            while (heavy) {
+                const int src = __ffs(heavy) - 1; heavy &= heavy - 1;
+                const uint64_t hm = __shfl_sync(0xffffffffu, m, src);
+                const int32_t hs0 = __shfl_sync(0xffffffffu, s0, src);
+                for (uint64_t j = lane; j < hm; j += 32) M.mark((uint64_t)sels[hs0 + j]);
+            }
+        }
     }
 }
-__global__ void __launch_bounds__(kThreads) probe_emit_kernel(uint64_t n, const uint32_t *__restrict__ vals, const uint64_t *__restrict__ pos, const uint64_t *__restrict__ total,
+// the minimum of 7 CTAs per SM is only there to steer ptxas: with it the kernel fits 32 registers without a spill, without it ptxas spills 4 bytes
+__global__ void __launch_bounds__(kThreads, 7) probe_emit_kernel(uint64_t n, const uint32_t *__restrict__ vals, const uint64_t *__restrict__ pos, const uint64_t *__restrict__ total,
                                                               const int32_t *__restrict__ offsets, const int32_t *__restrict__ sels, int join_type, uint64_t cap,
-                                                              int64_t *__restrict__ out_probe, int64_t *__restrict__ out_build, int64_t *count_out) {
+                                                              int64_t *__restrict__ out_probe, int64_t *__restrict__ out_build, int64_t *count_out, Marks M) {
     const unsigned lane = threadIdx.x & 31;
     const uint64_t nrounds = (n + 31) / 32;
+    // RIGHT, FULL and RIGHT SINGLE mark the build row of every pair they emit, and only when the whole result fits
+    const bool mark = M.words && *total <= cap;
     for (uint64_t w = (blockIdx.x * (uint64_t)kThreads + threadIdx.x) >> 5; w < nrounds; w += ((uint64_t)gridDim.x * kThreads) >> 5) {
         const uint64_t i = w * 32 + lane;
         uint32_t v = 0; uint64_t p = 0, c = 0;
         if (i < n) { v = vals[i]; p = pos[i]; c = (i + 1 < n ? pos[i + 1] : *total) - p; }
-        const bool pairs = (join_type == MO_JOIN_INNER || join_type == MO_JOIN_LEFT) && v;
+        const bool pairs = v && join_type != MO_JOIN_SEMI && join_type != MO_JOIN_ANTI;
         const int32_t s0 = (pairs && offsets) ? offsets[v - 1] : 0;
         if (c && c < 32) {
             for (uint64_t j = 0; j < c; j++) {
                 if (p + j >= cap) break;
+                const int64_t b = pairs ? (offsets ? (int64_t)sels[s0 + j] : (int64_t)v - 1) : -1;
                 out_probe[p + j] = (int64_t)i;
-                out_build[p + j] = pairs ? (offsets ? (int64_t)sels[s0 + j] : (int64_t)v - 1) : -1;
+                out_build[p + j] = b;
+                if (mark && pairs) M.mark((uint64_t)b);
             }
         }
         unsigned heavy = __ballot_sync(0xffffffffu, c >= 32);
@@ -328,43 +376,87 @@ __global__ void __launch_bounds__(kThreads) probe_emit_kernel(uint64_t n, const 
             const int32_t hs0 = __shfl_sync(0xffffffffu, s0, src);
             for (uint64_t j = lane; j < hc; j += 32) {
                 if (hp + j >= cap) break;
+                const int32_t b = sels[hs0 + j];          // >= 32 matches only happens with sels
                 out_probe[hp + j] = (int64_t)hi;
-                out_build[hp + j] = (int64_t)sels[hs0 + j];      // >= 32 matches only happens with sels
+                out_build[hp + j] = (int64_t)b;
+                if (mark) M.mark((uint64_t)b);
             }
         }
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) *count_out = (int64_t)*total;
 }
 
-// the output side shared by JOIN_PROBE and JOIN_PROBE_GIDS: args [0] probe_rows, [1] build_rows, [2] count, [5] / [6] sels; reads back the result
-// count and *bad (scal[1], set by the lookup) in one record
+// the output side shared by JOIN_PROBE and JOIN_PROBE_GIDS: args [0] probe_rows, [1] build_rows, [2] count, [5] / [6] sels, [8] the matched bitmap
+// (types MO_JOIN_RIGHT and above); reads back the record (kRecWords words at scal, [1] set by the lookup) in one copy
 template <class Lookup>
 int run_probe(ThreadCtx &t, Stager &st, mo_xcall_args_t *args, uint64_t len, int join_type, uint64_t ngroups, Lookup lookup, uint64_t *scal) {
     const uint64_t cap = args[0].dataSz / 8;
     const bool multi = args[5].pdata != nullptr;
+    const bool emits = join_type != MO_JOIN_RIGHT_SEMI && join_type != MO_JOIN_RIGHT_ANTI;
     int64_t *out_probe = (int64_t *)st.out(args[0].pdata, cap * 8);
     int64_t *out_build = (int64_t *)st.out(args[1].pdata, cap * 8);
     int64_t *count = (int64_t *)st.out(args[2].pdata, 8);
     const int32_t *offsets = multi ? (const int32_t *)st.in(args[5].pdata, (ngroups + 2) * 4) : nullptr;
     const int32_t *sels = multi ? (const int32_t *)st.in(args[6].pdata, args[6].dataSz) : nullptr;
-    uint32_t *vals = (uint32_t *)st.tmp(len * 4 + 4);
-    uint64_t *cnt = (uint64_t *)st.tmp((len + 1) * 8);
+    Marks M;
+    if (join_type >= MO_JOIN_RIGHT) {
+        const uint64_t words = args[8].dataSz / 8;
+        M.words = (unsigned long long *)st.out(args[8].pdata, words * 8, true);   // in/out: a host bitmap is uploaded and copied back
+        M.nbits = words * 64; M.single = join_type == MO_JOIN_RIGHT_SINGLE;
+        M.twice = (unsigned long long *)(scal + 3); M.past = (unsigned long long *)(scal + 4);
+    }
+    uint32_t *vals = emits ? (uint32_t *)st.tmp(len * 4 + 4) : nullptr;
+    uint64_t *cnt = emits ? (uint64_t *)st.tmp((len + 1) * 8) : nullptr;
     if (st.failed) return MO_RC_INTERNAL_ERROR;
     cudaEventRecord(t.kev0, t.stream);
-    probe_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(lookup, len, offsets, join_type, vals, cnt);
+    probe_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(lookup, len, offsets, sels, join_type, vals, cnt, M, (unsigned long long *)(scal + 2));
     MOB_LAUNCH_CHECK();
-    int rc = exclusive_scan(t, cnt, len, cnt, scal);
-    if (rc) { st.finish(); return rc; }
-    probe_emit_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(len, vals, cnt, scal, offsets, sels, join_type, cap, out_probe, out_build, count);
+    if (emits) {
+        int rc = exclusive_scan(t, cnt, len, cnt, scal);
+        if (rc) { st.finish(); return rc; }
+        const Marks EM = join_type == MO_JOIN_RIGHT || join_type == MO_JOIN_FULL || join_type == MO_JOIN_RIGHT_SINGLE ? M : Marks();
+        probe_emit_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(len, vals, cnt, scal, offsets, sels, join_type, cap, out_probe, out_build, count, EM);
+    } else {
+        MOB_CUDA_TRY(cudaMemsetAsync(count, 0, 8, t.stream));   // right semi / right anti: no pairs during the probe
+    }
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
-    uint64_t h[2] = {0, 0};
-    rc = read_back(t, h, scal, sizeof h);
+    uint64_t h[kRecWords] = {};
+    int rc = read_back(t, h, scal, sizeof h);
     int frc = st.finish();
     if (rc) return rc;
     if (h[1]) { set_error("join probe: a group id exceeds the group count (%llu)", (unsigned long long)ngroups); return MO_RC_INVALID_ARGUMENT; }
+    if (h[4]) { set_error("join probe: build row %llu lies past the matched bitmap (%llu rows)", (unsigned long long)~h[4], (unsigned long long)M.nbits); return MO_RC_INVALID_ARGUMENT; }
+    if (h[2]) { set_error("scalar subquery returns more than 1 row (probe row %llu)", (unsigned long long)~h[2]); return MO_RC_INTERNAL_ERROR; }
+    if (h[3]) { set_error("scalar subquery returns more than 1 row (build row %llu)", (unsigned long long)~h[3]); return MO_RC_INTERNAL_ERROR; }
     if (h[0] > cap) { set_error("join probe: %lld result rows exceed the output capacity (%llu); the count is reported, call again with larger buffers", (long long)h[0], (unsigned long long)cap); return MO_RC_OUT_OF_RANGE; }
     return frc;
+}
+
+// the join-type and matched-bitmap checks of JOIN_PROBE and JOIN_PROBE_GIDS; a unique map (no sels) names build rows 0 .. ngroups - 1, so its bitmap
+// must hold ngroups bits (with sels, a row past the bitmap is found on the device)
+int check_probe_type(const mo_xcall_args_t *args, int join_type, uint64_t ngroups, const char *what) {
+    if (join_type < MO_JOIN_INNER || join_type > MO_JOIN_RIGHT_SINGLE) { set_error("%s: join type %d", what, join_type); return MO_RC_INVALID_ARGUMENT; }
+    if (join_type < MO_JOIN_RIGHT) return MO_RC_SUCCESS;
+    if (!args[8].pdata) { set_error("%s: join type %d needs the matched bitmap in args[8]", what, join_type); return MO_RC_INVALID_ARGUMENT; }
+    if (!args[5].pdata && args[8].dataSz / 8 < (ngroups + 63) / 64) {
+        set_error("%s: the matched bitmap holds %llu rows, the build side has %llu", what, (unsigned long long)(args[8].dataSz / 8 * 64), (unsigned long long)ngroups);
+        return MO_RC_INVALID_ARGUMENT;
+    }
+    return MO_RC_SUCCESS;
+}
+
+// ---- JOIN_MATCHED_MERGE: syncBitmap's OR over the workers' bitmaps (join.go:650-676) ------------------------------------------------------------
+struct MergeInputs { const unsigned long long *p[MO_JOIN_MERGE_MAX]; };
+__global__ void __launch_bounds__(kThreads) matched_merge_kernel(MergeInputs in, int n, uint64_t words, uint64_t nbits, unsigned long long *out,
+                                                                 unsigned long long *twice) {
+    for (uint64_t w = blockIdx.x * (uint64_t)kThreads + threadIdx.x; w < words; w += (uint64_t)gridDim.x * kThreads) {
+        unsigned long long o = 0, d = 0;                 // d: bits set in two inputs (summed counts > the OR's count exactly when d != 0)
+        for (int k = 0; k < n; k++) { const unsigned long long x = in.p[k][w]; d |= o & x; o |= x; }
+        if (w == words - 1 && (nbits & 63)) { const unsigned long long live = (1ull << (nbits & 63)) - 1; o &= live; d &= live; }
+        out[w] = o;
+        if (twice && d) atomicMax(twice, ~(unsigned long long)(w * 64 + __ffsll((long long)d) - 1));   // ~row: 0 = none
+    }
 }
 
 }  // namespace
@@ -452,10 +544,10 @@ int xcall_join_probe(mo_xcall_args_t *args, uint64_t len) {
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     mo_join_params_t P;
     if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "join probe: mo_join_params_t")) return rc;
-    if (P.join_type < MO_JOIN_INNER || P.join_type > MO_JOIN_ANTI) { set_error("join probe: join type %d", P.join_type); return MO_RC_INVALID_ARGUMENT; }
     const uint64_t cap = args[0].dataSz / 8;
-    if (args[1].dataSz / 8 < cap || !args[2].pdata || args[2].dataSz < 8 || args[7].dataSz < 8 * len) { set_error("join probe: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
     const uint64_t ngroups = args[4].dataSz / 8;
+    if (int rc = check_probe_type(args, P.join_type, ngroups, "join probe")) return rc;
+    if (args[1].dataSz / 8 < cap || !args[2].pdata || args[2].dataSz < 8 || args[7].dataSz < 8 * len) { set_error("join probe: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
     if (args[5].pdata && args[5].dataSz < (ngroups + 2) * 4) { set_error("join probe: sels offsets shorter than the group count + 2"); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);
     DevTable T;
@@ -464,9 +556,9 @@ int xcall_join_probe(mo_xcall_args_t *args, uint64_t len) {
     if (rc) { st.finish(); return rc; }
     const uint64_t *keys = (const uint64_t *)st.in(args[7].pdata, 8 * len);
     const uint64_t *kn = (const uint64_t *)st.in(args[7].pnulls, args[7].pnulls ? ((len + 63) / 64) * 8 : 0);
-    uint64_t *scal = (uint64_t *)st.tmp(16);
+    uint64_t *scal = (uint64_t *)st.tmp(kRecWords * 8);
     if (st.failed) return MO_RC_INTERNAL_ERROR;
-    MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, 16, t.stream));
+    MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, kRecWords * 8, t.stream));
     return run_probe(t, st, args, len, P.join_type, ngroups, KeyLookup{keys, kn, T.key, T.id, T.mask}, scal);
 }
 
@@ -476,20 +568,57 @@ int xcall_join_probe_gids(mo_xcall_args_t *args, uint64_t len) {
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     mo_join_params_t P;
     if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "join probe gids: mo_join_params_t")) return rc;
-    if (P.join_type < MO_JOIN_INNER || P.join_type > MO_JOIN_ANTI) { set_error("join probe gids: join type %d", P.join_type); return MO_RC_INVALID_ARGUMENT; }
     int64_t ng;
     if (int rc = read_param(t, args[4], &ng, 8, 8, "join probe gids: [4] int64 ngroups")) return rc;
     if (ng < 0) { set_error("join probe gids: [4] must be an int64 ngroups >= 0"); return MO_RC_INVALID_ARGUMENT; }
     const uint64_t ngroups = (uint64_t)ng;
+    if (int rc = check_probe_type(args, P.join_type, ngroups, "join probe gids")) return rc;
     const uint64_t cap = args[0].dataSz / 8;
     if (args[1].dataSz / 8 < cap || !args[2].pdata || args[2].dataSz < 8 || args[7].dataSz < 8 * len) { set_error("join probe gids: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
     if (args[5].pdata && args[5].dataSz < (ngroups + 2) * 4) { set_error("join probe gids: sels offsets shorter than the group count + 2"); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);
     const uint64_t *gids = (const uint64_t *)st.in(args[7].pdata, 8 * len);
-    uint64_t *scal = (uint64_t *)st.tmp(16);
+    uint64_t *scal = (uint64_t *)st.tmp(kRecWords * 8);
     if (st.failed) return MO_RC_INTERNAL_ERROR;
-    MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, 16, t.stream));
+    MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, kRecWords * 8, t.stream));
     return run_probe(t, st, args, len, P.join_type, ngroups, GidLookup{gids, ngroups, (unsigned *)(scal + 1)}, scal);
+}
+
+// MO_XCALL_JOIN_MATCHED_MERGE: args [0] out bitmap uint64[(len + 63) / 64] ; [1] int32 n ; [2] mo_join_params_t ; [3 .. 3 + n) input bitmaps
+// (the same words).  len = build rows.  RIGHT SINGLE reads back the lowest bit set in two inputs; the other types complete as the Stager decides.
+int xcall_join_matched_merge(mo_xcall_args_t *args, uint64_t len) {
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    int32_t n;
+    if (int rc = read_param(t, args[1], &n, 4, 4, "join matched merge: [1] int32 n")) return rc;
+    mo_join_params_t P;
+    if (int rc = read_param(t, args[2], &P, sizeof P, sizeof P, "join matched merge: mo_join_params_t")) return rc;
+    if (P.join_type < MO_JOIN_RIGHT || P.join_type > MO_JOIN_RIGHT_SINGLE) { set_error("join matched merge: join type %d (a right-flavoured type, 5..9)", P.join_type); return MO_RC_INVALID_ARGUMENT; }
+    if (n < 1 || n > MO_JOIN_MERGE_MAX) { set_error("join matched merge: %d inputs (1..%d)", n, MO_JOIN_MERGE_MAX); return MO_RC_INVALID_ARGUMENT; }
+    const uint64_t words = (len + 63) / 64;
+    if (!args[0].pdata || args[0].dataSz < 8 * words) { set_error("join matched merge: the out bitmap holds fewer than %llu rows", (unsigned long long)len); return MO_RC_INVALID_ARGUMENT; }
+    for (int k = 0; k < n; k++)
+        if (!args[3 + k].pdata || args[3 + k].dataSz < 8 * words) { set_error("join matched merge: input %d holds fewer than %llu rows", k, (unsigned long long)len); return MO_RC_INVALID_ARGUMENT; }
+    if (words == 0) return MO_RC_SUCCESS;
+    const bool single = P.join_type == MO_JOIN_RIGHT_SINGLE;
+    Stager st(t);
+    MergeInputs in;
+    for (int k = 0; k < n; k++) in.p[k] = (const unsigned long long *)st.in(args[3 + k].pdata, 8 * words);
+    unsigned long long *out = (unsigned long long *)st.out(args[0].pdata, 8 * words);
+    unsigned long long *twice = single ? (unsigned long long *)st.tmp(8) : nullptr;
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    if (single) MOB_CUDA_TRY(cudaMemsetAsync(twice, 0, 8, t.stream));
+    cudaEventRecord(t.kev0, t.stream);
+    matched_merge_kernel<<<grid_for(words), kThreads, 0, t.stream>>>(in, n, words, len, out, twice);
+    cudaEventRecord(t.kev1, t.stream);
+    MOB_LAUNCH_CHECK();
+    if (!single) return st.complete();
+    unsigned long long h = 0;
+    int rc = read_back(t, &h, twice, 8);
+    int frc = st.finish();
+    if (rc) return rc;
+    if (h) { set_error("scalar subquery returns more than 1 row (build row %llu)", ~h); return MO_RC_INTERNAL_ERROR; }
+    return frc;
 }
 
 // MO_XCALL_STR_JOIN_FIND: args [0] vals uint64[len] ; [1] int64 ngroups ; [2] table bytes ; [3] table offsets uint64[ngroups + 1] ; [4] probe key

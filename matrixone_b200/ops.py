@@ -961,6 +961,24 @@ def _group_sels(groups, ngroups, nbuild):
     return offsets, sels[:int(cnt[0])]
 
 
+def matched_bitmap(nbuild):
+    """a zeroed matched-row bitmap for the right-flavoured join types: one bit per build row, LSB-first uint64 words"""
+    return np.zeros((nbuild + 63) // 64, dtype=np.uint64)
+
+
+def _matched_vec(matched, join_type):
+    """args[8] of JOIN_PROBE / JOIN_PROBE_GIDS: the matched bitmap (numpy uint64 words, updated in place, or a DeviceBuffer) for types >= JOIN_RIGHT"""
+    if join_type < capi.JOIN_RIGHT:
+        return []
+    if matched is None:
+        raise ValueError("join type %d needs the matched bitmap" % join_type)
+    if isinstance(matched, DeviceBuffer):
+        return [Vector(data_ptr=matched.ptr, data_nbytes=matched.nbytes, length=1)]
+    if not (isinstance(matched, np.ndarray) and matched.dtype == np.uint64 and matched.flags.c_contiguous):
+        raise ValueError("the matched bitmap is updated in place: pass a contiguous numpy uint64 array")
+    return [Vector(data=matched, length=len(matched))]
+
+
 def _probe_with(call, n, capacity):
     """the JOIN_PROBE capacity protocol: call(op, ob, cnt) -> (rc, msg); a too-small buffer reports the count and the call is repeated"""
     cap = capacity if capacity is not None else max(2 * n, 1024)
@@ -1010,9 +1028,9 @@ class StrJoinMap:
         xcall(capi.XCALL_STR_JOIN_FIND, [Vector(data=vals, length=n)] + self._table() + [Vector(data=kb, length=len(kb)), Vector(data=ko, nulls=nulls, length=n)], n)
         return vals
 
-    def probe(self, key_bytes, key_offsets, join_type=capi.JOIN_INNER, nulls=None, capacity=None):
+    def probe(self, key_bytes, key_offsets, join_type=capi.JOIN_INNER, nulls=None, capacity=None, matched=None):
         """(probe rows, build rows) of the join result in the reference's emission order, as JoinMap.probe"""
-        return probe_gids(self.find(key_bytes, key_offsets, nulls), self.ngroups, self.offsets, self.sels, join_type, capacity)
+        return probe_gids(self.find(key_bytes, key_offsets, nulls), self.ngroups, self.offsets, self.sels, join_type, capacity, matched)
 
     def release(self):
         if self.prepared:
@@ -1031,30 +1049,33 @@ def str_join_find_device(vals_dev, n, ngroups, table_bytes_dev, table_offsets_de
                                      Vector(data_ptr=offsets_dev.ptr, data_nbytes=8 * (n + 1), nulls_ptr=nulls_dev.ptr if nulls_dev is not None else None, length=n)], n)
 
 
-def probe_gids_device(vals_dev, n, ngroups, offsets_dev, sels_dev, join_type, out_probe_dev, out_build_dev, count_dev):
+def probe_gids_device(vals_dev, n, ngroups, offsets_dev, sels_dev, join_type, out_probe_dev, out_build_dev, count_dev, matched_dev=None):
     """JOIN_PROBE_GIDS on resident vectors: the pairs go to out_probe_dev / out_build_dev (int64, their size is the capacity) and their count to
-    count_dev; offsets_dev / sels_dev None = unique map.  Reads the count back (RC_OUT_OF_RANGE: the buffers are too small, the count is written)."""
+    count_dev; offsets_dev / sels_dev None = unique map; matched_dev = the matched bitmap (DeviceBuffer) of a right-flavoured type.  Reads the count
+    back (RC_OUT_OF_RANGE: the buffers are too small, the count is written)."""
     prm = np.array([join_type, 0], dtype=np.int32)
     vecs = [Vector(data_ptr=out_probe_dev.ptr, data_nbytes=out_probe_dev.nbytes, length=1), Vector(data_ptr=out_build_dev.ptr, data_nbytes=out_build_dev.nbytes, length=1),
             Vector(data_ptr=count_dev.ptr, data_nbytes=8, length=1), Vector(data=prm.view(np.uint8), length=1), Vector(data=np.array([ngroups], np.int64), length=1),
             Vector(data_ptr=offsets_dev.ptr, data_nbytes=offsets_dev.nbytes, length=ngroups + 2) if offsets_dev is not None else Vector(length=0),
             Vector(data_ptr=sels_dev.ptr, data_nbytes=sels_dev.nbytes, length=1) if sels_dev is not None else Vector(length=0),
-            Vector(data_ptr=vals_dev.ptr, data_nbytes=8 * n, length=n)]
+            Vector(data_ptr=vals_dev.ptr, data_nbytes=8 * n, length=n)] + _matched_vec(matched_dev, join_type)
     xcall(capi.XCALL_JOIN_PROBE_GIDS, vecs, n)
 
 
-def probe_gids(vals, ngroups, offsets, sels, join_type=capi.JOIN_INNER, capacity=None):
-    """JOIN_PROBE_GIDS: the JOIN_PROBE emission over given group ids (JOIN_FIND's or STR_JOIN_FIND's vals); offsets / sels None = unique map"""
+def probe_gids(vals, ngroups, offsets, sels, join_type=capi.JOIN_INNER, capacity=None, matched=None):
+    """JOIN_PROBE_GIDS: the JOIN_PROBE emission over given group ids (JOIN_FIND's or STR_JOIN_FIND's vals); offsets / sels None = unique map;
+    matched = the matched bitmap of a right-flavoured type (matched_bitmap(nbuild), updated in place)"""
     v = np.ascontiguousarray(vals, dtype=np.uint64)
     n = v.shape[0]
     prm = np.array([join_type, 0], dtype=np.int32)
+    mv = _matched_vec(matched, join_type)
 
     def call(op, ob, cnt):
         vecs = [Vector(data=op, length=len(op)), Vector(data=ob, length=len(ob)), Vector(data=cnt, length=1), Vector(data=prm.view(np.uint8), length=1),
                 Vector(data=np.array([ngroups], np.int64), length=1),
                 Vector(data=offsets, length=ngroups + 2) if offsets is not None else Vector(length=0),
                 Vector(data=sels, length=len(sels)) if sels is not None else Vector(length=0),
-                Vector(data=v, length=n)]
+                Vector(data=v, length=n)] + mv
         return xcall(capi.XCALL_JOIN_PROBE_GIDS, vecs, n, raise_on_error=False)
     return _probe_with(call, n, capacity)
 
@@ -1088,18 +1109,21 @@ class JoinMap:
         xcall(capi.XCALL_JOIN_FIND, [Vector(data=vals, length=n), Vector(data=self.table_keys, length=self.ngroups), Vector(data=k, nulls=nulls, length=n)], n)
         return vals
 
-    def probe(self, keys, join_type=capi.JOIN_INNER, nulls=None, capacity=None):
-        """(probe rows, build rows) of the join result in the reference's emission order; build row -1 = no build side (left outer / semi / anti)"""
+    def probe(self, keys, join_type=capi.JOIN_INNER, nulls=None, capacity=None, matched=None):
+        """(probe rows, build rows) of the join result in the reference's emission order; build row -1 = no build side (left outer / semi / anti /
+        full / single).  The right-flavoured types (JOIN_RIGHT and above) mark `matched` (matched_bitmap(nbuild), shared by every probe batch of
+        one join); join_build_rows then gives the build rows they add."""
         k = np.ascontiguousarray(keys, dtype=np.uint64)
         n = k.shape[0]
         prm = np.array([join_type, 0], dtype=np.int32)
+        mv = _matched_vec(matched, join_type)
 
         def call(op, ob, cnt):
             vecs = [Vector(data=op, length=len(op)), Vector(data=ob, length=len(ob)), Vector(data=cnt, length=1), Vector(data=prm.view(np.uint8), length=1),
                     Vector(data=self.table_keys, length=self.ngroups),
                     Vector(data=self.offsets, length=self.ngroups + 2) if self.offsets is not None else Vector(length=0),
                     Vector(data=self.sels, length=len(self.sels)) if self.sels is not None else Vector(length=0),
-                    Vector(data=k, nulls=nulls, length=n)]
+                    Vector(data=k, nulls=nulls, length=n)] + mv
             return xcall(capi.XCALL_JOIN_PROBE, vecs, n, raise_on_error=False)
         return _probe_with(call, n, capacity)
 
@@ -1108,6 +1132,45 @@ class JoinMap:
             lib = capi.load_library()
             lib.MoB200_JoinMapRelease(self.table_keys.ctypes.data)
             self.prepared = False
+
+
+def join_build_rows(matched, nbuild, join_type):
+    """hashjoin finalize (join.go:682-727): the build rows a right-flavoured join adds once every probe batch has marked `matched` -- the
+    unmatched ones, or for JOIN_RIGHT_SEMI the matched ones -- ascending; their probe-side columns are NULL (SHUFFLE with sel -1)"""
+    m = np.ascontiguousarray(matched, dtype=np.uint64)
+    sels = np.zeros(max(nbuild, 1), dtype=np.int64)
+    cnt = np.zeros(1, dtype=np.int64)
+    xcall(capi.XCALL_JOIN_BUILD_ROWS, [Vector(data=sels, length=nbuild), Vector(data=cnt, length=1), Vector(data=m, length=len(m)),
+                                       Vector(data=np.array([join_type, 0], np.int32).view(np.uint8), length=1)], nbuild)
+    return sels[:int(cnt[0])]
+
+
+def join_build_rows_device(matched_dev, nbuild, join_type, sels_ptr, count_ptr):
+    """JOIN_BUILD_ROWS on a resident bitmap: sels (int64[nbuild] capacity) and the count stay on the device; the call only enqueues work"""
+    xcall(capi.XCALL_JOIN_BUILD_ROWS, [Vector(data_ptr=sels_ptr, data_nbytes=8 * nbuild, length=nbuild), Vector(data_ptr=count_ptr, data_nbytes=8, length=1),
+                                       Vector(data_ptr=matched_dev.ptr, data_nbytes=8 * ((nbuild + 63) // 64), length=1),
+                                       Vector(data=np.array([join_type, 0], np.int32).view(np.uint8), length=1)], nbuild)
+
+
+def _merge_vecs(out, inputs, join_type):
+    return [out, Vector(data=np.array([len(inputs)], np.int32), length=1), Vector(data=np.array([join_type, 0], np.int32).view(np.uint8), length=1)] + inputs
+
+
+def join_matched_merge(bitmaps, nbuild, join_type):
+    """syncBitmap (join.go:650-676): the OR of the workers' matched bitmaps; JOIN_RIGHT_SINGLE fails (MoError) when a build row is set in two"""
+    words = (nbuild + 63) // 64
+    out = np.zeros(words, dtype=np.uint64)
+    ins = [Vector(data=np.ascontiguousarray(b, dtype=np.uint64), length=words) for b in bitmaps]
+    xcall(capi.XCALL_JOIN_MATCHED_MERGE, _merge_vecs(Vector(data=out, length=words), ins, join_type), nbuild)
+    return out
+
+
+def join_matched_merge_device(out_dev, bitmaps_dev, nbuild, join_type):
+    """JOIN_MATCHED_MERGE over resident bitmaps (DeviceBuffers; out_dev may be one of them): enqueue only, except JOIN_RIGHT_SINGLE, which reads
+    back whether a row is set in two inputs"""
+    words = (nbuild + 63) // 64
+    ins = [Vector(data_ptr=b.ptr, data_nbytes=8 * words, length=1) for b in bitmaps_dev]
+    xcall(capi.XCALL_JOIN_MATCHED_MERGE, _merge_vecs(Vector(data_ptr=out_dev.ptr, data_nbytes=8 * words, length=1), ins, join_type), nbuild)
 
 
 # ---------------------------------------------------------------------------------------------- Elkan k-means (csrc/kmeans.cu)
