@@ -344,6 +344,23 @@ typedef struct mo_kmeans_params_t { int64_t n, dim, k, max_iter; } mo_kmeans_par
 #define MO_JOIN_MERGE_MAX 64
 #define MO_XCALL_JOIN_MATCHED_MERGE 0x6015
 #define MO_XCALL_JOIN_BUILD_ROWS 0x6016
+/* ---- joins with a non-equality condition (NonEqCond, hashjoin join.go:468-498,570-611).  Three steps per probe batch:
+ *   1. JOIN_PROBE or JOIN_PROBE_GIDS with MO_JOIN_INNER: the candidate pairs, every (probe row, build row) whose keys are equal, in order.
+ *   2. SHUFFLE of the probe columns by the candidate probe rows and of the build columns by the candidate build rows, then the condition over
+ *      them with the expression entry points (GO_COMPARE, GO_ARITH, GO_MULTI_AND / OR, DEC_ARITH, ...): one bool (+ nulls) per candidate pair.
+ *   3. JOIN_COND: the join's result from the pairs and the condition.  Let P(i) = probe row i's candidates whose condition is true and not NULL,
+ *      in candidate order (empty for a row without candidates).  INNER: P(i) ; LEFT: P(i), or (i, -1) when P(i) is empty ; SEMI: (i, -1) once
+ *      when P(i) is non-empty ; ANTI: (i, -1) when P(i) is empty ; SINGLE: as LEFT, and |P(i)| > 1 fails ; RIGHT: P(i), marking its build rows ;
+ *      FULL: as LEFT, marking as RIGHT ; RIGHT_SEMI / RIGHT_ANTI: no pairs, marking as RIGHT ; RIGHT_SINGLE: as RIGHT, a build row marked a second
+ *      time (this call or an earlier one) fails.  Output order: probe rows ascending, each row's pairs in candidate order.  With a condition that
+ *      is always true the result equals JOIN_PROBE's for that type.  Capacity protocol, matched-bitmap rules and SINGLE errors are JOIN_PROBE's.
+ *      args: [0] probe_rows int64[cap] ; [1] build_rows int64[cap] ; [2] int64 count (out) ; [3] mo_join_params_t (type 0..9) ; [4] candidate
+ *      probe rows int64[npairs] (npairs = dataSz / 8) ; [5] candidate build rows int64[npairs] ; [6] the condition bool[npairs] (+pnulls) ;
+ *      [7] the matched bitmap (types 5..9; JOIN_PROBE's args[8]).  len = probe rows of the batch.  A candidate probe row outside [0, len) or below
+ *      the one before it, a negative build row, a build row past the bitmap or a short buffer: MO_RC_INVALID_ARGUMENT (naming the lowest bad
+ *      candidate position, or the build row).  One read-back, as JOIN_PROBE.  The reference evaluates the condition pair by pair and stops a semi
+ *      row at its first passing pair; here the caller evaluates every candidate, so an expression that fails on a later candidate fails here only. */
+#define MO_XCALL_JOIN_COND 0x6017
 typedef struct mo_join_params_t { int32_t join_type; int32_t reserved; } mo_join_params_t;
 #define MO_XCALL_JOIN_SELS 0x6010
 #define MO_XCALL_JOIN_FIND 0x6011

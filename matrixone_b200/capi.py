@@ -58,6 +58,8 @@ XCALL_STR_JOIN_FIND, XCALL_JOIN_PROBE_GIDS = 0x6013, 0x6014
 # right-flavoured and single joins (hashjoin types.go:317-381): types 5..9 mark the build side's matched-row bitmap; merge and finalize it
 JOIN_SINGLE, JOIN_RIGHT, JOIN_FULL, JOIN_RIGHT_SEMI, JOIN_RIGHT_ANTI, JOIN_RIGHT_SINGLE = 4, 5, 6, 7, 8, 9
 XCALL_JOIN_MATCHED_MERGE, XCALL_JOIN_BUILD_ROWS = 0x6015, 0x6016
+# joins with a non-equality condition: the join's result from the INNER candidate pairs and the condition evaluated over them
+XCALL_JOIN_COND = 0x6017
 JOIN_MERGE_MAX = 64
 STRKEY_MAX_COLS = 8
 

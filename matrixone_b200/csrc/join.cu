@@ -12,6 +12,8 @@
 //                exactly the order the reference appends them: probe rows ascending, within a row the sels ascending.  Counts -> exclusive scan ->
 //                positions; rows with >= 32 matches are written by their whole warp.  Left single, right, full, right semi / anti and right single
 //                (join.go:450-567) also mark the build side's matched-row bitmap or check the single-row rule.
+//   JOIN_COND = the same loop with a non-equality condition (join.go:468-498,570-611): the caller evaluates it over JOIN_PROBE's INNER pairs,
+//                this resolves those pairs into the join type's result.
 //   JOIN_MATCHED_MERGE = syncBitmap's OR over the workers' bitmaps (join.go:650-676); JOIN_BUILD_ROWS (colops.cu) = finalize's row list.
 //   byte-string keys   STR_JOIN_FIND = strHashmapIterator.Find over a STR_GROUP_IDS table (keytable.cuh's byte-string slots);
 //                JOIN_PROBE_GIDS = JOIN_PROBE's counting and emission over the group ids JOIN_FIND or STR_JOIN_FIND returned.
@@ -302,8 +304,8 @@ struct Marks {
         else if (!(words[r >> 6] & bit)) atomicOr(&words[r >> 6], bit);   // bits only ever go from 0 to 1: a set bit needs no atomic
     }
 };
-// the record a probe reads back in one copy: [0] result count, [1] a group id above ngroups, [2] ~(lowest LEFT SINGLE probe row with more than one
-// match), [3] ~(lowest build row matched twice), [4] ~(lowest build row past the bitmap); 0 = none
+// the record a probe reads back in one copy: [0] result count, [1] a group id above ngroups (JOIN_COND: ~(lowest malformed candidate)), [2] ~(lowest
+// LEFT SINGLE probe row with more than one match), [3] ~(lowest build row matched twice), [4] ~(lowest build row past the bitmap); 0 = none
 constexpr int kRecWords = 5;
 
 // counts per probe row of the pairs it emits.  RIGHT SEMI and RIGHT ANTI emit nothing: they mark here (groups of >= 32 sels by the whole warp)
@@ -456,6 +458,108 @@ __global__ void __launch_bounds__(kThreads) matched_merge_kernel(MergeInputs in,
         if (w == words - 1 && (nbits & 63)) { const unsigned long long live = (1ull << (nbits & 63)) - 1; o &= live; d &= live; }
         out[w] = o;
         if (twice && d) atomicMax(twice, ~(unsigned long long)(w * 64 + __ffsll((long long)d) - 1));   // ~row: 0 = none
+    }
+}
+
+// ---- JOIN_COND: a join with a non-equality condition (NonEqCond, join.go:468-498,570-611), resolved over the INNER candidate pairs ---------------
+// The caller evaluates the condition once per candidate pair; P(i) = probe row i's candidates whose condition is true and not NULL.  The record
+// is run_probe's, with [1] = ~(lowest malformed candidate position) in place of the bad group id.
+__device__ __forceinline__ bool cond_pass(const uint8_t *__restrict__ cond, const uint64_t *__restrict__ cnulls, uint64_t k) {
+    return cond[k] && !bm_test(cnulls, k);
+}
+
+// pass 1, over the pairs: validates them (probe rows in [0, len) and ascending, build rows >= 0 and, with a bitmap, inside it), gives every probe
+// row its candidate range [head, end) (candidates are sorted by probe row: segment heads and tails) and adds up its passing pairs in pc, one
+// atomic per warp and row.  RIGHT SEMI / RIGHT ANTI (head == nullptr) only mark.
+__global__ void __launch_bounds__(kThreads) cond_pairs_kernel(const int64_t *__restrict__ cp, const int64_t *__restrict__ cb, const uint8_t *__restrict__ cond,
+                                                              const uint64_t *__restrict__ cnulls, uint64_t npairs, uint64_t len, uint64_t *__restrict__ head,
+                                                              uint64_t *__restrict__ end, unsigned long long *__restrict__ pc, Marks M, unsigned long long *bad) {
+    const unsigned lane = threadIdx.x & 31;
+    for (uint64_t k0 = blockIdx.x * (uint64_t)kThreads + (threadIdx.x & ~31u); k0 < npairs; k0 += (uint64_t)gridDim.x * kThreads) {
+        const uint64_t k = k0 + lane;                    // the loop is warp-uniform: the warp aggregates its pass counts
+        int64_t p = -1;
+        bool f = false;
+        if (k < npairs) {
+            p = cp[k];
+            const int64_t b = cb[k];
+            if (p < 0 || (uint64_t)p >= len || b < 0 || (k && cp[k - 1] > p)) { atomicMax(bad, ~(unsigned long long)k); p = -1; }
+            else {
+                f = cond_pass(cond, cnulls, k);
+                if (M.past && (uint64_t)b >= M.nbits) atomicMax(M.past, ~(unsigned long long)b);
+                else if (f && !head) M.mark((uint64_t)b);
+                if (head) {
+                    if (k == 0 || cp[k - 1] != p) head[p] = k;
+                    if (k + 1 == npairs || cp[k + 1] != p) end[p] = k + 1;
+                }
+            }
+        }
+        if (head) {
+            const unsigned same = __match_any_sync(0xffffffffu, (unsigned long long)p), passing = __ballot_sync(0xffffffffu, f);
+            const unsigned c = __popc(passing & same);
+            if (p >= 0 && c && lane == (unsigned)__ffs(same) - 1) atomicAdd(&pc[p], (unsigned long long)c);
+        }
+    }
+}
+// pass 2, over the probe rows: pass count -> result rows of the row, in place
+__global__ void __launch_bounds__(kThreads) cond_count_kernel(uint64_t n, uint64_t *__restrict__ cnt, int join_type, unsigned long long *single_row) {
+    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
+        const uint64_t m = cnt[i];
+        uint64_t c;
+        switch (join_type) {
+        case MO_JOIN_LEFT: case MO_JOIN_FULL: c = m ? m : 1; break;
+        case MO_JOIN_SINGLE: c = m ? m : 1; if (m > 1) atomicMax(single_row, ~(unsigned long long)i); break;   // a second passing pair (join.go:587-589)
+        case MO_JOIN_SEMI: c = m ? 1 : 0; break;
+        case MO_JOIN_ANTI: c = m ? 0 : 1; break;
+        default: c = m; break;                           // inner, right, right single
+        }
+        cnt[i] = c;
+    }
+}
+// pass 3, over the probe rows: each passing pair is written at its row's start plus its rank among the row's passing pairs; a row that emits
+// without a passing pair writes (i, -1).  Rows with >= 32 candidates are walked by their whole warp, ranks from a ballot.  Nothing is written
+// when a candidate was malformed; RIGHT, FULL and RIGHT SINGLE mark only when the whole result fits.
+__global__ void __launch_bounds__(kThreads) cond_emit_kernel(uint64_t n, const uint64_t *__restrict__ head, const uint64_t *__restrict__ end, const uint64_t *__restrict__ pos,
+                                                             const uint64_t *__restrict__ rec, const int64_t *__restrict__ cb, const uint8_t *__restrict__ cond,
+                                                             const uint64_t *__restrict__ cnulls, int join_type, uint64_t cap, int64_t *__restrict__ out_probe,
+                                                             int64_t *__restrict__ out_build, int64_t *count_out, Marks M) {
+    const uint64_t total = rec[0];
+    if (blockIdx.x == 0 && threadIdx.x == 0) *count_out = (int64_t)total;
+    if (rec[1]) return;
+    const unsigned lane = threadIdx.x & 31;
+    const bool mark = M.words && total <= cap;
+    const bool pairs = join_type != MO_JOIN_SEMI && join_type != MO_JOIN_ANTI;
+    const uint64_t nrounds = (n + 31) / 32;
+    for (uint64_t w = (blockIdx.x * (uint64_t)kThreads + threadIdx.x) >> 5; w < nrounds; w += ((uint64_t)gridDim.x * kThreads) >> 5) {
+        const uint64_t i = w * 32 + lane;
+        uint64_t p = 0, c = 0, h = 0, e = 0;
+        if (i < n) { p = pos[i]; c = (i + 1 < n ? pos[i + 1] : total) - p; }
+        if (c && pairs) { h = head[i]; e = end[i]; }
+        if (c && (!pairs || e - h < 32)) {
+            uint64_t j = 0;
+            for (uint64_t k = h; k < e; k++) {
+                if (!cond_pass(cond, cnulls, k)) continue;
+                const int64_t b = cb[k];
+                if (p + j < cap) { out_probe[p + j] = (int64_t)i; out_build[p + j] = b; if (mark) M.mark((uint64_t)b); }
+                j++;
+            }
+            if (j == 0 && p < cap) { out_probe[p] = (int64_t)i; out_build[p] = -1; }
+        }
+        unsigned heavy = __ballot_sync(0xffffffffu, c && pairs && e - h >= 32);
+        while (heavy) {
+            const int src = __ffs(heavy) - 1; heavy &= heavy - 1;
+            const uint64_t hi = __shfl_sync(0xffffffffu, i, src), hp = __shfl_sync(0xffffffffu, p, src);
+            const uint64_t hh = __shfl_sync(0xffffffffu, h, src), he = __shfl_sync(0xffffffffu, e, src);
+            uint64_t base = 0;
+            for (uint64_t k0 = hh; k0 < he; k0 += 32) {
+                const uint64_t k = k0 + lane;
+                const bool f = k < he && cond_pass(cond, cnulls, k);
+                const unsigned ball = __ballot_sync(0xffffffffu, f);
+                const uint64_t q = hp + base + __popc(ball & ((1u << lane) - 1));
+                if (f && q < cap) { const int64_t b = cb[k]; out_probe[q] = (int64_t)hi; out_build[q] = b; if (mark) M.mark((uint64_t)b); }
+                base += __popc(ball);
+            }
+            if (base == 0 && lane == 0 && hp < cap) { out_probe[hp] = (int64_t)hi; out_build[hp] = -1; }
+        }
     }
 }
 
@@ -618,6 +722,77 @@ int xcall_join_matched_merge(mo_xcall_args_t *args, uint64_t len) {
     int frc = st.finish();
     if (rc) return rc;
     if (h) { set_error("scalar subquery returns more than 1 row (build row %llu)", ~h); return MO_RC_INTERNAL_ERROR; }
+    return frc;
+}
+
+// MO_XCALL_JOIN_COND: args [0..3] as JOIN_PROBE ; [4] candidate probe rows int64[npairs] ; [5] candidate build rows int64[npairs] ; [6] the
+// condition bool[npairs] (+pnulls) ; [7] the matched bitmap (types MO_JOIN_RIGHT and above).  len = probe rows of the batch.  Reads back the
+// record in one copy, as JOIN_PROBE does.
+int xcall_join_cond(mo_xcall_args_t *args, uint64_t len) {
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    mo_join_params_t P;
+    if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "join cond: mo_join_params_t")) return rc;
+    const int jt = P.join_type;
+    if (jt < MO_JOIN_INNER || jt > MO_JOIN_RIGHT_SINGLE) { set_error("join cond: join type %d", jt); return MO_RC_INVALID_ARGUMENT; }
+    if (jt >= MO_JOIN_RIGHT && !args[7].pdata) { set_error("join cond: join type %d needs the matched bitmap in args[7]", jt); return MO_RC_INVALID_ARGUMENT; }
+    const uint64_t cap = args[0].dataSz / 8, npairs = args[4].dataSz / 8;
+    if (args[1].dataSz / 8 < cap || !args[2].pdata || args[2].dataSz < 8 || args[5].dataSz < 8 * npairs || args[6].dataSz < npairs) {
+        set_error("join cond: buffers too small");
+        return MO_RC_INVALID_ARGUMENT;
+    }
+    const bool emits = jt != MO_JOIN_RIGHT_SEMI && jt != MO_JOIN_RIGHT_ANTI;
+    Stager st(t);
+    int64_t *out_probe = (int64_t *)st.out(args[0].pdata, cap * 8);
+    int64_t *out_build = (int64_t *)st.out(args[1].pdata, cap * 8);
+    int64_t *count = (int64_t *)st.out(args[2].pdata, 8);
+    const int64_t *cp = (const int64_t *)st.in(args[4].pdata, npairs * 8);
+    const int64_t *cb = (const int64_t *)st.in(args[5].pdata, npairs * 8);
+    const uint8_t *cond = (const uint8_t *)st.in(args[6].pdata, npairs);
+    const uint64_t *cn = (const uint64_t *)st.in(args[6].pnulls, args[6].pnulls ? ((npairs + 63) / 64) * 8 : 0);
+    uint64_t *scal = (uint64_t *)st.tmp(kRecWords * 8);
+    Marks M;
+    if (jt >= MO_JOIN_RIGHT) {
+        const uint64_t words = args[7].dataSz / 8;
+        M.words = (unsigned long long *)st.out(args[7].pdata, words * 8, true);   // in/out: a host bitmap is uploaded and copied back
+        M.nbits = words * 64; M.single = jt == MO_JOIN_RIGHT_SINGLE;
+        M.twice = (unsigned long long *)(scal + 3); M.past = (unsigned long long *)(scal + 4);
+    }
+    uint64_t *head = emits ? (uint64_t *)st.tmp(len * 8 + 8) : nullptr;
+    uint64_t *end = emits ? (uint64_t *)st.tmp(len * 8 + 8) : nullptr;
+    uint64_t *cnt = emits ? (uint64_t *)st.tmp(len * 8 + 8) : nullptr;
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, kRecWords * 8, t.stream));
+    if (emits) {
+        MOB_CUDA_TRY(cudaMemsetAsync(head, 0, len * 8, t.stream));
+        MOB_CUDA_TRY(cudaMemsetAsync(end, 0, len * 8, t.stream));
+        MOB_CUDA_TRY(cudaMemsetAsync(cnt, 0, len * 8, t.stream));
+    }
+    cudaEventRecord(t.kev0, t.stream);
+    cond_pairs_kernel<<<grid_for(npairs ? npairs : 1), kThreads, 0, t.stream>>>(cp, cb, cond, cn, npairs, len, head, end, (unsigned long long *)cnt, M,
+                                                                                 (unsigned long long *)(scal + 1));
+    MOB_LAUNCH_CHECK();
+    if (emits) {
+        cond_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(len, cnt, jt, (unsigned long long *)(scal + 2));
+        MOB_LAUNCH_CHECK();
+        int rc = exclusive_scan(t, cnt, len, cnt, scal);
+        if (rc) { st.finish(); return rc; }
+        const Marks EM = jt == MO_JOIN_RIGHT || jt == MO_JOIN_FULL || jt == MO_JOIN_RIGHT_SINGLE ? M : Marks();
+        cond_emit_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(len, head, end, cnt, scal, cb, cond, cn, jt, cap, out_probe, out_build, count, EM);
+    } else {
+        MOB_CUDA_TRY(cudaMemsetAsync(count, 0, 8, t.stream));   // right semi / right anti: marks only
+    }
+    cudaEventRecord(t.kev1, t.stream);
+    MOB_LAUNCH_CHECK();
+    uint64_t h[kRecWords] = {};
+    int rc = read_back(t, h, scal, sizeof h);
+    int frc = st.finish();
+    if (rc) return rc;
+    if (h[1]) { set_error("join cond: candidate %llu is malformed: its probe row lies outside [0, %llu) or below the one before it, or its build row is negative", (unsigned long long)~h[1], (unsigned long long)len); return MO_RC_INVALID_ARGUMENT; }
+    if (h[4]) { set_error("join cond: build row %llu lies past the matched bitmap (%llu rows)", (unsigned long long)~h[4], (unsigned long long)M.nbits); return MO_RC_INVALID_ARGUMENT; }
+    if (h[2]) { set_error("scalar subquery returns more than 1 row (probe row %llu)", (unsigned long long)~h[2]); return MO_RC_INTERNAL_ERROR; }
+    if (h[3]) { set_error("scalar subquery returns more than 1 row (build row %llu)", (unsigned long long)~h[3]); return MO_RC_INTERNAL_ERROR; }
+    if (h[0] > cap) { set_error("join cond: %lld result rows exceed the output capacity (%llu); the count is reported, call again with larger buffers", (long long)h[0], (unsigned long long)cap); return MO_RC_OUT_OF_RANGE; }
     return frc;
 }
 

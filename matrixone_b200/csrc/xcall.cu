@@ -42,6 +42,7 @@ int xcall_str_join_find(mo_xcall_args_t *args, uint64_t len);
 int xcall_join_probe_gids(mo_xcall_args_t *args, uint64_t len);
 int xcall_join_matched_merge(mo_xcall_args_t *args, uint64_t len);
 int xcall_join_build_rows(mo_xcall_args_t *args, uint64_t len);
+int xcall_join_cond(mo_xcall_args_t *args, uint64_t len);
 int tuning_set(const char *name, int value);
 }  // namespace mob
 
@@ -87,6 +88,7 @@ extern "C" int32_t XCall(int64_t runtimeId, int64_t funcId, uint8_t *errStr, uin
     else if (funcId == MO_XCALL_JOIN_PROBE_GIDS) rc = xcall_join_probe_gids(a, len);
     else if (funcId == MO_XCALL_JOIN_MATCHED_MERGE) rc = xcall_join_matched_merge(a, len);
     else if (funcId == MO_XCALL_JOIN_BUILD_ROWS) rc = xcall_join_build_rows(a, len);
+    else if (funcId == MO_XCALL_JOIN_COND) rc = xcall_join_cond(a, len);
     else if (funcId > 0x6100 && funcId <= 0x6100 + 24) rc = xcall_shuffle((int)(funcId - 0x6100), a, len);
     else if (funcId >= 0x6400 && funcId < 0x6400 + (5 << 8)) rc = xcall_group_agg((int)((funcId - 0x6400) >> 8), (int)((funcId - 0x6400) & 0xff), a, len);
     else if (funcId == MO_XCALL_Q6_MERGE) rc = xcall_q6_merge(a, len);

@@ -1173,6 +1173,38 @@ def join_matched_merge_device(out_dev, bitmaps_dev, nbuild, join_type):
     xcall(capi.XCALL_JOIN_MATCHED_MERGE, _merge_vecs(Vector(data_ptr=out_dev.ptr, data_nbytes=8 * words, length=1), ins, join_type), nbuild)
 
 
+def join_cond(cand_probe, cand_build, cond, nprobe, join_type, cond_nulls=None, capacity=None, matched=None):
+    """JOIN_COND: a join with a non-equality condition (NonEqCond, join.go:468-498,570-611) over one probe batch of nprobe rows.  cand_probe /
+    cand_build are the batch's JOIN_INNER pairs (JoinMap.probe, StrJoinMap.probe or probe_gids), cond the condition evaluated over them (one
+    bool per pair, cond_nulls its null bitmap words; NULL never passes).  Returns (probe rows, build rows) in the reference's order, as
+    JoinMap.probe does for join_type; `matched` as there."""
+    cp = np.ascontiguousarray(cand_probe, dtype=np.int64)
+    cb = np.ascontiguousarray(cand_build, dtype=np.int64)
+    c = np.ascontiguousarray(cond, dtype=np.bool_).view(np.uint8)
+    npairs = cp.shape[0]
+    prm = np.array([join_type, 0], dtype=np.int32)
+    mv = _matched_vec(matched, join_type)
+
+    def call(op, ob, cnt):
+        vecs = [Vector(data=op, length=len(op)), Vector(data=ob, length=len(ob)), Vector(data=cnt, length=1), Vector(data=prm.view(np.uint8), length=1),
+                Vector(data=cp, length=npairs), Vector(data=cb, length=npairs), _with_nulls(c, cond_nulls, npairs)] + mv
+        return xcall(capi.XCALL_JOIN_COND, vecs, nprobe, raise_on_error=False)
+    return _probe_with(call, max(npairs, nprobe), capacity)          # the result has at most npairs + nprobe rows: one call
+
+
+def join_cond_device(cand_probe_dev, cand_build_dev, cond_dev, cond_nulls_dev, npairs, nprobe, join_type, out_probe_dev, out_build_dev, count_dev,
+                     matched_dev=None):
+    """JOIN_COND on resident vectors (DeviceBuffers), the twin of probe_gids_device: npairs candidate pairs and their condition (cond_nulls_dev
+    None = no NULLs); the result goes to out_probe_dev / out_build_dev (int64, their size is the capacity) and its count to count_dev.  Reads the
+    count back (RC_OUT_OF_RANGE: the buffers are too small, the count is written)."""
+    prm = np.array([join_type, 0], dtype=np.int32)
+    vecs = [Vector(data_ptr=out_probe_dev.ptr, data_nbytes=out_probe_dev.nbytes, length=1), Vector(data_ptr=out_build_dev.ptr, data_nbytes=out_build_dev.nbytes, length=1),
+            Vector(data_ptr=count_dev.ptr, data_nbytes=8, length=1), Vector(data=prm.view(np.uint8), length=1),
+            Vector(data_ptr=cand_probe_dev.ptr, data_nbytes=8 * npairs, length=npairs), Vector(data_ptr=cand_build_dev.ptr, data_nbytes=8 * npairs, length=npairs),
+            Vector(data_ptr=cond_dev.ptr, data_nbytes=npairs, nulls_ptr=cond_nulls_dev.ptr if cond_nulls_dev is not None else None, length=npairs)]
+    xcall(capi.XCALL_JOIN_COND, vecs + _matched_vec(matched_dev, join_type), nprobe)
+
+
 # ---------------------------------------------------------------------------------------------- Elkan k-means (csrc/kmeans.cu)
 def kmeans_elkan(vectors, init_centroids, max_iter=500, rnd=None):
     """ElkanClusterer.Cluster (pkg/vectorindex/ivfflat/kmeans/elkans/clusterer.go:330-392), dense variant.  init_centroids: an array [k, dim],
