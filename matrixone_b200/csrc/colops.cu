@@ -22,6 +22,7 @@
 
 namespace mob {
 int exclusive_scan(ThreadCtx &t, const uint64_t *in, uint64_t n, uint64_t *out, uint64_t *total);   // join.cu
+int check_join_type(int join_type, const char *what, bool right_only);                              // join.cu
 int g_strkey_hash_bits = 0;
 }
 
@@ -658,7 +659,7 @@ int xcall_join_build_rows(mo_xcall_args_t *args, uint64_t len) {
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     mo_join_params_t P;
     if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "join build rows: mo_join_params_t")) return rc;
-    if (P.join_type < MO_JOIN_RIGHT || P.join_type > MO_JOIN_RIGHT_SINGLE) { set_error("join build rows: join type %d (a right-flavoured type, 5..9)", P.join_type); return MO_RC_INVALID_ARGUMENT; }
+    if (int rc = check_join_type(P.join_type, "join build rows", true)) return rc;
     const uint64_t words = (len + 63) / 64;
     if (!args[1].pdata || args[1].dataSz < 8 || (words && !args[2].pdata) || args[2].dataSz < 8 * words) { set_error("join build rows: count needs 8 bytes, the matched bitmap (len + 63) / 64 words"); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);

@@ -6,17 +6,18 @@
 //                exactly what GroupSels.Insert + Finalize (joinMapMsg.go:72-125: count, prefix sum, stable scatter) leave behind.
 //                Here: order-preserving compaction of the rows with an id, then the stable radix sort of order.cu by group id (sort_u32_pairs),
 //                offsets from a histogram + exclusive scan.
-//   probe side   JOIN_FIND = intHashMapIterator.Find (vals[i] = group id or 0; a NULL key never matches, zvals == 0).
-//                JOIN_PROBE = the emission loop of container.probe for the equality-only joins: per probe row the matched build rows in sels order
-//                (unique maps: build row = id - 1), for inner / left outer / left semi / left anti.  Output pairs (probe row, build row | -1) in
-//                exactly the order the reference appends them: probe rows ascending, within a row the sels ascending.  Counts -> exclusive scan ->
-//                positions; rows with >= 32 matches are written by their whole warp.  Left single, right, full, right semi / anti and right single
-//                (join.go:450-567) also mark the build side's matched-row bitmap or check the single-row rule.
-//   JOIN_COND = the same loop with a non-equality condition (join.go:468-498,570-611): the caller evaluates it over JOIN_PROBE's INNER pairs,
-//                this resolves those pairs into the join type's result.
+//   lookup       JOIN_FIND = intHashMapIterator.Find (vals[i] = group id or 0; a NULL key never matches, zvals == 0); STR_JOIN_FIND =
+//                strHashmapIterator.Find over a STR_GROUP_IDS table (keytable.cuh's byte-string slots).  One builder makes both kinds of table.
+//   result       JOIN_PROBE, JOIN_PROBE_GIDS and JOIN_COND are one pipeline, the emission loop of container.probe (join.go:450-611) for every
+//                join type: a first pass gives each probe row its matches and, by one type rule, its result rows; an exclusive scan turns the
+//                counts into positions; one emit pass writes the pairs (probe row, build row | -1) in exactly the order the reference appends
+//                them, probe rows ascending, within a row the build rows in order.  Only the row source of the emit pass differs:
+//                  JOIN_PROBE      the group of the probe row's key (JOIN_PROBE_GIDS: the group id JOIN_FIND or STR_JOIN_FIND returned) and its
+//                                  sels (unique maps: build row = id - 1), every build row a match;
+//                  JOIN_COND       the probe row's INNER candidate pairs (join.go:468-498,570-611), a match where the caller's non-equality
+//                                  condition passes.
+//                Right-flavoured types mark the build side's matched-row bitmap; LEFT SINGLE and RIGHT SINGLE check the single-row rule.
 //   JOIN_MATCHED_MERGE = syncBitmap's OR over the workers' bitmaps (join.go:650-676); JOIN_BUILD_ROWS (colops.cu) = finalize's row list.
-//   byte-string keys   STR_JOIN_FIND = strHashmapIterator.Find over a STR_GROUP_IDS table (keytable.cuh's byte-string slots);
-//                JOIN_PROBE_GIDS = JOIN_PROBE's counting and emission over the group ids JOIN_FIND or STR_JOIN_FIND returned.
 //   The hash table itself is not observable in the reference (random seeds): ids and pairs are.  The device table is rebuilt from table_keys per
 //   call (O(groups)) unless it was prepared with MoB200_JoinMapPrepare (cached per table_keys pointer).
 // All passes stream their inputs once; algorithmic bytes per probe row: 8 (key) + 16 per emitted pair + one random 8-byte table probe.
@@ -108,6 +109,16 @@ int exclusive_scan(ThreadCtx &t, const uint64_t *in, uint64_t n, uint64_t *out, 
     return MO_RC_SUCCESS;
 }
 
+// the join type of a join entry point (what): any type, or (right_only) a right-flavoured one, whose matched bitmap JOIN_MATCHED_MERGE and
+// JOIN_BUILD_ROWS (colops.cu) read
+int check_join_type(int join_type, const char *what, bool right_only) {
+    if (join_type < (right_only ? MO_JOIN_RIGHT : MO_JOIN_INNER) || join_type > MO_JOIN_RIGHT_SINGLE) {
+        set_error(right_only ? "%s: join type %d (a right-flavoured type, 5..9)" : "%s: join type %d", what, join_type);
+        return MO_RC_INVALID_ARGUMENT;
+    }
+    return MO_RC_SUCCESS;
+}
+
 namespace {
 
 // ---- JOIN_SELS ------------------------------------------------------------------------------------------------------------------------------------
@@ -145,16 +156,16 @@ __global__ void __launch_bounds__(kThreads) jt_build_kernel(const uint64_t *__re
         id[s] = (uint32_t)(g + 1);
     }
 }
-__device__ __forceinline__ uint32_t jt_find(const uint64_t *__restrict__ key, const uint32_t *__restrict__ id, uint64_t mask, uint64_t k) {
-    uint64_t s;
-    return kt_find(key, mask, k, s) ? id[s] : 0u;
-}
-__global__ void __launch_bounds__(kThreads) jt_find_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ knulls, uint64_t n, const uint64_t *__restrict__ tkey,
-                                                           const uint32_t *__restrict__ tid, uint64_t mask, uint64_t *__restrict__ vals) {
-    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
-        const bool isnull = knulls && ((knulls[i >> 6] >> (i & 63)) & 1ull);
-        vals[i] = isnull ? 0ull : (uint64_t)jt_find(tkey, tid, mask, keys[i]);
+// the group id of probe row i looked up by its key, 0 for a NULL or absent key (JOIN_FIND, JOIN_PROBE)
+struct KeyLookup {
+    const uint64_t *__restrict__ keys; const uint64_t *__restrict__ knulls; const uint64_t *__restrict__ tkey; const uint32_t *__restrict__ tid; uint64_t mask;
+    __device__ __forceinline__ uint32_t operator()(uint64_t i) const {
+        uint64_t s;
+        return !bm_test(knulls, i) && kt_find(tkey, mask, keys[i], s) ? tid[s] : 0u;
     }
+};
+__global__ void __launch_bounds__(kThreads) jt_find_kernel(KeyLookup lookup, uint64_t n, uint64_t *__restrict__ vals) {
+    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) vals[i] = lookup(i);
 }
 
 // ---- the string twin (STR_JOIN_FIND): keytable.cuh's byte-string slots over the table's bytes; slot row g is group g + 1 -------------------
@@ -189,97 +200,85 @@ void free_table(DevTable &T) {
     cudaFree((void *)T.sbytes); cudaFree((void *)T.soff);
 }
 
-int build_table(ThreadCtx &t, const uint64_t *dkeys, uint64_t ngroups, bool persistent, DevTable *out) {
+// the table of groups 1..ngroups, over the 8-byte keys dkeys or, when soff is given, over the byte strings sbytes / soff, all on the device; at
+// most half full.  The kind follows soff, never null for a string table (ngroups + 1 offsets); dkeys of an empty 8-byte table may be null.
+// persistent: key / id from cudaMalloc (a string table's bytes and offsets stay the caller's), else from the call's arena.
+int build_table(ThreadCtx &t, uint64_t ngroups, const uint64_t *dkeys, const uint8_t *sbytes, const uint64_t *soff, bool persistent, DevTable *out) {
     uint64_t slots = 64;
     while (slots < 2 * ngroups) slots <<= 1;
     DevTable T;
+    T.mask = slots - 1; T.ngroups = ngroups; T.cached = persistent; T.str = soff != nullptr; T.sbytes = sbytes; T.soff = soff;
+    const uint64_t nkey = T.str ? slots : slots + 1, nid = T.str ? 0 : slots + 1;   // the 8-byte table: the all-ones key in key / id[slots]
     if (persistent) {
-        if (cudaMalloc(&T.key, (slots + 1) * 8) != cudaSuccess || cudaMalloc(&T.id, (slots + 1) * 4) != cudaSuccess) {
+        if (cudaMalloc(&T.key, nkey * 8) != cudaSuccess || (nid && cudaMalloc(&T.id, nid * 4) != cudaSuccess)) {
             set_error("join map: cudaMalloc of a %llu-slot table failed", (unsigned long long)slots);
-            if (T.key) cudaFree(T.key);
+            cudaFree(T.key);
             return MO_RC_INTERNAL_ERROR;
         }
     } else {
-        T.key = (uint64_t *)arena_alloc(t, (slots + 1) * 8); T.id = (uint32_t *)arena_alloc(t, (slots + 1) * 4);
-        if (!T.key || !T.id) return MO_RC_INTERNAL_ERROR;
+        T.key = (uint64_t *)arena_alloc(t, nkey * 8);
+        T.id = nid ? (uint32_t *)arena_alloc(t, nid * 4) : nullptr;
+        if (!T.key || (nid && !T.id)) return MO_RC_INTERNAL_ERROR;
     }
-    T.mask = slots - 1; T.ngroups = ngroups; T.cached = persistent;
-    MOB_CUDA_TRY(cudaMemsetAsync(T.key, 0xff, (slots + 1) * 8, t.stream));   // every slot empty
-    MOB_CUDA_TRY(cudaMemsetAsync(T.id, 0, (slots + 1) * 4, t.stream));
+    cudaError_t e = cudaMemsetAsync(T.key, 0xff, nkey * 8, t.stream);   // every slot empty
+    if (e == cudaSuccess && nid) e = cudaMemsetAsync(T.id, 0, nid * 4, t.stream);
+    if (e != cudaSuccess) {
+        set_error("join map: clearing a %llu-slot table failed: %s", (unsigned long long)slots, cudaGetErrorString(e));
+        if (persistent) { cudaFree(T.key); cudaFree(T.id); }
+        return MO_RC_INTERNAL_ERROR;
+    }
     if (ngroups) {
-        jt_build_kernel<<<grid_for(ngroups), kThreads, 0, t.stream>>>(dkeys, ngroups, T.key, T.id, T.mask);
+        if (T.str) sjt_build_kernel<<<grid_for(ngroups), kThreads, 0, t.stream>>>(StrKeys{sbytes, soff, nullptr, nullptr, ngroups}, ngroups, T.key, T.mask, strkey_hash_mask());
+        else jt_build_kernel<<<grid_for(ngroups), kThreads, 0, t.stream>>>(dkeys, ngroups, T.key, T.id, T.mask);
         MOB_LAUNCH_CHECK();
     }
     *out = T;
     return MO_RC_SUCCESS;
+}
+
+// the table prepared under key (table_keys, or a string map's offsets pointer) for ngroups groups: true, with lk holding g_jm_mu shared for as long
+// as the caller reads the table, or false with lk released
+bool find_prepared(const void *key, uint64_t ngroups, bool str, DevTable *T, std::shared_lock<std::shared_mutex> &lk) {
+    lk = std::shared_lock<std::shared_mutex>(g_jm_mu);
+    auto it = g_jm.find(key);
+    if (it != g_jm.end() && it->second.ngroups == ngroups && it->second.str == str) { *T = it->second; return true; }
+    lk.unlock();
+    return false;
+}
+
+// makes T the table prepared under key, releasing the one it replaces
+void publish_prepared(const void *key, const DevTable &T) {
+    std::unique_lock<std::shared_mutex> lk(g_jm_mu);
+    auto it = g_jm.find(key);
+    if (it != g_jm.end()) free_table(it->second);
+    g_jm[key] = T;
 }
 
 // the table for this call: the prepared one (by the caller's table_keys pointer) or a scratch one in the arena
 int table_for(ThreadCtx &t, Stager &st, const mo_xcall_args_t &a, DevTable *T, std::shared_lock<std::shared_mutex> &lk) {
     const uint64_t ngroups = a.dataSz / 8;
-    lk = std::shared_lock<std::shared_mutex>(g_jm_mu);
-    auto it = g_jm.find(a.pdata);
-    if (it != g_jm.end() && it->second.ngroups == ngroups && !it->second.str) { *T = it->second; return MO_RC_SUCCESS; }
-    lk.unlock();
+    if (find_prepared(a.pdata, ngroups, false, T, lk)) return MO_RC_SUCCESS;
     const uint64_t *dkeys = (const uint64_t *)st.in(a.pdata, ngroups * 8);
     if (st.failed) return MO_RC_INTERNAL_ERROR;
-    return build_table(t, dkeys, ngroups, false, T);
-}
-
-// the string table of groups 1..ngroups whose bytes / offsets are on the device; persistent: slots from cudaMalloc (the caller owns the rest)
-int build_str_table(ThreadCtx &t, const uint8_t *dbytes, const uint64_t *doff, uint64_t ngroups, bool persistent, DevTable *out) {
-    uint64_t slots = 64;
-    while (slots < 2 * ngroups) slots <<= 1;
-    DevTable T;
-    if (persistent) {
-        if (cudaMalloc(&T.key, slots * 8) != cudaSuccess) { set_error("join map: cudaMalloc of a %llu-slot table failed", (unsigned long long)slots); return MO_RC_INTERNAL_ERROR; }
-    } else {
-        T.key = (uint64_t *)arena_alloc(t, slots * 8);
-        if (!T.key) return MO_RC_INTERNAL_ERROR;
-    }
-    T.mask = slots - 1; T.ngroups = ngroups; T.cached = persistent; T.str = true; T.sbytes = dbytes; T.soff = doff;
-    const cudaError_t e = cudaMemsetAsync(T.key, 0xff, slots * 8, t.stream);
-    if (e != cudaSuccess) {
-        set_error("join map: clearing a %llu-slot table failed: %s", (unsigned long long)slots, cudaGetErrorString(e));
-        if (persistent) cudaFree(T.key);
-        return MO_RC_INTERNAL_ERROR;
-    }
-    if (ngroups) {
-        sjt_build_kernel<<<grid_for(ngroups), kThreads, 0, t.stream>>>(StrKeys{dbytes, doff, nullptr, nullptr, ngroups}, ngroups, T.key, T.mask, strkey_hash_mask());
-        MOB_LAUNCH_CHECK();
-    }
-    *out = T;
-    return MO_RC_SUCCESS;
+    return build_table(t, ngroups, dkeys, nullptr, nullptr, false, T);
 }
 
 // the prepared string table keyed by the table offsets pointer, or a scratch one
 int str_table_for(ThreadCtx &t, Stager &st, const mo_xcall_args_t &bytes, const mo_xcall_args_t &offs, uint64_t ngroups, DevTable *T,
                   std::shared_lock<std::shared_mutex> &lk) {
-    lk = std::shared_lock<std::shared_mutex>(g_jm_mu);
-    auto it = g_jm.find(offs.pdata);
-    if (it != g_jm.end() && it->second.ngroups == ngroups && it->second.str) {
+    if (find_prepared(offs.pdata, ngroups, true, T, lk)) {
         // nothing is staged, but a table prepared from host memory keeps the call synchronous, as a staged one does
         st.device(bytes.pdata); st.device(offs.pdata);
-        *T = it->second;
         return MO_RC_SUCCESS;
     }
-    lk.unlock();
     const uint8_t *db = (const uint8_t *)st.in(bytes.pdata, bytes.dataSz);
     const uint64_t *doff = (const uint64_t *)st.in(offs.pdata, (ngroups + 1) * 8);
     if (st.failed) return MO_RC_INTERNAL_ERROR;
-    return build_str_table(t, db, doff, ngroups, false, T);
+    return build_table(t, ngroups, nullptr, db, doff, false, T);
 }
 
 // ---- JOIN_PROBE / JOIN_PROBE_GIDS ---------------------------------------------------------------------------------------------------------------
-// the group id of probe row i: looked up by its key (JOIN_PROBE) ...
-struct KeyLookup {
-    const uint64_t *__restrict__ keys; const uint64_t *__restrict__ knulls; const uint64_t *__restrict__ tkey; const uint32_t *__restrict__ tid; uint64_t mask;
-    __device__ __forceinline__ uint32_t operator()(uint64_t i) const {
-        const bool isnull = knulls && ((knulls[i >> 6] >> (i & 63)) & 1ull);
-        return isnull ? 0u : jt_find(tkey, tid, mask, keys[i]);
-    }
-};
-// ... or given (JOIN_PROBE_GIDS); an id above ngroups sets *bad
+// the group id of probe row i: KeyLookup (JOIN_PROBE), or given (JOIN_PROBE_GIDS); an id above ngroups sets *bad
 struct GidLookup {
     const uint64_t *__restrict__ gids; uint64_t ngroups; unsigned *bad;
     __device__ __forceinline__ uint32_t operator()(uint64_t i) const {
@@ -304,13 +303,26 @@ struct Marks {
         else if (!(words[r >> 6] & bit)) atomicOr(&words[r >> 6], bit);   // bits only ever go from 0 to 1: a set bit needs no atomic
     }
 };
-// the record a probe reads back in one copy: [0] result count, [1] a group id above ngroups (JOIN_COND: ~(lowest malformed candidate)), [2] ~(lowest
-// LEFT SINGLE probe row with more than one match), [3] ~(lowest build row matched twice), [4] ~(lowest build row past the bitmap); 0 = none
+// the record a join call reads back in one copy: [0] result count, [1] a group id above ngroups (JOIN_COND: ~(lowest malformed candidate)), [2]
+// ~(lowest LEFT SINGLE probe row with more than one match), [3] ~(lowest build row matched twice), [4] ~(lowest build row past the bitmap); 0 = none
 constexpr int kRecWords = 5;
 
-// counts per probe row of the pairs it emits.  RIGHT SEMI and RIGHT ANTI emit nothing: they mark here (groups of >= 32 sels by the whole warp)
-// and the call skips the scan and the emit pass (cnt == nullptr).  The types that emit pairs mark in the emit pass, once the result is known to
-// fit, so a call that fails with MO_RC_OUT_OF_RANGE leaves the bitmap as it was and its repeat marks each pair once.
+// the result rows of probe row i with m matches (JOIN_COND: passing pairs) for the join type; LEFT SINGLE records a row with more than one
+// (join.go:504-507,587-589).  RIGHT SEMI and RIGHT ANTI emit nothing: they only mark (join.go:452,549).
+__device__ __forceinline__ uint64_t result_rows(int join_type, uint64_t m, uint64_t i, unsigned long long *single_row) {
+    switch (join_type) {
+    case MO_JOIN_INNER: case MO_JOIN_RIGHT: case MO_JOIN_RIGHT_SINGLE: return m;
+    case MO_JOIN_LEFT: case MO_JOIN_FULL: return m ? m : 1;           // EmitUnmatchedProbe: one row with the build side NULL
+    case MO_JOIN_SINGLE: if (m > 1) atomicMax(single_row, ~(unsigned long long)i); return m ? m : 1;
+    case MO_JOIN_SEMI: return m ? 1 : 0;
+    case MO_JOIN_ANTI: return m ? 0 : 1;
+    default: return 0;
+    }
+}
+
+// counts per probe row of the rows it emits.  RIGHT SEMI and RIGHT ANTI mark here (groups of >= 32 sels by the whole warp) and the call skips
+// the scan and the emit pass (cnt == nullptr).  The types that emit pairs mark in the emit pass, once the result is known to fit, so a call that
+// fails with MO_RC_OUT_OF_RANGE leaves the bitmap as it was and its repeat marks each pair once.
 template <class Lookup>
 __global__ void __launch_bounds__(kThreads) probe_count_kernel(Lookup lookup, uint64_t n, const int32_t *__restrict__ offsets, const int32_t *__restrict__ sels,
                                                                int join_type, uint32_t *__restrict__ vals, uint64_t *__restrict__ cnt, Marks M,
@@ -324,15 +336,7 @@ __global__ void __launch_bounds__(kThreads) probe_count_kernel(Lookup lookup, ui
         if (i < n) {
             v = lookup(i);
             if (v) m = offsets ? (uint64_t)(offsets[v] - offsets[v - 1]) : 1ull;
-            uint64_t c;
-            switch (join_type) {
-            case MO_JOIN_INNER: case MO_JOIN_RIGHT: case MO_JOIN_RIGHT_SINGLE: c = m; break;
-            case MO_JOIN_LEFT: case MO_JOIN_FULL: c = m ? m : 1; break;      // EmitUnmatchedProbe: one row with the build side NULL
-            case MO_JOIN_SINGLE: c = m ? m : 1; if (m > 1) atomicMax(single_row, ~(unsigned long long)i); break;   // join.go:504-507
-            case MO_JOIN_SEMI: c = m ? 1 : 0; break;
-            case MO_JOIN_ANTI: c = m ? 0 : 1; break;
-            default: c = 0; break;                       // right semi / right anti: marks only (join.go:452,549)
-            }
+            const uint64_t c = result_rows(join_type, m, i, single_row);
             if (cnt) { vals[i] = m ? v : 0u; cnt[i] = c; }
         }
         if (mark_here) {
@@ -348,105 +352,21 @@ __global__ void __launch_bounds__(kThreads) probe_count_kernel(Lookup lookup, ui
         }
     }
 }
-// the minimum of 7 CTAs per SM is only there to steer ptxas: with it the kernel fits 32 registers without a spill, without it ptxas spills 4 bytes
-__global__ void __launch_bounds__(kThreads, 7) probe_emit_kernel(uint64_t n, const uint32_t *__restrict__ vals, const uint64_t *__restrict__ pos, const uint64_t *__restrict__ total,
-                                                              const int32_t *__restrict__ offsets, const int32_t *__restrict__ sels, int join_type, uint64_t cap,
-                                                              int64_t *__restrict__ out_probe, int64_t *__restrict__ out_build, int64_t *count_out, Marks M) {
-    const unsigned lane = threadIdx.x & 31;
-    const uint64_t nrounds = (n + 31) / 32;
-    // RIGHT, FULL and RIGHT SINGLE mark the build row of every pair they emit, and only when the whole result fits
-    const bool mark = M.words && *total <= cap;
-    for (uint64_t w = (blockIdx.x * (uint64_t)kThreads + threadIdx.x) >> 5; w < nrounds; w += ((uint64_t)gridDim.x * kThreads) >> 5) {
-        const uint64_t i = w * 32 + lane;
-        uint32_t v = 0; uint64_t p = 0, c = 0;
-        if (i < n) { v = vals[i]; p = pos[i]; c = (i + 1 < n ? pos[i + 1] : *total) - p; }
-        const bool pairs = v && join_type != MO_JOIN_SEMI && join_type != MO_JOIN_ANTI;
-        const int32_t s0 = (pairs && offsets) ? offsets[v - 1] : 0;
-        if (c && c < 32) {
-            for (uint64_t j = 0; j < c; j++) {
-                if (p + j >= cap) break;
-                const int64_t b = pairs ? (offsets ? (int64_t)sels[s0 + j] : (int64_t)v - 1) : -1;
-                out_probe[p + j] = (int64_t)i;
-                out_build[p + j] = b;
-                if (mark && pairs) M.mark((uint64_t)b);
-            }
-        }
-        unsigned heavy = __ballot_sync(0xffffffffu, c >= 32);
-        while (heavy) {                                   // rows with many matches are written by the whole warp, coalesced
-            const int src = __ffs(heavy) - 1; heavy &= heavy - 1;
-            const uint64_t hi = __shfl_sync(0xffffffffu, i, src), hp = __shfl_sync(0xffffffffu, p, src), hc = __shfl_sync(0xffffffffu, c, src);
-            const int32_t hs0 = __shfl_sync(0xffffffffu, s0, src);
-            for (uint64_t j = lane; j < hc; j += 32) {
-                if (hp + j >= cap) break;
-                const int32_t b = sels[hs0 + j];          // >= 32 matches only happens with sels
-                out_probe[hp + j] = (int64_t)hi;
-                out_build[hp + j] = (int64_t)b;
-                if (mark) M.mark((uint64_t)b);
-            }
-        }
-    }
-    if (blockIdx.x == 0 && threadIdx.x == 0) *count_out = (int64_t)*total;
-}
 
-// the output side shared by JOIN_PROBE and JOIN_PROBE_GIDS: args [0] probe_rows, [1] build_rows, [2] count, [5] / [6] sels, [8] the matched bitmap
-// (types MO_JOIN_RIGHT and above); reads back the record (kRecWords words at scal, [1] set by the lookup) in one copy
-template <class Lookup>
-int run_probe(ThreadCtx &t, Stager &st, mo_xcall_args_t *args, uint64_t len, int join_type, uint64_t ngroups, Lookup lookup, uint64_t *scal) {
-    const uint64_t cap = args[0].dataSz / 8;
-    const bool multi = args[5].pdata != nullptr;
-    const bool emits = join_type != MO_JOIN_RIGHT_SEMI && join_type != MO_JOIN_RIGHT_ANTI;
-    int64_t *out_probe = (int64_t *)st.out(args[0].pdata, cap * 8);
-    int64_t *out_build = (int64_t *)st.out(args[1].pdata, cap * 8);
-    int64_t *count = (int64_t *)st.out(args[2].pdata, 8);
-    const int32_t *offsets = multi ? (const int32_t *)st.in(args[5].pdata, (ngroups + 2) * 4) : nullptr;
-    const int32_t *sels = multi ? (const int32_t *)st.in(args[6].pdata, args[6].dataSz) : nullptr;
-    Marks M;
-    if (join_type >= MO_JOIN_RIGHT) {
-        const uint64_t words = args[8].dataSz / 8;
-        M.words = (unsigned long long *)st.out(args[8].pdata, words * 8, true);   // in/out: a host bitmap is uploaded and copied back
-        M.nbits = words * 64; M.single = join_type == MO_JOIN_RIGHT_SINGLE;
-        M.twice = (unsigned long long *)(scal + 3); M.past = (unsigned long long *)(scal + 4);
+// The emit pass reads each probe row's build rows from a row source: range(i, c, h, e) gives row i, which emits c rows, its entries [h, e);
+// build(k) is the build row of entry k and pass(k) whether the entry is a match.
+// JOIN_PROBE / JOIN_PROBE_GIDS: the matched group's sels (vals[i] = group id, 0 = no match), every entry a match, so the row's count from the scan
+// is its entry count.  A unique map has entry v - 1 = build row v - 1.
+struct ProbeRows {
+    const uint32_t *__restrict__ vals; const int32_t *__restrict__ offsets; const int32_t *__restrict__ sels;
+    __device__ __forceinline__ void range(uint64_t i, uint64_t c, uint64_t &h, uint64_t &e) const {
+        const uint32_t v = vals[i];
+        h = v ? (offsets ? (uint64_t)offsets[v - 1] : (uint64_t)v - 1) : 0;
+        e = v ? h + c : 0;
     }
-    uint32_t *vals = emits ? (uint32_t *)st.tmp(len * 4 + 4) : nullptr;
-    uint64_t *cnt = emits ? (uint64_t *)st.tmp((len + 1) * 8) : nullptr;
-    if (st.failed) return MO_RC_INTERNAL_ERROR;
-    cudaEventRecord(t.kev0, t.stream);
-    probe_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(lookup, len, offsets, sels, join_type, vals, cnt, M, (unsigned long long *)(scal + 2));
-    MOB_LAUNCH_CHECK();
-    if (emits) {
-        int rc = exclusive_scan(t, cnt, len, cnt, scal);
-        if (rc) { st.finish(); return rc; }
-        const Marks EM = join_type == MO_JOIN_RIGHT || join_type == MO_JOIN_FULL || join_type == MO_JOIN_RIGHT_SINGLE ? M : Marks();
-        probe_emit_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(len, vals, cnt, scal, offsets, sels, join_type, cap, out_probe, out_build, count, EM);
-    } else {
-        MOB_CUDA_TRY(cudaMemsetAsync(count, 0, 8, t.stream));   // right semi / right anti: no pairs during the probe
-    }
-    cudaEventRecord(t.kev1, t.stream);
-    MOB_LAUNCH_CHECK();
-    uint64_t h[kRecWords] = {};
-    int rc = read_back(t, h, scal, sizeof h);
-    int frc = st.finish();
-    if (rc) return rc;
-    if (h[1]) { set_error("join probe: a group id exceeds the group count (%llu)", (unsigned long long)ngroups); return MO_RC_INVALID_ARGUMENT; }
-    if (h[4]) { set_error("join probe: build row %llu lies past the matched bitmap (%llu rows)", (unsigned long long)~h[4], (unsigned long long)M.nbits); return MO_RC_INVALID_ARGUMENT; }
-    if (h[2]) { set_error("scalar subquery returns more than 1 row (probe row %llu)", (unsigned long long)~h[2]); return MO_RC_INTERNAL_ERROR; }
-    if (h[3]) { set_error("scalar subquery returns more than 1 row (build row %llu)", (unsigned long long)~h[3]); return MO_RC_INTERNAL_ERROR; }
-    if (h[0] > cap) { set_error("join probe: %lld result rows exceed the output capacity (%llu); the count is reported, call again with larger buffers", (long long)h[0], (unsigned long long)cap); return MO_RC_OUT_OF_RANGE; }
-    return frc;
-}
-
-// the join-type and matched-bitmap checks of JOIN_PROBE and JOIN_PROBE_GIDS; a unique map (no sels) names build rows 0 .. ngroups - 1, so its bitmap
-// must hold ngroups bits (with sels, a row past the bitmap is found on the device)
-int check_probe_type(const mo_xcall_args_t *args, int join_type, uint64_t ngroups, const char *what) {
-    if (join_type < MO_JOIN_INNER || join_type > MO_JOIN_RIGHT_SINGLE) { set_error("%s: join type %d", what, join_type); return MO_RC_INVALID_ARGUMENT; }
-    if (join_type < MO_JOIN_RIGHT) return MO_RC_SUCCESS;
-    if (!args[8].pdata) { set_error("%s: join type %d needs the matched bitmap in args[8]", what, join_type); return MO_RC_INVALID_ARGUMENT; }
-    if (!args[5].pdata && args[8].dataSz / 8 < (ngroups + 63) / 64) {
-        set_error("%s: the matched bitmap holds %llu rows, the build side has %llu", what, (unsigned long long)(args[8].dataSz / 8 * 64), (unsigned long long)ngroups);
-        return MO_RC_INVALID_ARGUMENT;
-    }
-    return MO_RC_SUCCESS;
-}
+    __device__ __forceinline__ int64_t build(uint64_t k) const { return offsets ? (int64_t)sels[k] : (int64_t)k; }
+    __device__ __forceinline__ bool pass(uint64_t) const { return true; }
+};
 
 // ---- JOIN_MATCHED_MERGE: syncBitmap's OR over the workers' bitmaps (join.go:650-676) ------------------------------------------------------------
 struct MergeInputs { const unsigned long long *p[MO_JOIN_MERGE_MAX]; };
@@ -462,11 +382,19 @@ __global__ void __launch_bounds__(kThreads) matched_merge_kernel(MergeInputs in,
 }
 
 // ---- JOIN_COND: a join with a non-equality condition (NonEqCond, join.go:468-498,570-611), resolved over the INNER candidate pairs ---------------
-// The caller evaluates the condition once per candidate pair; P(i) = probe row i's candidates whose condition is true and not NULL.  The record
-// is run_probe's, with [1] = ~(lowest malformed candidate position) in place of the bad group id.
+// The caller evaluates the condition once per candidate pair; P(i) = probe row i's candidates whose condition is true and not NULL.  Record word 1
+// holds ~(lowest malformed candidate position) in place of the bad group id.
 __device__ __forceinline__ bool cond_pass(const uint8_t *__restrict__ cond, const uint64_t *__restrict__ cnulls, uint64_t k) {
     return cond[k] && !bm_test(cnulls, k);
 }
+// the row source of the emit pass: row i's candidates [head[i], end[i]), a match where the condition passes
+struct CondRows {
+    const uint64_t *__restrict__ head; const uint64_t *__restrict__ end; const int64_t *__restrict__ cb; const uint8_t *__restrict__ cond;
+    const uint64_t *__restrict__ cnulls;
+    __device__ __forceinline__ void range(uint64_t i, uint64_t, uint64_t &h, uint64_t &e) const { h = head[i]; e = end[i]; }
+    __device__ __forceinline__ int64_t build(uint64_t k) const { return cb[k]; }
+    __device__ __forceinline__ bool pass(uint64_t k) const { return cond_pass(cond, cnulls, k); }
+};
 
 // pass 1, over the pairs: validates them (probe rows in [0, len) and ascending, build rows >= 0 and, with a bitmap, inside it), gives every probe
 // row its candidate range [head, end) (candidates are sorted by probe row: segment heads and tails) and adds up its passing pairs in pc, one
@@ -502,26 +430,17 @@ __global__ void __launch_bounds__(kThreads) cond_pairs_kernel(const int64_t *__r
 }
 // pass 2, over the probe rows: pass count -> result rows of the row, in place
 __global__ void __launch_bounds__(kThreads) cond_count_kernel(uint64_t n, uint64_t *__restrict__ cnt, int join_type, unsigned long long *single_row) {
-    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
-        const uint64_t m = cnt[i];
-        uint64_t c;
-        switch (join_type) {
-        case MO_JOIN_LEFT: case MO_JOIN_FULL: c = m ? m : 1; break;
-        case MO_JOIN_SINGLE: c = m ? m : 1; if (m > 1) atomicMax(single_row, ~(unsigned long long)i); break;   // a second passing pair (join.go:587-589)
-        case MO_JOIN_SEMI: c = m ? 1 : 0; break;
-        case MO_JOIN_ANTI: c = m ? 0 : 1; break;
-        default: c = m; break;                           // inner, right, right single
-        }
-        cnt[i] = c;
-    }
+    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads)
+        cnt[i] = result_rows(join_type, cnt[i], i, single_row);
 }
-// pass 3, over the probe rows: each passing pair is written at its row's start plus its rank among the row's passing pairs; a row that emits
-// without a passing pair writes (i, -1).  Rows with >= 32 candidates are walked by their whole warp, ranks from a ballot.  Nothing is written
-// when a candidate was malformed; RIGHT, FULL and RIGHT SINGLE mark only when the whole result fits.
-__global__ void __launch_bounds__(kThreads) cond_emit_kernel(uint64_t n, const uint64_t *__restrict__ head, const uint64_t *__restrict__ end, const uint64_t *__restrict__ pos,
-                                                             const uint64_t *__restrict__ rec, const int64_t *__restrict__ cb, const uint8_t *__restrict__ cond,
-                                                             const uint64_t *__restrict__ cnulls, int join_type, uint64_t cap, int64_t *__restrict__ out_probe,
-                                                             int64_t *__restrict__ out_build, int64_t *count_out, Marks M) {
+
+// ---- the emit pass, over the probe rows ------------------------------------------------------------------------------------------------------------
+// Each matching entry of a row is written at the row's scanned position plus its rank among the row's matches; a row that emits without a match
+// writes (i, -1), as SEMI and ANTI rows always do.  Rows with >= 32 entries are walked by their whole warp, ranks from a ballot.  Nothing is
+// written when record word 1 is set; RIGHT, FULL and RIGHT SINGLE mark (M.words) only when the whole result fits.
+template <class Rows>
+__global__ void __launch_bounds__(kThreads) emit_kernel(Rows R, uint64_t n, const uint64_t *__restrict__ pos, const uint64_t *__restrict__ rec, int join_type,
+                                                        uint64_t cap, int64_t *__restrict__ out_probe, int64_t *__restrict__ out_build, int64_t *count_out, Marks M) {
     const uint64_t total = rec[0];
     if (blockIdx.x == 0 && threadIdx.x == 0) *count_out = (int64_t)total;
     if (rec[1]) return;
@@ -533,18 +452,19 @@ __global__ void __launch_bounds__(kThreads) cond_emit_kernel(uint64_t n, const u
         const uint64_t i = w * 32 + lane;
         uint64_t p = 0, c = 0, h = 0, e = 0;
         if (i < n) { p = pos[i]; c = (i + 1 < n ? pos[i + 1] : total) - p; }
-        if (c && pairs) { h = head[i]; e = end[i]; }
-        if (c && (!pairs || e - h < 32)) {
+        if (c && pairs) R.range(i, c, h, e);
+        if (c && e - h < 32) {
             uint64_t j = 0;
+#pragma unroll 1   // unrolled, the probe's walk (no entry can fail) takes 40 registers and 6 CTAs per SM instead of 32 and 8
             for (uint64_t k = h; k < e; k++) {
-                if (!cond_pass(cond, cnulls, k)) continue;
-                const int64_t b = cb[k];
+                if (!R.pass(k)) continue;
+                const int64_t b = R.build(k);
                 if (p + j < cap) { out_probe[p + j] = (int64_t)i; out_build[p + j] = b; if (mark) M.mark((uint64_t)b); }
                 j++;
             }
             if (j == 0 && p < cap) { out_probe[p] = (int64_t)i; out_build[p] = -1; }
         }
-        unsigned heavy = __ballot_sync(0xffffffffu, c && pairs && e - h >= 32);
+        unsigned heavy = __ballot_sync(0xffffffffu, c && e - h >= 32);
         while (heavy) {
             const int src = __ffs(heavy) - 1; heavy &= heavy - 1;
             const uint64_t hi = __shfl_sync(0xffffffffu, i, src), hp = __shfl_sync(0xffffffffu, p, src);
@@ -552,15 +472,92 @@ __global__ void __launch_bounds__(kThreads) cond_emit_kernel(uint64_t n, const u
             uint64_t base = 0;
             for (uint64_t k0 = hh; k0 < he; k0 += 32) {
                 const uint64_t k = k0 + lane;
-                const bool f = k < he && cond_pass(cond, cnulls, k);
+                const bool f = k < he && R.pass(k);
                 const unsigned ball = __ballot_sync(0xffffffffu, f);
                 const uint64_t q = hp + base + __popc(ball & ((1u << lane) - 1));
-                if (f && q < cap) { const int64_t b = cb[k]; out_probe[q] = (int64_t)hi; out_build[q] = b; if (mark) M.mark((uint64_t)b); }
+                if (f && q < cap) { const int64_t b = R.build(k); out_probe[q] = (int64_t)hi; out_build[q] = b; if (mark) M.mark((uint64_t)b); }
                 base += __popc(ball);
             }
             if (base == 0 && lane == 0 && hp < cap) { out_probe[hp] = (int64_t)hi; out_build[hp] = -1; }
         }
     }
+}
+
+// The end of JOIN_PROBE, JOIN_PROBE_GIDS and JOIN_COND.  Stages args [0] probe_rows, [1] build_rows, [2] count and args[mi], the matched bitmap of
+// types MO_JOIN_RIGHT and above, and zeroes the record; first(M, record) launches the first pass, which leaves each probe row's result rows in cnt
+// or, for RIGHT SEMI / RIGHT ANTI (cnt == nullptr), marks.  Then the scan and the emit pass over R, and the record read back in one copy:
+// word1(h[1]) sets the caller's error for word 1, the others name the caller (what).
+template <class Rows, class First, class Word1>
+int join_tail(ThreadCtx &t, Stager &st, mo_xcall_args_t *args, int mi, int join_type, uint64_t len, uint64_t *cnt, Rows R, First first, const char *what,
+              Word1 word1) {
+    const uint64_t cap = args[0].dataSz / 8;
+    uint64_t *scal = (uint64_t *)st.tmp(kRecWords * 8);
+    int64_t *out_probe = (int64_t *)st.out(args[0].pdata, cap * 8);
+    int64_t *out_build = (int64_t *)st.out(args[1].pdata, cap * 8);
+    int64_t *count = (int64_t *)st.out(args[2].pdata, 8);
+    Marks M;
+    if (join_type >= MO_JOIN_RIGHT) {
+        const uint64_t words = args[mi].dataSz / 8;
+        M.words = (unsigned long long *)st.out(args[mi].pdata, words * 8, true);   // in/out: a host bitmap is uploaded and copied back
+        M.nbits = words * 64; M.single = join_type == MO_JOIN_RIGHT_SINGLE;
+        M.twice = (unsigned long long *)(scal + 3); M.past = (unsigned long long *)(scal + 4);
+    }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, kRecWords * 8, t.stream));
+    cudaEventRecord(t.kev0, t.stream);
+    if (int rc = first(M, scal)) return rc;
+    if (cnt) {
+        int rc = exclusive_scan(t, cnt, len, cnt, scal);
+        if (rc) { st.finish(); return rc; }
+        const Marks EM = join_type == MO_JOIN_RIGHT || join_type == MO_JOIN_FULL || join_type == MO_JOIN_RIGHT_SINGLE ? M : Marks();
+        emit_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(R, len, cnt, scal, join_type, cap, out_probe, out_build, count, EM);
+    } else {
+        MOB_CUDA_TRY(cudaMemsetAsync(count, 0, 8, t.stream));   // right semi / right anti: no pairs during the probe
+    }
+    cudaEventRecord(t.kev1, t.stream);
+    MOB_LAUNCH_CHECK();
+    uint64_t h[kRecWords] = {};
+    int rc = read_back(t, h, scal, sizeof h);
+    int frc = st.finish();
+    if (rc) return rc;
+    if (h[1]) { word1(h[1]); return MO_RC_INVALID_ARGUMENT; }
+    if (h[4]) { set_error("%s: build row %llu lies past the matched bitmap (%llu rows)", what, (unsigned long long)~h[4], (unsigned long long)M.nbits); return MO_RC_INVALID_ARGUMENT; }
+    if (h[2]) { set_error("scalar subquery returns more than 1 row (probe row %llu)", (unsigned long long)~h[2]); return MO_RC_INTERNAL_ERROR; }
+    if (h[3]) { set_error("scalar subquery returns more than 1 row (build row %llu)", (unsigned long long)~h[3]); return MO_RC_INTERNAL_ERROR; }
+    if (h[0] > cap) { set_error("%s: %lld result rows exceed the output capacity (%llu); the count is reported, call again with larger buffers", what, (long long)h[0], (unsigned long long)cap); return MO_RC_OUT_OF_RANGE; }
+    return frc;
+}
+
+// JOIN_PROBE and JOIN_PROBE_GIDS after the lookup's inputs: args [5] / [6] sels, [8] the matched bitmap; lookup_at(record) is the lookup, which may
+// set record word 1
+template <class LookupAt>
+int run_probe(ThreadCtx &t, Stager &st, mo_xcall_args_t *args, uint64_t len, int join_type, uint64_t ngroups, LookupAt lookup_at) {
+    const bool multi = args[5].pdata != nullptr;
+    const bool emits = join_type != MO_JOIN_RIGHT_SEMI && join_type != MO_JOIN_RIGHT_ANTI;
+    const int32_t *offsets = multi ? (const int32_t *)st.in(args[5].pdata, (ngroups + 2) * 4) : nullptr;
+    const int32_t *sels = multi ? (const int32_t *)st.in(args[6].pdata, args[6].dataSz) : nullptr;
+    uint32_t *vals = emits ? (uint32_t *)st.tmp(len * 4 + 4) : nullptr;
+    uint64_t *cnt = emits ? (uint64_t *)st.tmp((len + 1) * 8) : nullptr;
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    return join_tail(t, st, args, 8, join_type, len, cnt, ProbeRows{vals, offsets, sels}, [&](const Marks &M, uint64_t *rec) {
+        probe_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(lookup_at(rec), len, offsets, sels, join_type, vals, cnt, M, (unsigned long long *)(rec + 2));
+        MOB_LAUNCH_CHECK();
+        return MO_RC_SUCCESS;
+    }, "join probe", [&](uint64_t) { set_error("join probe: a group id exceeds the group count (%llu)", (unsigned long long)ngroups); });
+}
+
+// the argument checks of JOIN_PROBE and JOIN_PROBE_GIDS; a unique map (no sels) names build rows 0 .. ngroups - 1, so its bitmap must hold ngroups
+// bits (with sels, a row past the bitmap is found on the device)
+int check_probe_args(const mo_xcall_args_t *args, uint64_t len, int join_type, uint64_t ngroups, const char *what) {
+    if (int rc = check_join_type(join_type, what, false)) return rc;
+    if (join_type >= MO_JOIN_RIGHT && !args[8].pdata) { set_error("%s: join type %d needs the matched bitmap in args[8]", what, join_type); return MO_RC_INVALID_ARGUMENT; }
+    if (join_type >= MO_JOIN_RIGHT && !args[5].pdata && args[8].dataSz / 8 < (ngroups + 63) / 64) {
+        set_error("%s: the matched bitmap holds %llu rows, the build side has %llu", what, (unsigned long long)(args[8].dataSz / 8 * 64), (unsigned long long)ngroups);
+        return MO_RC_INVALID_ARGUMENT;
+    }
+    if (args[1].dataSz / 8 < args[0].dataSz / 8 || !args[2].pdata || args[2].dataSz < 8 || args[7].dataSz < 8 * len) { set_error("%s: buffers too small", what); return MO_RC_INVALID_ARGUMENT; }
+    if (args[5].pdata && args[5].dataSz < (ngroups + 2) * 4) { set_error("%s: sels offsets shorter than the group count + 2", what); return MO_RC_INVALID_ARGUMENT; }
+    return MO_RC_SUCCESS;
 }
 
 }  // namespace
@@ -635,7 +632,7 @@ int xcall_join_find(mo_xcall_args_t *args, uint64_t len) {
     const uint64_t *kn = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? ((len + 63) / 64) * 8 : 0);
     if (st.failed) return MO_RC_INTERNAL_ERROR;
     cudaEventRecord(t.kev0, t.stream);
-    jt_find_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(keys, kn, len, T.key, T.id, T.mask, vals);
+    jt_find_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(KeyLookup{keys, kn, T.key, T.id, T.mask}, len, vals);
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
     return st.finish();
@@ -648,11 +645,8 @@ int xcall_join_probe(mo_xcall_args_t *args, uint64_t len) {
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     mo_join_params_t P;
     if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "join probe: mo_join_params_t")) return rc;
-    const uint64_t cap = args[0].dataSz / 8;
     const uint64_t ngroups = args[4].dataSz / 8;
-    if (int rc = check_probe_type(args, P.join_type, ngroups, "join probe")) return rc;
-    if (args[1].dataSz / 8 < cap || !args[2].pdata || args[2].dataSz < 8 || args[7].dataSz < 8 * len) { set_error("join probe: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
-    if (args[5].pdata && args[5].dataSz < (ngroups + 2) * 4) { set_error("join probe: sels offsets shorter than the group count + 2"); return MO_RC_INVALID_ARGUMENT; }
+    if (int rc = check_probe_args(args, len, P.join_type, ngroups, "join probe")) return rc;
     Stager st(t);
     DevTable T;
     std::shared_lock<std::shared_mutex> lk;
@@ -660,10 +654,7 @@ int xcall_join_probe(mo_xcall_args_t *args, uint64_t len) {
     if (rc) { st.finish(); return rc; }
     const uint64_t *keys = (const uint64_t *)st.in(args[7].pdata, 8 * len);
     const uint64_t *kn = (const uint64_t *)st.in(args[7].pnulls, args[7].pnulls ? ((len + 63) / 64) * 8 : 0);
-    uint64_t *scal = (uint64_t *)st.tmp(kRecWords * 8);
-    if (st.failed) return MO_RC_INTERNAL_ERROR;
-    MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, kRecWords * 8, t.stream));
-    return run_probe(t, st, args, len, P.join_type, ngroups, KeyLookup{keys, kn, T.key, T.id, T.mask}, scal);
+    return run_probe(t, st, args, len, P.join_type, ngroups, [&](uint64_t *) { return KeyLookup{keys, kn, T.key, T.id, T.mask}; });
 }
 
 // MO_XCALL_JOIN_PROBE_GIDS: args [0..3], [5], [6] as JOIN_PROBE ; [4] int64 ngroups ; [7] vals uint64[len] (group ids, 0 = no match)
@@ -676,16 +667,10 @@ int xcall_join_probe_gids(mo_xcall_args_t *args, uint64_t len) {
     if (int rc = read_param(t, args[4], &ng, 8, 8, "join probe gids: [4] int64 ngroups")) return rc;
     if (ng < 0) { set_error("join probe gids: [4] must be an int64 ngroups >= 0"); return MO_RC_INVALID_ARGUMENT; }
     const uint64_t ngroups = (uint64_t)ng;
-    if (int rc = check_probe_type(args, P.join_type, ngroups, "join probe gids")) return rc;
-    const uint64_t cap = args[0].dataSz / 8;
-    if (args[1].dataSz / 8 < cap || !args[2].pdata || args[2].dataSz < 8 || args[7].dataSz < 8 * len) { set_error("join probe gids: buffers too small"); return MO_RC_INVALID_ARGUMENT; }
-    if (args[5].pdata && args[5].dataSz < (ngroups + 2) * 4) { set_error("join probe gids: sels offsets shorter than the group count + 2"); return MO_RC_INVALID_ARGUMENT; }
+    if (int rc = check_probe_args(args, len, P.join_type, ngroups, "join probe gids")) return rc;
     Stager st(t);
     const uint64_t *gids = (const uint64_t *)st.in(args[7].pdata, 8 * len);
-    uint64_t *scal = (uint64_t *)st.tmp(kRecWords * 8);
-    if (st.failed) return MO_RC_INTERNAL_ERROR;
-    MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, kRecWords * 8, t.stream));
-    return run_probe(t, st, args, len, P.join_type, ngroups, GidLookup{gids, ngroups, (unsigned *)(scal + 1)}, scal);
+    return run_probe(t, st, args, len, P.join_type, ngroups, [&](uint64_t *rec) { return GidLookup{gids, ngroups, (unsigned *)(rec + 1)}; });
 }
 
 // MO_XCALL_JOIN_MATCHED_MERGE: args [0] out bitmap uint64[(len + 63) / 64] ; [1] int32 n ; [2] mo_join_params_t ; [3 .. 3 + n) input bitmaps
@@ -697,7 +682,7 @@ int xcall_join_matched_merge(mo_xcall_args_t *args, uint64_t len) {
     if (int rc = read_param(t, args[1], &n, 4, 4, "join matched merge: [1] int32 n")) return rc;
     mo_join_params_t P;
     if (int rc = read_param(t, args[2], &P, sizeof P, sizeof P, "join matched merge: mo_join_params_t")) return rc;
-    if (P.join_type < MO_JOIN_RIGHT || P.join_type > MO_JOIN_RIGHT_SINGLE) { set_error("join matched merge: join type %d (a right-flavoured type, 5..9)", P.join_type); return MO_RC_INVALID_ARGUMENT; }
+    if (int rc = check_join_type(P.join_type, "join matched merge", true)) return rc;
     if (n < 1 || n > MO_JOIN_MERGE_MAX) { set_error("join matched merge: %d inputs (1..%d)", n, MO_JOIN_MERGE_MAX); return MO_RC_INVALID_ARGUMENT; }
     const uint64_t words = (len + 63) / 64;
     if (!args[0].pdata || args[0].dataSz < 8 * words) { set_error("join matched merge: the out bitmap holds fewer than %llu rows", (unsigned long long)len); return MO_RC_INVALID_ARGUMENT; }
@@ -734,7 +719,7 @@ int xcall_join_cond(mo_xcall_args_t *args, uint64_t len) {
     mo_join_params_t P;
     if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "join cond: mo_join_params_t")) return rc;
     const int jt = P.join_type;
-    if (jt < MO_JOIN_INNER || jt > MO_JOIN_RIGHT_SINGLE) { set_error("join cond: join type %d", jt); return MO_RC_INVALID_ARGUMENT; }
+    if (int rc = check_join_type(jt, "join cond", false)) return rc;
     if (jt >= MO_JOIN_RIGHT && !args[7].pdata) { set_error("join cond: join type %d needs the matched bitmap in args[7]", jt); return MO_RC_INVALID_ARGUMENT; }
     const uint64_t cap = args[0].dataSz / 8, npairs = args[4].dataSz / 8;
     if (args[1].dataSz / 8 < cap || !args[2].pdata || args[2].dataSz < 8 || args[5].dataSz < 8 * npairs || args[6].dataSz < npairs) {
@@ -743,57 +728,32 @@ int xcall_join_cond(mo_xcall_args_t *args, uint64_t len) {
     }
     const bool emits = jt != MO_JOIN_RIGHT_SEMI && jt != MO_JOIN_RIGHT_ANTI;
     Stager st(t);
-    int64_t *out_probe = (int64_t *)st.out(args[0].pdata, cap * 8);
-    int64_t *out_build = (int64_t *)st.out(args[1].pdata, cap * 8);
-    int64_t *count = (int64_t *)st.out(args[2].pdata, 8);
     const int64_t *cp = (const int64_t *)st.in(args[4].pdata, npairs * 8);
     const int64_t *cb = (const int64_t *)st.in(args[5].pdata, npairs * 8);
     const uint8_t *cond = (const uint8_t *)st.in(args[6].pdata, npairs);
     const uint64_t *cn = (const uint64_t *)st.in(args[6].pnulls, args[6].pnulls ? ((npairs + 63) / 64) * 8 : 0);
-    uint64_t *scal = (uint64_t *)st.tmp(kRecWords * 8);
-    Marks M;
-    if (jt >= MO_JOIN_RIGHT) {
-        const uint64_t words = args[7].dataSz / 8;
-        M.words = (unsigned long long *)st.out(args[7].pdata, words * 8, true);   // in/out: a host bitmap is uploaded and copied back
-        M.nbits = words * 64; M.single = jt == MO_JOIN_RIGHT_SINGLE;
-        M.twice = (unsigned long long *)(scal + 3); M.past = (unsigned long long *)(scal + 4);
-    }
     uint64_t *head = emits ? (uint64_t *)st.tmp(len * 8 + 8) : nullptr;
     uint64_t *end = emits ? (uint64_t *)st.tmp(len * 8 + 8) : nullptr;
     uint64_t *cnt = emits ? (uint64_t *)st.tmp(len * 8 + 8) : nullptr;
     if (st.failed) return MO_RC_INTERNAL_ERROR;
-    MOB_CUDA_TRY(cudaMemsetAsync(scal, 0, kRecWords * 8, t.stream));
     if (emits) {
         MOB_CUDA_TRY(cudaMemsetAsync(head, 0, len * 8, t.stream));
         MOB_CUDA_TRY(cudaMemsetAsync(end, 0, len * 8, t.stream));
         MOB_CUDA_TRY(cudaMemsetAsync(cnt, 0, len * 8, t.stream));
     }
-    cudaEventRecord(t.kev0, t.stream);
-    cond_pairs_kernel<<<grid_for(npairs ? npairs : 1), kThreads, 0, t.stream>>>(cp, cb, cond, cn, npairs, len, head, end, (unsigned long long *)cnt, M,
-                                                                                 (unsigned long long *)(scal + 1));
-    MOB_LAUNCH_CHECK();
-    if (emits) {
-        cond_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(len, cnt, jt, (unsigned long long *)(scal + 2));
+    return join_tail(t, st, args, 7, jt, len, cnt, CondRows{head, end, cb, cond, cn}, [&](const Marks &M, uint64_t *rec) {
+        cond_pairs_kernel<<<grid_for(npairs ? npairs : 1), kThreads, 0, t.stream>>>(cp, cb, cond, cn, npairs, len, head, end, (unsigned long long *)cnt, M,
+                                                                                     (unsigned long long *)(rec + 1));
         MOB_LAUNCH_CHECK();
-        int rc = exclusive_scan(t, cnt, len, cnt, scal);
-        if (rc) { st.finish(); return rc; }
-        const Marks EM = jt == MO_JOIN_RIGHT || jt == MO_JOIN_FULL || jt == MO_JOIN_RIGHT_SINGLE ? M : Marks();
-        cond_emit_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(len, head, end, cnt, scal, cb, cond, cn, jt, cap, out_probe, out_build, count, EM);
-    } else {
-        MOB_CUDA_TRY(cudaMemsetAsync(count, 0, 8, t.stream));   // right semi / right anti: marks only
-    }
-    cudaEventRecord(t.kev1, t.stream);
-    MOB_LAUNCH_CHECK();
-    uint64_t h[kRecWords] = {};
-    int rc = read_back(t, h, scal, sizeof h);
-    int frc = st.finish();
-    if (rc) return rc;
-    if (h[1]) { set_error("join cond: candidate %llu is malformed: its probe row lies outside [0, %llu) or below the one before it, or its build row is negative", (unsigned long long)~h[1], (unsigned long long)len); return MO_RC_INVALID_ARGUMENT; }
-    if (h[4]) { set_error("join cond: build row %llu lies past the matched bitmap (%llu rows)", (unsigned long long)~h[4], (unsigned long long)M.nbits); return MO_RC_INVALID_ARGUMENT; }
-    if (h[2]) { set_error("scalar subquery returns more than 1 row (probe row %llu)", (unsigned long long)~h[2]); return MO_RC_INTERNAL_ERROR; }
-    if (h[3]) { set_error("scalar subquery returns more than 1 row (build row %llu)", (unsigned long long)~h[3]); return MO_RC_INTERNAL_ERROR; }
-    if (h[0] > cap) { set_error("join cond: %lld result rows exceed the output capacity (%llu); the count is reported, call again with larger buffers", (long long)h[0], (unsigned long long)cap); return MO_RC_OUT_OF_RANGE; }
-    return frc;
+        if (emits) {
+            cond_count_kernel<<<grid_for(len ? len : 1), kThreads, 0, t.stream>>>(len, cnt, jt, (unsigned long long *)(rec + 2));
+            MOB_LAUNCH_CHECK();
+        }
+        return MO_RC_SUCCESS;
+    }, "join cond", [&](uint64_t w) {
+        set_error("join cond: candidate %llu is malformed: its probe row lies outside [0, %llu) or below the one before it, or its build row is negative",
+                  (unsigned long long)~w, (unsigned long long)len);
+    });
 }
 
 // MO_XCALL_STR_JOIN_FIND: args [0] vals uint64[len] ; [1] int64 ngroups ; [2] table bytes ; [3] table offsets uint64[ngroups + 1] ; [4] probe key
@@ -839,13 +799,10 @@ extern "C" int32_t MoB200_JoinMapPrepare(const void *table_keys, uint64_t ngroup
     const uint64_t *dkeys = (const uint64_t *)st.in(table_keys, ngroups * 8);
     if (st.failed) return MO_RC_INTERNAL_ERROR;
     DevTable T;
-    int rc = build_table(t, dkeys, ngroups, true, &T);
+    int rc = build_table(t, ngroups, dkeys, nullptr, nullptr, true, &T);
     int frc = st.finish();
     if (rc || frc) { if (!rc) free_table(T); return rc ? rc : frc; }
-    std::unique_lock<std::shared_mutex> lk(g_jm_mu);
-    auto it = g_jm.find(table_keys);
-    if (it != g_jm.end()) free_table(it->second);
-    g_jm[table_keys] = T;
+    publish_prepared(table_keys, T);
     return MO_RC_SUCCESS;
 }
 
@@ -870,7 +827,7 @@ extern "C" int32_t MoB200_StrJoinMapPrepare(const void *table_bytes, const void 
     int rc = MO_RC_SUCCESS;
     if (nbytes && cudaMemcpyAsync(db, table_bytes, nbytes, cudaMemcpyDefault, t.stream) != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
     if (!rc && cudaMemcpyAsync(doff, table_offsets, (ngroups + 1) * 8, cudaMemcpyDefault, t.stream) != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
-    if (!rc) rc = build_str_table(t, db, doff, ngroups, true, &T);
+    if (!rc) rc = build_table(t, ngroups, nullptr, db, doff, true, &T);
     if (!rc && cudaStreamSynchronize(t.stream) != cudaSuccess) rc = MO_RC_INTERNAL_ERROR;
     arena_reset(t);
     if (rc) {
@@ -879,10 +836,7 @@ extern "C" int32_t MoB200_StrJoinMapPrepare(const void *table_bytes, const void 
         cudaFree(db); cudaFree(doff);
         return rc;
     }
-    std::unique_lock<std::shared_mutex> lk(g_jm_mu);
-    auto it = g_jm.find(table_offsets);
-    if (it != g_jm.end()) free_table(it->second);
-    g_jm[table_offsets] = T;
+    publish_prepared(table_offsets, T);
     return MO_RC_SUCCESS;
 }
 

@@ -36,6 +36,10 @@ def go():
         lib.og_multi_logic.argtypes = [_i32, _vp, _vp, _i32, _vp, _vp, _vp, _u64]
         lib.og_filter_sels.restype = _i64
         lib.og_filter_sels.argtypes = [_vp, _vp, _u64, _vp]
+        lib.og_shuffle_fixed.restype = None
+        lib.og_shuffle_fixed.argtypes = [_vp, _vp, _vp, _i64, _i32]
+        lib.og_nulls_filter.restype = None
+        lib.og_nulls_filter.argtypes = [_vp, _u64, _vp, _i64, _vp]
         for sfx in ("f32", "f64"):
             getattr(lib, "og_km_init_bounds_" + sfx).restype = None
             getattr(lib, "og_km_init_bounds_" + sfx).argtypes = [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp]

@@ -6,7 +6,7 @@ import pytest
 
 import oracle_lib as O
 from matrixone_b200 import capi, ops
-from matrixone_b200.vector import bitmap_from_bools
+from matrixone_b200.vector import Vector, bitmap_from_bools, xcall
 
 pytestmark = pytest.mark.gpu
 
@@ -95,3 +95,31 @@ def test_empty_sides(gpu):
     p, b = jm2.probe(np.zeros(0, np.uint64), capi.JOIN_INNER)
     assert len(p) == 0
     jm2.release()
+
+
+def test_empty_table_without_a_pointer(gpu):
+    """an empty build side passed with no pointer (a Go nil slice, an empty tensor) is an empty 8-byte table, scratch or prepared: the all-ones
+    key, which has a slot of its own, matches nothing"""
+    keys = np.array([2**64 - 1, 0, 5], np.uint64)
+    prm = {jt: np.array([jt, 0], np.int32).view(np.uint8) for jt in (capi.JOIN_INNER, capi.JOIN_LEFT)}
+
+    def find():
+        vals = np.full(3, 7, np.uint64)
+        xcall(capi.XCALL_JOIN_FIND, [Vector(data=vals, length=3), Vector(length=0), Vector(data=keys, length=3)], 3)
+        return vals
+
+    def probe(jt):
+        op, ob, cnt = np.zeros(8, np.int64), np.zeros(8, np.int64), np.zeros(1, np.int64)
+        xcall(capi.XCALL_JOIN_PROBE, [Vector(data=op, length=8), Vector(data=ob, length=8), Vector(data=cnt, length=1), Vector(data=prm[jt], length=1),
+                                      Vector(length=0), Vector(length=0), Vector(length=0), Vector(data=keys, length=3)], 3)
+        return op[:cnt[0]], ob[:cnt[0]]
+
+    lib = capi.load_library()
+    for prepared in (False, True):
+        if prepared:
+            capi.check(lib.MoB200_JoinMapPrepare(None, 0), lib)
+        assert (find() == 0).all()
+        assert len(probe(capi.JOIN_INNER)[0]) == 0
+        p, b = probe(capi.JOIN_LEFT)
+        assert (p == [0, 1, 2]).all() and (b == -1).all()
+    lib.MoB200_JoinMapRelease(None)

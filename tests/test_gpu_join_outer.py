@@ -216,6 +216,10 @@ def test_bitmap_missing_short_or_past(gpu):
     with pytest.raises(capi.MoError, match="build row 298 lies past the matched bitmap"):
         jm.probe(np.array([149], np.uint64), capi.JOIN_RIGHT_SEMI, matched=np.zeros(4, np.uint64))
     jm.release()
+    matched = ops.matched_bitmap(2)                  # a group id above ngroups fails the call before it writes or marks anything
+    with pytest.raises(capi.MoError, match="exceeds the group count"):
+        ops.probe_gids(np.array([1, 2, 9], np.uint64), 2, None, None, capi.JOIN_RIGHT, matched=matched)
+    assert not matched.any()
 
 
 def test_device_pointers(gpu):

@@ -7,8 +7,8 @@
               INNER; RIGHT + JOIN_BUILD_ROWS; RIGHT SEMI (a probe that emits nothing) + JOIN_BUILD_ROWS
   probe_str   10^7 probe rows of 16-byte string keys in 10^6-row batches: STR_JOIN_FIND + JOIN_PROBE_GIDS, INNER against RIGHT + finalize
   shuffle     SHUFFLE(8) and SHUFFLE(24) over 10^8 random sels (a tenth of them -1 in the `null_sels` rows), with a destination bitmap
---parent-lib loads a second build of libmo_b200.so (another commit) and times its INNER probe and SHUFFLE (without -1 sels, which it does
-not define) on the same buffers, alternating with this build's.  Every probe call reads its result count back, as a caller must.
+--parent-lib loads a second build of libmo_b200.so (another commit) and times its probe arms (parent_*) and SHUFFLE (without -1 sels, which
+it does not define) on the same buffers, alternating with this build's.  Every probe call reads its result count back, as a caller must.
 Prints one JSON line per measurement and, first, the card and its power limit."""
 import argparse
 import ctypes as C
@@ -103,10 +103,11 @@ def bench_probe_int(libs, reps, emit):
                 call(lib, capi.XCALL_JOIN_BUILD_ROWS, [dv(sels, nbuild), dv(scnt), dv(matched), prm(jt)], nbuild)
         return run
 
-    arms = {"inner": probe(libs["this"], capi.JOIN_INNER), "right+finalize": probe(libs["this"], capi.JOIN_RIGHT),
-            "right_semi+finalize": probe(libs["this"], capi.JOIN_RIGHT_SEMI)}
-    if "parent" in libs:
-        arms["parent_inner"] = probe(libs["parent"], capi.JOIN_INNER)
+    arms = {}
+    for name, lib in libs.items():
+        pre = "" if name == "this" else name + "_"
+        arms.update({pre + "inner": probe(lib, capi.JOIN_INNER), pre + "right+finalize": probe(lib, capi.JOIN_RIGHT),
+                     pre + "right_semi+finalize": probe(lib, capi.JOIN_RIGHT_SEMI)})
     med, raw = alternate(arms, reps)
     rows = nbatches * batch
     for k, ms in med.items():
@@ -117,7 +118,6 @@ def bench_probe_int(libs, reps, emit):
 
 
 def bench_probe_str(libs, reps, emit):
-    lib = libs["this"]
     nbuild, batch, nbatches = 1_000_000, 1_000_000, 10
     r = np.random.default_rng(2)
     bkeys = r.permutation(2 * nbuild)[:nbuild]
@@ -133,9 +133,10 @@ def bench_probe_str(libs, reps, emit):
     matched = torch.zeros((nbuild + 63) // 64, dtype=torch.int64, device="cuda")
     sels, scnt = torch.empty(nbuild, dtype=torch.int64, device="cuda"), torch.zeros(1, dtype=torch.int64, device="cuda")
     ng = Vector(data=np.array([jm.ngroups], np.int64), length=1)
-    capi.check(lib.MoB200_StrJoinMapPrepare(C.c_void_p(dtb.data_ptr()), C.c_void_p(dto.data_ptr()), jm.ngroups), lib)
+    for lib in libs.values():
+        capi.check(lib.MoB200_StrJoinMapPrepare(C.c_void_p(dtb.data_ptr()), C.c_void_p(dto.data_ptr()), jm.ngroups), lib)
 
-    def probe(jt):
+    def probe(lib, jt):
         def run():
             if jt >= capi.JOIN_RIGHT:
                 matched.zero_()
@@ -147,11 +148,16 @@ def bench_probe_str(libs, reps, emit):
                 call(lib, capi.XCALL_JOIN_BUILD_ROWS, [dv(sels, nbuild), dv(scnt), dv(matched), prm(jt)], nbuild)
         return run
 
-    med, raw = alternate({"inner": probe(capi.JOIN_INNER), "right+finalize": probe(capi.JOIN_RIGHT)}, reps)
+    arms = {}
+    for name, lib in libs.items():
+        pre = "" if name == "this" else name + "_"
+        arms.update({pre + "inner": probe(lib, capi.JOIN_INNER), pre + "right+finalize": probe(lib, capi.JOIN_RIGHT)})
+    med, raw = alternate(arms, reps)
     for k, ms in med.items():
         emit({"bench": "probe_str16", "arm": k, "build_rows": nbuild, "probe_rows": nbatches * batch, "ms": round(ms, 3),
               "probe_rows_per_s": nbatches * batch / (ms / 1e3), "runs_ms": raw[k]})
-    lib.MoB200_JoinMapRelease(C.c_void_p(dto.data_ptr()))
+    for lib in libs.values():
+        lib.MoB200_JoinMapRelease(C.c_void_p(dto.data_ptr()))
     jm.release()
 
 
