@@ -231,6 +231,27 @@ typedef struct { int32_t div0_null; int32_t reserved; int64_t err_row; } mo_go_p
 #define MO_XCALL_GO_BETWEEN(T) (0x5000 + (T))
 #define MO_XCALL_GO_MULTI_AND 0x5100
 #define MO_XCALL_GO_MULTI_OR 0x5101
+/* ---- string predicates (csrc/strpred.cu), the GO conventions above.  Operands are what Vector.FillRawPtrLen gives: pdata = 24-byte cells
+ * (dataSz = 24 * len; dataSz == 24 with len != 1 is a const operand), parea / areaSz = the area, pnulls = the nulls (a const operand: bit 0).
+ *   COMPARE(op, T) for T = CHAR, VARCHAR, BINARY, VARBINARY, BLOB, TEXT, DATALINK (func_compare.go:224-226,353-360,744-748,871-875,1125-1129,
+ *                  1252-1256): == / != are bytes.Equal, > >= < <= bytes.Compare -- unsigned bytes, a proper prefix first, zero bytes count, no
+ *                  trimming or collation.  Args as COMPARE.  JSON and the vector types stay refused.
+ *   GO_LIKE        likeFn (func_builtin_regexp.go:51-69).  args: [0] result bool[len] + pnulls (in/out) ; [1] the string ; [2] the pattern.
+ *                  A const NULL pattern nulls every row.  A const pattern that optimizeRuleForLike (:91-280) takes is matched by its byte-level
+ *                  rule: empty; `%`; `_` (one BYTE); one literal byte; exact / `_lit` / `%lit` / `lit_` / `lit%` / `%lit%` / `%lit_` / `_lit%` with
+ *                  no `_` or `%` inside (escapes removed by RemoveEscapeChar, which keeps a trailing lone backslash; `\` as the next-to-last byte
+ *                  makes the last byte a literal, so `\%` is a prefix match on a backslash); and `%a%b%...%` without `_` or `\%` (ordered
+ *                  bytes.Index of the pieces, escapes kept as bytes).  Any other pattern, and every column pattern (len == 1: the pattern is a
+ *                  column), is regularMatchForLikeOp (:618-672), ^(?s:...)$ over RUNES decoded by utf8.DecodeRune (an invalid, overlong or
+ *                  surrogate sequence is (U+FFFD, 1)): `_` one rune, `%` any run of runes, `\x` the literal rune x, a trailing `\` a literal
+ *                  backslash; an invalid pattern byte is a literal U+FFFD, which matches U+FFFD and any invalid subject byte.
+ *                  NOT LIKE is Logic_VecNot of the result.
+ * Both: values of any length.  Rows whose result null bit is set on entry are skipped; on return the bitmap holds rnulls | n1 | n2.  Cells of
+ * NULL and skipped rows are never read.  A non-inline cell that points outside [0, areaSz), or any when there is no area, fails the call with
+ * MO_RC_INVALID_ARGUMENT naming the operand and its lowest such row.  Device cells, areas, nulls and result: the call enqueues one kernel and
+ * reads back one small status record (the bad-cell check), which synchronises the calling thread's stream once; a const pattern is read on
+ * the host before that (a device one is copied back first, as a device parameter block is). */
+#define MO_XCALL_GO_LIKE 0x5800
 
 /* ---- the standalone column operators of the colexec pipeline (csrc/colops.cu).  Host or device pointers; when every data pointer and
  * nulls bitmap of every vector is a device pointer (or NULL) FILTER_SELS and SHUFFLE only enqueue work (asynchronous form, as

@@ -124,6 +124,9 @@ int read_param(ThreadCtx &t, const mo_xcall_args_t &a, void *dst, size_t min, si
 
 int write_param(ThreadCtx &t, void *dst, const void *src, size_t bytes);
 
+// comparison operators: the op of MO_XCALL_GO_COMPARE(op, T) and the order of the Numeric_Vec* entry points
+enum { CMP_EQ = 0, CMP_NE, CMP_GT, CMP_GE, CMP_LT, CMP_LE };
+
 // element width in bytes of a fixed-width MO_T_* type, 0 for any other type
 inline int type_size(int T) {
     switch (T) {

@@ -21,7 +21,6 @@ constexpr int LEFT_IS_SCALAR = 1, RIGHT_IS_SCALAR = 2;  // cgo/mo_impl.h:37-38
 constexpr unsigned ST_OVERFLOW = 1u, ST_DIVZERO = 2u;
 
 enum { AR_ADD = 0, AR_SUB, AR_MUL, AR_DIV, AR_MOD, AR_INTDIV };
-enum { CMP_EQ = 0, CMP_NE, CMP_GT, CMP_GE, CMP_LT, CMP_LE };
 
 template <int BYTES> __device__ __forceinline__ void store_bytes(void *dst, const void *src) {
     if (BYTES == 1) *(uint8_t *)dst = *(const uint8_t *)src;

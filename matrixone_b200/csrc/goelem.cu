@@ -28,7 +28,6 @@ namespace {
 
 constexpr int kThreads = 256;
 enum { OP_ADD = 0, OP_SUB, OP_MUL, OP_DIV, OP_MOD };
-enum { CMP_EQ = 0, CMP_NE, CMP_GT, CMP_GE, CMP_LT, CMP_LE };
 constexpr unsigned long long kNoRow = ~0ull;
 
 // ---- overflow-checked scalar arithmetic (arithmetic_overflow_check.go): returns true when the row must fail -----------------
@@ -409,6 +408,8 @@ int run_go_multi_logic(ThreadCtx &t, int is_or, mo_xcall_args_t *args, uint64_t 
 
 namespace mob {
 
+int go_str_compare(ThreadCtx &t, int op, mo_xcall_args_t *args, uint64_t len);
+
 int xcall_go_elementwise(int64_t funcId, mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
@@ -444,6 +445,8 @@ int xcall_go_elementwise(int64_t funcId, mo_xcall_args_t *args, uint64_t len) {
         case MO_T_UINT64: return run_go_compare<uint64_t>(t, op, args, len);
         case MO_T_FLOAT32: return run_go_compare<float>(t, op, args, len);
         case MO_T_FLOAT64: return run_go_compare<double>(t, op, args, len);
+        case MO_T_CHAR: case MO_T_VARCHAR: case MO_T_BINARY: case MO_T_VARBINARY: case MO_T_BLOB: case MO_T_TEXT: case MO_T_DATALINK:
+            return go_str_compare(t, op, args, len);   // strpred.cu
         }
         set_error("go compare: unsupported type %d", T);
         return MO_RC_INVALID_ARGUMENT;

@@ -15,7 +15,7 @@ import ctypes as C
 import numpy as np
 
 from . import capi
-from .vector import DeviceBuffer, Vector, varlena_bytes_column, xcall
+from .vector import DeviceBuffer, Vector, bitmap_to_bools, varlena_bytes_column, xcall
 
 
 def _vec(x, length=None, itemsize=None):
@@ -1264,3 +1264,67 @@ def vector_unmarshal_device(src_dev, nbytes, data_dev, area_dev, nulls_dev):
             Vector(data_ptr=src_dev.ptr, data_nbytes=nbytes, length=1)]
     xcall(capi.XCALL_VECTOR_UNMARSHAL, vecs, 1)
     return VectorView.from_buffer_copy(view.tobytes())
+
+
+# ------------------------------------------------------------------------------------------------ string predicates (csrc/strpred.cu)
+def _str_operand(x, nulls):
+    """a list of bytes (one element = a const operand) or a (cells, area) pair in the vector layout -> Vector"""
+    if isinstance(x, list):
+        x = varlena_bytes_column(x)
+    cells = np.ascontiguousarray(x[0], dtype=np.uint8).reshape(-1)
+    area = None if x[1] is None else np.ascontiguousarray(x[1], dtype=np.uint8)
+    return Vector(data=cells, nulls=nulls, area=area, length=cells.shape[0] // 24)
+
+
+def _str_pred(fid, a, b, a_nulls, b_nulls, rnulls, length):
+    va, vb = _str_operand(a, a_nulls), _str_operand(b, b_nulls)
+    n = length if length is not None else max(va.length, vb.length)
+    r = np.zeros(max(n, 1), dtype=np.uint8)
+    rn = np.zeros(max((n + 63) // 64, 1), dtype=np.uint64) if rnulls is None else np.array(rnulls, dtype=np.uint64)
+    xcall(fid, [Vector(data=r[:n], nulls=rn, length=n), va, vb], n)
+    return r[:n].astype(bool), bitmap_to_bools(rn, n)
+
+
+def str_compare(op, T, a, b, a_nulls=None, b_nulls=None, rnulls=None, length=None):
+    """a <op> b over varlena operands (T = capi.T_CHAR / T_VARCHAR / T_TEXT / ...): = and != are bytes.Equal, the orderings bytes.Compare.
+    a, b: a list of bytes (one element = const) or a (cells, area) pair; *_nulls: bitmap words; rnulls: the result bitmap on entry (rows set
+    there are skipped).  Returns (values bool[n], nulls bool[n])."""
+    return _str_pred(capi.XCALL_GO_COMPARE(op, T), a, b, a_nulls, b_nulls, rnulls, length)
+
+
+def like(col, pattern, col_nulls=None, pattern_nulls=None, rnulls=None, length=None):
+    """col LIKE pattern (likeFn): pattern is bytes (a const pattern), a list of bytes or a (cells, area) pair.  NOT LIKE is the negation of
+    the values with the same nulls.  Returns (values bool[n], nulls bool[n])."""
+    if isinstance(pattern, (bytes, bytearray)):
+        pattern = [bytes(pattern)]
+    return _str_pred(capi.XCALL_GO_LIKE, col, pattern, col_nulls, pattern_nulls, rnulls, length)
+
+
+def _str_device_vec(x, nulls, n):
+    cells, area = x if isinstance(x, tuple) else (x, None)
+    return Vector(data_ptr=cells.ptr, data_nbytes=cells.nbytes, nulls_ptr=nulls.ptr if nulls is not None else None, length=n,
+                  area_ptr=area.ptr if area is not None else None, area_nbytes=area.nbytes if area is not None else 0)
+
+
+def _str_pred_device(fid, a, b, n, out_dev, out_nulls_dev, a_nulls, b_nulls):
+    xcall(fid, [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n),
+                _str_device_vec(a, a_nulls, n), _str_device_vec(b, b_nulls, n)], n)
+
+
+def str_compare_device(op, T, a, b, n, out_dev, out_nulls_dev, a_nulls=None, b_nulls=None):
+    """the form on resident vectors: a, b are (cells, area) DeviceBuffer pairs (area None: every value inline; 24 bytes of cells = const);
+    out_dev (bool[n]) and out_nulls_dev (its bitmap, in/out) are DeviceBuffers.  Enqueues one kernel and reads back one status record."""
+    _str_pred_device(capi.XCALL_GO_COMPARE(op, T), a, b, n, out_dev, out_nulls_dev, a_nulls, b_nulls)
+
+
+def like_device(col, pattern, n, out_dev, out_nulls_dev, col_nulls=None, pattern_nulls=None):
+    """LIKE on resident vectors, as str_compare_device; the pattern is a (cells, area) pair of DeviceBuffers or of host arrays (a const
+    pattern read on the host)."""
+    if isinstance(pattern, (bytes, bytearray)):
+        pattern = varlena_bytes_column([bytes(pattern)])
+    if isinstance(pattern[0], np.ndarray):
+        pv = _str_operand(pattern, pattern_nulls)
+    else:
+        pv = _str_device_vec(pattern, pattern_nulls, n)
+    xcall(capi.XCALL_GO_LIKE, [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n),
+                               _str_device_vec(col, col_nulls, n), pv], n)
