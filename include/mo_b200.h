@@ -221,7 +221,15 @@ typedef struct mo_agg_state_t { uint64_t bits; int64_t count; int64_t rc; } mo_a
  *                                                        null input -> result false AND null bit set
  *   MULTI_AND / MULTI_OR                                 args: [0] result bool[len] + pnulls (out)  [1] int32 operand count n (<= 16)
  *                                                              [2 .. 2 + n) bool operands (+ pnulls); const = 1 byte
- * T = types.T id (MO_T_*); DATE compares as int32, TIME / DATETIME / TIMESTAMP as int64. */
+ * T = types.T id (MO_T_*); DATE compares as int32, TIME / DATETIME / TIMESTAMP as int64.
+ *   COMPARE(op, DECIMAL64 | DECIMAL128)  valueDecimalCompare (func_compare.go:426-667), csrc/decimal.cu.  Args as COMPARE plus [3] mo_dec_params_t
+ *                  {scale1 of a, scale2 of b} (required; 0..18 for DECIMAL64, 0..38 for DECIMAL128, else MO_RC_INVALID_ARGUMENT).  The side with the
+ *                  lower scale is scaled up by the difference (Decimal64.Scale / Decimal128.Scale), then the values compare signed.  The Go wrapper
+ *                  drops Scale's error: a scale-up that overflows compares the value unscaled, and a Decimal64 scale-up between 2^63 and 2^64
+ *                  wraps (unsigned Mul64, sign restored).  Never fails on data; all-device operands give an enqueue-only call (a const
+ *                  operand's null word is read on the device).
+ *   BETWEEN(DECIMAL64 | DECIMAL128)      CompareDecimal64 / 128 (operator_between.go:68-73): a raw signed compare, the bounds already at the
+ *                  column's scale (8- / 16-byte bounds, host or device). */
 typedef struct { int32_t div0_null; int32_t reserved; int64_t err_row; } mo_go_params_t;   /* err_row: out, -1 = no error */
 #define MO_XCALL_GO_ARITH(op, T) (0x4000 + ((op) << 8) + (T))
 #define MO_XCALL_GO_COMPARE(op, T) (0x4800 + ((op) << 8) + (T))
@@ -472,10 +480,26 @@ typedef struct mo_order_params_t {
  *   DEC_SUM(width)        SUM / AVG accumulation of a decimal column into Decimal128 sums + int64 counts per group (count 0 = NULL; AVG divides at
  *                         Flush), sumDecimal64FastExec / sumDecimal128FastExec.batchFill, pkg/sql/colexec/aggexec/sum_decimal_fast.go -- exact and
  *                         order independent.  args: [0] sums Decimal128 per group (in/out) ; [1] counts int64 per group (in/out) ;
- *                         [2] groups uint64[len] (1-based, 0 = skip) or pdata NULL for one group ; [3] the column (+pnulls) */
+ *                         [2] groups uint64[len] (1-based, 0 = skip) or pdata NULL for one group ; [3] the column (+pnulls)
+ *   DEC_ARITH(3, width)   / : d64Div / d128Div (arith_decimal_fast.go:734-1055, 4096-4320), equal to Decimal128.Div (decimal.go:1403-1446).
+ *                         Result Decimal128 for both widths, scale = min(12, scale1 + 6) raised to at least scale1; the dividend is scaled by
+ *                         10^(scale - scale1 + scale2) and divided with round half up (Div128; a divisor of 2^64 or more takes Div128's estimate,
+ *                         whose signed Less rounds an odd estimate down once the scaled dividend reaches 2^126; past 127 bits the Decimal256
+ *                         Div256 fallback).  Params mo_dec_div_params_t (a 16-byte mo_dec_params_t means div0_error = 0).  A zero divisor makes
+ *                         the row NULL, or with div0_error fails the call with MO_RC_DIVISION_BY_ZERO "division by zero"; a quotient past
+ *                         127 bits fails with MO_RC_INVALID_ARGUMENT "Decimal128 Div overflow".  The first failing row in row order, of either
+ *                         kind, wins and goes to err_row; rows before it hold their results.  A const zero divisor fails at row 0 (or nulls every
+ *                         row) whatever the row nulls, as the Go loop checks it before any row.
+ *   DEC_AVG(width)        AVG's Flush over DEC_SUM's state: decAvg (aggexec/sumavg2.go:545-559) = Decimal128.Div(sum, count) with its error
+ *                         dropped (the value Div keeps is written).  Result scale AvgReturnType: max(12, scale) capped at scale + 6.  args: [0] result
+ *                         Decimal128 per group + pnulls (out: count 0 = NULL, the value is then the sum) ; [1] sums ; [2] counts ; [3] mo_dec_params_t
+ *                         with scale1 = the argument's scale (0..18 / 0..38; the rest is not read).  len = the group count.  Never fails on data;
+ *                         all-device arguments give an enqueue-only call. */
 typedef struct mo_dec_params_t { int32_t scale1, scale2; int64_t err_row; } mo_dec_params_t;
+typedef struct mo_dec_div_params_t { int32_t scale1, scale2; int64_t err_row; int32_t div0_error, reserved; } mo_dec_div_params_t;
 #define MO_XCALL_DEC_ARITH(op, width) (0x7000 + ((op) << 8) + (width))
 #define MO_XCALL_DEC_SUM(width) (0x7400 + (width))
+#define MO_XCALL_DEC_AVG(width) (0x7500 + (width))
 
 /* ---- the generic fused operator: scan -> filter -> project -> (hash) group -> aggregate in ONE pass over the columns (csrc/plan.cu).
  * What the colexec pipeline runs per block as table_scan -> filter -> projection -> group (filter.go:87-153, evalExpression.go:575-640,

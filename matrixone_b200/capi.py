@@ -302,5 +302,16 @@ def XCALL_DEC_SUM(width):
     return 0x7400 + width
 
 
+def XCALL_DEC_AVG(width):
+    return 0x7500 + width
+
+
+DEC_OP_DIV = 3
+
+
 class DecParams(C.Structure):
     _fields_ = [("scale1", C.c_int32), ("scale2", C.c_int32), ("err_row", C.c_int64)]
+
+
+class DecDivParams(C.Structure):
+    _fields_ = [("scale1", C.c_int32), ("scale2", C.c_int32), ("err_row", C.c_int64), ("div0_error", C.c_int32), ("reserved", C.c_int32)]

@@ -3,6 +3,9 @@
 //
 //   MO_XCALL_DEC_ARITH(op, width)   d64Add / d64Sub / d64Mul / d128Add / d128Sub / d128Mul, pkg/sql/plan/function/arith_decimal_fast.go
 //   MO_XCALL_DEC_SUM(width)         sumDecimal64FastExec / sumDecimal128FastExec.batchFill, pkg/sql/colexec/aggexec/sum_decimal_fast.go
+//   MO_XCALL_DEC_ARITH(3, width)    d64Div / d128Div (arith_decimal_fast.go:734-1055, 4096-4320) = Decimal128.Div, result Decimal128
+//   MO_XCALL_DEC_AVG(width)         decAvg over DEC_SUM's state, pkg/sql/colexec/aggexec/sumavg2.go:545-559
+//   MO_XCALL_GO_COMPARE(op, DECIMAL64 | DECIMAL128)   valueDecimalCompare, pkg/sql/plan/function/func_compare.go:426-667
 //
 // Pure integer work, bit-exact: Decimal64 = int64 unscaled value, Decimal128 = two's-complement {B0_63, B64_127}; the scales travel in
 // the parameter block.  Conventions are those of the Go elementwise engine (goelem.cu): result nulls pre-filled by the caller
@@ -64,16 +67,214 @@ __device__ __forceinline__ void mag_div_pow10(uint64_t m[4], int k) {
     mag_div_once(m, kPow10[19]); mag_div_once(m, kPow10[k - 19]);
 }
 
-struct DecParams { int32_t scale1, scale2; int64_t err_row; };
+// ---- decimal division, restated limb by limb from the Go code (pkg/container/types/decimal.go, arith_decimal_fast.go) ----------------------
+// Only the signed comparisons and the sign-aware right shifts of the Go types are signed; every add, subtract and left shift wraps.
+__device__ __forceinline__ uint64_t shl64(uint64_t x, int s) { return s >= 64 ? 0 : x << s; }   // Go: a shift by >= 64 gives 0
+__device__ __forceinline__ uint64_t shr64(uint64_t x, int s) { return s >= 64 ? 0 : x >> s; }
+__device__ __forceinline__ u128 d128_minus(u128 x) { return (u128)0 - x; }                  // Decimal128.Minus: two's complement
+// Decimal128.Right (:297-313): the magnitude is shifted and the sign restored
+__device__ __forceinline__ u128 d128_right(u128 x, int n) {
+    const bool sign = (uint64_t)(x >> 64) >> 63;
+    if (sign) x = d128_minus(x);
+    const uint64_t lo = (uint64_t)x, hi = (uint64_t)(x >> 64);
+    uint64_t ylo, yhi;
+    if (n > 64) { yhi = 0; ylo = shr64(hi, n - 64); }
+    else { yhi = shr64(hi, n); ylo = shr64(lo, n) | shl64(hi, 64 - n); }
+    const u128 y = ((u128)yhi << 64) | ylo;
+    return sign ? d128_minus(y) : y;
+}
+// Decimal128.Mul128 (:841-861) for y < 2^64, as Div128 calls it on a divisor x >= 2^64: on overflow it returns the partial product
+__device__ __forceinline__ u128 d128_mul128_go(u128 x, uint64_t y) {
+    const uint64_t xlo = (uint64_t)x, xhi = (uint64_t)(x >> 64);
+    u128 z = (u128)xlo * y;
+    const u128 w = (u128)xhi * y;                                                // x.B64_127 == 0: Mul64(x.B0_63, y.B64_127 = 0) = 0
+    const uint64_t w_b0 = (uint64_t)(w >> 64), w_b64 = (uint64_t)w;              // w.B0_63, w.B64_127 = bits.Mul64(...): hi, lo
+    if (w_b0 != 0 || (w_b64 >> 63) || ((uint64_t)(z >> 64) >> 63)) return z;
+    z += (u128)w_b64 << 64;
+    return z;
+}
+// Decimal128.Div128 (:982-1017) on a non-negative dividend: round half up for a 64-bit divisor; above that the quotient is estimated from
+// the divisor's top 64 bits and rounded by the signed Less of x.Left(1), which wraps negative for x >= 2^126
+__device__ __forceinline__ u128 d128_div128_go(u128 x, u128 y) {
+    const uint64_t yhi = (uint64_t)(y >> 64);
+    if (yhi == 0) {
+        const uint64_t d = (uint64_t)y;
+        const uint64_t qh = (uint64_t)(x >> 64) / d, r1 = (uint64_t)(x >> 64) % d;
+        const u128 cur = ((u128)r1 << 64) | (uint64_t)x;
+        const uint64_t ql = (uint64_t)(cur / d), rem = (uint64_t)(cur % d);
+        u128 q = ((u128)qh << 64) | ql;
+        if (rem * 2 >= d || (rem >> 63)) q += 1;
+        return q;
+    }
+    if ((i128)x < (i128)y) return 0;
+    const int n = __clzll((long long)yhi);
+    const uint64_t d = (uint64_t)d128_right(y, 64 - n);
+    uint64_t v = (uint64_t)(x / d);                                              // bits.Div64(x.hi, x.lo, d): x.hi < 2^63 <= d
+    v >>= 63 - n;
+    if ((v & 1) == 0) return v >> 1;
+    const u128 z = d128_mul128_go(y, v);
+    return (i128)(x << 1) < (i128)z ? (u128)(v >> 1) : (u128)((v >> 1) + 1);
+}
+
+struct U256 { uint64_t w[4]; };   // Decimal256 {B0_63, B64_127, B128_191, B192_255}
+__device__ __forceinline__ bool u256_zero(const U256 &x) { return (x.w[0] | x.w[1] | x.w[2] | x.w[3]) == 0; }
+__device__ __forceinline__ U256 u256_minus(U256 x) {
+    U256 y; uint64_t c = 1;
+#pragma unroll
+    for (int k = 0; k < 4; k++) { y.w[k] = ~x.w[k] + c; c = (c && y.w[k] == 0) ? 1 : 0; }
+    return y;
+}
+__device__ __forceinline__ U256 u256_add(const U256 &x, const U256 &y) {
+    U256 z; uint64_t c = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++) { const uint64_t s = x.w[k] + y.w[k]; const uint64_t s2 = s + c; c = (s < x.w[k]) || (s2 < s); z.w[k] = s2; }
+    return z;
+}
+__device__ __forceinline__ U256 u256_left1(const U256 &x) {
+    U256 y; y.w[0] = x.w[0] << 1;
+#pragma unroll
+    for (int k = 1; k < 4; k++) y.w[k] = (x.w[k] << 1) | (x.w[k - 1] >> 63);
+    return y;
+}
+// Decimal256.Right(1) (:330-350): sign-aware
+__device__ __forceinline__ U256 u256_right1(U256 x) {
+    const bool sign = x.w[3] >> 63;
+    if (sign) x = u256_minus(x);
+    U256 y;
+#pragma unroll
+    for (int k = 0; k < 3; k++) y.w[k] = (x.w[k] >> 1) | (x.w[k + 1] << 63);
+    y.w[3] = x.w[3] >> 1;
+    return sign ? u256_minus(y) : y;
+}
+// Decimal256.Less: signed
+__device__ __forceinline__ bool u256_less(const U256 &x, const U256 &y) {
+    if ((x.w[3] >> 63) != (y.w[3] >> 63)) return x.w[3] >> 63;
+    for (int k = 3; k >= 0; k--) if (x.w[k] != y.w[k]) return x.w[k] < y.w[k];
+    return false;
+}
+// d256Mul1Limb (arith_decimal_fast.go:1735-1746): false when the product leaves 255 bits
+__device__ __forceinline__ bool u256_mul1(U256 &x, uint64_t p) {
+    uint64_t h[4], l[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) { l[k] = x.w[k] * p; h[k] = __umul64hi(x.w[k], p); }
+    x.w[0] = l[0];
+    uint64_t c = 0;
+#pragma unroll
+    for (int k = 1; k < 4; k++) { const uint64_t s = l[k] + h[k - 1]; const uint64_t s2 = s + c; c = (s < l[k]) || (s2 < s); x.w[k] = s2; }
+    return (h[3] | c | (x.w[3] >> 63)) == 0;
+}
+enum { DIV_OK = 0, DIV_OVERFLOW = 1, DIV_SCALE_OVERFLOW = 2, DIV_NO_END = 3 };
+// Decimal256.Div256 (:1041-1081) of a non-negative x by 0 < y < 2^128.  The long division compares signed: a dividend with bit 254 set
+// (bit 255 after the first doubling) gives 0, and when the divisor is shifted out to zero the Go loop never ends (DIV_NO_END).
+__device__ int u256_div256_go(U256 x, U256 y, U256 &z) {
+    x = u256_left1(x);
+    z = U256{{0, 0, 0, 0}};
+    if ((y.w[1] | y.w[2] | y.w[3]) == 0) {
+        const uint64_t d = y.w[0];
+        uint64_t rem = 0;
+        for (int k = 3; k >= 0; k--) { const u128 cur = ((u128)rem << 64) | x.w[k]; z.w[k] = (uint64_t)(cur / d); rem = (uint64_t)(cur % d); }
+    } else {
+        U256 w{{1, 0, 0, 0}};
+        while (!u256_less(x, y)) {                                               // y.Compare(x) <= 0
+            y = u256_left1(y); w = u256_left1(w);
+            if (u256_zero(y)) return DIV_NO_END;
+        }
+        while (!u256_zero(y)) {
+            y = u256_right1(y); w = u256_right1(w);
+            if (!u256_less(x, y)) { z = u256_add(z, w); x = u256_add(x, u256_minus(y)); }
+        }
+    }
+    const bool odd = z.w[0] & 1;
+    z = u256_right1(z);
+    if (odd) z = u256_add(z, U256{{1, 0, 0, 0}});
+    return DIV_OK;
+}
+
+// x / y at scale adjustment adj = resultScale - scale1 + scale2 (>= 0), y != 0: d128DivOne (arith_decimal_fast.go:970-1012), which the
+// inline 64-bit path d128DivInline equals wherever it applies, and Decimal128.Div (decimal.go:1403-1446) for AVG.  DIV_OVERFLOW leaves in z
+// the value Decimal128.Div keeps (the quotient's low 128 bits, signed); DIV_SCALE_OVERFLOW leaves |x|.
+__device__ int dec_div(i128 xs, i128 ys, int adj, i128 &out) {
+    const bool neg = (xs < 0) != (ys < 0);
+    const u128 x = xs < 0 ? d128_minus((u128)xs) : (u128)xs, y = ys < 0 ? d128_minus((u128)ys) : (u128)ys;   // d128Abs: |MIN| stays 2^127
+    // d128MulPow10 (:431-439): |x| * 10^adj < 2^127, in at most two limbs of 10^19
+    bool fits = adj <= 38;
+    u128 z = x;
+    if (fits) {
+        int rest = adj;
+        do {
+            const int k = rest > 19 ? 19 : rest; rest -= k;
+            const uint64_t p = kPow10[k], lo = (uint64_t)z, hi = (uint64_t)(z >> 64);
+            uint64_t zh = __umul64hi(lo, p);
+            if (hi) { const uint64_t ch = __umul64hi(hi, p), cl = hi * p; const uint64_t s = zh + cl; if (ch | (s < zh) | (s >> 63)) { fits = false; break; } zh = s; }
+            else if (zh >> 63) { fits = false; break; }
+            z = ((u128)zh << 64) | (lo * p);
+        } while (rest > 0);
+    }
+    if (fits) {
+        z = d128_div128_go(z, y);
+        out = (i128)(neg ? d128_minus(z) : z);
+        return DIV_OK;
+    }
+    U256 x2{{(uint64_t)x, (uint64_t)(x >> 64), 0, 0}}, y2{{(uint64_t)y, (uint64_t)(y >> 64), 0, 0}}, q;
+    for (int rest = adj; ;) {                                                    // d256MulPow10 (:1750-1758)
+        const int k = rest > 19 ? 19 : rest; rest -= k;
+        if (!u256_mul1(x2, kPow10[k])) { out = (i128)x; return DIV_SCALE_OVERFLOW; }
+        if (rest <= 0) break;
+    }
+    const int rc = u256_div256_go(x2, y2, q);
+    z = ((u128)q.w[1] << 64) | q.w[0];
+    out = (i128)(neg ? d128_minus(z) : z);
+    if (rc != DIV_OK) return rc;
+    return (q.w[3] | q.w[2] | (q.w[1] >> 63)) ? DIV_OVERFLOW : DIV_OK;
+}
+
+// Decimal64.Scale / Decimal128.Scale (decimal.go:352-392, 438-480) up by d as the compare wrapper calls them: the error is dropped and the
+// value comes back unscaled.  Decimal64 scales |x| by an unsigned Mul64 (no error below 2^64) and restores the sign, so it can wrap.
+__device__ __forceinline__ int64_t d64_scale_cmp(int64_t x, int d) {
+    if (d == 0 || x == 0) return x;
+    const uint64_t sign = (uint64_t)x >> 63, ab = sign ? 0ull - (uint64_t)x : (uint64_t)x;
+    if (__umul64hi(ab, kPow10[d])) return x;
+    const uint64_t z = ab * kPow10[d];
+    return (int64_t)(sign ? 0ull - z : z);
+}
+__device__ __forceinline__ i128 d128_scale_cmp(i128 x, int d) {
+    if (d == 0) return x;
+    i128 v = x;
+    if (d > 19) { if (!d128_scale_up(v, 19)) return x; d -= 19; }
+    return d128_scale_up(v, d) ? v : x;
+}
+
+// the scale of a quotient and of an AVG: min(12, scale1 + 6), raised to at least scale1 (Decimal128.Div, AvgReturnType)
+inline int div_scale(int s1) { int s = 12; if (s > s1 + 6) s = s1 + 6; if (s < s1) s = s1; return s; }
+template <int W> constexpr int kMaxScale() { return W == 64 ? 18 : 38; }
+
+struct DecParams { int32_t scale1, scale2; int64_t err_row; int32_t div0_error, reserved; };   // div0_error: DIV only
+constexpr size_t kDecParamsV1 = 16;   // {scale1, scale2, err_row}: what + - * read and every op writes back
 
 __device__ __forceinline__ bool row_null(const uint64_t *rnulls, uint64_t i) { return (rnulls[i >> 6] >> (i & 63)) & 1ull; }
 
-// OP: 0 add, 1 sub, 2 mul.  W: 64 or 128 (operand width).  d64 mul produces d128.
+// first_bad holds 2 * row + kind (kind 1 = division by zero), so the atomicMin finds the first failing row and why it failed
+// OP: 0 add, 1 sub, 2 mul, 3 div.  W: 64 or 128 (operand width).  d64 mul and div produce d128.
 template <int OP, int W>
 __global__ void __launch_bounds__(kThreads)
 dec_arith_kernel(void *__restrict__ r, const void *__restrict__ a, const void *__restrict__ b, uint64_t n, int c1, int c2, int d1, int d2, int adj,
-                 const uint64_t *__restrict__ rnulls, unsigned long long *first_bad) {
+                 uint64_t *__restrict__ rnulls, int div0_error, unsigned long long *first_bad) {
     for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
+        if (OP == 3) {
+            const i128 x = W == 64 ? (i128)reinterpret_cast<const int64_t *>(a)[c1 ? 0 : i] : d128_get(reinterpret_cast<const D128 *>(a)[c1 ? 0 : i]);
+            const i128 y = W == 64 ? (i128)reinterpret_cast<const int64_t *>(b)[c2 ? 0 : i] : d128_get(reinterpret_cast<const D128 *>(b)[c2 ? 0 : i]);
+            // a const zero divisor fails or nulls the whole vector before any row is looked at; a vector one only the rows it reaches
+            if (y == 0 && (c2 || !row_null(rnulls, i))) {
+                if (div0_error) atomicMin(first_bad, 2ull * i + 1);
+                else atomicOr(reinterpret_cast<unsigned long long *>(&rnulls[i >> 6]), 1ull << (i & 63));
+                continue;
+            }
+            if (row_null(rnulls, i)) continue;
+            i128 z;
+            if (dec_div(x, y, adj, z) != DIV_OK) atomicMin(first_bad, 2ull * i);
+            else reinterpret_cast<D128 *>(r)[i] = d128_put(z);
+            continue;
+        }
         if (row_null(rnulls, i)) continue;
         bool bad = false;
         if (W == 64 && OP != 2) {
@@ -119,12 +320,15 @@ dec_arith_kernel(void *__restrict__ r, const void *__restrict__ a, const void *_
                 reinterpret_cast<D128 *>(r)[i] = d128_put(v);
             }
         }
-        if (bad) atomicMin(first_bad, (unsigned long long)i);
+        if (bad) atomicMin(first_bad, 2ull * i);
     }
 }
 
-// rnulls |= n1 | n2 (non-const operands), tail bits cleared; a const NULL operand nulls every row
-__global__ void dec_nulls_kernel(uint64_t *rnulls, const uint64_t *n1, const uint64_t *n2, uint64_t n, int all_null) {
+// rnulls |= n1 | n2 (non-const operands), tail bits cleared; a const NULL operand nulls every row.  cn1 / cn2: the null words of const
+// operands, read here so that a call on resident operands needs no read-back
+__global__ void dec_nulls_kernel(uint64_t *rnulls, const uint64_t *n1, const uint64_t *n2, uint64_t n, int all_null,
+                                 const uint64_t *cn1 = nullptr, const uint64_t *cn2 = nullptr) {
+    if ((cn1 && (cn1[0] & 1)) || (cn2 && (cn2[0] & 1))) all_null = 1;
     const uint64_t nw = (n + 63) >> 6;
     for (uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < nw; w += (uint64_t)gridDim.x * blockDim.x) {
         uint64_t v = all_null ? ~0ull : rnulls[w];
@@ -172,16 +376,19 @@ dec_sum_kernel(const uint64_t *__restrict__ groups, const void *__restrict__ col
 
 template <int OP, int W>
 int run_dec_arith(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
-    const size_t in_sz = W / 8, out_sz = (OP == 2 || W == 128) ? 16 : 8;
+    const size_t in_sz = W / 8, out_sz = (OP >= 2 || W == 128) ? 16 : 8;
     const uint64_t nwords = (len + 63) / 64;
     const bool c1 = args[1].dataSz == in_sz && len > 1, c2 = args[2].dataSz == in_sz && len > 1;
     if ((!c1 && args[1].dataSz < in_sz * len) || (!c2 && args[2].dataSz < in_sz * len) || args[0].dataSz < out_sz * len || !args[0].pnulls) {
         set_error("decimal arith: vectors shorter than len, or result without a null bitmap"); return MO_RC_INVALID_ARGUMENT;
     }
-    DecParams P;
-    if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "decimal arith: params {scale1, scale2, err_row}")) return rc;
+    DecParams P{0, 0, -1, 0, 0};
+    if (int rc = read_param(t, args[3], &P, kDecParamsV1, OP == 3 ? sizeof P : kDecParamsV1, "decimal arith: params {scale1, scale2, err_row}")) return rc;
     int d1 = 0, d2 = 0, adj = 0;
-    if (OP == 2) { int d = 12; if (P.scale1 > d) d = P.scale1; if (P.scale2 > d) d = P.scale2; if (P.scale1 + P.scale2 < d) d = P.scale1 + P.scale2; adj = d - P.scale1 - P.scale2; }
+    if (OP == 3) {
+        if (P.scale1 < 0 || P.scale2 < 0 || P.scale1 > kMaxScale<W>() || P.scale2 > kMaxScale<W>()) { set_error("decimal arith: scales out of range"); return MO_RC_INVALID_ARGUMENT; }
+        adj = div_scale(P.scale1) - P.scale1 + P.scale2;
+    } else if (OP == 2) { int d = 12; if (P.scale1 > d) d = P.scale1; if (P.scale2 > d) d = P.scale2; if (P.scale1 + P.scale2 < d) d = P.scale1 + P.scale2; adj = d - P.scale1 - P.scale2; }
     else { d1 = P.scale2 > P.scale1 ? P.scale2 - P.scale1 : 0; d2 = P.scale1 > P.scale2 ? P.scale1 - P.scale2 : 0; }
     if (P.scale1 < 0 || P.scale2 < 0 || d1 > (W == 64 ? 18 : 19) || d2 > (W == 64 ? 18 : 19) || -adj > 38) { set_error("decimal arith: scales out of range"); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);
@@ -205,7 +412,7 @@ int run_dec_arith(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
         const uint64_t work = (len + kThreads - 1) / kThreads;
         if ((uint64_t)grid > work) grid = (int)work;
         cudaEventRecord(t.kev0, t.stream);
-        dec_arith_kernel<OP, W><<<grid, kThreads, 0, t.stream>>>(r, a, b, len, c1 ? 1 : 0, c2 ? 1 : 0, d1, d2, adj, rn, dbad);
+        dec_arith_kernel<OP, W><<<grid, kThreads, 0, t.stream>>>(r, a, b, len, c1 ? 1 : 0, c2 ? 1 : 0, d1, d2, adj, rn, P.div0_error, dbad);
         cudaEventRecord(t.kev1, t.stream);
         MOB_LAUNCH_CHECK();
     }
@@ -213,11 +420,13 @@ int run_dec_arith(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
     int rc = read_back(t, &bad, dbad, 8);
     if (rc) { st.finish(); return rc; }
     int frc = st.finish();
-    P.err_row = bad == kNoRow ? -1 : (int64_t)bad;
-    const int wrc = write_param(t, args[3].pdata, &P, sizeof P);
+    P.err_row = bad == kNoRow ? -1 : (int64_t)(bad >> 1);
+    const int wrc = write_param(t, args[3].pdata, &P, kDecParamsV1);
     if (frc || wrc) return frc ? frc : wrc;
     if (bad == kNoRow) return MO_RC_SUCCESS;
-    set_error("invalid input: Decimal%d %s overflow at row %llu", W, OP == 0 ? "Add" : (OP == 1 ? "Sub" : "Mul"), bad);
+    if (bad & 1) { set_error("division by zero"); return MO_RC_DIVISION_BY_ZERO; }
+    if (OP == 3) { set_error("invalid input: Decimal128 Div overflow at row %llu", bad >> 1); return MO_RC_INVALID_ARGUMENT; }
+    set_error("invalid input: Decimal%d %s overflow at row %llu", W, OP == 0 ? "Add" : (OP == 1 ? "Sub" : "Mul"), bad >> 1);
     return MO_RC_INVALID_ARGUMENT;
 }
 
@@ -255,6 +464,121 @@ int run_dec_sum(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
     return frc;
 }
 
+
+// GO_COMPARE(op, DECIMAL64 | DECIMAL128), valueDecimalCompare (func_compare.go:426-667): SIDE 1 scales a up by d, SIDE 2 scales b, SIDE 0
+// compares as stored.  Decimal64.Less / Decimal128.Less are signed compares.
+template <typename T> __device__ __forceinline__ bool dec_cmp(T x, T y, int op) {
+    switch (op) {
+    case CMP_EQ: return x == y; case CMP_NE: return x != y;
+    case CMP_GT: return x > y;  case CMP_GE: return x >= y;
+    case CMP_LT: return x < y;  default: return x <= y;
+    }
+}
+template <int W, int SIDE>
+__global__ void __launch_bounds__(kThreads)
+dec_cmp_kernel(uint8_t *__restrict__ r, const void *__restrict__ a, const void *__restrict__ b, uint64_t n, int c1, int c2, int d, int op,
+               const uint64_t *__restrict__ rnulls) {
+    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
+        if (row_null(rnulls, i)) continue;
+        bool v;
+        if (W == 64) {
+            int64_t x = reinterpret_cast<const int64_t *>(a)[c1 ? 0 : i], y = reinterpret_cast<const int64_t *>(b)[c2 ? 0 : i];
+            if (SIDE == 1) x = d64_scale_cmp(x, d); else if (SIDE == 2) y = d64_scale_cmp(y, d);
+            v = dec_cmp(x, y, op);
+        } else {
+            i128 x = d128_get(reinterpret_cast<const D128 *>(a)[c1 ? 0 : i]), y = d128_get(reinterpret_cast<const D128 *>(b)[c2 ? 0 : i]);
+            if (SIDE == 1) x = d128_scale_cmp(x, d); else if (SIDE == 2) y = d128_scale_cmp(y, d);
+            v = dec_cmp(x, y, op);
+        }
+        r[i] = v ? 1 : 0;
+    }
+}
+
+// AVG's Flush over DEC_SUM's state: decAvg (aggexec/sumavg2.go:545-559) = Decimal128.Div(sum, count) with Div's error dropped; count 0 is
+// NULL and keeps the sum as the value.  One warp writes one aligned 32-bit half of the result bitmap.
+__global__ void __launch_bounds__(kThreads)
+dec_avg_kernel(D128 *__restrict__ r, uint32_t *__restrict__ rnulls32, const D128 *__restrict__ sums, const int64_t *__restrict__ cnts, uint64_t n,
+               int adj) {
+    const uint64_t n64 = (n + 63) & ~63ull;
+    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n64; i += (uint64_t)gridDim.x * kThreads) {
+        const bool in = i < n;
+        const int64_t c = in ? cnts[i] : 0;
+        if (in) {
+            const D128 s = sums[i];
+            if (c == 0) r[i] = s;
+            else { i128 z; dec_div(d128_get(s), (i128)c, adj, z); r[i] = d128_put(z); }
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, in && c == 0);
+        if ((threadIdx.x & 31) == 0) rnulls32[i >> 5] = m;
+    }
+}
+
+int grid_for(uint64_t len) {
+    int grid = num_sms() * 8;
+    const uint64_t work = (len + kThreads - 1) / kThreads;
+    if ((uint64_t)grid > work) grid = (int)(work ? work : 1);
+    return grid;
+}
+
+template <int W>
+int run_dec_compare(ThreadCtx &t, int op, mo_xcall_args_t *args, uint64_t len) {
+    const size_t sz = W / 8;
+    const uint64_t nwords = (len + 63) / 64;
+    const bool c1 = args[1].dataSz == sz && len > 1, c2 = args[2].dataSz == sz && len > 1;
+    if ((!c1 && args[1].dataSz < sz * len) || (!c2 && args[2].dataSz < sz * len) || args[0].dataSz < len || !args[0].pnulls) {
+        set_error("go compare: vectors shorter than len, or the result has no null bitmap"); return MO_RC_INVALID_ARGUMENT;
+    }
+    DecParams P{0, 0, -1, 0, 0};
+    if (int rc = read_param(t, args[3], &P, kDecParamsV1, kDecParamsV1, "go compare: decimal params {scale1, scale2, err_row}")) return rc;
+    if (P.scale1 < 0 || P.scale2 < 0 || P.scale1 > kMaxScale<W>() || P.scale2 > kMaxScale<W>()) {
+        set_error("go compare: decimal scales out of range 0..%d", kMaxScale<W>()); return MO_RC_INVALID_ARGUMENT;
+    }
+    const int m = P.scale2 - P.scale1;
+    Stager st(t);
+    uint8_t *r = (uint8_t *)st.out(args[0].pdata, len, true);
+    uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, true);
+    const void *a = st.in(args[1].pdata, c1 ? sz : sz * len);
+    const void *b = st.in(args[2].pdata, c2 ? sz : sz * len);
+    const uint64_t *n1 = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? (c1 ? 8 : nwords * 8) : 0);
+    const uint64_t *n2 = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? (c2 ? 8 : nwords * 8) : 0);
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    dec_nulls_kernel<<<(unsigned)((nwords + 255) / 256 > 1024 ? 1024 : (nwords + 255) / 256), 256, 0, t.stream>>>(
+        rn, c1 ? nullptr : n1, c2 ? nullptr : n2, len, 0, c1 ? n1 : nullptr, c2 ? n2 : nullptr);
+    MOB_LAUNCH_CHECK();
+    cudaEventRecord(t.kev0, t.stream);
+    const int grid = grid_for(len), cc1 = c1 ? 1 : 0, cc2 = c2 ? 1 : 0;
+    if (m > 0) dec_cmp_kernel<W, 1><<<grid, kThreads, 0, t.stream>>>(r, a, b, len, cc1, cc2, m, op, rn);
+    else if (m < 0) dec_cmp_kernel<W, 2><<<grid, kThreads, 0, t.stream>>>(r, a, b, len, cc1, cc2, -m, op, rn);
+    else dec_cmp_kernel<W, 0><<<grid, kThreads, 0, t.stream>>>(r, a, b, len, cc1, cc2, 0, op, rn);
+    cudaEventRecord(t.kev1, t.stream);
+    MOB_LAUNCH_CHECK();
+    return st.complete();
+}
+
+template <int W>
+int run_dec_avg(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
+    const uint64_t nwords = (len + 63) / 64;
+    if (args[0].dataSz < 16 * len || !args[0].pnulls || args[1].dataSz < 16 * len || args[2].dataSz < 8 * len) {
+        set_error("decimal avg: result, sums (16 bytes per group) or counts (8 per group) shorter than len, or the result has no null bitmap");
+        return MO_RC_INVALID_ARGUMENT;
+    }
+    DecParams P{0, 0, -1, 0, 0};
+    if (int rc = read_param(t, args[3], &P, sizeof(int32_t), kDecParamsV1, "decimal avg: params {scale1 = the argument's scale}")) return rc;
+    if (P.scale1 < 0 || P.scale1 > kMaxScale<W>()) { set_error("decimal avg: scale out of range 0..%d", kMaxScale<W>()); return MO_RC_INVALID_ARGUMENT; }
+    Stager st(t);
+    D128 *r = (D128 *)st.out(args[0].pdata, 16 * len, false);
+    uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, false);
+    const D128 *sums = (const D128 *)st.in(args[1].pdata, 16 * len);
+    const int64_t *cnts = (const int64_t *)st.in(args[2].pdata, 8 * len);
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    cudaEventRecord(t.kev0, t.stream);
+    dec_avg_kernel<<<grid_for((len + 63) & ~63ull), kThreads, 0, t.stream>>>(r, reinterpret_cast<uint32_t *>(rn), sums, cnts, len,
+                                                                               div_scale(P.scale1) - P.scale1);
+    cudaEventRecord(t.kev1, t.stream);
+    MOB_LAUNCH_CHECK();
+    return st.complete();
+}
+
 }  // namespace
 
 namespace mob {
@@ -264,9 +588,29 @@ int xcall_dec_arith(int op, int width, mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     if (len == 0) return MO_RC_SUCCESS;
-    if (width == 64) { if (op == 0) return run_dec_arith<0, 64>(t, args, len); if (op == 1) return run_dec_arith<1, 64>(t, args, len); if (op == 2) return run_dec_arith<2, 64>(t, args, len); }
-    if (width == 128) { if (op == 0) return run_dec_arith<0, 128>(t, args, len); if (op == 1) return run_dec_arith<1, 128>(t, args, len); if (op == 2) return run_dec_arith<2, 128>(t, args, len); }
-    set_error("decimal arith: op 0..2 (+ - *), width 64 or 128");
+    if (width == 64) {
+        if (op == 0) return run_dec_arith<0, 64>(t, args, len); if (op == 1) return run_dec_arith<1, 64>(t, args, len);
+        if (op == 2) return run_dec_arith<2, 64>(t, args, len); if (op == 3) return run_dec_arith<3, 64>(t, args, len);
+    }
+    if (width == 128) {
+        if (op == 0) return run_dec_arith<0, 128>(t, args, len); if (op == 1) return run_dec_arith<1, 128>(t, args, len);
+        if (op == 2) return run_dec_arith<2, 128>(t, args, len); if (op == 3) return run_dec_arith<3, 128>(t, args, len);
+    }
+    set_error("decimal arith: op 0..3 (+ - * /), width 64 or 128");
+    return MO_RC_INVALID_ARGUMENT;
+}
+// MO_XCALL_GO_COMPARE(op, DECIMAL64 | DECIMAL128), routed here by goelem.cu: args as GO_COMPARE plus [3] mo_dec_params_t (the scales)
+int go_dec_compare(ThreadCtx &t, int op, int T, mo_xcall_args_t *args, uint64_t len) {
+    return T == MO_T_DECIMAL64 ? run_dec_compare<64>(t, op, args, len) : run_dec_compare<128>(t, op, args, len);
+}
+// MO_XCALL_DEC_AVG(width): args [0] result Decimal128 per group (+pnulls out) ; [1] sums ; [2] counts (DEC_SUM's state) ; [3] mo_dec_params_t
+int xcall_dec_avg(int width, mo_xcall_args_t *args, uint64_t len) {
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    if (len == 0) return MO_RC_SUCCESS;
+    if (width == 64) return run_dec_avg<64>(t, args, len);
+    if (width == 128) return run_dec_avg<128>(t, args, len);
+    set_error("decimal avg: width 64 or 128");
     return MO_RC_INVALID_ARGUMENT;
 }
 // MO_XCALL_DEC_SUM(width): args [0] sums Decimal128 per group (in/out) ; [1] counts int64 per group (in/out) ; [2] groups uint64[len] or NULL (one group) ; [3] column (+pnulls)

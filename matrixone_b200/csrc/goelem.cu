@@ -169,6 +169,12 @@ __global__ void go_nulls_kernel(uint64_t *rnulls, const uint64_t *n1, const uint
     }
 }
 
+// a Decimal128 as stored {B0_63, B64_127}: two 8-byte words, so a column needs only 8-byte alignment; orders as a signed 128-bit value
+struct Dec128 { uint64_t lo; int64_t hi; };
+__host__ __device__ __forceinline__ bool operator<(const Dec128 &x, const Dec128 &y) { return x.hi != y.hi ? x.hi < y.hi : x.lo < y.lo; }
+__host__ __device__ __forceinline__ bool operator>=(const Dec128 &x, const Dec128 &y) { return !(x < y); }
+__host__ __device__ __forceinline__ bool operator<=(const Dec128 &x, const Dec128 &y) { return !(y < x); }
+
 // between: null input -> res = false and the null bit set; one warp covers an aligned 32-row half word of the bitmap
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
@@ -409,6 +415,7 @@ int run_go_multi_logic(ThreadCtx &t, int is_or, mo_xcall_args_t *args, uint64_t 
 namespace mob {
 
 int go_str_compare(ThreadCtx &t, int op, mo_xcall_args_t *args, uint64_t len);
+int go_dec_compare(ThreadCtx &t, int op, int T, mo_xcall_args_t *args, uint64_t len);
 
 int xcall_go_elementwise(int64_t funcId, mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
@@ -447,6 +454,7 @@ int xcall_go_elementwise(int64_t funcId, mo_xcall_args_t *args, uint64_t len) {
         case MO_T_FLOAT64: return run_go_compare<double>(t, op, args, len);
         case MO_T_CHAR: case MO_T_VARCHAR: case MO_T_BINARY: case MO_T_VARBINARY: case MO_T_BLOB: case MO_T_TEXT: case MO_T_DATALINK:
             return go_str_compare(t, op, args, len);   // strpred.cu
+        case MO_T_DECIMAL64: case MO_T_DECIMAL128: return go_dec_compare(t, op, T, args, len);   // decimal.cu
         }
         set_error("go compare: unsupported type %d", T);
         return MO_RC_INVALID_ARGUMENT;
@@ -471,6 +479,9 @@ int xcall_go_elementwise(int64_t funcId, mo_xcall_args_t *args, uint64_t len) {
         case MO_T_UINT64: return run_go_between<uint64_t>(t, args, len);
         case MO_T_FLOAT32: return run_go_between<float>(t, args, len);
         case MO_T_FLOAT64: return run_go_between<double>(t, args, len);
+        // CompareDecimal64 / 128 (operator_between.go:68-73): the planner casts the bounds to the column's type, so a raw signed compare (DECIMAL64 as int64, DECIMAL128 as Dec128)
+        case MO_T_DECIMAL64: return run_go_between<int64_t>(t, args, len);
+        case MO_T_DECIMAL128: return run_go_between<Dec128>(t, args, len);
         }
         set_error("go between: unsupported type %d", T);
         return MO_RC_INVALID_ARGUMENT;

@@ -19,6 +19,7 @@ int xcall_agg_merge(int op, int T, mo_xcall_args_t *args, uint64_t len);
 int xcall_plan(mo_xcall_args_t *args, uint64_t len);
 int xcall_dec_arith(int op, int width, mo_xcall_args_t *args, uint64_t len);
 int xcall_dec_sum(int width, mo_xcall_args_t *args, uint64_t len);
+int xcall_dec_avg(int width, mo_xcall_args_t *args, uint64_t len);
 int xcall_filter_sels(mo_xcall_args_t *args, uint64_t len);
 int xcall_shuffle(int szof, mo_xcall_args_t *args, uint64_t len);
 int xcall_pack_keys(mo_xcall_args_t *args, uint64_t len);
@@ -71,8 +72,9 @@ extern "C" int32_t XCall(int64_t runtimeId, int64_t funcId, uint8_t *errStr, uin
     else if (funcId >= 0x1000 && funcId < 0x1000 + (5 << 8)) rc = xcall_agg((int)((funcId - 0x1000) >> 8), (int)((funcId - 0x1000) & 0xff), a, len);
     else if (funcId >= 0x1800 && funcId < 0x1800 + (5 << 8)) rc = xcall_agg_merge((int)((funcId - 0x1800) >> 8), (int)((funcId - 0x1800) & 0xff), a, len);
     else if (funcId == MO_XCALL_PLAN) rc = xcall_plan(a, len);
-    else if (funcId >= 0x7000 && funcId < 0x7300) rc = xcall_dec_arith((int)((funcId - 0x7000) >> 8), (int)(funcId & 0xff), a, len);
+    else if (funcId >= 0x7000 && funcId < 0x7400) rc = xcall_dec_arith((int)((funcId - 0x7000) >> 8), (int)(funcId & 0xff), a, len);
     else if (funcId >= 0x7400 && funcId < 0x7500) rc = xcall_dec_sum((int)(funcId & 0xff), a, len);
+    else if (funcId >= 0x7500 && funcId < 0x7600) rc = xcall_dec_avg((int)(funcId & 0xff), a, len);
     else if (funcId == MO_XCALL_FILTER_SELS) rc = xcall_filter_sels(a, len);
     else if (funcId == MO_XCALL_PACK_KEYS) rc = xcall_pack_keys(a, len);
     else if (funcId == MO_XCALL_GROUP_IDS) rc = xcall_group_ids(a, len);

@@ -931,6 +931,103 @@ def dec_sum(width, col, sums, counts, groups=None, nulls=None, n=None):
                                       _with_nulls(c.view(np.uint8).reshape(-1), nulls, n)], n)
 
 
+def _dec_bytes(x):
+    return x if isinstance(x, DeviceBuffer) else np.ascontiguousarray(x).view(np.uint8).reshape(-1)
+
+
+def _dec_result_nulls(n, rnulls):
+    return np.zeros((n + 63) // 64, dtype=np.uint64) if rnulls is None else np.ascontiguousarray(rnulls, dtype=np.uint64).copy()
+
+
+def dec_compare(op, width, a, b, scale1, scale2, n, n1=None, n2=None, rnulls=None):
+    """a <op> b over DECIMAL64 (int64 arrays) or DECIMAL128 (uint64[n, 2] {lo, hi}) operands at scales scale1 / scale2 (valueDecimalCompare:
+    the lower-scale side is scaled up, a failed scale-up compares unscaled).  A 1-row operand is const; rnulls: the result bitmap on entry
+    (rows set there are skipped).  Returns (values uint8[n], result nulls words)."""
+    r = np.zeros(n, dtype=np.uint8)
+    rn = _dec_result_nulls(n, rnulls)
+    xcall(capi.XCALL_GO_COMPARE(op, capi.T_DECIMAL64 if width == 64 else capi.T_DECIMAL128),
+          [Vector(data=r, nulls=rn, length=n), _with_nulls(_dec_bytes(a), n1, n), _with_nulls(_dec_bytes(b), n2, n),
+           _params_vec(capi.DecParams(scale1, scale2, -1))], n)
+    return r, rn
+
+
+def dec_compare_device(op, width, a, b, scale1, scale2, n, out_dev, out_nulls_dev, n1=None, n2=None):
+    """dec_compare on resident operands (DeviceBuffers; one element's bytes = const) into out_dev (bool[n]) and out_nulls_dev (its bitmap,
+    in/out): enqueue-only, nothing is read back or synchronised"""
+    xcall(capi.XCALL_GO_COMPARE(op, capi.T_DECIMAL64 if width == 64 else capi.T_DECIMAL128),
+          [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n), _with_nulls(a, n1, n), _with_nulls(b, n2, n),
+           _params_vec(capi.DecParams(scale1, scale2, -1))], n)
+
+
+def _dec_bound(width, v):
+    v = int(v)
+    if width == 64:
+        return np.array([v], dtype=np.int64)
+    return np.array([v & ((1 << 64) - 1), (v >> 64) & ((1 << 64) - 1)], dtype=np.uint64)
+
+
+def dec_between(width, col, lo, hi, n, nulls=None):
+    """col BETWEEN lo AND hi over a decimal column, the bounds (Python ints) already at the column's scale: a raw signed compare.  A NULL
+    row gives false and a NULL result.  col may be a numpy array or a DeviceBuffer.  Returns (values uint8[n], result nulls words)."""
+    r = np.zeros(n, dtype=np.uint8)
+    rn = np.zeros((n + 63) // 64, dtype=np.uint64)
+    xcall(capi.XCALL_GO_BETWEEN(capi.T_DECIMAL64 if width == 64 else capi.T_DECIMAL128),
+          [Vector(data=r, nulls=rn, length=n), _with_nulls(_dec_bytes(col), nulls, n), Vector(data=_dec_bound(width, lo), length=1, const=True),
+           Vector(data=_dec_bound(width, hi), length=1, const=True)], n)
+    return r, rn
+
+
+def dec_between_device(width, col, lo, hi, n, out_dev, out_nulls_dev, nulls=None):
+    """dec_between on a resident column into resident outputs (out_nulls_dev zeroed by the caller)"""
+    xcall(capi.XCALL_GO_BETWEEN(capi.T_DECIMAL64 if width == 64 else capi.T_DECIMAL128),
+          [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n), _with_nulls(col, nulls, n),
+           Vector(data=_dec_bound(width, lo), length=1, const=True), Vector(data=_dec_bound(width, hi), length=1, const=True)], n)
+
+
+def dec_div(width, a, b, scale1, scale2, n, n1=None, n2=None, rnulls=None, div0_error=False):
+    """a / b (d64Div / d128Div): the result is Decimal128 uint64[n, 2] at scale min(12, scale1 + 6) raised to at least scale1.  A zero divisor
+    makes the row NULL, or fails the call with RC_DIVISION_BY_ZERO when div0_error.  Returns (rc, result, result nulls words, err_row, msg):
+    rc is 0, RC_INVALID_ARGUMENT ("Decimal128 Div overflow") or RC_DIVISION_BY_ZERO, err_row the first failing row or -1."""
+    r = np.zeros((n, 2), dtype=np.uint64)
+    rn = _dec_result_nulls(n, rnulls)
+    prm = np.frombuffer(bytes(capi.DecDivParams(scale1, scale2, -1, 1 if div0_error else 0, 0)), dtype=np.uint8).copy()
+    rc, msg = xcall(capi.XCALL_DEC_ARITH(capi.DEC_OP_DIV, width),
+                    [Vector(data=r.view(np.uint8).reshape(-1), nulls=rn, length=n), _with_nulls(_dec_bytes(a), n1, n), _with_nulls(_dec_bytes(b), n2, n),
+                     Vector(data=prm, length=1, const=True)], n, raise_on_error=False)
+    if rc not in (0, capi.RC_INVALID_ARGUMENT, capi.RC_DIVISION_BY_ZERO):
+        raise capi.MoError(rc, msg)
+    return rc, r, rn, int(prm.view(np.int64)[1]), msg
+
+
+def dec_div_device(width, a, b, scale1, scale2, n, out_dev, out_nulls_dev, n1=None, n2=None, div0_error=False):
+    """dec_div on resident operands into resident outputs (out_nulls_dev in/out).  One read-back of the first failing row; returns
+    (rc, err_row, msg)."""
+    prm = np.frombuffer(bytes(capi.DecDivParams(scale1, scale2, -1, 1 if div0_error else 0, 0)), dtype=np.uint8).copy()
+    rc, msg = xcall(capi.XCALL_DEC_ARITH(capi.DEC_OP_DIV, width),
+                    [Vector(data_ptr=out_dev.ptr, data_nbytes=16 * n, nulls_ptr=out_nulls_dev.ptr, length=n), _with_nulls(a, n1, n),
+                     _with_nulls(b, n2, n), Vector(data=prm, length=1, const=True)], n, raise_on_error=False)
+    if rc not in (0, capi.RC_INVALID_ARGUMENT, capi.RC_DIVISION_BY_ZERO):
+        raise capi.MoError(rc, msg)
+    return rc, int(prm.view(np.int64)[1]), msg
+
+
+def dec_avg(width, sums, counts, scale):
+    """AVG's Flush over DEC_SUM's state (decAvg): sums uint64[g, 2], counts int64[g], scale = the argument's scale.  Returns (result
+    uint64[g, 2] at scale max(12, scale) capped at scale + 6, result nulls words: count 0 is NULL)."""
+    g = counts.shape[0]
+    r = np.zeros((g, 2), dtype=np.uint64)
+    rn = np.zeros((g + 63) // 64, dtype=np.uint64)
+    xcall(capi.XCALL_DEC_AVG(width), [Vector(data=r.view(np.uint8).reshape(-1), nulls=rn, length=g), _vec(_dec_bytes(sums), g),
+                                      _vec(np.ascontiguousarray(counts, dtype=np.int64), g), _params_vec(capi.DecParams(scale, 0, -1))], g)
+    return r, rn
+
+
+def dec_avg_device(width, sums, counts, g, scale, out_dev, out_nulls_dev):
+    """dec_avg on resident state (DeviceBuffers) into resident outputs: enqueue-only"""
+    xcall(capi.XCALL_DEC_AVG(width), [Vector(data_ptr=out_dev.ptr, data_nbytes=16 * g, nulls_ptr=out_nulls_dev.ptr, length=g), _vec(sums, g),
+                                      _vec(counts, g), _params_vec(capi.DecParams(scale, 0, -1))], g)
+
+
 # ---------------------------------------------------------------------------------------------- normalize_l2 (vector-valued)
 def normalize_l2(cells, area, length, dtype=np.float32, nulls=None):
     """normalize_l2(v) over a varlena vector column (moarray.NormalizeL2, pkg/vectorize/moarray/external.go:262-285).  Returns
