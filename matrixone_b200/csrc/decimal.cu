@@ -8,27 +8,24 @@
 //   MO_XCALL_GO_COMPARE(op, DECIMAL64 | DECIMAL128)   valueDecimalCompare, pkg/sql/plan/function/func_compare.go:426-667
 //
 // Pure integer work, bit-exact: Decimal64 = int64 unscaled value, Decimal128 = two's-complement {B0_63, B64_127}; the scales travel in
-// the parameter block.  Conventions are those of the Go elementwise engine (goelem.cu): result nulls pre-filled by the caller
-// (NOT selectList), OR-ed with the operand nulls; the FIRST offending row in row order fails the call ("Decimal64 Add overflow",
-// "scale overflow", "Decimal128 Mul overflow" -> MO_RC_INVALID_ARGUMENT = moerr ErrInvalidInput) and is reported in the parameter block.
+// the parameter block.  The operand protocol is the Go elementwise engine's (goengine.cuh); the FIRST offending row in row order fails the
+// call ("Decimal64 Add overflow", "scale overflow", "Decimal128 Mul overflow" -> MO_RC_INVALID_ARGUMENT = moerr ErrInvalidInput).
 // 128-bit sums are accumulated as two 64-bit atomics with an explicit carry: integer addition is associative, so the result is exact
 // and run-to-run identical whatever the order.
-#include "common.cuh"
+#include "goengine.cuh"
 #include <cstring>
 
 using namespace mob;
 
 namespace {
 
-constexpr int kThreads = 256;
-constexpr unsigned long long kNoRow = ~0ull;
+constexpr int kCtasPerSm = 8;
 
-struct D128 { uint64_t lo, hi; };
 typedef unsigned __int128 u128;
 typedef __int128 i128;
 
-__device__ __forceinline__ i128 d128_get(D128 v) { return (i128)(((u128)v.hi << 64) | v.lo); }
-__device__ __forceinline__ D128 d128_put(i128 x) { D128 r; r.lo = (uint64_t)(u128)x; r.hi = (uint64_t)((u128)x >> 64); return r; }
+__device__ __forceinline__ i128 d128_get(Dec128 v) { return (i128)(((u128)(uint64_t)v.hi << 64) | v.lo); }
+__device__ __forceinline__ Dec128 d128_put(i128 x) { Dec128 r; r.lo = (uint64_t)(u128)x; r.hi = (int64_t)((u128)x >> 64); return r; }
 
 __constant__ uint64_t kPow10[20] = {1ull, 10ull, 100ull, 1000ull, 10000ull, 100000ull, 1000000ull, 10000000ull, 100000000ull, 1000000000ull,
     10000000000ull, 100000000000ull, 1000000000000ull, 10000000000000ull, 100000000000000ull, 1000000000000000ull, 10000000000000000ull,
@@ -253,7 +250,7 @@ constexpr size_t kDecParamsV1 = 16;   // {scale1, scale2, err_row}: what + - * r
 
 __device__ __forceinline__ bool row_null(const uint64_t *rnulls, uint64_t i) { return (rnulls[i >> 6] >> (i & 63)) & 1ull; }
 
-// first_bad holds 2 * row + kind (kind 1 = division by zero), so the atomicMin finds the first failing row and why it failed
+// the failure record's kind: 1 = division by zero
 // OP: 0 add, 1 sub, 2 mul, 3 div.  W: 64 or 128 (operand width).  d64 mul and div produce d128.
 template <int OP, int W>
 __global__ void __launch_bounds__(kThreads)
@@ -261,18 +258,18 @@ dec_arith_kernel(void *__restrict__ r, const void *__restrict__ a, const void *_
                  uint64_t *__restrict__ rnulls, int div0_error, unsigned long long *first_bad) {
     for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
         if (OP == 3) {
-            const i128 x = W == 64 ? (i128)reinterpret_cast<const int64_t *>(a)[c1 ? 0 : i] : d128_get(reinterpret_cast<const D128 *>(a)[c1 ? 0 : i]);
-            const i128 y = W == 64 ? (i128)reinterpret_cast<const int64_t *>(b)[c2 ? 0 : i] : d128_get(reinterpret_cast<const D128 *>(b)[c2 ? 0 : i]);
+            const i128 x = W == 64 ? (i128)reinterpret_cast<const int64_t *>(a)[c1 ? 0 : i] : d128_get(reinterpret_cast<const Dec128 *>(a)[c1 ? 0 : i]);
+            const i128 y = W == 64 ? (i128)reinterpret_cast<const int64_t *>(b)[c2 ? 0 : i] : d128_get(reinterpret_cast<const Dec128 *>(b)[c2 ? 0 : i]);
             // a const zero divisor fails or nulls the whole vector before any row is looked at; a vector one only the rows it reaches
             if (y == 0 && (c2 || !row_null(rnulls, i))) {
-                if (div0_error) atomicMin(first_bad, 2ull * i + 1);
+                if (div0_error) note_failure(first_bad, i, 1);
                 else atomicOr(reinterpret_cast<unsigned long long *>(&rnulls[i >> 6]), 1ull << (i & 63));
                 continue;
             }
             if (row_null(rnulls, i)) continue;
             i128 z;
-            if (dec_div(x, y, adj, z) != DIV_OK) atomicMin(first_bad, 2ull * i);
-            else reinterpret_cast<D128 *>(r)[i] = d128_put(z);
+            if (dec_div(x, y, adj, z) != DIV_OK) note_failure(first_bad, i);
+            else reinterpret_cast<Dec128 *>(r)[i] = d128_put(z);
             continue;
         }
         if (row_null(rnulls, i)) continue;
@@ -293,18 +290,18 @@ dec_arith_kernel(void *__restrict__ r, const void *__restrict__ a, const void *_
             mag_div_pow10(m, -adj);
             i128 v = (i128)(((u128)m[1] << 64) | m[0]);
             if ((x < 0) != (y < 0)) v = -v;
-            reinterpret_cast<D128 *>(r)[i] = d128_put(v);
+            reinterpret_cast<Dec128 *>(r)[i] = d128_put(v);
         } else if (OP != 2) {
-            i128 x = d128_get(reinterpret_cast<const D128 *>(a)[c1 ? 0 : i]), y = d128_get(reinterpret_cast<const D128 *>(b)[c2 ? 0 : i]);
+            i128 x = d128_get(reinterpret_cast<const Dec128 *>(a)[c1 ? 0 : i]), y = d128_get(reinterpret_cast<const Dec128 *>(b)[c2 ? 0 : i]);
             if ((d1 && !d128_scale_up(x, d1)) || (d2 && !d128_scale_up(y, d2))) bad = true;
             else {
                 const i128 z = (i128)(OP == 1 ? (u128)x - (u128)y : (u128)x + (u128)y);
                 const bool sx = x < 0, sy = y < 0, sz = z < 0;
                 bad = OP == 1 ? (sx != sy && sx != sz) : (sx == sy && sx != sz);
-                reinterpret_cast<D128 *>(r)[i] = d128_put(z);
+                reinterpret_cast<Dec128 *>(r)[i] = d128_put(z);
             }
         } else {
-            const i128 x = d128_get(reinterpret_cast<const D128 *>(a)[c1 ? 0 : i]), y = d128_get(reinterpret_cast<const D128 *>(b)[c2 ? 0 : i]);
+            const i128 x = d128_get(reinterpret_cast<const Dec128 *>(a)[c1 ? 0 : i]), y = d128_get(reinterpret_cast<const Dec128 *>(b)[c2 ? 0 : i]);
             const u128 ax = x < 0 ? (u128)0 - (u128)x : (u128)x, ay = y < 0 ? (u128)0 - (u128)y : (u128)y;
             const uint64_t xl = (uint64_t)ax, xh = (uint64_t)(ax >> 64), yl = (uint64_t)ay, yh = (uint64_t)(ay >> 64);
             uint64_t m[4];
@@ -317,24 +314,10 @@ dec_arith_kernel(void *__restrict__ r, const void *__restrict__ a, const void *_
             else {
                 i128 v = (i128)(((u128)m[1] << 64) | m[0]);
                 if ((x < 0) != (y < 0)) v = -v;
-                reinterpret_cast<D128 *>(r)[i] = d128_put(v);
+                reinterpret_cast<Dec128 *>(r)[i] = d128_put(v);
             }
         }
-        if (bad) atomicMin(first_bad, 2ull * i);
-    }
-}
-
-// rnulls |= n1 | n2 (non-const operands), tail bits cleared; a const NULL operand nulls every row.  cn1 / cn2: the null words of const
-// operands, read here so that a call on resident operands needs no read-back
-__global__ void dec_nulls_kernel(uint64_t *rnulls, const uint64_t *n1, const uint64_t *n2, uint64_t n, int all_null,
-                                 const uint64_t *cn1 = nullptr, const uint64_t *cn2 = nullptr) {
-    if ((cn1 && (cn1[0] & 1)) || (cn2 && (cn2[0] & 1))) all_null = 1;
-    const uint64_t nw = (n + 63) >> 6;
-    for (uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < nw; w += (uint64_t)gridDim.x * blockDim.x) {
-        uint64_t v = all_null ? ~0ull : rnulls[w];
-        if (!all_null) { if (n1) v |= n1[w]; if (n2) v |= n2[w]; }
-        if (w == nw - 1 && (n & 63)) { if (all_null) v = rnulls[w] | ((1ull << (n & 63)) - 1); else v &= (1ull << (n & 63)) - 1; }
-        rnulls[w] = v;
+        if (bad) note_failure(first_bad, i);
     }
 }
 
@@ -363,7 +346,7 @@ dec_sum_kernel(const uint64_t *__restrict__ groups, const void *__restrict__ col
         if (nulls && ((nulls[i >> 6] >> (i & 63)) & 1ull)) continue;
         uint64_t lo, hi;
         if (W == 64) { const int64_t v = reinterpret_cast<const int64_t *>(col)[i]; lo = (uint64_t)v; hi = v < 0 ? ~0ull : 0ull; }   // Decimal128FromDecimal64: sign extension
-        else { const D128 v = reinterpret_cast<const D128 *>(col)[i]; lo = v.lo; hi = v.hi; }
+        else { const Dec128 v = reinterpret_cast<const Dec128 *>(col)[i]; lo = v.lo; hi = (uint64_t)v.hi; }
         if (SMEM) { atomic_add128(&s_acc[2 * (g - 1)], lo, hi); atomicAdd(&s_cnt[g - 1], 1ull); }
         else { atomic_add128(&sums[2 * (g - 1)], lo, hi); atomicAdd(&cnts[g - 1], 1ull); }
     }
@@ -376,12 +359,14 @@ dec_sum_kernel(const uint64_t *__restrict__ groups, const void *__restrict__ col
 
 template <int OP, int W>
 int run_dec_arith(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
+    const char *what = "decimal arith";
     const size_t in_sz = W / 8, out_sz = (OP >= 2 || W == 128) ? 16 : 8;
-    const uint64_t nwords = (len + 63) / 64;
-    const bool c1 = args[1].dataSz == in_sz && len > 1, c2 = args[2].dataSz == in_sz && len > 1;
-    if ((!c1 && args[1].dataSz < in_sz * len) || (!c2 && args[2].dataSz < in_sz * len) || args[0].dataSz < out_sz * len || !args[0].pnulls) {
-        set_error("decimal arith: vectors shorter than len, or result without a null bitmap"); return MO_RC_INVALID_ARGUMENT;
-    }
+    Stager st(t);
+    void *r; uint64_t *rn;
+    Operand a, b;
+    if (int rc = stage_result(st, args[0], out_sz, len, true, true, what, r, rn)) return rc;
+    if (int rc = stage_operand(st, args[1], in_sz, len, what, 1, a)) return rc;
+    if (int rc = stage_operand(st, args[2], in_sz, len, what, 2, b)) return rc;
     DecParams P{0, 0, -1, 0, 0};
     if (int rc = read_param(t, args[3], &P, kDecParamsV1, OP == 3 ? sizeof P : kDecParamsV1, "decimal arith: params {scale1, scale2, err_row}")) return rc;
     int d1 = 0, d2 = 0, adj = 0;
@@ -391,42 +376,23 @@ int run_dec_arith(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
     } else if (OP == 2) { int d = 12; if (P.scale1 > d) d = P.scale1; if (P.scale2 > d) d = P.scale2; if (P.scale1 + P.scale2 < d) d = P.scale1 + P.scale2; adj = d - P.scale1 - P.scale2; }
     else { d1 = P.scale2 > P.scale1 ? P.scale2 - P.scale1 : 0; d2 = P.scale1 > P.scale2 ? P.scale1 - P.scale2 : 0; }
     if (P.scale1 < 0 || P.scale2 < 0 || d1 > (W == 64 ? 18 : 19) || d2 > (W == 64 ? 18 : 19) || -adj > 38) { set_error("decimal arith: scales out of range"); return MO_RC_INVALID_ARGUMENT; }
-    Stager st(t);
-    void *r = st.out(args[0].pdata, out_sz * len, true);
-    uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, true);
-    const void *a = st.in(args[1].pdata, c1 ? in_sz : in_sz * len);
-    const void *b = st.in(args[2].pdata, c2 ? in_sz : in_sz * len);
-    const uint64_t *n1 = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? (c1 ? 8 : nwords * 8) : 0);
-    const uint64_t *n2 = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? (c2 ? 8 : nwords * 8) : 0);
-    unsigned long long *dbad = (unsigned long long *)st.tmp(8);
-    if (st.failed) return MO_RC_INTERNAL_ERROR;
-    uint64_t h1 = 0, h2 = 0;
-    if (c1 && n1) { int rc = read_back(t, &h1, n1, 8); if (rc) { st.finish(); return rc; } }
-    if (c2 && n2) { int rc = read_back(t, &h2, n2, 8); if (rc) { st.finish(); return rc; } }
-    const bool all_null = (c1 && (h1 & 1)) || (c2 && (h2 & 1));
-    MOB_CUDA_TRY(cudaMemsetAsync(dbad, 0xff, 8, t.stream));
-    dec_nulls_kernel<<<(unsigned)((nwords + 255) / 256 > 1024 ? 1024 : (nwords + 255) / 256), 256, 0, t.stream>>>(rn, c1 ? nullptr : n1, c2 ? nullptr : n2, len, all_null ? 1 : 0);
-    MOB_LAUNCH_CHECK();
+    RowRecord rec;
+    if (int rc = rec.arm(t, st)) return rc;
+    bool all_null;   // a const NULL operand nulls every row before a const zero divisor is looked at
+    if (int rc = merge_nulls(t, rn, len, a, b, &all_null)) return rc;
     if (!all_null) {
-        int grid = num_sms() * 8;
-        const uint64_t work = (len + kThreads - 1) / kThreads;
-        if ((uint64_t)grid > work) grid = (int)work;
         cudaEventRecord(t.kev0, t.stream);
-        dec_arith_kernel<OP, W><<<grid, kThreads, 0, t.stream>>>(r, a, b, len, c1 ? 1 : 0, c2 ? 1 : 0, d1, d2, adj, rn, P.div0_error, dbad);
+        dec_arith_kernel<OP, W><<<grid_rows(len, kCtasPerSm), kThreads, 0, t.stream>>>(r, a.data, b.data, len, a.cst, b.cst, d1, d2, adj, rn,
+                                                                                      P.div0_error, rec.dev);
         cudaEventRecord(t.kev1, t.stream);
         MOB_LAUNCH_CHECK();
     }
-    unsigned long long bad = kNoRow;
-    int rc = read_back(t, &bad, dbad, 8);
-    if (rc) { st.finish(); return rc; }
-    int frc = st.finish();
-    P.err_row = bad == kNoRow ? -1 : (int64_t)(bad >> 1);
-    const int wrc = write_param(t, args[3].pdata, &P, kDecParamsV1);
-    if (frc || wrc) return frc ? frc : wrc;
-    if (bad == kNoRow) return MO_RC_SUCCESS;
-    if (bad & 1) { set_error("division by zero"); return MO_RC_DIVISION_BY_ZERO; }
-    if (OP == 3) { set_error("invalid input: Decimal128 Div overflow at row %llu", bad >> 1); return MO_RC_INVALID_ARGUMENT; }
-    set_error("invalid input: Decimal%d %s overflow at row %llu", W, OP == 0 ? "Add" : (OP == 1 ? "Sub" : "Mul"), bad >> 1);
+    if (int rc = rec.read(t)) return rc;
+    if (int rc = rec.finish(t, st, args[3].pdata, &P, kDecParamsV1, P.err_row)) return rc;
+    if (!rec.failed()) return MO_RC_SUCCESS;
+    if (rec.kind() == 1) { set_error("division by zero"); return MO_RC_DIVISION_BY_ZERO; }
+    if (OP == 3) { set_error("invalid input: Decimal128 Div overflow at row %llu", (unsigned long long)rec.row()); return MO_RC_INVALID_ARGUMENT; }
+    set_error("invalid input: Decimal%d %s overflow at row %llu", W, OP == 0 ? "Add" : (OP == 1 ? "Sub" : "Mul"), (unsigned long long)rec.row());
     return MO_RC_INVALID_ARGUMENT;
 }
 
@@ -447,9 +413,7 @@ int run_dec_sum(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
     if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(dbad, 0, 4, t.stream));
     if (len) {
-        int grid = num_sms() * 8;
-        const uint64_t work = (len + kThreads - 1) / kThreads;
-        if ((uint64_t)grid > work) grid = (int)work;
+        const int grid = grid_rows(len, kCtasPerSm);
         cudaEventRecord(t.kev0, t.stream);
         if (ngroups <= (uint64_t)kSumSlots) dec_sum_kernel<W, true><<<grid, kThreads, 0, t.stream>>>(groups, col, nulls, len, ngroups, sums, cnts, dbad);
         else dec_sum_kernel<W, false><<<grid, kThreads, 0, t.stream>>>(groups, col, nulls, len, ngroups, sums, cnts, dbad);
@@ -467,13 +431,6 @@ int run_dec_sum(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
 
 // GO_COMPARE(op, DECIMAL64 | DECIMAL128), valueDecimalCompare (func_compare.go:426-667): SIDE 1 scales a up by d, SIDE 2 scales b, SIDE 0
 // compares as stored.  Decimal64.Less / Decimal128.Less are signed compares.
-template <typename T> __device__ __forceinline__ bool dec_cmp(T x, T y, int op) {
-    switch (op) {
-    case CMP_EQ: return x == y; case CMP_NE: return x != y;
-    case CMP_GT: return x > y;  case CMP_GE: return x >= y;
-    case CMP_LT: return x < y;  default: return x <= y;
-    }
-}
 template <int W, int SIDE>
 __global__ void __launch_bounds__(kThreads)
 dec_cmp_kernel(uint8_t *__restrict__ r, const void *__restrict__ a, const void *__restrict__ b, uint64_t n, int c1, int c2, int d, int op,
@@ -484,11 +441,11 @@ dec_cmp_kernel(uint8_t *__restrict__ r, const void *__restrict__ a, const void *
         if (W == 64) {
             int64_t x = reinterpret_cast<const int64_t *>(a)[c1 ? 0 : i], y = reinterpret_cast<const int64_t *>(b)[c2 ? 0 : i];
             if (SIDE == 1) x = d64_scale_cmp(x, d); else if (SIDE == 2) y = d64_scale_cmp(y, d);
-            v = dec_cmp(x, y, op);
+            v = cmp_op(x, y, op);
         } else {
-            i128 x = d128_get(reinterpret_cast<const D128 *>(a)[c1 ? 0 : i]), y = d128_get(reinterpret_cast<const D128 *>(b)[c2 ? 0 : i]);
+            i128 x = d128_get(reinterpret_cast<const Dec128 *>(a)[c1 ? 0 : i]), y = d128_get(reinterpret_cast<const Dec128 *>(b)[c2 ? 0 : i]);
             if (SIDE == 1) x = d128_scale_cmp(x, d); else if (SIDE == 2) y = d128_scale_cmp(y, d);
-            v = dec_cmp(x, y, op);
+            v = cmp_op(x, y, op);
         }
         r[i] = v ? 1 : 0;
     }
@@ -497,14 +454,14 @@ dec_cmp_kernel(uint8_t *__restrict__ r, const void *__restrict__ a, const void *
 // AVG's Flush over DEC_SUM's state: decAvg (aggexec/sumavg2.go:545-559) = Decimal128.Div(sum, count) with Div's error dropped; count 0 is
 // NULL and keeps the sum as the value.  One warp writes one aligned 32-bit half of the result bitmap.
 __global__ void __launch_bounds__(kThreads)
-dec_avg_kernel(D128 *__restrict__ r, uint32_t *__restrict__ rnulls32, const D128 *__restrict__ sums, const int64_t *__restrict__ cnts, uint64_t n,
+dec_avg_kernel(Dec128 *__restrict__ r, uint32_t *__restrict__ rnulls32, const Dec128 *__restrict__ sums, const int64_t *__restrict__ cnts, uint64_t n,
                int adj) {
     const uint64_t n64 = (n + 63) & ~63ull;
     for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n64; i += (uint64_t)gridDim.x * kThreads) {
         const bool in = i < n;
         const int64_t c = in ? cnts[i] : 0;
         if (in) {
-            const D128 s = sums[i];
+            const Dec128 s = sums[i];
             if (c == 0) r[i] = s;
             else { i128 z; dec_div(d128_get(s), (i128)c, adj, z); r[i] = d128_put(z); }
         }
@@ -513,43 +470,27 @@ dec_avg_kernel(D128 *__restrict__ r, uint32_t *__restrict__ rnulls32, const D128
     }
 }
 
-int grid_for(uint64_t len) {
-    int grid = num_sms() * 8;
-    const uint64_t work = (len + kThreads - 1) / kThreads;
-    if ((uint64_t)grid > work) grid = (int)(work ? work : 1);
-    return grid;
-}
-
 template <int W>
 int run_dec_compare(ThreadCtx &t, int op, mo_xcall_args_t *args, uint64_t len) {
-    const size_t sz = W / 8;
-    const uint64_t nwords = (len + 63) / 64;
-    const bool c1 = args[1].dataSz == sz && len > 1, c2 = args[2].dataSz == sz && len > 1;
-    if ((!c1 && args[1].dataSz < sz * len) || (!c2 && args[2].dataSz < sz * len) || args[0].dataSz < len || !args[0].pnulls) {
-        set_error("go compare: vectors shorter than len, or the result has no null bitmap"); return MO_RC_INVALID_ARGUMENT;
-    }
+    const char *what = "go compare";
+    Stager st(t);
+    uint8_t *r; uint64_t *rn;
+    Operand a, b;
+    if (int rc = stage_result(st, args[0], 1, len, true, true, what, r, rn)) return rc;
+    if (int rc = stage_operand(st, args[1], W / 8, len, what, 1, a)) return rc;
+    if (int rc = stage_operand(st, args[2], W / 8, len, what, 2, b)) return rc;
     DecParams P{0, 0, -1, 0, 0};
     if (int rc = read_param(t, args[3], &P, kDecParamsV1, kDecParamsV1, "go compare: decimal params {scale1, scale2, err_row}")) return rc;
     if (P.scale1 < 0 || P.scale2 < 0 || P.scale1 > kMaxScale<W>() || P.scale2 > kMaxScale<W>()) {
         set_error("go compare: decimal scales out of range 0..%d", kMaxScale<W>()); return MO_RC_INVALID_ARGUMENT;
     }
     const int m = P.scale2 - P.scale1;
-    Stager st(t);
-    uint8_t *r = (uint8_t *)st.out(args[0].pdata, len, true);
-    uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, true);
-    const void *a = st.in(args[1].pdata, c1 ? sz : sz * len);
-    const void *b = st.in(args[2].pdata, c2 ? sz : sz * len);
-    const uint64_t *n1 = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? (c1 ? 8 : nwords * 8) : 0);
-    const uint64_t *n2 = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? (c2 ? 8 : nwords * 8) : 0);
-    if (st.failed) return MO_RC_INTERNAL_ERROR;
-    dec_nulls_kernel<<<(unsigned)((nwords + 255) / 256 > 1024 ? 1024 : (nwords + 255) / 256), 256, 0, t.stream>>>(
-        rn, c1 ? nullptr : n1, c2 ? nullptr : n2, len, 0, c1 ? n1 : nullptr, c2 ? n2 : nullptr);
-    MOB_LAUNCH_CHECK();
+    if (int rc = merge_nulls(t, rn, len, a, b, nullptr)) return rc;   // the const null words are read on the device: no read-back
     cudaEventRecord(t.kev0, t.stream);
-    const int grid = grid_for(len), cc1 = c1 ? 1 : 0, cc2 = c2 ? 1 : 0;
-    if (m > 0) dec_cmp_kernel<W, 1><<<grid, kThreads, 0, t.stream>>>(r, a, b, len, cc1, cc2, m, op, rn);
-    else if (m < 0) dec_cmp_kernel<W, 2><<<grid, kThreads, 0, t.stream>>>(r, a, b, len, cc1, cc2, -m, op, rn);
-    else dec_cmp_kernel<W, 0><<<grid, kThreads, 0, t.stream>>>(r, a, b, len, cc1, cc2, 0, op, rn);
+    const int grid = grid_rows(len, kCtasPerSm), c1 = a.cst, c2 = b.cst;
+    if (m > 0) dec_cmp_kernel<W, 1><<<grid, kThreads, 0, t.stream>>>(r, a.data, b.data, len, c1, c2, m, op, rn);
+    else if (m < 0) dec_cmp_kernel<W, 2><<<grid, kThreads, 0, t.stream>>>(r, a.data, b.data, len, c1, c2, -m, op, rn);
+    else dec_cmp_kernel<W, 0><<<grid, kThreads, 0, t.stream>>>(r, a.data, b.data, len, c1, c2, 0, op, rn);
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
     return st.complete();
@@ -557,22 +498,20 @@ int run_dec_compare(ThreadCtx &t, int op, mo_xcall_args_t *args, uint64_t len) {
 
 template <int W>
 int run_dec_avg(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
-    const uint64_t nwords = (len + 63) / 64;
-    if (args[0].dataSz < 16 * len || !args[0].pnulls || args[1].dataSz < 16 * len || args[2].dataSz < 8 * len) {
-        set_error("decimal avg: result, sums (16 bytes per group) or counts (8 per group) shorter than len, or the result has no null bitmap");
-        return MO_RC_INVALID_ARGUMENT;
+    if (args[1].dataSz < 16 * len || args[2].dataSz < 8 * len) {
+        set_error("decimal avg: sums (16 bytes per group) or counts (8 per group) shorter than len"); return MO_RC_INVALID_ARGUMENT;
     }
     DecParams P{0, 0, -1, 0, 0};
     if (int rc = read_param(t, args[3], &P, sizeof(int32_t), kDecParamsV1, "decimal avg: params {scale1 = the argument's scale}")) return rc;
     if (P.scale1 < 0 || P.scale1 > kMaxScale<W>()) { set_error("decimal avg: scale out of range 0..%d", kMaxScale<W>()); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);
-    D128 *r = (D128 *)st.out(args[0].pdata, 16 * len, false);
-    uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, false);
-    const D128 *sums = (const D128 *)st.in(args[1].pdata, 16 * len);
+    Dec128 *r; uint64_t *rn;
+    if (int rc = stage_result(st, args[0], 16, len, false, false, "decimal avg", r, rn)) return rc;
+    const Dec128 *sums = (const Dec128 *)st.in(args[1].pdata, 16 * len);
     const int64_t *cnts = (const int64_t *)st.in(args[2].pdata, 8 * len);
     if (st.failed) return MO_RC_INTERNAL_ERROR;
     cudaEventRecord(t.kev0, t.stream);
-    dec_avg_kernel<<<grid_for((len + 63) & ~63ull), kThreads, 0, t.stream>>>(r, reinterpret_cast<uint32_t *>(rn), sums, cnts, len,
+    dec_avg_kernel<<<grid_rows((len + 63) & ~63ull, kCtasPerSm), kThreads, 0, t.stream>>>(r, reinterpret_cast<uint32_t *>(rn), sums, cnts, len,
                                                                                div_scale(P.scale1) - P.scale1);
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();

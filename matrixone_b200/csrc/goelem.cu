@@ -8,14 +8,13 @@
 //   compare                                      func_compare.go:285,677,804,931,1058,1185
 //   between                                      operator_between.go:138-199
 //   n-ary three-valued AND / OR                  logicalOperator.go:36-102, 104-168
-// whose conventions differ: rows whose result-null bit is set are skipped (the result null bitmap arrives pre-filled with
-// NOT selectList, baseTemplate.go:473-486, and leaves as rnulls | n1 | n2), the first offending row (in row order) fails the
-// call with ErrOutOfRange / ErrDivByZero, a zero divisor makes the row NULL when the session's mode says so.
+// whose operand protocol (const operands, const NULL, skipped rows, the null merge, the first failing row) is goengine.cuh's.  The
+// first offending row fails the call with ErrOutOfRange / ErrDivByZero; a zero divisor makes the row NULL when the session's mode says so.
 //
 // funcIds and argument layout: include/mo_b200.h (MO_XCALL_GO_*).  One thread per row, fully coalesced; the first offender is
 // an atomicMin over row numbers, so the error is the one the serial Go loop raises.  Rows before it hold their results, as the
 // Go loop leaves them; rows after it are unspecified (Go leaves them unwritten; the batch is discarded on error either way).
-#include "common.cuh"
+#include "goengine.cuh"
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -26,9 +25,7 @@ using namespace mob;
 
 namespace {
 
-constexpr int kThreads = 256;
 enum { OP_ADD = 0, OP_SUB, OP_MUL, OP_DIV, OP_MOD };
-constexpr unsigned long long kNoRow = ~0ull;
 
 // ---- overflow-checked scalar arithmetic (arithmetic_overflow_check.go): returns true when the row must fail -----------------
 template <typename T> __device__ __forceinline__ bool go_add(T a, T b, T &r) {
@@ -86,7 +83,7 @@ go_arith_kernel(T *__restrict__ r, const T *__restrict__ a, const T *__restrict_
         if (OP == OP_DIV || OP == OP_MOD) {
             if (y == (T)0) {
                 if (div0_null) atomicOr(reinterpret_cast<unsigned long long *>(&rnulls[i >> 6]), 1ull << (i & 63));
-                else atomicMin(first_bad, (unsigned long long)i);
+                else note_failure(first_bad, i);
                 continue;
             }
             if (OP == OP_DIV) v = (T)(x / y);                   // floats only (the host rejects integer types)
@@ -94,18 +91,11 @@ go_arith_kernel(T *__restrict__ r, const T *__restrict__ a, const T *__restrict_
         } else if (OP == OP_ADD) bad = go_add<T>(x, y, v);
         else if (OP == OP_SUB) bad = go_sub<T>(x, y, v);
         else bad = go_mul<T>(x, y, v);
-        if (bad) { atomicMin(first_bad, (unsigned long long)i); continue; }
+        if (bad) { note_failure(first_bad, i); continue; }
         r[i] = v;
     }
 }
 
-template <typename T> __device__ __forceinline__ bool go_cmp(T x, T y, int op) {
-    switch (op) {
-    case CMP_EQ: return x == y; case CMP_NE: return x != y;
-    case CMP_GT: return x > y;  case CMP_GE: return x >= y;
-    case CMP_LT: return x < y;  default: return x <= y;
-    }
-}
 // 8 consecutive rows of a column as 128-bit loads (the group never straddles a bitmap word: 8 | 64)
 template <typename T> __device__ __forceinline__ void load8(const T *p, uint64_t i0, bool cst, T *out) {
     if (cst) {
@@ -144,7 +134,7 @@ go_compare_kernel(uint8_t *__restrict__ r, const T *__restrict__ a, const T *__r
         load8<T>(a, i0, c1 != 0, x); load8<T>(b, i0, c2 != 0, y);
         uint64_t packed = 0;
 #pragma unroll
-        for (int j = 0; j < 8; j++) packed |= (uint64_t)(go_cmp<T>(round_scale<T>(x[j], pw), round_scale<T>(y[j], pw), op) ? 1 : 0) << (8 * j);
+        for (int j = 0; j < 8; j++) packed |= (uint64_t)(cmp_op<T>(round_scale<T>(x[j], pw), round_scale<T>(y[j], pw), op) ? 1 : 0) << (8 * j);
         if (nb == 0) *reinterpret_cast<uint64_t *>(r + i0) = packed;
         else {
 #pragma unroll
@@ -154,12 +144,15 @@ go_compare_kernel(uint8_t *__restrict__ r, const T *__restrict__ a, const T *__r
     // rows not covered by whole groups (all rows when the buffers are not 16-byte aligned)
     for (uint64_t i = ngroups * 8 + blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
         if (bm_test(rnulls, i)) continue;
-        r[i] = go_cmp<T>(round_scale<T>(a[c1 ? 0 : i], pw), round_scale<T>(b[c2 ? 0 : i], pw), op) ? 1 : 0;
+        r[i] = cmp_op<T>(round_scale<T>(a[c1 ? 0 : i], pw), round_scale<T>(b[c2 ? 0 : i], pw), op) ? 1 : 0;
     }
 }
 
-// rnulls |= n1 | n2 (operands that are not const), tail bits cleared; or "all rows null" (a const NULL operand)
-__global__ void go_nulls_kernel(uint64_t *rnulls, const uint64_t *n1, const uint64_t *n2, uint64_t n, int all_null) {
+// rnulls |= n1 | n2 (operands that are not const), tail bits cleared; or "all rows null" (a const NULL operand, known on the host or read
+// here from cn1 / cn2, so that a call on resident operands needs no read-back)
+__global__ void go_nulls_kernel(uint64_t *rnulls, const uint64_t *n1, const uint64_t *n2, uint64_t n, int all_null, const uint64_t *cn1,
+                                const uint64_t *cn2) {
+    if ((cn1 && (cn1[0] & 1)) || (cn2 && (cn2[0] & 1))) all_null = 1;
     const uint64_t nw = (n + 63) >> 6;
     for (uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < nw; w += (uint64_t)gridDim.x * blockDim.x) {
         uint64_t v = all_null ? ~0ull : rnulls[w];
@@ -168,12 +161,6 @@ __global__ void go_nulls_kernel(uint64_t *rnulls, const uint64_t *n1, const uint
         rnulls[w] = v;
     }
 }
-
-// a Decimal128 as stored {B0_63, B64_127}: two 8-byte words, so a column needs only 8-byte alignment; orders as a signed 128-bit value
-struct Dec128 { uint64_t lo; int64_t hi; };
-__host__ __device__ __forceinline__ bool operator<(const Dec128 &x, const Dec128 &y) { return x.hi != y.hi ? x.hi < y.hi : x.lo < y.lo; }
-__host__ __device__ __forceinline__ bool operator>=(const Dec128 &x, const Dec128 &y) { return !(x < y); }
-__host__ __device__ __forceinline__ bool operator<=(const Dec128 &x, const Dec128 &y) { return !(y < x); }
 
 // between: null input -> res = false and the null bit set; one warp covers an aligned 32-row half word of the bitmap
 template <typename T>
@@ -234,11 +221,7 @@ go_multi_logic_kernel(uint8_t *__restrict__ r, uint32_t *__restrict__ rnulls32, 
     (void)any_null_from;
 }
 
-int grid_rows(uint64_t n) {
-    uint64_t b = (n + kThreads - 1) / kThreads;
-    const uint64_t cap = (uint64_t)num_sms() * 16;
-    return (int)(b > cap ? cap : (b ? b : 1));
-}
+constexpr int kCtasPerSm = 16;
 
 const char *type_name(int T) {
     switch (T) {
@@ -258,50 +241,35 @@ struct GoParams { int32_t div0_null; int32_t pad; int64_t err_row; };
 
 template <typename T, int OP>
 int run_go_arith(ThreadCtx &t, int Tid, mo_xcall_args_t *args, uint64_t len) {
-    const uint64_t nwords = (len + 63) / 64;
-    const bool c1 = args[1].dataSz == sizeof(T) && len > 1, c2 = args[2].dataSz == sizeof(T) && len > 1;
-    if ((!c1 && args[1].dataSz < sizeof(T) * len) || (!c2 && args[2].dataSz < sizeof(T) * len) || args[0].dataSz < sizeof(T) * len || !args[0].pnulls) {
-        set_error("go arithmetic: vectors shorter than len, or the result has no null bitmap"); return MO_RC_INVALID_ARGUMENT;
-    }
+    const char *what = "go arithmetic";
+    Stager st(t);
+    T *r; uint64_t *rn;
+    Operand a, b;
+    if (int rc = stage_result(st, args[0], sizeof(T), len, true, true, what, r, rn)) return rc;
+    if (int rc = stage_operand(st, args[1], sizeof(T), len, what, 1, a)) return rc;
+    if (int rc = stage_operand(st, args[2], sizeof(T), len, what, 2, b)) return rc;
     GoParams P{0, 0, -1};
     const bool has_params = args[3].pdata && args[3].dataSz >= sizeof P;   // optional
     if (has_params) { int rc = read_param(t, args[3], &P, sizeof P, sizeof P, "go arithmetic: params"); if (rc) return rc; }
-    Stager st(t);
-    T *r = (T *)st.out(args[0].pdata, sizeof(T) * len, true);
-    uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, true);
-    const T *a = (const T *)st.in(args[1].pdata, c1 ? sizeof(T) : sizeof(T) * len);
-    const T *b = (const T *)st.in(args[2].pdata, c2 ? sizeof(T) : sizeof(T) * len);
-    const uint64_t *n1 = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? (c1 ? 8 : nwords * 8) : 0);
-    const uint64_t *n2 = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? (c2 ? 8 : nwords * 8) : 0);
-    unsigned long long *dbad = (unsigned long long *)st.tmp(16);
-    if (st.failed) return MO_RC_INTERNAL_ERROR;
-    // const NULL operand: every row is NULL (baseTemplate.go:600-700)
-    uint64_t h1 = 0, h2 = 0;
-    if (c1 && n1) { int rc = read_back(t, &h1, n1, 8); if (rc) { st.finish(); return rc; } }
-    if (c2 && n2) { int rc = read_back(t, &h2, n2, 8); if (rc) { st.finish(); return rc; } }
-    const bool all_null = (c1 && (h1 & 1)) || (c2 && (h2 & 1));
-    go_nulls_kernel<<<(unsigned)((nwords + 255) / 256 > 1024 ? 1024 : (nwords + 255) / 256), 256, 0, t.stream>>>(rn, c1 ? nullptr : n1, c2 ? nullptr : n2, len, all_null ? 1 : 0);
-    MOB_LAUNCH_CHECK();
-    unsigned long long bad = kNoRow;
+    RowRecord rec;
+    if (int rc = rec.arm(t, st)) return rc;
+    bool all_null;   // a const NULL operand: every row is NULL (baseTemplate.go:600-700)
+    if (int rc = merge_nulls(t, rn, len, a, b, &all_null)) return rc;
+    const T *pa = (const T *)a.data, *pb = (const T *)b.data;
     if (!all_null) {
-        MOB_CUDA_TRY(cudaMemsetAsync(dbad, 0xff, 8, t.stream));
         cudaEventRecord(t.kev0, t.stream);
-        go_arith_kernel<T, OP><<<grid_rows(len), kThreads, 0, t.stream>>>(r, a, b, len, c1 ? 1 : 0, c2 ? 1 : 0, rn, P.div0_null, dbad);
+        go_arith_kernel<T, OP><<<grid_rows(len, kCtasPerSm), kThreads, 0, t.stream>>>(r, pa, pb, len, a.cst, b.cst, rn, P.div0_null, rec.dev);
         cudaEventRecord(t.kev1, t.stream);
         MOB_LAUNCH_CHECK();
-        int rc = read_back(t, &bad, dbad, 8);
-        if (rc) { st.finish(); return rc; }
+        if (int rc = rec.read(t)) return rc;
     }
     T xa = 0, xb = 0;
-    if (bad != kNoRow) {   // operands of the offending row for the message (moerr.NewOutOfRange(ctx, "int64", "(%d + %d)", v1, v2))
-        read_back(t, &xa, a + (c1 ? 0 : bad), sizeof(T));
-        read_back(t, &xb, b + (c2 ? 0 : bad), sizeof(T));
+    if (rec.failed()) {   // operands of the offending row for the message (moerr.NewOutOfRange(ctx, "int64", "(%d + %d)", v1, v2))
+        read_back(t, &xa, pa + (a.cst ? 0 : rec.row()), sizeof(T));
+        read_back(t, &xb, pb + (b.cst ? 0 : rec.row()), sizeof(T));
     }
-    int frc = st.finish();
-    if (frc) return frc;
-    P.err_row = bad == kNoRow ? -1 : (int64_t)bad;
-    if (has_params) { frc = write_param(t, args[3].pdata, &P, sizeof P); if (frc) return frc; }
-    if (bad == kNoRow) return MO_RC_SUCCESS;
+    if (int rc = rec.finish(t, st, has_params ? args[3].pdata : nullptr, &P, sizeof P, P.err_row)) return rc;
+    if (!rec.failed()) return MO_RC_SUCCESS;
     if (OP == OP_DIV || OP == OP_MOD) { set_error("division by zero"); return MO_RC_DIVISION_BY_ZERO; }
     char sa[48], sb[48];
     fmt_val<T>(sa, sizeof sa, xa); fmt_val<T>(sb, sizeof sb, xb);
@@ -326,29 +294,21 @@ int go_arith_op(ThreadCtx &t, int op, int Tid, mo_xcall_args_t *args, uint64_t l
 
 template <typename T>
 int run_go_compare(ThreadCtx &t, int op, mo_xcall_args_t *args, uint64_t len, double pw = 0.0) {
-    const uint64_t nwords = (len + 63) / 64;
-    const bool c1 = args[1].dataSz == sizeof(T) && len > 1, c2 = args[2].dataSz == sizeof(T) && len > 1;
-    if ((!c1 && args[1].dataSz < sizeof(T) * len) || (!c2 && args[2].dataSz < sizeof(T) * len) || args[0].dataSz < len || !args[0].pnulls) {
-        set_error("go compare: vectors shorter than len, or the result has no null bitmap"); return MO_RC_INVALID_ARGUMENT;
-    }
+    const char *what = "go compare";
     Stager st(t);
-    uint8_t *r = (uint8_t *)st.out(args[0].pdata, len, true);
-    uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, true);
-    const T *a = (const T *)st.in(args[1].pdata, c1 ? sizeof(T) : sizeof(T) * len);
-    const T *b = (const T *)st.in(args[2].pdata, c2 ? sizeof(T) : sizeof(T) * len);
-    const uint64_t *n1 = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? (c1 ? 8 : nwords * 8) : 0);
-    const uint64_t *n2 = (const uint64_t *)st.in(args[2].pnulls, args[2].pnulls ? (c2 ? 8 : nwords * 8) : 0);
-    if (st.failed) return MO_RC_INTERNAL_ERROR;
-    uint64_t h1 = 0, h2 = 0;
-    if (c1 && n1) { int rc = read_back(t, &h1, n1, 8); if (rc) { st.finish(); return rc; } }
-    if (c2 && n2) { int rc = read_back(t, &h2, n2, 8); if (rc) { st.finish(); return rc; } }
-    const bool all_null = (c1 && (h1 & 1)) || (c2 && (h2 & 1));
-    go_nulls_kernel<<<(unsigned)((nwords + 255) / 256 > 1024 ? 1024 : (nwords + 255) / 256), 256, 0, t.stream>>>(rn, c1 ? nullptr : n1, c2 ? nullptr : n2, len, all_null ? 1 : 0);
-    MOB_LAUNCH_CHECK();
+    uint8_t *r; uint64_t *rn;
+    Operand a, b;
+    if (int rc = stage_result(st, args[0], 1, len, true, true, what, r, rn)) return rc;
+    if (int rc = stage_operand(st, args[1], sizeof(T), len, what, 1, a)) return rc;
+    if (int rc = stage_operand(st, args[2], sizeof(T), len, what, 2, b)) return rc;
+    bool all_null;   // a const NULL operand: every row is NULL (baseTemplate.go:600-700)
+    if (int rc = merge_nulls(t, rn, len, a, b, &all_null)) return rc;
     if (!all_null) {
+        const T *pa = (const T *)a.data, *pb = (const T *)b.data;
         cudaEventRecord(t.kev0, t.stream);
-        const int vec_ok = ((((uintptr_t)r) | ((uintptr_t)a) | ((uintptr_t)b)) & 15) == 0 ? 1 : 0;
-        go_compare_kernel<T><<<grid_rows(vec_ok ? (len + 7) / 8 : len), kThreads, 0, t.stream>>>(r, a, b, len, c1 ? 1 : 0, c2 ? 1 : 0, rn, op, vec_ok, pw);
+        const int vec_ok = ((((uintptr_t)r) | ((uintptr_t)pa) | ((uintptr_t)pb)) & 15) == 0 ? 1 : 0;
+        go_compare_kernel<T><<<grid_rows(vec_ok ? (len + 7) / 8 : len, kCtasPerSm), kThreads, 0, t.stream>>>(r, pa, pb, len, a.cst, b.cst, rn, op,
+                                                                                                             vec_ok, pw);
         cudaEventRecord(t.kev1, t.stream);
         MOB_LAUNCH_CHECK();
     }
@@ -357,54 +317,46 @@ int run_go_compare(ThreadCtx &t, int op, mo_xcall_args_t *args, uint64_t len, do
 
 template <typename T>
 int run_go_between(ThreadCtx &t, mo_xcall_args_t *args, uint64_t len) {
-    const uint64_t nwords = (len + 63) / 64;
-    if (args[1].dataSz < sizeof(T) * len || args[2].dataSz < sizeof(T) || args[3].dataSz < sizeof(T) || args[0].dataSz < len || !args[0].pnulls) {
-        set_error("go between: vectors shorter than len, bounds missing, or the result has no null bitmap"); return MO_RC_INVALID_ARGUMENT;
+    // the column is never const: a one-element column with len > 1 is short
+    if (args[1].dataSz < sizeof(T) * len) {
+        set_error("go between: the column holds %llu bytes, %llu needed", (unsigned long long)args[1].dataSz, (unsigned long long)(sizeof(T) * len));
+        return MO_RC_INVALID_ARGUMENT;
     }
     T lo, hi;
     if (int rc = read_param(t, args[2], &lo, sizeof lo, sizeof lo, "go between: lo")) return rc;
     if (int rc = read_param(t, args[3], &hi, sizeof hi, sizeof hi, "go between: hi")) return rc;
     Stager st(t);
-    uint8_t *r = (uint8_t *)st.out(args[0].pdata, len, false);
-    uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, true);
+    uint8_t *r; uint64_t *rn;
+    if (int rc = stage_result(st, args[0], 1, len, false, true, "go between", r, rn)) return rc;
     const T *col = (const T *)st.in(args[1].pdata, sizeof(T) * len);
-    const uint64_t *nulls = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? nwords * 8 : 0);
+    const uint64_t *nulls = (const uint64_t *)st.in(args[1].pnulls, args[1].pnulls ? ((len + 63) / 64) * 8 : 0);
     if (st.failed) return MO_RC_INTERNAL_ERROR;
     cudaEventRecord(t.kev0, t.stream);
-    go_between_kernel<T><<<grid_rows(len), kThreads, 0, t.stream>>>(r, col, lo, hi, len, nulls, reinterpret_cast<uint32_t *>(rn));
+    go_between_kernel<T><<<grid_rows(len, kCtasPerSm), kThreads, 0, t.stream>>>(r, col, lo, hi, len, nulls, reinterpret_cast<uint32_t *>(rn));
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
     return st.finish();
 }
 
 int run_go_multi_logic(ThreadCtx &t, int is_or, mo_xcall_args_t *args, uint64_t len) {
-    const uint64_t nwords = (len + 63) / 64;
+    const char *what = "go logic";
     int32_t nparams = 0;
     if (int rc = read_param(t, args[1], &nparams, 4, 4, "go logic: parameter count")) return rc;
     if (nparams < 1 || nparams > kMaxLogicParams) { set_error("go logic: 1..%d operands", kMaxLogicParams); return MO_RC_INVALID_ARGUMENT; }
-    if (args[0].dataSz < len || !args[0].pnulls) { set_error("go logic: result shorter than len, or without a null bitmap"); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);
-    uint8_t *r = (uint8_t *)st.out(args[0].pdata, len, false);
-    uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, nwords * 8, false);
+    uint8_t *r; uint64_t *rn;
+    if (int rc = stage_result(st, args[0], 1, len, false, false, what, r, rn)) return rc;
     LogicParams P; P.n = nparams;
     for (int k = 0; k < nparams; k++) {
-        const mo_xcall_args_t &a = args[2 + k];
-        const bool cst = a.dataSz == 1 && len > 1;
-        if (!cst && a.dataSz < len) { st.finish(); set_error("go logic: operand %d shorter than len", k); return MO_RC_INVALID_ARGUMENT; }
-        P.p[k].col = (const uint8_t *)st.in(a.pdata, cst ? 1 : len);
-        P.p[k].nulls = (const uint64_t *)st.in(a.pnulls, a.pnulls ? (cst ? 8 : nwords * 8) : 0);
-        P.p[k].kind = cst ? 1 : 0;
-        if (cst && P.p[k].nulls) {
-            uint64_t h = 0;
-            int rc = read_back(t, &h, P.p[k].nulls, 8);
-            if (rc) { st.finish(); return rc; }
-            if (h & 1) P.p[k].kind = 2;
-        }
+        Operand o;
+        bool is_null;
+        if (int rc = stage_operand(st, args[2 + k], 1, len, what, 2 + k, o)) return rc;
+        if (int rc = const_null(t, o.cnull(), is_null)) return rc;
+        P.p[k] = LogicParam{(const uint8_t *)o.data, o.nulls, is_null ? 2 : (o.cst ? 1 : 0)};
     }
-    if (st.failed) return MO_RC_INTERNAL_ERROR;
-    MOB_CUDA_TRY(cudaMemsetAsync(rn, 0, nwords * 8, t.stream));
+    MOB_CUDA_TRY(cudaMemsetAsync(rn, 0, ((len + 63) / 64) * 8, t.stream));
     cudaEventRecord(t.kev0, t.stream);
-    go_multi_logic_kernel<<<grid_rows(len), kThreads, 0, t.stream>>>(r, reinterpret_cast<uint32_t *>(rn), len, P, is_or, 0);
+    go_multi_logic_kernel<<<grid_rows(len, kCtasPerSm), kThreads, 0, t.stream>>>(r, reinterpret_cast<uint32_t *>(rn), len, P, is_or, 0);
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
     return st.finish();
@@ -413,6 +365,29 @@ int run_go_multi_logic(ThreadCtx &t, int is_or, mo_xcall_args_t *args, uint64_t 
 }  // namespace
 
 namespace mob {
+
+int read_const(ThreadCtx &t, void *dst, const void *p, size_t bytes) {
+    if (!bytes) return MO_RC_SUCCESS;
+    if (!is_device_ptr(p)) { memcpy(dst, p, bytes); return MO_RC_SUCCESS; }
+    if (bytes <= t.pinned_sz) return read_back(t, dst, p, bytes);
+    MOB_CUDA_TRY(cudaMemcpyAsync(dst, p, bytes, cudaMemcpyDeviceToHost, t.stream));
+    MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
+    return MO_RC_SUCCESS;
+}
+
+int merge_nulls(ThreadCtx &t, uint64_t *rnulls, uint64_t n, const Operand &a, const Operand &b, bool *all_null) {
+    bool null1 = false, null2 = false;
+    if (all_null) {
+        if (int rc = const_null(t, a.cnull(), null1)) return rc;
+        if (int rc = const_null(t, b.cnull(), null2)) return rc;
+        *all_null = null1 || null2;
+    }
+    const uint64_t blocks = ((n + 63) / 64 + 255) / 256;
+    go_nulls_kernel<<<(unsigned)(blocks > 1024 ? 1024 : blocks), 256, 0, t.stream>>>(rnulls, a.col_nulls(), b.col_nulls(), n, null1 || null2,
+                                                                                   all_null ? nullptr : a.cnull(), all_null ? nullptr : b.cnull());
+    MOB_LAUNCH_CHECK();
+    return MO_RC_SUCCESS;
+}
 
 int go_str_compare(ThreadCtx &t, int op, mo_xcall_args_t *args, uint64_t len);
 int go_dec_compare(ThreadCtx &t, int op, int T, mo_xcall_args_t *args, uint64_t len);

@@ -3,13 +3,14 @@
 //   LIKE          opBuiltInRegexp.likeFn, func_builtin_regexp.go:51-69: a const pattern that optimizeRuleForLike (:91-280) takes is
 //                 matched by its byte-level rule ("tier A"); any other pattern by regularMatchForLikeOp (:618-672), ^(?s:...)$ over runes
 //                 ("tier B"), which a wildcard-only glob matcher decides exactly: `_` is one rune, `%` any run of runes.
-// funcIds and argument layout: include/mo_b200.h (MO_XCALL_GO_COMPARE over the varlena types, MO_XCALL_GO_LIKE).
+// funcIds and argument layout: include/mo_b200.h (MO_XCALL_GO_COMPARE over the varlena types, MO_XCALL_GO_LIKE); the operand protocol:
+// goengine.cuh.
 //
 // Every launch is one grid-stride row kernel: one thread per row, so the 24-byte cells and the bool result are read and written by
 // consecutive lanes.  A warp owns 32 consecutive rows, i.e. one half word of the result null bitmap, which its ballot writes whole: rnulls
 // | n1 | n2 (a const NULL operand: every row) with no second pass.  Cells of NULL and skipped rows are never read.  A non-inline cell outside
 // its area is recorded as the lowest such row per operand in a small status record, which the call reads back -- its one synchronise.
-#include "common.cuh"
+#include "goengine.cuh"
 #include <cstdio>
 #include <string>
 #include <vector>
@@ -18,14 +19,14 @@ using namespace mob;
 
 namespace {
 
-constexpr int kThreads = 256;
+constexpr int kCtasPerSm = 16;
 constexpr uint32_t kSmemAux = 16384;   // a const pattern's literals / tokens up to this size are copied to shared memory, longer ones stay in global
 enum { LIKE_EXACT = 0, LIKE_PREFIX, LIKE_SUFFIX, LIKE_CHAIN };
 constexpr int32_t kAny1 = -1, kAnySeq = -2;   // tier-B tokens; a literal rune is its code point (>= 0)
 constexpr int32_t kRuneError = 0xFFFD;
 
-// one varlena operand as the kernels see it (cst: a const vector, every row reads cell 0)
-struct StrCol { const uint8_t *cells; const uint8_t *area; uint64_t area_sz; const uint64_t *nulls; int cst; };
+// one varlena operand as the kernels see it: the cells at data (cst: a const vector, every row reads cell 0), its area and its nulls
+using StrCol = Operand;
 
 // ~(lowest row whose cell points outside its area) per operand, 0 = none
 struct Status { unsigned long long bad_inv[2]; };
@@ -50,8 +51,8 @@ struct Str {
 // into the cell for an inline value, and reading it back byte by byte would load the cell again; here the cell is loaded once as three
 // 8-byte words and an inline value is read out of those registers (Str::at).
 __device__ __forceinline__ bool load_str(const StrCol &c, uint64_t row, Str &s) {
-    const uint8_t *cell = c.cells + 24 * (c.cst ? 0 : row);
-    if ((reinterpret_cast<uintptr_t>(c.cells) & 7) == 0) {
+    const uint8_t *cell = (const uint8_t *)c.data + 24 * (c.cst ? 0 : row);
+    if ((reinterpret_cast<uintptr_t>(c.data) & 7) == 0) {
         const uint64_t *q = reinterpret_cast<const uint64_t *>(cell);
         s.w0 = __ldg(q); s.w1 = __ldg(q + 1); s.w2 = __ldg(q + 2);
     } else {
@@ -175,8 +176,7 @@ struct CmpPred {
             const bool eq = x.len == y.len && str_cmp(x, y) == 0;
             return op == CMP_EQ ? eq : !eq;
         }
-        const int c = str_cmp(x, y);
-        switch (op) { case CMP_GT: return c > 0; case CMP_GE: return c >= 0; case CMP_LT: return c < 0; default: return c <= 0; }
+        return cmp_op(str_cmp(x, y), 0, op);
     }
 };
 // tier A: aux = u32 segment lengths [nseg] + their bytes.  EXACT: len == s + L + e and v[s, s + L) == lit ; PREFIX: v[s, s + L) == lit ;
@@ -256,28 +256,6 @@ str_row_kernel(uint8_t *__restrict__ r, uint32_t *__restrict__ rn32, uint64_t n,
     }
 }
 
-int grid_rows(uint64_t n) {
-    uint64_t b = (n + kThreads - 1) / kThreads;
-    const uint64_t cap = (uint64_t)num_sms() * 16;
-    return (int)(b > cap ? cap : (b ? b : 1));
-}
-
-// stages operand args[k] (24-byte cells + area + nulls); cst = dataSz == 24 with len != 1
-int stage_operand(Stager &st, const mo_xcall_args_t &a, uint64_t len, StrCol &c, const char *what, int k) {
-    c = StrCol{};
-    c.cst = a.dataSz == MO_VARLENA_SZ && len != 1;
-    if (!a.pdata || (!c.cst && a.dataSz < (uint64_t)MO_VARLENA_SZ * len)) {
-        set_error("%s: operand %d holds %llu bytes of cells, %llu needed", what, k, (unsigned long long)a.dataSz,
-                  (unsigned long long)(MO_VARLENA_SZ * len));
-        return MO_RC_INVALID_ARGUMENT;
-    }
-    const uint64_t rows = c.cst ? 1 : len;
-    c.cells = (const uint8_t *)st.in(a.pdata, MO_VARLENA_SZ * rows);
-    c.nulls = (const uint64_t *)st.in(a.pnulls, a.pnulls ? ((rows + 63) / 64) * 8 : 0);
-    if (a.parea && a.areaSz) { c.area = (const uint8_t *)st.in(a.parea, a.areaSz); c.area_sz = a.areaSz; }
-    return MO_RC_SUCCESS;
-}
-
 // enqueues the row kernel, reads back the status record and names the lowest bad cell
 template <class P>
 int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, const StrCol &a, const StrCol &b, const P &pred,
@@ -286,23 +264,23 @@ int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, c
     const uint32_t aux_len = (uint32_t)aux_host.size();
     if (aux_len) {
         aux = (uint8_t *)st.tmp(aux_len);
-        if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+        if (st.failed) return MO_RC_INTERNAL_ERROR;
         // pageable source: the runtime copies it into its own staging before this returns, so the vector may go out of scope
         if (cudaMemcpyAsync(aux, aux_host.data(), aux_len, cudaMemcpyHostToDevice, t.stream) != cudaSuccess) {
-            st.finish(); set_error("%s: pattern upload failed", what); return MO_RC_INTERNAL_ERROR;
+            set_error("%s: pattern upload failed", what); return MO_RC_INTERNAL_ERROR;
         }
     }
     Status *dst = (Status *)st.tmp(sizeof(Status));
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
-    if (cudaMemsetAsync(dst, 0, sizeof(Status), t.stream) != cudaSuccess) { st.finish(); set_error("%s: memset failed", what); return MO_RC_INTERNAL_ERROR; }
+    if (st.failed) return MO_RC_INTERNAL_ERROR;
+    if (cudaMemsetAsync(dst, 0, sizeof(Status), t.stream) != cudaSuccess) { set_error("%s: memset failed", what); return MO_RC_INTERNAL_ERROR; }
     const size_t smem = aux_len && aux_len <= kSmemAux ? aux_len : 0;
     cudaEventRecord(t.kev0, t.stream);
-    str_row_kernel<P><<<grid_rows(len), kThreads, smem, t.stream>>>(r, reinterpret_cast<uint32_t *>(rn), len, a, b, pred, aux, aux_len, all_null, dst);
+    str_row_kernel<P><<<grid_rows(len, kCtasPerSm), kThreads, smem, t.stream>>>(r, reinterpret_cast<uint32_t *>(rn), len, a, b, pred, aux, aux_len, all_null, dst);
     cudaEventRecord(t.kev1, t.stream);
     g_launches.fetch_add(1, std::memory_order_relaxed);
-    if (cudaError_t e = cudaGetLastError()) { st.finish(); set_error("%s: kernel launch failed: %s", what, cudaGetErrorString(e)); return MO_RC_INTERNAL_ERROR; }
+    if (cudaError_t e = cudaGetLastError()) { set_error("%s: kernel launch failed: %s", what, cudaGetErrorString(e)); return MO_RC_INTERNAL_ERROR; }
     Status hs;
-    if (int rc = read_back(t, &hs, dst, sizeof hs)) { st.finish(); return rc; }
+    if (int rc = read_back(t, &hs, dst, sizeof hs)) return rc;
     for (int k = 0; k < 2; k++) {
         if (!hs.bad_inv[k]) continue;
         int rc = st.finish();
@@ -313,39 +291,19 @@ int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, c
     return st.complete();
 }
 
-int check_result(const mo_xcall_args_t &r, uint64_t len, const char *what) {
-    if (!r.pdata || r.dataSz < len || !r.pnulls) {
-        set_error("%s: the result is shorter than len, or has no null bitmap", what);
-        return MO_RC_INVALID_ARGUMENT;
-    }
-    return MO_RC_SUCCESS;
-}
-
 // ---- LIKE, host side
-int host_copy(ThreadCtx &t, void *dst, const void *src, size_t bytes, bool dev) {
-    if (!bytes) return MO_RC_SUCCESS;
-    if (!dev) { memcpy(dst, src, bytes); return MO_RC_SUCCESS; }
-    MOB_CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, t.stream));
-    MOB_CUDA_TRY(cudaStreamSynchronize(t.stream));
-    return MO_RC_SUCCESS;
-}
-
-// the const pattern's value.  rc != 0: a bad cell (error set).  *is_null: the const NULL pattern.
+// the const pattern's value, read from the caller's memory.  rc != 0: a bad cell (error set).  *is_null: the const NULL pattern.
 int read_const_pattern(ThreadCtx &t, const mo_xcall_args_t &a, std::string &pat, bool &is_null) {
-    is_null = false;
-    if (a.pnulls) {
-        uint64_t w = 0;
-        if (int rc = host_copy(t, &w, a.pnulls, 8, is_device_ptr(a.pnulls))) return rc;
-        if (w & 1) { is_null = true; return MO_RC_SUCCESS; }
-    }
+    if (int rc = const_null(t, (const uint64_t *)a.pnulls, is_null)) return rc;
+    if (is_null) return MO_RC_SUCCESS;
     uint8_t cell[MO_VARLENA_SZ];
-    if (int rc = host_copy(t, cell, a.pdata, MO_VARLENA_SZ, is_device_ptr(a.pdata))) return rc;
+    if (int rc = read_const(t, cell, a.pdata, MO_VARLENA_SZ)) return rc;
     if (cell[0] <= MO_VARLENA_INLINE_SZ) { pat.assign((const char *)cell + 1, cell[0]); return MO_RC_SUCCESS; }
     uint32_t off, len;
     memcpy(&off, cell + 4, 4); memcpy(&len, cell + 8, 4);
     if (!a.parea || (uint64_t)off + len > a.areaSz) { set_error("go like: operand 2 row 0: varlena cell outside its area"); return MO_RC_INVALID_ARGUMENT; }
     pat.resize(len);
-    return host_copy(t, &pat[0], a.parea + off, len, is_device_ptr(a.parea));
+    return read_const(t, &pat[0], a.parea + off, len);
 }
 
 // functionUtil.RemoveEscapeChar: `\x` -> x; a trailing lone backslash is kept
@@ -426,14 +384,12 @@ namespace mob {
 // MO_XCALL_GO_COMPARE(op, T) for the varlena types (goelem.cu routes them here)
 int go_str_compare(ThreadCtx &t, int op, mo_xcall_args_t *args, uint64_t len) {
     const char *what = "go compare";
-    if (int rc = check_result(args[0], len, what)) return rc;
     Stager st(t);
-    uint8_t *r = (uint8_t *)st.out(args[0].pdata, len, true);
-    uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, ((len + 63) / 64) * 8, true);
-    StrCol a, b;
-    if (int rc = stage_operand(st, args[1], len, a, what, 1)) { st.finish(); return rc; }
-    if (int rc = stage_operand(st, args[2], len, b, what, 2)) { st.finish(); return rc; }
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
+    uint8_t *r; uint64_t *rn;
+    Operand a, b;
+    if (int rc = stage_result(st, args[0], 1, len, true, true, what, r, rn)) return rc;
+    if (int rc = stage_operand(st, args[1], MO_VARLENA_SZ, len, what, 1, a)) return rc;
+    if (int rc = stage_operand(st, args[2], MO_VARLENA_SZ, len, what, 2, b)) return rc;
     return run_rows(t, st, r, rn, len, a, b, CmpPred{op}, std::vector<uint8_t>(), 0, what);
 }
 
@@ -443,22 +399,20 @@ int xcall_go_like(mo_xcall_args_t *args, uint64_t len) {
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     if (len == 0) return MO_RC_SUCCESS;
     const char *what = "go like";
-    if (int rc = check_result(args[0], len, what)) return rc;
-    const bool pat_const = args[2].dataSz == MO_VARLENA_SZ && len != 1;
+    Stager st(t);
+    uint8_t *r; uint64_t *rn;
+    Operand a, b;
+    if (int rc = stage_result(st, args[0], 1, len, true, true, what, r, rn)) return rc;
+    if (int rc = stage_operand(st, args[1], MO_VARLENA_SZ, len, what, 1, a)) return rc;
+    if (!is_const(args[2], MO_VARLENA_SZ, len)) {
+        if (int rc = stage_operand(st, args[2], MO_VARLENA_SZ, len, what, 2, b)) return rc;
+        return run_rows(t, st, r, rn, len, a, b, LikeBColPred{}, std::vector<uint8_t>(), 0, what);
+    }
+    // a const pattern is read on the host, from the caller's memory
     std::string pat;
     bool pat_null = false;
-    if (pat_const) {
-        if (!args[2].pdata) { set_error("go like: operand 2 has no cells"); return MO_RC_INVALID_ARGUMENT; }
-        if (int rc = read_const_pattern(t, args[2], pat, pat_null)) return rc;
-    }
-    Stager st(t);
-    uint8_t *r = (uint8_t *)st.out(args[0].pdata, len, true);
-    uint64_t *rn = (uint64_t *)st.out(args[0].pnulls, ((len + 63) / 64) * 8, true);
-    StrCol a, b{};
-    if (int rc = stage_operand(st, args[1], len, a, what, 1)) { st.finish(); return rc; }
-    if (!pat_const) { if (int rc = stage_operand(st, args[2], len, b, what, 2)) { st.finish(); return rc; } }
-    if (st.failed) { st.finish(); return MO_RC_INTERNAL_ERROR; }
-    if (!pat_const) return run_rows(t, st, r, rn, len, a, b, LikeBColPred{}, std::vector<uint8_t>(), 0, what);
+    if (!args[2].pdata) { set_error("go like: operand 2 has no cells"); return MO_RC_INVALID_ARGUMENT; }
+    if (int rc = read_const_pattern(t, args[2], pat, pat_null)) return rc;
     if (pat_null) return run_rows(t, st, r, rn, len, a, b, LikeBColPred{}, std::vector<uint8_t>(), 1, what);   // every row NULL
     int mode;
     uint32_t s, e;

@@ -53,11 +53,11 @@ def _operands(rng, dt, n, op):
 
 @pytest.mark.parametrize("T", sorted(TYPES))
 @pytest.mark.parametrize("op", [0, 1, 2, 3, 4])
-@pytest.mark.parametrize("shape", ["vv", "vc", "cv"])
+@pytest.mark.parametrize("shape", ["vv", "vc", "cv", "cnull", "nullc"])
 @pytest.mark.parametrize("case", ["clean", "offender", "div0_null"])
 def test_go_arithmetic_matches_oracle(gpu, T, op, shape, case):
     dt = TYPES[T]
-    rng = np.random.default_rng(T * 1000 + op * 100 + ["vv", "vc", "cv"].index(shape) * 10 + ["clean", "offender", "div0_null"].index(case))
+    rng = np.random.default_rng(T * 1000 + op * 100 + ["vv", "vc", "cv", "cnull", "nullc"].index(shape) * 10 + ["clean", "offender", "div0_null"].index(case))
     n = N
     a, b = _operands(rng, dt, n, op)
     if case != "div0_null" and op in (3, 4):
@@ -73,13 +73,13 @@ def test_go_arithmetic_matches_oracle(gpu, T, op, shape, case):
     if case == "offender" and np.issubdtype(dt, np.floating) and op in (0, 1):
         rows = rng.choice(n, 2, replace=False)
         a[rows] = np.finfo(dt).max; b[rows] = np.finfo(dt).max if op == 0 else -np.finfo(dt).max
-    c1, c2 = shape == "cv", shape == "vc"
+    c1, c2 = shape in ("cv", "nullc"), shape in ("vc", "cnull")   # cnull / nullc: a const NULL b / a nulls every row
     if c1: a = a[:1].copy()
     if c2:
         b = b[:1].copy()
         if case == "clean" and op in (3, 4) and b[0] == 0: b[0] = 3
-    n1 = None if c1 else _rand_nulls(rng, n, 0.05)
-    n2 = None if c2 else _rand_nulls(rng, n, 0.05)
+    n1 = np.array([1], dtype=np.uint64) if shape == "nullc" else (None if c1 else _rand_nulls(rng, n, 0.05))
+    n2 = np.array([1], dtype=np.uint64) if shape == "cnull" else (None if c2 else _rand_nulls(rng, n, 0.05))
     sel = _rand_nulls(rng, n, 0.1)                    # NOT selectList, pre-filled by the caller
     div0_null = 1 if case == "div0_null" else 0
     # oracle
@@ -91,13 +91,15 @@ def test_go_arithmetic_matches_oracle(gpu, T, op, shape, case):
     params = np.zeros(2, dtype=np.int64); params.view(np.int32)[0] = div0_null; params[1] = -1
     rc1, msg = xcall(capi.XCALL_GO_ARITH(op, T), [Vector(data=r1, nulls=rn1, length=n), Vector(data=a, nulls=n1, length=n),
                                                     Vector(data=b, nulls=n2, length=n), Vector(data=params.view(np.uint8), length=n)], n, raise_on_error=False)
-    assert rc1 == rc0, (rc1, rc0, msg)
     if op == 3 and not np.issubdtype(dt, np.floating):
         # "/" is defined on floats only (arithmetic.go:481-514): the oracle and the library both refuse integer operands, and the
-        # library leaves the result, its nulls and the offending-row slot untouched
-        assert rc0 == capi.RC_INVALID_ARGUMENT and "not defined" in msg, (rc0, msg)
+        # library leaves the result, its nulls and the offending-row slot untouched.  The library refuses the type before it looks at
+        # the operands, so a const NULL operand does not change that; the oracle nulls every row first.
+        assert rc1 == capi.RC_INVALID_ARGUMENT and "not defined" in msg, (rc1, msg)
+        assert rc0 == (0 if shape in ("cnull", "nullc") else capi.RC_INVALID_ARGUMENT), rc0
         assert (r1 == 77).all() and (rn1 == sel).all() and params[1] == -1
         return
+    assert rc1 == rc0, (rc1, rc0, msg)
     if rc0 == 0:
         assert params[1] == -1
         assert (rn1 == rn0).all()

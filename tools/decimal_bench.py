@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Decimal comparisons, division and AVG on resident columns, one GPU, one process.
 
-    python tools/decimal_bench.py [--rows N] [--runs R] [--out FILE]
+    python tools/decimal_bench.py [--rows N] [--runs R] [--parent-lib PATH] [--out FILE]
 
 Shapes, over --rows rows (default 10^8) of device-generated values: the int64 compare a > b and the decimal64 compare on the same bytes at
 equal scales (2, 2) and at unequal scales (2, 4: every left value is scaled up), the decimal128 compare at (2, 2), DIV at scales (2, 2) for
@@ -10,6 +10,8 @@ estimate-and-correct path), and DEC_AVG over --rows groups.  Every call is the a
 kernel_ms is the library's CUDA events around the call's kernel (MoB200_LastKernelMs), a median of --runs runs alternating over the
 shapes after one warm-up of each.  bytes = the operand bytes read + the result bytes written (bitmaps excluded); GB/s = bytes over
 kernel_ms, next to the H100 SXM data-sheet HBM3 peak of 3.35 TB/s.  The card's name and power limit are read in the same call.
+--parent-lib loads a second build of libmo_b200.so (another commit) and times every shape on it too (parent_*), alternating with this build
+call by call, so that both see the same card state.
 """
 import argparse
 import ctypes as C
@@ -50,12 +52,16 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=100_000_000)
     ap.add_argument("--runs", type=int, default=7)
+    ap.add_argument("--parent-lib", default=None)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("decimal_bench: no CUDA device (the measurement needs the H100)")
-    lib = capi.load_library()
-    capi.check(lib.MoB200_Init(0), lib)
+    libs = {"": capi.load_library()}
+    if a.parent_lib:
+        libs["parent_"] = capi.load_library(a.parent_lib)
+    for lib in libs.values():
+        capi.check(lib.MoB200_Init(0), lib)
     name, power = card()
     n = a.rows
     g = torch.Generator(device="cuda").manual_seed(1)
@@ -80,20 +86,20 @@ def main():
     torch.cuda.synchronize()
 
     def cmp_call(fid, x, y, extra):
-        def f():
+        def f(lib):
             rn.zero_()
-            xcall(fid, [dvec(res8, n, rn), dvec(x, n), dvec(y, n)] + extra, n)
+            xcall(fid, [dvec(res8, n, rn), dvec(x, n), dvec(y, n)] + extra, n, lib=lib)
         return f
 
     def div_call(width, x, y):
-        def f():
+        def f(lib):
             rn.zero_()
             xcall(capi.XCALL_DEC_ARITH(capi.DEC_OP_DIV, width), [dvec(res16, n, rn), dvec(x, n), dvec(y, n),
-                                                                 params(capi.DecDivParams(2, 2, -1, 0, 0))], n)
+                                                                 params(capi.DecDivParams(2, 2, -1, 0, 0))], n, lib=lib)
         return f
 
-    def avg_call():
-        xcall(capi.XCALL_DEC_AVG(64), [dvec(res16, n, rn), dvec(d128a, n), dvec(cnts, n), params(capi.DecParams(2, 0, -1))], n)
+    def avg_call(lib):
+        xcall(capi.XCALL_DEC_AVG(64), [dvec(res16, n, rn), dvec(d128a, n), dvec(cnts, n), params(capi.DecParams(2, 0, -1))], n, lib=lib)
 
     shapes = [
         ("int64 compare a > b", cmp_call(capi.XCALL_GO_COMPARE(capi.CMP_GT, capi.T_INT64), i64a, i64b, []), 8 + 8 + 1),
@@ -108,22 +114,24 @@ def main():
         ("decimal128 div, 128-bit divisor", div_call(128, big_x, big_y), 16 + 16 + 16),
         ("DEC_AVG", avg_call, 16 + 8 + 16),
     ]
-    times = {s[0]: [] for s in shapes}
+    times = {p + s[0]: [] for s in shapes for p in libs}
 
-    def run(f):
-        f()
+    def run(lib, f):
+        f(lib)
         capi.check(lib.MoB200_Sync(), lib)
         ms = C.c_float()
         capi.check(lib.MoB200_LastKernelMs(C.byref(ms)), lib)
         return ms.value
 
     for _, f, _ in shapes:
-        run(f)
+        for lib in libs.values():
+            run(lib, f)
     for _ in range(a.runs):
         for label, f, _ in shapes:
-            times[label].append(run(f))
+            for p, lib in libs.items():
+                times[p + label].append(run(lib, f))
     res = {"card": name, "power_limit": power, "rows": n, "runs": a.runs, "hbm_peak_gbps": HBM_PEAK_BPS / 1e9, "shapes": {}}
-    for label, _, per_row in shapes:
+    for label, per_row in ((p + s[0], s[2]) for s in shapes for p in libs):
         k = statistics.median(times[label])
         nbytes = per_row * n
         res["shapes"][label] = {"kernel_ms": round(k, 3), "g_rows_per_s": round(n / (k * 1e-3) / 1e9, 2), "bytes": nbytes,

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """String predicates on resident columns: GO_LIKE and GO_COMPARE over varlena columns in the TPC-H shapes, one GPU, one process.
 
-    python tools/strpred_bench.py [--rows N] [--runs R] [--chunk C] [--out FILE]
+    python tools/strpred_bench.py [--rows N] [--runs R] [--chunk C] [--parent-lib PATH] [--out FILE]
 
 Shapes, over --rows rows (default 10^8) of generated values in the TPC-H formats: p_type LIKE 'PROMO%' (Q14), p_type LIKE '%BRASS' (Q2),
 p_name LIKE '%green%' (Q9), o_comment NOT LIKE '%special%requests%' (Q13's wording; NOT is the negation of the same kernel's result), the
@@ -11,6 +11,8 @@ chunk, asynchronous form, const pattern in host memory.  kernel_ms sums the libr
 call_ms is the whole run between events on the library's stream, the per-call status read-back included.  Both are medians of --runs runs,
 alternating over the shapes.  bytes = cells (24 per row) + the area bytes of the non-inline values + the bool result; GB/s = bytes over
 kernel_ms, next to the H100 SXM data-sheet HBM3 peak of 3.35 TB/s.  The card's name and power limit are read in the same call.
+--parent-lib loads a second build of libmo_b200.so (another commit) and times every shape on it too (parent_*), alternating with this build
+run by run, so that both see the same card state.
 """
 import argparse
 import ctypes as C
@@ -101,8 +103,9 @@ class Chunk:
         return Vector(data_ptr=self.cells.data_ptr(), data_nbytes=24 * self.n, length=self.n,
                       area_ptr=None if a is None else a.data_ptr(), area_nbytes=0 if a is None else a.numel())
 
-    def call(self, fid, const):
-        xcall(fid, [Vector(data_ptr=self.out.data_ptr(), data_nbytes=self.n, nulls_ptr=self.outn.data_ptr(), length=self.n), self.vec(), const], self.n)
+    def call(self, lib, fid, const):
+        xcall(fid, [Vector(data_ptr=self.out.data_ptr(), data_nbytes=self.n, nulls_ptr=self.outn.data_ptr(), length=self.n), self.vec(), const], self.n,
+              lib=lib)
 
 
 def const_vec(value):
@@ -115,12 +118,16 @@ def main():
     ap.add_argument("--rows", type=int, default=100_000_000)
     ap.add_argument("--runs", type=int, default=5)
     ap.add_argument("--chunk", type=int, default=1 << 24)
+    ap.add_argument("--parent-lib", default=None)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("strpred_bench: no CUDA device (the measurement needs the H100)")
-    lib = capi.load_library()
-    capi.check(lib.MoB200_Init(0), lib)
+    libs = {"": capi.load_library()}
+    if a.parent_lib:
+        libs["parent_"] = capi.load_library(a.parent_lib)
+    for lib in libs.values():
+        capi.check(lib.MoB200_Init(0), lib)
     name, power = card()
     rng = np.random.default_rng(1)
     g = torch.Generator(device="cuda").manual_seed(1)
@@ -142,15 +149,15 @@ def main():
               ("o_comment LIKE '%a_b%' (rune level)", "o_comment", capi.XCALL_GO_LIKE, b"%a_b%"),
               ("l_shipmode = 'MAIL'", "l_shipmode", capi.XCALL_GO_COMPARE(capi.CMP_EQ, capi.T_CHAR), b"MAIL"),
               ("p_brand <> 'Brand#45'", "p_brand", capi.XCALL_GO_COMPARE(capi.CMP_NE, capi.T_CHAR), b"Brand#45")]
-    times = {s[0]: ([], []) for s in shapes}
+    times = {p + s[0]: ([], []) for s in shapes for p in libs}
 
-    def run(shape):
+    def run(shape, lib=libs[""]):
         label, kind, fid, value = shape
         cv = const_vec(value)
         kms = 0.0
         capi.check(lib.MoB200_TimerStart(), lib)
         for ch in cols[kind]:
-            ch.call(fid, cv)
+            ch.call(lib, fid, cv)
             ms = C.c_float()
             capi.check(lib.MoB200_LastKernelMs(C.byref(ms)), lib)
             kms += ms.value
@@ -159,22 +166,25 @@ def main():
         return kms, tot.value
 
     for s in shapes:                                   # warm-up of every shape
-        run(s)
+        for lib in libs.values():
+            run(s, lib)
     for _ in range(a.runs):
         for s in shapes:
-            k, t = run(s)
-            times[s[0]][0].append(k)
-            times[s[0]][1].append(t)
+            for p, lib in libs.items():
+                k, t = run(s, lib)
+                times[p + s[0]][0].append(k)
+                times[p + s[0]][1].append(t)
     hits = {}
     for s in shapes:                                   # the rows each shape's LIKE / compare admits (a column's chunks share one result buffer)
         run(s)
         hits[s[0]] = sum(int(ch.out.sum()) for ch in cols[s[1]])
     res = {"card": name, "power_limit": power, "rows": a.rows, "chunk": a.chunk, "runs": a.runs, "hbm_peak_gbps": HBM_PEAK_BPS / 1e9, "shapes": {}}
-    for label, kind, fid, value in shapes:
-        k, t = statistics.median(times[label][0]), statistics.median(times[label][1])
+    for (label, kind, fid, value), p in ((s, p) for s in shapes for p in libs):
+        k, t = statistics.median(times[p + label][0]), statistics.median(times[p + label][1])
         nbytes = sum(24 * ch.n + ch.area_read + ch.n for ch in cols[kind])
-        res["shapes"][label] = {"kernel_ms": round(k, 3), "call_ms": round(t, 3), "bytes": nbytes, "gbps": round(nbytes / (k * 1e-3) / 1e9, 1),
-                                "share_of_hbm_peak": round(nbytes / (k * 1e-3) / HBM_PEAK_BPS, 3), "matches": hits[label]}
+        res["shapes"][p + label] = {"kernel_ms": round(k, 3), "call_ms": round(t, 3), "bytes": nbytes, "gbps": round(nbytes / (k * 1e-3) / 1e9, 1),
+                                    "share_of_hbm_peak": round(nbytes / (k * 1e-3) / HBM_PEAK_BPS, 3), "spread_ms": [round(min(times[p + label][0]), 3),
+                                    round(max(times[p + label][0]), 3)], "matches": hits[label]}
     line = json.dumps(res)
     print(line)
     if a.out:
