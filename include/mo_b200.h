@@ -260,6 +260,28 @@ typedef struct { int32_t div0_null; int32_t reserved; int64_t err_row; } mo_go_p
  * reads back one small status record (the bad-cell check), which synchronises the calling thread's stream once; a const pattern is read on
  * the host before that (a device one is copied back first, as a device parameter block is). */
 #define MO_XCALL_GO_LIKE 0x5800
+/* ---- list membership: x IN (v1, ..., vm) and x NOT IN (...), operator_in.go (overloads list_operator.go:541-808 and :1094-), the GO
+ * conventions above.  Fixed-width T in csrc/goelem.cu, the varlena T in csrc/strpred.cu.
+ *   IN(T) / NOT_IN(T)  args: [0] result bool[len] + pnulls (in/out) ; [1] the column (+ pnulls; a const is one element) ; [2] the list:
+ *                      nvalues elements (+ pnulls; the varlena types: 24-byte cells + area) ; [3] mo_in_params_t (required, host or device).
+ *   T = UINT8..64, INT8..64, FLOAT32 / 64, DECIMAL64 / 128, DATE, TIME, DATETIME, TIMESTAMP, BOOL, UUID, YEAR (int16), CHAR, VARCHAR, TEXT,
+ *       BLOB, BINARY, VARBINARY.  Any other T is refused.
+ *   The set is Go's map[T]bool or map[string]bool of the list (op.init): NULL elements are skipped, so a const NULL or all-NULL list is the
+ *   empty set.  Equality is Go map equality: the raw value's bits (+0.0 and -0.0 are one key; a NaN is never found, so a NaN row is IN-false
+ *   and NOT-IN-true; decimals and UUIDs compare raw, unscaled -- the planner casts the list to the column's type), and bytes for the strings
+ *   (no trimming, no collation).  A NULL row is NULL; every other row is `found` (IN) or `!found` (NOT IN) with a clear null bit, so a NULL in
+ *   the list never nulls a row: 2 NOT IN (1, NULL) is true.  A const NULL column nulls every row.  Rows whose result null bit is set on entry
+ *   are skipped; on return the bitmap holds rnulls | the column's nulls (a const NULL column: every row), the bits past len cleared.
+ *   The set is built per call into a hash table in the calling thread's scratch: 8-byte-or-narrower values keyed on their bits, 16-byte
+ *   values (DECIMAL128, UUID) and strings as a hash tag and a list index.  Launches: nvalues == 0, or a host list whose nvalues elements
+ *   are all NULL -> the probe only (1 kernel); else the build and the probe (2 kernels; a device list's NULL elements are skipped by the
+ *   build, whose launch does not depend on them).  Fixed-width T with device operands and a host block only enqueue work; the varlena T read back one
+ *   status record, as GO_LIKE does, and a non-inline cell outside its area, in the column or in a non-NULL list element, fails the call
+ *   with MO_RC_INVALID_ARGUMENT naming the operand and its lowest such row.  A negative nvalues or one above 2^31 - 1, a list shorter than
+ *   nvalues elements and a missing block are refused with MO_RC_INVALID_ARGUMENT. */
+typedef struct mo_in_params_t { int64_t nvalues; } mo_in_params_t;
+#define MO_XCALL_GO_IN(T) (0x5900 + (T))
+#define MO_XCALL_GO_NOT_IN(T) (0x5A00 + (T))
 
 /* ---- the standalone column operators of the colexec pipeline (csrc/colops.cu).  Host or device pointers; when every data pointer and
  * nulls bitmap of every vector is a device pointer (or NULL) FILTER_SELS and SHUFFLE only enqueue work (asynchronous form, as

@@ -130,6 +130,16 @@ def XCALL_GO_BETWEEN(T):
 
 XCALL_GO_MULTI_AND, XCALL_GO_MULTI_OR = 0x5100, 0x5101
 XCALL_GO_LIKE = 0x5800
+
+
+def XCALL_GO_IN(T):
+    return 0x5900 + T
+
+
+def XCALL_GO_NOT_IN(T):
+    return 0x5A00 + T
+
+
 CMP_EQ, CMP_NE, CMP_GT, CMP_GE, CMP_LT, CMP_LE = 0, 1, 2, 3, 4, 5
 Q1_MAX_GROUPS = 8
 

@@ -15,6 +15,8 @@
 // an atomicMin over row numbers, so the error is the one the serial Go loop raises.  Rows before it hold their results, as the
 // Go loop leaves them; rows after it are unspecified (Go leaves them unwritten; the batch is discarded on error either way).
 #include "goengine.cuh"
+#include "keytable.cuh"
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -362,6 +364,145 @@ int run_go_multi_logic(ThreadCtx &t, int is_or, mo_xcall_args_t *args, uint64_t 
     return st.finish();
 }
 
+// ---- IN / NOT IN over fixed-width values (operator_in.go, opOperatorFixedIn): Go's map[T]bool of the list, as a keytable.cuh table.
+// Values of 8 bytes or fewer are keyed on their bits (kt_insert / kt_find): mask + 2 key slots, then one word that is 1 when the all-ones
+// key is in the set (that key owns slot mask + 1, which kt_find reports as found whether it was inserted or not).  16-byte values (DECIMAL128,
+// UUID) are kt_insert_str words, an XXH3 tag and the list index of the value, compared as two 8-byte words: mask + 1 slots.
+struct V16 { uint64_t lo, hi; };
+
+// the key of a value; false for a NaN, which no Go map lookup finds.  -0.0 is keyed as +0.0 (they are one key of a Go map).
+template <typename T> __device__ __forceinline__ bool in_key(T v, uint64_t &key) {
+    if constexpr (std::is_floating_point<T>::value) {
+        if (v != v) return false;
+        if (v == (T)0) v = (T)0;
+    }
+    key = 0;
+    memcpy(&key, &v, sizeof(T));
+    return true;
+}
+__device__ __forceinline__ uint64_t v16_hash(V16 v) { return xxh3::hash_bytes(reinterpret_cast<const uint8_t *>(&v), 16, 0).lo; }
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) go_in_build_kernel(uint64_t *keys, uint64_t mask, const T *__restrict__ vals,
+                                                               const uint64_t *__restrict__ vnulls, uint64_t m) {
+    for (uint64_t j = blockIdx.x * (uint64_t)kThreads + threadIdx.x; j < m; j += (uint64_t)gridDim.x * kThreads) {
+        uint64_t key, slot;
+        if (bm_test(vnulls, j) || !in_key(vals[j], key)) continue;
+        if (key == kEmptyKey) keys[mask + 2] = 1;
+        else kt_insert(keys, mask, key, slot);
+    }
+}
+__global__ void __launch_bounds__(kThreads) go_in_build16_kernel(uint64_t *slots, uint64_t mask, const V16 *__restrict__ vals,
+                                                                 const uint64_t *__restrict__ vnulls, uint64_t m) {
+    for (uint64_t j = blockIdx.x * (uint64_t)kThreads + threadIdx.x; j < m; j += (uint64_t)gridDim.x * kThreads) {
+        if (bm_test(vnulls, j)) continue;
+        const V16 v = vals[j];
+        const uint64_t h = v16_hash(v);
+        kt_insert_str(slots, mask, h, str_word(h, j), [&](uint32_t r) { const V16 w = vals[r]; return w.lo == v.lo && w.hi == v.hi; });
+    }
+}
+
+// the probe's view of the set; words == 0: the empty set.  stage() copies the table into shared memory when it fits kInSmemBytes.
+struct InTable {
+    const uint64_t *t; uint64_t mask, words;
+    __device__ __forceinline__ void stage(uint64_t *sm) {
+        if (!words || words * 8 > kInSmemBytes) return;
+        for (uint64_t k = threadIdx.x; k < words; k += kThreads) sm[k] = t[k];
+        __syncthreads();
+        t = sm;
+    }
+};
+struct NarrowSet {
+    InTable tab;
+    template <typename T> __device__ __forceinline__ bool has(T v) const {
+        uint64_t key, slot;
+        if (!tab.words || !in_key(v, key)) return false;
+        return key == kEmptyKey ? tab.t[tab.mask + 2] != 0 : kt_find(tab.t, tab.mask, key, slot);
+    }
+};
+struct WideSet {
+    InTable tab; const V16 *vals;
+    __device__ __forceinline__ bool has(V16 v) const {
+        uint32_t row;
+        if (!tab.words) return false;
+        return kt_find_str(tab.t, tab.mask, v16_hash(v), [&](uint32_t r) { const V16 w = vals[r]; return w.lo == v.lo && w.hi == v.hi; }, row);
+    }
+};
+
+// a thread owns 8 consecutive rows, i.e. one byte of the result bitmap, which it writes whole: rnulls | the column's nulls (a const NULL column:
+// every row), bits past n cleared.  The loop covers every byte of the last bitmap word.  Rows null on exit are not written.
+template <typename T, class Set>
+__global__ void __launch_bounds__(kThreads)
+go_in_kernel(uint8_t *__restrict__ r, uint8_t *__restrict__ rn8, const T *__restrict__ col, const uint8_t *__restrict__ cn8, int cst,
+             uint64_t n, Set set, int negate, int vec_ok) {
+    extern __shared__ uint64_t sm_table[];
+    set.tab.stage(sm_table);
+    const bool cnull = cst && cn8 && (cn8[0] & 1);
+    const uint64_t nbytes = ((n + 63) >> 6) * 8;
+    for (uint64_t g = blockIdx.x * (uint64_t)kThreads + threadIdx.x; g < nbytes; g += (uint64_t)gridDim.x * kThreads) {
+        const uint64_t i0 = g * 8;
+        const unsigned valid = i0 >= n ? 0u : (n - i0 >= 8 ? 0xffu : (1u << (n - i0)) - 1);
+        unsigned nb = cnull ? 0xffu : rn8[g] | (!cst && cn8 ? cn8[g] : 0u);
+        nb &= valid;
+        rn8[g] = (uint8_t)nb;
+        if (nb == valid) continue;
+        if (vec_ok && valid == 0xffu) {
+            T x[8];
+            load8<T>(col, i0, cst != 0, x);
+            uint64_t packed = 0;
+#pragma unroll
+            for (int j = 0; j < 8; j++) packed |= (uint64_t)(set.has(x[j]) ? 1 ^ negate : negate) << (8 * j);
+            if (nb == 0) { *reinterpret_cast<uint64_t *>(r + i0) = packed; continue; }
+#pragma unroll
+            for (int j = 0; j < 8; j++) if (!((nb >> j) & 1u)) r[i0 + j] = (uint8_t)(packed >> (8 * j));
+            continue;
+        }
+        for (int j = 0; j < 8; j++)
+            if (((valid & ~nb) >> j) & 1u) r[i0 + j] = (uint8_t)(set.has(col[cst ? 0 : i0 + j]) ? 1 ^ negate : negate);
+    }
+}
+
+// launches: the build (nvalues > 0), then the probe.  Every pointer a device one and a host block: enqueue only.
+template <typename T>
+int run_go_in(ThreadCtx &t, int negate, mo_xcall_args_t *args, uint64_t len) {
+    const char *what = negate ? "go not in" : "go in";
+    constexpr bool wide = sizeof(T) == 16;
+    Stager st(t);
+    uint8_t *r; uint64_t *rn;
+    Operand a, l;
+    uint64_t m, mask;
+    if (int rc = stage_result(st, args[0], 1, len, true, true, what, r, rn)) return rc;
+    if (int rc = stage_operand(st, args[1], sizeof(T), len, what, 1, a)) return rc;
+    if (int rc = stage_in_list(t, st, args, sizeof(T), what, l, m, mask)) return rc;
+    InTable tab{nullptr, mask, 0};
+    if (m) {
+        tab.words = wide ? mask + 1 : mask + 3;
+        uint64_t *keys = (uint64_t *)st.tmp(tab.words * 8);
+        if (st.failed) return MO_RC_INTERNAL_ERROR;
+        MOB_CUDA_TRY(cudaMemsetAsync(keys, 0xff, tab.words * 8, t.stream));
+        if (!wide) MOB_CUDA_TRY(cudaMemsetAsync(keys + mask + 2, 0, 8, t.stream));
+        if constexpr (wide) go_in_build16_kernel<<<grid_rows(m, kCtasPerSm), kThreads, 0, t.stream>>>(keys, mask, (const V16 *)l.data, l.nulls, m);
+        else go_in_build_kernel<T><<<grid_rows(m, kCtasPerSm), kThreads, 0, t.stream>>>(keys, mask, (const T *)l.data, l.nulls, m);
+        MOB_LAUNCH_CHECK();
+        tab.t = keys;
+    }
+    const bool smem = tab.words && tab.words * 8 <= kInSmemBytes;
+    // every CTA copies the table: fewer, longer-lived CTAs when it is large (about 64 KB of copies per SM)
+    const int ctas = smem ? (int)std::max<uint64_t>(2, std::min<uint64_t>(kCtasPerSm, 65536 / (tab.words * 8))) : kCtasPerSm;
+    const int vec_ok = ((((uintptr_t)r) | ((uintptr_t)a.data)) & 15) == 0 ? 1 : 0;
+    const uint64_t nbytes = ((len + 63) / 64) * 8;
+    cudaEventRecord(t.kev0, t.stream);
+    if constexpr (wide)
+        go_in_kernel<V16, WideSet><<<grid_rows(nbytes, ctas), kThreads, smem ? tab.words * 8 : 0, t.stream>>>(
+            r, (uint8_t *)rn, (const V16 *)a.data, (const uint8_t *)a.nulls, a.cst, len, WideSet{tab, (const V16 *)l.data}, negate, vec_ok);
+    else
+        go_in_kernel<T, NarrowSet><<<grid_rows(nbytes, ctas), kThreads, smem ? tab.words * 8 : 0, t.stream>>>(
+            r, (uint8_t *)rn, (const T *)a.data, (const uint8_t *)a.nulls, a.cst, len, NarrowSet{tab}, negate, vec_ok);
+    cudaEventRecord(t.kev1, t.stream);
+    MOB_LAUNCH_CHECK();
+    return st.complete();
+}
+
 }  // namespace
 
 namespace mob {
@@ -463,6 +604,29 @@ int xcall_go_elementwise(int64_t funcId, mo_xcall_args_t *args, uint64_t len) {
     }
     if (funcId == 0x5100 || funcId == 0x5101) return run_go_multi_logic(t, (int)(funcId & 1), args, len);
     return -1;
+}
+
+int go_str_in(ThreadCtx &t, int negate, mo_xcall_args_t *args, uint64_t len);
+
+// MO_XCALL_GO_IN(T) / MO_XCALL_GO_NOT_IN(T): equality is on the raw bits, so the integer types share a kernel per width
+int xcall_go_in(int negate, int T, mo_xcall_args_t *args, uint64_t len) {
+    ThreadCtx &t = tctx();
+    if (!t.ready) return MO_RC_INTERNAL_ERROR;
+    if (len == 0) return MO_RC_SUCCESS;
+    switch (T) {
+    case MO_T_BOOL: case MO_T_INT8: case MO_T_UINT8: return run_go_in<uint8_t>(t, negate, args, len);
+    case MO_T_INT16: case MO_T_UINT16: case MO_T_YEAR: return run_go_in<uint16_t>(t, negate, args, len);
+    case MO_T_INT32: case MO_T_UINT32: case MO_T_DATE: return run_go_in<uint32_t>(t, negate, args, len);
+    case MO_T_INT64: case MO_T_UINT64: case MO_T_TIME: case MO_T_DATETIME: case MO_T_TIMESTAMP: case MO_T_DECIMAL64:
+        return run_go_in<uint64_t>(t, negate, args, len);
+    case MO_T_FLOAT32: return run_go_in<float>(t, negate, args, len);
+    case MO_T_FLOAT64: return run_go_in<double>(t, negate, args, len);
+    case MO_T_DECIMAL128: case MO_T_UUID: return run_go_in<V16>(t, negate, args, len);
+    case MO_T_CHAR: case MO_T_VARCHAR: case MO_T_TEXT: case MO_T_BLOB: case MO_T_BINARY: case MO_T_VARBINARY:
+        return go_str_in(t, negate, args, len);   // strpred.cu
+    }
+    set_error("%s: unsupported type %d", negate ? "go not in" : "go in", T);
+    return MO_RC_INVALID_ARGUMENT;
 }
 
 }  // namespace mob

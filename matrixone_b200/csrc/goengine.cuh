@@ -1,5 +1,6 @@
 // goengine.cuh -- the operand protocol of the Go expression calls: GO_ARITH, GO_COMPARE, GO_COMPARE_F32_SCALE, GO_BETWEEN, MULTI_AND / OR
-// (goelem.cu), varlena GO_COMPARE and GO_LIKE (strpred.cu), DEC_ARITH, decimal GO_COMPARE and DEC_AVG (decimal.cu).
+// (goelem.cu), varlena GO_COMPARE and GO_LIKE (strpred.cu), DEC_ARITH, decimal GO_COMPARE and DEC_AVG (decimal.cu), GO_IN / GO_NOT_IN
+// (goelem.cu, its varlena types in strpred.cu).
 //
 // Every one of these calls follows the Go engine's per-batch template (pkg/sql/plan/function/baseTemplate.go:457-728), and this header is
 // the one place that implements it:
@@ -10,6 +11,7 @@
 //   - the first failing row in row order fails the call, and its index goes to the parameter block's err_row.
 // Each entry point keeps only what is its own: its parameter block, the kernel it launches, and how it turns a failure into a message.
 #pragma once
+#include <cstdio>
 #include "common.cuh"
 
 namespace mob {
@@ -38,11 +40,8 @@ struct Operand {
     const uint64_t *cnull() const { return cst ? nulls : nullptr; }       // a const operand's null word, where a kernel can read it
 };
 
-// stages args[k] of `what` (elem bytes per row: sizeof(T), 8, 16, or 24 for varlena cells, whose area is staged too)
-inline int stage_operand(Stager &st, const mo_xcall_args_t &a, size_t elem, uint64_t len, const char *what, int k, Operand &o) {
-    o = Operand{};
-    o.cst = is_const(a, elem, len);
-    const uint64_t rows = o.cst ? 1 : len;
+// stages `rows` elements of args[k] of `what` (elem bytes per row: sizeof(T), 8, 16, or 24 for varlena cells, whose area is staged too)
+inline int stage_rows(Stager &st, const mo_xcall_args_t &a, size_t elem, uint64_t rows, const char *what, int k, Operand &o) {
     if (!a.pdata || a.dataSz < elem * rows) {
         set_error("%s: operand %d holds %llu bytes, %llu needed", what, k, (unsigned long long)a.dataSz, (unsigned long long)(elem * rows));
         return MO_RC_INVALID_ARGUMENT;
@@ -51,6 +50,44 @@ inline int stage_operand(Stager &st, const mo_xcall_args_t &a, size_t elem, uint
     o.nulls = (const uint64_t *)st.in(a.pnulls, a.pnulls ? ((rows + 63) / 64) * 8 : 0);
     if (elem == MO_VARLENA_SZ && a.parea && a.areaSz) { o.area = (const uint8_t *)st.in(a.parea, a.areaSz); o.area_sz = a.areaSz; }
     return st.failed ? MO_RC_INTERNAL_ERROR : MO_RC_SUCCESS;
+}
+// stages the operand args[k] of a len-row call: a const one is one element
+inline int stage_operand(Stager &st, const mo_xcall_args_t &a, size_t elem, uint64_t len, const char *what, int k, Operand &o) {
+    o = Operand{};
+    o.cst = is_const(a, elem, len);
+    return stage_rows(st, a, elem, o.cst ? 1 : len, what, k, o);
+}
+
+// ---- IN / NOT IN (goelem.cu, strpred.cu): the list of args[2] with nvalues from the mo_in_params_t of args[3]; the set's hash table has
+// the least power-of-two slot count >= 2 * nvalues (load <= 1/2, so kt_find / kt_find_str always meet an empty slot), and the probe copies
+// a table of at most kInSmemBytes into each CTA's shared memory, reading it from global memory (L2) otherwise
+constexpr uint64_t kInSmemBytes = 16384;
+constexpr int64_t kInMaxValues = 0x7fffffff;   // list indices fit the 31-bit row of a kt_insert_str word
+inline int stage_in_list(ThreadCtx &t, Stager &st, mo_xcall_args_t *args, size_t elem, const char *what, Operand &l, uint64_t &m, uint64_t &mask) {
+    mo_in_params_t P;
+    char pw[64];
+    snprintf(pw, sizeof pw, "%s: params", what);
+    if (int rc = read_param(t, args[3], &P, sizeof P, sizeof P, pw)) return rc;
+    if (P.nvalues < 0 || P.nvalues > kInMaxValues) {
+        set_error("%s: nvalues %lld outside 0..%lld", what, (long long)P.nvalues, (long long)kInMaxValues);
+        return MO_RC_INVALID_ARGUMENT;
+    }
+    m = (uint64_t)P.nvalues;
+    l = Operand{};
+    mask = 0;
+    if (!m) return MO_RC_SUCCESS;
+    uint64_t cap = 2;
+    while (cap < 2 * m) cap <<= 1;
+    mask = cap - 1;
+    if (int rc = stage_rows(st, args[2], elem, m, what, 2, l)) return rc;
+    // a host list whose elements are all NULL is the empty set, known without a read-back: no table and no build (a device list's null
+    // words stay on the device, and its build inserts nothing)
+    const uint64_t *w = (const uint64_t *)args[2].pnulls;
+    if (!w || is_device_ptr(w)) return MO_RC_SUCCESS;
+    for (uint64_t k = 0; k < m / 64; k++) if (w[k] != ~0ull) return MO_RC_SUCCESS;
+    if ((m & 63) && (~w[m / 64] & ((1ull << (m & 63)) - 1))) return MO_RC_SUCCESS;
+    m = mask = 0;
+    return MO_RC_SUCCESS;
 }
 
 // stages the result args[0] and its required null bitmap; preload_* uploads a host buffer's content first (the kernel leaves rows alone)

@@ -11,6 +11,8 @@
 // | n1 | n2 (a const NULL operand: every row) with no second pass.  Cells of NULL and skipped rows are never read.  A non-inline cell outside
 // its area is recorded as the lowest such row per operand in a small status record, which the call reads back -- its one synchronise.
 #include "goengine.cuh"
+#include "keytable.cuh"
+#include <algorithm>
 #include <cstdio>
 #include <string>
 #include <vector>
@@ -21,6 +23,7 @@ namespace {
 
 constexpr int kCtasPerSm = 16;
 constexpr uint32_t kSmemAux = 16384;   // a const pattern's literals / tokens up to this size are copied to shared memory, longer ones stay in global
+static_assert(kSmemAux == kInSmemBytes, "an IN table is an aux block: one shared-memory budget for both IN paths");
 enum { LIKE_EXACT = 0, LIKE_PREFIX, LIKE_SUFFIX, LIKE_CHAIN };
 constexpr int32_t kAny1 = -1, kAnySeq = -2;   // tier-B tokens; a literal rune is its code point (>= 0)
 constexpr int32_t kRuneError = 0xFFFD;
@@ -256,23 +259,18 @@ str_row_kernel(uint8_t *__restrict__ r, uint32_t *__restrict__ rn32, uint64_t n,
     }
 }
 
-// enqueues the row kernel, reads back the status record and names the lowest bad cell
+// the status record, zeroed on the stream
+Status *arm_status(ThreadCtx &t, Stager &st, const char *what) {
+    Status *dst = (Status *)st.tmp(sizeof(Status));
+    if (st.failed) return nullptr;
+    if (cudaMemsetAsync(dst, 0, sizeof(Status), t.stream) != cudaSuccess) { set_error("%s: memset failed", what); return nullptr; }
+    return dst;
+}
+
+// enqueues the row kernel over the device aux block, reads back the status record dst and names the lowest bad cell
 template <class P>
 int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, const StrCol &a, const StrCol &b, const P &pred,
-             const std::vector<uint8_t> &aux_host, int all_null, const char *what) {
-    uint8_t *aux = nullptr;
-    const uint32_t aux_len = (uint32_t)aux_host.size();
-    if (aux_len) {
-        aux = (uint8_t *)st.tmp(aux_len);
-        if (st.failed) return MO_RC_INTERNAL_ERROR;
-        // pageable source: the runtime copies it into its own staging before this returns, so the vector may go out of scope
-        if (cudaMemcpyAsync(aux, aux_host.data(), aux_len, cudaMemcpyHostToDevice, t.stream) != cudaSuccess) {
-            set_error("%s: pattern upload failed", what); return MO_RC_INTERNAL_ERROR;
-        }
-    }
-    Status *dst = (Status *)st.tmp(sizeof(Status));
-    if (st.failed) return MO_RC_INTERNAL_ERROR;
-    if (cudaMemsetAsync(dst, 0, sizeof(Status), t.stream) != cudaSuccess) { set_error("%s: memset failed", what); return MO_RC_INTERNAL_ERROR; }
+             const uint8_t *aux, uint32_t aux_len, int all_null, const char *what, Status *dst) {
     const size_t smem = aux_len && aux_len <= kSmemAux ? aux_len : 0;
     cudaEventRecord(t.kev0, t.stream);
     str_row_kernel<P><<<grid_rows(len, kCtasPerSm), kThreads, smem, t.stream>>>(r, reinterpret_cast<uint32_t *>(rn), len, a, b, pred, aux, aux_len, all_null, dst);
@@ -290,6 +288,56 @@ int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, c
     }
     return st.complete();
 }
+// the same with a host aux block (a const pattern), uploaded first
+template <class P>
+int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, const StrCol &a, const StrCol &b, const P &pred,
+             const std::vector<uint8_t> &aux_host, int all_null, const char *what) {
+    uint8_t *aux = nullptr;
+    const uint32_t aux_len = (uint32_t)aux_host.size();
+    if (aux_len) {
+        aux = (uint8_t *)st.tmp(aux_len);
+        if (st.failed) return MO_RC_INTERNAL_ERROR;
+        // pageable source: the runtime copies it into its own staging before this returns, so the vector may go out of scope
+        if (cudaMemcpyAsync(aux, aux_host.data(), aux_len, cudaMemcpyHostToDevice, t.stream) != cudaSuccess) {
+            set_error("%s: pattern upload failed", what); return MO_RC_INTERNAL_ERROR;
+        }
+    }
+    Status *dst = arm_status(t, st, what);
+    if (!dst) return MO_RC_INTERNAL_ERROR;
+    return run_rows(t, st, r, rn, len, a, b, pred, aux, aux_len, all_null, what, dst);
+}
+
+// ---- IN / NOT IN (opOperatorStrIn): Go's map[string]bool of the list as kt_insert_str words (an XXH3 tag and the list index of the value)
+// in mask + 1 slots, which the row kernel takes as its aux block -- in shared memory up to kSmemAux (== kInSmemBytes) bytes
+__device__ __forceinline__ uint64_t str_hash_of(const StrCol &c, uint64_t row, const Str &s) {
+    const uint8_t *p = s.inl ? (const uint8_t *)c.data + 24 * (c.cst ? 0 : row) + 1 : s.p;
+    return xxh3::hash_bytes(p, s.len, 0).lo;
+}
+__device__ __forceinline__ bool str_eq(const Str &x, const Str &y) { return x.len == y.len && str_cmp(x, y) == 0; }
+
+// list element j (not NULL) into the set; a bad cell is recorded as operand 2's
+__global__ void __launch_bounds__(kThreads) in_str_build_kernel(uint64_t *slots, uint64_t mask, StrCol l, uint64_t m, Status *st) {
+    for (uint64_t j = blockIdx.x * (uint64_t)kThreads + threadIdx.x; j < m; j += (uint64_t)gridDim.x * kThreads) {
+        Str v;
+        if (bm_test(l.nulls, j)) continue;
+        if (!load_str(l, j, v)) { atomicMax(&st->bad_inv[1], ~(unsigned long long)j); continue; }
+        const uint64_t h = str_hash_of(l, j, v);
+        kt_insert_str(slots, mask, h, str_word(h, j), [&](uint32_t r) { Str w; return load_str(l, r, w) && str_eq(v, w); });
+    }
+}
+// b = the list (its nulls are the build's, not the row kernel's); aux = the slots, none for the empty set
+struct InPred {
+    uint64_t mask; int negate;
+    __device__ __forceinline__ bool operator()(const StrCol &a, const StrCol &b, uint64_t i, const uint8_t *aux, bool &bad1, bool &bad2) const {
+        Str x;
+        uint32_t row;
+        bad2 = false; bad1 = !load_str(a, i, x);
+        if (bad1 || !aux) return negate;
+        const bool found = kt_find_str(reinterpret_cast<const uint64_t *>(aux), mask, str_hash_of(a, i, x),
+                                       [&](uint32_t r) { Str y; return load_str(b, r, y) && str_eq(x, y); }, row);
+        return found != (negate != 0);
+    }
+};
 
 // ---- LIKE, host side
 // the const pattern's value, read from the caller's memory.  rc != 0: a bad cell (error set).  *is_null: the const NULL pattern.
@@ -391,6 +439,34 @@ int go_str_compare(ThreadCtx &t, int op, mo_xcall_args_t *args, uint64_t len) {
     if (int rc = stage_operand(st, args[1], MO_VARLENA_SZ, len, what, 1, a)) return rc;
     if (int rc = stage_operand(st, args[2], MO_VARLENA_SZ, len, what, 2, b)) return rc;
     return run_rows(t, st, r, rn, len, a, b, CmpPred{op}, std::vector<uint8_t>(), 0, what);
+}
+
+// MO_XCALL_GO_IN(T) / MO_XCALL_GO_NOT_IN(T) for the varlena types (goelem.cu routes them here).  Launches: the build (nvalues > 0), then
+// the row kernel; one read-back of the status record.
+int go_str_in(ThreadCtx &t, int negate, mo_xcall_args_t *args, uint64_t len) {
+    const char *what = negate ? "go not in" : "go in";
+    Stager st(t);
+    uint8_t *r; uint64_t *rn;
+    Operand a, l;
+    uint64_t m, mask;
+    if (int rc = stage_result(st, args[0], 1, len, true, true, what, r, rn)) return rc;
+    if (int rc = stage_operand(st, args[1], MO_VARLENA_SZ, len, what, 1, a)) return rc;
+    if (int rc = stage_in_list(t, st, args, MO_VARLENA_SZ, what, l, m, mask)) return rc;
+    Status *dst = arm_status(t, st, what);
+    if (!dst) return MO_RC_INTERNAL_ERROR;
+    uint64_t *slots = nullptr;
+    const uint64_t bytes = m ? (mask + 1) * 8 : 0;
+    if (m) {
+        slots = (uint64_t *)st.tmp(bytes);
+        if (st.failed) return MO_RC_INTERNAL_ERROR;
+        MOB_CUDA_TRY(cudaMemsetAsync(slots, 0xff, bytes, t.stream));
+        in_str_build_kernel<<<grid_rows(m, kCtasPerSm), kThreads, 0, t.stream>>>(slots, mask, l, m, dst);
+        MOB_LAUNCH_CHECK();
+    }
+    StrCol lb = l;
+    lb.nulls = nullptr;
+    return run_rows(t, st, r, rn, len, a, lb, InPred{mask, negate}, (const uint8_t *)slots, (uint32_t)std::min<uint64_t>(bytes, 0xffffffffu), 0,
+                    what, dst);
 }
 
 // MO_XCALL_GO_LIKE: args [0] bool result (+pnulls in/out) ; [1] the string ; [2] the pattern

@@ -45,6 +45,7 @@ int xcall_join_matched_merge(mo_xcall_args_t *args, uint64_t len);
 int xcall_join_build_rows(mo_xcall_args_t *args, uint64_t len);
 int xcall_join_cond(mo_xcall_args_t *args, uint64_t len);
 int xcall_go_like(mo_xcall_args_t *args, uint64_t len);
+int xcall_go_in(int negate, int T, mo_xcall_args_t *args, uint64_t len);
 int tuning_set(const char *name, int value);
 }  // namespace mob
 
@@ -98,6 +99,7 @@ extern "C" int32_t XCall(int64_t runtimeId, int64_t funcId, uint8_t *errStr, uin
     else if (funcId == MO_XCALL_Q1_MERGE) rc = xcall_q1_merge(a, len);
     else if (funcId >= 0x4000 && funcId < 0x5800) rc = xcall_go_elementwise(funcId, a, len);
     else if (funcId == MO_XCALL_GO_LIKE) rc = xcall_go_like(a, len);
+    else if (funcId >= 0x5900 && funcId < 0x5B00) rc = xcall_go_in((int)(funcId >= 0x5A00), (int)(funcId & 0xff), a, len);
     else if (funcId == MO_XCALL_Q6_FILTER_SUM) rc = xcall_q6(a, len);
     else if (funcId == MO_XCALL_Q1_GROUP_AGG) rc = xcall_q1(a, len);
     else if (funcId == MO_XCALL_Q6_DEC_FILTER_SUM) rc = xcall_q6_dec(a, len);

@@ -1425,3 +1425,38 @@ def like_device(col, pattern, n, out_dev, out_nulls_dev, col_nulls=None, pattern
         pv = _str_device_vec(pattern, pattern_nulls, n)
     xcall(capi.XCALL_GO_LIKE, [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n),
                                _str_device_vec(col, col_nulls, n), pv], n)
+
+
+# ------------------------------------------------------------------------------- IN / NOT IN (csrc/goelem.cu, csrc/strpred.cu)
+def _in_operand(T, x, nulls):
+    if T in capi.T_VARLENA:
+        return _str_operand(x, nulls)
+    a = np.ascontiguousarray(x)
+    return Vector(data=a, nulls=nulls, length=a.shape[0])
+
+
+def go_in(T, col, values, negate=False, col_nulls=None, values_nulls=None, rnulls=None, length=None):
+    """col IN values (NOT IN with negate), operator_in.go: values is the list, with its NULL elements skipped; a NULL row is NULL, every
+    other row is its membership (NOT IN: its negation).  Fixed-width T: numpy arrays of the column's element type (DECIMAL128 / UUID:
+    16-byte rows); the varlena T: a list of bytes or a (cells, area) pair.  A one-element col is a const.  rnulls: the result bitmap on entry
+    (rows set there are skipped).  Returns (values bool[n], nulls bool[n])."""
+    vc, vl = _in_operand(T, col, col_nulls), _in_operand(T, values, values_nulls)
+    n = length if length is not None else vc.length
+    r = np.zeros(max(n, 1), dtype=np.uint8)
+    rn = np.zeros(max((n + 63) // 64, 1), dtype=np.uint64) if rnulls is None else np.array(rnulls, dtype=np.uint64)
+    fid = capi.XCALL_GO_NOT_IN(T) if negate else capi.XCALL_GO_IN(T)
+    xcall(fid, [Vector(data=r[:n], nulls=rn, length=n), vc, vl, Vector(data=np.array([vl.length], np.int64))], n)
+    return r[:n].astype(bool), bitmap_to_bools(rn, n)
+
+
+def go_in_device(T, col, values, nvalues, n, out_dev, out_nulls_dev, negate=False, col_nulls=None, values_nulls=None):
+    """IN / NOT IN on resident vectors: col and values are DeviceBuffers (the varlena T: (cells, area) pairs, area None when every value is
+    inline), nulls DeviceBuffers or None; out_dev (bool[n]) and out_nulls_dev (its bitmap, in/out) DeviceBuffers.  The parameter block stays
+    on the host, so a fixed-width call only enqueues work; a varlena call reads back one status record."""
+    def dev(x, nulls, rows):
+        if T in capi.T_VARLENA:
+            return _str_device_vec(x, nulls, rows)
+        return Vector(data_ptr=x.ptr, data_nbytes=x.nbytes, nulls_ptr=nulls.ptr if nulls is not None else None, length=rows)
+    fid = capi.XCALL_GO_NOT_IN(T) if negate else capi.XCALL_GO_IN(T)
+    xcall(fid, [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n), dev(col, col_nulls, n),
+                dev(values, values_nulls, nvalues), Vector(data=np.array([nvalues], np.int64))], n)
