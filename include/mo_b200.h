@@ -282,6 +282,45 @@ typedef struct { int32_t div0_null; int32_t reserved; int64_t err_row; } mo_go_p
 typedef struct mo_in_params_t { int64_t nvalues; } mo_in_params_t;
 #define MO_XCALL_GO_IN(T) (0x5900 + (T))
 #define MO_XCALL_GO_NOT_IN(T) (0x5A00 + (T))
+/* ---- conditional values: CASE WHEN c1 THEN v1 ... [ELSE z] END, IF(c, a, b) and COALESCE(a, b, ...), csrc/caseexpr.cu.  caseFn / generalCaseFn /
+ * strCaseFn (operatorSet.go:144-316), iffFn (:389-) and CoalesceGeneral / CoalesceStr (func_binary.go:938-993).
+ *   GO_CASE(T)      args: [0] the result (T[len] + pnulls in/out; the string T: 24-byte cells + an area whose areaSz is its capacity) ; [1]
+ *                   mo_case_params_t (required, host or device) ; [2 + 2j] condition j (bool) ; [3 + 2j] value j (T) ; [2 + 2n] the ELSE value
+ *                   when has_else.  n = the WHEN count, 1..1024 ; has_else 0 or 1.  A row takes value j of the first j whose condition is
+ *                   non-NULL and true (NULL when that value is NULL); with no such j it takes ELSE, or NULL without one.  IF(c, a, b) is
+ *                   GO_CASE with n = 1 and an ELSE: a NULL or false condition takes b.
+ *   GO_COALESCE(T)  args: [0] the result ; [1] mo_case_params_t with n = the operand count (1..1024) and has_else 0 ; [2 .. 2 + n) the
+ *                   operands (T).  A row takes its first non-NULL operand, or NULL.
+ *   T = BOOL, BIT, INT8..64, UINT8..64, FLOAT32 / 64, DATE, TIME, DATETIME, TIMESTAMP, DECIMAL64, DECIMAL128, UUID, ENUM (fixed width: the
+ *       value's bytes are selected, never interpreted, so -0.0 and NaN payloads pass unchanged) and CHAR, VARCHAR, BLOB, TEXT, DATALINK (strings).
+ *       Any other T is refused (caseFn panics on BINARY / VARBINARY).
+ *   Operands follow the GO conventions above with one difference: merge_nulls does NOT apply.  A const operand is one element when len > 1;
+ *   a const NULL condition never matches, and a const NULL value gives NULL only on the rows that choose it.  Rows whose result null bit is
+ *   set on entry are skipped and their value bytes / cells left as they were; every other row the call makes NULL gets zero value bytes
+ *   (a string: the empty inline cell), and the bits past len in the last result word are cleared.  A condition or value is read only on
+ *   the rows that reach it, so the rows a short-circuit left unset (GO_CASE_SELECT below) are never read: a condition on the rows no
+ *   earlier WHEN took, a value on the rows that choose it.
+ *   Strings: each chosen value is copied, as AppendBytes does: up to 23 bytes inline in its cell (zero-padded), longer ones into the result
+ *   area in row order with no padding, the cell {0xffffffff, offset, length, 0...}.  area_len (out) is set to the bytes the result needs.
+ *   More than areaSz, or more than 2^32 - 1: MO_RC_OUT_OF_RANGE, area_len still written, cells, area and bitmap unchanged, so the call may be
+ *   repeated with an area of area_len bytes.  A chosen non-inline cell outside its operand's area fails with MO_RC_INVALID_ARGUMENT naming
+ *   the operand (its argument index) and the lowest row that chose it (a const operand too); cells that are not chosen are never read.
+ *   Launches: fixed width 1 (enqueue-only with device operands and a host block) ; strings 3 (pick, scan, write; the write is not launched
+ *   when the call fails), with one read-back of a status record (the bad cell and the area total) between the scan and the write.
+ *   Refused with MO_RC_INVALID_ARGUMENT: another T, n outside 1..1024, has_else not 0 / 1 or set for COALESCE, a short operand or result, a
+ *   result without a null bitmap, a missing block.
+ *   GO_CASE_SELECT  the select lists of EvalCase / EvalIff (evalExpression.go:501-573) as null-prefill words (a set bit: skip the row).  args:
+ *                   [0] uint64 words out: THEN j's prefill ; [1] uint64 words in / out: the remaining rows' complement (rows taken by an earlier
+ *                   WHEN, or not selected) ; [2] condition j (bool + pnulls; a const is one element; rows set in [1] are not read).  With
+ *                   took = ~[1] & cond & ~cond_nulls:  [0] = ~took (bits past len set) ; [1] |= took.  One kernel, enqueue-only.  A caller
+ *                   starts with [1] = NOT selectList and, per WHEN, evaluates the condition under a copy of [1] as its prefill, calls
+ *                   GO_CASE_SELECT and evaluates THEN j under [0]; ELSE is evaluated under the final [1].  CASE never raises an error from a
+ *                   branch a row does not reach (CASE WHEN d <> 0 THEN x / d ELSE 0 END). */
+typedef struct mo_case_params_t { int32_t n; int32_t has_else; int64_t area_len; } mo_case_params_t;
+#define MO_CASE_MAX_WHENS 1024
+#define MO_XCALL_GO_CASE(T) (0x5B00 + (T))
+#define MO_XCALL_GO_COALESCE(T) (0x5C00 + (T))
+#define MO_XCALL_GO_CASE_SELECT 0x5D00
 
 /* ---- the standalone column operators of the colexec pipeline (csrc/colops.cu).  Host or device pointers; when every data pointer and
  * nulls bitmap of every vector is a device pointer (or NULL) FILTER_SELS and SHUFFLE only enqueue work (asynchronous form, as

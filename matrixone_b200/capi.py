@@ -140,6 +140,23 @@ def XCALL_GO_NOT_IN(T):
     return 0x5A00 + T
 
 
+def XCALL_GO_CASE(T):
+    return 0x5B00 + T
+
+
+def XCALL_GO_COALESCE(T):
+    return 0x5C00 + T
+
+
+XCALL_GO_CASE_SELECT = 0x5D00
+CASE_MAX_WHENS = 1024
+
+
+class CaseParams(C.Structure):
+    """mo_case_params_t: n = WHEN count (GO_CASE) or operand count (GO_COALESCE); area_len (out) = the area bytes a string result needs"""
+    _fields_ = [("n", C.c_int32), ("has_else", C.c_int32), ("area_len", C.c_int64)]
+
+
 CMP_EQ, CMP_NE, CMP_GT, CMP_GE, CMP_LT, CMP_LE = 0, 1, 2, 3, 4, 5
 Q1_MAX_GROUPS = 8
 

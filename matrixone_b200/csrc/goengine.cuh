@@ -1,6 +1,7 @@
 // goengine.cuh -- the operand protocol of the Go expression calls: GO_ARITH, GO_COMPARE, GO_COMPARE_F32_SCALE, GO_BETWEEN, MULTI_AND / OR
 // (goelem.cu), varlena GO_COMPARE and GO_LIKE (strpred.cu), DEC_ARITH, decimal GO_COMPARE and DEC_AVG (decimal.cu), GO_IN / GO_NOT_IN
-// (goelem.cu, its varlena types in strpred.cu).
+// (goelem.cu, its varlena types in strpred.cu), and GO_CASE / GO_COALESCE (caseexpr.cu), which stage their operands here but apply no null
+// merge: a NULL operand only matters on the rows that choose it.
 //
 // Every one of these calls follows the Go engine's per-batch template (pkg/sql/plan/function/baseTemplate.go:457-728), and this header is
 // the one place that implements it:
@@ -155,6 +156,49 @@ template <typename T> __device__ __forceinline__ bool cmp_op(T x, T y, int op) {
     case CMP_GT: return x > y;  case CMP_GE: return x >= y;
     case CMP_LT: return x < y;  default: return x <= y;
     }
+}
+#endif
+
+// ---- varlena values (strpred.cu, caseexpr.cu)
+#ifdef __CUDACC__
+// A value.  An inline one (<= 23 bytes) stays in the three registers of its cell load; a long one is read from the area.
+struct Str {
+    uint64_t w0, w1, w2;
+    const uint8_t *p;
+    uint32_t len;
+    bool inl;
+    __device__ __forceinline__ uint32_t at(uint32_t j) const {
+        if (inl) {
+            const uint32_t k = j + 1;
+            const uint64_t w = k < 8 ? w0 : (k < 16 ? w1 : w2);
+            return (uint32_t)(w >> (8 * (k & 7))) & 0xffu;
+        }
+        return __ldg(p + j);
+    }
+};
+
+// false: a non-inline cell without an area or outside it -- varlena_ref's rule (common.cuh), restated because varlena_ref returns a pointer
+// into the cell for an inline value, and reading it back byte by byte would load the cell again; here the cell is loaded once as three
+// 8-byte words and an inline value is read out of those registers (Str::at).
+__device__ __forceinline__ bool load_str(const Operand &c, uint64_t row, Str &s) {
+    const uint8_t *cell = (const uint8_t *)c.data + 24 * (c.cst ? 0 : row);
+    if ((reinterpret_cast<uintptr_t>(c.data) & 7) == 0) {
+        const uint64_t *q = reinterpret_cast<const uint64_t *>(cell);
+        s.w0 = __ldg(q); s.w1 = __ldg(q + 1); s.w2 = __ldg(q + 2);
+    } else {
+        s.w0 = s.w1 = s.w2 = 0;
+#pragma unroll
+        for (int k = 0; k < 8; k++) {
+            s.w0 |= (uint64_t)__ldg(cell + k) << (8 * k);
+            s.w1 |= (uint64_t)__ldg(cell + 8 + k) << (8 * k);
+            s.w2 |= (uint64_t)__ldg(cell + 16 + k) << (8 * k);
+        }
+    }
+    const uint32_t b0 = (uint32_t)(s.w0 & 0xff);
+    if (b0 <= MO_VARLENA_INLINE_SZ) { s.inl = true; s.len = b0; s.p = nullptr; return true; }
+    const uint32_t off = (uint32_t)(s.w0 >> 32), len = (uint32_t)s.w1;
+    s.inl = false; s.len = len; s.p = c.area + off;
+    return c.area && (uint64_t)off + len <= c.area_sz;
 }
 #endif
 

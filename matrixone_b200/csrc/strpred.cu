@@ -34,46 +34,6 @@ using StrCol = Operand;
 // ~(lowest row whose cell points outside its area) per operand, 0 = none
 struct Status { unsigned long long bad_inv[2]; };
 
-// A value.  An inline one (<= 23 bytes) stays in the three registers of its cell load; a long one is read from the area.
-struct Str {
-    uint64_t w0, w1, w2;
-    const uint8_t *p;
-    uint32_t len;
-    bool inl;
-    __device__ __forceinline__ uint32_t at(uint32_t j) const {
-        if (inl) {
-            const uint32_t k = j + 1;
-            const uint64_t w = k < 8 ? w0 : (k < 16 ? w1 : w2);
-            return (uint32_t)(w >> (8 * (k & 7))) & 0xffu;
-        }
-        return __ldg(p + j);
-    }
-};
-
-// false: a non-inline cell without an area or outside it -- varlena_ref's rule (common.cuh), restated because varlena_ref returns a pointer
-// into the cell for an inline value, and reading it back byte by byte would load the cell again; here the cell is loaded once as three
-// 8-byte words and an inline value is read out of those registers (Str::at).
-__device__ __forceinline__ bool load_str(const StrCol &c, uint64_t row, Str &s) {
-    const uint8_t *cell = (const uint8_t *)c.data + 24 * (c.cst ? 0 : row);
-    if ((reinterpret_cast<uintptr_t>(c.data) & 7) == 0) {
-        const uint64_t *q = reinterpret_cast<const uint64_t *>(cell);
-        s.w0 = __ldg(q); s.w1 = __ldg(q + 1); s.w2 = __ldg(q + 2);
-    } else {
-        s.w0 = s.w1 = s.w2 = 0;
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            s.w0 |= (uint64_t)__ldg(cell + k) << (8 * k);
-            s.w1 |= (uint64_t)__ldg(cell + 8 + k) << (8 * k);
-            s.w2 |= (uint64_t)__ldg(cell + 16 + k) << (8 * k);
-        }
-    }
-    const uint32_t b0 = (uint32_t)(s.w0 & 0xff);
-    if (b0 <= MO_VARLENA_INLINE_SZ) { s.inl = true; s.len = b0; s.p = nullptr; return true; }
-    const uint32_t off = (uint32_t)(s.w0 >> 32), len = (uint32_t)s.w1;
-    s.inl = false; s.len = len; s.p = c.area + off;
-    return c.area && (uint64_t)off + len <= c.area_sz;
-}
-
 // bytes.Compare
 __device__ __forceinline__ int str_cmp(const Str &x, const Str &y) {
     const uint32_t m = x.len < y.len ? x.len : y.len;

@@ -46,6 +46,8 @@ int xcall_join_build_rows(mo_xcall_args_t *args, uint64_t len);
 int xcall_join_cond(mo_xcall_args_t *args, uint64_t len);
 int xcall_go_like(mo_xcall_args_t *args, uint64_t len);
 int xcall_go_in(int negate, int T, mo_xcall_args_t *args, uint64_t len);
+int xcall_go_case(int coalesce, int T, mo_xcall_args_t *args, uint64_t len);
+int xcall_case_select(mo_xcall_args_t *args, uint64_t len);
 int tuning_set(const char *name, int value);
 }  // namespace mob
 
@@ -100,6 +102,8 @@ extern "C" int32_t XCall(int64_t runtimeId, int64_t funcId, uint8_t *errStr, uin
     else if (funcId >= 0x4000 && funcId < 0x5800) rc = xcall_go_elementwise(funcId, a, len);
     else if (funcId == MO_XCALL_GO_LIKE) rc = xcall_go_like(a, len);
     else if (funcId >= 0x5900 && funcId < 0x5B00) rc = xcall_go_in((int)(funcId >= 0x5A00), (int)(funcId & 0xff), a, len);
+    else if (funcId >= 0x5B00 && funcId < 0x5D00) rc = xcall_go_case((int)(funcId >= 0x5C00), (int)(funcId & 0xff), a, len);
+    else if (funcId == MO_XCALL_GO_CASE_SELECT) rc = xcall_case_select(a, len);
     else if (funcId == MO_XCALL_Q6_FILTER_SUM) rc = xcall_q6(a, len);
     else if (funcId == MO_XCALL_Q1_GROUP_AGG) rc = xcall_q1(a, len);
     else if (funcId == MO_XCALL_Q6_DEC_FILTER_SUM) rc = xcall_q6_dec(a, len);

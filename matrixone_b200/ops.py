@@ -1460,3 +1460,137 @@ def go_in_device(T, col, values, nvalues, n, out_dev, out_nulls_dev, negate=Fals
     fid = capi.XCALL_GO_NOT_IN(T) if negate else capi.XCALL_GO_IN(T)
     xcall(fid, [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n), dev(col, col_nulls, n),
                 dev(values, values_nulls, nvalues), Vector(data=np.array([nvalues], np.int64))], n)
+
+
+# --------------------------------------------------------------- CASE, IF, COALESCE and the CASE select lists (csrc/caseexpr.cu)
+# value bytes per row of the GO_CASE / GO_COALESCE types; the varlena types are 24-byte cells plus an area
+CASE_WIDTH = {capi.T_BOOL: 1, capi.T_INT8: 1, capi.T_UINT8: 1, capi.T_INT16: 2, capi.T_UINT16: 2, capi.T_ENUM: 2, capi.T_INT32: 4,
+              capi.T_UINT32: 4, capi.T_FLOAT32: 4, capi.T_DATE: 4, capi.T_INT64: 8, capi.T_UINT64: 8, capi.T_FLOAT64: 8, capi.T_TIME: 8,
+              capi.T_DATETIME: 8, capi.T_TIMESTAMP: 8, capi.T_DECIMAL64: 8, capi.T_BIT: 8, capi.T_DECIMAL128: 16, capi.T_UUID: 16}
+CASE_STR_TYPES = (capi.T_CHAR, capi.T_VARCHAR, capi.T_BLOB, capi.T_TEXT, capi.T_DATALINK)
+
+
+def _case_value_dtype(T):
+    return {1: np.uint8, 2: np.uint16, 4: np.uint32, 8: np.uint64, 16: np.uint64}[CASE_WIDTH[T]] if T not in capi.NP_OF_T else capi.NP_OF_T[T]
+
+
+def _case_operand(T, op, is_cond=False):
+    """(data, nulls) -> Vector.  A condition is a bool array; a fixed-width value any array of the type's bytes per row (16-byte types:
+    uint64[k, 2]); a string value a list of bytes or a (cells, area) pair.  One row is a const operand."""
+    data, nulls = op
+    if not is_cond and T in CASE_STR_TYPES:
+        return _str_operand(data, nulls)
+    a = np.ascontiguousarray(data)
+    rows = a.shape[0]
+    return Vector(data=a.view(np.uint8).reshape(-1), nulls=nulls, length=rows)
+
+
+def _case_run(fid, T, vecs, nsel, has_else, n, rnulls, area_cap):
+    rn = np.zeros(max((n + 63) // 64, 1), dtype=np.uint64) if rnulls is None else np.array(rnulls, dtype=np.uint64)
+    prm = np.frombuffer(bytes(capi.CaseParams(nsel, has_else, 0)), dtype=np.uint8).copy()
+    pv = Vector(data=prm, length=1)
+    if T not in CASE_STR_TYPES:
+        w = CASE_WIDTH.get(T, 8)
+        r = np.zeros(max(n, 1) * w, dtype=np.uint8)
+        xcall(fid, [Vector(data=r[:n * w], nulls=rn, length=n), pv] + vecs, n)
+        out = r[:n * w].view(_case_value_dtype(T))
+        return (out.reshape(n, 2) if w == 16 else out), bitmap_to_bools(rn, n)
+    cap = area_cap if area_cap is not None else sum(int(v.area.nbytes) for v in vecs if v.area is not None)
+    cells = np.zeros(max(n, 1) * 24, dtype=np.uint8)
+    for attempt in range(2):
+        area = np.zeros(cap, dtype=np.uint8)
+        rc, msg = xcall(fid, [Vector(data=cells[:24 * n], nulls=rn, area=area, length=n), pv] + vecs, n, raise_on_error=False)
+        need = int(prm.view(np.int64)[1])
+        if rc == capi.RC_OUT_OF_RANGE and attempt == 0 and area_cap is None:
+            cap = need                     # the JOIN_PROBE capacity protocol: the call left the result unchanged; repeat with area_len
+            continue
+        if rc:
+            raise capi.MoError(rc, "xcall xfunc failed, error code %d, %s" % (rc, msg))
+        return cells[:24 * n], area[:need], bitmap_to_bools(rn, n)
+
+
+def go_case(T, conds, values, else_value=None, rnulls=None, length=None, area_cap=None):
+    """CASE WHEN conds[0] THEN values[0] ... [ELSE else_value] END (caseFn).  Every operand is a (data, nulls) pair, nulls = bitmap words or
+    None; a one-row operand is a const.  rnulls: the result bitmap on entry (rows set there are skipped).  Fixed-width T returns (values,
+    nulls bool[n]); the string T returns (cells uint8[24 n], area, nulls bool[n]), the area sized by the call (area_cap: a fixed capacity,
+    RC_OUT_OF_RANGE raised when it is too small)."""
+    if len(conds) != len(values):
+        raise ValueError("one value per condition")
+    vecs = []
+    for c, v in zip(conds, values):
+        vecs += [_case_operand(T, c, True), _case_operand(T, v)]
+    if else_value is not None:
+        vecs.append(_case_operand(T, else_value))
+    n = length if length is not None else max(v.length for v in vecs)
+    return _case_run(capi.XCALL_GO_CASE(T), T, vecs, len(conds), 0 if else_value is None else 1, n, rnulls, area_cap)
+
+
+def go_iff(T, cond, a, b, rnulls=None, length=None, area_cap=None):
+    """IF(cond, a, b) (iffFn): CASE with one WHEN and an ELSE -- a NULL or false condition takes b"""
+    return go_case(T, [cond], [a], b, rnulls, length, area_cap)
+
+
+def go_coalesce(T, operands, rnulls=None, length=None, area_cap=None):
+    """COALESCE(operands...) (CoalesceGeneral / CoalesceStr): the first non-NULL operand, or NULL.  Operands and results as go_case."""
+    vecs = [_case_operand(T, o) for o in operands]
+    n = length if length is not None else max(v.length for v in vecs)
+    return _case_run(capi.XCALL_GO_COALESCE(T), T, vecs, len(operands), 0, n, rnulls, area_cap)
+
+
+def _case_device_vec(T, op, rows, is_cond=False):
+    data, nulls = op
+    if not is_cond and T in CASE_STR_TYPES:
+        return _str_device_vec(data, nulls, rows)
+    return Vector(data_ptr=data.ptr, data_nbytes=data.nbytes, nulls_ptr=nulls.ptr if nulls is not None else None, length=rows)
+
+
+def _case_device(fid, T, vecs, nsel, has_else, n, out_dev, out_nulls_dev, out_area_dev):
+    prm = np.frombuffer(bytes(capi.CaseParams(nsel, has_else, 0)), dtype=np.uint8).copy()
+    if T in CASE_STR_TYPES:
+        res = Vector(data_ptr=out_dev.ptr, data_nbytes=24 * n, nulls_ptr=out_nulls_dev.ptr, length=n,
+                     area_ptr=out_area_dev.ptr if out_area_dev is not None else None, area_nbytes=out_area_dev.nbytes if out_area_dev is not None else 0)
+    else:
+        res = Vector(data_ptr=out_dev.ptr, data_nbytes=CASE_WIDTH.get(T, 8) * n, nulls_ptr=out_nulls_dev.ptr, length=n)
+    rc, msg = xcall(fid, [res, Vector(data=prm, length=1)] + vecs, n, raise_on_error=False)
+    if rc and not (rc == capi.RC_OUT_OF_RANGE and T in CASE_STR_TYPES):
+        raise capi.MoError(rc, "xcall xfunc failed, error code %d, %s" % (rc, msg))
+    return rc, int(prm.view(np.int64)[1])
+
+
+def go_case_device(T, conds, values, else_value, n, out_dev, out_nulls_dev, out_area_dev=None):
+    """go_case on resident operands: (data, nulls) pairs of DeviceBuffers (a string value's data is a (cells, area) pair; one element's bytes
+    = const) into out_dev (T[n] or 24-byte cells), out_nulls_dev (its bitmap, in/out) and out_area_dev (strings: the area, its size the
+    capacity).  The parameter block stays on the host: a fixed-width call only enqueues work.  Returns (rc, area_len): rc is 0, or
+    RC_OUT_OF_RANGE for a string result whose area is smaller than area_len (the result is then unchanged)."""
+    vecs = []
+    for c, v in zip(conds, values):
+        vecs += [_case_device_vec(T, c, n, True), _case_device_vec(T, v, n)]
+    if else_value is not None:
+        vecs.append(_case_device_vec(T, else_value, n))
+    return _case_device(capi.XCALL_GO_CASE(T), T, vecs, len(conds), 0 if else_value is None else 1, n, out_dev, out_nulls_dev, out_area_dev)
+
+
+def go_coalesce_device(T, operands, n, out_dev, out_nulls_dev, out_area_dev=None):
+    """go_coalesce on resident operands, as go_case_device"""
+    vecs = [_case_device_vec(T, o, n) for o in operands]
+    return _case_device(capi.XCALL_GO_COALESCE(T), T, vecs, len(operands), 0, n, out_dev, out_nulls_dev, out_area_dev)
+
+
+def case_select(rem_words, cond, cond_nulls, n):
+    """one WHEN of EvalCase's select lists as null-prefill words (set = skip the row): rem_words = the rows already taken or not selected
+    (start with NOT selectList), cond the WHEN's bool values (one element: const) and cond_nulls its bitmap words or None.  Returns
+    (THEN's prefill words, the new remaining words)."""
+    w = (n + 63) // 64
+    then = np.zeros(max(w, 1), dtype=np.uint64)
+    rem = np.array(rem_words, dtype=np.uint64).reshape(-1)[:w].copy()
+    c = np.ascontiguousarray(cond).view(np.uint8).reshape(-1)
+    xcall(capi.XCALL_GO_CASE_SELECT, [Vector(data=then[:w], length=n), Vector(data=rem, length=n), Vector(data=c, nulls=cond_nulls, length=c.shape[0])], n)
+    return then[:w], rem
+
+
+def case_select_device(then_dev, rem_dev, cond_dev, cond_nulls_dev, n):
+    """case_select on resident words and condition (DeviceBuffers): enqueue-only"""
+    wb = 8 * ((n + 63) // 64)
+    xcall(capi.XCALL_GO_CASE_SELECT, [Vector(data_ptr=then_dev.ptr, data_nbytes=wb, length=n), Vector(data_ptr=rem_dev.ptr, data_nbytes=wb, length=n),
+                                      Vector(data_ptr=cond_dev.ptr, data_nbytes=cond_dev.nbytes, nulls_ptr=cond_nulls_dev.ptr if cond_nulls_dev is not None else None,
+                                             length=n)], n)
