@@ -180,7 +180,9 @@ typedef struct mo_xcall_args_t {
  * funcId = MO_XCALL_AGG(op, T).  args: [0] result: pdata -> one 8-byte value (int64 / uint64 / float64, or the
  * column type for MIN/MAX, zero-extended), pnulls -> 1-word bitmap, bit 0 set when the result is NULL
  * (all-null input); [1] the column (fixed width, pnulls optional).  len = rows.
- * SUM over signed ints returns MO_RC_OUT_OF_RANGE exactly when the serial Go loop would (int64OfCheck). */
+ * SUM over signed ints returns MO_RC_OUT_OF_RANGE exactly when the serial Go loop would (int64OfCheck).  MIN / MAX return the bits of
+ * the first row that reaches the extreme, as the serial loop's strict compare does: -0.0 and 0.0 tie, so the zero of the earlier row is
+ * kept, and a NaN in the first non-null row is kept with its payload. */
 #define MO_AGG_SUM 0
 #define MO_AGG_COUNT 1   /* COUNT(col): non-null rows; result int64 */
 #define MO_AGG_MIN 2
@@ -344,7 +346,8 @@ typedef struct mo_case_params_t { int32_t n; int32_t has_else; int64_t area_len;
  * GROUP_AGG(op, T)  sumAvgExec / countColumnExec / minMaxExecFixed .BatchFill (sumavg2.go:133-199, count2.go:120-146, minmax2.go:49-80) into a
  *              caller-owned state that persists across batches: SUM into int64 / uint64 / float64 (overflow -> MO_RC_OUT_OF_RANGE exactly when
  *              the serial loop would fail), AVG = SUM + counts, COUNT into int64, MIN / MAX in 8-byte slots (value in the low bytes) with the
- *              first-value-initialises / strict-compare rule incl. NaN.  A group is NULL until its first value (state pnulls, in/out).
+ *              first-value-initialises / strict-compare rule incl. NaN: the bits of the first row that reaches the extreme (-0.0 and
+ *              0.0 tie: the earlier row's zero, a state's zero before a later batch's).  A group is NULL until its first value (state pnulls, in/out).
  *              args: [0] state 8 bytes per group (+pnulls) ; [1] counts int64 per group (AVG: required) ; [2] groups uint64[len] ; [3] column (+pnulls)
  * float64 group sums are accumulated with atomics: the association order is not fixed, results agree with the serial loop to ~1e-13 relative. */
 #define MO_XCALL_FILTER_SELS 0x6000

@@ -27,7 +27,8 @@ enum Kind { K_SUM_SIGNED = 0, K_SUM_UNSIGNED = 1, K_SUM_FLOAT = 2, K_MIN = 3, K_
 //  SUM_SIGNED  : w0 = two's-complement (wrapping) sum ; w2 = max |v| : if max|v| * (non-null rows) fits int64 no prefix can overflow (w3 unused)
 //  SUM_UNSIGNED: w0,w1 = sum (lo,hi)
 //  SUM_FLOAT   : d = sum (double)
-//  MIN / MAX   : w0 = value bits (zero-extended), w1 = smallest row index of a non-null row (floats: NaN rule)
+//  MIN / MAX   : w0 = value bits (zero-extended), w1 = smallest row index of a non-null row (floats: NaN rule), w2 = the row of w0
+//                (the first row that reaches the extreme, so -0.0 and 0.0 tie as the serial loop ties them)
 //  all         : cnt = non-null rows
 struct Rec { uint64_t w0, w1, w2, w3; double d; uint64_t cnt; uint64_t pad0, pad1; };
 // signed SUM: can a prefix of the serial sum leave int64?  Not if every |v| <= INT64_MAX / rows (then even the sum of all magnitudes fits).
@@ -49,6 +50,7 @@ struct Acc {
     T mm;
     bool has = false;
     uint64_t first = ~0ull;
+    uint64_t at = ~0ull;   // MIN / MAX: the row the kept value came from
 
     __device__ __forceinline__ void add(T v, uint64_t row) {
         cnt++;
@@ -62,9 +64,10 @@ struct Acc {
         } else if (KIND == K_SUM_FLOAT) {
             d = d + (double)v;  // sums[g] += float64(val), sumavg2.go:153
         } else {
-            if (!has) { has = true; mm = v; first = row; }
-            else if (KIND == K_MIN ? (v < mm) : (v > mm)) mm = v;       // strict compare, minmax2.go:73
-            else if (mm != mm && !(v != v)) { /* running value NaN but not the global first row: Go would never hold it */ mm = v; }
+            // a thread sees its rows in rising order, so the strict compare keeps the first row of a tie (-0.0 before 0.0)
+            if (!has) { has = true; mm = v; first = row; at = row; }
+            else if (KIND == K_MIN ? (v < mm) : (v > mm)) { mm = v; at = row; }       // strict compare, minmax2.go:73
+            else if (mm != mm && !(v != v)) { /* running value NaN but not the global first row: Go would never hold it */ mm = v; at = row; }
         }
     }
     __device__ __forceinline__ void merge(const Rec &r) {
@@ -74,18 +77,19 @@ struct Acc {
         else if (KIND == K_SUM_FLOAT) { d = d + r.d; }
         else {
             T v = from_bits<T>(r.w0);
-            if (!has) { has = true; mm = v; first = r.w1; }
+            if (!has) { has = true; mm = v; first = r.w1; at = r.w2; }
             else {
                 if (r.w1 < first) first = r.w1;
-                if (KIND == K_MIN ? (v < mm) : (v > mm)) mm = v;
-                else if (mm != mm && !(v != v)) mm = v;
+                // an equal value from an earlier row wins: the serial loop keeps the first row that reaches the extreme
+                if ((KIND == K_MIN ? (v < mm) : (v > mm)) || (v == mm && r.w2 < at)) { mm = v; at = r.w2; }
+                else if (mm != mm && !(v != v)) { mm = v; at = r.w2; }
             }
         }
         cnt += r.cnt;
     }
     __device__ __forceinline__ Rec rec() const {
         Rec r; r.w0 = w0; r.w1 = w1; r.w2 = w2; r.w3 = w3; r.d = d; r.cnt = cnt; r.pad0 = r.pad1 = 0;
-        if (KIND == K_MIN || KIND == K_MAX) { r.w0 = has ? to_bits<T>(mm) : 0; r.w1 = first; }
+        if (KIND == K_MIN || KIND == K_MAX) { r.w0 = has ? to_bits<T>(mm) : 0; r.w1 = first; r.w2 = at; }
         return r;
     }
 };

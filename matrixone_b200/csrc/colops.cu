@@ -418,6 +418,7 @@ __device__ __forceinline__ void agg_update(unsigned long long *a0, unsigned long
     else if (KIND == G_MIN_FLT || KIND == G_MAX_FLT) {
         const double d = (double)v;
         if (d == d) { if (KIND == G_MIN_FLT) atomicMin(a0, flt_key(d)); else atomicMax(a0, flt_key(d)); }
+        if (d == 0.0) atomicMin(a2, (unsigned long long)row);   // flt_key folds -0.0 into 0.0: the first zero row gives the sign
         atomicMin(a1, (unsigned long long)row);   // first non-null row of the group in this batch (the NaN rule needs it)
     }
     atomicAdd(cnt, 1ull);
@@ -427,7 +428,8 @@ template <int KIND>
 __global__ void __launch_bounds__(kThreads)
 agg_temp_init_kernel(AggTemp A, uint64_t ngroups) {
     for (uint64_t g = blockIdx.x * (uint64_t)kThreads + threadIdx.x; g < ngroups; g += (uint64_t)gridDim.x * kThreads) {
-        A.a0[g] = a0_identity<KIND>(); A.a1[g] = (KIND == G_MIN_FLT || KIND == G_MAX_FLT) ? ~0ull : 0ull; A.a2[g] = 0; A.cnt[g] = 0;
+        A.a0[g] = a0_identity<KIND>(); A.a1[g] = (KIND == G_MIN_FLT || KIND == G_MAX_FLT) ? ~0ull : 0ull;
+        A.a2[g] = (KIND == G_MIN_FLT || KIND == G_MAX_FLT) ? ~0ull : 0ull; A.cnt[g] = 0;
     }
 }
 
@@ -439,7 +441,8 @@ group_agg_kernel(const uint64_t *__restrict__ groups, const T *__restrict__ col,
     const int rep_mask = (1 << rep_shift) - 1;
     if (SMEM) {
         for (int s = threadIdx.x; s < (int)(ngroups << rep_shift); s += kThreads) {
-            s0[s] = a0_identity<KIND>(); s1[s] = (KIND == G_MIN_FLT || KIND == G_MAX_FLT) ? ~0ull : 0ull; s2[s] = 0; sc[s] = 0;
+            s0[s] = a0_identity<KIND>(); s1[s] = (KIND == G_MIN_FLT || KIND == G_MAX_FLT) ? ~0ull : 0ull;
+            s2[s] = (KIND == G_MIN_FLT || KIND == G_MAX_FLT) ? ~0ull : 0ull; sc[s] = 0;
         }
         __syncthreads();
     }
@@ -465,7 +468,7 @@ group_agg_kernel(const uint64_t *__restrict__ groups, const T *__restrict__ col,
             else if (KIND == G_MAX_INT) atomicMax(reinterpret_cast<long long *>(&A.a0[g]), (long long)s0[s]);
             else if (KIND == G_MIN_UINT || KIND == G_MIN_FLT) atomicMin(&A.a0[g], s0[s]);
             else if (KIND == G_MAX_UINT || KIND == G_MAX_FLT) atomicMax(&A.a0[g], s0[s]);
-            if (KIND == G_MIN_FLT || KIND == G_MAX_FLT) atomicMin(&A.a1[g], s1[s]);
+            if (KIND == G_MIN_FLT || KIND == G_MAX_FLT) { atomicMin(&A.a1[g], s1[s]); if (s2[s] != ~0ull) atomicMin(&A.a2[g], s2[s]); }
             atomicAdd(&A.cnt[g], sc[s]);
         }
     }
@@ -506,7 +509,10 @@ agg_fold_kernel(uint64_t *__restrict__ state, uint64_t *__restrict__ snulls, int
             double cur = was_null ? first : (sizeof(T) == 4 ? (double)__uint_as_float((unsigned)state[g]) : __longlong_as_double((long long)state[g]));
             if (cur == cur) {
                 const bool any = KIND == G_MIN_FLT ? A.a0[g] != ~0ull : A.a0[g] != 0ull;
-                if (any) { const double b = flt_unkey(A.a0[g]); if (KIND == G_MIN_FLT ? b < cur : b > cur) cur = b; }
+                if (any) {   // a zero extreme takes its sign from the batch's first zero row; an equal earlier value stays (strict compare)
+                    const double b = A.a0[g] == flt_key(0.0) ? (double)col[A.a2[g]] : flt_unkey(A.a0[g]);
+                    if (KIND == G_MIN_FLT ? b < cur : b > cur) cur = b;
+                }
             }
             if (sizeof(T) == 4) state[g] = (uint64_t)__float_as_uint((float)cur); else state[g] = (uint64_t)__double_as_longlong(cur);
         }
