@@ -17,7 +17,7 @@
 //
 //   Kernel shape: one thread per key; the filter words are random 8-byte reads (L2-resident for filters up to ~100 MB), keys stream coalesced.
 //   Algorithmic bytes per key: elemsz + 1 result byte + k x 32-byte sectors of the filter.
-#include "common.cuh"
+#include "column.cuh"
 #include "bloom_internal.cuh"
 #include "keytable.cuh"
 #include <cstdio>
@@ -79,10 +79,9 @@ __device__ __forceinline__ bool key_of(const KeySrc &K, uint64_t i, const uint8_
     if (i * K.elemsz + (K.varlena ? (uint64_t)MO_VARLENA_SZ : K.elemsz) > K.len) return false;   // the reference's  j < len  loop bound (a trailing partial element is not read)
     if (!K.varlena) { *p = K.keys + i * K.elemsz; *n = K.elemsz; return true; }
     const uint8_t *c = K.keys + i * K.elemsz;
-    if (c[0] <= MO_VARLENA_INLINE_SZ) { *p = c + 1; *n = c[0]; return true; }
-    const uint32_t off = xxh3::rd32(c + 4), ln = xxh3::rd32(c + 8);
-    if (!K.area || (uint64_t)off + ln > K.area_len) return false;   // (the reference would read out of bounds here; such a row is skipped)
-    *p = K.area + off; *n = ln;
+    const VarlenaCell v = varlena_cell(c[0], xxh3::rd32(c + 4), xxh3::rd32(c + 8), K.area, K.area_len);
+    if (!v.ok) return false;   // (the reference would read out of bounds here; such a row is skipped)
+    *p = v.inl ? c + 1 : K.area + v.off; *n = v.len;
     return true;
 }
 

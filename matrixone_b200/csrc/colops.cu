@@ -17,7 +17,7 @@
 // ballots for bitmaps, a single-pass decoupled look-back scan for the order-preserving compaction.
 #include "common.cuh"
 #include "keytable.cuh"
-#include "varlena.cuh"
+#include "column.cuh"
 #include <cstring>
 
 namespace mob {
@@ -204,29 +204,27 @@ pack_keys_kernel(uint64_t *__restrict__ keys, uint32_t *__restrict__ skip32, uin
 // column its uint16 little-endian length + its bytes; a NULL is the marker 1 alone (has_null) or makes the row's key empty and skipped
 // =========================================================================================================
 static_assert(MO_STRKEY_MAX_COLS <= MO_ORDER_MAX_KEYS, "one VarlenaStat entry per key column");
-struct StrKeyCols {
-    const uint8_t *col[MO_STRKEY_MAX_COLS]; const uint64_t *nulls[MO_STRKEY_MAX_COLS]; const uint8_t *area[MO_STRKEY_MAX_COLS];
-    uint64_t area_sz[MO_STRKEY_MAX_COLS]; int size[MO_STRKEY_MAX_COLS] /* 0 = varlena cells */; int cst[MO_STRKEY_MAX_COLS]; int n;
-};
+struct StrKeyCols { Operand col[MO_STRKEY_MAX_COLS]; int size[MO_STRKEY_MAX_COLS] /* 0 = varlena cells */; int n; };
 
 // the length of row i's key; its bytes too when out is set.  skip = a NULL in has_null = 0 mode (the key is then empty).
 __device__ __forceinline__ uint64_t strkey_row(const StrKeyCols &K, uint64_t i, int has_null, uint8_t *out, bool &skip) {
     uint64_t off = 0;
     skip = false;
     for (int k = 0; k < K.n; k++) {
-        const uint64_t r = K.cst[k] ? 0 : i;
-        const bool isnull = bm_test(K.nulls[k], r);
+        const Operand &c = K.col[k];
+        const uint64_t r = c.cst ? 0 : i;
+        const bool isnull = bm_test(c.nulls, r);
         if (has_null) {
             if (out) out[off] = isnull ? 1 : 0;
             off++;
             if (isnull) continue;
         } else if (isnull) { skip = true; return 0; }
         if (K.size[k]) {
-            const uint8_t *p = K.col[k] + r * (uint64_t)K.size[k];
+            const uint8_t *p = (const uint8_t *)c.data + r * (uint64_t)K.size[k];
             if (out) for (int b = 0; b < K.size[k]; b++) out[off + b] = p[b];
             off += K.size[k];
         } else {
-            const VarlenaRef v = varlena_ref(K.col[k], r, K.area[k], K.area_sz[k]);
+            const VarlenaRef v = varlena_ref((const uint8_t *)c.data, r, c.area, c.area_sz);
             if (out) {
                 out[off] = (uint8_t)v.len; out[off + 1] = (uint8_t)(v.len >> 8);
                 for (uint32_t b = 0; b < v.len; b++) out[off + 2 + b] = v.ptr[b];
@@ -810,27 +808,18 @@ int xcall_pack_str_keys(mo_xcall_args_t *args, uint64_t len) {
     if (P.ncols < 1 || P.ncols > MO_STRKEY_MAX_COLS) { set_error("pack str keys: %d key columns (1..%d)", P.ncols, MO_STRKEY_MAX_COLS); return MO_RC_INVALID_ARGUMENT; }
     if (!args[1].pdata || args[1].dataSz < 8 * (len + 1)) { set_error("pack str keys: the offsets need len + 1 entries"); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);
-    StrKeyCols K;
-    memset(&K, 0, sizeof K);
+    StrKeyCols K{};
     K.n = P.ncols;
     for (int k = 0; k < K.n; k++) {
         const mo_xcall_args_t &a = args[3 + k];
         const int T = P.col_type[k];
-        const bool var = is_varlena(T);
-        const uint64_t esz = var ? MO_VARLENA_SZ : (uint64_t)key_type_size(T);
+        const uint64_t esz = key_elem_size(T);
         if (!esz) { st.finish(); set_error("pack str keys: column %d has unsupported type %d", k, T); return MO_RC_INVALID_ARGUMENT; }
-        const bool cst = len != 1 && a.dataSz == esz;
-        if (!cst && a.dataSz < esz * len) { st.finish(); set_error("pack str keys: column %d holds %llu bytes, %llu needed", k, (unsigned long long)a.dataSz, (unsigned long long)(esz * len)); return MO_RC_INVALID_ARGUMENT; }
-        if ((len || cst) && !a.pdata) { st.finish(); set_error("pack str keys: column %d has no data", k); return MO_RC_INVALID_ARGUMENT; }
-        const uint64_t rows = cst ? 1 : len;
-        K.col[k] = (const uint8_t *)st.in(a.pdata, rows * esz);
-        K.nulls[k] = (const uint64_t *)st.in(a.pnulls, a.pnulls ? ((rows + 63) / 64) * 8 : 0);
-        K.size[k] = var ? 0 : (int)esz;
-        K.cst[k] = cst ? 1 : 0;
-        if (var && a.parea && a.areaSz) {
-            K.area[k] = (const uint8_t *)st.in(a.parea, a.areaSz);
-            K.area_sz[k] = a.areaSz;
-        }
+        if (!is_const(a, esz, len) && a.dataSz < esz * len) { st.finish(); set_error("pack str keys: column %d holds %llu bytes, %llu needed", k, (unsigned long long)a.dataSz, (unsigned long long)(esz * len)); return MO_RC_INVALID_ARGUMENT; }
+        if (!a.pdata && (len || a.dataSz == esz)) { st.finish(); set_error("pack str keys: column %d has no data", k); return MO_RC_INVALID_ARGUMENT; }
+        // the checks above are the call's own; stage_operand's size check cannot fail after them
+        if (len) { if (int rc = stage_operand(st, a, esz, len, "pack str keys", 3 + k, K.col[k])) return rc; }
+        K.size[k] = is_varlena(T) ? 0 : (int)esz;
     }
     uint64_t *off = (uint64_t *)st.out(args[1].pdata, 8 * (len + 1));
     uint32_t *skip = (uint32_t *)st.out(args[1].pnulls, args[1].pnulls ? ((len + 63) / 64) * 8 : 0);
@@ -838,10 +827,8 @@ int xcall_pack_str_keys(mo_xcall_args_t *args, uint64_t len) {
     Rec *rec = (Rec *)st.tmp(sizeof(Rec));
     if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(rec, 0, sizeof(Rec), t.stream));
-    for (int k = 0; k < K.n; k++) {
-        if (K.size[k] || !len) continue;
-        int rc = varlena_stat(t, K.col[k], K.nulls[k], K.area[k], K.area_sz[k], K.cst[k] ? 1 : len, &rec->vs, k);
-        if (rc) { st.finish(); return rc; }
+    if (len) {
+        if (int rc = varlena_stats(t, K.col, P.col_type, K.n, len, &rec->vs)) { st.finish(); return rc; }
     }
     int grid = num_sms() * 8;
     const uint64_t work = (len + kThreads - 1) / kThreads;

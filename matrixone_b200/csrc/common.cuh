@@ -182,23 +182,6 @@ __device__ __forceinline__ void st_stream16(void *p, int4 v) {
 
 __device__ __forceinline__ bool bm_test(const uint64_t *p, uint64_t i) { return p && ((p[i >> 6] >> (i & 63)) & 1ull); }
 
-// varlena cell i, cgo/xcall.h:47-61 (== pkg/container/types/bytes.go:61-115): bs[0] <= 23 inline, else u32[1] = offset into the area and
-// u32[2] = length.  ok = false when a non-inline cell has no area or points outside [0, areaSz).
-struct VarlenaRef { const uint8_t *ptr; uint32_t len; bool ok; };
-__device__ __forceinline__ VarlenaRef varlena_ref(const uint8_t *cells, uint64_t i, const uint8_t *area, uint64_t areaSz) {
-    const uint8_t *c = cells + 24 * i;
-    VarlenaRef r; r.ok = true;
-    const uint8_t b0 = c[0];
-    if (b0 <= MO_VARLENA_INLINE_SZ) { r.ptr = c + 1; r.len = b0; }
-    else {
-        uint32_t off, len;
-        memcpy(&off, c + 4, 4); memcpy(&len, c + 8, 4);
-        r.ptr = area + off; r.len = len;
-        if (!area || (uint64_t)off + len > areaSz) r.ok = false;
-    }
-    return r;
-}
-
 // total order on non-NaN doubles as unsigned integers, so that MIN / MAX states can use the integer atomics; -0.0 is folded onto +0.0 (they
 // compare equal in the reference too)
 __device__ __forceinline__ unsigned long long flt_key(double d) {

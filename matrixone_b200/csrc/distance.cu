@@ -15,7 +15,7 @@
 // serial `sum += chunk` chain with 96 shuffle+add pairs and was instruction/MIO-bound at 0.55 of the HBM rate; cosine with
 // its three chains at 0.19).  The ring (5 stages, or 3 when both operands are per-row) is what keeps ~128 KB per SM in flight.
 // Algorithmic bytes per row = 2 * dim * sizeof(T) (one side const: dim * sizeof(T)) + 24 per varlena cell + 8 for the result.
-#include "common.cuh"
+#include "column.cuh"
 #include "godist.cuh"
 #include <cstring>
 
@@ -33,10 +33,8 @@ using namespace mob::godist;
 
 template <typename T, int KIND, bool TWO>
 __global__ void __launch_bounds__(kThreads)
-rowdist_kernel(double *__restrict__ res, const uint64_t *__restrict__ rnulls, uint64_t n,
-               const uint8_t *__restrict__ cells1, const uint8_t *__restrict__ area1, uint64_t area1Sz, bool const1,
-               const uint8_t *__restrict__ cells2, const uint8_t *__restrict__ area2, uint64_t area2Sz, bool const2,
-               unsigned *status) {
+rowdist_kernel(double *__restrict__ res, const uint64_t *__restrict__ rnulls, uint64_t n, const __grid_constant__ Operand x1,
+               const __grid_constant__ Operand x2, unsigned *status) {
     using Cfg = RingCfg<TWO>;
     using Acc = RowAcc<T, KIND>;
     constexpr int NST = Cfg::kStages;
@@ -47,12 +45,12 @@ rowdist_kernel(double *__restrict__ res, const uint64_t *__restrict__ rnulls, ui
     const uint64_t nwarps = ((uint64_t)gridDim.x * kThreads) >> 5;
     int xc_dim = 0;
     if (Acc::kXc) {  // dim = c1.len / sizeof(T) from the FIRST cell of arg 1, xcall.c:40,55
-        Ref r0 = varlena_ref(cells1, 0, area1, area1Sz);
+        Ref r0 = varlena_ref((const uint8_t *)x1.data, 0, x1.area, x1.area_sz);
         xc_dim = r0.ok ? (int)(r0.len / sizeof(T)) : 0;
     }
     // the per-row ("x") side is arg 1 unless only arg 1 is const; every kind is symmetric in its operands bit for bit
     // ((a-b)^2 == (b-a)^2, products commute, the cosine denominator sqrt(n1)*sqrt(n2) commutes)
-    const bool swap = !TWO && const1 && !const2;
+    const bool swap = !TWO && x1.cst && !x2.cst;
     unsigned st = 0;
     for (uint64_t base = warp * 32; base < n; base += nwarps * 32) {
         const uint64_t i = base + lane;
@@ -60,8 +58,8 @@ rowdist_kernel(double *__restrict__ res, const uint64_t *__restrict__ rnulls, ui
         int dim = 0; bool good = false;
         const uint8_t *px = nullptr, *pq = nullptr;
         if (live) {
-            Ref a = varlena_ref(cells1, const1 ? 0 : i, area1, area1Sz);
-            Ref b = Acc::kOne ? a : varlena_ref(cells2, const2 ? 0 : i, area2, area2Sz);
+            Ref a = varlena_ref((const uint8_t *)x1.data, x1.cst ? 0 : i, x1.area, x1.area_sz);
+            Ref b = Acc::kOne ? a : varlena_ref((const uint8_t *)x2.data, x2.cst ? 0 : i, x2.area, x2.area_sz);
             if (!a.ok || !b.ok) st |= ST_AREA;
             else if (Acc::kOne && a.len < sizeof(T)) st |= ST_EMPTY;   // "cannot normalize empty vector", distance_func.go:413-415
             else if (Acc::kXc) {
@@ -113,25 +111,36 @@ rowdist_kernel(double *__restrict__ res, const uint64_t *__restrict__ rnulls, ui
     if (lane == 0 && st) atomicOr(status, st);
 }
 
+// argument k's cells and area, its size and data checked by the caller.  Only the result's bitmap says which rows are NULL, so the argument's is not staged; and a zero-byte area
+// still bounds an empty value at offset 0, as it always has here.
+int stage_vectors(Stager &st, const mo_xcall_args_t &arg, uint64_t len, const char *what, int k, Operand &o) {
+    mo_xcall_args_t a = arg;
+    a.pnulls = nullptr;
+    if (int rc = stage_operand(st, a, MO_VARLENA_SZ, len, what, k, o)) return rc;
+    if (!o.area) o.area = a.parea;
+    return MO_RC_SUCCESS;
+}
+
 template <typename T, int KIND>
 int run_rowdist(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     if (len == 0) return MO_RC_SUCCESS;
     if (!args[0].pdata || args[0].dataSz < 8 * len) { set_error("distance: result vector shorter than len"); return MO_RC_INVALID_ARGUMENT; }
-    const bool c1 = args[1].dataSz == MO_VARLENA_SZ, c2 = args[2].dataSz == MO_VARLENA_SZ;   // const detection, xcall.c:38-39
-    if ((!c1 && args[1].dataSz < 24 * len) || (!c2 && args[2].dataSz < 24 * len)) { set_error("distance: argument vector shorter than len"); return MO_RC_INVALID_ARGUMENT; }
+    for (int k = 1; k <= 2; k++) {
+        if (!is_const(args[k], MO_VARLENA_SZ, len) && args[k].dataSz < 24 * len) { set_error("distance: argument vector shorter than len"); return MO_RC_INVALID_ARGUMENT; }
+        if (!args[k].pdata) { set_error("distance: argument %d has no data", k); return MO_RC_INVALID_ARGUMENT; }
+    }
     Stager st(t);
-    const uint8_t *cells1 = (const uint8_t *)st.in(args[1].pdata, args[1].dataSz);
-    const uint8_t *cells2 = (const uint8_t *)st.in(args[2].pdata, args[2].dataSz);
-    const uint8_t *area1 = (const uint8_t *)st.in(args[1].parea, args[1].areaSz);
-    const uint8_t *area2 = (const uint8_t *)st.in(args[2].parea, args[2].areaSz);
+    Operand x1, x2;
+    if (int rc = stage_vectors(st, args[1], len, "distance", 1, x1)) return rc;
+    if (int rc = stage_vectors(st, args[2], len, "distance", 2, x2)) return rc;
     const uint64_t *rn = (const uint64_t *)st.in(args[0].pnulls, args[0].pnulls ? ((len + 63) / 64) * 8 : 0);
     double *res = (double *)st.out(args[0].pdata, 8 * len, args[0].pnulls != nullptr);
     unsigned *dstatus = (unsigned *)st.tmp(4);
     if (st.failed) return MO_RC_INTERNAL_ERROR;
     MOB_CUDA_TRY(cudaMemsetAsync(dstatus, 0, 4, t.stream));
-    const bool two = !c1 && !c2;
+    const bool two = !x1.cst && !x2.cst;
     const uint64_t warps = (len + 31) / 32;
     uint64_t blocks = (warps + kThreads / 32 - 1) / (kThreads / 32);
     const uint64_t cap = (uint64_t)num_sms() * 2;   // 2 CTAs per SM by shared memory (95 / 111 KB each)
@@ -141,8 +150,8 @@ int run_rowdist(mo_xcall_args_t *args, uint64_t len) {
     if (two && !attr2) { MOB_CUDA_TRY(cudaFuncSetAttribute(rowdist_kernel<T, KIND, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr2 = true; }
     if (!two && !attr1) { MOB_CUDA_TRY(cudaFuncSetAttribute(rowdist_kernel<T, KIND, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr1 = true; }
     cudaEventRecord(t.kev0, t.stream);
-    if (two) rowdist_kernel<T, KIND, true><<<(unsigned)blocks, kThreads, smem, t.stream>>>(res, rn, len, cells1, area1, args[1].areaSz, c1, cells2, area2, args[2].areaSz, c2, dstatus);
-    else rowdist_kernel<T, KIND, false><<<(unsigned)blocks, kThreads, smem, t.stream>>>(res, rn, len, cells1, area1, args[1].areaSz, c1, cells2, area2, args[2].areaSz, c2, dstatus);
+    if (two) rowdist_kernel<T, KIND, true><<<(unsigned)blocks, kThreads, smem, t.stream>>>(res, rn, len, x1, x2, dstatus);
+    else rowdist_kernel<T, KIND, false><<<(unsigned)blocks, kThreads, smem, t.stream>>>(res, rn, len, x1, x2, dstatus);
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
     unsigned status = 0;
@@ -187,19 +196,18 @@ __device__ __forceinline__ bool live_below(const uint64_t *rnulls, uint64_t i, i
 template <typename T>
 __global__ void __launch_bounds__(256)
 normalize_write_kernel(uint8_t *__restrict__ ocells, uint8_t *__restrict__ oarea, const uint64_t *__restrict__ rnulls, uint64_t n,
-                       const uint8_t *__restrict__ cells, const uint8_t *__restrict__ area, uint64_t areaSz, bool cst, const double *__restrict__ norms) {
+                       const __grid_constant__ Operand in, const double *__restrict__ norms) {
     const int lane = threadIdx.x & 31;
     const uint64_t warp = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5, nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
     for (uint64_t i = warp; i < n; i += nwarps) {
         uint8_t *oc = ocells + 24 * i;
         if (bm_test(rnulls, i)) { if (lane < 24) oc[lane] = 0; continue; }          // NULL row: an empty inline cell
-        const uint8_t *c = cells + 24 * (cst ? 0 : i);
-        const Ref a = varlena_ref(cells, cst ? 0 : i, area, areaSz);
+        const uint8_t *c = (const uint8_t *)in.data + 24 * (in.cst ? 0 : i);
+        const Ref a = varlena_ref((const uint8_t *)in.data, in.cst ? 0 : i, in.area, in.area_sz);
         if (!a.ok || a.len < sizeof(T)) continue;                                   // reported by pass 1
         const int dim = (int)(a.len / sizeof(T));
         const double norm = norms[i];
-        const bool inl = c[0] <= MO_VARLENA_INLINE_SZ;
-        if (inl) {   // <= 23 bytes: the vector lives in the cell
+        if (a.inl) {   // <= 23 bytes: the vector lives in the cell
             if (lane == 0) oc[0] = c[0];
             if (lane >= 1 && lane < 24 && lane > (int)a.len) oc[lane] = 0;
             if (lane < dim) {
@@ -214,8 +222,8 @@ normalize_write_kernel(uint8_t *__restrict__ ocells, uint8_t *__restrict__ oarea
             continue;
         }
         if (lane < 24) oc[lane] = c[lane];
-        if (cst && live_below(rnulls, i, lane)) continue;                           // a const input: one vector, written once
-        uint8_t *dst = oarea + (a.ptr - area);
+        if (in.cst && live_below(rnulls, i, lane)) continue;                        // a const input: one vector, written once
+        uint8_t *dst = oarea + (a.ptr - in.area);
         if (((((uintptr_t)a.ptr) | ((uintptr_t)dst)) & 15) == 0) {
             constexpr int EPV = 16 / (int)sizeof(T);
             const int nv = dim / EPV;
@@ -249,13 +257,13 @@ int run_normalize(mo_xcall_args_t *args, uint64_t len) {
     ThreadCtx &t = tctx();
     if (!t.ready) return MO_RC_INTERNAL_ERROR;
     if (len == 0) return MO_RC_SUCCESS;
-    const bool c1 = args[1].dataSz == MO_VARLENA_SZ && len > 1;
     if (!args[0].pdata || args[0].dataSz < 24 * len) { set_error("normalize_l2: result vector shorter than len"); return MO_RC_INVALID_ARGUMENT; }
-    if (!c1 && args[1].dataSz < 24 * len) { set_error("normalize_l2: argument vector shorter than len"); return MO_RC_INVALID_ARGUMENT; }
+    if (!is_const(args[1], MO_VARLENA_SZ, len) && args[1].dataSz < 24 * len) { set_error("normalize_l2: argument vector shorter than len"); return MO_RC_INVALID_ARGUMENT; }
+    if (!args[1].pdata) { set_error("normalize_l2: argument 1 has no data"); return MO_RC_INVALID_ARGUMENT; }
     if (args[1].areaSz && (!args[0].parea || args[0].areaSz < args[1].areaSz)) { set_error("normalize_l2: the result area must be at least as large as the argument's (it mirrors its layout)"); return MO_RC_INVALID_ARGUMENT; }
     Stager st(t);
-    const uint8_t *cells = (const uint8_t *)st.in(args[1].pdata, c1 ? 24 : 24 * len);
-    const uint8_t *area = (const uint8_t *)st.in(args[1].parea, args[1].areaSz);
+    Operand x;
+    if (int rc = stage_vectors(st, args[1], len, "normalize_l2", 1, x)) return rc;
     const uint64_t *rn = (const uint64_t *)st.in(args[0].pnulls, args[0].pnulls ? ((len + 63) / 64) * 8 : 0);
     uint8_t *ocells = (uint8_t *)st.out(args[0].pdata, 24 * len);
     uint8_t *oarea = args[1].areaSz ? (uint8_t *)st.out(args[0].parea, args[1].areaSz, true) : nullptr;
@@ -270,11 +278,11 @@ int run_normalize(mo_xcall_args_t *args, uint64_t len) {
     static bool attr = false;
     if (!attr) { MOB_CUDA_TRY(cudaFuncSetAttribute(rowdist_kernel<T, K_GO_NORM, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
     cudaEventRecord(t.kev0, t.stream);
-    rowdist_kernel<T, K_GO_NORM, false><<<(unsigned)blocks, kThreads, smem, t.stream>>>(norms, rn, len, cells, area, args[1].areaSz, c1, cells, area, args[1].areaSz, c1, dstatus);
+    rowdist_kernel<T, K_GO_NORM, false><<<(unsigned)blocks, kThreads, smem, t.stream>>>(norms, rn, len, x, x, dstatus);
     MOB_LAUNCH_CHECK();
     uint64_t wblocks = (len + 7) / 8;
     if (wblocks > (uint64_t)num_sms() * 8) wblocks = (uint64_t)num_sms() * 8;
-    normalize_write_kernel<T><<<(unsigned)wblocks, 256, 0, t.stream>>>(ocells, oarea, rn, len, cells, area, args[1].areaSz, c1, norms);
+    normalize_write_kernel<T><<<(unsigned)wblocks, 256, 0, t.stream>>>(ocells, oarea, rn, len, x, norms);
     cudaEventRecord(t.kev1, t.stream);
     MOB_LAUNCH_CHECK();
     unsigned status = 0;

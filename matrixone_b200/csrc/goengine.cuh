@@ -13,7 +13,7 @@
 // Each entry point keeps only what is its own: its parameter block, the kernel it launches, and how it turns a failure into a message.
 #pragma once
 #include <cstdio>
-#include "common.cuh"
+#include "column.cuh"
 
 namespace mob {
 
@@ -26,38 +26,7 @@ inline int grid_rows(uint64_t n, int ctas_per_sm) {
     return (int)(b > cap ? cap : (b ? b : 1));
 }
 
-// ---- operands
-// the one const rule
-inline bool is_const(const mo_xcall_args_t &a, size_t elem, uint64_t len) { return a.dataSz == elem && len > 1; }
-
-// a staged operand: data (and a varlena operand's area) and nulls in device memory
-struct Operand {
-    const void *data = nullptr;
-    const uint64_t *nulls = nullptr;
-    int cst = 0;                        // a const operand: every row reads element 0
-    const uint8_t *area = nullptr;
-    uint64_t area_sz = 0;
-    const uint64_t *col_nulls() const { return cst ? nullptr : nulls; }   // the bitmap the null merge ORs in
-    const uint64_t *cnull() const { return cst ? nulls : nullptr; }       // a const operand's null word, where a kernel can read it
-};
-
-// stages `rows` elements of args[k] of `what` (elem bytes per row: sizeof(T), 8, 16, or 24 for varlena cells, whose area is staged too)
-inline int stage_rows(Stager &st, const mo_xcall_args_t &a, size_t elem, uint64_t rows, const char *what, int k, Operand &o) {
-    if (!a.pdata || a.dataSz < elem * rows) {
-        set_error("%s: operand %d holds %llu bytes, %llu needed", what, k, (unsigned long long)a.dataSz, (unsigned long long)(elem * rows));
-        return MO_RC_INVALID_ARGUMENT;
-    }
-    o.data = st.in(a.pdata, elem * rows);
-    o.nulls = (const uint64_t *)st.in(a.pnulls, a.pnulls ? ((rows + 63) / 64) * 8 : 0);
-    if (elem == MO_VARLENA_SZ && a.parea && a.areaSz) { o.area = (const uint8_t *)st.in(a.parea, a.areaSz); o.area_sz = a.areaSz; }
-    return st.failed ? MO_RC_INTERNAL_ERROR : MO_RC_SUCCESS;
-}
-// stages the operand args[k] of a len-row call: a const one is one element
-inline int stage_operand(Stager &st, const mo_xcall_args_t &a, size_t elem, uint64_t len, const char *what, int k, Operand &o) {
-    o = Operand{};
-    o.cst = is_const(a, elem, len);
-    return stage_rows(st, a, elem, o.cst ? 1 : len, what, k, o);
-}
+// ---- operands: Operand, is_const, stage_operand and stage_rows (column.cuh)
 
 // ---- IN / NOT IN (goelem.cu, strpred.cu): the list of args[2] with nvalues from the mo_in_params_t of args[3]; the set's hash table has
 // the least power-of-two slot count >= 2 * nvalues (load <= 1/2, so kt_find / kt_find_str always meet an empty slot), and the probe copies
@@ -156,49 +125,6 @@ template <typename T> __device__ __forceinline__ bool cmp_op(T x, T y, int op) {
     case CMP_GT: return x > y;  case CMP_GE: return x >= y;
     case CMP_LT: return x < y;  default: return x <= y;
     }
-}
-#endif
-
-// ---- varlena values (strpred.cu, caseexpr.cu)
-#ifdef __CUDACC__
-// A value.  An inline one (<= 23 bytes) stays in the three registers of its cell load; a long one is read from the area.
-struct Str {
-    uint64_t w0, w1, w2;
-    const uint8_t *p;
-    uint32_t len;
-    bool inl;
-    __device__ __forceinline__ uint32_t at(uint32_t j) const {
-        if (inl) {
-            const uint32_t k = j + 1;
-            const uint64_t w = k < 8 ? w0 : (k < 16 ? w1 : w2);
-            return (uint32_t)(w >> (8 * (k & 7))) & 0xffu;
-        }
-        return __ldg(p + j);
-    }
-};
-
-// false: a non-inline cell without an area or outside it -- varlena_ref's rule (common.cuh), restated because varlena_ref returns a pointer
-// into the cell for an inline value, and reading it back byte by byte would load the cell again; here the cell is loaded once as three
-// 8-byte words and an inline value is read out of those registers (Str::at).
-__device__ __forceinline__ bool load_str(const Operand &c, uint64_t row, Str &s) {
-    const uint8_t *cell = (const uint8_t *)c.data + 24 * (c.cst ? 0 : row);
-    if ((reinterpret_cast<uintptr_t>(c.data) & 7) == 0) {
-        const uint64_t *q = reinterpret_cast<const uint64_t *>(cell);
-        s.w0 = __ldg(q); s.w1 = __ldg(q + 1); s.w2 = __ldg(q + 2);
-    } else {
-        s.w0 = s.w1 = s.w2 = 0;
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            s.w0 |= (uint64_t)__ldg(cell + k) << (8 * k);
-            s.w1 |= (uint64_t)__ldg(cell + 8 + k) << (8 * k);
-            s.w2 |= (uint64_t)__ldg(cell + 16 + k) << (8 * k);
-        }
-    }
-    const uint32_t b0 = (uint32_t)(s.w0 & 0xff);
-    if (b0 <= MO_VARLENA_INLINE_SZ) { s.inl = true; s.len = b0; s.p = nullptr; return true; }
-    const uint32_t off = (uint32_t)(s.w0 >> 32), len = (uint32_t)s.w1;
-    s.inl = false; s.len = len; s.p = c.area + off;
-    return c.area && (uint64_t)off + len <= c.area_sz;
 }
 #endif
 

@@ -43,7 +43,7 @@
 // makes that set approach len: correct, no faster than the full sort.  String keys with a common leading prefix of 8 bytes or more (or 7 after
 // a NULL flag) are such a case.
 #include "common.cuh"
-#include "varlena.cuh"
+#include "column.cuh"
 #include <cstring>
 
 namespace mob {
@@ -453,7 +453,7 @@ __global__ void __launch_bounds__(kThreads) select_flag_kernel(OrderSpec S, uint
     }
 }
 
-// ---- varlena keys: the one read-back record (varlena.cuh), and the run numbers of a sort by rounds -----------------------------------------
+// ---- varlena keys: the one read-back record (column.cuh), and the run numbers of a sort by rounds -----------------------------------------
 __global__ void __launch_bounds__(kThreads)
 varlena_stat_kernel(const uint8_t *__restrict__ cells, const uint64_t *__restrict__ nulls, const uint8_t *area, uint64_t area_sz, uint64_t n,
                     VarlenaStat *vs, int k) {
@@ -549,15 +549,18 @@ run_number_kernel(Pairs<uint64_t> B, const uint64_t *__restrict__ m_ptr, const R
     }
 }
 
-int segment_bits(int T) { return 8 * key_type_size(T); }
-
 }  // namespace
 
 namespace mob {
 
-int varlena_stat(ThreadCtx &t, const uint8_t *cells, const uint64_t *nulls, const uint8_t *area, uint64_t area_sz, uint64_t n, VarlenaStat *vs, int k) {
-    varlena_stat_kernel<<<grid_for(n), kThreads, 0, t.stream>>>(cells, nulls, area, area_sz, n, vs, k);
-    MOB_LAUNCH_CHECK();
+int varlena_stats(ThreadCtx &t, const Operand *col, const int *type, int n, uint64_t len, VarlenaStat *vs) {
+    for (int k = 0; k < n; k++) {
+        if (!is_varlena(type[k])) continue;
+        const Operand &c = col[k];
+        const uint64_t rows = c.cst ? 1 : len;
+        varlena_stat_kernel<<<grid_for(rows), kThreads, 0, t.stream>>>((const uint8_t *)c.data, c.nulls, c.area, c.area_sz, rows, vs, k);
+        MOB_LAUNCH_CHECK();
+    }
     return MO_RC_SUCCESS;
 }
 
@@ -603,30 +606,26 @@ int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
     int bit = 0, ns = 0;
     Stager st(t);
     OrderSeg base[MO_ORDER_MAX_KEYS];
+    Operand key[MO_ORDER_MAX_KEYS];
+    int type[MO_ORDER_MAX_KEYS];
     bool has_var = false, ext = false;   // ext: a varlena or UUID key, order_word<true>
     for (int k = 0; k < P.nkeys; k++) {
         const mo_xcall_args_t &a = args[2 + k];
-        const int T = P.key[k].col_type, fl = P.key[k].flags;
+        const int T = type[k] = P.key[k].col_type, fl = P.key[k].flags;
         const bool var = is_varlena(T);
-        const int vbits = var ? 8 * MO_VARLENA_SZ : segment_bits(T);
-        if (!vbits) { st.finish(); set_error("order sels: key %d has unsupported type %d", k, T); return MO_RC_INVALID_ARGUMENT; }
-        const uint64_t esz = (uint64_t)vbits / 8;
-        const bool cst = len != 1 && a.dataSz == esz;
-        if (!cst && a.dataSz < esz * len) { st.finish(); set_error("order sels: key %d holds %llu bytes, %llu needed", k, (unsigned long long)a.dataSz, (unsigned long long)(esz * len)); return MO_RC_INVALID_ARGUMENT; }
-        if ((len || cst) && !a.pdata) { st.finish(); set_error("order sels: key %d has no data", k); return MO_RC_INVALID_ARGUMENT; }
+        const uint64_t esz = key_elem_size(T);
+        if (!esz) { st.finish(); set_error("order sels: key %d has unsupported type %d", k, T); return MO_RC_INVALID_ARGUMENT; }
+        if (!is_const(a, esz, len) && a.dataSz < esz * len) { st.finish(); set_error("order sels: key %d holds %llu bytes, %llu needed", k, (unsigned long long)a.dataSz, (unsigned long long)(esz * len)); return MO_RC_INVALID_ARGUMENT; }
+        if (!a.pdata && (len || a.dataSz == esz)) { st.finish(); set_error("order sels: key %d has no data", k); return MO_RC_INVALID_ARGUMENT; }
+        // the checks above are the call's own; stage_operand's size check cannot fail after them
+        if (len) { if (int rc = stage_operand(st, a, esz, len, "order sels", 2 + k, key[k])) return rc; }
         const bool desc = (fl & MO_ORDER_DESC) != 0;
         const bool nulls_last = (fl & MO_ORDER_NULLS_FIRST) ? false : (fl & MO_ORDER_NULLS_LAST) ? true : desc;
-        const uint64_t rows = cst ? 1 : len;
-        const uint8_t *col = (const uint8_t *)st.in(a.pdata, cst ? esz : esz * len);
-        const uint64_t *nulls = (const uint64_t *)st.in(a.pnulls, a.pnulls ? ((rows + 63) / 64) * 8 : 0);
         OrderSeg &b = base[k];
         b = OrderSeg{};
         // BIT, YEAR and ENUM order as their storage types uint64, int16 and uint16
-        b.col = col; b.nulls = nulls; b.type = T == MO_T_BIT ? MO_T_UINT64 : T == MO_T_YEAR ? MO_T_INT16 : T == MO_T_ENUM ? MO_T_UINT16 : T; b.cst = cst; b.desc = desc; b.nulls_last = nulls_last; b.bits = vbits;
-        if (var && a.parea && a.areaSz) {
-            b.area = (const uint8_t *)st.in(a.parea, a.areaSz);
-            b.area_sz = a.areaSz;
-        }
+        b.col = (const uint8_t *)key[k].data; b.nulls = key[k].nulls; b.area = key[k].area; b.area_sz = key[k].area_sz; b.cst = key[k].cst;
+        b.type = T == MO_T_BIT ? MO_T_UINT64 : T == MO_T_YEAR ? MO_T_INT16 : T == MO_T_ENUM ? MO_T_UINT16 : T; b.desc = desc; b.nulls_last = nulls_last; b.bits = 8 * (int)esz;
         has_var = has_var || var;
         ext = ext || var || T == MO_T_UUID;
     }
@@ -636,13 +635,9 @@ int xcall_order_sels(mo_xcall_args_t *args, uint64_t len) {
         VarlenaStat *vs = (VarlenaStat *)st.tmp(sizeof(VarlenaStat));
         if (st.failed) return MO_RC_INTERNAL_ERROR;
         MOB_CUDA_TRY(cudaMemsetAsync(vs, 0, sizeof(VarlenaStat), t.stream));
-        for (int k = 0; k < P.nkeys; k++) {
-            if (!is_varlena(base[k].type)) continue;
-            const uint64_t rows = base[k].cst ? 1 : len;
-            int rc = varlena_stat(t, base[k].col, base[k].nulls, base[k].area, base[k].area_sz, rows, vs, k);
-            if (rc) { st.finish(); return rc; }
-        }
-        int rc = read_back(t, &vstat, vs, sizeof vstat);
+        int rc = varlena_stats(t, key, type, P.nkeys, len, vs);
+        if (rc) { st.finish(); return rc; }
+        rc = read_back(t, &vstat, vs, sizeof vstat);
         if (rc) { st.finish(); return rc; }
         rc = varlena_stat_error(vstat, P.nkeys, "order sels: key");
         if (rc) { st.finish(); return rc; }

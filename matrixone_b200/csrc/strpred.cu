@@ -28,9 +28,6 @@ enum { LIKE_EXACT = 0, LIKE_PREFIX, LIKE_SUFFIX, LIKE_CHAIN };
 constexpr int32_t kAny1 = -1, kAnySeq = -2;   // tier-B tokens; a literal rune is its code point (>= 0)
 constexpr int32_t kRuneError = 0xFFFD;
 
-// one varlena operand as the kernels see it: the cells at data (cst: a const vector, every row reads cell 0), its area and its nulls
-using StrCol = Operand;
-
 // ~(lowest row whose cell points outside its area) per operand, 0 = none
 struct Status { unsigned long long bad_inv[2]; };
 
@@ -131,7 +128,7 @@ __device__ __forceinline__ bool glob_match(const Str &v, const P &pat) {
 // ---- the per-row predicates: value of row i; bad1 / bad2 set when that operand's cell is bad (the row is then not written)
 struct CmpPred {
     int op;
-    __device__ __forceinline__ bool operator()(const StrCol &a, const StrCol &b, uint64_t i, const uint8_t *, bool &bad1, bool &bad2) const {
+    __device__ __forceinline__ bool operator()(const Operand &a, const Operand &b, uint64_t i, const uint8_t *, bool &bad1, bool &bad2) const {
         Str x, y;
         bad1 = !load_str(a, i, x); bad2 = !load_str(b, i, y);
         if (bad1 || bad2) return false;
@@ -146,7 +143,7 @@ struct CmpPred {
 // SUFFIX: v[len - e - L, len - e) == lit (both need len >= s + L + e) ; CHAIN: ordered bytes.Index of every segment
 struct LikeAPred {
     int mode; uint32_t s, e, nseg;
-    __device__ __forceinline__ bool operator()(const StrCol &a, const StrCol &, uint64_t i, const uint8_t *aux, bool &bad1, bool &bad2) const {
+    __device__ __forceinline__ bool operator()(const Operand &a, const Operand &, uint64_t i, const uint8_t *aux, bool &bad1, bool &bad2) const {
         Str v;
         bad2 = false; bad1 = !load_str(a, i, v);
         if (bad1) return false;
@@ -170,7 +167,7 @@ struct LikeAPred {
 };
 struct LikeBConstPred {      // aux = int32 tokens [ntok]
     uint32_t ntok;
-    __device__ __forceinline__ bool operator()(const StrCol &a, const StrCol &, uint64_t i, const uint8_t *aux, bool &bad1, bool &bad2) const {
+    __device__ __forceinline__ bool operator()(const Operand &a, const Operand &, uint64_t i, const uint8_t *aux, bool &bad1, bool &bad2) const {
         Str v;
         bad2 = false; bad1 = !load_str(a, i, v);
         if (bad1) return false;
@@ -178,7 +175,7 @@ struct LikeBConstPred {      // aux = int32 tokens [ntok]
     }
 };
 struct LikeBColPred {
-    __device__ __forceinline__ bool operator()(const StrCol &a, const StrCol &b, uint64_t i, const uint8_t *, bool &bad1, bool &bad2) const {
+    __device__ __forceinline__ bool operator()(const Operand &a, const Operand &b, uint64_t i, const uint8_t *, bool &bad1, bool &bad2) const {
         Str v, p;
         bad1 = !load_str(a, i, v); bad2 = !load_str(b, i, p);
         if (bad1 || bad2) return false;
@@ -190,7 +187,7 @@ struct LikeBColPred {
 // The loop runs to a multiple of 64 so that every word of the bitmap is written whole (bits past n cleared).
 template <class P>
 __global__ void __launch_bounds__(kThreads)
-str_row_kernel(uint8_t *__restrict__ r, uint32_t *__restrict__ rn32, uint64_t n, StrCol a, StrCol b, P pred, const uint8_t *aux, uint32_t aux_len,
+str_row_kernel(uint8_t *__restrict__ r, uint32_t *__restrict__ rn32, uint64_t n, Operand a, Operand b, P pred, const uint8_t *aux, uint32_t aux_len,
                int all_null, Status *st) {
     extern __shared__ __align__(16) uint8_t sm_aux[];
     const uint8_t *ax = aux;
@@ -229,7 +226,7 @@ Status *arm_status(ThreadCtx &t, Stager &st, const char *what) {
 
 // enqueues the row kernel over the device aux block, reads back the status record dst and names the lowest bad cell
 template <class P>
-int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, const StrCol &a, const StrCol &b, const P &pred,
+int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, const Operand &a, const Operand &b, const P &pred,
              const uint8_t *aux, uint32_t aux_len, int all_null, const char *what, Status *dst) {
     const size_t smem = aux_len && aux_len <= kSmemAux ? aux_len : 0;
     cudaEventRecord(t.kev0, t.stream);
@@ -250,7 +247,7 @@ int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, c
 }
 // the same with a host aux block (a const pattern), uploaded first
 template <class P>
-int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, const StrCol &a, const StrCol &b, const P &pred,
+int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, const Operand &a, const Operand &b, const P &pred,
              const std::vector<uint8_t> &aux_host, int all_null, const char *what) {
     uint8_t *aux = nullptr;
     const uint32_t aux_len = (uint32_t)aux_host.size();
@@ -269,14 +266,14 @@ int run_rows(ThreadCtx &t, Stager &st, uint8_t *r, uint64_t *rn, uint64_t len, c
 
 // ---- IN / NOT IN (opOperatorStrIn): Go's map[string]bool of the list as kt_insert_str words (an XXH3 tag and the list index of the value)
 // in mask + 1 slots, which the row kernel takes as its aux block -- in shared memory up to kSmemAux (== kInSmemBytes) bytes
-__device__ __forceinline__ uint64_t str_hash_of(const StrCol &c, uint64_t row, const Str &s) {
+__device__ __forceinline__ uint64_t str_hash_of(const Operand &c, uint64_t row, const Str &s) {
     const uint8_t *p = s.inl ? (const uint8_t *)c.data + 24 * (c.cst ? 0 : row) + 1 : s.p;
     return xxh3::hash_bytes(p, s.len, 0).lo;
 }
 __device__ __forceinline__ bool str_eq(const Str &x, const Str &y) { return x.len == y.len && str_cmp(x, y) == 0; }
 
 // list element j (not NULL) into the set; a bad cell is recorded as operand 2's
-__global__ void __launch_bounds__(kThreads) in_str_build_kernel(uint64_t *slots, uint64_t mask, StrCol l, uint64_t m, Status *st) {
+__global__ void __launch_bounds__(kThreads) in_str_build_kernel(uint64_t *slots, uint64_t mask, Operand l, uint64_t m, Status *st) {
     for (uint64_t j = blockIdx.x * (uint64_t)kThreads + threadIdx.x; j < m; j += (uint64_t)gridDim.x * kThreads) {
         Str v;
         if (bm_test(l.nulls, j)) continue;
@@ -288,7 +285,7 @@ __global__ void __launch_bounds__(kThreads) in_str_build_kernel(uint64_t *slots,
 // b = the list (its nulls are the build's, not the row kernel's); aux = the slots, none for the empty set
 struct InPred {
     uint64_t mask; int negate;
-    __device__ __forceinline__ bool operator()(const StrCol &a, const StrCol &b, uint64_t i, const uint8_t *aux, bool &bad1, bool &bad2) const {
+    __device__ __forceinline__ bool operator()(const Operand &a, const Operand &b, uint64_t i, const uint8_t *aux, bool &bad1, bool &bad2) const {
         Str x;
         uint32_t row;
         bad2 = false; bad1 = !load_str(a, i, x);
@@ -306,12 +303,13 @@ int read_const_pattern(ThreadCtx &t, const mo_xcall_args_t &a, std::string &pat,
     if (is_null) return MO_RC_SUCCESS;
     uint8_t cell[MO_VARLENA_SZ];
     if (int rc = read_const(t, cell, a.pdata, MO_VARLENA_SZ)) return rc;
-    if (cell[0] <= MO_VARLENA_INLINE_SZ) { pat.assign((const char *)cell + 1, cell[0]); return MO_RC_SUCCESS; }
-    uint32_t off, len;
-    memcpy(&off, cell + 4, 4); memcpy(&len, cell + 8, 4);
-    if (!a.parea || (uint64_t)off + len > a.areaSz) { set_error("go like: operand 2 row 0: varlena cell outside its area"); return MO_RC_INVALID_ARGUMENT; }
-    pat.resize(len);
-    return read_const(t, &pat[0], a.parea + off, len);
+    uint32_t w[3];
+    memcpy(w, cell, sizeof w);
+    const VarlenaCell v = varlena_cell(w[0], w[1], w[2], a.parea, a.areaSz);
+    if (!v.ok) { set_error("go like: operand 2 row 0: varlena cell outside its area"); return MO_RC_INVALID_ARGUMENT; }
+    if (v.inl) { pat.assign((const char *)cell + 1, v.len); return MO_RC_SUCCESS; }
+    pat.resize(v.len);
+    return read_const(t, &pat[0], a.parea + v.off, v.len);
 }
 
 // functionUtil.RemoveEscapeChar: `\x` -> x; a trailing lone backslash is kept
@@ -423,7 +421,7 @@ int go_str_in(ThreadCtx &t, int negate, mo_xcall_args_t *args, uint64_t len) {
         in_str_build_kernel<<<grid_rows(m, kCtasPerSm), kThreads, 0, t.stream>>>(slots, mask, l, m, dst);
         MOB_LAUNCH_CHECK();
     }
-    StrCol lb = l;
+    Operand lb = l;
     lb.nulls = nullptr;
     return run_rows(t, st, r, rn, len, a, lb, InPred{mask, negate}, (const uint8_t *)slots, (uint32_t)std::min<uint64_t>(bytes, 0xffffffffu), 0,
                     what, dst);

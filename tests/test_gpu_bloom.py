@@ -6,6 +6,7 @@ import os
 import numpy as np
 import pytest
 
+import cell_edges as E
 from matrixone_b200 import capi
 from matrixone_b200.vector import bitmap_from_bools, varlena_column
 
@@ -135,6 +136,43 @@ def test_varlena_cells_all_length_classes(libs):
     ours.bloomfilter_test_and_add_varlena(a, _p(pcells), pcells.nbytes, 24, n, _p(parea), parea.nbytes, None, 0, _p(ra))
     ref.bloomfilter_test_and_add_varlena(b, _p(pcells), pcells.nbytes, 24, n, _p(parea), parea.nbytes, None, 0, _p(rb))
     assert (ra == rb).all() and _bytes(ours, a) == _bytes(ref, b)
+    ours.bloomfilter_free(a); ref.bloomfilter_free(b)
+    # the cell edges.  A bad cell (ending a byte past the area, or wrapping 32 bits) is skipped, NULL or not: no bit is set and its result
+    # byte is not written; the reference would read out of bounds there, so it is given a good cell whose key is already in the filter.
+    m = 50
+    vals = [bytes([i]) * 40 for i in range(m)]
+    e, ea = E.edges(vals, 5, 6, 7)
+    g = e.reshape(m, 24).copy()
+    g[6] = g[7] = g[0]
+    g = g.reshape(-1)
+    a, b = ours.bloomfilter_init_with_seed(1 << 14, 4, 7), ref.bloomfilter_init_with_seed(1 << 14, 4, 7)
+    ours.bloomfilter_add_varlena(a, _p(e), e.nbytes, 24, m, _p(ea), ea.nbytes, None, 0)
+    ref.bloomfilter_add_varlena(b, _p(g), g.nbytes, 24, m, _p(ea), ea.nbytes, None, 0)
+    assert _bytes(ours, a) == _bytes(ref, b)
+    probe, parea = E.edges([bytes([i]) * 40 for i in range(m - 25, 2 * m - 25)], 5, 6, 7)
+    gp = probe.reshape(m, 24).copy()
+    gp[6] = gp[7] = gp[0]
+    rb = np.zeros(m, np.uint8)
+    ref.bloomfilter_test_varlena(b, _p(gp), gp.nbytes, 24, m, _p(parea), parea.nbytes, None, 0, _p(rb))
+    good = ~np.isin(np.arange(m), [6, 7])
+    null6 = bitmap_from_bools(np.arange(m) == 6)
+    for nl in (None, null6):
+        ra = np.full(m, 9, np.uint8)
+        ours.bloomfilter_test_varlena(a, _p(probe), probe.nbytes, 24, m, _p(parea), parea.nbytes, _p(nl), 0 if nl is None else nl.nbytes, _p(ra))
+        assert (ra[~good] == 9).all() and (ra[good] == rb[good]).all()
+    for shift in E.SHIFTS:                                       # device cells 8-byte but not 16-byte aligned, and 1-byte misaligned
+        owner, dc = E.on_device(probe, shift)
+        ra = np.full(m, 9, np.uint8)
+        ours.bloomfilter_test_varlena(a, dc.ptr, probe.nbytes, 24, m, _p(parea), parea.nbytes, None, 0, _p(ra))
+        owner.free()
+        assert (ra[~good] == 9).all() and (ra[good] == rb[good]).all(), shift
+    ra = np.full(m, 9, np.uint8)                                 # non-inline cells without an area: every row skipped
+    ours.bloomfilter_test_varlena(a, _p(probe), probe.nbytes, 24, m, None, 0, None, 0, _p(ra))
+    assert (ra == 9).all()
+    for k in (1, 2):                                             # one cell: rows past the key buffer are not touched
+        ra = np.full(k, 9, np.uint8)
+        ours.bloomfilter_test_varlena(a, _p(probe), 24, 24, k, _p(parea), parea.nbytes, None, 0, _p(ra))
+        assert ra[0] == rb[0] and (ra[1:] == 9).all()
     ours.bloomfilter_free(a); ref.bloomfilter_free(b)
 
 

@@ -9,8 +9,9 @@ import numpy as np
 import pytest
 
 import case_reference as R
+import cell_edges as E
 from matrixone_b200 import capi, ops
-from matrixone_b200.vector import DeviceBuffer, bitmap_from_bools, bitmap_to_bools, varlena_bytes_column
+from matrixone_b200.vector import DeviceBuffer, Vector, bitmap_from_bools, bitmap_to_bools, varlena_bytes_column, xcall
 from test_gpu_go_operands import ONE_NULL, Arg, call, rand_bits, words
 
 torch = pytest.importorskip("torch")
@@ -215,6 +216,35 @@ def test_bad_cells_only_where_chosen(gpu, device):
     rc, msg, _, _, out = call(gpu, capi.XCALL_GO_CASE(capi.T_VARCHAR), args, n, device=device)
     assert rc == 0, msg
     assert out[(0, "pdata")] == R.str_bytes(vals, bytes(24 * n))[0]
+    if not device:
+        return
+    # THEN cells on the device 8-byte but not 16-byte aligned (three 8-byte loads) and 1-byte misaligned (byte loads); a value that ends
+    # at the area's end is good, one a byte past it or whose end wraps 32 bits is not
+    vals = [b"%03d" % i * 10 for i in range(n)]
+    c = (np.arange(n) % 3 == 0).astype(np.uint8)
+    ec, ea = E.edges(vals, 6, None, None)
+    els, elsa = varlena_bytes_column([b"else value longer than the inline cell"])
+
+    def case(then_ptr):
+        r, rn, rarea = np.zeros(24 * n, np.uint8), np.zeros(words(n), np.uint64), np.zeros(40 * n, np.uint8)
+        prm = np.frombuffer(bytes(capi.CaseParams(1, 1, 0)), np.uint8).copy()
+        vecs = [Vector(data=r, nulls=rn, area=rarea, length=n), Vector(data=prm), Vector(data=c, length=n),
+                Vector(data=ec if then_ptr is None else None, data_ptr=then_ptr, data_nbytes=ec.nbytes, area=ea, length=n),
+                Vector(data=els, area=elsa, length=n)]
+        rc, msg = xcall(capi.XCALL_GO_CASE(capi.T_VARCHAR), vecs, n, raise_on_error=False)
+        return rc, msg, r.tobytes() + rarea.tobytes()
+
+    rc, msg, want = case(None)
+    assert rc == 0, msg
+    for shift in E.SHIFTS:
+        for cells, bad_row in ((ec, None), (E.edges(vals, 6, 9, 30)[0], 9), (E.edges(vals, 6, None, 12)[0], 12)):
+            owner, dc = E.on_device(cells, shift)
+            rc, msg, got = case(dc.ptr)
+            owner.free()
+            if bad_row is None:
+                assert rc == 0 and got == want, (shift, msg)
+            else:
+                assert rc == capi.RC_INVALID_ARGUMENT and "operand 3 row %d" % bad_row in msg, (shift, msg)
 
 
 def test_ten_million_rows(gpu):

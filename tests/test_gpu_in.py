@@ -7,6 +7,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import cell_edges as E
 import in_reference as R
 from matrixone_b200 import capi, ops
 from matrixone_b200.vector import DeviceBuffer, bitmap_from_bools, bitmap_to_bools, varlena_bytes_column
@@ -317,3 +318,26 @@ def test_bad_cells_are_named(gpu):
     skip = np.zeros(n, bool); skip[[7, 19, 200]] = True                    # skipped rows are not read
     got, gn = ops.go_in(capi.T_VARCHAR, _bad(col, [7, 19, 200]), vals, rnulls=bitmap_from_bools(skip))
     assert (gn == skip).all() and not got[~skip].any()
+    # device column cells 8-byte but not 16-byte aligned (three 8-byte loads) and 1-byte misaligned (byte loads); a value that ends at the
+    # area's end is good, one a byte past it or whose end wraps 32 bits is not
+    col = [b"%03d" % (i % 70) * 10 for i in range(n)]
+    vals = [b"%03d" % i * 10 for i in range(0, 100, 2)]
+    want, _ = ops.go_in(capi.T_VARCHAR, col, vals)
+    want[5] = want[-1]
+    cells, area = E.edges(col, 5, None, None)
+    lc, la = varlena_bytes_column(vals)
+    dlc, dla, darea = DeviceBuffer.from_numpy(lc), DeviceBuffer.from_numpy(la), DeviceBuffer.from_numpy(area)
+    for shift in E.SHIFTS:
+        for c, bad_row in ((cells, None), (E.edges(col, 5, 19, 40)[0], 19), (E.edges(col, 5, None, 23)[0], 23)):
+            owner, dc = E.on_device(c, shift)
+            out, outn = DeviceBuffer(n), DeviceBuffer.from_numpy(np.zeros((n + 63) // 64, np.uint64))
+            if bad_row is None:
+                ops.go_in_device(capi.T_VARCHAR, (dc, darea), (dlc, dla), m, n, out, outn)
+                assert (out.to_numpy(np.uint8).astype(bool) == want).all(), shift
+            else:
+                with pytest.raises(capi.MoError, match="operand 1 row %d" % bad_row):
+                    ops.go_in_device(capi.T_VARCHAR, (dc, darea), (dlc, dla), m, n, out, outn)
+            for x in (owner, out, outn):
+                x.free()
+    for x in (dlc, dla, darea):
+        x.free()

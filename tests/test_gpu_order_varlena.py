@@ -332,6 +332,34 @@ def test_bad_cells_are_rejected_with_the_lowest_row(gpu):
     assert rc == capi.RC_INVALID_ARGUMENT and msg
     rc, _ = call(cells[:24 * 50], area)                    # short cells
     assert rc == capi.RC_INVALID_ARGUMENT
+    # the cell rule's edges: a value that ends at the area's end is good, one whose end wraps 32 bits is not
+    e = cells.reshape(n, 24).copy()
+    e.view(np.uint32)[17, 1], e.view(np.uint32)[17, 2] = len(area) - len(v[-1]), len(v[-1])
+    assert call(e.reshape(-1), area)[0] == 0 and (sels == _want([v[:17] + [v[-1]] + v[18:]], [None], [0], n)).all()
+    e.view(np.uint32)[5, 1], e.view(np.uint32)[5, 2] = 0xFFFFFFF0, 0x20
+    rc, msg = call(e.reshape(-1), area)
+    assert rc == capi.RC_INVALID_ARGUMENT and "key 0 row 5" in msg, msg
+    # device cells 8-byte but not 16-byte aligned, and 1-byte misaligned
+    for off in (8, 1):
+        buf = DeviceBuffer(c.nbytes + 16)
+        dv = buf.view(c.nbytes, off)
+        capi.check(buf.lib.MoB200_Upload(dv.ptr, c.ctypes.data, c.nbytes), buf.lib)
+        vecs = [Vector(data=sels, length=n), ops._params_vec(ops._order_params([capi.T_VARCHAR], [0], -1, False)),
+                Vector(data_ptr=dv.ptr, data_nbytes=c.nbytes, area=area, length=n)]
+        rc, msg = xcall(capi.XCALL_ORDER_SELS, vecs, n, raise_on_error=False)
+        assert rc == capi.RC_INVALID_ARGUMENT and "key 0 row 17" in msg, (off, msg)
+        capi.check(buf.lib.MoB200_Upload(dv.ptr, cells.ctypes.data, cells.nbytes), buf.lib)
+        assert xcall(capi.XCALL_ORDER_SELS, vecs, n, raise_on_error=False)[0] == 0 and (sels == _want([v], [None], [0], n)).all()
+        buf.free()
+    # one cell: a const key at len 2, a one-row column at len 1 -- both read cell 0
+    for m in (1, 2):
+        out = np.full(m, -1, np.int64)
+        for cell, rc_want in ((cells[:24], 0), (c.reshape(-1)[17 * 24:18 * 24], capi.RC_INVALID_ARGUMENT)):
+            vecs = [Vector(data=out, length=m), ops._params_vec(ops._order_params([capi.T_VARCHAR], [0], -1, False)),
+                    Vector(data=cell.copy(), area=area, length=m)]
+            rc, msg = xcall(capi.XCALL_ORDER_SELS, vecs, m, raise_on_error=False)
+            assert rc == rc_want and (rc == 0 or "key 0 row 0" in msg), (m, msg)
+            assert rc or list(out) == list(range(m))
 
 
 @pytest.mark.parametrize("T", [capi.T_BIT, capi.T_YEAR, capi.T_ENUM, capi.T_UUID])

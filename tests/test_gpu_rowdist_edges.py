@@ -14,10 +14,11 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import cell_edges as E
 import oracle_lib as O
 import rowdist_columns as R
 from matrixone_b200 import capi
-from matrixone_b200.vector import DeviceBuffer, Vector, bitmap_from_bools, varlena_column_from_matrix, xcall
+from matrixone_b200.vector import DeviceBuffer, Vector, bitmap_from_bools, varlena_bytes_column, varlena_column_from_matrix, xcall
 
 pytestmark = pytest.mark.gpu
 
@@ -415,3 +416,53 @@ def test_error_rows_in_a_valid_warp(gpu, dt):
     ce = R.Column(rows, dt, col.stores(), [(3 * i + 1) % 16 for i in range(col.n)])
     rc, msg, _, _ = _normalize_call(dt, ce, ce.n)
     assert rc != 0 and "empty" in msg, msg
+    # the cell edges: a vector that ends at the area's end is good; one that ends a byte past it, or whose end wraps 32 bits, is not
+    m = 40
+    rng = np.random.default_rng(3)
+    rows = [rng.standard_normal(8).astype(dt) for _ in range(m)]
+    vals = [r.tobytes() for r in rows]
+    qc, qa = varlena_bytes_column([vals[0]])
+
+    def l2(cells, area, n=m, nulls=None, dev=None):
+        res = np.full(n, SENT)
+        xv = Vector(data=cells, area=area, length=n) if dev is None else Vector(data_ptr=dev.ptr, data_nbytes=dev.nbytes, area=area, length=n)
+        rc, msg = xcall(FID[dt][R.L2SQ], [Vector(data=res, nulls=None if nulls is None else bitmap_from_bools(nulls), length=n), xv,
+                                          Vector(data=qc, area=qa, length=n)], n, raise_on_error=False)
+        return rc, msg, res
+
+    def norm(cells, area, n=m, dev=None):
+        oc, oa = np.zeros(24 * n, np.uint8), np.zeros(max(area.nbytes if area is not None else 0, 1), np.uint8)
+        xv = Vector(data=cells, area=area, length=n) if dev is None else Vector(data_ptr=dev.ptr, data_nbytes=dev.nbytes, area=area, length=n)
+        return xcall(NORM_FID[dt], [Vector(data=oc, area=oa, length=n), xv], n, raise_on_error=False)
+
+    cells, area = varlena_bytes_column(vals)
+    rc, msg, base = l2(cells, area)
+    assert rc == 0, msg
+    rc, msg, res = l2(*E.edges(vals, 5, None, None))
+    assert rc == 0 and res[5] == base[-1] and (np.delete(res, 5) == np.delete(base, 5)).all(), msg
+    assert norm(*E.edges(vals, 5, None, None))[0] == 0
+    for past, wrap in ((6, None), (None, 7)):
+        for rc, msg in (l2(*E.edges(vals, None, past, wrap))[:2], norm(*E.edges(vals, None, past, wrap))):
+            assert rc == capi.RC_INVALID_ARGUMENT and "outside" in msg, (past, wrap, msg)
+    nl = np.isin(np.arange(m), [6, 7])                              # bad cells in NULL rows are never read
+    rc, msg, res = l2(*E.edges(vals, None, 6, 7), nulls=nl)
+    assert rc == 0 and (res[nl] == SENT).all() and (res[~nl] == base[~nl]).all(), msg
+    for rc, msg in (l2(cells, None)[:2], norm(cells, None)):       # non-inline cells without an area
+        assert rc == capi.RC_INVALID_ARGUMENT and "outside" in msg, msg
+    e, ea = E.edges(vals, 0, 1, None)                               # one cell: a const at len 2, a one-row column at len 1
+    for k in (1, 2):
+        rc, msg, res = l2(e[:24], ea, n=k)
+        assert rc == 0 and (res == base[-1]).all(), msg
+        assert norm(e[:24], ea, n=k)[0] == 0
+        for rc, msg in (l2(e[24:48], ea, n=k)[:2], norm(e[24:48], ea, n=k)):
+            assert rc == capi.RC_INVALID_ARGUMENT and "outside" in msg, (k, msg)
+    for shift in E.SHIFTS:                                          # device cells 8-byte but not 16-byte aligned, and 1-byte misaligned
+        for c, ok in ((cells, True), (E.edges(vals, None, 6, None)[0], False)):
+            owner, dc = E.on_device(c, shift)
+            rc, msg, res = l2(None, area, dev=dc)
+            nrc, nmsg = norm(None, area, dev=dc)
+            owner.free()
+            if ok:
+                assert rc == 0 and (res == base).all() and nrc == 0, (shift, msg, nmsg)
+            else:
+                assert rc == nrc == capi.RC_INVALID_ARGUMENT and "outside" in msg and "outside" in nmsg, (shift, msg, nmsg)

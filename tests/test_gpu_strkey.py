@@ -5,6 +5,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import cell_edges as E
 import oracle_lib as O
 import strkey_reference as R
 from matrixone_b200 import capi, ops
@@ -106,6 +107,45 @@ def test_pack_errors(gpu):
         ops.pack_str_keys([[b"a", b"b" * 65536]], [capi.T_TEXT])
     with pytest.raises(capi.MoError, match="unsupported type"):
         ops.pack_str_keys([np.zeros(3, np.int64)], [999])
+    # the cell edges: a value that ends at the area's end is good; one that ends a byte past it, or whose end wraps 32 bits, is not
+    types = [capi.T_INT32, capi.T_VARCHAR]
+    want = ops.pack_str_keys([col0, vals[:2] + [vals[-1]] + vals[3:]], types)
+    got = ops.pack_str_keys([col0, E.edges(vals, 2, None, None)], types)
+    assert got[0].tobytes() == want[0].tobytes() and (got[1] == want[1]).all()
+    for past, wrap, row in ((5, None, 5), (None, 4, 4), (6, 3, 3)):
+        with pytest.raises(capi.MoError, match="column 1 row %d" % row):
+            ops.pack_str_keys([col0, E.edges(vals, None, past, wrap)], types)
+    nm = bitmap_from_bools(np.isin(np.arange(n), [3, 6]))          # bad cells in NULL rows are never read
+    got = ops.pack_str_keys([col0, E.edges(vals, None, 6, 3)], types, [None, nm])
+    want = ops.pack_str_keys([col0, vals], types, [None, nm])
+    assert got[0].tobytes() == want[0].tobytes()
+    with pytest.raises(capi.MoError, match="column 1 row 0"):      # non-inline cells without an area
+        ops.pack_str_keys([col0, (cells, None)], types)
+    # one cell: a const column at len 2, a one-row column at len 1
+    e, ea = E.edges(vals, 0, 1, None)
+    for m in (1, 2):
+        got = ops.pack_str_keys([(e[:24], ea)], [capi.T_VARCHAR], length=m)
+        want = ops.pack_str_keys([[vals[-1]] * m], [capi.T_VARCHAR], length=m)
+        assert got[0].tobytes() == want[0].tobytes() and (got[1] == want[1]).all()
+        with pytest.raises(capi.MoError, match="column 0 row 0"):
+            ops.pack_str_keys([(e[24:48], ea)], [capi.T_VARCHAR], length=m)
+    # device cells 8-byte but not 16-byte aligned, and 1-byte misaligned
+    want = ops.pack_str_keys([vals], [capi.T_VARCHAR])
+    darea = DeviceBuffer.from_numpy(area)
+    for shift in E.SHIFTS:
+        for c, bad_row in ((cells, None), (E.edges(vals, None, 7, None)[0], 7)):
+            owner, dc = E.on_device(c, shift)
+            db, do = DeviceBuffer(4096), DeviceBuffer(8 * (n + 1))
+            if bad_row is None:
+                ops.pack_str_keys_device([(dc, darea)], None, [capi.T_VARCHAR], n, db, do)
+                assert db.to_numpy(np.uint8)[:len(want[0])].tobytes() == want[0].tobytes(), shift
+                assert (do.to_numpy(np.uint64, n + 1) == want[1]).all(), shift
+            else:
+                with pytest.raises(capi.MoError, match="column 0 row 7"):
+                    ops.pack_str_keys_device([(dc, darea)], None, [capi.T_VARCHAR], n, db, do)
+            for b in (owner, db, do):
+                b.free()
+    darea.free()
 
 
 def _names(ids):

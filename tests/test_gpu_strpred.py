@@ -7,6 +7,7 @@ import pytest
 from matrixone_b200 import capi, ops
 from matrixone_b200.vector import DeviceBuffer, Vector, bitmap_from_bools, bitmap_to_bools, varlena_bytes_column, xcall
 
+import cell_edges as E
 import like_reference as L
 
 pytestmark = pytest.mark.gpu
@@ -198,6 +199,47 @@ def test_bad_cell_named_at_lowest_row():
     skip = np.zeros(n, bool); skip[[3, 17, 40]] = True            # skipped rows are not read either
     got, gn = ops.like(bad, b"%x%", rnulls=bitmap_from_bools(skip))
     assert (gn == skip).all() and got[~skip].all()
+    # the cell rule's edges: a value that ends at the area's end is good, one whose end wraps 32 bits is not
+    cells, area = varlena_bytes_column(vals)
+    e = cells.reshape(n, 24).copy()
+    u = e.view(np.uint32)
+    u[17, 1], u[17, 2] = area.size - 30, 30
+    got, _ = ops.str_compare(capi.CMP_EQ, capi.T_VARCHAR, vals, (e.reshape(-1), area))
+    assert got.all()
+    u[5, 1], u[5, 2] = 0xFFFFFFF0, 0x20
+    with pytest.raises(capi.MoError, match="operand 2 row 5"):
+        ops.str_compare(capi.CMP_EQ, capi.T_VARCHAR, vals, (e.reshape(-1), area))
+    # a const pattern's cell, read on the host: ending at the area's end is good; a byte past it, a 32-bit wrap or no area is not
+    pats = [b"%" + b"y" * 30 + b"%", b"%" + b"x" * 28 + b"%"]
+    pe, pa = E.edges(pats, 0, 1, None)
+    pw, pwa = E.edges(pats, None, None, 0)
+    for k in (n, 1):                                              # a const at len n; at len 1 the one cell is a column
+        got, _ = ops.like(vals[:k], (pe[:24], pa), length=k)
+        assert got.all()
+        for bad_pat in ((pe[24:48], pa), (pw[:24], pwa), (pe[:24], None)):
+            with pytest.raises(capi.MoError, match="operand 2 row 0"):
+                ops.like(vals[:k], bad_pat, length=k)
+    got, gn = ops.like(vals, (pe[24:48], pa), pattern_nulls=np.array([1], np.uint64))   # a const NULL pattern's cell is never read
+    assert gn.all()
+    # device cells 8-byte but not 16-byte aligned (three 8-byte loads), and 1-byte misaligned (byte loads)
+    b = [v[::-1] + b"!" for v in vals]
+    want, _ = ops.str_compare(capi.CMP_LT, capi.T_TEXT, vals, b)
+    bc, ba = varlena_bytes_column(b)
+    dbc, dba, darea = DeviceBuffer.from_numpy(bc), DeviceBuffer.from_numpy(ba), DeviceBuffer.from_numpy(area)
+    for shift in E.SHIFTS:
+        for c, bad_row in ((cells, None), (E.edges(vals, None, 17, 40)[0], 17)):
+            owner, dc = E.on_device(c, shift)
+            out, outn = DeviceBuffer(n), DeviceBuffer.from_numpy(np.zeros((n + 63) // 64, np.uint64))
+            if bad_row is None:
+                ops.str_compare_device(capi.CMP_LT, capi.T_TEXT, (dc, darea), (dbc, dba), n, out, outn)
+                assert (out.to_numpy(np.uint8).astype(bool) == want).all(), shift
+            else:
+                with pytest.raises(capi.MoError, match="operand 1 row 17"):
+                    ops.str_compare_device(capi.CMP_LT, capi.T_TEXT, (dc, darea), (dbc, dba), n, out, outn)
+            for x in (owner, out, outn):
+                x.free()
+    for x in (dbc, dba, darea):
+        x.free()
 
 
 def test_in_and_not_in_through_the_string_map():

@@ -77,6 +77,7 @@ def order_case(lib, name, cols, nulls, types, flags, n, limit, yard, runs, warmu
     nout = n if limit is None else limit
     out = torch.empty(max(nout, 1), dtype=torch.int64, device="cuda")
     call = lambda: ops.order_sels_device(cols, nulls, types, flags, n, out.data_ptr(), limit=limit)  # noqa: E731
+    torch.cuda.synchronize()   # the columns are written on torch's stream; the library's own stream does not wait for it
     lib_t, yard_t = alternate(runs, warmup, lambda: lib_ms(lib, call), lambda: torch_ms(yard))
     ok = check(out[:nout]) if check else None
     del out
