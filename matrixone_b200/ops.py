@@ -15,41 +15,45 @@ import ctypes as C
 import numpy as np
 
 from . import capi
-from .vector import DeviceBuffer, Vector, bitmap_to_bools, varlena_bytes_column, xcall
+from .vector import VARLENA_SZ, DeviceBuffer, Vector, bitmap_to_bools, varlena_bytes_column, xcall
 
 
-def _vec(x, length=None, itemsize=None):
-    """numpy array / DeviceBuffer / (DeviceBuffer, nbytes) -> Vector"""
-    if isinstance(x, Vector):
-        return x
-    if isinstance(x, DeviceBuffer):
-        return Vector(data_ptr=x.ptr, data_nbytes=x.nbytes, length=length)
-    a = np.ascontiguousarray(x)
-    return Vector(data=a, length=length if length is not None else a.shape[0])
+def _vec(x, length=None, nulls=None, dtype=None):
+    """one input column of a call -> Vector.  x: a numpy array (converted to dtype when one is given), a DeviceBuffer, a (cells, area) pair
+    of either kind (area None: every value inline) or a list of bytes (a varlena column); nulls: bitmap words (numpy) or a DeviceBuffer.
+    Its row count (the bits of its nulls) is length, else the host array's rows (a varlena column's cells)."""
+    if isinstance(x, list):
+        x = varlena_bytes_column(x)
+    data, area = x if isinstance(x, tuple) else (x, None)
+    if isinstance(data, DeviceBuffer):
+        return Vector(data, nulls, area, length=length)
+    if isinstance(x, tuple):
+        data = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1)
+        area = None if area is None else np.ascontiguousarray(area, dtype=np.uint8)
+        rows = data.shape[0] // VARLENA_SZ
+    else:
+        data = np.ascontiguousarray(data, dtype)
+        rows = data.shape[0]
+    return Vector(data, nulls, area, length=rows if length is None else length)
 
 
-def _params_vec(struct):
-    buf = np.frombuffer(bytes(struct), dtype=np.uint8).copy()
+def _params_vec(block):
+    """a parameter block or scalar argument (a ctypes struct or a small numpy array) -> a one-row Vector over a copy of its bytes; a call
+    that writes back into the block (err_row, area_len) is read from the Vector's data"""
+    buf = np.frombuffer(bytes(block), dtype=np.uint8).copy()
     return Vector(data=buf, length=1, const=True)
 
 
 # ------------------------------------------------------------------------------------------------ aggregates
-def _agg(op, T, col, nulls=None, length=None):
+def _agg(op, T, col, nulls, length, words=1):
+    """MO_XCALL_AGG of one column into `words` result words: (rc, result, is_null)"""
     n = length if length is not None else (col.nbytes // np.dtype(capi.NP_OF_T[T]).itemsize if isinstance(col, DeviceBuffer) else len(col))
-    res = np.zeros(1, dtype=np.uint64)
+    res = np.zeros(words, dtype=np.uint64)
     rn = np.zeros(1, dtype=np.uint64)
-    rv = Vector(data=res, nulls=rn, length=1)
-    cv = _vec(col, n)
-    if nulls is not None:
-        if isinstance(nulls, DeviceBuffer):
-            cv.nulls_ptr = nulls.ptr
-        else:
-            cv.nulls = np.ascontiguousarray(nulls, dtype=np.uint64)
-    cv.length = n
-    rc, msg = xcall(capi.XCALL_AGG(op, T), [rv, cv], n, raise_on_error=False)
+    rc, msg = xcall(capi.XCALL_AGG(op, T), [Vector(data=res, nulls=rn, length=1), _vec(col, n, nulls)], n, raise_on_error=False)
     if rc not in (0, capi.RC_OUT_OF_RANGE):
         raise capi.MoError(rc, msg)
-    return rc, res, bool(rv.nulls[0] & np.uint64(1))
+    return rc, res, bool(rn[0] & np.uint64(1))
 
 
 def agg_sum(T, col, nulls=None, length=None):
@@ -89,14 +93,18 @@ def agg_max(T, col, nulls=None, length=None):
 
 
 # ------------------------------------------------------------------------------------------------ TPC-H shapes
+def _scan_args(out, cols, n, params):
+    """the arguments of the fused scans (Q6, Q6 over decimals, Q1): the result, the columns, the parameter block"""
+    return [out] + [_vec(c, n) for c in cols] + [_params_vec(params)]
+
+
 def q6_filter_sum(shipdate, discount, quantity, extendedprice, n, date_lo, date_hi, disc_lo, disc_hi, qty_hi):
     """SUM(l_extendedprice*l_discount) WHERE ... (q6.sql).  Returns (sum, qualifying_rows, is_null)."""
     res = np.zeros(2, dtype=np.float64)
     rn = np.zeros(1, dtype=np.uint64)
-    rv = Vector(data=res, nulls=rn, length=1)
-    p = capi.Q6Params(date_lo, date_hi, disc_lo, disc_hi, qty_hi)
-    xcall(capi.XCALL_Q6_FILTER_SUM, [rv, _vec(shipdate, n), _vec(discount, n), _vec(quantity, n), _vec(extendedprice, n), _params_vec(p)], n)
-    return float(res[0]), int(res.view(np.int64)[1]), bool(rv.nulls[0] & np.uint64(1))
+    xcall(capi.XCALL_Q6_FILTER_SUM, _scan_args(Vector(data=res, nulls=rn, length=1), (shipdate, discount, quantity, extendedprice), n,
+                                               capi.Q6Params(date_lo, date_hi, disc_lo, disc_hi, qty_hi)), n)
+    return float(res[0]), int(res.view(np.int64)[1]), bool(rn[0] & np.uint64(1))
 
 
 Q6_RESULT_BYTES = 16
@@ -107,8 +115,8 @@ def q6_filter_sum_device(shipdate, discount, quantity, extendedprice, n, date_lo
     """asynchronous form: resident columns, result {f64 sum, i64 rows} written to caller-owned DEVICE memory at out_ptr, nothing is
     read back and the calling thread's stream is not synchronised (the partial Group of a multi-GPU scan)"""
     rv = Vector(data_ptr=out_ptr, data_nbytes=Q6_RESULT_BYTES, nulls_ptr=out_nulls_ptr, length=1)
-    p = capi.Q6Params(date_lo, date_hi, disc_lo, disc_hi, qty_hi)
-    xcall(capi.XCALL_Q6_FILTER_SUM, [rv, _vec(shipdate, n), _vec(discount, n), _vec(quantity, n), _vec(extendedprice, n), _params_vec(p)], n)
+    xcall(capi.XCALL_Q6_FILTER_SUM, _scan_args(rv, (shipdate, discount, quantity, extendedprice), n,
+                                               capi.Q6Params(date_lo, date_hi, disc_lo, disc_hi, qty_hi)), n)
 
 
 def q6_merge_device(parts_ptr, nparts, out_ptr, out_nulls_ptr=None):
@@ -140,19 +148,14 @@ def q6_dec_result_from_bytes(raw, null_word=None):
             "is_null": r.count == 0 if null_word is None else bool(int(null_word) & 1)}
 
 
-def _q6_dec_args(rv, shipdate, discount, quantity, extendedprice, n, date_lo, date_hi, disc_lo, disc_hi, qty_hi, scale, row_base):
-    p = capi.Q6DecParams(date_lo, date_hi, disc_lo, disc_hi, qty_hi, scale, 0, row_base)
-    return [rv, _vec(shipdate, n), _vec(discount, n), _vec(quantity, n), _vec(extendedprice, n), _params_vec(p)]
-
-
 def q6_dec_filter_sum(shipdate, discount, quantity, extendedprice, n, date_lo, date_hi, disc_lo, disc_hi, qty_hi, scale, row_base=0):
     """TPC-H Q6 over DECIMAL columns: shipdate int32 days, the three measures Decimal64 (int64 unscaled) at `scale` (0..4), the constants
     already unscaled at `scale`.  Returns the q6_dec_result_from_bytes dict; a Decimal128 Add overflow comes back as rc / err_row (the
     failing row + row_base)."""
     res = np.zeros(Q6_DEC_RESULT_BYTES, dtype=np.uint8)
     rn = np.zeros(1, dtype=np.uint64)
-    rc, msg = xcall(capi.XCALL_Q6_DEC_FILTER_SUM, _q6_dec_args(Vector(data=res, nulls=rn, length=1), shipdate, discount, quantity, extendedprice,
-                                                               n, date_lo, date_hi, disc_lo, disc_hi, qty_hi, scale, row_base), n,
+    rc, msg = xcall(capi.XCALL_Q6_DEC_FILTER_SUM, _scan_args(Vector(data=res, nulls=rn, length=1), (shipdate, discount, quantity, extendedprice), n,
+                                                             capi.Q6DecParams(date_lo, date_hi, disc_lo, disc_hi, qty_hi, scale, 0, row_base)), n,
                     raise_on_error=False)
     if rc not in (0, capi.RC_INVALID_ARGUMENT):
         raise capi.MoError(rc, msg)
@@ -166,8 +169,8 @@ def q6_dec_filter_sum_device(shipdate, discount, quantity, extendedprice, n, dat
                              out_nulls_ptr=None, row_base=0):
     """asynchronous form: resident columns, mo_q6_dec_result_t written to DEVICE memory at out_ptr, nothing read back or synchronised"""
     rv = Vector(data_ptr=out_ptr, data_nbytes=Q6_DEC_RESULT_BYTES, nulls_ptr=out_nulls_ptr, length=1)
-    xcall(capi.XCALL_Q6_DEC_FILTER_SUM, _q6_dec_args(rv, shipdate, discount, quantity, extendedprice, n, date_lo, date_hi, disc_lo, disc_hi,
-                                                     qty_hi, scale, row_base), n)
+    xcall(capi.XCALL_Q6_DEC_FILTER_SUM, _scan_args(rv, (shipdate, discount, quantity, extendedprice), n,
+                                                   capi.Q6DecParams(date_lo, date_hi, disc_lo, disc_hi, qty_hi, scale, 0, row_base)), n)
 
 
 def q6_dec_merge(parts_bytes, nparts):
@@ -206,9 +209,9 @@ def q1_result_from_bytes(raw):
 
 def q1_group_agg_device(shipdate, quantity, extendedprice, discount, tax, returnflag, linestatus, n, cutoff, out_ptr, row_base=0):
     """asynchronous form of q1_group_agg: mo_q1_result_t written to DEVICE memory at out_ptr; first_row values are offset by row_base"""
-    rv = Vector(data_ptr=out_ptr, data_nbytes=Q1_RESULT_BYTES, length=1)
-    xcall(capi.XCALL_Q1_GROUP_AGG, [rv, _vec(shipdate, n), _vec(quantity, n), _vec(extendedprice, n), _vec(discount, n), _vec(tax, n),
-                                     _vec(returnflag, n), _vec(linestatus, n), _params_vec(capi.Q1Params(cutoff, 0, row_base))], n)
+    xcall(capi.XCALL_Q1_GROUP_AGG, _scan_args(Vector(data_ptr=out_ptr, data_nbytes=Q1_RESULT_BYTES, length=1),
+                                              (shipdate, quantity, extendedprice, discount, tax, returnflag, linestatus), n,
+                                              capi.Q1Params(cutoff, 0, row_base)), n)
 
 
 def q1_merge_device(parts_ptr, nparts, out_ptr):
@@ -226,11 +229,8 @@ def q1_merge(parts_bytes, nparts):
 
 def agg_state_device(op, T, col, nulls, n, out_ptr, out_nulls_ptr=None):
     """asynchronous MO_XCALL_AGG: mo_agg_state_t (24 bytes) written to DEVICE memory"""
-    cv = _vec(col, n)
-    if nulls is not None:
-        cv.nulls_ptr = nulls.ptr
-    cv.length = n
-    xcall(capi.XCALL_AGG(op, T), [Vector(data_ptr=out_ptr, data_nbytes=capi.AGG_STATE_BYTES, nulls_ptr=out_nulls_ptr, length=1), cv], n)
+    xcall(capi.XCALL_AGG(op, T), [Vector(data_ptr=out_ptr, data_nbytes=capi.AGG_STATE_BYTES, nulls_ptr=out_nulls_ptr, length=1),
+                                  _vec(col, n, nulls)], n)
 
 
 def agg_merge_device(op, T, parts_ptr, nparts, out_ptr, out_bytes=capi.AGG_STATE_BYTES, out_nulls_ptr=None):
@@ -240,20 +240,7 @@ def agg_merge_device(op, T, parts_ptr, nparts, out_ptr, out_bytes=capi.AGG_STATE
 
 def agg_state(op, T, col, nulls=None, length=None):
     """synchronous partial state (bits, count, rc) of one column"""
-    n = length if length is not None else (col.nbytes // np.dtype(capi.NP_OF_T[T]).itemsize if isinstance(col, DeviceBuffer) else len(col))
-    res = np.zeros(3, dtype=np.uint64)
-    rn = np.zeros(1, dtype=np.uint64)
-    cv = _vec(col, n)
-    if nulls is not None:
-        if isinstance(nulls, DeviceBuffer):
-            cv.nulls_ptr = nulls.ptr
-        else:
-            cv.nulls = np.ascontiguousarray(nulls, dtype=np.uint64)
-    cv.length = n
-    rc, msg = xcall(capi.XCALL_AGG(op, T), [Vector(data=res, nulls=rn, length=1), cv], n, raise_on_error=False)
-    if rc not in (0, capi.RC_OUT_OF_RANGE):
-        raise capi.MoError(rc, msg)
-    return res
+    return _agg(op, T, col, nulls, length, 3)[1]
 
 
 def agg_merge(op, T, states, final=True):
@@ -273,18 +260,10 @@ def agg_merge(op, T, states, final=True):
 def q1_group_agg(shipdate, quantity, extendedprice, discount, tax, returnflag, linestatus, n, cutoff, row_base=0):
     """TPC-H Q1 grouped aggregates (q1.sql).  returnflag/linestatus: packed uint8 columns or varlena cell buffers.
     Returns a list of dicts in first-seen group order."""
-    res = np.zeros(C.sizeof(capi.Q1Result), dtype=np.uint8)
-    rv = Vector(data=res, length=1)
-    cut = _params_vec(capi.Q1Params(cutoff, 0, row_base))
-    xcall(capi.XCALL_Q1_GROUP_AGG, [rv, _vec(shipdate, n), _vec(quantity, n), _vec(extendedprice, n), _vec(discount, n), _vec(tax, n),
-                                     _vec(returnflag, n), _vec(linestatus, n), cut], n)
-    r = capi.Q1Result.from_buffer_copy(res.tobytes())
-    out = []
-    for g in range(r.ngroups):
-        s = r.groups[g]
-        out.append({k: getattr(s, k) for k in ("returnflag", "linestatus", "first_row", "sum_qty", "sum_base_price", "sum_disc_price",
-                                               "sum_charge", "avg_qty", "avg_price", "avg_disc", "sum_disc", "count_order")})
-    return out
+    res = np.zeros(Q1_RESULT_BYTES, dtype=np.uint8)
+    xcall(capi.XCALL_Q1_GROUP_AGG, _scan_args(Vector(data=res, length=1), (shipdate, quantity, extendedprice, discount, tax, returnflag, linestatus),
+                                              n, capi.Q1Params(cutoff, 0, row_base)), n)
+    return _q1_groups(capi.Q1Result.from_buffer_copy(res.tobytes()))
 
 
 # ------------------------------------------------------------------------------------------------ vector search
@@ -296,17 +275,41 @@ def _filter_vec(filt):
     """the mo_search_filter_t argument of a filtered search.  filt: key bitmap words (numpy uint64, host) or a DeviceBuffer of them
     (bit `key` set = admitted), or a bloom filter handle (bloomfilter_t * from the library's bloomfilter_* symbols, as int / c_void_p)"""
     if isinstance(filt, DeviceBuffer):
-        d = capi.SearchFilter(capi.SEARCH_FILTER_KEY_BITMAP, 0, filt.ptr, filt.nbytes // 8)
-        return _params_vec(d), None
+        return _params_vec(capi.SearchFilter(capi.SEARCH_FILTER_KEY_BITMAP, 0, filt.ptr, filt.nbytes // 8))
     if isinstance(filt, np.ndarray):
         w = np.ascontiguousarray(filt, dtype=np.uint64).reshape(-1)
-        d = capi.SearchFilter(capi.SEARCH_FILTER_KEY_BITMAP, 0, w.ctypes.data, w.size)
-        return _params_vec(d), w
+        v = _params_vec(capi.SearchFilter(capi.SEARCH_FILTER_KEY_BITMAP, 0, w.ctypes.data, w.size))
+        v._keep.append(w)                       # the block holds the words' address
+        return v
     if isinstance(filt, C.c_void_p):
         filt = filt.value
     if isinstance(filt, int):
-        return _params_vec(capi.SearchFilter(capi.SEARCH_FILTER_KEY_BLOOM, 0, filt, 0)), None
+        return _params_vec(capi.SearchFilter(capi.SEARCH_FILTER_KEY_BLOOM, 0, filt, 0))
     raise TypeError("filter: numpy uint64 key bitmap, DeviceBuffer key bitmap, or bloom filter handle")
+
+
+def _queries(queries, dim):
+    """(query Vector, nq): float32 rows, resident (DeviceBuffer) or host"""
+    if isinstance(queries, DeviceBuffer):
+        nq = queries.nbytes // (4 * dim)
+        return _vec(queries, nq), nq
+    q = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, dim)
+    return _vec(q.reshape(-1), q.shape[0]), q.shape[0]
+
+
+def _search(fids, out, nq, limit, args, filter):
+    """one top-k search call: fids = (unfiltered, filtered) XCall ids; the keys / distances go to out = (keys_ptr, distances_ptr), device
+    memory the caller owns (returns None, None), or to host arrays that are returned"""
+    if out is not None:
+        keys = dists = None
+        res = [Vector(data_ptr=p, data_nbytes=nq * limit * 8, length=nq) for p in out]
+    else:
+        keys = np.zeros(nq * limit, dtype=np.int64)
+        dists = np.zeros(nq * limit, dtype=np.float64)
+        res = [Vector(data=keys, length=nq), Vector(data=dists, length=nq)]
+    extra = [] if filter is None else [_filter_vec(filter)]
+    xcall(fids[filter is not None], res + args + extra, nq)
+    return keys, dists
 
 
 class BruteForceIndex:
@@ -336,31 +339,13 @@ class BruteForceIndex:
         """out = (keys_device_ptr, distances_device_ptr): results stay in caller-owned device memory (int64 / float64, nq*limit
         each) and nothing is returned -- the form a multi-GPU caller hands straight to NCCL.
         filter: search only the rows whose key (key_base + row) the filter admits (see _filter_vec)"""
-        if isinstance(queries, DeviceBuffer):
-            nq = queries.nbytes // (4 * self.dim)
-            qv = Vector(data_ptr=queries.ptr, data_nbytes=queries.nbytes, length=nq)
-        else:
-            q = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, self.dim)
-            nq = q.shape[0]
-            qv = Vector(data=q.reshape(-1), length=nq)
+        qv, nq = _queries(queries, self.dim)
         if limit == 0 or nq == 0:
             return np.zeros(0, dtype=np.int64), np.zeros(0, dtype=np.float64)
         p = _search_params(self.n, self.dim, nq, limit, self.metric, key_base=self.key_base)
-        dv = Vector(data_ptr=self.buf.ptr, data_nbytes=self.n * self.dim * 4, length=self.n)
-        fid, extra, keep = capi.XCALL_BRUTEFORCE_TOPK_F32, [], None
-        if filter is not None:
-            fv, keep = _filter_vec(filter)
-            fid, extra = capi.XCALL_BRUTEFORCE_TOPK_FILTERED_F32, [fv]
-        if out is not None:
-            kv = Vector(data_ptr=out[0], data_nbytes=nq * limit * 8, length=nq)
-            dvv = Vector(data_ptr=out[1], data_nbytes=nq * limit * 8, length=nq)
-            xcall(fid, [kv, dvv, dv, qv, _params_vec(p)] + extra, nq)
-            return None
-        keys = np.zeros(nq * limit, dtype=np.int64)
-        dists = np.zeros(nq * limit, dtype=np.float64)
-        xcall(fid, [Vector(data=keys, length=nq), Vector(data=dists, length=nq), dv, qv, _params_vec(p)] + extra, nq)
-        del keep
-        return keys, dists
+        keys, dists = _search((capi.XCALL_BRUTEFORCE_TOPK_F32, capi.XCALL_BRUTEFORCE_TOPK_FILTERED_F32), out, nq, limit,
+                              [_vec(self.buf.view(self.n * self.dim * 4), self.n), qv, _params_vec(p)], filter)
+        return None if out is not None else (keys, dists)
 
     def destroy(self):
         if self.buf is not None and getattr(self, "prepared", False):
@@ -453,35 +438,11 @@ class IvfflatSearchIndex:
 
     def search(self, queries, limit, nprobe, sqrt_out=False, out=None, filter=None):
         """filter: search only the entries whose primary key (row id) the filter admits, in the lists the unfiltered search probes"""
-        if isinstance(queries, DeviceBuffer):
-            nq = queries.nbytes // (4 * self.dim)
-            qvec = Vector(data_ptr=queries.ptr, data_nbytes=queries.nbytes, length=nq)
-        else:
-            q = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, self.dim)
-            nq = q.shape[0]
-            qvec = Vector(data=q.reshape(-1), length=nq)
-        if out is not None:     # results stay in caller-owned device memory (see BruteForceIndex.search)
-            keys = dists = None
-            kv = Vector(data_ptr=out[0], data_nbytes=nq * limit * 8, length=nq)
-            dvv = Vector(data_ptr=out[1], data_nbytes=nq * limit * 8, length=nq)
-        else:
-            keys = np.zeros(nq * limit, dtype=np.int64)
-            dists = np.zeros(nq * limit, dtype=np.float64)
-            kv, dvv = Vector(data=keys, length=nq), Vector(data=dists, length=nq)
+        qvec, nq = _queries(queries, self.dim)
         p = _search_params(self.n, self.dim, nq, limit, self.metric, nprobe=nprobe, sqrt_out=int(sqrt_out), nlist=self.nlist)
-        fid, extra, keep = capi.XCALL_IVF_TOPK_F32, [], None
-        if filter is not None:
-            fv, keep = _filter_vec(filter)
-            fid, extra = capi.XCALL_IVF_TOPK_FILTERED_F32, [fv]
-        xcall(fid, [
-            kv, dvv,
-            Vector(data_ptr=self.d_data.ptr, data_nbytes=self.d_data.nbytes, length=self.n),
-            qvec, _params_vec(p),
-            Vector(data_ptr=self.d_cent.ptr, data_nbytes=self.d_cent.nbytes, length=self.nlist),
-            Vector(data_ptr=self.d_off.ptr, data_nbytes=self.d_off.nbytes, length=self.nlist + 1),
-            Vector(data_ptr=self.d_ids.ptr, data_nbytes=self.d_ids.nbytes, length=self.n)] + extra, nq)
-        del keep
-        return keys, dists
+        return _search((capi.XCALL_IVF_TOPK_F32, capi.XCALL_IVF_TOPK_FILTERED_F32), out, nq, limit,
+                       [_vec(self.d_data, self.n), qvec, _params_vec(p), _vec(self.d_cent, self.nlist),
+                        _vec(self.d_off, self.nlist + 1), _vec(self.d_ids, self.n)], filter)
 
     def destroy(self):
         if self.prepared:
@@ -492,51 +453,37 @@ class IvfflatSearchIndex:
 
 def topk_merge_device(keys_ptr, dists_ptr, nshards, nq, k, out_keys_ptr, out_dists_ptr):
     """topk_merge on device-resident [nshards, nq, k] results (e.g. straight out of an NCCL all_gather); outputs stay on the device"""
-    p = _search_params(nshards, 0, nq, k, 0)
     xcall(capi.XCALL_TOPK_MERGE, [Vector(data_ptr=out_keys_ptr, data_nbytes=nq * k * 8, length=nq), Vector(data_ptr=out_dists_ptr, data_nbytes=nq * k * 8, length=nq),
                                   Vector(data_ptr=keys_ptr, data_nbytes=nshards * nq * k * 8, length=nq),
-                                  Vector(data_ptr=dists_ptr, data_nbytes=nshards * nq * k * 8, length=nq), _params_vec(p)], nq)
+                                  Vector(data_ptr=dists_ptr, data_nbytes=nshards * nq * k * 8, length=nq), _params_vec(_search_params(nshards, 0, nq, k, 0))], nq)
 
 
 def topk_merge(keys_shards, dists_shards, nq, k):
     """merge [nshards, nq, k] per-shard results (final keys, float64 distances) into the global top-k."""
     ks = np.ascontiguousarray(keys_shards, dtype=np.int64).reshape(-1)
     ds = np.ascontiguousarray(dists_shards, dtype=np.float64).reshape(-1)
-    nsh = ks.shape[0] // (nq * k)
     keys = np.zeros(nq * k, dtype=np.int64)
     dists = np.zeros(nq * k, dtype=np.float64)
-    p = _search_params(nsh, 0, nq, k, 0)
     xcall(capi.XCALL_TOPK_MERGE, [Vector(data=keys, length=nq), Vector(data=dists, length=nq), Vector(data=ks, length=nq),
-                                  Vector(data=ds, length=nq), _params_vec(p)], nq)
+                                  Vector(data=ds, length=nq), _params_vec(_search_params(ks.shape[0] // (nq * k), 0, nq, k, 0))], nq)
     return keys, dists
 
 
 # ------------------------------------------------------------------------------------------------ column operators (csrc/colops.cu)
-def _with_nulls(x, nulls, length):
-    v = _vec(x, length)
-    if nulls is not None:
-        if isinstance(nulls, DeviceBuffer):
-            v.nulls_ptr = nulls.ptr
-        else:
-            v.nulls = np.ascontiguousarray(nulls, dtype=np.uint64)
-    v.length = length
-    return v
-
-
 def filter_sels(bools, nulls=None, length=None):
     """Filter.Call inner loop (filter.go:116-152): ascending row numbers with (!null && true).  Host arrays in, numpy sels out."""
     b = np.ascontiguousarray(bools, dtype=np.uint8)
     n = length if length is not None else b.shape[0]
     sels = np.zeros(max(n, 1), dtype=np.int64)
     cnt = np.zeros(1, dtype=np.int64)
-    xcall(capi.XCALL_FILTER_SELS, [Vector(data=sels, length=n), Vector(data=cnt, length=1), _with_nulls(b, nulls, n)], n)
+    xcall(capi.XCALL_FILTER_SELS, [Vector(data=sels, length=n), Vector(data=cnt, length=1), _vec(b, n, nulls)], n)
     return sels[:int(cnt[0])]
 
 
 def filter_sels_device(bools_dev, nulls_dev, n, sels_ptr, count_ptr):
     """asynchronous form on resident vectors: sels (int64[n] capacity) and the count stay on the device"""
-    bv = Vector(data_ptr=bools_dev.ptr, data_nbytes=n, nulls_ptr=nulls_dev.ptr if nulls_dev is not None else None, length=n)
-    xcall(capi.XCALL_FILTER_SELS, [Vector(data_ptr=sels_ptr, data_nbytes=8 * n, length=n), Vector(data_ptr=count_ptr, data_nbytes=8, length=1), bv], n)
+    xcall(capi.XCALL_FILTER_SELS, [Vector(data_ptr=sels_ptr, data_nbytes=8 * n, length=n), Vector(data_ptr=count_ptr, data_nbytes=8, length=1),
+                                   _vec(bools_dev.view(n), n, nulls_dev)], n)
 
 
 def shuffle(src, sels, src_nulls=None, want_nulls=False):
@@ -546,7 +493,7 @@ def shuffle(src, sels, src_nulls=None, want_nulls=False):
     m = s.shape[0]
     dst = np.zeros(m, dtype=a.dtype)
     dn = np.zeros((m + 63) // 64, dtype=np.uint64) if want_nulls else None
-    sv = Vector(data=a.view(np.uint8).reshape(-1), nulls=src_nulls, length=a.shape[0])
+    sv = _vec(a, a.shape[0], src_nulls)
     xcall(capi.XCALL_SHUFFLE(a.dtype.itemsize), [Vector(data=dst.view(np.uint8).reshape(-1), nulls=dn, length=m), sv, Vector(data=s, length=m)], m)
     return (dst, dn) if want_nulls else dst
 
@@ -567,6 +514,23 @@ def _order_params(types, flags, limit, has_row_ids):
     return p
 
 
+def _key_type(c):
+    """ORDER_SELS' default key type: VARCHAR for a varlena key, DECIMAL128 for uint64[n, 2], else the dtype's type"""
+    if isinstance(c, (list, tuple)):
+        return capi.T_VARCHAR
+    c = np.asarray(c)
+    return capi.T_DECIMAL128 if c.ndim == 2 else _T_OF_DTYPE.get(c.dtype)
+
+
+def _order_args(sels, types, flags, limit, keys, row_ids):
+    """ORDER_SELS' arguments: the sels result, the parameter block, one Vector per key, the optional row ids"""
+    return [sels, _params_vec(_order_params(types, flags, limit, row_ids is not None))] + keys + ([] if row_ids is None else [row_ids])
+
+
+def _order_rows(n, limit):
+    return n if limit is None or limit < 0 or limit >= n else int(limit)
+
+
 def order_sels(cols, nulls, flags, limit=None, row_ids=None, types=None, length=None):
     """Order / Top (order.go:103, top.go:445): the row permutation by the key columns, or its first `limit` rows; reorder payload columns
     with shuffle().  cols: numpy key columns (a 1-element array = const key; DECIMAL128 as uint64[n, 2] {lo, hi}); nulls: per key bitmap
@@ -574,27 +538,13 @@ def order_sels(cols, nulls, flags, limit=None, row_ids=None, types=None, length=
     DATE / DECIMAL64 and friends order as their storage type).  A varlena key (CHAR, VARCHAR, TEXT, BLOB ...; its type must be given, or
     VARCHAR is assumed) is a list of bytes or a (cells, area) pair of uint8 arrays in the vector layout (vector.varlena_bytes_column).
     row_ids (int64[n]): the merge form -- ties break by them.  Returns int64 sels."""
-    keys = []                                    # (data bytes, area or None, rows)
-    for c in cols:
-        if isinstance(c, list):
-            c = varlena_bytes_column(c)
-        if isinstance(c, tuple):
-            cells, area = np.ascontiguousarray(c[0], dtype=np.uint8).reshape(-1), c[1]
-            keys.append((cells, None if area is None else np.ascontiguousarray(area, dtype=np.uint8), cells.shape[0] // 24, capi.T_VARCHAR))
-        else:
-            c = np.ascontiguousarray(c)
-            keys.append((c.view(np.uint8).reshape(-1), None, c.shape[0], capi.T_DECIMAL128 if c.ndim == 2 else _T_OF_DTYPE.get(c.dtype)))
-    types = list(types) if types is not None else [k[3] for k in keys]
-    nulls = list(nulls) if nulls is not None else [None] * len(cols)
-    n = length if length is not None else (len(row_ids) if row_ids is not None else max(k[2] for k in keys))
-    nout = n if limit is None or limit < 0 or limit >= n else int(limit)
+    keys = [_vec(c, nulls=nl) for c, nl in zip(cols, nulls if nulls is not None else [None] * len(cols))]
+    types = list(types) if types is not None else [_key_type(c) for c in cols]
+    n = length if length is not None else (len(row_ids) if row_ids is not None else max(k.length for k in keys))
+    nout = _order_rows(n, limit)
     sels = np.zeros(max(nout, 1), dtype=np.int64)
-    vecs = [Vector(data=sels[:nout], length=nout), _params_vec(_order_params(types, flags, limit, row_ids is not None))]
-    for (data, area, rows, _), nl in zip(keys, nulls):
-        vecs.append(Vector(data=data, nulls=nl, area=area, length=rows))
-    if row_ids is not None:
-        vecs.append(Vector(data=np.ascontiguousarray(row_ids, dtype=np.int64), length=n))
-    xcall(capi.XCALL_ORDER_SELS, vecs, n)
+    rv = None if row_ids is None else _vec(row_ids, n, dtype=np.int64)
+    xcall(capi.XCALL_ORDER_SELS, _order_args(Vector(data=sels[:nout], length=nout), types, flags, limit, keys, rv), n)
     return sels[:nout]
 
 
@@ -602,16 +552,10 @@ def order_sels_device(cols, nulls, types, flags, n, sels_ptr, limit=None, row_id
     """asynchronous form on resident vectors (DeviceBuffer key columns, nulls and row ids): enqueues the order and returns; sels_ptr
     (device, int64[min(limit, n)]) holds the result once the calling thread's stream has run it.  A varlena key is a (cells, area)
     pair of DeviceBuffers (area None: every value inline); such a call reads back one small record first, so it synchronises once."""
-    nulls = list(nulls) if nulls is not None else [None] * len(cols)
-    nout = n if limit is None or limit < 0 or limit >= n else int(limit)
-    vecs = [Vector(data_ptr=sels_ptr, data_nbytes=8 * nout, length=nout), _params_vec(_order_params(types, flags, limit, row_ids is not None))]
-    for c, nl in zip(cols, nulls):
-        c, area = c if isinstance(c, tuple) else (c, None)
-        vecs.append(Vector(data_ptr=c.ptr, data_nbytes=c.nbytes, nulls_ptr=nl.ptr if nl is not None else None, length=n,
-                           area_ptr=area.ptr if area is not None else None, area_nbytes=area.nbytes if area is not None else 0))
-    if row_ids is not None:
-        vecs.append(Vector(data_ptr=row_ids.ptr, data_nbytes=8 * n, length=n))
-    xcall(capi.XCALL_ORDER_SELS, vecs, n)
+    keys = [_vec(c, n, nl) for c, nl in zip(cols, nulls if nulls is not None else [None] * len(cols))]
+    nout = _order_rows(n, limit)
+    rv = None if row_ids is None else _vec(row_ids.view(8 * n), n)
+    xcall(capi.XCALL_ORDER_SELS, _order_args(Vector(data_ptr=sels_ptr, data_nbytes=8 * nout, length=nout), types, flags, limit, keys, rv), n)
 
 
 def pack_keys(cols, nulls=None, has_null=True, length=None):
@@ -620,11 +564,8 @@ def pack_keys(cols, nulls=None, has_null=True, length=None):
     n = length if length is not None else max(len(c) for c in cols)
     keys = np.zeros(n, dtype=np.uint64)
     skip = None if has_null else np.zeros((n + 63) // 64, dtype=np.uint64)
-    prm = np.asarray([len(cols), 1 if has_null else 0], dtype=np.int32)
-    vecs = [Vector(data=keys, nulls=skip, length=n), Vector(data=prm.view(np.uint8), length=1, const=True)]
-    for i, c in enumerate(cols):
-        c = np.ascontiguousarray(c)
-        vecs.append(Vector(data=c.view(np.uint8).reshape(-1), nulls=None if nulls is None else nulls[i], length=n))
+    vecs = [Vector(data=keys, nulls=skip, length=n), _params_vec(np.asarray([len(cols), 1 if has_null else 0], dtype=np.int32))]
+    vecs += [_vec(c, n, None if nulls is None else nulls[i]) for i, c in enumerate(cols)]
     xcall(capi.XCALL_PACK_KEYS, vecs, n)
     return keys, skip
 
@@ -641,14 +582,13 @@ class GroupTable:
         n = k.shape[0]
         groups = np.zeros(n, dtype=np.uint64)
         xcall(capi.XCALL_GROUP_IDS, [Vector(data=groups, length=n), Vector(data=self.ngroups, length=1), Vector(data=self.keys, length=self.keys.shape[0]),
-                                     Vector(data=k, nulls=skip, length=n)], n)
+                                     _vec(k, n, skip)], n)
         return groups
 
     def insert_device(self, keys_dev, n, groups_dev, d_ngroups, d_table_keys, capacity):
         """all vectors resident (DeviceBuffer); the group count is read back by the call (it sizes the next operator's state)"""
-        xcall(capi.XCALL_GROUP_IDS, [Vector(data_ptr=groups_dev.ptr, data_nbytes=8 * n, length=n), Vector(data_ptr=d_ngroups.ptr, data_nbytes=8, length=1),
-                                     Vector(data_ptr=d_table_keys.ptr, data_nbytes=8 * capacity, length=capacity),
-                                     Vector(data_ptr=keys_dev.ptr, data_nbytes=8 * n, length=n)], n)
+        xcall(capi.XCALL_GROUP_IDS, [Vector(groups_dev.view(8 * n), length=n), Vector(d_ngroups.view(8), length=1),
+                                     Vector(d_table_keys.view(8 * capacity), length=capacity), _vec(keys_dev.view(8 * n), n)], n)
 
 
 def _strkey_params(types, has_null):
@@ -661,32 +601,25 @@ def _strkey_params(types, has_null):
     return p
 
 
+def _strkey_args(out, offsets, types, has_null, cols):
+    """PACK_STR_KEYS' arguments: the key bytes, the offsets (and skip bitmap), the parameter block, one Vector per column"""
+    return [out, offsets, _params_vec(_strkey_params(types, has_null))] + cols
+
+
 def pack_str_keys(cols, types, nulls=None, has_null=True, length=None, capacity=None):
     """strHashmapIterator.encodeHashKeys (strhashmap.go:92-385): the byte-string key of every row.  cols: per key column a numpy array (fixed
     width; a 1-element array = const), or for a varlena type a list of bytes or a (cells, area) pair in the vector layout; types: MO_T_* per
     column; nulls: per column bitmap words or None.  Returns (key bytes uint8[], offsets uint64[n + 1], skip bitmap words or None): row i's key is
     bytes[off[i]:off[i + 1]]; skip (has_null=False) marks the rows that join no group."""
-    data = []
-    for c in cols:
-        if isinstance(c, list):
-            c = varlena_bytes_column(c)
-        if isinstance(c, tuple):
-            cells = np.ascontiguousarray(c[0], dtype=np.uint8).reshape(-1)
-            data.append((cells, None if c[1] is None else np.ascontiguousarray(c[1], dtype=np.uint8), cells.shape[0] // 24))
-        else:
-            c = np.ascontiguousarray(c)
-            data.append((c.view(np.uint8).reshape(-1), None, c.shape[0]))
-    n = length if length is not None else max(d[2] for d in data)
-    nulls = list(nulls) if nulls is not None else [None] * len(cols)
+    data = [_vec(c, nulls=nl) for c, nl in zip(cols, nulls if nulls is not None else [None] * len(cols))]
+    n = length if length is not None else max(d.length for d in data)
     off = np.zeros(n + 1, dtype=np.uint64)
     skip = None if has_null else np.zeros((n + 63) // 64, dtype=np.uint64)
     cap = capacity if capacity is not None else 16 * n
-    prm = _params_vec(_strkey_params(types, has_null))
     while True:
         out = np.zeros(max(cap, 1), dtype=np.uint8)
-        vecs = [Vector(data=out[:cap], length=cap), Vector(data=off, nulls=skip, length=n), prm]
-        vecs += [Vector(data=d, nulls=nl, area=a, length=rows) for (d, a, rows), nl in zip(data, nulls)]
-        rc, msg = xcall(capi.XCALL_PACK_STR_KEYS, vecs, n, raise_on_error=False)
+        rc, msg = xcall(capi.XCALL_PACK_STR_KEYS, _strkey_args(Vector(data=out[:cap], length=cap), Vector(data=off, nulls=skip, length=n), types,
+                                                               has_null, data), n, raise_on_error=False)
         if rc == capi.RC_OUT_OF_RANGE and capacity is None:       # off[n] holds the size needed
             cap = int(off[n])
             continue
@@ -698,15 +631,9 @@ def pack_str_keys(cols, types, nulls=None, has_null=True, length=None, capacity=
 def pack_str_keys_device(cols, nulls, types, n, bytes_dev, offsets_dev, skip_dev=None, has_null=True):
     """the form on resident vectors: cols are DeviceBuffers or, for varlena types, (cells, area) DeviceBuffer pairs (area None: every value
     inline); key bytes go to bytes_dev (its whole size is the capacity), offsets (uint64[n + 1]) to offsets_dev.  Reads back one record."""
-    nulls = list(nulls) if nulls is not None else [None] * len(cols)
-    vecs = [Vector(data_ptr=bytes_dev.ptr, data_nbytes=bytes_dev.nbytes, length=n),
-            Vector(data_ptr=offsets_dev.ptr, data_nbytes=8 * (n + 1), nulls_ptr=skip_dev.ptr if skip_dev is not None else None, length=n),
-            _params_vec(_strkey_params(types, has_null))]
-    for c, nl in zip(cols, nulls):
-        c, area = c if isinstance(c, tuple) else (c, None)
-        vecs.append(Vector(data_ptr=c.ptr, data_nbytes=c.nbytes, nulls_ptr=nl.ptr if nl is not None else None, length=n,
-                           area_ptr=area.ptr if area is not None else None, area_nbytes=area.nbytes if area is not None else 0))
-    xcall(capi.XCALL_PACK_STR_KEYS, vecs, n)
+    cv = [_vec(c, n, nl) for c, nl in zip(cols, nulls if nulls is not None else [None] * len(cols))]
+    xcall(capi.XCALL_PACK_STR_KEYS, _strkey_args(Vector(bytes_dev, length=n), Vector(offsets_dev.view(8 * (n + 1)), skip_dev, length=n), types,
+                                                 has_null, cv), n)
 
 
 class StrGroupTable:
@@ -735,8 +662,8 @@ class StrGroupTable:
         before = int(self.ngroups[0])
         for attempt in range(2):
             vecs = [Vector(data=groups, length=n), Vector(data=self.ngroups, length=1), Vector(data=self.bytes, length=self.bytes.shape[0]),
-                    Vector(data=self.offsets, length=self.offsets.shape[0]), Vector(data=kb, length=kb.shape[0]), Vector(data=ko, nulls=skip, length=n),
-                    Vector(data=fr, length=n) if first_rows else Vector(length=0)]
+                    Vector(data=self.offsets, length=self.offsets.shape[0]), Vector(data=kb, length=kb.shape[0]), _vec(ko, n, skip),
+                    Vector(data=fr, length=n)]
             rc, msg = xcall(capi.XCALL_STR_GROUP_IDS, vecs, n, raise_on_error=False)
             if rc == capi.RC_INVALID_ARGUMENT and "capacity" in msg and attempt == 0:
                 # at most n new groups and their bytes: this size always fits
@@ -752,13 +679,9 @@ class StrGroupTable:
 
     def insert_device(self, bytes_dev, offsets_dev, n, groups_dev, d_ngroups, table_bytes_dev, table_offsets_dev, first_rows_dev=None, skip_dev=None):
         """every vector resident (DeviceBuffer; d_ngroups may be a host int64[1] array instead); the table is the caller's and does not grow"""
-        ngv = Vector(data=d_ngroups, length=1) if isinstance(d_ngroups, np.ndarray) else Vector(data_ptr=d_ngroups.ptr, data_nbytes=8, length=1)
-        vecs = [Vector(data_ptr=groups_dev.ptr, data_nbytes=8 * n, length=n), ngv,
-                Vector(data_ptr=table_bytes_dev.ptr, data_nbytes=table_bytes_dev.nbytes, length=1),
-                Vector(data_ptr=table_offsets_dev.ptr, data_nbytes=table_offsets_dev.nbytes, length=1),
-                Vector(data_ptr=bytes_dev.ptr, data_nbytes=bytes_dev.nbytes, length=n),
-                Vector(data_ptr=offsets_dev.ptr, data_nbytes=8 * (n + 1), nulls_ptr=skip_dev.ptr if skip_dev is not None else None, length=n),
-                Vector(data_ptr=first_rows_dev.ptr, data_nbytes=8 * n, length=n) if first_rows_dev is not None else Vector(length=0)]
+        vecs = [Vector(groups_dev.view(8 * n), length=n), Vector(d_ngroups if isinstance(d_ngroups, np.ndarray) else d_ngroups.view(8), length=1),
+                Vector(table_bytes_dev, length=1), Vector(table_offsets_dev, length=1), Vector(bytes_dev, length=n),
+                _vec(offsets_dev.view(8 * (n + 1)), n, skip_dev), Vector(None if first_rows_dev is None else first_rows_dev.view(8 * n), length=n)]
         xcall(capi.XCALL_STR_GROUP_IDS, vecs, n)
 
     def keys(self):
@@ -772,8 +695,8 @@ def group_agg(op, T, state, state_nulls, counts, groups, col, col_nulls=None, le
     g = np.ascontiguousarray(groups, dtype=np.uint64)
     n = length if length is not None else g.shape[0]
     sv = Vector(data=state.view(np.uint8).reshape(-1), nulls=state_nulls, length=state.shape[0])
-    cv = Vector(data=counts, length=state.shape[0]) if counts is not None else Vector(length=0)
-    colv = _with_nulls(np.ascontiguousarray(col).view(np.uint8).reshape(-1), col_nulls, n) if col is not None else _with_nulls(np.zeros(0, dtype=np.uint8), col_nulls, n)
+    cv = Vector(data=counts, length=state.shape[0])
+    colv = _vec(col if col is not None else np.zeros(0, dtype=np.uint8), n, col_nulls)
     rc, msg = xcall(capi.XCALL_GROUP_AGG(op, T), [sv, cv, Vector(data=g, length=n), colv], n, raise_on_error=False)
     if rc not in (0, capi.RC_OUT_OF_RANGE):
         raise capi.MoError(rc, msg)
@@ -849,17 +772,12 @@ class FusedPlan:
         """cols: numpy arrays or DeviceBuffers (one per declared column); nulls: optional list of bitmap words (numpy / DeviceBuffer / None).
         out_ptr: device result buffer of result_bytes(max_groups) -> asynchronous form, returns None.  Else a list of group dicts
         {key, first_row, rows, aggs: [(value, count), ...]} in first-seen order."""
-        vecs = []
-        for i, c in enumerate(cols):
-            nb = None if nulls is None else nulls[i]
-            vecs.append(_with_nulls(c if isinstance(c, DeviceBuffer) else np.ascontiguousarray(c).view(np.uint8).reshape(-1), nb, n))
+        vecs = [_vec(c, n, None if nulls is None else nulls[i]) for i, c in enumerate(cols)]
         nbytes = self.result_bytes(max_groups)
-        if out_ptr is not None:
-            xcall(capi.XCALL_PLAN, [Vector(data_ptr=out_ptr, data_nbytes=nbytes, length=1), _params_vec(self.P)] + vecs, n)
-            return None
-        res = np.zeros(nbytes, dtype=np.uint8)
-        xcall(capi.XCALL_PLAN, [Vector(data=res, length=1), _params_vec(self.P)] + vecs, n)
-        return self.parse(res.tobytes())
+        res = np.zeros(nbytes, dtype=np.uint8) if out_ptr is None else None
+        rv = Vector(data=res, length=1) if out_ptr is None else Vector(data_ptr=out_ptr, data_nbytes=nbytes, length=1)
+        xcall(capi.XCALL_PLAN, [rv, _params_vec(self.P)] + vecs, n)
+        return None if out_ptr is not None else self.parse(res.tobytes())
 
     def parse(self, raw):
         h = capi.PlanHeader.from_buffer_copy(raw[:C.sizeof(capi.PlanHeader)])
@@ -911,32 +829,39 @@ def dec_arith(op, width, a, b, scale1, scale2, n, n1=None, n2=None, rnulls=None)
     const vector.  Returns (rc, result, result nulls words, err_row); result is int64[n] (64-bit + -) or uint64[n, 2]."""
     out128 = op == 2 or width == 128
     r = np.zeros((n, 2), dtype=np.uint64) if out128 else np.zeros(n, dtype=np.int64)
-    rn = np.zeros((n + 63) // 64, dtype=np.uint64) if rnulls is None else np.ascontiguousarray(rnulls, dtype=np.uint64).copy()
-    prm = np.frombuffer(bytes(capi.DecParams(scale1, scale2, -1)), dtype=np.uint8).copy()
-    av = Vector(data=np.ascontiguousarray(a).view(np.uint8).reshape(-1), nulls=n1, length=n)
-    bv = Vector(data=np.ascontiguousarray(b).view(np.uint8).reshape(-1), nulls=n2, length=n)
-    rc, msg = xcall(capi.XCALL_DEC_ARITH(op, width), [Vector(data=r.view(np.uint8).reshape(-1), nulls=rn, length=n), av, bv, Vector(data=prm, length=1, const=True)], n,
-                    raise_on_error=False)
+    rn = _dec_result_nulls(n, rnulls)
+    args = _dec_args(Vector(data=r.view(np.uint8).reshape(-1), nulls=rn, length=n), a, b, n, n1, n2, capi.DecParams(scale1, scale2, -1))
+    rc, msg = xcall(capi.XCALL_DEC_ARITH(op, width), args, n, raise_on_error=False)
     if rc not in (0, capi.RC_INVALID_ARGUMENT):
         raise capi.MoError(rc, msg)
-    return rc, r, rn, int(prm.view(np.int64)[1])
+    return rc, r, rn, _err_row(args[3])
+
+
+def _dec_args(out, a, b, n, n1, n2, params):
+    """the arguments of a binary decimal call (DEC_ARITH, GO_COMPARE): the result, both operands (one element = const), the parameter block"""
+    return [out, _vec(a, n, n1), _vec(b, n, n2), _params_vec(params)]
+
+
+def _err_row(params):
+    """the first failing row a decimal call writes back into its parameter block (-1: none)"""
+    return int(params.data.view(np.int64)[1])
 
 
 def dec_sum(width, col, sums, counts, groups=None, nulls=None, n=None):
     """SUM/AVG accumulation into sums uint64[ngroups, 2] (Decimal128) and counts int64[ngroups], in place"""
     c = np.ascontiguousarray(col)
     n = n if n is not None else (c.shape[0])
-    gv = Vector(data=np.ascontiguousarray(groups, dtype=np.uint64), length=n) if groups is not None else Vector(length=0)
+    gv = Vector(data=None if groups is None else np.ascontiguousarray(groups, dtype=np.uint64), length=n)
     xcall(capi.XCALL_DEC_SUM(width), [Vector(data=sums.view(np.uint8).reshape(-1), length=sums.shape[0]), Vector(data=counts, length=counts.shape[0]), gv,
-                                      _with_nulls(c.view(np.uint8).reshape(-1), nulls, n)], n)
-
-
-def _dec_bytes(x):
-    return x if isinstance(x, DeviceBuffer) else np.ascontiguousarray(x).view(np.uint8).reshape(-1)
+                                      _vec(c, n, nulls)], n)
 
 
 def _dec_result_nulls(n, rnulls):
     return np.zeros((n + 63) // 64, dtype=np.uint64) if rnulls is None else np.ascontiguousarray(rnulls, dtype=np.uint64).copy()
+
+
+def _dec_compare_id(op, width):
+    return capi.XCALL_GO_COMPARE(op, capi.T_DECIMAL64 if width == 64 else capi.T_DECIMAL128)
 
 
 def dec_compare(op, width, a, b, scale1, scale2, n, n1=None, n2=None, rnulls=None):
@@ -945,18 +870,19 @@ def dec_compare(op, width, a, b, scale1, scale2, n, n1=None, n2=None, rnulls=Non
     (rows set there are skipped).  Returns (values uint8[n], result nulls words)."""
     r = np.zeros(n, dtype=np.uint8)
     rn = _dec_result_nulls(n, rnulls)
-    xcall(capi.XCALL_GO_COMPARE(op, capi.T_DECIMAL64 if width == 64 else capi.T_DECIMAL128),
-          [Vector(data=r, nulls=rn, length=n), _with_nulls(_dec_bytes(a), n1, n), _with_nulls(_dec_bytes(b), n2, n),
-           _params_vec(capi.DecParams(scale1, scale2, -1))], n)
+    xcall(_dec_compare_id(op, width), _dec_args(Vector(data=r, nulls=rn, length=n), a, b, n, n1, n2, capi.DecParams(scale1, scale2, -1)), n)
     return r, rn
 
 
 def dec_compare_device(op, width, a, b, scale1, scale2, n, out_dev, out_nulls_dev, n1=None, n2=None):
     """dec_compare on resident operands (DeviceBuffers; one element's bytes = const) into out_dev (bool[n]) and out_nulls_dev (its bitmap,
     in/out): enqueue-only, nothing is read back or synchronised"""
-    xcall(capi.XCALL_GO_COMPARE(op, capi.T_DECIMAL64 if width == 64 else capi.T_DECIMAL128),
-          [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n), _with_nulls(a, n1, n), _with_nulls(b, n2, n),
-           _params_vec(capi.DecParams(scale1, scale2, -1))], n)
+    xcall(_dec_compare_id(op, width), _dec_args(Vector(out_dev.view(n), out_nulls_dev, length=n), a, b, n, n1, n2, capi.DecParams(scale1, scale2, -1)), n)
+
+
+def _between_args(out, width, col, lo, hi, n, nulls):
+    """GO_BETWEEN's arguments over a decimal column: the result, the column, the two bounds as one-element consts"""
+    return [out, _vec(col, n, nulls), _params_vec(_dec_bound(width, lo)), _params_vec(_dec_bound(width, hi))]
 
 
 def _dec_bound(width, v):
@@ -972,16 +898,23 @@ def dec_between(width, col, lo, hi, n, nulls=None):
     r = np.zeros(n, dtype=np.uint8)
     rn = np.zeros((n + 63) // 64, dtype=np.uint64)
     xcall(capi.XCALL_GO_BETWEEN(capi.T_DECIMAL64 if width == 64 else capi.T_DECIMAL128),
-          [Vector(data=r, nulls=rn, length=n), _with_nulls(_dec_bytes(col), nulls, n), Vector(data=_dec_bound(width, lo), length=1, const=True),
-           Vector(data=_dec_bound(width, hi), length=1, const=True)], n)
+          _between_args(Vector(data=r, nulls=rn, length=n), width, col, lo, hi, n, nulls), n)
     return r, rn
 
 
 def dec_between_device(width, col, lo, hi, n, out_dev, out_nulls_dev, nulls=None):
     """dec_between on a resident column into resident outputs (out_nulls_dev zeroed by the caller)"""
     xcall(capi.XCALL_GO_BETWEEN(capi.T_DECIMAL64 if width == 64 else capi.T_DECIMAL128),
-          [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n), _with_nulls(col, nulls, n),
-           Vector(data=_dec_bound(width, lo), length=1, const=True), Vector(data=_dec_bound(width, hi), length=1, const=True)], n)
+          _between_args(Vector(out_dev.view(n), out_nulls_dev, length=n), width, col, lo, hi, n, nulls), n)
+
+
+def _dec_div(width, out, a, b, scale1, scale2, n, n1, n2, div0_error):
+    """DEC_ARITH's Div: (rc, err_row, msg); rc 0, RC_INVALID_ARGUMENT or RC_DIVISION_BY_ZERO, any other code is raised"""
+    args = _dec_args(out, a, b, n, n1, n2, capi.DecDivParams(scale1, scale2, -1, 1 if div0_error else 0, 0))
+    rc, msg = xcall(capi.XCALL_DEC_ARITH(capi.DEC_OP_DIV, width), args, n, raise_on_error=False)
+    if rc not in (0, capi.RC_INVALID_ARGUMENT, capi.RC_DIVISION_BY_ZERO):
+        raise capi.MoError(rc, msg)
+    return rc, _err_row(args[3]), msg
 
 
 def dec_div(width, a, b, scale1, scale2, n, n1=None, n2=None, rnulls=None, div0_error=False):
@@ -990,25 +923,18 @@ def dec_div(width, a, b, scale1, scale2, n, n1=None, n2=None, rnulls=None, div0_
     rc is 0, RC_INVALID_ARGUMENT ("Decimal128 Div overflow") or RC_DIVISION_BY_ZERO, err_row the first failing row or -1."""
     r = np.zeros((n, 2), dtype=np.uint64)
     rn = _dec_result_nulls(n, rnulls)
-    prm = np.frombuffer(bytes(capi.DecDivParams(scale1, scale2, -1, 1 if div0_error else 0, 0)), dtype=np.uint8).copy()
-    rc, msg = xcall(capi.XCALL_DEC_ARITH(capi.DEC_OP_DIV, width),
-                    [Vector(data=r.view(np.uint8).reshape(-1), nulls=rn, length=n), _with_nulls(_dec_bytes(a), n1, n), _with_nulls(_dec_bytes(b), n2, n),
-                     Vector(data=prm, length=1, const=True)], n, raise_on_error=False)
-    if rc not in (0, capi.RC_INVALID_ARGUMENT, capi.RC_DIVISION_BY_ZERO):
-        raise capi.MoError(rc, msg)
-    return rc, r, rn, int(prm.view(np.int64)[1]), msg
+    rc, err_row, msg = _dec_div(width, Vector(data=r.view(np.uint8).reshape(-1), nulls=rn, length=n), a, b, scale1, scale2, n, n1, n2, div0_error)
+    return rc, r, rn, err_row, msg
 
 
 def dec_div_device(width, a, b, scale1, scale2, n, out_dev, out_nulls_dev, n1=None, n2=None, div0_error=False):
     """dec_div on resident operands into resident outputs (out_nulls_dev in/out).  One read-back of the first failing row; returns
     (rc, err_row, msg)."""
-    prm = np.frombuffer(bytes(capi.DecDivParams(scale1, scale2, -1, 1 if div0_error else 0, 0)), dtype=np.uint8).copy()
-    rc, msg = xcall(capi.XCALL_DEC_ARITH(capi.DEC_OP_DIV, width),
-                    [Vector(data_ptr=out_dev.ptr, data_nbytes=16 * n, nulls_ptr=out_nulls_dev.ptr, length=n), _with_nulls(a, n1, n),
-                     _with_nulls(b, n2, n), Vector(data=prm, length=1, const=True)], n, raise_on_error=False)
-    if rc not in (0, capi.RC_INVALID_ARGUMENT, capi.RC_DIVISION_BY_ZERO):
-        raise capi.MoError(rc, msg)
-    return rc, int(prm.view(np.int64)[1]), msg
+    return _dec_div(width, Vector(out_dev.view(16 * n), out_nulls_dev, length=n), a, b, scale1, scale2, n, n1, n2, div0_error)
+
+
+def _dec_avg_args(out, sums, counts, g, scale):
+    return [out, _vec(sums, g), _vec(counts, g, dtype=np.int64), _params_vec(capi.DecParams(scale, 0, -1))]
 
 
 def dec_avg(width, sums, counts, scale):
@@ -1017,15 +943,13 @@ def dec_avg(width, sums, counts, scale):
     g = counts.shape[0]
     r = np.zeros((g, 2), dtype=np.uint64)
     rn = np.zeros((g + 63) // 64, dtype=np.uint64)
-    xcall(capi.XCALL_DEC_AVG(width), [Vector(data=r.view(np.uint8).reshape(-1), nulls=rn, length=g), _vec(_dec_bytes(sums), g),
-                                      _vec(np.ascontiguousarray(counts, dtype=np.int64), g), _params_vec(capi.DecParams(scale, 0, -1))], g)
+    xcall(capi.XCALL_DEC_AVG(width), _dec_avg_args(Vector(data=r.view(np.uint8).reshape(-1), nulls=rn, length=g), sums, counts, g, scale), g)
     return r, rn
 
 
 def dec_avg_device(width, sums, counts, g, scale, out_dev, out_nulls_dev):
     """dec_avg on resident state (DeviceBuffers) into resident outputs: enqueue-only"""
-    xcall(capi.XCALL_DEC_AVG(width), [Vector(data_ptr=out_dev.ptr, data_nbytes=16 * g, nulls_ptr=out_nulls_dev.ptr, length=g), _vec(sums, g),
-                                      _vec(counts, g), _params_vec(capi.DecParams(scale, 0, -1))], g)
+    xcall(capi.XCALL_DEC_AVG(width), _dec_avg_args(Vector(out_dev.view(16 * g), out_nulls_dev, length=g), sums, counts, g, scale), g)
 
 
 # ---------------------------------------------------------------------------------------------- normalize_l2 (vector-valued)
@@ -1038,7 +962,7 @@ def normalize_l2(cells, area, length, dtype=np.float32, nulls=None):
     oarea = np.zeros(max(area.nbytes, 1), dtype=np.uint8)
     res = Vector(data=ocells, area=oarea, nulls=None if nulls is None else np.array(nulls, dtype=np.uint64, copy=True), length=length)
     fid = capi.XCALL_GO_NORMALIZE_L2_F32 if np.dtype(dtype) == np.float32 else capi.XCALL_GO_NORMALIZE_L2_F64
-    xcall(fid, [res, Vector(data=cells, area=area, length=length)], length)
+    xcall(fid, [res, _vec((cells, area), length)], length)
     return ocells, oarea[:area.nbytes]
 
 
@@ -1069,25 +993,48 @@ def _matched_vec(matched, join_type):
         return []
     if matched is None:
         raise ValueError("join type %d needs the matched bitmap" % join_type)
-    if isinstance(matched, DeviceBuffer):
-        return [Vector(data_ptr=matched.ptr, data_nbytes=matched.nbytes, length=1)]
-    if not (isinstance(matched, np.ndarray) and matched.dtype == np.uint64 and matched.flags.c_contiguous):
+    if not isinstance(matched, DeviceBuffer) and not (isinstance(matched, np.ndarray) and matched.dtype == np.uint64 and matched.flags.c_contiguous):
         raise ValueError("the matched bitmap is updated in place: pass a contiguous numpy uint64 array")
-    return [Vector(data=matched, length=len(matched))]
+    return [Vector(data=matched, length=1)]
 
 
-def _probe_with(call, n, capacity):
-    """the JOIN_PROBE capacity protocol: call(op, ob, cnt) -> (rc, msg); a too-small buffer reports the count and the call is repeated"""
+def _join_type(join_type):
+    return _params_vec(np.array([join_type, 0], dtype=np.int32))
+
+
+def _ngroups(ngroups):
+    return _params_vec(np.array([ngroups], np.int64))
+
+
+def _probe_args(outs, join_type, args, matched):
+    """the arguments of JOIN_PROBE, JOIN_PROBE_GIDS and JOIN_COND: probe rows, build rows, count, join type, the call's own, the matched bitmap"""
+    return outs + [_join_type(join_type)] + args + _matched_vec(matched, join_type)
+
+
+def _probe_with(fid, join_type, args, matched, n, length, capacity):
+    """the JOIN_PROBE capacity protocol on host results: a too-small buffer reports the count and the call is repeated"""
     cap = capacity if capacity is not None else max(2 * n, 1024)
     while True:
         op, ob, cnt = np.zeros(cap, np.int64), np.zeros(cap, np.int64), np.zeros(1, np.int64)
-        rc, msg = call(op, ob, cnt)
+        outs = [Vector(data=op, length=cap), Vector(data=ob, length=cap), Vector(data=cnt, length=1)]
+        rc, msg = xcall(fid, _probe_args(outs, join_type, args, matched), length, raise_on_error=False)
         if rc == capi.RC_OUT_OF_RANGE and capacity is None:
             cap = int(cnt[0])
             continue
         if rc:
             raise capi.MoError(rc, msg)
         return op[:int(cnt[0])], ob[:int(cnt[0])]
+
+
+def _probe_gids_args(ngroups, offsets, sels, vals):
+    """JOIN_PROBE_GIDS' own arguments: the group count, the GroupSels (None: unique map), the group ids"""
+    return [_ngroups(ngroups), Vector(data=offsets, length=ngroups + 2), Vector(data=sels, length=1), vals]
+
+
+def _str_find_args(vals, ngroups, table_bytes, table_offsets, key_bytes, key_offsets, nulls, n):
+    """STR_JOIN_FIND's arguments: the ids, the table (group count, bytes, offsets), the probe keys' bytes and offsets with their nulls"""
+    return [Vector(data=vals, length=n), _ngroups(ngroups), Vector(data=table_bytes, length=1), Vector(data=table_offsets, length=1),
+            Vector(data=key_bytes, length=n), _vec(key_offsets, n, nulls)]
 
 
 class StrJoinMap:
@@ -1112,17 +1059,13 @@ class StrJoinMap:
     def hash_on_unique(self):
         return self.offsets is None
 
-    def _table(self):
-        return [Vector(data=np.array([self.ngroups], np.int64), length=1), Vector(data=self.table_bytes, length=len(self.table_bytes)),
-                Vector(data=self.table_offsets, length=self.ngroups + 1)]
-
     def find(self, key_bytes, key_offsets, nulls=None):
         """strHashmapIterator.Find: 1-based group id per probe key, 0 = no match"""
         ko = np.ascontiguousarray(key_offsets, dtype=np.uint64)
         n = ko.shape[0] - 1
         vals = np.zeros(n, dtype=np.uint64)
         kb = np.ascontiguousarray(key_bytes, dtype=np.uint8)
-        xcall(capi.XCALL_STR_JOIN_FIND, [Vector(data=vals, length=n)] + self._table() + [Vector(data=kb, length=len(kb)), Vector(data=ko, nulls=nulls, length=n)], n)
+        xcall(capi.XCALL_STR_JOIN_FIND, _str_find_args(vals, self.ngroups, self.table_bytes, self.table_offsets, kb, ko, nulls, n), n)
         return vals
 
     def probe(self, key_bytes, key_offsets, join_type=capi.JOIN_INNER, nulls=None, capacity=None, matched=None):
@@ -1139,24 +1082,17 @@ class StrJoinMap:
 def str_join_find_device(vals_dev, n, ngroups, table_bytes_dev, table_offsets_dev, bytes_dev, offsets_dev, nulls_dev=None):
     """STR_JOIN_FIND on resident vectors (DeviceBuffers): enqueues the lookup of n probe keys (bytes_dev, offsets_dev uint64[n + 1]) in a table
     STR_GROUP_IDS built (ngroups is a host int); vals_dev (uint64[n]) holds the ids once the calling thread's stream has run it"""
-    xcall(capi.XCALL_STR_JOIN_FIND, [Vector(data_ptr=vals_dev.ptr, data_nbytes=8 * n, length=n), Vector(data=np.array([ngroups], np.int64), length=1),
-                                     Vector(data_ptr=table_bytes_dev.ptr, data_nbytes=table_bytes_dev.nbytes, length=1),
-                                     Vector(data_ptr=table_offsets_dev.ptr, data_nbytes=8 * (ngroups + 1), length=1),
-                                     Vector(data_ptr=bytes_dev.ptr, data_nbytes=bytes_dev.nbytes, length=n),
-                                     Vector(data_ptr=offsets_dev.ptr, data_nbytes=8 * (n + 1), nulls_ptr=nulls_dev.ptr if nulls_dev is not None else None, length=n)], n)
+    xcall(capi.XCALL_STR_JOIN_FIND, _str_find_args(vals_dev.view(8 * n), ngroups, table_bytes_dev, table_offsets_dev.view(8 * (ngroups + 1)), bytes_dev,
+                                                   offsets_dev.view(8 * (n + 1)), nulls_dev, n), n)
 
 
 def probe_gids_device(vals_dev, n, ngroups, offsets_dev, sels_dev, join_type, out_probe_dev, out_build_dev, count_dev, matched_dev=None):
     """JOIN_PROBE_GIDS on resident vectors: the pairs go to out_probe_dev / out_build_dev (int64, their size is the capacity) and their count to
     count_dev; offsets_dev / sels_dev None = unique map; matched_dev = the matched bitmap (DeviceBuffer) of a right-flavoured type.  Reads the count
     back (RC_OUT_OF_RANGE: the buffers are too small, the count is written)."""
-    prm = np.array([join_type, 0], dtype=np.int32)
-    vecs = [Vector(data_ptr=out_probe_dev.ptr, data_nbytes=out_probe_dev.nbytes, length=1), Vector(data_ptr=out_build_dev.ptr, data_nbytes=out_build_dev.nbytes, length=1),
-            Vector(data_ptr=count_dev.ptr, data_nbytes=8, length=1), Vector(data=prm.view(np.uint8), length=1), Vector(data=np.array([ngroups], np.int64), length=1),
-            Vector(data_ptr=offsets_dev.ptr, data_nbytes=offsets_dev.nbytes, length=ngroups + 2) if offsets_dev is not None else Vector(length=0),
-            Vector(data_ptr=sels_dev.ptr, data_nbytes=sels_dev.nbytes, length=1) if sels_dev is not None else Vector(length=0),
-            Vector(data_ptr=vals_dev.ptr, data_nbytes=8 * n, length=n)] + _matched_vec(matched_dev, join_type)
-    xcall(capi.XCALL_JOIN_PROBE_GIDS, vecs, n)
+    outs = [Vector(data=out_probe_dev, length=1), Vector(data=out_build_dev, length=1), Vector(data=count_dev.view(8), length=1)]
+    args = _probe_gids_args(ngroups, offsets_dev, sels_dev, Vector(data=vals_dev.view(8 * n), length=n))
+    xcall(capi.XCALL_JOIN_PROBE_GIDS, _probe_args(outs, join_type, args, matched_dev), n)
 
 
 def probe_gids(vals, ngroups, offsets, sels, join_type=capi.JOIN_INNER, capacity=None, matched=None):
@@ -1164,17 +1100,7 @@ def probe_gids(vals, ngroups, offsets, sels, join_type=capi.JOIN_INNER, capacity
     matched = the matched bitmap of a right-flavoured type (matched_bitmap(nbuild), updated in place)"""
     v = np.ascontiguousarray(vals, dtype=np.uint64)
     n = v.shape[0]
-    prm = np.array([join_type, 0], dtype=np.int32)
-    mv = _matched_vec(matched, join_type)
-
-    def call(op, ob, cnt):
-        vecs = [Vector(data=op, length=len(op)), Vector(data=ob, length=len(ob)), Vector(data=cnt, length=1), Vector(data=prm.view(np.uint8), length=1),
-                Vector(data=np.array([ngroups], np.int64), length=1),
-                Vector(data=offsets, length=ngroups + 2) if offsets is not None else Vector(length=0),
-                Vector(data=sels, length=len(sels)) if sels is not None else Vector(length=0),
-                Vector(data=v, length=n)] + mv
-        return xcall(capi.XCALL_JOIN_PROBE_GIDS, vecs, n, raise_on_error=False)
-    return _probe_with(call, n, capacity)
+    return _probe_with(capi.XCALL_JOIN_PROBE_GIDS, join_type, _probe_gids_args(ngroups, offsets, sels, Vector(data=v, length=n)), matched, n, n, capacity)
 
 
 class JoinMap:
@@ -1212,17 +1138,9 @@ class JoinMap:
         one join); join_build_rows then gives the build rows they add."""
         k = np.ascontiguousarray(keys, dtype=np.uint64)
         n = k.shape[0]
-        prm = np.array([join_type, 0], dtype=np.int32)
-        mv = _matched_vec(matched, join_type)
-
-        def call(op, ob, cnt):
-            vecs = [Vector(data=op, length=len(op)), Vector(data=ob, length=len(ob)), Vector(data=cnt, length=1), Vector(data=prm.view(np.uint8), length=1),
-                    Vector(data=self.table_keys, length=self.ngroups),
-                    Vector(data=self.offsets, length=self.ngroups + 2) if self.offsets is not None else Vector(length=0),
-                    Vector(data=self.sels, length=len(self.sels)) if self.sels is not None else Vector(length=0),
-                    Vector(data=k, nulls=nulls, length=n)] + mv
-            return xcall(capi.XCALL_JOIN_PROBE, vecs, n, raise_on_error=False)
-        return _probe_with(call, n, capacity)
+        args = [Vector(data=self.table_keys, length=self.ngroups), Vector(data=self.offsets, length=self.ngroups + 2), Vector(data=self.sels, length=1),
+                _vec(k, n, nulls)]
+        return _probe_with(capi.XCALL_JOIN_PROBE, join_type, args, matched, n, n, capacity)
 
     def release(self):
         if self.prepared:
@@ -1237,20 +1155,18 @@ def join_build_rows(matched, nbuild, join_type):
     m = np.ascontiguousarray(matched, dtype=np.uint64)
     sels = np.zeros(max(nbuild, 1), dtype=np.int64)
     cnt = np.zeros(1, dtype=np.int64)
-    xcall(capi.XCALL_JOIN_BUILD_ROWS, [Vector(data=sels, length=nbuild), Vector(data=cnt, length=1), Vector(data=m, length=len(m)),
-                                       Vector(data=np.array([join_type, 0], np.int32).view(np.uint8), length=1)], nbuild)
+    xcall(capi.XCALL_JOIN_BUILD_ROWS, [Vector(data=sels, length=nbuild), Vector(data=cnt, length=1), Vector(data=m, length=1), _join_type(join_type)], nbuild)
     return sels[:int(cnt[0])]
 
 
 def join_build_rows_device(matched_dev, nbuild, join_type, sels_ptr, count_ptr):
     """JOIN_BUILD_ROWS on a resident bitmap: sels (int64[nbuild] capacity) and the count stay on the device; the call only enqueues work"""
     xcall(capi.XCALL_JOIN_BUILD_ROWS, [Vector(data_ptr=sels_ptr, data_nbytes=8 * nbuild, length=nbuild), Vector(data_ptr=count_ptr, data_nbytes=8, length=1),
-                                       Vector(data_ptr=matched_dev.ptr, data_nbytes=8 * ((nbuild + 63) // 64), length=1),
-                                       Vector(data=np.array([join_type, 0], np.int32).view(np.uint8), length=1)], nbuild)
+                                       Vector(data=matched_dev.view(8 * ((nbuild + 63) // 64)), length=1), _join_type(join_type)], nbuild)
 
 
 def _merge_vecs(out, inputs, join_type):
-    return [out, Vector(data=np.array([len(inputs)], np.int32), length=1), Vector(data=np.array([join_type, 0], np.int32).view(np.uint8), length=1)] + inputs
+    return [out, _params_vec(np.array([len(inputs)], np.int32)), _join_type(join_type)] + inputs
 
 
 def join_matched_merge(bitmaps, nbuild, join_type):
@@ -1266,8 +1182,13 @@ def join_matched_merge_device(out_dev, bitmaps_dev, nbuild, join_type):
     """JOIN_MATCHED_MERGE over resident bitmaps (DeviceBuffers; out_dev may be one of them): enqueue only, except JOIN_RIGHT_SINGLE, which reads
     back whether a row is set in two inputs"""
     words = (nbuild + 63) // 64
-    ins = [Vector(data_ptr=b.ptr, data_nbytes=8 * words, length=1) for b in bitmaps_dev]
-    xcall(capi.XCALL_JOIN_MATCHED_MERGE, _merge_vecs(Vector(data_ptr=out_dev.ptr, data_nbytes=8 * words, length=1), ins, join_type), nbuild)
+    ins = [Vector(data=b.view(8 * words), length=1) for b in bitmaps_dev]
+    xcall(capi.XCALL_JOIN_MATCHED_MERGE, _merge_vecs(Vector(data=out_dev.view(8 * words), length=1), ins, join_type), nbuild)
+
+
+def _cond_args(cand_probe, cand_build, cond, cond_nulls, npairs):
+    """JOIN_COND's own arguments: the candidate pairs and their condition"""
+    return [_vec(cand_probe, npairs), _vec(cand_build, npairs), _vec(cond, npairs, cond_nulls)]
 
 
 def join_cond(cand_probe, cand_build, cond, nprobe, join_type, cond_nulls=None, capacity=None, matched=None):
@@ -1279,14 +1200,8 @@ def join_cond(cand_probe, cand_build, cond, nprobe, join_type, cond_nulls=None, 
     cb = np.ascontiguousarray(cand_build, dtype=np.int64)
     c = np.ascontiguousarray(cond, dtype=np.bool_).view(np.uint8)
     npairs = cp.shape[0]
-    prm = np.array([join_type, 0], dtype=np.int32)
-    mv = _matched_vec(matched, join_type)
-
-    def call(op, ob, cnt):
-        vecs = [Vector(data=op, length=len(op)), Vector(data=ob, length=len(ob)), Vector(data=cnt, length=1), Vector(data=prm.view(np.uint8), length=1),
-                Vector(data=cp, length=npairs), Vector(data=cb, length=npairs), _with_nulls(c, cond_nulls, npairs)] + mv
-        return xcall(capi.XCALL_JOIN_COND, vecs, nprobe, raise_on_error=False)
-    return _probe_with(call, max(npairs, nprobe), capacity)          # the result has at most npairs + nprobe rows: one call
+    # the result has at most npairs + nprobe rows: one call
+    return _probe_with(capi.XCALL_JOIN_COND, join_type, _cond_args(cp, cb, c, cond_nulls, npairs), matched, max(npairs, nprobe), nprobe, capacity)
 
 
 def join_cond_device(cand_probe_dev, cand_build_dev, cond_dev, cond_nulls_dev, npairs, nprobe, join_type, out_probe_dev, out_build_dev, count_dev,
@@ -1294,12 +1209,9 @@ def join_cond_device(cand_probe_dev, cand_build_dev, cond_dev, cond_nulls_dev, n
     """JOIN_COND on resident vectors (DeviceBuffers), the twin of probe_gids_device: npairs candidate pairs and their condition (cond_nulls_dev
     None = no NULLs); the result goes to out_probe_dev / out_build_dev (int64, their size is the capacity) and its count to count_dev.  Reads the
     count back (RC_OUT_OF_RANGE: the buffers are too small, the count is written)."""
-    prm = np.array([join_type, 0], dtype=np.int32)
-    vecs = [Vector(data_ptr=out_probe_dev.ptr, data_nbytes=out_probe_dev.nbytes, length=1), Vector(data_ptr=out_build_dev.ptr, data_nbytes=out_build_dev.nbytes, length=1),
-            Vector(data_ptr=count_dev.ptr, data_nbytes=8, length=1), Vector(data=prm.view(np.uint8), length=1),
-            Vector(data_ptr=cand_probe_dev.ptr, data_nbytes=8 * npairs, length=npairs), Vector(data_ptr=cand_build_dev.ptr, data_nbytes=8 * npairs, length=npairs),
-            Vector(data_ptr=cond_dev.ptr, data_nbytes=npairs, nulls_ptr=cond_nulls_dev.ptr if cond_nulls_dev is not None else None, length=npairs)]
-    xcall(capi.XCALL_JOIN_COND, vecs + _matched_vec(matched_dev, join_type), nprobe)
+    outs = [Vector(data=out_probe_dev, length=1), Vector(data=out_build_dev, length=1), Vector(data=count_dev.view(8), length=1)]
+    args = _cond_args(cand_probe_dev.view(8 * npairs), cand_build_dev.view(8 * npairs), cond_dev.view(npairs), cond_nulls_dev, npairs)
+    xcall(capi.XCALL_JOIN_COND, _probe_args(outs, join_type, args, matched_dev), nprobe)
 
 
 # ---------------------------------------------------------------------------------------------- Elkan k-means (csrc/kmeans.cu)
@@ -1321,8 +1233,8 @@ def kmeans_elkan(vectors, init_centroids, max_iter=500, rnd=None):
     cent = np.ascontiguousarray(init_centroids, dtype=v.dtype).copy()
     k = cent.shape[0]
     assign = np.zeros(n, dtype=np.int64); iters = np.zeros(1, dtype=np.int64)
-    prm = np.array([n, dim, k, max_iter], dtype=np.int64)
-    vecs = [Vector(data=cent.reshape(-1), length=k * dim), Vector(data=assign, length=n), Vector(data=iters, length=1), Vector(data=prm.view(np.uint8), length=1),
+    vecs = [Vector(data=cent.reshape(-1), length=k * dim), Vector(data=assign, length=n), Vector(data=iters, length=1),
+            _params_vec(np.array([n, dim, k, max_iter], dtype=np.int64)),
             Vector(data=v.reshape(-1), length=n * dim),
             Vector(data=np.ascontiguousarray(rnd, dtype=np.float32), length=len(rnd)) if rnd is not None and len(rnd) else Vector(length=0)]
     xcall(capi.XCALL_KMEANS_ELKAN_F32 if v.dtype == np.float32 else capi.XCALL_KMEANS_ELKAN_F64, vecs, n)
@@ -1355,26 +1267,15 @@ def vector_unmarshal_device(src_dev, nbytes, data_dev, area_dev, nulls_dev):
     """Vector.UnmarshalBinary on the device: src_dev holds the marshalled bytes (e.g. straight out of lz4 decode), the sections are copied to the
     aligned DeviceBuffers given.  Returns the VectorView."""
     view = np.zeros(C.sizeof(VectorView), dtype=np.uint8)
-    vecs = [Vector(data=view, length=1), Vector(data_ptr=data_dev.ptr, data_nbytes=data_dev.nbytes, length=1),
-            Vector(data_ptr=area_dev.ptr, data_nbytes=area_dev.nbytes, length=1) if area_dev is not None else Vector(length=0),
-            Vector(data_ptr=nulls_dev.ptr, data_nbytes=nulls_dev.nbytes, length=1) if nulls_dev is not None else Vector(length=0),
-            Vector(data_ptr=src_dev.ptr, data_nbytes=nbytes, length=1)]
+    vecs = [Vector(data=view, length=1), Vector(data=data_dev, length=1), Vector(data=area_dev, length=1), Vector(data=nulls_dev, length=1),
+            Vector(data=src_dev.view(nbytes), length=1)]
     xcall(capi.XCALL_VECTOR_UNMARSHAL, vecs, 1)
     return VectorView.from_buffer_copy(view.tobytes())
 
 
 # ------------------------------------------------------------------------------------------------ string predicates (csrc/strpred.cu)
-def _str_operand(x, nulls):
-    """a list of bytes (one element = a const operand) or a (cells, area) pair in the vector layout -> Vector"""
-    if isinstance(x, list):
-        x = varlena_bytes_column(x)
-    cells = np.ascontiguousarray(x[0], dtype=np.uint8).reshape(-1)
-    area = None if x[1] is None else np.ascontiguousarray(x[1], dtype=np.uint8)
-    return Vector(data=cells, nulls=nulls, area=area, length=cells.shape[0] // 24)
-
-
 def _str_pred(fid, a, b, a_nulls, b_nulls, rnulls, length):
-    va, vb = _str_operand(a, a_nulls), _str_operand(b, b_nulls)
+    va, vb = _vec(a, nulls=a_nulls), _vec(b, nulls=b_nulls)
     n = length if length is not None else max(va.length, vb.length)
     r = np.zeros(max(n, 1), dtype=np.uint8)
     rn = np.zeros(max((n + 63) // 64, 1), dtype=np.uint64) if rnulls is None else np.array(rnulls, dtype=np.uint64)
@@ -1397,15 +1298,8 @@ def like(col, pattern, col_nulls=None, pattern_nulls=None, rnulls=None, length=N
     return _str_pred(capi.XCALL_GO_LIKE, col, pattern, col_nulls, pattern_nulls, rnulls, length)
 
 
-def _str_device_vec(x, nulls, n):
-    cells, area = x if isinstance(x, tuple) else (x, None)
-    return Vector(data_ptr=cells.ptr, data_nbytes=cells.nbytes, nulls_ptr=nulls.ptr if nulls is not None else None, length=n,
-                  area_ptr=area.ptr if area is not None else None, area_nbytes=area.nbytes if area is not None else 0)
-
-
 def _str_pred_device(fid, a, b, n, out_dev, out_nulls_dev, a_nulls, b_nulls):
-    xcall(fid, [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n),
-                _str_device_vec(a, a_nulls, n), _str_device_vec(b, b_nulls, n)], n)
+    xcall(fid, [Vector(data=out_dev.view(n), nulls=out_nulls_dev, length=n), _vec(a, n, a_nulls), _vec(b, n, b_nulls)], n)
 
 
 def str_compare_device(op, T, a, b, n, out_dev, out_nulls_dev, a_nulls=None, b_nulls=None):
@@ -1418,34 +1312,22 @@ def like_device(col, pattern, n, out_dev, out_nulls_dev, col_nulls=None, pattern
     """LIKE on resident vectors, as str_compare_device; the pattern is a (cells, area) pair of DeviceBuffers or of host arrays (a const
     pattern read on the host)."""
     if isinstance(pattern, (bytes, bytearray)):
-        pattern = varlena_bytes_column([bytes(pattern)])
-    if isinstance(pattern[0], np.ndarray):
-        pv = _str_operand(pattern, pattern_nulls)
-    else:
-        pv = _str_device_vec(pattern, pattern_nulls, n)
-    xcall(capi.XCALL_GO_LIKE, [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n),
-                               _str_device_vec(col, col_nulls, n), pv], n)
+        pattern = [bytes(pattern)]
+    _str_pred_device(capi.XCALL_GO_LIKE, col, pattern, n, out_dev, out_nulls_dev, col_nulls, pattern_nulls)
 
 
 # ------------------------------------------------------------------------------- IN / NOT IN (csrc/goelem.cu, csrc/strpred.cu)
-def _in_operand(T, x, nulls):
-    if T in capi.T_VARLENA:
-        return _str_operand(x, nulls)
-    a = np.ascontiguousarray(x)
-    return Vector(data=a, nulls=nulls, length=a.shape[0])
-
-
 def go_in(T, col, values, negate=False, col_nulls=None, values_nulls=None, rnulls=None, length=None):
     """col IN values (NOT IN with negate), operator_in.go: values is the list, with its NULL elements skipped; a NULL row is NULL, every
     other row is its membership (NOT IN: its negation).  Fixed-width T: numpy arrays of the column's element type (DECIMAL128 / UUID:
     16-byte rows); the varlena T: a list of bytes or a (cells, area) pair.  A one-element col is a const.  rnulls: the result bitmap on entry
     (rows set there are skipped).  Returns (values bool[n], nulls bool[n])."""
-    vc, vl = _in_operand(T, col, col_nulls), _in_operand(T, values, values_nulls)
+    vc, vl = _vec(col, nulls=col_nulls), _vec(values, nulls=values_nulls)
     n = length if length is not None else vc.length
     r = np.zeros(max(n, 1), dtype=np.uint8)
     rn = np.zeros(max((n + 63) // 64, 1), dtype=np.uint64) if rnulls is None else np.array(rnulls, dtype=np.uint64)
     fid = capi.XCALL_GO_NOT_IN(T) if negate else capi.XCALL_GO_IN(T)
-    xcall(fid, [Vector(data=r[:n], nulls=rn, length=n), vc, vl, Vector(data=np.array([vl.length], np.int64))], n)
+    xcall(fid, [Vector(data=r[:n], nulls=rn, length=n), vc, vl, _params_vec(np.array([vl.length], np.int64))], n)
     return r[:n].astype(bool), bitmap_to_bools(rn, n)
 
 
@@ -1453,13 +1335,9 @@ def go_in_device(T, col, values, nvalues, n, out_dev, out_nulls_dev, negate=Fals
     """IN / NOT IN on resident vectors: col and values are DeviceBuffers (the varlena T: (cells, area) pairs, area None when every value is
     inline), nulls DeviceBuffers or None; out_dev (bool[n]) and out_nulls_dev (its bitmap, in/out) DeviceBuffers.  The parameter block stays
     on the host, so a fixed-width call only enqueues work; a varlena call reads back one status record."""
-    def dev(x, nulls, rows):
-        if T in capi.T_VARLENA:
-            return _str_device_vec(x, nulls, rows)
-        return Vector(data_ptr=x.ptr, data_nbytes=x.nbytes, nulls_ptr=nulls.ptr if nulls is not None else None, length=rows)
     fid = capi.XCALL_GO_NOT_IN(T) if negate else capi.XCALL_GO_IN(T)
-    xcall(fid, [Vector(data_ptr=out_dev.ptr, data_nbytes=n, nulls_ptr=out_nulls_dev.ptr, length=n), dev(col, col_nulls, n),
-                dev(values, values_nulls, nvalues), Vector(data=np.array([nvalues], np.int64))], n)
+    xcall(fid, [Vector(data=out_dev.view(n), nulls=out_nulls_dev, length=n), _vec(col, n, col_nulls), _vec(values, nvalues, values_nulls),
+                _params_vec(np.array([nvalues], np.int64))], n)
 
 
 # --------------------------------------------------------------- CASE, IF, COALESCE and the CASE select lists (csrc/caseexpr.cu)
@@ -1474,33 +1352,37 @@ def _case_value_dtype(T):
     return {1: np.uint8, 2: np.uint16, 4: np.uint32, 8: np.uint64, 16: np.uint64}[CASE_WIDTH[T]] if T not in capi.NP_OF_T else capi.NP_OF_T[T]
 
 
-def _case_operand(T, op, is_cond=False):
-    """(data, nulls) -> Vector.  A condition is a bool array; a fixed-width value any array of the type's bytes per row (16-byte types:
-    uint64[k, 2]); a string value a list of bytes or a (cells, area) pair.  One row is a const operand."""
-    data, nulls = op
-    if not is_cond and T in CASE_STR_TYPES:
-        return _str_operand(data, nulls)
-    a = np.ascontiguousarray(data)
-    rows = a.shape[0]
-    return Vector(data=a.view(np.uint8).reshape(-1), nulls=nulls, length=rows)
+def _when_then(conds, values, else_value):
+    """GO_CASE's operands in argument order: c1, v1, ... [, else]"""
+    if len(conds) != len(values):
+        raise ValueError("one value per condition")
+    return [o for cv in zip(conds, values) for o in cv] + ([] if else_value is None else [else_value])
 
 
-def _case_run(fid, T, vecs, nsel, has_else, n, rnulls, area_cap):
+def _case_call(fid, res, nsel, has_else, vecs, n):
+    """one GO_CASE / GO_COALESCE call: (rc, msg, area_len), area_len the bytes a string result's area needs"""
+    prm = _params_vec(capi.CaseParams(nsel, has_else, 0))
+    rc, msg = xcall(fid, [res, prm] + vecs, n, raise_on_error=False)
+    return rc, msg, int(prm.data.view(np.int64)[1])
+
+
+def _case_run(fid, T, operands, nsel, has_else, rnulls, length, area_cap):
+    vecs = [_vec(d, nulls=nl) for d, nl in operands]
+    n = length if length is not None else max(v.length for v in vecs)
     rn = np.zeros(max((n + 63) // 64, 1), dtype=np.uint64) if rnulls is None else np.array(rnulls, dtype=np.uint64)
-    prm = np.frombuffer(bytes(capi.CaseParams(nsel, has_else, 0)), dtype=np.uint8).copy()
-    pv = Vector(data=prm, length=1)
     if T not in CASE_STR_TYPES:
         w = CASE_WIDTH.get(T, 8)
         r = np.zeros(max(n, 1) * w, dtype=np.uint8)
-        xcall(fid, [Vector(data=r[:n * w], nulls=rn, length=n), pv] + vecs, n)
+        rc, msg, _ = _case_call(fid, Vector(data=r[:n * w], nulls=rn, length=n), nsel, has_else, vecs, n)
+        if rc:
+            raise capi.MoError(rc, "xcall xfunc failed, error code %d, %s" % (rc, msg))
         out = r[:n * w].view(_case_value_dtype(T))
         return (out.reshape(n, 2) if w == 16 else out), bitmap_to_bools(rn, n)
     cap = area_cap if area_cap is not None else sum(int(v.area.nbytes) for v in vecs if v.area is not None)
     cells = np.zeros(max(n, 1) * 24, dtype=np.uint8)
     for attempt in range(2):
         area = np.zeros(cap, dtype=np.uint8)
-        rc, msg = xcall(fid, [Vector(data=cells[:24 * n], nulls=rn, area=area, length=n), pv] + vecs, n, raise_on_error=False)
-        need = int(prm.view(np.int64)[1])
+        rc, msg, need = _case_call(fid, Vector(data=cells[:24 * n], nulls=rn, area=area, length=n), nsel, has_else, vecs, n)
         if rc == capi.RC_OUT_OF_RANGE and attempt == 0 and area_cap is None:
             cap = need                     # the JOIN_PROBE capacity protocol: the call left the result unchanged; repeat with area_len
             continue
@@ -1514,15 +1396,8 @@ def go_case(T, conds, values, else_value=None, rnulls=None, length=None, area_ca
     None; a one-row operand is a const.  rnulls: the result bitmap on entry (rows set there are skipped).  Fixed-width T returns (values,
     nulls bool[n]); the string T returns (cells uint8[24 n], area, nulls bool[n]), the area sized by the call (area_cap: a fixed capacity,
     RC_OUT_OF_RANGE raised when it is too small)."""
-    if len(conds) != len(values):
-        raise ValueError("one value per condition")
-    vecs = []
-    for c, v in zip(conds, values):
-        vecs += [_case_operand(T, c, True), _case_operand(T, v)]
-    if else_value is not None:
-        vecs.append(_case_operand(T, else_value))
-    n = length if length is not None else max(v.length for v in vecs)
-    return _case_run(capi.XCALL_GO_CASE(T), T, vecs, len(conds), 0 if else_value is None else 1, n, rnulls, area_cap)
+    operands = _when_then(conds, values, else_value)
+    return _case_run(capi.XCALL_GO_CASE(T), T, operands, len(conds), 0 if else_value is None else 1, rnulls, length, area_cap)
 
 
 def go_iff(T, cond, a, b, rnulls=None, length=None, area_cap=None):
@@ -1532,29 +1407,16 @@ def go_iff(T, cond, a, b, rnulls=None, length=None, area_cap=None):
 
 def go_coalesce(T, operands, rnulls=None, length=None, area_cap=None):
     """COALESCE(operands...) (CoalesceGeneral / CoalesceStr): the first non-NULL operand, or NULL.  Operands and results as go_case."""
-    vecs = [_case_operand(T, o) for o in operands]
-    n = length if length is not None else max(v.length for v in vecs)
-    return _case_run(capi.XCALL_GO_COALESCE(T), T, vecs, len(operands), 0, n, rnulls, area_cap)
+    return _case_run(capi.XCALL_GO_COALESCE(T), T, operands, len(operands), 0, rnulls, length, area_cap)
 
 
-def _case_device_vec(T, op, rows, is_cond=False):
-    data, nulls = op
-    if not is_cond and T in CASE_STR_TYPES:
-        return _str_device_vec(data, nulls, rows)
-    return Vector(data_ptr=data.ptr, data_nbytes=data.nbytes, nulls_ptr=nulls.ptr if nulls is not None else None, length=rows)
-
-
-def _case_device(fid, T, vecs, nsel, has_else, n, out_dev, out_nulls_dev, out_area_dev):
-    prm = np.frombuffer(bytes(capi.CaseParams(nsel, has_else, 0)), dtype=np.uint8).copy()
-    if T in CASE_STR_TYPES:
-        res = Vector(data_ptr=out_dev.ptr, data_nbytes=24 * n, nulls_ptr=out_nulls_dev.ptr, length=n,
-                     area_ptr=out_area_dev.ptr if out_area_dev is not None else None, area_nbytes=out_area_dev.nbytes if out_area_dev is not None else 0)
-    else:
-        res = Vector(data_ptr=out_dev.ptr, data_nbytes=CASE_WIDTH.get(T, 8) * n, nulls_ptr=out_nulls_dev.ptr, length=n)
-    rc, msg = xcall(fid, [res, Vector(data=prm, length=1)] + vecs, n, raise_on_error=False)
+def _case_device(fid, T, operands, nsel, has_else, n, out_dev, out_nulls_dev, out_area_dev):
+    width = 24 if T in CASE_STR_TYPES else CASE_WIDTH.get(T, 8)
+    res = Vector(data=out_dev.view(width * n), nulls=out_nulls_dev, area=out_area_dev if T in CASE_STR_TYPES else None, length=n)
+    rc, msg, area_len = _case_call(fid, res, nsel, has_else, [_vec(d, n, nl) for d, nl in operands], n)
     if rc and not (rc == capi.RC_OUT_OF_RANGE and T in CASE_STR_TYPES):
         raise capi.MoError(rc, "xcall xfunc failed, error code %d, %s" % (rc, msg))
-    return rc, int(prm.view(np.int64)[1])
+    return rc, area_len
 
 
 def go_case_device(T, conds, values, else_value, n, out_dev, out_nulls_dev, out_area_dev=None):
@@ -1562,18 +1424,13 @@ def go_case_device(T, conds, values, else_value, n, out_dev, out_nulls_dev, out_
     = const) into out_dev (T[n] or 24-byte cells), out_nulls_dev (its bitmap, in/out) and out_area_dev (strings: the area, its size the
     capacity).  The parameter block stays on the host: a fixed-width call only enqueues work.  Returns (rc, area_len): rc is 0, or
     RC_OUT_OF_RANGE for a string result whose area is smaller than area_len (the result is then unchanged)."""
-    vecs = []
-    for c, v in zip(conds, values):
-        vecs += [_case_device_vec(T, c, n, True), _case_device_vec(T, v, n)]
-    if else_value is not None:
-        vecs.append(_case_device_vec(T, else_value, n))
-    return _case_device(capi.XCALL_GO_CASE(T), T, vecs, len(conds), 0 if else_value is None else 1, n, out_dev, out_nulls_dev, out_area_dev)
+    operands = _when_then(conds, values, else_value)
+    return _case_device(capi.XCALL_GO_CASE(T), T, operands, len(conds), 0 if else_value is None else 1, n, out_dev, out_nulls_dev, out_area_dev)
 
 
 def go_coalesce_device(T, operands, n, out_dev, out_nulls_dev, out_area_dev=None):
     """go_coalesce on resident operands, as go_case_device"""
-    vecs = [_case_device_vec(T, o, n) for o in operands]
-    return _case_device(capi.XCALL_GO_COALESCE(T), T, vecs, len(operands), 0, n, out_dev, out_nulls_dev, out_area_dev)
+    return _case_device(capi.XCALL_GO_COALESCE(T), T, operands, len(operands), 0, n, out_dev, out_nulls_dev, out_area_dev)
 
 
 def case_select(rem_words, cond, cond_nulls, n):
@@ -1584,13 +1441,12 @@ def case_select(rem_words, cond, cond_nulls, n):
     then = np.zeros(max(w, 1), dtype=np.uint64)
     rem = np.array(rem_words, dtype=np.uint64).reshape(-1)[:w].copy()
     c = np.ascontiguousarray(cond).view(np.uint8).reshape(-1)
-    xcall(capi.XCALL_GO_CASE_SELECT, [Vector(data=then[:w], length=n), Vector(data=rem, length=n), Vector(data=c, nulls=cond_nulls, length=c.shape[0])], n)
+    xcall(capi.XCALL_GO_CASE_SELECT, [Vector(data=then[:w], length=n), Vector(data=rem, length=n), _vec(c, nulls=cond_nulls)], n)
     return then[:w], rem
 
 
 def case_select_device(then_dev, rem_dev, cond_dev, cond_nulls_dev, n):
     """case_select on resident words and condition (DeviceBuffers): enqueue-only"""
     wb = 8 * ((n + 63) // 64)
-    xcall(capi.XCALL_GO_CASE_SELECT, [Vector(data_ptr=then_dev.ptr, data_nbytes=wb, length=n), Vector(data_ptr=rem_dev.ptr, data_nbytes=wb, length=n),
-                                      Vector(data_ptr=cond_dev.ptr, data_nbytes=cond_dev.nbytes, nulls_ptr=cond_nulls_dev.ptr if cond_nulls_dev is not None else None,
-                                             length=n)], n)
+    xcall(capi.XCALL_GO_CASE_SELECT, [Vector(data=then_dev.view(wb), length=n), Vector(data=rem_dev.view(wb), length=n),
+                                      _vec(cond_dev, n, cond_nulls_dev)], n)

@@ -177,7 +177,7 @@ class PinnedArray:
 
 # ---------------------------------------------------------------------------------------------- Vector
 class Vector:
-    """Minimal vector.Vector: host numpy buffers OR device pointers (ptr + nbytes)."""
+    """Minimal vector.Vector: data / nulls / area are host numpy buffers or DeviceBuffers, or raw device pointers (ptr + nbytes)."""
 
     def __init__(self, data=None, nulls=None, area=None, length=None, const=False,
                  data_ptr=None, data_nbytes=0, nulls_ptr=None, area_ptr=None, area_nbytes=0):
@@ -188,28 +188,31 @@ class Vector:
         self.nulls_ptr, self.area_ptr, self.area_nbytes = nulls_ptr, area_ptr, area_nbytes
         self._keep = []
 
+    def _raw(self, x, dtype=None):
+        """(address, bytes, buffer) of a DeviceBuffer, or of x as a contiguous host array kept alive with this Vector"""
+        if isinstance(x, DeviceBuffer):
+            return x.ptr, x.nbytes, x
+        x = np.ascontiguousarray(x, dtype)
+        self._keep.append(x)
+        return x.ctypes.data, x.nbytes, x
+
     def fill_raw_ptr_len(self):
-        """[pnulls, nbits, pdata, dataSz, parea, areaSz] -- Vector.FillRawPtrLen, vector.go:5161-5172"""
+        """[pnulls, nbits, pdata, dataSz, parea, areaSz] -- Vector.FillRawPtrLen, vector.go:5161-5172.  An empty host area passes no
+        pointer; a device area always passes its own."""
         a = capi.XCallArgs()
         if self.data_ptr is not None:
             a.pdata, a.dataSz = self.data_ptr, self.data_nbytes
         elif self.data is not None:
-            d = np.ascontiguousarray(self.data)
-            self._keep.append(d)
-            a.pdata, a.dataSz = d.ctypes.data, d.nbytes
+            a.pdata, a.dataSz, _ = self._raw(self.data)
         if self.nulls_ptr is not None:
             a.pnulls, a.nullCnt = self.nulls_ptr, self.length
         elif self.nulls is not None:
-            w = np.ascontiguousarray(self.nulls, dtype=np.uint64)
-            self._keep.append(w)
-            self.nulls = w
-            a.pnulls, a.nullCnt = w.ctypes.data, self.length
+            a.pnulls, _, self.nulls = self._raw(self.nulls, np.uint64)
+            a.nullCnt = self.length
         if self.area_ptr is not None:
             a.parea, a.areaSz = self.area_ptr, self.area_nbytes
-        elif self.area is not None and len(self.area):
-            ar = np.ascontiguousarray(self.area)
-            self._keep.append(ar)
-            a.parea, a.areaSz = ar.ctypes.data, ar.nbytes
+        elif isinstance(self.area, DeviceBuffer) or (self.area is not None and len(self.area)):
+            a.parea, a.areaSz, _ = self._raw(self.area)
         return a
 
 
